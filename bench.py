@@ -1,6 +1,6 @@
 #!/usr/bin/env python
 """bench.py -- ALS iterations/sec and top-k predictions/sec on the BASELINE.json workload (configs[1]: rank 64,
-1M users x 100k items, 100M synthetic implicit ratings), B200-native path vs the CPU restatement of the reference.
+1M users x 100k items, 100M synthetic implicit ratings), H100-native path vs the CPU restatement of the reference.
 
 One "step" = one ALS iteration (item half-step + user half-step) over the whole rating set.
   value    : iterations/sec with ratings + CSR already resident in HBM (CUDA events on the library stream)
@@ -13,6 +13,8 @@ One "step" = one ALS iteration (item half-step + user half-step) over the whole 
   cpu_baseline / --impl reference : the oracle (C/OpenMP restatement of MLlib ALS) timed on the host's physical cores
              over FULL iterations of the same workload
   topk     : top-k predictions/sec through pio_als_recommend / pio_als_similar with host buffers
+  --dump-outputs DIR : after the timed steps, what they computed (the factors a caller of pio_als_run receives) as
+             DIR/<name>.npy, so that two builds can be compared output for output on identical seeded inputs
 See DESIGN.md for the roofline arithmetic.
 """
 import argparse
@@ -137,37 +139,28 @@ class ClockSampler:
                 "reasons": sorted(reasons), "samples": len(sm), "how": "nvidia-smi -lms 20"}
 
 
-def traffic_from_profiles(workload):
-    """dram__bytes_read+write of ONE launch of the dominant kernel, from the committed ncu --set full capture (null if none)."""
-    p = ROOT / "profiles" / "traffic.json"
+def gpu_identity(index=0):
+    """Name, power limit and maximum SM clock of the card the numbers were measured on (nvidia-smi, read-only query)."""
+    q = "name,power.limit,clocks.max.sm"
     try:
-        return json.loads(p.read_text())[workload]["dram_bytes_per_launch"]
+        out = subprocess.run(["nvidia-smi", f"--id={index}", f"--query-gpu={q}", "--format=csv,noheader,nounits"],
+                             capture_output=True, text=True, timeout=30).stdout.strip().split(",")
+        return {"name": out[0].strip(), "power_limit_w": float(out[1]), "sm_max_mhz": float(out[2])}
     except Exception:
-        return None
+        return {"name": None, "power_limit_w": None, "sm_max_mhz": None}
+
+
+# H100 SXM data-sheet rates (dense): 3.35 TB/s HBM3, 989 TFLOP/s BF16; FP32 FFMA and FP64 DFMA from 132 SMs x 128 / 64
+# lanes x 2 flops x 1.98 GHz (the maximum boost clock).  They are denominators of the roofline fractions, not rates
+# this program reached; a card with a lower power limit clocks lower.
+H100_SMS, H100_BOOST_GHZ = 132, 1.98
 
 
 def measured_peaks():
-    """HBM GB/s, dense bf16 TFLOP/s (driver-written MEASURED_PEAKS.json), FP32 FFMA TFLOP/s (profiles/peaks_r02.json,
-    measured by tools/peaks.cu on this pool; nominal 148 x 128 x 2 x 1.965 GHz otherwise)."""
-    hbm, bf16, src = 6650.0, 1590.0, "fallback"
-    p = ROOT / "MEASURED_PEAKS.json"
-    if p.exists():
-        d = json.loads(p.read_text())
-        hbm, bf16, src = d.get("hbm_gbs", hbm), d.get("bf16_tflops", bf16), "measured"
-    fp32, fp32_src = 148 * 128 * 2 * 1.965e9 / 1e12, "nominal 148 SM x 128 lanes x 2 x 1.965 GHz"
-    mma_tf32 = dfma = None
-    q = ROOT / "profiles" / "peaks_r02.json"
-    if q.exists():
-        try:
-            d = json.loads(q.read_text())
-            if d.get("ffma_tflops"):
-                fp32, fp32_src = float(d["ffma_tflops"]), "measured (tools/peaks.cu, profiles/peaks_r02.json)"
-            mma_tf32 = d.get("mma_sync_tf32_tflops")
-            dfma = d.get("dfma_tflops")
-        except Exception:
-            pass
-    return {"hbm": hbm, "bf16": bf16, "src": src, "fp32": fp32, "fp32_src": fp32_src, "mma_tf32": mma_tf32,
-            "dfma": dfma or 148 * 64 * 2 * 1.965e9 / 1e12}
+    """Roofline denominators: H100 SXM data-sheet HBM and BF16 rates, nominal FP32 FFMA and FP64 DFMA rates."""
+    return {"hbm": 3350.0, "bf16": 989.0, "src": "H100 SXM data sheet",
+            "fp32": H100_SMS * 128 * 2 * H100_BOOST_GHZ / 1e3, "fp32_src": "nominal 132 SM x 128 lanes x 2 x 1.98 GHz",
+            "mma_tf32": None, "dfma": H100_SMS * 64 * 2 * H100_BOOST_GHZ / 1e3}
 
 
 # ---------------------------------------------------------------------------------------------------------
@@ -201,10 +194,12 @@ def load_oracle():
                 flags = next(ln for ln in open("/proc/cpuinfo") if ln.startswith("flags"))
             except Exception:
                 pass
-            so = o._SO.parent / f"libals_oracle_native_{hashlib.sha1(flags.encode()).hexdigest()[:10]}.so"
-            if not so.exists() or so.stat().st_mtime < o._SRC.stat().st_mtime:
-                subprocess.run(["gcc", "-O3", "-march=native", "-fopenmp", "-fPIC", "-shared", "-fvisibility=hidden",
-                                "-o", str(so), str(o._SRC), "-lm"], check=True)
+            # built in a temporary directory: the source tree may be read-only and stays untouched
+            import tempfile
+            tmp = Path(tempfile.mkdtemp(prefix="pio_bench_"))
+            so = tmp / f"libals_oracle_native_{hashlib.sha1(flags.encode()).hexdigest()[:10]}.so"
+            subprocess.run(["gcc", "-O3", "-march=native", "-fopenmp", "-fPIC", "-shared", "-fvisibility=hidden",
+                            "-o", str(so), str(o._SRC), "-lm"], check=True)
             o._lib = ctypes.CDLL(str(so))
             o._lib.oracle_num_threads.restype = ctypes.c_int
     except Exception:
@@ -356,8 +351,8 @@ def topk_bench(native, o, cores, m, nu, ni, k, uf, itf, uh, ih, peaks, dev):
         "roofline": {"bound": "fp64", "achieved": 2.0 * nq * ni * k / dt / 1e12, "peak": peaks["dfma"], "unit": "TFLOP/s",
                      "frac": 2.0 * nq * ni * k / dt / 1e12 / peaks["dfma"],
                      "note": "scores are accumulated in fp64 in index order (bit-identical to the JVM's ddot), so the bound "
-                             "is the DFMA pipe: one DFMA per (query, item, feature); peak = tools/peaks.cu "
-                             "(profiles/peaks_r02.json). Includes the H2D / D2H copies of the call.",
+                             "is the DFMA pipe: one DFMA per (query, item, feature); peak = nominal H100 SXM DFMA rate. "
+                             "Includes the H2D / D2H copies of the call.",
                      "hbm_frac_per_16_queries": nq / 16.0 * scan_bytes / dt / 1e9 / peaks["hbm"]}}
     # similarproduct path (A9, BASELINE.json configs[3]): cosine top-20 over 1 M item vectors (unit-norm Gaussian, rank 64),
     # 10 k queries of 1-5 items, one pio_als_similar_batch call on an imported item-only model
@@ -459,6 +454,8 @@ def main():
     ap.add_argument("--no-e2e", action="store_true")
     ap.add_argument("--no-parity", action="store_true")
     ap.add_argument("--no-topk", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the factors of the last timed step as DIR/<name>.npy (float32, <= 64 MB in all)")
     args = ap.parse_args()
     nu, ni, nnz, k, implicit = WORKLOADS[args.workload]
     rank = int(os.environ.get("RANK", "0"))
@@ -468,7 +465,7 @@ def main():
                f"{'implicit' if implicit else 'explicit'} ratings")
     config = {"workload": wl_name, "lambda": LAMBDA, "alpha": ALPHA, "seed": SEED,
               "dedup": "sum" if implicit else "none",
-              "l2": "inputs (1.6 GB of CSR + 282 MB of factors per iteration at c2) exceed the 126 MB L2",
+              "l2": "inputs (1.6 GB of CSR + 282 MB of factors per iteration at c2) exceed the 50 MB L2",
               "parallelism": (f"rows and input events sharded x{args.gpus}, ratings routed to row owners by NCCL send/recv, "
                               "factor all-gather per half-iteration") if args.gpus > 1 else "1 GPU"}
 
@@ -549,6 +546,8 @@ def main():
     if rank == 0:
         uf_T, itf_T, uh, ih = m.get_factors()
     checksum = factor_checksum(uf_T, itf_T) if rank == 0 else None
+    if rank == 0 and args.dump_outputs:
+        dump_outputs(args.dump_outputs, uf_T, itf_T, uh, ih)
     if want_parity:
         m.run(1)
         if rank == 0:
@@ -634,9 +633,9 @@ def main():
     side_bytes = {"user": 8 * nnz_eff + 4 * nua * k + 4 * nia * k, "item": 8 * nnz_eff + 4 * nia * k + 4 * nua * k}
     side_ms = {"user": ph["user_solve_ms"] / args.steps, "item": ph["item_solve_ms"] / args.steps}
     side_kernel = {"user": ph["user_kernel"], "item": ph["item_kernel"]}
-    side_tc = {sd: side_kernel[sd] != "fp32" for sd in side_kernel}   # Gramian on tensor cores (tcgen05 or mma.sync)
+    side_tc = {sd: side_kernel[sd] != "fp32" for sd in side_kernel}   # Gramian on tensor cores (wgmma or mma.sync)
     kernel_names = {"fp32": "als_solve_kernel (gather + FP32 Gramian + warp Cholesky)",
-                    "tcgen05": "tc::als_solve_tc_kernel (tcgen05 split-TF32 Gramian + warp Cholesky)",
+                    "wgmma": "tc::als_solve_tc_kernel (wgmma split-TF32 Gramian + warp Cholesky)",
                     "mma": "mm::als_solve_mma_kernel (one warp per row: mma.sync 3xTF32 Gramian + warp Cholesky)",
                     "pair": "pr::als_solve_pair_kernel (two rows per warp: mma.sync 3xTF32 Gramian + lockstep Cholesky)"}
     fp32_peak = peaks["fp32"]
@@ -668,8 +667,6 @@ def main():
         "peak_source": peaks["fp32_src"] if not side_tc[dom] else
                        f"{peak_src} dense bf16 / 2 = tf32 MMA rate, / 3 because an fp32-class product is three TF32 MMAs",
         "ms_per_launch": d["ms_per_launch"],
-        "traffic": traffic_from_profiles(args.workload),
-        "traffic_unit": "dram bytes of this launch, from the committed ncu --set full capture (profiles/traffic.json)",
         "per_gpu": True,
         "hbm": {"achieved": d["achieved_gbs"], "peak": hbm_peak, "unit": "GB/s", "frac": d["achieved_gbs"] / hbm_peak,
                 "peak_source": peak_src, "algorithmic_bytes_per_launch": d["algorithmic_bytes"]},
@@ -682,7 +679,8 @@ def main():
     out = {"metric": "ALS iterations/sec", "value": value, "unit": "iterations/s", "n_gpus": args.gpus,
            "steps": args.steps, "warmup": args.warmup, "ms_per_step": dev_ms / args.steps,
            "higher_is_better": True, "scaling": "strong", "vs_baseline": None, "dtype": "f32",
-           "data": "synthetic", "config": config, "clocks": clocks, "gpu_launches": int(launches),
+           "data": "synthetic", "config": config, "gpu": gpu_identity(dev), "clocks": clocks,
+           "gpu_launches": int(launches),
            "wall_ms_per_step": wall_ms / args.steps, "ingest_ms": ingest_ms, "nnz_after_dedup": int(nnz_eff),
            "factor_checksum": checksum,
            "factor_checksum_note": f"crc32(user factors) || crc32(item factors) after {args.warmup}+{args.steps} iterations "
@@ -727,6 +725,32 @@ def main():
             rc = rc or 4
     print(json.dumps(out))
     return rc
+
+
+DUMP_BYTES = 60_000_000   # under 64 MB in all
+
+
+def dump_outputs(out_dir, uf, itf, uh, ih):
+    """The factors after the last timed step as float32 .npy files.  Matrices that do not fit the 64 MB budget are
+    sampled: a fixed, seeded set of rows (the same for every run with the same arguments), with the row numbers
+    stored next to them."""
+    d = Path(out_dir)
+    d.mkdir(parents=True, exist_ok=True)
+    arrays = {"user_factors": uf, "item_factors": itf}
+    flags = {"user_has_factor": uh, "item_has_factor": ih}
+    budget = DUMP_BYTES - sum(4 * a.shape[0] for a in flags.values()) - (1 << 20)
+    total = sum(a.nbytes for a in arrays.values())
+    rng = np.random.default_rng(SEED)
+    for name, a in arrays.items():
+        if total > budget:
+            share = int(budget * a.nbytes / total)
+            n = min(a.shape[0], max(1, share // (a.shape[1] * 4 + 8)))
+            rows = np.sort(rng.choice(a.shape[0], n, replace=False))
+            np.save(d / f"{name}_rows.npy", rows.astype(np.float64))
+            a = a[rows]
+        np.save(d / f"{name}.npy", np.ascontiguousarray(a, np.float32))
+    for name, a in flags.items():
+        np.save(d / f"{name}.npy", a.astype(np.float32))
 
 
 def nccl_id_2(native, rank, world):

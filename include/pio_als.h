@@ -1,5 +1,5 @@
 /*
- * pio_als.h -- C ABI of the B200-native ALS hot path for PredictionIO engine templates.
+ * pio_als.h -- C ABI of the H100-native ALS hot path for PredictionIO engine templates.
  *
  * This is the drop-in boundary: exactly what a JNI shim in a `native-als` Scala module
  * binds in place of the Spark-MLlib calls the templates make today (INTEGRATION.md shows
@@ -12,7 +12,7 @@
  * core/src/main/scala/org/apache/predictionio/workflow/CreateServer.scala:508-510).
  *
  * There is NO CPU fallback: every entry point that computes fails with
- * PIO_ALS_ERR_CUDA when no sm_100 device / CUDA runtime is usable.
+ * PIO_ALS_ERR_CUDA when no sm_90 device / CUDA runtime is usable.
  *
  * Reference interfaces replaced (paths relative to the reference repository root):
  *   pio_als_create + pio_als_set_ratings_coo + pio_als_run + pio_als_get_factors  (or the
@@ -104,7 +104,7 @@ typedef struct pio_als_stats {
 } pio_als_stats;
 
 PIO_API int pio_als_abi_version(void);
-/* number of visible sm_100 devices, or PIO_ALS_ERR_CUDA */
+/* number of visible sm_90 devices, or PIO_ALS_ERR_CUDA */
 PIO_API int pio_als_device_count(void);
 PIO_API int pio_als_nccl_unique_id(uint8_t out_id[128]);
 
@@ -145,8 +145,8 @@ PIO_API int pio_als_set_init(pio_als_handle* h, const float* user_factors, const
 PIO_API int pio_als_run(pio_als_handle* h, int n_iters);
 /* Device-time breakdown of the last pio_als_run (CUDA events on the handle's stream), for bench.py's roofline:
  * out[0] item half-step solve kernels (ms, summed over the run), out[1] user half-step solve kernels, out[2] YtY
- * kernels, out[3] all-gathers, out[4]/out[5] = solve kernel of the item / user side (0 FP32 CUDA-core kernel, 1 tcgen05
- * kernel, 2 warp-level mma.sync kernel), out[6] iterations of that run, out[7] reserved.  No reference counterpart (Spark's stage timings,
+ * kernels, out[3] all-gathers, out[4]/out[5] = solve kernel of the item / user side (0 FP32 CUDA-core kernel, 1 wgmma
+ * kernel, 2 warp-level mma.sync kernel, 3 pair kernel), out[6] iterations of that run, out[7] reserved.  No reference counterpart (Spark's stage timings,
  * core/.../workflow/CoreWorkflow.scala:74-81, are the nearest thing). */
 PIO_API int pio_als_get_phase_ms(pio_als_handle* h, double out[8]);
 

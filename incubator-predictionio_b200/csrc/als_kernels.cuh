@@ -1,4 +1,4 @@
-// als_kernels.cuh -- the ALS half-iteration on sm_100a.
+// als_kernels.cuh -- the ALS half-iteration on sm_90a (H100).
 //
 // Replaces MLlib's `computeFactors` (SURVEY.md 8(c)-5/6; called through als.run at
 // examples/scala-parallel-recommendation/blacklist-items/src/main/scala/ALSAlgorithm.scala:86):

@@ -4,7 +4,7 @@
 //
 // Why a third kernel: the FP32 kernel (als_kernels.cuh) is bound by shared-memory bandwidth by construction (an 8x8
 // register block reads 1 byte of operands per FMA = the SM's 128 B/clk) and spends 137 warp instructions per rating;
-// the tcgen05 kernel (als_tc_kernel.cuh) wins on long rows but needs half of its sixteen warps for the producer
+// the wgmma kernel (als_tc_kernel.cuh) is built for long rows but needs half of its sixteen warps for the producer
 // pipeline, so on short rows (the user side of the headline workload: ~100 ratings per row) it is bound by its eight
 // solver warps.  Here every warp gathers, accumulates AND solves its own row: a chunk of 8 ratings costs 16 LDS.32
 // (each loaded value serves as A and as B fragment), a cvt/subtract split, 60 mma.sync and 80 FADD -- ~30 warp

@@ -170,7 +170,7 @@ __device__ __forceinline__ void accumulate_row(const SolveParams& p, long long b
 #pragma unroll
       for (int e = 0; e < 4; ++e) {
         // Veltkamp split: h = the 11 leading bits of v rounded to nearest (exactly a TF32 value), v - h exact; three
-        // FMA-pipe instructions instead of the ~5 ALU instructions cvt.rna.tf32 expands to on sm_100.  |v - h| <= 2^-11 |v|;
+        // FMA-pipe instructions instead of the ALU sequence cvt.rna.tf32 expands to.  |v - h| <= 2^-11 |v|;
         // the dropped lo*lo term is 2^-22.
         // (intrinsics: the compiler must not contract c - (c - v) into FMAs, which would return v itself)
         const float c = __fmul_rn(v[e], 8193.f);       // 2^13 + 1

@@ -1,37 +1,32 @@
-// als_tc_kernel.cuh -- rank 33..64 ALS half-step with the Gramian on the 5th-gen tensor cores (tcgen05 + TMEM).
+// als_tc_kernel.cuh -- rank 33..64 ALS half-step with the Gramian on the Hopper tensor cores (wgmma).
 //
 // Same mathematics as als_solve_kernel (als_kernels.cuh) for KP = 64, but  A = sum (s y)(s y)^T  is a
-// split-precision SYRK on tcgen05:
-//   every gathered, sqrt(c1)-scaled source row x (64 floats) is staged as  [hi | lo]  (128 floats),
-//   hi = the top 10 mantissa bits of x, lo = x - hi (exact);  8 ratings form one K-block in the MN-major
-//   SWIZZLE_128B_BASE32B UMMA shared-memory layout (per 32 columns a 1 KB atom: one 128-byte row per
-//   rating, its four 32-byte chunks XOR-swizzled by rating%4) -- the only MN-major layout kind::tf32
-//   accepts (verified with tools/umma_probe.cu; the un-swizzled MN-major forms silently produce 0);
-//   per K-block ONE  tcgen05.mma.cta_group::1.kind::tf32  with A = all 128 staged columns (M = 128) and
-//   B = the 64 hi columns (N = 64, K = 8) accumulates  D = [hi^T hi ; lo^T hi]  into a 128-lane x 64-column
-//   TMEM accumulator (row r in lane r); the drain forms  A = HH + LH + LH^T  (the dropped lo^T lo term is
-//   ~2^-20 relative).  TMEM (512 columns) holds two batches of four rows: the MMAs of batch b+1 overlap the
-//   drain of batch b.
+// split-precision SYRK on wgmma:
+//   every gathered, sqrt(c1)-scaled source row x is split into hi (top 10 mantissa bits) and lo = x - hi (exact);
+//   8 ratings form one K-block of two 64 x 8 tiles (hi, lo) in the K-major, un-swizzled wgmma layout (tf32 wgmma
+//   reads both operands K-major only: features are M / N, ratings are K).  Per K-block three m64n64k8 wgmmas add
+//   lo hi^T + hi lo^T + hi hi^T to the team's register accumulator (lo lo^T, ~2^-20 relative, is dropped).  The
+//   tensor core's fp32 accumulation truncates, so a chain covers one 24-rating stage; stage sums are added into A in
+//   shared memory with round-to-nearest fp32 adds.
 //
 // Warp roles (512 threads, 1 CTA per SM, persistent; degree-sorted rows are dealt statically: groups of
 // NTEAM*NSLOT consecutive rows go to the CTAs in snake order):
-//   warp 0              scheduler + MMA issuer, warp-parallel: lane t*4+s keeps row lane (team t, slot s) in
-//                       registers, builds the flat stage list of a batch with shuffles, publishes it, issues the
-//                       batch's MMAs from one lane and commits to mbarriers
+//   warp 0              scheduler, warp-parallel: lane t*4+s keeps row lane (team t, slot s) in registers, builds
+//                       the flat stage list of a batch with shuffles and publishes it
 //   warps 1..NGATHER    gather warps: gw owns every NGATHER-th stage; source indices two stages ahead in
 //                       registers, 12 LDGSTS per 24-rating stage into the raw ring (rows padded to 288 bytes),
 //                       completion by cp.async.mbarrier.arrive.noinc
 //   next NCONV warps    converters: cw owns the stages whose number inside their segment is cw mod NCONV: LDS.128
-//                       of the raw rows, scale, hi/lo split, 24 conflict-free STS.128 into the UMMA stage ring,
+//                       of the raw rows, scale, hi/lo split, 96 conflict-free STS.32 into the wgmma stage ring,
 //                       fence.proxy.async, arrive on full[stage]; right-hand side b reduced at segment ends
-//   last 4*NTEAM warps  teams of four warps (one per TMEM lane quarter): drain the four accumulators of their
-//                       batch (tcgen05.ld: two warps store HH, two add LH and then its transpose), then each
-//                       warp Cholesky-solves one of the four rows (chol_solve_warp<PACKED_IN>), or - split mode -
-//                       stores the normal equations for als_solve_packed_kernel.
-// A batch = up to four (row, rating-segment) pairs, one per TMEM accumulator (64 columns each); rows longer
-// than SEG ratings are accumulated segment by segment with fp32 adds in shared memory between segments (bounds
-// the length of any single tensor-core accumulation chain).  Every sum has a fixed order that depends on the
-// row alone, so results do not depend on the grid or on how rows are sharded over GPUs.
+//   last 4*NTEAM warps  teams of four warps = one warpgroup each: issue the wgmmas of their batch stage by stage
+//                       (the stage is released when they complete), add the accumulator of every finished
+//                       segment into its A slot in shared memory, then each warp Cholesky-solves one of the four
+//                       rows (chol_solve_warp<PACKED_IN>), or - split mode - stores the normal equations for
+//                       als_solve_packed_kernel.  While one team solves, the other one consumes the stages.
+// A batch = up to four (row, rating-segment) pairs, accumulated one after the other; rows longer than SEG ratings
+// take several batches.  Every sum has a fixed order that depends on the row alone, so results do not depend on the
+// grid or on how rows are sharded over GPUs.
 // Every blocking mbarrier wait has a watchdog (mbar_wait): a protocol error traps with a diagnostic.
 // This header is included once per role partition (pio_als.cu): TC_NS names the namespace, TC_NTEAM / TC_NCONV /
 // TC_NGATHER / TC_NSTAGE / TC_NRAW fix how the sixteen warps and the shared memory of the CTA are divided.
@@ -52,20 +47,21 @@ namespace pio {
 namespace TC_NS {
 
 constexpr int KP = 64;
-constexpr int NCOL = 128;                        // staged columns per rating: [hi | lo]
-constexpr int ACOL = 64;                         // TMEM columns of one accumulator
-constexpr int KB_RATINGS = 8;                    // K of one tf32 MMA
-constexpr int KB_BYTES = KB_RATINGS * NCOL * 4;  // 4096
+constexpr int KB_RATINGS = 8;                    // K of one tf32 wgmma
+constexpr int CORE_K_BYTES = 144;                // leading byte offset: the second 4-rating core matrix of a feature group
+constexpr int CORE_M_BYTES = 288;                // stride byte offset: the next group of 8 features
+constexpr int TILE_BYTES = (KP / 8) * CORE_M_BYTES;   // one 64 x 8 operand tile (hi or lo): 2304
+constexpr int KB_BYTES = 2 * TILE_BYTES;         // hi tile, lo tile: 4608
 constexpr int STAGE_KB = 3;                      // one K-block per producer warp
 constexpr int STAGE_RATINGS = STAGE_KB * KB_RATINGS;  // 24
-constexpr int STAGE_BYTES = STAGE_KB * KB_BYTES;      // 12288
-constexpr int NSTAGE = TC_NSTAGE;                 // UMMA stage ring
+constexpr int STAGE_BYTES = STAGE_KB * KB_BYTES;      // 13824
+constexpr int NSTAGE = TC_NSTAGE;                 // wgmma stage ring
 constexpr int NRAW = TC_NRAW;                          // raw ring: stages of gathered rows in flight
 constexpr int RAW_ROW = 288;                     // bytes per gathered row in the raw ring (256 + 32 pad: conflict-free LDS.128)
 constexpr int NGATHER = TC_NGATHER;                       // gather warps (each owns every NGATHER-th stage)
 constexpr int NCONV = TC_NCONV;                         // converter warps (each owns every NCONV-th stage)
 constexpr int CONV0 = 1 + NGATHER;               // first converter warp
-constexpr int TEAM0 = CONV0 + NCONV;             // first drain+solve warp (a multiple of 4: warp%4 = TMEM lane quarter = slot)
+constexpr int TEAM0 = CONV0 + NCONV;             // first team warp (a multiple of 4: every team is one warpgroup)
 static_assert(TEAM0 % 4 == 0, "team warps must start at a multiple of four");
 constexpr int SEG = 21 * STAGE_RATINGS;          // 504 ratings per accumulation segment
 constexpr int NTEAM = TC_NTEAM;                   // drain + solve teams of four warps
@@ -78,7 +74,7 @@ constexpr int OFF21 = H * (H + 1) / 2;           // 528
 constexpr int OFF22 = OFF21 + H * L21S;          // 1680
 constexpr int ASLOT = OFF22 + H * (H + 1) / 2;   // 2208 floats
 
-// one UMMA stage (<= 24 ratings of one segment), pre-expanded by the scheduler so producers need no bookkeeping
+// one wgmma stage (<= 24 ratings of one segment), pre-expanded by the scheduler so producers need no bookkeeping
 struct StageEnt {
   long long beg;   // offset of the stage's first rating in idx/val
   int valid;       // ratings in this stage (1..24)
@@ -91,14 +87,14 @@ struct BatchDesc {
   int first[NSLOT];  // segment starts its row (overwrite the A slot instead of accumulating)
   int last[NSLOT];   // segment ends its row (solve after draining)
   int exit;
-  int seq;           // global batch number (selects the TMEM accumulator set)
+  unsigned stage0;   // global number of the batch's first stage (ring slot stage0 % NSTAGE)
   int nstages;
   int pad;
   StageEnt st[MAX_STAGES];
 };
 
 struct Smem {
-  alignas(1024) unsigned char stage[NSTAGE][STAGE_BYTES];
+  alignas(128) unsigned char stage[NSTAGE][STAGE_BYTES];
   alignas(16) float aslot[NTEAM][NSLOT][ASLOT];
   alignas(16) float bslot[NTEAM][NSLOT][KP];
   alignas(16) float bstage[NTEAM][2][NSLOT][KP];
@@ -109,15 +105,12 @@ struct Smem {
   alignas(16) float dinv[NTEAM * NSLOT][KP];
   BatchDesc desc[NTEAM][2];   // double-buffered per team: batch n+1 is produced while the team still solves batch n
   alignas(8) unsigned long long full[NSTAGE];
-  unsigned long long empty[NSTAGE];
   unsigned long long descfull[NTEAM][2];
-  unsigned long long accfull[NTEAM][2];
   unsigned long long teamdone[NTEAM][2];
   unsigned long long bfull[NTEAM][2];
-  unsigned long long tmemfree[2];
   unsigned long long rawfull[NRAW];    // gather warp -> converters (transaction-count barrier)
   unsigned long long rawempty[NRAW];   // converters -> gather warp
-  unsigned int tmem_base;
+  unsigned consumed;   // stages whose wgmmas have completed; the teams consume the ring strictly in stage order
 };
 
 // ---- PTX wrappers -------------------------------------------------------------------------
@@ -144,8 +137,9 @@ __device__ __forceinline__ bool mbar_try(unsigned long long* bar, uint32_t parit
 // Blocking wait with a watchdog: a protocol error must end the kernel with a diagnostic, never hang the GPU.
 __device__ __noinline__ void mbar_timeout(unsigned long long* bar, uint32_t parity) {
   extern __shared__ __align__(1024) unsigned char tc_smem_base_[];
-  if ((threadIdx.x & 31) == 0) printf("pio tc kernel: mbarrier wait timed out: cta %d warp %d lane %d barrier word %d (full4 empty4 descfull6 accfull6 teamdone6 bfull6 tmemfree2 rawfull6 rawempty6) parity %u\n", (int)blockIdx.x,
-         (int)(threadIdx.x >> 5), (int)(threadIdx.x & 31), (int)(s32(bar) - s32(tc_smem_base_) - (uint32_t)offsetof(Smem, full)) / 8, parity);
+  if ((threadIdx.x & 31) == 0) printf("pio tc kernel: mbarrier wait timed out: cta %d warp %d lane %d barrier word %d (full%d descfull%d teamdone%d bfull%d rawfull%d rawempty%d) parity %u\n", (int)blockIdx.x,
+         (int)(threadIdx.x >> 5), (int)(threadIdx.x & 31), (int)(s32(bar) - s32(tc_smem_base_) - (uint32_t)offsetof(Smem, full)) / 8,
+         NSTAGE, 2 * NTEAM, 2 * NTEAM, 2 * NTEAM, NRAW, NRAW, parity);
   __trap();
 }
 __device__ __forceinline__ void mbar_wait(unsigned long long* bar, uint32_t parity) {
@@ -153,6 +147,31 @@ __device__ __forceinline__ void mbar_wait(unsigned long long* bar, uint32_t pari
   const long long t0 = clock64();
   while (!mbar_try(bar, parity)) {
     if (clock64() - t0 > 16000000000ll) mbar_timeout(bar, parity);   // ~8 s (a half-step takes tens of ms; tools like compute-sanitizer slow the kernel ~100x)
+  }
+}
+// the consumed-stage counter: written by one thread of the consuming team (release), polled by converters and teams
+// (acquire).  Counting instead of a parity barrier per slot: a waiter may be several laps of the ring ahead of the
+// stage it needs, which a phase parity cannot tell apart.
+__device__ __forceinline__ uint32_t ld_acquire(const unsigned* p) {
+  uint32_t v;
+  asm volatile("ld.acquire.cta.shared::cta.u32 %0, [%1];" : "=r"(v) : "r"(s32(p)) : "memory");
+  return v;
+}
+__device__ __forceinline__ void st_release(unsigned* p, uint32_t v) {
+  asm volatile("st.release.cta.shared::cta.u32 [%0], %1;" ::"r"(s32(p)), "r"(v) : "memory");
+}
+// until *cnt >= target (wrap-safe), with the same watchdog as mbar_wait
+__device__ __forceinline__ void wait_count(const unsigned* cnt, uint32_t target) {
+  if ((int)(ld_acquire(cnt) - target) >= 0) return;
+  const long long t0 = clock64();
+  while ((int)(ld_acquire(cnt) - target) < 0) {
+    __nanosleep(100);
+    if (clock64() - t0 > 16000000000ll) {
+      if ((threadIdx.x & 31) == 0)
+        printf("pio tc kernel: stage count wait timed out: cta %d warp %d count %u target %u\n", (int)blockIdx.x,
+               (int)(threadIdx.x >> 5), ld_acquire(cnt), target);
+      __trap();
+    }
   }
 }
 __device__ __forceinline__ bool mbar_test(unsigned long long* bar, uint32_t parity) {
@@ -170,39 +189,30 @@ __device__ __forceinline__ bool mbar_test(unsigned long long* bar, uint32_t pari
 }
 __device__ __forceinline__ void fence_barrier_init() { asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
 __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tmem_alloc(unsigned int* dst_smem, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(s32(dst_smem)), "r"(ncols) : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void umma_tf32(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accum) {
+// warpgroup-wide wgmma plumbing: fence before the first wgmma that touches registers written by other instructions,
+// commit the issued wgmmas as one group, wait until none is pending
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_wait_all() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
+// keeps the compiler from moving accesses of an accumulator register across the asynchronous wgmma
+__device__ __forceinline__ void acc_fence(float& r) { asm volatile("" : "+f"(r)::"memory"); }
+// D[m][n] (+)= sum_k A[m][k] B[n][k] over one K-block of 8 ratings: m64n64k8, tf32 operands from shared memory,
+// fp32 accumulator in the registers of the warpgroup (warp w holds rows 16w..16w+15; see drain below)
+__device__ __forceinline__ void wgmma_tf32(float (&d)[32], uint64_t adesc, uint64_t bdesc, uint32_t accum) {
   asm volatile(
       "{\n"
       ".reg .pred p;\n"
-      "setp.ne.b32 p, %4, 0;\n"
-      "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n"
-      "}" ::"r"(tmem_d),
-      "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accum)
+      "setp.ne.b32 p, %34, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n64k8.f32.tf32.tf32 "
+      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, "
+      "%32, %33, p, 1, 1;\n"
+      "}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]),
+        "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]),
+        "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]),
+        "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "l"(adesc), "l"(bdesc), "r"(accum)
       : "memory");
-}
-__device__ __forceinline__ void umma_commit(unsigned long long* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(s32(bar)) : "memory");
-}
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, float (&v)[16]) {
-  uint32_t r[16];
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr)
-      : "memory");
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-  for (int i = 0; i < 16; ++i) v[i] = __uint_as_float(r[i]);
 }
 // the mbarrier receives one arrival from this thread once all of its earlier cp.async copies have landed
 __device__ __forceinline__ void cp_async_mbar_arrive_noinc(unsigned long long* bar) {
@@ -234,18 +244,6 @@ __device__ __forceinline__ void cp_async_wait_dyn(uint32_t pend) {
     default: cp_async_wait<8>(); break;
   }
 }
-__device__ __forceinline__ void tmem_ld16_nowait(uint32_t taddr, float* v) {
-  uint32_t r[16];
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr)
-      : "memory");
-#pragma unroll
-  for (int i = 0; i < 16; ++i) v[i] = __uint_as_float(r[i]);
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void named_bar_sync(int id, int nthreads) {
   asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
 }
@@ -257,23 +255,20 @@ __device__ __forceinline__ float tf32_round(float x) {
   return __uint_as_float(__float_as_uint(x) & 0xFFFFE000u);
 }
 
-// shared-memory matrix descriptor (cute/arch/mma_sm100_desc.hpp SmemDescriptor): MN-major,
-// layout_type SWIZZLE_128B_BASE32B = 1 at [61,64); start address >> 4 at [0,14); LBO = stride between
-// 32-column atoms (1024 B) >> 4 at [16,30); SBO = stride between groups of 4 ratings (512 B) >> 4 at [32,46);
-// version 1 at [46,48).  Element (rating k, column mn) of a K-block sits at
-//   (mn/32)*1024 + k*128 + ((((mn%32)/8) ^ (k%4)) * 32) + (mn%8)*4      (tools/umma_probe.cu: exact).
+// wgmma shared-memory matrix descriptor, K-major without swizzle: start address >> 4 at [0,14); leading byte offset
+// (between the two 4-rating core matrices of a K-block) >> 4 at [16,30); stride byte offset (between groups of 8
+// features) >> 4 at [32,46); layout type 0 (no swizzle) at [62,64).  Element (feature f, rating k) of a 64 x 8 tile
+// sits at  (f/8)*CORE_M_BYTES + (k/4)*CORE_K_BYTES + (f%8)*16 + (k%4)*4.
 __device__ __forceinline__ uint64_t make_desc(uint32_t smem_addr) {
   uint64_t d = 0;
   d |= (uint64_t)((smem_addr >> 4) & 0x3FFF);
-  d |= (uint64_t)((1024 >> 4) & 0x3FFF) << 16;
-  d |= (uint64_t)((512 >> 4) & 0x3FFF) << 32;
-  d |= (uint64_t)1 << 46;
-  d |= (uint64_t)1 << 61;
+  d |= (uint64_t)((CORE_K_BYTES >> 4) & 0x3FFF) << 16;
+  d |= (uint64_t)((CORE_M_BYTES >> 4) & 0x3FFF) << 32;
   return d;
 }
-// instruction descriptor (cute/arch/mma_sm100_desc.hpp InstrDescriptor): c_format F32 = 1 at [4,6),
-// a/b format TF32 = 2 at [7,10)/[10,13), a/b major MN = 1 at bits 15/16, N>>3 at [17,23), M>>4 at [24,29).
-constexpr uint32_t IDESC = (1u << 4) | (2u << 7) | (2u << 10) | (1u << 15) | (1u << 16) | ((64u >> 3) << 17) | ((128u >> 4) << 24);   // M = 128 ([hi|lo] columns), N = 64 (hi columns)
+__device__ __forceinline__ int tile_off(int f, int k) {
+  return (f >> 3) * CORE_M_BYTES + (k >> 2) * CORE_K_BYTES + (f & 7) * 16 + (k & 3) * 4;
+}
 
 static_assert(sizeof(Smem) + 1024 <= 232448, "shared memory budget (227 KB) exceeded");
 
@@ -291,15 +286,15 @@ __global__ void __launch_bounds__(NTHREADS, 1) als_solve_tc_kernel(const TcParam
   // direct cast (no integer round-trip) so the compiler keeps the shared address space: LDS/STS, not generic LD/ST
   extern __shared__ __align__(1024) unsigned char smem_raw[];
   Smem& sm = *reinterpret_cast<Smem*>(smem_raw);
-  if (threadIdx.x == 0 && (s32(smem_raw) & 1023u) != 0u) __trap();   // UMMA swizzle atoms need 1 KB alignment
+  if (threadIdx.x == 0 && (s32(smem_raw) & 127u) != 0u) __trap();   // the stage ring is laid out for 128-byte alignment
   const SolveParams& p = tp.sp;
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
 
   if (tid == 0) {
     for (int i = 0; i < NSTAGE; ++i) {
       mbar_init(&sm.full[i], 1);
-      mbar_init(&sm.empty[i], 1);
     }
+    sm.consumed = 0;
     for (int i = 0; i < NRAW; ++i) {
       mbar_init(&sm.rawfull[i], 32);   // every lane of the gather warp: cp.async.mbarrier.arrive.noinc
       mbar_init(&sm.rawempty[i], 1);
@@ -307,19 +302,12 @@ __global__ void __launch_bounds__(NTHREADS, 1) als_solve_tc_kernel(const TcParam
     for (int t = 0; t < NTEAM; ++t)
       for (int bf = 0; bf < 2; ++bf) {
         mbar_init(&sm.descfull[t][bf], 1);
-        mbar_init(&sm.accfull[t][bf], 1);
         mbar_init(&sm.teamdone[t][bf], NSLOT);
         mbar_init(&sm.bfull[t][bf], 1);
       }
-    mbar_init(&sm.tmemfree[0], NSLOT);
-    mbar_init(&sm.tmemfree[1], NSLOT);
     fence_barrier_init();
   }
-  if (warp == 0) tmem_alloc(&sm.tmem_base, 512);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = sm.tmem_base;
 
   long long tacc[8] = {0, 0, 0, 0, 0, 0, 0, 0};
   // per-role cycle counters are compiled in only with -DPIO_TC_TIMING=1 (tools/tc_timing.py); the default build carries no
@@ -330,11 +318,8 @@ __global__ void __launch_bounds__(NTHREADS, 1) als_solve_tc_kernel(const TcParam
 #define T_END(i) do { if (timing) tacc[i] += clock64() - t0_; } while (0)
   const long long tstart_ = timing ? clock64() : 0;
 
-  // register rebalancing: scheduler/producer warpgroup gives registers to the three drain+solve warpgroups
-  // (setmaxnreg rebalancing was tried and removed: shrinking the producer warpgroup forced its state into local memory)
-
   if (warp == 0) {
-    // ================= scheduler + MMA issuer =================
+    // ================= scheduler =================
     // Warp-parallel: lane li = t*4+s (< 12) keeps the state of row lane (team t, slot s) in registers; every control
     // decision is warp-uniform.  Static row assignment (no atomics): rows are degree-sorted; groups of 12 consecutive
     // rows are dealt to the CTAs in snake order, lane li of this CTA takes row  g*12 + li  of its k-th group g.  The row
@@ -357,15 +342,8 @@ __global__ void __launch_bounds__(NTHREADS, 1) als_solve_tc_kernel(const TcParam
     if (nx_row >= 0) { nx_beg = p.ptr[nx_row]; nx_end = p.ptr[nx_row + 1]; }
     uint32_t exited = 0;
     uint32_t nbp = 0;                // batches published per team, 8 bits each (only the low two bits are ever used)
-    uint32_t it = 0;                 // global stage counter
-    uint32_t nmma_batches = 0;
-    uint32_t nbuilt = 0;             // batches with work, in publish order == MMA order
+    uint32_t it = 0;                 // global stage counter: stages are produced and consumed in publish order
     auto nb_of = [&](int t) -> int { return (int)((nbp >> (8 * t)) & 3u); };
-    // batch n of team t lives in buffer n&1; the buffer is free once batch n-2 (its previous user) is done
-    auto team_free = [&](int t) -> bool {
-      const int n = nb_of(t);
-      return mbar_test(&sm.teamdone[t][n & 1], ((n >> 1) & 1) ^ 1);
-    };
     // publish the next batch of team t; returns false when the team has nothing left (an exit descriptor is published)
     auto build = [&](int t) -> bool {
       const int nbt = nb_of(t);
@@ -435,9 +413,9 @@ __global__ void __launch_bounds__(NTHREADS, 1) als_solve_tc_kernel(const TcParam
       if (lane == 0) {
         d.nstages = ns;
         d.exit = any ? 0 : 1;
-        d.seq = any ? (int)nbuilt : 0;
+        d.stage0 = it;
       }
-      if (any) ++nbuilt;
+      it += (uint32_t)ns;
       __syncwarp();
       if (lane == 0) mbar_arrive(&sm.descfull[t][bf]);
       nbp = (nbp & ~(0xffu << (8 * t))) | ((((nbp >> (8 * t)) + 1u) & 3u) << (8 * t));
@@ -445,77 +423,16 @@ __global__ void __launch_bounds__(NTHREADS, 1) als_solve_tc_kernel(const TcParam
       T_END(3);
       return any;
     };
-    // software pipeline: the descriptor of batch b+1 is published before the MMAs of batch b are issued,
-    // unless b+1 belongs to the same team as b (then its teamdone can only complete after b's MMAs).
-    int b = 0;
-    bool have[2] = {false, false};
-    int team_of[2] = {0, 0};
-    int buf_of[2] = {0, 0};
+    // teams in round-robin order, skipping those that have exited (the producers walk the descriptors in the same
+    // order); build() waits until the team's descriptor buffer is free, i.e. its batch before last is solved
     int cursor = 0;
-    auto next_team = [&]() -> int {
-      for (int k = 0; k < NTEAM; ++k) {
-        const int t = (cursor + k) % NTEAM;
-        if (!((exited >> t) & 1u)) return t;
-      }
-      return -1;
-    };
-    // returns true when publishing for slot `nxt` is settled (a batch was found or every team exited)
-    auto try_publish = [&](int cur, int nxt, bool allow_cur) -> bool {
-      while (true) {
-        const int t = next_team();
-        if (t < 0) return true;
-        if (!allow_cur && have[cur] && !team_free(t)) return false;  // do not stall the MMAs of `cur`
-        cursor = (t + 1) % NTEAM;
-        team_of[nxt] = t;
-        buf_of[nxt] = nb_of(t) & 1;
-        if (build(t)) { have[nxt] = true; return true; }
-      }
-    };
-    try_publish(1, 0, true);
     while (true) {
-      const int cur = b & 1, nxt = cur ^ 1;
-      have[nxt] = false;
-      const bool settled = try_publish(cur, nxt, false);
-      if (have[cur]) {
-        const int t = team_of[cur];
-        const BatchDesc& d = sm.desc[t][buf_of[cur]];
-        const uint32_t set = nmma_batches & 1;                         // TMEM accumulator set of this batch
-        T_BEGIN();
-        mbar_wait(&sm.tmemfree[set], ((nmma_batches >> 1) & 1) ^ 1);   // batch b-2 (same set) has been drained
-        T_END(1);
-        tc_fence_after();
-        const int nstg = d.nstages;
-        for (int i = 0; i < nstg; ++i, ++it) {
-          const int st = it % NSTAGE;
-          const int valid = d.st[i].valid;
-          const int info = d.st[i].info;
-          T_BEGIN();
-          mbar_wait(&sm.full[st], (it / NSTAGE) & 1);
-          T_END(2);
-          tc_fence_after();
-          T_BEGIN();
-          if (lane == 0) {
-            const int nkb = (valid + KB_RATINGS - 1) / KB_RATINGS;
-            const uint32_t base = s32(&sm.stage[st][0]);
-            const uint32_t acc = tmem + set * (NSLOT * ACOL) + (info & 3) * ACOL;
-            for (int kb = 0; kb < nkb; ++kb) {
-              // A = all 128 staged columns [hi | lo] (M = 128), B = the 64 hi columns (N = 64):
-              // D rows 0..63 = hi^T hi, rows 64..127 = lo^T hi; the drain adds lo^T hi and its transpose to hi^T hi
-              const uint64_t dh = make_desc(base + kb * KB_BYTES);
-              umma_tf32(acc, dh, dh, IDESC, ((info & 16) && kb == 0) ? 0u : 1u);
-            }
-            umma_commit(&sm.empty[st]);
-          }
-          __syncwarp();
-          T_END(4);
-        }
-        if (lane == 0) umma_commit(&sm.accfull[t][buf_of[cur]]);
-        __syncwarp();
-        ++nmma_batches;
-      }
-      if (!settled) try_publish(cur, nxt, true);
-      if (!have[nxt]) break;
-      ++b;
+      int t = -1;
+      for (int k = 0; k < NTEAM && t < 0; ++k)
+        if (!((exited >> ((cursor + k) % NTEAM)) & 1u)) t = (cursor + k) % NTEAM;
+      if (t < 0) break;
+      cursor = (t + 1) % NTEAM;
+      build(t);
     }
     __syncwarp();
   } else if (warp < TEAM0) {
@@ -524,8 +441,8 @@ __global__ void __launch_bounds__(NTHREADS, 1) als_solve_tc_kernel(const TcParam
     //          copy per rating into the raw ring (completion counted on rawfull[]); source indices are loaded
     //          two stages ahead into a register shift queue.
     // converters: converter cw owns the stages whose number inside their segment is cw mod NCONV: it waits for the
-    //          raw rows, scales, splits hi/lo and writes all three K-blocks of the UMMA tile (three independent
-    //          pieces of work per dependency chain), then hands the stage to the MMA issuer.
+    //          raw rows, scales, splits hi/lo and writes all three K-blocks of the wgmma tiles (three independent
+    //          pieces of work per dependency chain), then hands the stage to the team that consumes it.
     // cursor over the published stage lists (scalars only)
     uint32_t c_ex = 0, c_par = 0;
     int c_cur = 0, c_t = 0, c_b = 0, c_i = -1, c_n = 0;
@@ -601,6 +518,9 @@ __global__ void __launch_bounds__(NTHREADS, 1) als_solve_tc_kernel(const TcParam
         if (qval1 < 0) fetch(qn1, qbeg1, qval1, qidx1, false);
         const int rs = qn0 % NRAW;
         T_BEGIN();
+        // the slot's previous use (stage qn0 - NRAW) must have been loaded by its converter; waiting for the consumption of
+        // stage qn0 - 2 NRAW first keeps this wait less than one lap ahead of the slot, so its parity is unambiguous
+        wait_count(&sm.consumed, qn0 + 1 - 2 * NRAW);
         mbar_wait(&sm.rawempty[rs], ((qn0 / NRAW) & 1) ^ 1);   // the converter is done with this raw slot
         T_END(1);
         T_BEGIN();
@@ -624,7 +544,7 @@ __global__ void __launch_bounds__(NTHREADS, 1) als_solve_tc_kernel(const TcParam
       // (kr%4 = 0..3) x 2 halves of one 32-byte chunk -> its 8 STS.128 hit 8 distinct 16-byte bank groups
       const int kr = ((lane >> 3) & 1) * 4 + (lane & 3);
       const int sgb = ((lane >> 2) & 1) + 2 * (lane >> 4);
-      uint32_t it = 0;   // global stage counter (UMMA ring + raw ring)
+      uint32_t it = 0;   // global stage counter (wgmma ring + raw ring)
       uint32_t qs = 0;   // stage number inside the current segment: decides the owner, so that the grouping of a row's
                          // right-hand-side partial sums depends on the row alone (not on what else this CTA processes)
       float bacc[4][4];
@@ -645,6 +565,7 @@ __global__ void __launch_bounds__(NTHREADS, 1) als_solve_tc_kernel(const TcParam
           const int rs = it % NRAW;
           const int st = it % NSTAGE;
           T_BEGIN();
+          wait_count(&sm.consumed, it + 1 - NRAW);             // stage it - NRAW has landed (keeps the parity below unambiguous)
           mbar_wait(&sm.rawfull[rs], (it / NRAW) & 1);           // gathered rows have landed
           T_END(1);
           T_BEGIN();
@@ -668,7 +589,7 @@ __global__ void __launch_bounds__(NTHREADS, 1) als_solve_tc_kernel(const TcParam
           if (lane == 0) mbar_arrive(&sm.rawempty[rs]);
           T_END(3);
           T_BEGIN();
-          mbar_wait(&sm.empty[st], ((it / NSTAGE) & 1) ^ 1);     // UMMA stage is free
+          wait_count(&sm.consumed, it + 1 - NSTAGE);            // wgmma stage is free: stage it - NSTAGE consumed
           T_END(2);
           T_BEGIN();
 #pragma unroll
@@ -684,11 +605,14 @@ __global__ void __launch_bounds__(NTHREADS, 1) als_solve_tc_kernel(const TcParam
                 wb = cval;
                 sc = 1.f;
               }
-              unsigned char* kbp = &sm.stage[st][0] + kb * KB_BYTES + kr * 128;
+              unsigned char* kbp = &sm.stage[st][0] + kb * KB_BYTES;
 #pragma unroll
               for (int j = 0; j < 4; ++j) {
                 const int sg = sgb + 4 * j;
-                const int off = (sg >> 3) * 1024 + ((((sg & 7) >> 1) ^ (kr & 3)) * 32) + (sg & 1) * 16;
+                // features 4sg..4sg+3 of rating kr: four 4-byte stores 16 bytes apart; over the warp the rating halves
+                // (144 B = 4 banks apart), feature groups (288 B = 8 banks) and sgb parity (64 B = 16 banks) spread
+                // the 32 lanes over 32 distinct banks
+                const int off = tile_off(4 * sg, kr);
                 const float4 yy = y[kb][j];
                 bacc[j][0] = fmaf(wb, yy.x, bacc[j][0]);
                 bacc[j][1] = fmaf(wb, yy.y, bacc[j][1]);
@@ -699,8 +623,10 @@ __global__ void __launch_bounds__(NTHREADS, 1) als_solve_tc_kernel(const TcParam
                 float4 hi, lo;
                 hi.x = tf32_round(x.x); hi.y = tf32_round(x.y); hi.z = tf32_round(x.z); hi.w = tf32_round(x.w);
                 lo.x = x.x - hi.x; lo.y = x.y - hi.y; lo.z = x.z - hi.z; lo.w = x.w - hi.w;
-                *reinterpret_cast<float4*>(kbp + off) = hi;          // columns 4sg..4sg+3 of the hi half
-                *reinterpret_cast<float4*>(kbp + 2048 + off) = lo;   // same columns of the lo half (mn + 64)
+                float* ph = reinterpret_cast<float*>(kbp + off);
+                float* pl = reinterpret_cast<float*>(kbp + TILE_BYTES + off);
+                ph[0] = hi.x; ph[4] = hi.y; ph[8] = hi.z; ph[12] = hi.w;
+                pl[0] = lo.x; pl[4] = lo.y; pl[8] = lo.z; pl[12] = lo.w;
               }
             }
           }
@@ -750,11 +676,27 @@ __global__ void __launch_bounds__(NTHREADS, 1) als_solve_tc_kernel(const TcParam
       }
     }
   } else {
-    // ================= teams: drain + solve =================
+    // ================= teams: wgmma + solve =================
     const int t = (warp - TEAM0) / 4;
     const int slot = (warp - TEAM0) % 4;     // the row this warp solves
-    const int q = warp & 3;              // TMEM lane quarter this warp may read
+    const int wq = warp & 3;                 // rank of this warp in its warpgroup: accumulator rows 16wq..16wq+15
     const int barid = 2 + t;
+    float acc[32];
+#pragma unroll
+    for (int i = 0; i < 32; ++i) acc[i] = 0.f;
+    // accumulator -> A slot (packed lower triangle, as chol_solve_warp<PACKED_IN> reads it), overwriting for the first
+    // stage of a row, adding otherwise.  Fragment of m64n64: acc[i] is row 16wq + lane/4 + 8((i/2)%2), column
+    // 8(i/4) + 2(lane%4) + i%2; every element has one owner thread, so the adds need no synchronisation.
+    auto drain = [&](float* as, bool overwrite) {
+#pragma unroll
+      for (int i = 0; i < 32; ++i) {
+        const int r = 16 * wq + (lane >> 2) + 8 * ((i >> 1) & 1);
+        const int c = 8 * (i >> 2) + 2 * (lane & 3) + (i & 1);
+        if (c > r) continue;
+        const int o = r < H ? r * (r + 1) / 2 + c : (c < H ? OFF21 + (r - H) * L21S + c : OFF22 + (r - H) * (r - H + 1) / 2 + (c - H));
+        as[o] = overwrite ? acc[i] : as[o] + acc[i];
+      }
+    };
     int nb = 0;
     while (true) {
       const int bf = nb & 1;
@@ -764,90 +706,48 @@ __global__ void __launch_bounds__(NTHREADS, 1) als_solve_tc_kernel(const TcParam
       T_END(0);
       const BatchDesc& d = sm.desc[t][bf];
       if (d.exit) break;
-      T_BEGIN();
-      mbar_wait(&sm.accfull[t][bf], ph);
-      T_END(1);
-      tc_fence_after();
       // every warp of the team must have finished solving the previous batch before any A slot is overwritten
       named_bar_sync(barid, 128);
-      T_BEGIN();
-      // ---- drain: the accumulator is 128 lanes x 64 columns: lane r < 64 = row r of hi^T hi, lane 64 + r = row r of
-      // lo^T hi (LH).  A = HH + LH + LH^T: warps q = 0,1 store/accumulate their HH rows, then warps q = 2,3 add the lower
-      // part of their LH rows, then (after a team barrier) its transpose - a fixed order, so the sums are deterministic.
-      const uint32_t set = (uint32_t)d.seq & 1u;
-      const int drow = (q & 1) * 32 + lane;
-      auto load_slot = [&](int s, float* v) {
-        const uint32_t taddr = tmem + ((uint32_t)(q * 32) << 16) + set * (NSLOT * ACOL) + (uint32_t)(s * ACOL);
-        tmem_ld16_nowait(taddr, &v[0]);
-        tmem_ld16_nowait(taddr + 16, &v[16]);
-        tmem_ld16_nowait(taddr + 32, &v[32]);
-        tmem_ld16_nowait(taddr + 48, &v[48]);
-        tmem_ld_wait();
-      };
-      // row `drow` of a 64x64 block into the lower-triangle slot (columns <= drow), overwriting or accumulating
-      auto put_lower = [&](float* as, const float* v, bool overwrite) {
-        if (drow < H) {
-          float* rowp = as + drow * (drow + 1) / 2;
-#pragma unroll
-          for (int c = 0; c < H; ++c)
-            if (c <= drow) rowp[c] = overwrite ? v[c] : rowp[c] + v[c];
-        } else {
-          float4* r4 = reinterpret_cast<float4*>(as + OFF21 + (drow - H) * L21S);
-#pragma unroll
-          for (int c = 0; c < H; c += 4) {
-            float4 o = make_float4(v[c], v[c + 1], v[c + 2], v[c + 3]);
-            if (!overwrite) { const float4 e = r4[c / 4]; o.x += e.x; o.y += e.y; o.z += e.z; o.w += e.w; }
-            r4[c / 4] = o;
-          }
-          float* rowp = as + OFF22 + (drow - H) * (drow - H + 1) / 2;
-#pragma unroll
-          for (int c = 0; c < H; ++c)
-            if (c <= drow - H) rowp[c] = overwrite ? v[H + c] : rowp[c] + v[H + c];
+      // this batch's turn: every earlier stage has been consumed (by the other teams), so the slot of each of its stages
+      // is at most one lap ahead and the parity wait on full[] below is unambiguous
+      wait_count(&sm.consumed, d.stage0);
+      __syncwarp();
+      // ---- the batch's stages in order: slot 0's segment, then slot 1's, ...; every stage's sum goes into its slot's A
+      // (fp32 adds in stage order: deterministic)
+      const int nst = d.nstages;
+      for (int i = 0; i < nst; ++i) {
+        const uint32_t g = d.stage0 + (uint32_t)i;
+        const int st = (int)(g % NSTAGE);
+        const int valid = d.st[i].valid;
+        const int info = d.st[i].info;
+        T_BEGIN();
+        mbar_wait(&sm.full[st], (g / NSTAGE) & 1);
+        __syncwarp();   // wgmma is warp-synchronous: reconverge after the polling loop
+        T_END(1);
+        T_BEGIN();
+        const int nkb = (valid + KB_RATINGS - 1) / KB_RATINGS;
+        const uint32_t base = s32(&sm.stage[st][0]);
+        wgmma_fence();
+        for (int kb = 0; kb < nkb; ++kb) {   // the small cross terms first; the first wgmma of the stage starts from zero
+          const uint64_t dh = make_desc(base + kb * KB_BYTES);
+          const uint64_t dl = make_desc(base + kb * KB_BYTES + TILE_BYTES);
+          wgmma_tf32(acc, dl, dh, kb == 0 ? 0u : 1u);                      // lo hi^T
+          wgmma_tf32(acc, dh, dl, 1u);                                     // hi lo^T
         }
-      };
-      if (q < 2) {
-#pragma unroll 1
-        for (int s = 0; s < NSLOT; ++s) {
-          if (d.row[s] < 0) continue;
-          float v[64];
-          load_slot(s, v);
-          put_lower(&sm.aslot[t][s][0], v, d.first[s] != 0);
+        for (int kb = 0; kb < nkb; ++kb) {
+          const uint64_t dh = make_desc(base + kb * KB_BYTES);
+          wgmma_tf32(acc, dh, dh, 1u);                                     // hi hi^T
         }
-      }
-      named_bar_sync(barid, 128);
-      if (q >= 2) {
-#pragma unroll 1
-        for (int s = 0; s < NSLOT; ++s) {
-          if (d.row[s] < 0) continue;
-          float v[64];
-          load_slot(s, v);
-          put_lower(&sm.aslot[t][s][0], v, false);
-        }
-      }
-      named_bar_sync(barid, 128);
-      if (q >= 2) {
-#pragma unroll 1
-        for (int s = 0; s < NSLOT; ++s) {
-          if (d.row[s] < 0) continue;
-          float v[64];
-          load_slot(s, v);
-          float* as = &sm.aslot[t][s][0];
-          // transpose: LH[drow][c] (c >= drow) goes to A[c][drow]; consecutive lanes -> consecutive addresses
-          if (drow < H) {
+        wgmma_commit();
+        wgmma_wait_all();
 #pragma unroll
-            for (int c = 0; c < H; ++c)
-              if (c >= drow) as[c * (c + 1) / 2 + drow] += v[c];
-#pragma unroll
-            for (int c = H; c < KP; ++c) as[OFF21 + (c - H) * L21S + drow] += v[c];
-          } else {
-#pragma unroll
-            for (int c = H; c < KP; ++c)
-              if (c >= drow) as[OFF22 + (c - H) * (c - H + 1) / 2 + (drow - H)] += v[c];
-          }
-        }
+        for (int j = 0; j < 32; ++j) acc_fence(acc[j]);
+        named_bar_sync(barid, 128);                                      // no warp of the team reads the stage any more
+        if (wq == 0 && lane == 0) st_release(&sm.consumed, g + 1);
+        drain(&sm.aslot[t][info & 3][0], (info & 16) && d.first[info & 3] != 0);
+        T_END(2);
       }
       __syncwarp();
-      T_END(2);
       // right-hand side of this segment
       T_BEGIN();
       mbar_wait(&sm.bfull[t][bf], ph);
@@ -859,9 +759,6 @@ __global__ void __launch_bounds__(NTHREADS, 1) als_solve_tc_kernel(const TcParam
           if (d.row[s] >= 0) sm.bslot[t][s][c] = d.first[s] ? sm.bstage[t][bf][s][c] : sm.bslot[t][s][c] + sm.bstage[t][bf][s][c];
         }
       }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&sm.tmemfree[set]);
       T_BEGIN();
       named_bar_sync(barid, 128);
       T_END(4);
@@ -897,9 +794,6 @@ __global__ void __launch_bounds__(NTHREADS, 1) als_solve_tc_kernel(const TcParam
     tacc[7] = clock64() - tstart_;
     for (int i = 0; i < 8; ++i) tp.timing[((size_t)blockIdx.x * 16 + warp) * 8 + i] = tacc[i];
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 0) tmem_dealloc(tmem, 512);
 }
 
 // ---- split mode, second half: one warp per row solves the normal equations the tensor-core kernel left in `in`

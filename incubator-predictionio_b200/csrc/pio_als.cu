@@ -1,6 +1,6 @@
 // pio_als.cu -- C-ABI implementation (see include/pio_als.h for the reference interfaces each
 // entry point replaces).  Host orchestration only; all arithmetic is in the CUDA kernels of
-// als_kernels.cuh / sort_scan.cuh / topk.cuh.  No CPU fallback: without a usable sm_100 device
+// als_kernels.cuh / sort_scan.cuh / topk.cuh.  No CPU fallback: without a usable sm_90 device
 // every computing entry point returns PIO_ALS_ERR_CUDA.
 #include "../../include/pio_als.h"
 
@@ -23,14 +23,14 @@
 #include "als_kernels.cuh"
 #include "als_mma_kernel.cuh"
 #include "als_pair_kernel.cuh"
-// the tcgen05 half-step kernel; the header is parametrised by the role partition of its sixteen warps.  Measured at C2:
-// 2 gather + 5 converter warps + 2 solve teams (below) beats 1 + 2 + 3 teams on long rows AND on short rows (user side
-// 38 ms vs 86 ms: two converter warps cannot feed the MMAs), so only this partition is instantiated.
+// the wgmma half-step kernel; the header is parametrised by the role partition of its sixteen warps: 2 gather +
+// 5 converter warps + 2 teams (one warpgroup each, so that one team consumes stages while the other solves).  Six
+// wgmma stages and seven raw stages fill the 227 KB of shared memory a block may use.
 #define TC_NS tc
 #define TC_NTEAM 2
 #define TC_NCONV 5
 #define TC_NGATHER 2
-#define TC_NSTAGE 7
+#define TC_NSTAGE 6
 #define TC_NRAW 7
 #include "als_tc_kernel.cuh"
 #undef TC_NS
@@ -596,9 +596,9 @@ static int build_side(pio_als_handle* h, Side& row, const Side& col, const int* 
   // run and the single-GPU run take the same path for the same row
   row.use_tc = h->use_tc && h->KP == 64 && row.n > 0 && (double)nnz_global / (double)row.n >= h->tc_min_deg;
   row.use_pair = !row.use_tc && h->KP == 64 && h->use_mma && h->use_pair;
-  // one warp (mma kernels) or one accumulator slot (tcgen05 kernel) carries a whole row.  Pair kernel: rows up to 1024
+  // one warp (mma kernels) or one A slot (wgmma kernel) carries a whole row.  Pair kernel: rows up to 1024
   // ratings stay whole, longer rows become 512-rating parts of the same kernel (two-level summation); round-1 mma /
-  // tcgen05 kernels: rows up to 8192 ratings whole, longer rows as 2016-rating parts on the FP32 kernel; FP32 kernel
+  // wgmma kernels: rows up to 8192 ratings whole, longer rows as 2016-rating parts on the FP32 kernel; FP32 kernel
   // (other ranks): cut at 4096
   // rank 65..128: every row is a work-list row (FP32 Gramian kernel -> partial normal equations -> lockstep finish kernel)
   row.heavy_t = h->KP == 128 ? 0 : row.use_pair ? h->pair_seg_t : (row.use_tc || (h->KP == 64 && h->use_mma)) ? HEAVY_T_TC : HEAVY_T;
@@ -982,11 +982,10 @@ static cudaError_t launch_solve_one(pio_als_handle* h, const SolveParams& p, int
   return cudaGetLastError();
 }
 
-// Gramians on tcgen05 (als_tc_kernel.cuh): persistent, one CTA per SM, rows assigned statically.  A = role partition.
+// Gramians on wgmma (als_tc_kernel.cuh): persistent, one CTA per SM, rows assigned statically.  A = role partition.
 // Split mode (PIO_ALS_TC_SPLIT=1, off by default): the kernel only accumulates and stores the normal equations of a
-// tile of rows; a second kernel solves them with every warp of the SM.  Measured at C2: item side 15.0 vs 15.4 ms fused,
-// user side 39.7 vs 38.2 ms fused (the one-warp 64x64 Cholesky is latency-bound, ~50-70 k cycles per row, so twelve
-// solver warps per SM at 168 registers do not beat the fused ones overlapped with the MMAs).
+// tile of rows; a second kernel solves them with every warp of the SM (the one-warp 64x64 Cholesky is latency-bound,
+// so more solver warps per SM can help where the fused solves do not overlap the MMAs well).
 template <class A>
 static cudaError_t launch_tc(pio_als_handle* h, Side& dst, const SolveParams& p, bool imp, int nlight) {
   cudaError_t e = cudaSuccess;
@@ -1446,7 +1445,7 @@ int pio_als_device_count(void) {
   int ok = 0;
   for (int d = 0; d < n; ++d) {
     cudaDeviceProp pr;
-    if (cudaGetDeviceProperties(&pr, d) == cudaSuccess && pr.major == 10) ++ok;
+    if (cudaGetDeviceProperties(&pr, d) == cudaSuccess && pr.major == 9 && pr.minor == 0) ++ok;
   }
   return ok;
 }
@@ -1472,8 +1471,8 @@ static int create_common(pio_als_handle* h) {
   if (h->cfg.device < 0 || h->cfg.device >= ndev) return fail(nullptr, PIO_ALS_ERR_ARG, "bad device %d", h->cfg.device);
   cudaDeviceProp pr;
   if (cudaGetDeviceProperties(&pr, h->cfg.device) != cudaSuccess) return fail(nullptr, PIO_ALS_ERR_CUDA, "cudaGetDeviceProperties");
-  if (pr.major != 10)
-    return fail(nullptr, PIO_ALS_ERR_CUDA, "device %d is sm_%d%d; this library is built for sm_100a (B200) only",
+  if (pr.major != 9 || pr.minor != 0)
+    return fail(nullptr, PIO_ALS_ERR_CUDA, "device %d is sm_%d%d; this library is built for sm_90a (H100) only",
                 h->cfg.device, pr.major, pr.minor);
   h->sm_count = pr.multiProcessorCount;
   h->st.sm_count = pr.multiProcessorCount;
@@ -1511,9 +1510,9 @@ static int create_common(pio_als_handle* h) {
   }
   {
     // Rank 33..64 kernel selection.  Default: the pair kernel (als_pair_kernel.cuh: mma.sync 3xTF32 Gramian, two rows per
-    // warp, lockstep Cholesky) for every side -- measured at C2 it is the fastest on both sides (user half-step 18.7 ms,
-    // item half-step 12.9 ms vs 17.1 ms for the tcgen05 kernel) and, with rows above 1024 ratings summed in two
-    // levels, inside the parity bound on long rows.  PIO_ALS_TC=1: the tcgen05 Gramian kernel (als_tc_kernel.cuh) for
+    // warp, lockstep Cholesky) for every side -- every warp gathers, accumulates and solves, so it needs no producer
+    // warps -- and, with rows above 1024 ratings summed in two levels, it stays inside the parity bound on long rows.
+    // PIO_ALS_TC=1: the wgmma Gramian kernel (als_tc_kernel.cuh) for
     // every side (PIO_ALS_TC_MIN_DEG=n: only sides averaging >= n ratings per row); PIO_ALS_MMA=1: the round-1
     // one-warp-per-row mma.sync kernel; PIO_ALS_MMA=0: the FP32 CUDA-core kernel.
     const char* env = getenv("PIO_ALS_TC");
@@ -1758,7 +1757,7 @@ int pio_als_get_phase_ms(pio_als_handle* h, double out[8]) {
   if (!h || !out) return PIO_ALS_ERR_ARG;
   std::lock_guard<std::mutex> lk(h->mu);
   for (int i = 0; i < 8; ++i) out[i] = h->phase_ms[i];
-  // kernel of the rows below the heavy-row threshold: 0 = FP32 (als_solve_kernel), 1 = tcgen05, 2 = mma.sync
+  // kernel of the rows below the heavy-row threshold: 0 = FP32 (als_solve_kernel), 1 = wgmma, 2 = mma.sync
   const bool mma = h->KP == 64 && h->use_mma;
   out[4] = h->I.use_tc ? 1.0 : h->I.use_pair ? 3.0 : (mma ? 2.0 : 0.0);
   out[5] = h->U.use_tc ? 1.0 : h->U.use_pair ? 3.0 : (mma ? 2.0 : 0.0);

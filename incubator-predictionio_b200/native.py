@@ -2,7 +2,7 @@
 
 This is the Python stand-in for the JNI shim a ``native-als`` Scala module would carry
 (INTEGRATION.md): it only marshals host buffers and status codes; no arithmetic happens here
-and there is no CPU fallback -- if the CUDA library is missing or no B200 is visible every
+and there is no CPU fallback -- if the CUDA library is missing or no H100 is visible every
 call raises ``NativeError``.
 """
 from __future__ import annotations
@@ -35,7 +35,7 @@ EXPORTED_SYMBOLS = [
 ]
 
 
-_KERNEL_NAMES = {0: "fp32", 1: "tcgen05", 2: "mma", 3: "pair"}
+_KERNEL_NAMES = {0: "fp32", 1: "wgmma", 2: "mma", 3: "pair"}
 
 
 class NativeError(RuntimeError):
@@ -64,12 +64,12 @@ class Stats(C.Structure):
     ]
 
 
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17",
+NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
               "-Xcompiler", "-fPIC,-fvisibility=hidden", "-shared"]
 
 
 def build(force: bool = False, verbose: bool = False) -> Path:
-    """nvcc cross-compile of csrc/pio_als.cu for sm_100a into the in-tree libpio_als.so."""
+    """nvcc cross-compile of csrc/pio_als.cu for sm_90a (H100) into the in-tree libpio_als.so."""
     srcs = sorted(CSRC.glob("*.cu")) + sorted(CSRC.glob("*.cuh")) + [REPO_ROOT / "include" / "pio_als.h"]
     if LIB_PATH.exists() and not force and all(LIB_PATH.stat().st_mtime >= s.stat().st_mtime for s in srcs):
         return LIB_PATH

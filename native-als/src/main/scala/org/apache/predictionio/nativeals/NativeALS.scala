@@ -8,7 +8,7 @@
  *   ALS.trainImplicit(ratings, rank, iterations, lambda, -1, 1.0, seed)
  *                                           examples/scala-parallel-similarproduct/multi-events-multi-algos/src/main/scala/ALSAlgorithm.scala:121-128
  * and the same result fields the templates read (rank, userFeatures, productFeatures, recommendProducts).
- * All arithmetic happens in libpio_als.so (CUDA, sm_100a) behind the JNI shim src/main/c/pio_als_jni.c; this file only
+ * All arithmetic happens in libpio_als.so (CUDA, sm_90a) behind the JNI shim src/main/c/pio_als_jni.c; this file only
  * collects the ratings to primitive arrays and owns the native handle.
  */
 package org.apache.predictionio.nativeals

@@ -13,7 +13,7 @@ import pio_b200  # noqa: E402,F401  (registers the package under an importable n
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a real B200 (run with -m gpu on the GPU box)")
+    config.addinivalue_line("markers", "gpu: needs a real H100 (run with -m gpu on a machine that has one)")
 
 
 @pytest.fixture(scope="session")

@@ -1,5 +1,5 @@
 """CPU tests of the drop-in boundary: the C-ABI library loads, exports every symbol that
-include/pio_als.h declares, and fails loudly (no CPU fallback) when no B200 is visible."""
+include/pio_als.h declares, and fails loudly (no CPU fallback) when no H100 is visible."""
 import re
 from pathlib import Path
 
@@ -21,7 +21,7 @@ def test_library_exports_every_declared_symbol(native):
 
 def test_no_cpu_fallback_without_gpu(native):
     if native.device_count() > 0:
-        pytest.skip("a B200 is visible; the no-GPU failure path cannot be exercised")
+        pytest.skip("an H100 is visible; the no-GPU failure path cannot be exercised")
     with pytest.raises(native.NativeError) as ei:
         native.NativeALS(rank=10, n_users=10, n_items=10)
     assert ei.value.code == native.ERR_CUDA

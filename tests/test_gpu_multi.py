@@ -1,4 +1,4 @@
-"""Multi-GPU parity (-m gpu, needs >= 2 B200s; skipped otherwise): row-sharded training with the NCCL factor
+"""Multi-GPU parity (-m gpu, needs >= 2 H100s; skipped otherwise): row-sharded training with the NCCL factor
 all-gather gives bit-identical factors to the single-GPU run (every row's arithmetic is independent of the
 sharding), and therefore the same parity with the oracle."""
 import os
@@ -30,7 +30,7 @@ WORKER = textwrap.dedent("""
         dist.broadcast(t, 0)
         return bytes(t.cpu().tolist())
     # (rank, implicit, users, items, ratings, PIO_ALS_TC, dedup, sharded input): rank 64 runs the pair kernel (mma.sync +
-    # lockstep Cholesky) or, with PIO_ALS_TC=1, the tcgen05 kernel; the 30-item cases have heavy item rows (parts + finish
+    # lockstep Cholesky) or, with PIO_ALS_TC=1, the wgmma kernel; the 30-item cases have heavy item rows (parts + finish
     # kernels); rank 128 runs the FP32 Gramian + lockstep finish path.  sharded: every rank passes only its slice of the
     # events (pio_als_set_ratings_coo_sharded) -- the result must still be bit-identical to the single-GPU run.
     cases = ((64, True, 6000, 900, 150000, "", 1, False), (10, False, 3000, 500, 40000, "", 0, False),

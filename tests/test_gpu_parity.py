@@ -69,7 +69,7 @@ def test_trained_factors_within_tolerance(native, oracle, rank, implicit, iters)
 
 @pytest.mark.parametrize("implicit", [True, False])
 def test_tensor_core_gramian_path(native, oracle, monkeypatch, implicit):
-    """PIO_ALS_TC=1 routes every side of rank 33..64 through the tcgen05 split-TF32 SYRK kernel
+    """PIO_ALS_TC=1 routes every side of rank 33..64 through the wgmma split-TF32 SYRK kernel
     (als_tc_kernel.cuh): same tolerance, including rows longer than one 504-rating accumulation segment and > 8192
     (parts on the FP32 kernel + finish kernel)."""
     monkeypatch.setenv("PIO_ALS_TC", "1")
@@ -87,7 +87,7 @@ def test_tensor_core_gramian_path(native, oracle, monkeypatch, implicit):
 
 
 def test_tensor_core_split_mode_matches_fused(native, oracle, monkeypatch):
-    """PIO_ALS_TC_SPLIT=1: the tcgen05 kernel stores the normal equations and als_solve_packed_kernel solves them;
+    """PIO_ALS_TC_SPLIT=1: the wgmma kernel stores the normal equations and als_solve_packed_kernel solves them;
     same arithmetic as the fused kernel -> bit-identical factors."""
     monkeypatch.setenv("PIO_ALS_TC", "1")
     nu, ni, nnz = 30000, 60, 500000
@@ -144,7 +144,7 @@ def test_config_c1_recommendation_template(native, oracle):
     assert np.abs(pg - po).max() <= 1e-3 * max(1.0, np.abs(po).max())
 
 
-@pytest.mark.parametrize("path", ["fp32", "mma", "pair", "tcgen05"])
+@pytest.mark.parametrize("path", ["fp32", "mma", "pair", "wgmma"])
 def test_heavy_rows_split_mode(native, oracle, monkeypatch, path):
     """Items with far more ratings than the heavy-row threshold are cut into parts (pair kernel: 512-rating parts above
     1024 ratings, summed by als_finish_pair_kernel; the other kernels: 2016-rating parts on the FP32 kernel +
@@ -156,7 +156,7 @@ def test_heavy_rows_split_mode(native, oracle, monkeypatch, path):
         monkeypatch.setenv("PIO_ALS_MMA", "0")
     elif path == "mma":
         monkeypatch.setenv("PIO_ALS_MMA", "1")
-    elif path == "tcgen05":
+    elif path == "wgmma":
         monkeypatch.setenv("PIO_ALS_TC", "1")
     nu, ni, nnz = 20000, 40, 400000
     u, i, r = synth.synth_ratings(nu, ni, nnz, seed=9, implicit=True)
@@ -172,7 +172,7 @@ def test_heavy_rows_split_mode(native, oracle, monkeypatch, path):
 
 def test_rank64_kernel_selection(native, oracle, monkeypatch):
     """Rank 64 default: both sides on the pair kernel; PIO_ALS_TC=1 + PIO_ALS_TC_MIN_DEG=256 puts the item side (rows
-    average >= 256 ratings) on the tcgen05 kernel, PIO_ALS_MMA=1 selects the round-1 mma.sync kernel, PIO_ALS_MMA=0 the
+    average >= 256 ratings) on the wgmma kernel, PIO_ALS_MMA=1 selects the round-1 mma.sync kernel, PIO_ALS_MMA=0 the
     FP32 kernel.  All are within tolerance of the oracle and of each other, and really are different code paths."""
     for v in ("PIO_ALS_TC", "PIO_ALS_TC_MIN_DEG", "PIO_ALS_MMA"):
         monkeypatch.delenv(v, raising=False)
@@ -180,7 +180,7 @@ def test_rank64_kernel_selection(native, oracle, monkeypatch):
     for implicit in (True, False):
         u, i, r = synth.synth_ratings(nu, ni, nnz, seed=21, implicit=implicit)
         res = {}
-        for path, env in (("pair", {}), ("tcgen05", {"PIO_ALS_TC": "1", "PIO_ALS_TC_MIN_DEG": "256"}),
+        for path, env in (("pair", {}), ("wgmma", {"PIO_ALS_TC": "1", "PIO_ALS_TC_MIN_DEG": "256"}),
                           ("mma", {"PIO_ALS_MMA": "1"}), ("fp32", {"PIO_ALS_MMA": "0"})):
             for k, v in env.items():
                 monkeypatch.setenv(k, v)
@@ -192,9 +192,9 @@ def test_rank64_kernel_selection(native, oracle, monkeypatch):
             res[path] = g
             for k in env:
                 monkeypatch.delenv(k)
-        for a in ("mma", "pair", "tcgen05"):
+        for a in ("mma", "pair", "wgmma"):
             assert frob_rel(res[a][1], res["fp32"][1]) <= TOL
-        assert not np.array_equal(res["pair"][1], res["fp32"][1]) and not np.array_equal(res["pair"][1], res["tcgen05"][1])
+        assert not np.array_equal(res["pair"][1], res["fp32"][1]) and not np.array_equal(res["pair"][1], res["wgmma"][1])
         assert not np.array_equal(res["pair"][1], res["mma"][1])
 
 
@@ -243,7 +243,7 @@ def test_dedup_modes_match_host_preparation(native, oracle, mode):
     assert frob_rel(g[0], o[0]) <= TOL and frob_rel(g[1], o[1]) <= TOL
 
 
-@pytest.mark.parametrize("rank,tc", [(12, None), (64, None), (64, "1")])   # FP32 kernel, mma.sync kernel, tcgen05 kernel
+@pytest.mark.parametrize("rank,tc", [(12, None), (64, None), (64, "1")])   # FP32 kernel, mma.sync kernel, wgmma kernel
 def test_implicit_negative_and_zero_preferences(native, oracle, monkeypatch, rank, tc):
     monkeypatch.delenv("PIO_ALS_TC", raising=False)
     if tc:

@@ -1,6 +1,6 @@
 """Relative Frobenius error of the factors against the fp64-accumulating oracle for the solve kernels, on the
 ill-conditioned explicit case (rank 64, lambda 0.01, fewer ratings per row than the rank) and a well-conditioned implicit one.
-PIO_ALS_MMA=0 -> FP32 kernel, default -> mma.sync kernel, PIO_ALS_TC=1 -> tcgen05 kernel."""
+PIO_ALS_MMA=0 -> FP32 kernel, default -> mma.sync kernel, PIO_ALS_TC=1 -> wgmma kernel."""
 import os, sys
 sys.path.insert(0, os.path.join(os.path.dirname(os.path.abspath(__file__)), ".."))
 import numpy as np

@@ -14,7 +14,7 @@ from pio_b200 import native  # noqa: E402
 
 def main():
     out = {}
-    for N, n in ((64, 148 * 24 * 4), (128, 148 * 6 * 4)):
+    for N, n in ((64, 132 * 24 * 4), (128, 132 * 6 * 4)):   # four waves of the 132 SMs of an H100
         rng = np.random.default_rng(0)
         Y = rng.standard_normal((64, 2 * N, N)).astype(np.float32)
         A = np.einsum("nri,nrj->nij", Y, Y).astype(np.float32)

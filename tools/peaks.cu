@@ -1,8 +1,8 @@
-// tools/peaks.cu -- measured denominators that MEASURED_PEAKS.json does not carry (VERDICT r1 item 9):
-//   * FP32 FFMA throughput of the CUDA cores (the roofline of the FP32 half-step kernel, nominally 148 x 128 x 2 x f),
+// tools/peaks.cu -- measured denominators for the rooflines of the solve kernels:
+//   * FP32 FFMA throughput of the CUDA cores (the roofline of the FP32 half-step kernel, nominally 132 x 128 x 2 x f on an H100 SXM),
 //   * mma.sync m16n8k8 TF32 throughput (the warp-level tensor path the rank-64 pair kernel accumulates on),
 //   * warp shuffle and shared-memory LDS.128 issue rates (the other two pipes the solve leans on).
-// Build: nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o tools/peaks tools/peaks.cu ; run on the GPU box, prints JSON.
+// Build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o tools/peaks tools/peaks.cu ; run on an H100, prints JSON.
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <stdio.h>
