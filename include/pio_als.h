@@ -100,8 +100,19 @@ typedef struct pio_als_stats {
   int32_t n_users_active;   /* users owning a factor */
   int32_t n_items_active;
   int32_t sm_count;
-  int32_t reserved;
+  int32_t last_score_path;  /* PIO_ALS_PATH_* bits: the scoring kernels the last recommend / similar call launched */
 } pio_als_stats;
+
+/* pio_als_stats.last_score_path: which scoring kernels ran (DESIGN.md 4.6); reset when each scoring call
+ * starts, before its arguments are checked, so a rejected call or one with nothing to score leaves 0 */
+#define PIO_ALS_PATH_SCORE_ONE 0x01    /* fused single-query kernel (one launch, result in mapped host memory) */
+#define PIO_ALS_PATH_DOT_BLOCKED 0x02  /* blocked batch recommend kernel (rank <= 64, topk <= 32) */
+#define PIO_ALS_PATH_COS_BLOCKED 0x04  /* blocked batch similar kernel (rank <= 64, topk <= 32) */
+#define PIO_ALS_PATH_DOT_BATCHED 0x08  /* general recommend kernel (one item per thread, groups of 16 users) */
+#define PIO_ALS_PATH_COS_MULTI 0x10    /* similar kernel for groups of 8 queries with <= 40 query vectors */
+#define PIO_ALS_PATH_COS_BATCHED 0x20  /* long single similar query, query vectors in shared memory */
+#define PIO_ALS_PATH_COS_FALLBACK 0x40 /* long single similar query too large for shared memory */
+#define PIO_ALS_PATH_MULTI_PASS 0x80   /* more than one pass of <= 128 results (topk > 128) */
 
 PIO_API int pio_als_abi_version(void);
 /* number of visible sm_90 devices, or PIO_ALS_ERR_CUDA */

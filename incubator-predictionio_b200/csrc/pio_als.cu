@@ -16,6 +16,7 @@
 #include <chrono>
 #include <deque>
 #include <exception>
+#include <map>
 #include <mutex>
 #include <string>
 #include <vector>
@@ -1831,17 +1832,41 @@ static int serve_reserve(pio_als_handle* h, size_t dev_bytes, size_t host_bytes)
 }
 static inline size_t al256(size_t x) { return (x + 255) & ~(size_t)255; }
 
+// cudaFuncSetAttribute(MaxDynamicSharedMemorySize) SETS a kernel's limit on the current device, it does not raise it.  A
+// kernel launched from several call sites therefore needs one record of the limit in place, shared by all handles and
+// threads of the process: this one only ever raises it, per kernel and device.
+static int ensure_dyn_smem(pio_als_handle* h, const void* kernel, size_t bytes) {
+  static std::mutex mu;
+  static std::map<std::pair<const void*, int>, size_t> limit;
+  std::lock_guard<std::mutex> lk(mu);
+  size_t& cur = limit[std::make_pair(kernel, h->cfg.device)];
+  if (cur >= bytes) return PIO_ALS_OK;
+  CK(h, cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes));
+  cur = bytes;
+  return PIO_ALS_OK;
+}
+#define ENSURE_SMEM(h, kernel, bytes)                                    \
+  do {                                                                   \
+    const int rc_ = ensure_dyn_smem(h, (const void*)(kernel), (bytes)); \
+    if (rc_) return rc_;                                                 \
+  } while (0)
+// after every launch of a scoring call: count it, record which scoring kernel ran (pio_als_stats.last_score_path; 0 for
+// gathers and merges) and fail on a launch error -- a kernel that never started would leave stale candidates behind
+#define SCORE_LAUNCHED(h, path)             \
+  do {                                      \
+    LAUNCHED(h);                            \
+    (h)->st.last_score_path |= (path);      \
+    CK(h, cudaGetLastError());              \
+  } while (0)
+
 extern "C++" {
 template <int KPT>
 static int launch_dot_blocked_kp(pio_als_handle* h, dim3 grid, size_t smem, const float* d_xq, const uint8_t* d_valid, int nq,
                                  const uint8_t* d_mask, const double* d_weight, int topk, ScoreIdx* d_cand) {
-  static size_t attr_smem[64] = {};
-  if (h->cfg.device < 64 && attr_smem[h->cfg.device] < smem) {
-    CK(h, cudaFuncSetAttribute(score_dot_blocked_kernel<KPT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    attr_smem[h->cfg.device] = smem;
-  }
+  ENSURE_SMEM(h, score_dot_blocked_kernel<KPT>, smem);
   score_dot_blocked_kernel<KPT><<<grid, 32 * DB_WARPS, smem, h->stream>>>(h->I.F, h->I.n_internal, d_xq, d_valid, nq,
                                                                          h->I.cand_ext, d_mask, d_weight, topk, d_cand);
+  SCORE_LAUNCHED(h, PIO_ALS_PATH_DOT_BLOCKED);
   return PIO_ALS_OK;
 }
 }  // extern "C++"
@@ -1850,14 +1875,11 @@ template <int KPT>
 static int launch_cos_blocked_kp(pio_als_handle* h, dim3 grid, size_t smem, const float* d_qf, const int* d_bq0, const int* d_bv0,
                                  int n_bins, const int* d_vq, const long long* d_qptr, const int* d_qid, const uint8_t* d_mask,
                                  const double* d_weight, int keep, int topk, ScoreIdx* d_cand) {
-  static size_t attr_smem[64] = {};
-  if (h->cfg.device < 64 && attr_smem[h->cfg.device] < smem) {
-    CK(h, cudaFuncSetAttribute(score_cos_blocked_kernel<KPT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    attr_smem[h->cfg.device] = smem;
-  }
+  ENSURE_SMEM(h, score_cos_blocked_kernel<KPT>, smem);
   score_cos_blocked_kernel<KPT><<<grid, 32 * DB_WARPS, smem, h->stream>>>(h->I.F, h->I.n_internal, h->cfg.rank, d_qf, d_bq0, d_bv0,
                                                                          n_bins, d_vq, d_qptr, d_qid, h->I.cand_ext, d_mask,
                                                                          d_weight, keep, topk, d_cand);
+  SCORE_LAUNCHED(h, PIO_ALS_PATH_COS_BLOCKED);
   return PIO_ALS_OK;
 }
 }  // extern "C++"
@@ -1902,25 +1924,19 @@ static int recommend_small(pio_als_handle* h, const int32_t* users, int n, int t
   if (item_mask) CK(h, cudaMemcpyAsync(d_mask, item_mask, (size_t)h->I.n, cudaMemcpyHostToDevice, st));
   if (item_weight) CK(h, cudaMemcpyAsync(d_weight, item_weight, sizeof(double) * (size_t)h->I.n, cudaMemcpyHostToDevice, st));
   const size_t sb_smem = sizeof(double) * (size_t)KP * SB_QB + sb_tile_bytes(KP) + (sizeof(double) + sizeof(int)) * (size_t)SB_QB * topk;
-  {
-    static size_t attr_smem[64] = {};
-    if (h->cfg.device < 64 && attr_smem[h->cfg.device] < sb_smem) {
-      CK(h, cudaFuncSetAttribute(score_dot_topk_batched_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sb_smem));
-      attr_smem[h->cfg.device] = sb_smem;
-    }
-  }
+  ENSURE_SMEM(h, score_dot_topk_batched_kernel, sb_smem);
   IdList ids;
   for (int q = 0; q < n; ++q) ids.v[q] = users[q];
   gather_rows_ids_kernel<<<n, 64, 0, st>>>(h->U.F, KP, ids, h->U.perm, h->U.deg, h->U.n, d_xq, d_valid);
-  LAUNCHED(h);
+  SCORE_LAUNCHED(h, 0);
   score_dot_topk_batched_kernel<<<dim3(gx, 1), SB_THREADS, sb_smem, st>>>(h->I.F, h->I.n_internal, KP, d_xq, d_valid, n,
                                                                          h->I.cand_ext, d_mask, d_weight, nullptr, topk, d_cand);
-  LAUNCHED(h);
+  SCORE_LAUNCHED(h, PIO_ALS_PATH_DOT_BATCHED);
   int* m_oi = (int*)(h->srv_host_dev + ho_i);
   float* m_os = (float*)(h->srv_host_dev + ho_s);
   int* m_oc = (int*)(h->srv_host_dev + ho_c);
   topk_merge_kernel<<<n, TK_THREADS, 0, st>>>(d_cand, gx * topk, topk, topk, 0, m_oi, m_os, m_oc, nullptr);
-  LAUNCHED(h);
+  SCORE_LAUNCHED(h, 0);
   CK(h, cudaStreamSynchronize(st));
   memcpy(out_items, h->srv_host + ho_i, sizeof(int) * (size_t)n * topk);
   memcpy(out_scores, h->srv_host + ho_s, sizeof(float) * (size_t)n * topk);
@@ -1962,23 +1978,17 @@ static int similar_small(pio_als_handle* h, const int32_t* query_items, int nq, 
   for (int q = 0; q < nq; ++q) { ids.v[q] = query_items[q]; hvq[q] = 0; hqid[q] = query_items[q]; }
   const size_t smem = sizeof(double) * ((size_t)KP * SM_NV + SM_NV) + sb_tile_bytes(KP) +
                       (sizeof(double) + sizeof(int)) * (size_t)SM_QG * topk + sizeof(int) * (SM_NV + SM_QG * SM_QIDS) + 16;
-  {
-    static size_t attr_smem[64] = {};
-    if (h->cfg.device < 64 && attr_smem[h->cfg.device] < smem) {
-      CK(h, cudaFuncSetAttribute(score_cos_topk_multi_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-      attr_smem[h->cfg.device] = smem;
-    }
-  }
+  ENSURE_SMEM(h, score_cos_topk_multi_kernel, smem);
   gather_rows_ids_kernel<<<nq, 64, 0, st>>>(h->I.F, KP, ids, h->I.perm, h->I.deg, h->I.n, d_qf, nullptr);
-  LAUNCHED(h);
+  SCORE_LAUNCHED(h, 0);
   score_cos_topk_multi_kernel<<<dim3(gx, 1), SB_THREADS, smem, st>>>(
       h->I.F, h->I.n_internal, KP, k, d_qf, (const int*)(h->srv_host_dev + ho_g), (const int*)(h->srv_host_dev + ho_vq),
       (const long long*)(h->srv_host_dev + ho_qp), (const int*)(h->srv_host_dev + ho_qid), 1, h->I.cand_ext, d_mask, d_weight,
       nullptr, (flags & PIO_ALS_SIM_KEEP_QUERY_ITEMS) ? 1 : 0, topk, d_cand);
-  LAUNCHED(h);
+  SCORE_LAUNCHED(h, PIO_ALS_PATH_COS_MULTI);
   topk_merge_kernel<<<1, TK_THREADS, 0, st>>>(d_cand, gx * topk, topk, topk, 0, (int*)(h->srv_host_dev + ho_i),
                                               (float*)(h->srv_host_dev + ho_s), (int*)(h->srv_host_dev + ho_c), nullptr);
-  LAUNCHED(h);
+  SCORE_LAUNCHED(h, 0);
   CK(h, cudaStreamSynchronize(st));
   memcpy(out_items, h->srv_host + ho_i, sizeof(int) * (size_t)topk);
   memcpy(out_scores, h->srv_host + ho_s, sizeof(float) * (size_t)topk);
@@ -1990,26 +2000,24 @@ static int similar_small(pio_als_handle* h, const int32_t* query_items, int nq, 
 // nq <= S1_MAXNV query items.  The host waits on a sequence flag in the mapped arena instead of a stream synchronisation.
 extern "C++" {
 template <bool COS, int NVP, int KPT>
-static void launch_score_one_kp(pio_als_handle* h, int gx, size_t smem, const Side& q, const OneQuery& qry, const uint8_t* d_mask,
-                                const double* d_weight, int keep, int topk, ScoreIdx* d_cand, int* m_oi, float* m_os, int* m_oc,
-                                unsigned* m_flag, unsigned seq, unsigned long long* m_trace) {
-  static size_t attr_smem[64] = {};
-  if (h->cfg.device < 64 && attr_smem[h->cfg.device] < smem) {
-    cudaFuncSetAttribute(score_one_kernel<COS, NVP, KPT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    attr_smem[h->cfg.device] = smem;
-  }
+static int launch_score_one_kp(pio_als_handle* h, int gx, size_t smem, const Side& q, const OneQuery& qry, const uint8_t* d_mask,
+                               const double* d_weight, int keep, int topk, ScoreIdx* d_cand, int* m_oi, float* m_os, int* m_oc,
+                               unsigned* m_flag, unsigned seq, unsigned long long* m_trace) {
+  ENSURE_SMEM(h, (score_one_kernel<COS, NVP, KPT>), smem);
   unsigned long long* g_thr = reinterpret_cast<unsigned long long*>(h->srv_counter + 2);
   score_one_kernel<COS, NVP, KPT><<<gx, S1_THREADS, smem, h->stream>>>(
       h->I.F, h->I.n_internal, h->cfg.rank, q.F, q.perm, q.deg, q.n, qry, h->I.cand_ext, d_mask, d_weight, keep, topk, d_cand,
       h->srv_counter, g_thr, m_oi, m_os, m_oc, m_flag, seq, m_trace);
+  SCORE_LAUNCHED(h, PIO_ALS_PATH_SCORE_ONE);
+  return PIO_ALS_OK;
 }
 template <bool COS, int NVP>
-static void launch_score_one(pio_als_handle* h, int gx, size_t smem, const Side& q, const OneQuery& qry, const uint8_t* d_mask,
-                             const double* d_weight, int keep, int topk, ScoreIdx* d_cand, int* m_oi, float* m_os, int* m_oc,
-                             unsigned* m_flag, unsigned seq, unsigned long long* m_trace) {
-  if (h->KP == 16) launch_score_one_kp<COS, NVP, 16>(h, gx, smem, q, qry, d_mask, d_weight, keep, topk, d_cand, m_oi, m_os, m_oc, m_flag, seq, m_trace);
-  else if (h->KP == 32) launch_score_one_kp<COS, NVP, 32>(h, gx, smem, q, qry, d_mask, d_weight, keep, topk, d_cand, m_oi, m_os, m_oc, m_flag, seq, m_trace);
-  else launch_score_one_kp<COS, NVP, 64>(h, gx, smem, q, qry, d_mask, d_weight, keep, topk, d_cand, m_oi, m_os, m_oc, m_flag, seq, m_trace);
+static int launch_score_one(pio_als_handle* h, int gx, size_t smem, const Side& q, const OneQuery& qry, const uint8_t* d_mask,
+                            const double* d_weight, int keep, int topk, ScoreIdx* d_cand, int* m_oi, float* m_os, int* m_oc,
+                            unsigned* m_flag, unsigned seq, unsigned long long* m_trace) {
+  if (h->KP == 16) return launch_score_one_kp<COS, NVP, 16>(h, gx, smem, q, qry, d_mask, d_weight, keep, topk, d_cand, m_oi, m_os, m_oc, m_flag, seq, m_trace);
+  if (h->KP == 32) return launch_score_one_kp<COS, NVP, 32>(h, gx, smem, q, qry, d_mask, d_weight, keep, topk, d_cand, m_oi, m_os, m_oc, m_flag, seq, m_trace);
+  return launch_score_one_kp<COS, NVP, 64>(h, gx, smem, q, qry, d_mask, d_weight, keep, topk, d_cand, m_oi, m_os, m_oc, m_flag, seq, m_trace);
 }
 }  // extern "C++"
 
@@ -2059,14 +2067,13 @@ static int serve_one(pio_als_handle* h, bool cos, const int32_t* ids, int nq, in
   unsigned long long* m_trace = h->serve_trace ? (unsigned long long*)(h->srv_host_dev + ho_trace) : nullptr;
   const auto t_call = std::chrono::steady_clock::now();
 #define PIO_S1(C, N) launch_score_one<C, N>(h, gx, smem, q, qry, d_mask, d_weight, keep, topk, d_cand, m_oi, m_os, m_oc, m_flag, seq, m_trace)
-  if (!cos) PIO_S1(false, 1);
-  else if (nvp == 1) PIO_S1(true, 1);
-  else if (nvp == 2) PIO_S1(true, 2);
-  else if (nvp == 4) PIO_S1(true, 4);
-  else PIO_S1(true, 8);
+  if (!cos) rc = PIO_S1(false, 1);
+  else if (nvp == 1) rc = PIO_S1(true, 1);
+  else if (nvp == 2) rc = PIO_S1(true, 2);
+  else if (nvp == 4) rc = PIO_S1(true, 4);
+  else rc = PIO_S1(true, 8);
 #undef PIO_S1
-  LAUNCHED(h);
-  CK(h, cudaGetLastError());
+  if (rc) return rc;
   for (unsigned spins = 1; *flag != seq; ++spins) {
     if ((spins & 0x3FFFu) == 0) {   // a faulted kernel never writes the flag: ask the stream now and then
       const cudaError_t e = cudaStreamQuery(st);
@@ -2099,10 +2106,11 @@ static int serve_one(pio_als_handle* h, bool cos, const int32_t* ids, int nq, in
 int pio_als_recommend(pio_als_handle* h, const int32_t* users, int n, int topk, const uint8_t* item_mask,
                       const double* item_weight, int32_t* out_items, float* out_scores, int32_t* out_count) {
   if (!h) return PIO_ALS_ERR_ARG;
+  std::lock_guard<std::mutex> lk(h->mu);
+  h->st.last_score_path = 0;   // also for a call that launches nothing
   if (n < 0 || topk < 1) return fail(h, PIO_ALS_ERR_ARG, "topk must be >= 1 and n >= 0");
   if (n == 0) return PIO_ALS_OK;
   if (!users || !out_items || !out_scores) return fail(h, PIO_ALS_ERR_ARG, "null argument");
-  std::lock_guard<std::mutex> lk(h->mu);
   if (!h->U.F || !h->I.F || !h->I.cand_ext) return fail(h, PIO_ALS_ERR_STATE, "no model");
   CK(h, cudaSetDevice(h->cfg.device));
   if (n == 1 && serve_one_ok(h, 1, topk))   // the serving case: one query, one launch
@@ -2128,13 +2136,6 @@ int pio_als_recommend(pio_als_handle* h, const int32_t* users, int n, int topk, 
   if (gx < 1) gx = 1;
   const size_t sb_smem = sizeof(double) * (size_t)KP * SB_QB + sb_tile_bytes(KP) +
                          (sizeof(double) + sizeof(int)) * (size_t)SB_QB * pass_max;
-  {
-    static size_t attr_smem[64] = {};
-    if (h->cfg.device < 64 && attr_smem[h->cfg.device] < sb_smem) {
-      CK(h, cudaFuncSetAttribute(score_dot_topk_batched_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sb_smem));
-      attr_smem[h->cfg.device] = sb_smem;
-    }
-  }
   // blocked kernel (two items x 16 queries per thread, independent warps): rank <= 64, topk <= DB_MAXK
   const bool blocked = h->score_blocked && KP <= 64 && topk <= DB_MAXK;
   if (blocked) {
@@ -2142,6 +2143,8 @@ int pio_als_recommend(pio_als_handle* h, const int32_t* users, int n, int topk, 
     gx = (h->sm_count + ngroups - 1) / ngroups;
     if (gx > (nsteps + 7) / 8) gx = (nsteps + 7) / 8;   // at least eight steps per warp: the pools must warm up
     if (gx < 1) gx = 1;
+  } else {
+    ENSURE_SMEM(h, score_dot_topk_batched_kernel, sb_smem);
   }
   const int lists = blocked ? gx * DB_RINGS : gx;        // candidate lists per query
   CK(h, tmp.alloc(&d_users, (size_t)n));
@@ -2162,9 +2165,10 @@ int pio_als_recommend(pio_als_handle* h, const int32_t* users, int n, int topk, 
   }
   if (topk > TK_MAXK) CK(h, tmp.alloc(&d_bound, (size_t)n));
   gather_rows_kernel<<<n, 64, 0, st>>>(h->U.F, KP, d_users, n, h->U.perm, h->U.deg, h->U.n, d_xq, d_valid);
-  LAUNCHED(h);
+  SCORE_LAUNCHED(h, 0);
   for (int done = 0; done < topk; done += TK_MAXK) {
     const int pk = topk - done < TK_MAXK ? topk - done : TK_MAXK;
+    if (done > 0) h->st.last_score_path |= PIO_ALS_PATH_MULTI_PASS;
     // grid.y is limited to 65535 query groups per launch
     for (int g0 = 0; g0 < ngroups; g0 += 32768) {
       const int ng = ngroups - g0 < 32768 ? ngroups - g0 : 32768;
@@ -2179,12 +2183,12 @@ int pio_als_recommend(pio_als_handle* h, const int32_t* users, int n, int topk, 
         score_dot_topk_batched_kernel<<<dim3(gx, ng), SB_THREADS, sb_smem, st>>>(
             h->I.F, h->I.n_internal, KP, d_xq + (size_t)q0 * KP, d_valid + q0, nq, h->I.cand_ext, d_mask, d_weight,
             (done > 0) ? d_bound + q0 : nullptr, pk, d_cand + (size_t)q0 * lists * pk);
+        SCORE_LAUNCHED(h, PIO_ALS_PATH_DOT_BATCHED);
       }
-      LAUNCHED(h);
     }
     // the candidate lists of a query are [lists][pk] entries, stored with stride pk
     topk_merge_kernel<<<n, TK_THREADS, 0, st>>>(d_cand, lists * pk, pk, topk, done, d_oi, d_os, d_oc, d_bound);
-    LAUNCHED(h);
+    SCORE_LAUNCHED(h, 0);
   }
   CK(h, cudaMemcpyAsync(out_items, d_oi, sizeof(int) * (size_t)n * topk, cudaMemcpyDeviceToHost, st));
   CK(h, cudaMemcpyAsync(out_scores, d_os, sizeof(float) * (size_t)n * topk, cudaMemcpyDeviceToHost, st));
@@ -2212,7 +2216,7 @@ static int similar_one(pio_als_handle* h, const int32_t* query_items, int nq, in
   CK(h, tmp.alloc(&d_valid, (size_t)nq));
   CK(h, cudaMemcpyAsync(d_q, query_items, sizeof(int) * nq, cudaMemcpyHostToDevice, st));
   gather_rows_kernel<<<nq, 64, 0, st>>>(h->I.F, KP, d_q, nq, h->I.perm, h->I.deg, h->I.n, d_qf, d_valid);
-  LAUNCHED(h);
+  SCORE_LAUNCHED(h, 0);
   std::vector<uint8_t> valid(nq);
   CK(h, cudaMemcpyAsync(valid.data(), d_valid, (size_t)nq, cudaMemcpyDeviceToHost, st));
   CK(h, cudaStreamSynchronize(st));
@@ -2237,11 +2241,7 @@ static int similar_one(pio_als_handle* h, const int32_t* query_items, int nq, in
   if (batched) {
     const int nt = (h->I.n_internal + SB_THREADS - 1) / SB_THREADS;
     ntiles = 2 * h->sm_count < (nt + 7) / 8 ? 2 * h->sm_count : (nt + 7) / 8;   // = CTAs (>= 8 tiles each)
-    static size_t attr_smem[64] = {};
-    if (h->cfg.device < 64 && attr_smem[h->cfg.device] < sc_smem) {
-      CK(h, cudaFuncSetAttribute(score_cos_topk_batched_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sc_smem));
-      attr_smem[h->cfg.device] = sc_smem;
-    }
+    ENSURE_SMEM(h, score_cos_topk_batched_kernel, sc_smem);
   }
   ScoreIdx *d_cand = nullptr, *d_bound = nullptr;
   int *d_oi = nullptr, *d_oc = nullptr;
@@ -2255,16 +2255,19 @@ static int similar_one(pio_als_handle* h, const int32_t* query_items, int nq, in
   for (int done = 0; done < topk; done += TK_MAXK) {
     const int pk = topk - done < TK_MAXK ? topk - done : TK_MAXK;
     const ScoreIdx* bnd = done > 0 ? d_bound : nullptr;
-    if (batched)
+    if (done > 0) h->st.last_score_path |= PIO_ALS_PATH_MULTI_PASS;
+    if (batched) {
       score_cos_topk_batched_kernel<<<ntiles, SB_THREADS, sc_smem, st>>>(h->I.F, h->I.n_internal, KP, k, d_qc, d_q, nq, nqv,
                                                                          h->I.cand_ext, d_mask, d_weight, bnd, keep_query, pk,
                                                                          d_cand);
-    else
+      SCORE_LAUNCHED(h, PIO_ALS_PATH_COS_BATCHED);
+    } else {
       score_cos_topk_kernel<<<ntiles, TK_THREADS, 0, st>>>(h->I.F, h->I.n_internal, KP, k, d_qc, d_q, nq, nqv, h->I.cand_ext,
                                                            d_mask, d_weight, bnd, keep_query, pk, d_cand);
-    LAUNCHED(h);
+      SCORE_LAUNCHED(h, PIO_ALS_PATH_COS_FALLBACK);
+    }
     topk_merge_kernel<<<1, TK_THREADS, 0, st>>>(d_cand, npools * pk, pk, topk, done, d_oi, d_os, d_oc, d_bound);
-    LAUNCHED(h);
+    SCORE_LAUNCHED(h, 0);
   }
   CK(h, cudaMemcpyAsync(out_items, d_oi, sizeof(int) * topk, cudaMemcpyDeviceToHost, st));
   CK(h, cudaMemcpyAsync(out_scores, d_os, sizeof(float) * topk, cudaMemcpyDeviceToHost, st));
@@ -2280,13 +2283,14 @@ int pio_als_similar_batch(pio_als_handle* h, const int64_t* q_ptr, const int32_t
                           const uint8_t* item_mask, const double* item_weight, int flags, int32_t* out_items,
                           float* out_scores, int32_t* out_count) {
   if (!h) return PIO_ALS_ERR_ARG;
+  std::lock_guard<std::mutex> lk(h->mu);
+  h->st.last_score_path = 0;   // also for a call that launches nothing
   if (n_queries < 0 || topk < 1) return fail(h, PIO_ALS_ERR_ARG, "topk must be >= 1 and n_queries >= 0");
   if (n_queries == 0) return PIO_ALS_OK;
   if (!q_ptr || !out_items || !out_scores) return fail(h, PIO_ALS_ERR_ARG, "null argument");
   for (int j = 0; j < n_queries; ++j)
     if (q_ptr[j + 1] < q_ptr[j] || (q_ptr[j + 1] > q_ptr[j] && !q_items))
       return fail(h, PIO_ALS_ERR_ARG, "q_ptr must be non-decreasing offsets into q_items");
-  std::lock_guard<std::mutex> lk(h->mu);
   if (!h->I.F || !h->I.cand_ext) return fail(h, PIO_ALS_ERR_STATE, "no model");
   CK(h, cudaSetDevice(h->cfg.device));
   if (n_queries == 1 && serve_one_ok(h, (int)std::min<long long>(q_ptr[1] - q_ptr[0], 1 << 20), topk))   // the serving case
@@ -2321,7 +2325,7 @@ int pio_als_similar_batch(pio_als_handle* h, const int64_t* q_ptr, const int32_t
     CK(h, tmp.alloc(&d_valid, (size_t)total));
     CK(h, cudaMemcpyAsync(d_qid, q_items + q_ptr[0], sizeof(int) * total, cudaMemcpyHostToDevice, st));
     gather_rows_kernel<<<(unsigned)total, 64, 0, st>>>(h->I.F, KP, d_qid, (int)total, h->I.perm, h->I.deg, h->I.n, d_qf_all, d_valid);
-    LAUNCHED(h);
+    SCORE_LAUNCHED(h, 0);
     std::vector<uint8_t> valid((size_t)total);
     CK(h, cudaMemcpyAsync(valid.data(), d_valid, (size_t)total, cudaMemcpyDeviceToHost, st));
     CK(h, cudaStreamSynchronize(st));
@@ -2373,7 +2377,7 @@ int pio_als_similar_batch(pio_als_handle* h, const int64_t* q_ptr, const int32_t
           CK(h, cudaMemcpyAsync(d_vq, bvq.data(), sizeof(int) * nvec, cudaMemcpyHostToDevice, st));
           CK(h, cudaMemcpyAsync(d_vsrc, bvsrc.data(), sizeof(int) * nvec, cudaMemcpyHostToDevice, st));
           copy_rows_kernel<<<nvec, 64, 0, st>>>(d_qf_all, KP, d_vsrc, d_qfc);
-          LAUNCHED(h);
+          SCORE_LAUNCHED(h, 0);
         }
         const int nsteps = (h->I.n_internal + DB_RINGS * DB_ROWS - 1) / (DB_RINGS * DB_ROWS);
         int gx = (h->sm_count + ngroups - 1) / ngroups;
@@ -2391,10 +2395,9 @@ int pio_als_similar_batch(pio_als_handle* h, const int64_t* q_ptr, const int32_t
           const int brc = launch_cos_blocked(h, dim3(gx, ng), smem, d_qfc, d_bq0 + (size_t)g0 * DB_WPR, d_bv0 + (size_t)g0 * DB_WPR,
                                              n_bins - g0 * DB_WPR, d_vq, d_qptr, d_qid, d_mask, d_weight, keep_query, topk, d_cand);
           if (brc) return brc;
-          LAUNCHED(h);
         }
         topk_merge_kernel<<<n_queries, TK_THREADS, 0, st>>>(d_cand, lists * topk, topk, topk, 0, d_oi, d_os, d_oc, nullptr);
-        LAUNCHED(h);
+        SCORE_LAUNCHED(h, 0);
         CK(h, cudaMemcpyAsync(out_items, d_oi, sizeof(int) * (size_t)n_queries * topk, cudaMemcpyDeviceToHost, st));
         CK(h, cudaMemcpyAsync(out_scores, d_os, sizeof(float) * (size_t)n_queries * topk, cudaMemcpyDeviceToHost, st));
         if (out_count) CK(h, cudaMemcpyAsync(out_count, d_oc, sizeof(int) * (size_t)n_queries, cudaMemcpyDeviceToHost, st));
@@ -2434,7 +2437,7 @@ int pio_als_similar_batch(pio_als_handle* h, const int64_t* q_ptr, const int32_t
         CK(h, cudaMemcpyAsync(d_vq, vq.data(), sizeof(int) * nvec, cudaMemcpyHostToDevice, st));
         CK(h, cudaMemcpyAsync(d_vsrc, vsrc.data(), sizeof(int) * nvec, cudaMemcpyHostToDevice, st));
         copy_rows_kernel<<<nvec, 64, 0, st>>>(d_qf_all, KP, d_vsrc, d_qfc);
-        LAUNCHED(h);
+        SCORE_LAUNCHED(h, 0);
       }
       const int pass_max = topk < TK_MAXK ? topk : TK_MAXK;
       const int ntiles = (h->I.n_internal + SB_THREADS - 1) / SB_THREADS;
@@ -2443,13 +2446,7 @@ int pio_als_similar_batch(pio_als_handle* h, const int64_t* q_ptr, const int32_t
       if (gx < 1) gx = 1;
       const size_t smem = sizeof(double) * ((size_t)KP * SM_NV + SM_NV) + sb_tile_bytes(KP) +
                           (sizeof(double) + sizeof(int)) * (size_t)SM_QG * pass_max + sizeof(int) * (SM_NV + SM_QG * SM_QIDS) + 16;
-      {
-        static size_t attr_smem[64] = {};
-        if (h->cfg.device < 64 && attr_smem[h->cfg.device] < smem) {
-          CK(h, cudaFuncSetAttribute(score_cos_topk_multi_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-          attr_smem[h->cfg.device] = smem;
-        }
-      }
+      ENSURE_SMEM(h, score_cos_topk_multi_kernel, smem);
       CK(h, tmp.alloc(&d_cand, (size_t)n_queries * gx * pass_max));
       CK(h, tmp.alloc(&d_oi, (size_t)n_queries * topk));
       CK(h, tmp.alloc(&d_os, (size_t)n_queries * topk));
@@ -2458,6 +2455,7 @@ int pio_als_similar_batch(pio_als_handle* h, const int64_t* q_ptr, const int32_t
       const int keep_query = (flags & PIO_ALS_SIM_KEEP_QUERY_ITEMS) ? 1 : 0;
       for (int done = 0; done < topk; done += TK_MAXK) {
         const int pk = topk - done < TK_MAXK ? topk - done : TK_MAXK;
+        if (done > 0) h->st.last_score_path |= PIO_ALS_PATH_MULTI_PASS;
         for (int g0 = 0; g0 < ngroups; g0 += 32768) {
           const int ng = ngroups - g0 < 32768 ? ngroups - g0 : 32768;
           const int qa = g0 * SM_QG;
@@ -2465,10 +2463,10 @@ int pio_als_similar_batch(pio_als_handle* h, const int64_t* q_ptr, const int32_t
           score_cos_topk_multi_kernel<<<dim3(gx, ng), SB_THREADS, smem, st>>>(
               h->I.F, h->I.n_internal, KP, k, d_qfc, d_gvec0 + g0, d_vq, d_qptr + qa, d_qid, nq, h->I.cand_ext, d_mask,
               d_weight, done > 0 ? d_bound + qa : nullptr, keep_query, pk, d_cand + (size_t)qa * gx * pk);
-          LAUNCHED(h);
+          SCORE_LAUNCHED(h, PIO_ALS_PATH_COS_MULTI);
         }
         topk_merge_kernel<<<n_queries, TK_THREADS, 0, st>>>(d_cand, gx * pk, pk, topk, done, d_oi, d_os, d_oc, d_bound);
-        LAUNCHED(h);
+        SCORE_LAUNCHED(h, 0);
       }
       CK(h, cudaMemcpyAsync(out_items, d_oi, sizeof(int) * (size_t)n_queries * topk, cudaMemcpyDeviceToHost, st));
       CK(h, cudaMemcpyAsync(out_scores, d_os, sizeof(float) * (size_t)n_queries * topk, cudaMemcpyDeviceToHost, st));
@@ -2491,7 +2489,11 @@ int pio_als_similar_batch(pio_als_handle* h, const int64_t* q_ptr, const int32_t
 int pio_als_similar(pio_als_handle* h, const int32_t* query_items, int nq, int topk, const uint8_t* item_mask,
                     const double* item_weight, int flags, int32_t* out_items, float* out_scores, int32_t* out_count) {
   if (!h) return PIO_ALS_ERR_ARG;
-  if (nq < 0) return fail(h, PIO_ALS_ERR_ARG, "nq < 0");
+  if (nq < 0) {
+    std::lock_guard<std::mutex> lk(h->mu);
+    h->st.last_score_path = 0;
+    return fail(h, PIO_ALS_ERR_ARG, "nq < 0");
+  }
   const int64_t ptr[2] = {0, nq};
   return pio_als_similar_batch(h, ptr, query_items, 1, topk, item_mask, item_weight, flags, out_items, out_scores, out_count);
 }

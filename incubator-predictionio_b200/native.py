@@ -60,8 +60,13 @@ class Stats(C.Structure):
         ("last_run_ms", C.c_double), ("last_solve_ms", C.c_double), ("last_gram_ms", C.c_double),
         ("last_comm_ms", C.c_double), ("last_ingest_ms", C.c_double),
         ("n_users_active", C.c_int32), ("n_items_active", C.c_int32), ("sm_count", C.c_int32),
-        ("reserved", C.c_int32),
+        ("last_score_path", C.c_int32),
     ]
+
+
+# pio_als_stats.last_score_path bits (PIO_ALS_PATH_* in pio_als.h)
+SCORE_PATH_BITS = {"score_one": 0x01, "dot_blocked": 0x02, "cos_blocked": 0x04, "dot_batched": 0x08, "cos_multi": 0x10,
+                   "cos_batched": 0x20, "cos_fallback": 0x40, "multi_pass": 0x80}
 
 
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
@@ -329,7 +334,10 @@ class NativeALS:
     def stats(self) -> dict:
         st = Stats()
         self._check(lib().pio_als_get_stats(self._h, C.byref(st)))
-        return {name: getattr(st, name) for name, _ in Stats._fields_ if name != "reserved"}
+        out = {name: getattr(st, name) for name, _ in Stats._fields_}
+        # the scoring kernels of the last recommend / similar call, as a set of SCORE_PATH_BITS names
+        out["last_score_path"] = {name for name, bit in SCORE_PATH_BITS.items() if st.last_score_path & bit}
+        return out
 
     def phase_ms(self) -> dict:
         """Device-time breakdown of the last run (pio_als_get_phase_ms)."""
