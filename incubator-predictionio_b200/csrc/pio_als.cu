@@ -19,6 +19,7 @@
 #include <map>
 #include <mutex>
 #include <string>
+#include <type_traits>
 #include <vector>
 
 #include "als_kernels.cuh"
@@ -42,6 +43,7 @@
 #undef TC_NRAW
 #include "sort_scan.cuh"
 #include "topk.cuh"
+#include "score_plan.h"
 #include "ids_encode.cuh"
 #include "cooc.cuh"
 
@@ -1809,6 +1811,9 @@ int pio_als_train(pio_als_handle* h, const int32_t* user, const int32_t* item, c
   return pio_als_get_factors(h, user_out, item_out, user_has, item_has);
 }
 
+}  // extern "C"
+
+// ---- top-k scoring: score_plan.h decides what runs, the helpers below launch it ----------------------------------------
 namespace pio {
 static int serve_reserve(pio_als_handle* h, size_t dev_bytes, size_t host_bytes) {
   if (h->srv_dev_cap < dev_bytes) {
@@ -1832,6 +1837,16 @@ static int serve_reserve(pio_als_handle* h, size_t dev_bytes, size_t host_bytes)
 }
 static inline size_t al256(size_t x) { return (x + 255) & ~(size_t)255; }
 
+// the layout of a serving arena: blocks in call order, each starting on a 256-byte boundary
+struct ArenaLayout {
+  size_t bytes = 0;
+  size_t take(size_t n) {
+    const size_t at = bytes;
+    bytes = al256(bytes + n);
+    return at;
+  }
+};
+
 // cudaFuncSetAttribute(MaxDynamicSharedMemorySize) SETS a kernel's limit on the current device, it does not raise it.  A
 // kernel launched from several call sites therefore needs one record of the limit in place, shared by all handles and
 // threads of the process: this one only ever raises it, per kernel and device.
@@ -1845,129 +1860,233 @@ static int ensure_dyn_smem(pio_als_handle* h, const void* kernel, size_t bytes) 
   cur = bytes;
   return PIO_ALS_OK;
 }
-#define ENSURE_SMEM(h, kernel, bytes)                                    \
-  do {                                                                   \
-    const int rc_ = ensure_dyn_smem(h, (const void*)(kernel), (bytes)); \
-    if (rc_) return rc_;                                                 \
-  } while (0)
-// after every launch of a scoring call: count it, record which scoring kernel ran (pio_als_stats.last_score_path; 0 for
-// gathers and merges) and fail on a launch error -- a kernel that never started would leave stale candidates behind
-#define SCORE_LAUNCHED(h, path)             \
-  do {                                      \
-    LAUNCHED(h);                            \
-    (h)->st.last_score_path |= (path);      \
-    CK(h, cudaGetLastError());              \
-  } while (0)
 
-extern "C++" {
-template <int KPT>
-static int launch_dot_blocked_kp(pio_als_handle* h, dim3 grid, size_t smem, const float* d_xq, const uint8_t* d_valid, int nq,
-                                 const uint8_t* d_mask, const double* d_weight, int topk, ScoreIdx* d_cand) {
-  ENSURE_SMEM(h, score_dot_blocked_kernel<KPT>, smem);
-  score_dot_blocked_kernel<KPT><<<grid, 32 * DB_WARPS, smem, h->stream>>>(h->I.F, h->I.n_internal, d_xq, d_valid, nq,
-                                                                         h->I.cand_ext, d_mask, d_weight, topk, d_cand);
-  SCORE_LAUNCHED(h, PIO_ALS_PATH_DOT_BLOCKED);
+// Every launch of a scoring call goes through here: raise the kernel's dynamic shared-memory limit when it takes any,
+// launch on the handle's stream, count the launch, record which scoring kernel ran (path: its PIO_ALS_PATH_* bit, 0 for
+// gathers, copies and merges) and fail on a launch error -- a kernel that never started would leave stale candidates
+// behind.
+template <typename... KArgs, typename... Args>
+static int score_launch(pio_als_handle* h, void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, unsigned path,
+                        Args... args) {
+  if (smem) {
+    const int rc = ensure_dyn_smem(h, (const void*)kernel, smem);
+    if (rc) return rc;
+  }
+  kernel<<<grid, block, smem, h->stream>>>(args...);
+  LAUNCHED(h);
+  h->st.last_score_path |= path;
+  CK(h, cudaGetLastError());
   return PIO_ALS_OK;
 }
-}  // extern "C++"
-extern "C++" {
-template <int KPT>
-static int launch_cos_blocked_kp(pio_als_handle* h, dim3 grid, size_t smem, const float* d_qf, const int* d_bq0, const int* d_bv0,
-                                 int n_bins, const int* d_vq, const long long* d_qptr, const int* d_qid, const uint8_t* d_mask,
-                                 const double* d_weight, int keep, int topk, ScoreIdx* d_cand) {
-  ENSURE_SMEM(h, score_cos_blocked_kernel<KPT>, smem);
-  score_cos_blocked_kernel<KPT><<<grid, 32 * DB_WARPS, smem, h->stream>>>(h->I.F, h->I.n_internal, h->cfg.rank, d_qf, d_bq0, d_bv0,
-                                                                         n_bins, d_vq, d_qptr, d_qid, h->I.cand_ext, d_mask,
-                                                                         d_weight, keep, topk, d_cand);
-  SCORE_LAUNCHED(h, PIO_ALS_PATH_COS_BLOCKED);
-  return PIO_ALS_OK;
-}
-}  // extern "C++"
-static int launch_cos_blocked(pio_als_handle* h, dim3 grid, size_t smem, const float* d_qf, const int* d_bq0, const int* d_bv0,
-                              int n_bins, const int* d_vq, const long long* d_qptr, const int* d_qid, const uint8_t* d_mask,
-                              const double* d_weight, int keep, int topk, ScoreIdx* d_cand) {
-  if (h->KP == 16)
-    return launch_cos_blocked_kp<16>(h, grid, smem, d_qf, d_bq0, d_bv0, n_bins, d_vq, d_qptr, d_qid, d_mask, d_weight, keep, topk, d_cand);
-  if (h->KP == 32)
-    return launch_cos_blocked_kp<32>(h, grid, smem, d_qf, d_bq0, d_bv0, n_bins, d_vq, d_qptr, d_qid, d_mask, d_weight, keep, topk, d_cand);
-  return launch_cos_blocked_kp<64>(h, grid, smem, d_qf, d_bq0, d_bv0, n_bins, d_vq, d_qptr, d_qid, d_mask, d_weight, keep, topk, d_cand);
-}
-static int launch_dot_blocked(pio_als_handle* h, dim3 grid, size_t smem, const float* d_xq, const uint8_t* d_valid, int nq,
-                              const uint8_t* d_mask, const double* d_weight, int topk, ScoreIdx* d_cand) {
-  if (h->KP == 16) return launch_dot_blocked_kp<16>(h, grid, smem, d_xq, d_valid, nq, d_mask, d_weight, topk, d_cand);
-  if (h->KP == 32) return launch_dot_blocked_kp<32>(h, grid, smem, d_xq, d_valid, nq, d_mask, d_weight, topk, d_cand);
-  return launch_dot_blocked_kp<64>(h, grid, smem, d_xq, d_valid, nq, d_mask, d_weight, topk, d_cand);
+
+template <int N>
+using IntC = std::integral_constant<int, N>;
+// f(IntC<KP>()) for the handle's padded rank: the blocked and single-query kernels exist for KP 16, 32 and 64
+template <class F>
+static int with_kp(int kp, F&& f) {
+  if (kp == 16) return f(IntC<16>());
+  if (kp == 32) return f(IntC<32>());
+  return f(IntC<64>());
 }
 
-// recommend for n <= SB_QB users and topk <= TK_MAXK: three launches and one synchronisation
-static int recommend_small(pio_als_handle* h, const int32_t* users, int n, int topk, const uint8_t* item_mask,
-                           const double* item_weight, int32_t* out_items, float* out_scores, int32_t* out_count) {
+static ScoreEnv score_env(const pio_als_handle* h) {
+  return ScoreEnv{h->KP, h->sm_count, h->I.n_internal, h->serve_fused, h->score_blocked};
+}
+
+struct DevFilter {
+  uint8_t* mask = nullptr;
+  double* weight = nullptr;
+};
+// arena bytes of a call's item mask and weights (either may be absent)
+static size_t filter_bytes(const pio_als_handle* h, const uint8_t* mask, const double* weight) {
+  return al256(mask ? (size_t)h->I.n : 0) + al256(weight ? sizeof(double) * (size_t)h->I.n : 0);
+}
+// the call's item mask and weights on the device: in call scratch, or (tmp == nullptr) in the device arena at `at`
+static int upload_filter(pio_als_handle* h, const uint8_t* mask, const double* weight, Scratch* tmp, size_t at, DevFilter* f) {
+  const size_t n = (size_t)h->I.n;
+  if (mask) {
+    if (tmp) CK(h, tmp->alloc(&f->mask, n));
+    else f->mask = h->srv_dev + at;
+    CK(h, cudaMemcpyAsync(f->mask, mask, n, cudaMemcpyHostToDevice, h->stream));
+  }
+  if (weight) {
+    if (tmp) CK(h, tmp->alloc(&f->weight, n));
+    else f->weight = (double*)(h->srv_dev + at + al256(mask ? n : 0));
+    CK(h, cudaMemcpyAsync(f->weight, weight, sizeof(double) * n, cudaMemcpyHostToDevice, h->stream));
+  }
+  return PIO_ALS_OK;
+}
+
+// where the merge writes: ids, scores and counts of every query, and the bounds of the next pass (multi-pass plans)
+struct MergeOut {
+  int* items = nullptr;
+  float* scores = nullptr;
+  int* count = nullptr;
+  ScoreIdx* bound = nullptr;
+};
+// device results of n queries in call scratch
+static int alloc_results(pio_als_handle* h, Scratch& tmp, int n, int topk, bool bound, MergeOut* o) {
+  CK(h, tmp.alloc(&o->items, (size_t)n * topk));
+  CK(h, tmp.alloc(&o->scores, (size_t)n * topk));
+  CK(h, tmp.alloc(&o->count, (size_t)n));
+  if (bound) CK(h, tmp.alloc(&o->bound, (size_t)n));
+  return PIO_ALS_OK;
+}
+// device results to the caller: three copies and one synchronisation
+static int deliver(pio_als_handle* h, const MergeOut& o, int n, int topk, int32_t* items, float* scores, int32_t* count) {
   cudaStream_t st = h->stream;
+  CK(h, cudaMemcpyAsync(items, o.items, sizeof(int) * (size_t)n * topk, cudaMemcpyDeviceToHost, st));
+  CK(h, cudaMemcpyAsync(scores, o.scores, sizeof(float) * (size_t)n * topk, cudaMemcpyDeviceToHost, st));
+  if (count) CK(h, cudaMemcpyAsync(count, o.count, sizeof(int) * (size_t)n, cudaMemcpyDeviceToHost, st));
+  CK(h, cudaStreamSynchronize(st));
+  return PIO_ALS_OK;
+}
+// results of the serving paths, in the mapped host arena: ids, scores and counts of up to cap queries
+struct MappedOut {
+  size_t items, scores, count;
+  MappedOut(ArenaLayout& host, int cap, int topk)
+      : items(host.take(sizeof(int) * (size_t)cap * topk)), scores(host.take(sizeof(float) * (size_t)cap * topk)),
+        count(host.take(sizeof(int) * (size_t)cap)) {}
+  MergeOut dev(const pio_als_handle* h) const {
+    MergeOut o;
+    o.items = (int*)(h->srv_host_dev + items);
+    o.scores = (float*)(h->srv_host_dev + scores);
+    o.count = (int*)(h->srv_host_dev + count);
+    return o;
+  }
+  // once the writer has finished
+  void copy(const pio_als_handle* h, int n, int topk, int32_t* out_items, float* out_scores, int32_t* out_count) const {
+    memcpy(out_items, h->srv_host + items, sizeof(int) * (size_t)n * topk);
+    memcpy(out_scores, h->srv_host + scores, sizeof(float) * (size_t)n * topk);
+    if (out_count) memcpy(out_count, h->srv_host + count, sizeof(int) * (size_t)n);
+  }
+};
+
+// one launch of a pass: the query groups [g0, g0 + grid.y)
+struct Chunk {
+  dim3 grid;               // (gx, groups of this launch)
+  int g0;                  // first group
+  int q0, nq;              // first query and queries of these groups (plans with qpg > 0)
+  int pk;                  // results of this pass
+  const ScoreIdx* bound;   // bound of the first query (nullptr in the first pass)
+  ScoreIdx* cand;          // candidate lists of the first query
+};
+// The passes of a plan: in each, the scoring launches (launch(chunk), at most p.chunk query groups each), then the
+// merge of every query's candidate lists into the results; the last result of a full pass bounds the next one.
+template <class Launch>
+static int run_passes(pio_als_handle* h, const ScorePlan& p, int n_queries, int topk, ScoreIdx* cand, const MergeOut& out,
+                      Launch&& launch) {
+  for (int done = 0; done < topk; done += TK_MAXK) {
+    const int pk = topk - done < TK_MAXK ? topk - done : TK_MAXK;
+    if (done > 0) h->st.last_score_path |= PIO_ALS_PATH_MULTI_PASS;
+    for (int g0 = 0; g0 < p.ngroups; g0 += p.chunk) {
+      const int ng = p.ngroups - g0 < p.chunk ? p.ngroups - g0 : p.chunk;
+      Chunk c;
+      c.grid = dim3(p.gx, ng);
+      c.g0 = g0;
+      c.q0 = g0 * p.qpg;
+      c.nq = n_queries - c.q0 < ng * p.qpg ? n_queries - c.q0 : ng * p.qpg;
+      c.pk = pk;
+      c.bound = done > 0 ? out.bound + c.q0 : nullptr;
+      c.cand = cand + (size_t)c.q0 * p.lists * pk;
+      const int rc = launch(c);
+      if (rc) return rc;
+    }
+    // the candidate lists of a query are [lists][pk] entries, stored with stride pk
+    const int rc = score_launch(h, topk_merge_kernel, dim3(n_queries), dim3(TK_THREADS), 0, 0, (const ScoreIdx*)cand,
+                                p.lists * pk, pk, topk, done, out.items, out.scores, out.count, out.bound);
+    if (rc) return rc;
+  }
+  return PIO_ALS_OK;
+}
+
+// the recommend kernel of the plan for the users of chunk c (xq / valid: the gathered user vectors)
+static int launch_dot(pio_als_handle* h, const ScorePlan& p, const Chunk& c, const float* d_xq, const uint8_t* d_valid,
+                      const DevFilter& f) {
+  const float* xq = d_xq + (size_t)c.q0 * h->KP;
+  if (p.kernel == PIO_ALS_PATH_DOT_BLOCKED)
+    return with_kp(h->KP, [&](auto kp) {
+      return score_launch(h, score_dot_blocked_kernel<decltype(kp)::value>, c.grid, dim3(p.threads), p.smem, p.kernel, h->I.F,
+                          h->I.n_internal, xq, d_valid + c.q0, c.nq, h->I.cand_ext, f.mask, f.weight, c.pk, c.cand);
+    });
+  return score_launch(h, score_dot_topk_batched_kernel, c.grid, dim3(p.threads), p.smem, p.kernel, h->I.F, h->I.n_internal,
+                      h->KP, xq, d_valid + c.q0, c.nq, h->I.cand_ext, f.mask, f.weight, c.bound, c.pk, c.cand);
+}
+
+// the query vectors of a similar batch on the device: the vectors (qf), the first query (q0, bins only) and the first
+// vector (v0) of every bin / group, the query of every vector (vq) and the id list of every query (qptr / qid)
+struct CosQueries {
+  const float* qf;
+  const int* q0;
+  const int* v0;
+  int n_bins;
+  const int* vq;
+  const long long* qptr;
+  const int* qid;
+  int keep;   // PIO_ALS_SIM_KEEP_QUERY_ITEMS
+};
+// the batch similar kernel of the plan for the bins / groups of chunk c
+static int launch_cos(pio_als_handle* h, const ScorePlan& p, const Chunk& c, const CosQueries& q, const DevFilter& f) {
+  if (p.kernel == PIO_ALS_PATH_COS_BLOCKED)
+    return with_kp(h->KP, [&](auto kp) {
+      return score_launch(h, score_cos_blocked_kernel<decltype(kp)::value>, c.grid, dim3(p.threads), p.smem, p.kernel, h->I.F,
+                          h->I.n_internal, h->cfg.rank, q.qf, q.q0 + (size_t)c.g0 * DB_WPR, q.v0 + (size_t)c.g0 * DB_WPR,
+                          q.n_bins - c.g0 * DB_WPR, q.vq, q.qptr, q.qid, h->I.cand_ext, f.mask, f.weight, q.keep, c.pk, c.cand);
+    });
+  return score_launch(h, score_cos_topk_multi_kernel, c.grid, dim3(p.threads), p.smem, p.kernel, h->I.F, h->I.n_internal,
+                      h->KP, h->cfg.rank, q.qf, q.v0 + c.g0, q.vq, q.qptr + c.q0, q.qid, c.nq, h->I.cand_ext, f.mask, f.weight,
+                      c.bound, q.keep, c.pk, c.cand);
+}
+
+// R2: n <= SB_QB users, topk <= TK_MAXK, in the serving arenas: three launches and one synchronisation
+static int recommend_small(pio_als_handle* h, const ScorePlan& p, const int32_t* users, int n, int topk,
+                           const uint8_t* item_mask, const double* item_weight, int32_t* out_items, float* out_scores,
+                           int32_t* out_count) {
   const int KP = h->KP;
-  const int ntiles = (h->I.n_internal + SB_THREADS - 1) / SB_THREADS;
-  int gx = 2 * h->sm_count;
-  if (gx > (ntiles + 7) / 8) gx = (ntiles + 7) / 8;
-  if (gx < 1) gx = 1;
-  const size_t o_xq = 0, o_valid = al256(o_xq + sizeof(float) * SB_QB * KP), o_cand = al256(o_valid + SB_QB),
-               o_mask = al256(o_cand + sizeof(ScoreIdx) * (size_t)SB_QB * gx * topk),
-               o_w = al256(o_mask + (item_mask ? (size_t)h->I.n : 0)),
-               dev_bytes = al256(o_w + (item_weight ? sizeof(double) * (size_t)h->I.n : 0));
-  const size_t ho_i = 0, ho_s = al256(sizeof(int) * (size_t)SB_QB * topk), ho_c = ho_s + al256(sizeof(float) * (size_t)SB_QB * topk),
-               host_bytes = ho_c + al256(sizeof(int) * SB_QB);
-  int rc = serve_reserve(h, dev_bytes, host_bytes);
+  ArenaLayout dev, host;
+  const size_t o_xq = dev.take(sizeof(float) * SB_QB * KP), o_valid = dev.take(SB_QB),
+               o_cand = dev.take(sizeof(ScoreIdx) * (size_t)SB_QB * p.gx * topk),
+               o_filter = dev.take(filter_bytes(h, item_mask, item_weight));
+  const MappedOut res(host, SB_QB, topk);
+  int rc = serve_reserve(h, dev.bytes, host.bytes);
   if (rc) return rc;
   float* d_xq = (float*)(h->srv_dev + o_xq);
   uint8_t* d_valid = h->srv_dev + o_valid;
-  ScoreIdx* d_cand = (ScoreIdx*)(h->srv_dev + o_cand);
-  uint8_t* d_mask = item_mask ? h->srv_dev + o_mask : nullptr;
-  double* d_weight = item_weight ? (double*)(h->srv_dev + o_w) : nullptr;
-  if (item_mask) CK(h, cudaMemcpyAsync(d_mask, item_mask, (size_t)h->I.n, cudaMemcpyHostToDevice, st));
-  if (item_weight) CK(h, cudaMemcpyAsync(d_weight, item_weight, sizeof(double) * (size_t)h->I.n, cudaMemcpyHostToDevice, st));
-  const size_t sb_smem = sizeof(double) * (size_t)KP * SB_QB + sb_tile_bytes(KP) + (sizeof(double) + sizeof(int)) * (size_t)SB_QB * topk;
-  ENSURE_SMEM(h, score_dot_topk_batched_kernel, sb_smem);
+  DevFilter f;
+  rc = upload_filter(h, item_mask, item_weight, nullptr, o_filter, &f);
+  if (rc) return rc;
   IdList ids;
   for (int q = 0; q < n; ++q) ids.v[q] = users[q];
-  gather_rows_ids_kernel<<<n, 64, 0, st>>>(h->U.F, KP, ids, h->U.perm, h->U.deg, h->U.n, d_xq, d_valid);
-  SCORE_LAUNCHED(h, 0);
-  score_dot_topk_batched_kernel<<<dim3(gx, 1), SB_THREADS, sb_smem, st>>>(h->I.F, h->I.n_internal, KP, d_xq, d_valid, n,
-                                                                         h->I.cand_ext, d_mask, d_weight, nullptr, topk, d_cand);
-  SCORE_LAUNCHED(h, PIO_ALS_PATH_DOT_BATCHED);
-  int* m_oi = (int*)(h->srv_host_dev + ho_i);
-  float* m_os = (float*)(h->srv_host_dev + ho_s);
-  int* m_oc = (int*)(h->srv_host_dev + ho_c);
-  topk_merge_kernel<<<n, TK_THREADS, 0, st>>>(d_cand, gx * topk, topk, topk, 0, m_oi, m_os, m_oc, nullptr);
-  SCORE_LAUNCHED(h, 0);
-  CK(h, cudaStreamSynchronize(st));
-  memcpy(out_items, h->srv_host + ho_i, sizeof(int) * (size_t)n * topk);
-  memcpy(out_scores, h->srv_host + ho_s, sizeof(float) * (size_t)n * topk);
-  if (out_count) memcpy(out_count, h->srv_host + ho_c, sizeof(int) * (size_t)n);
+  rc = score_launch(h, gather_rows_ids_kernel, dim3(n), dim3(64), 0, 0, h->U.F, KP, ids, h->U.perm, h->U.deg, h->U.n, d_xq,
+                    d_valid);
+  if (rc) return rc;
+  rc = run_passes(h, p, n, topk, (ScoreIdx*)(h->srv_dev + o_cand), res.dev(h),
+                  [&](const Chunk& c) { return launch_dot(h, p, c, d_xq, d_valid, f); });
+  if (rc) return rc;
+  CK(h, cudaStreamSynchronize(h->stream));
+  res.copy(h, n, topk, out_items, out_scores, out_count);
   return PIO_ALS_OK;
 }
 
-// one similar() query with nq <= SM_NV items and topk <= TK_MAXK: query items without a factor enter as zero vectors (their
-// cosine terms are exactly 0, like the reference skipping them), so no host round trip is needed to compact the query
-static int similar_small(pio_als_handle* h, const int32_t* query_items, int nq, int topk, const uint8_t* item_mask,
-                         const double* item_weight, int flags, int32_t* out_items, float* out_scores, int32_t* out_count) {
-  cudaStream_t st = h->stream;
-  const int KP = h->KP, k = h->cfg.rank;
-  const int ntiles = (h->I.n_internal + SB_THREADS - 1) / SB_THREADS;
-  int gx = 2 * h->sm_count;
-  if (gx > (ntiles + 7) / 8) gx = (ntiles + 7) / 8;
-  if (gx < 1) gx = 1;
-  const size_t o_qf = 0, o_cand = al256(sizeof(float) * SM_NV * KP), o_mask = al256(o_cand + sizeof(ScoreIdx) * (size_t)gx * topk),
-               o_w = al256(o_mask + (item_mask ? (size_t)h->I.n : 0)),
-               dev_bytes = al256(o_w + (item_weight ? sizeof(double) * (size_t)h->I.n : 0));
+// S2: one similar() query with nq <= SM_NV items and topk <= TK_MAXK, in the serving arenas: query items without a factor
+// enter as zero vectors (their cosine terms are exactly 0, like the reference skipping them), so no host round trip is
+// needed to compact the query
+static int similar_small(pio_als_handle* h, const ScorePlan& p, const int32_t* query_items, int nq, int topk,
+                         const uint8_t* item_mask, const double* item_weight, int flags, int32_t* out_items,
+                         float* out_scores, int32_t* out_count) {
+  ArenaLayout dev, host;
+  const size_t o_qf = dev.take(sizeof(float) * SM_NV * h->KP), o_cand = dev.take(sizeof(ScoreIdx) * (size_t)p.gx * topk),
+               o_filter = dev.take(filter_bytes(h, item_mask, item_weight));
   // mapped host arena: results, then the tiny query description the kernel reads over PCIe
-  const size_t ho_i = 0, ho_s = al256(sizeof(int) * (size_t)topk), ho_c = ho_s + al256(sizeof(float) * (size_t)topk),
-               ho_g = ho_c + 256, ho_vq = ho_g + 256, ho_qp = ho_vq + 256, ho_qid = ho_qp + 256, host_bytes = ho_qid + 256;
-  int rc = serve_reserve(h, dev_bytes, host_bytes);
+  const MappedOut res(host, 1, topk);
+  const size_t ho_g = host.take(sizeof(int) * 2), ho_vq = host.take(sizeof(int) * SM_NV),
+               ho_qp = host.take(sizeof(long long) * 2), ho_qid = host.take(sizeof(int) * SM_NV);
+  int rc = serve_reserve(h, dev.bytes, host.bytes);
   if (rc) return rc;
   float* d_qf = (float*)(h->srv_dev + o_qf);
-  ScoreIdx* d_cand = (ScoreIdx*)(h->srv_dev + o_cand);
-  uint8_t* d_mask = item_mask ? h->srv_dev + o_mask : nullptr;
-  double* d_weight = item_weight ? (double*)(h->srv_dev + o_w) : nullptr;
-  if (item_mask) CK(h, cudaMemcpyAsync(d_mask, item_mask, (size_t)h->I.n, cudaMemcpyHostToDevice, st));
-  if (item_weight) CK(h, cudaMemcpyAsync(d_weight, item_weight, sizeof(double) * (size_t)h->I.n, cudaMemcpyHostToDevice, st));
+  DevFilter f;
+  rc = upload_filter(h, item_mask, item_weight, nullptr, o_filter, &f);
+  if (rc) return rc;
   int* hg = (int*)(h->srv_host + ho_g);
   int* hvq = (int*)(h->srv_host + ho_vq);
   long long* hqp = (long long*)(h->srv_host + ho_qp);
@@ -1976,103 +2095,69 @@ static int similar_small(pio_als_handle* h, const int32_t* query_items, int nq, 
   hqp[0] = 0; hqp[1] = nq;
   IdList ids;
   for (int q = 0; q < nq; ++q) { ids.v[q] = query_items[q]; hvq[q] = 0; hqid[q] = query_items[q]; }
-  const size_t smem = sizeof(double) * ((size_t)KP * SM_NV + SM_NV) + sb_tile_bytes(KP) +
-                      (sizeof(double) + sizeof(int)) * (size_t)SM_QG * topk + sizeof(int) * (SM_NV + SM_QG * SM_QIDS) + 16;
-  ENSURE_SMEM(h, score_cos_topk_multi_kernel, smem);
-  gather_rows_ids_kernel<<<nq, 64, 0, st>>>(h->I.F, KP, ids, h->I.perm, h->I.deg, h->I.n, d_qf, nullptr);
-  SCORE_LAUNCHED(h, 0);
-  score_cos_topk_multi_kernel<<<dim3(gx, 1), SB_THREADS, smem, st>>>(
-      h->I.F, h->I.n_internal, KP, k, d_qf, (const int*)(h->srv_host_dev + ho_g), (const int*)(h->srv_host_dev + ho_vq),
-      (const long long*)(h->srv_host_dev + ho_qp), (const int*)(h->srv_host_dev + ho_qid), 1, h->I.cand_ext, d_mask, d_weight,
-      nullptr, (flags & PIO_ALS_SIM_KEEP_QUERY_ITEMS) ? 1 : 0, topk, d_cand);
-  SCORE_LAUNCHED(h, PIO_ALS_PATH_COS_MULTI);
-  topk_merge_kernel<<<1, TK_THREADS, 0, st>>>(d_cand, gx * topk, topk, topk, 0, (int*)(h->srv_host_dev + ho_i),
-                                              (float*)(h->srv_host_dev + ho_s), (int*)(h->srv_host_dev + ho_c), nullptr);
-  SCORE_LAUNCHED(h, 0);
-  CK(h, cudaStreamSynchronize(st));
-  memcpy(out_items, h->srv_host + ho_i, sizeof(int) * (size_t)topk);
-  memcpy(out_scores, h->srv_host + ho_s, sizeof(float) * (size_t)topk);
-  if (out_count) *out_count = *(int*)(h->srv_host + ho_c);
+  rc = score_launch(h, gather_rows_ids_kernel, dim3(nq), dim3(64), 0, 0, h->I.F, h->KP, ids, h->I.perm, h->I.deg, h->I.n,
+                    d_qf, (uint8_t*)nullptr);
+  if (rc) return rc;
+  const CosQueries q{d_qf, nullptr, (const int*)(h->srv_host_dev + ho_g), 1, (const int*)(h->srv_host_dev + ho_vq),
+                     (const long long*)(h->srv_host_dev + ho_qp), (const int*)(h->srv_host_dev + ho_qid),
+                     (flags & PIO_ALS_SIM_KEEP_QUERY_ITEMS) ? 1 : 0};
+  rc = run_passes(h, p, 1, topk, (ScoreIdx*)(h->srv_dev + o_cand), res.dev(h),
+                  [&](const Chunk& c) { return launch_cos(h, p, c, q, f); });
+  if (rc) return rc;
+  CK(h, cudaStreamSynchronize(h->stream));
+  res.copy(h, 1, topk, out_items, out_scores, out_count);
   return PIO_ALS_OK;
 }
 
-// ONE query in ONE launch (score_one_kernel): recommend for one user (cos = false, ids[0] = the user) or similar for
-// nq <= S1_MAXNV query items.  The host waits on a sequence flag in the mapped arena instead of a stream synchronisation.
-extern "C++" {
-template <bool COS, int NVP, int KPT>
-static int launch_score_one_kp(pio_als_handle* h, int gx, size_t smem, const Side& q, const OneQuery& qry, const uint8_t* d_mask,
-                               const double* d_weight, int keep, int topk, ScoreIdx* d_cand, int* m_oi, float* m_os, int* m_oc,
-                               unsigned* m_flag, unsigned seq, unsigned long long* m_trace) {
-  ENSURE_SMEM(h, (score_one_kernel<COS, NVP, KPT>), smem);
-  unsigned long long* g_thr = reinterpret_cast<unsigned long long*>(h->srv_counter + 2);
-  score_one_kernel<COS, NVP, KPT><<<gx, S1_THREADS, smem, h->stream>>>(
-      h->I.F, h->I.n_internal, h->cfg.rank, q.F, q.perm, q.deg, q.n, qry, h->I.cand_ext, d_mask, d_weight, keep, topk, d_cand,
-      h->srv_counter, g_thr, m_oi, m_os, m_oc, m_flag, seq, m_trace);
-  SCORE_LAUNCHED(h, PIO_ALS_PATH_SCORE_ONE);
-  return PIO_ALS_OK;
-}
-template <bool COS, int NVP>
-static int launch_score_one(pio_als_handle* h, int gx, size_t smem, const Side& q, const OneQuery& qry, const uint8_t* d_mask,
-                            const double* d_weight, int keep, int topk, ScoreIdx* d_cand, int* m_oi, float* m_os, int* m_oc,
-                            unsigned* m_flag, unsigned seq, unsigned long long* m_trace) {
-  if (h->KP == 16) return launch_score_one_kp<COS, NVP, 16>(h, gx, smem, q, qry, d_mask, d_weight, keep, topk, d_cand, m_oi, m_os, m_oc, m_flag, seq, m_trace);
-  if (h->KP == 32) return launch_score_one_kp<COS, NVP, 32>(h, gx, smem, q, qry, d_mask, d_weight, keep, topk, d_cand, m_oi, m_os, m_oc, m_flag, seq, m_trace);
-  return launch_score_one_kp<COS, NVP, 64>(h, gx, smem, q, qry, d_mask, d_weight, keep, topk, d_cand, m_oi, m_os, m_oc, m_flag, seq, m_trace);
-}
-}  // extern "C++"
-
-static bool serve_one_ok(const pio_als_handle* h, int nq, int topk) {
-  return h->serve_fused && h->KP <= 64 && topk <= TK_MAXK && nq >= 1 && nq <= S1_MAXNV;
-}
-
-static int serve_one(pio_als_handle* h, bool cos, const int32_t* ids, int nq, int topk, const uint8_t* item_mask,
-                     const double* item_weight, int flags, int32_t* out_items, float* out_scores, int32_t* out_count) {
+// R1 / S1: ONE query in ONE launch (score_one_kernel): recommend for one user (cos = false, ids[0] = the user) or similar
+// for nq <= S1_MAXNV query items.  The host waits on a sequence flag in the mapped arena instead of a stream
+// synchronisation.
+static int serve_one(pio_als_handle* h, const ScorePlan& p, bool cos, const int32_t* ids, int nq, int topk,
+                     const uint8_t* item_mask, const double* item_weight, int flags, int32_t* out_items, float* out_scores,
+                     int32_t* out_count) {
   cudaStream_t st = h->stream;
-  const int KP = h->KP;
-  const int ntiles = (h->I.n_internal + S1_THREADS - 1) / S1_THREADS;
-  int gx = h->sm_count < ntiles ? h->sm_count : ntiles;
-  if (gx > S1_THREADS) gx = S1_THREADS;   // the list merge reads one list head per thread
-  if (gx < 1) gx = 1;
-  const int nvp = !cos ? 1 : nq <= 1 ? 1 : nq <= 2 ? 2 : nq <= 4 ? 4 : 8;
-  const size_t o_cand = 0, o_mask = al256(sizeof(ScoreIdx) * (size_t)gx * topk),
-               o_w = al256(o_mask + (item_mask ? (size_t)h->I.n : 0)),
-               dev_bytes = al256(o_w + (item_weight ? sizeof(double) * (size_t)h->I.n : 0));
-  const size_t ho_i = 0, ho_s = al256(sizeof(int) * (size_t)topk), ho_c = ho_s + al256(sizeof(float) * (size_t)topk),
-               ho_flag = ho_c + 256, ho_trace = ho_flag + 256, host_bytes = ho_trace + 256;
-  const bool fresh_host = h->srv_host_cap < host_bytes;
-  int rc = serve_reserve(h, dev_bytes, host_bytes);
+  ArenaLayout dev, host;
+  const size_t o_cand = dev.take(sizeof(ScoreIdx) * (size_t)p.gx * topk),
+               o_filter = dev.take(filter_bytes(h, item_mask, item_weight));
+  const MappedOut res(host, 1, topk);
+  const size_t ho_flag = host.take(sizeof(unsigned)), ho_trace = host.take(sizeof(unsigned long long) * 8);
+  const bool fresh_host = h->srv_host_cap < host.bytes;
+  int rc = serve_reserve(h, dev.bytes, host.bytes);
   if (rc) return rc;
   if (fresh_host) memset(h->srv_host, 0, h->srv_host_cap);
   if (!h->srv_counter) {
     CK(h, cudaMalloc((void**)&h->srv_counter, 256));
     CK(h, cudaMemsetAsync(h->srv_counter, 0, 256, st));
   }
-  ScoreIdx* d_cand = (ScoreIdx*)(h->srv_dev + o_cand);
-  uint8_t* d_mask = item_mask ? h->srv_dev + o_mask : nullptr;
-  double* d_weight = item_weight ? (double*)(h->srv_dev + o_w) : nullptr;
-  if (item_mask) CK(h, cudaMemcpyAsync(d_mask, item_mask, (size_t)h->I.n, cudaMemcpyHostToDevice, st));
-  if (item_weight) CK(h, cudaMemcpyAsync(d_weight, item_weight, sizeof(double) * (size_t)h->I.n, cudaMemcpyHostToDevice, st));
+  DevFilter f;
+  rc = upload_filter(h, item_mask, item_weight, nullptr, o_filter, &f);
+  if (rc) return rc;
   OneQuery qry;
   qry.nq = nq;
   for (int t = 0; t < S1_MAXNV; ++t) qry.ids[t] = t < nq ? ids[t] : -1;
   const unsigned seq = ++h->srv_seq ? h->srv_seq : ++h->srv_seq;   // never 0: a fresh arena reads 0
   volatile unsigned* flag = (volatile unsigned*)(h->srv_host + ho_flag);
-  int* m_oi = (int*)(h->srv_host_dev + ho_i);
-  float* m_os = (float*)(h->srv_host_dev + ho_s);
-  int* m_oc = (int*)(h->srv_host_dev + ho_c);
+  const MergeOut m = res.dev(h);
   unsigned* m_flag = (unsigned*)(h->srv_host_dev + ho_flag);
-  const size_t smem = s1_smem_bytes(KP, nvp, topk);
+  unsigned long long* m_trace = h->serve_trace ? (unsigned long long*)(h->srv_host_dev + ho_trace) : nullptr;
+  unsigned long long* g_thr = reinterpret_cast<unsigned long long*>(h->srv_counter + 2);
+  ScoreIdx* d_cand = (ScoreIdx*)(h->srv_dev + o_cand);
   const int keep = (flags & PIO_ALS_SIM_KEEP_QUERY_ITEMS) ? 1 : 0;
   const Side& q = cos ? h->I : h->U;
-  unsigned long long* m_trace = h->serve_trace ? (unsigned long long*)(h->srv_host_dev + ho_trace) : nullptr;
+  const auto launch = [&](auto c, auto nvp, auto kp) {
+    return score_launch(h, score_one_kernel<decltype(c)::value, decltype(nvp)::value, decltype(kp)::value>, dim3(p.gx),
+                        dim3(p.threads), p.smem, p.kernel, h->I.F, h->I.n_internal, h->cfg.rank, q.F, q.perm, q.deg, q.n, qry,
+                        h->I.cand_ext, f.mask, f.weight, keep, topk, d_cand, h->srv_counter, g_thr, m.items, m.scores,
+                        m.count, m_flag, seq, m_trace);
+  };
   const auto t_call = std::chrono::steady_clock::now();
-#define PIO_S1(C, N) launch_score_one<C, N>(h, gx, smem, q, qry, d_mask, d_weight, keep, topk, d_cand, m_oi, m_os, m_oc, m_flag, seq, m_trace)
-  if (!cos) rc = PIO_S1(false, 1);
-  else if (nvp == 1) rc = PIO_S1(true, 1);
-  else if (nvp == 2) rc = PIO_S1(true, 2);
-  else if (nvp == 4) rc = PIO_S1(true, 4);
-  else rc = PIO_S1(true, 8);
-#undef PIO_S1
+  rc = with_kp(h->KP, [&](auto kp) {
+    if (!cos) return launch(std::false_type(), IntC<1>(), kp);
+    if (p.nvp == 1) return launch(std::true_type(), IntC<1>(), kp);
+    if (p.nvp == 2) return launch(std::true_type(), IntC<2>(), kp);
+    if (p.nvp == 4) return launch(std::true_type(), IntC<4>(), kp);
+    return launch(std::true_type(), IntC<8>(), kp);
+  });
   if (rc) return rc;
   for (unsigned spins = 1; *flag != seq; ++spins) {
     if ((spins & 0x3FFFu) == 0) {   // a faulted kernel never writes the flag: ask the stream now and then
@@ -2094,113 +2179,68 @@ static int serve_one(pio_als_handle* h, bool cos, const int32_t* ids, int nq, in
             "%.1f us, cta merge + arrival %.1f us, list merge %.1f us, system fence %.1f us\n", host_us, (t[5] - t[0]) * 1e-3,
             (t[6] - t[5]) * 1e-3, (t[1] - t[6]) * 1e-3, (t[2] - t[1]) * 1e-3, (t[3] - t[2]) * 1e-3, (t[4] - t[3]) * 1e-3);
   }
-  memcpy(out_items, h->srv_host + ho_i, sizeof(int) * (size_t)topk);
-  memcpy(out_scores, h->srv_host + ho_s, sizeof(float) * (size_t)topk);
-  if (out_count) *out_count = *(int*)(h->srv_host + ho_c);
+  res.copy(h, 1, topk, out_items, out_scores, out_count);
   return PIO_ALS_OK;
 }
-}  // namespace pio
 
-// Scoring passes: at most TK_MAXK results per pass; a query asking for more runs further passes, each bounded by the last
-// result of the one before (topk.cuh below_bound).
-int pio_als_recommend(pio_als_handle* h, const int32_t* users, int n, int topk, const uint8_t* item_mask,
-                      const double* item_weight, int32_t* out_items, float* out_scores, int32_t* out_count) {
-  if (!h) return PIO_ALS_ERR_ARG;
-  std::lock_guard<std::mutex> lk(h->mu);
-  h->st.last_score_path = 0;   // also for a call that launches nothing
-  if (n < 0 || topk < 1) return fail(h, PIO_ALS_ERR_ARG, "topk must be >= 1 and n >= 0");
-  if (n == 0) return PIO_ALS_OK;
-  if (!users || !out_items || !out_scores) return fail(h, PIO_ALS_ERR_ARG, "null argument");
-  if (!h->U.F || !h->I.F || !h->I.cand_ext) return fail(h, PIO_ALS_ERR_STATE, "no model");
-  CK(h, cudaSetDevice(h->cfg.device));
-  if (n == 1 && serve_one_ok(h, 1, topk))   // the serving case: one query, one launch
-    return serve_one(h, false, users, 1, topk, item_mask, item_weight, 0, out_items, out_scores, out_count);
-  if (n <= SB_QB && topk <= TK_MAXK)   // a few queries
-    return recommend_small(h, users, n, topk, item_mask, item_weight, out_items, out_scores, out_count);
+// S3 / S4: a gathered similar batch (qf_all / valid: the vector of every query id and whether it owns a factor), its
+// queries in the bins / groups q0 of the plan
+static int similar_groups(pio_als_handle* h, const ScorePlan& p, const std::vector<int>& q0, const int64_t* q_ptr,
+                          int n_queries, int topk, const std::vector<uint8_t>& valid, const float* d_qf_all,
+                          const int* d_qid, const DevFilter& f, int flags, Scratch& tmp, int32_t* out_items,
+                          float* out_scores, int32_t* out_count) {
   cudaStream_t st = h->stream;
   const int KP = h->KP;
-  Scratch tmp(h);
-  int* d_users = nullptr;
-  float* d_xq = nullptr;
-  uint8_t *d_valid = nullptr, *d_mask = nullptr;
-  double* d_weight = nullptr;
-  ScoreIdx *d_cand = nullptr, *d_bound = nullptr;
-  int *d_oi = nullptr, *d_oc = nullptr;
-  float* d_os = nullptr;
-  const int pass_max = topk < TK_MAXK ? topk : TK_MAXK;
-  // batched scoring: groups of SB_QB queries share every staged item tile; GX persistent CTAs per group
-  const int ngroups = (n + SB_QB - 1) / SB_QB;
-  const int ntiles = (h->I.n_internal + SB_THREADS - 1) / SB_THREADS;
-  int gx = (2 * h->sm_count + ngroups - 1) / ngroups;
-  if (gx > (ntiles + 7) / 8) gx = (ntiles + 7) / 8;   // at least eight tiles per CTA: the pools must warm up
-  if (gx < 1) gx = 1;
-  const size_t sb_smem = sizeof(double) * (size_t)KP * SB_QB + sb_tile_bytes(KP) +
-                         (sizeof(double) + sizeof(int)) * (size_t)SB_QB * pass_max;
-  // blocked kernel (two items x 16 queries per thread, independent warps): rank <= 64, topk <= DB_MAXK
-  const bool blocked = h->score_blocked && KP <= 64 && topk <= DB_MAXK;
-  if (blocked) {
-    const int nsteps = (h->I.n_internal + DB_RINGS * DB_ROWS - 1) / (DB_RINGS * DB_ROWS);
-    gx = (h->sm_count + ngroups - 1) / ngroups;
-    if (gx > (nsteps + 7) / 8) gx = (nsteps + 7) / 8;   // at least eight steps per warp: the pools must warm up
-    if (gx < 1) gx = 1;
-  } else {
-    ENSURE_SMEM(h, score_dot_topk_batched_kernel, sb_smem);
+  const bool bins = p.kernel == PIO_ALS_PATH_COS_BLOCKED;
+  // the vectors that own a factor, bin / group after bin / group, query order kept: their row in qf_all, their query
+  // (global in a bin, inside the group in S4) and the first vector of every bin / group
+  std::vector<int> v0, vsrc, vq;
+  for (size_t g = 0; g + 1 < q0.size(); ++g) {
+    v0.push_back((int)vsrc.size());
+    for (int j = q0[g]; j < q0[g + 1]; ++j)
+      for (long long t = q_ptr[j]; t < q_ptr[j + 1]; ++t)
+        if (valid[(size_t)(t - q_ptr[0])]) {
+          vsrc.push_back((int)(t - q_ptr[0]));
+          vq.push_back(bins ? j : j - q0[g]);
+        }
   }
-  const int lists = blocked ? gx * DB_RINGS : gx;        // candidate lists per query
-  CK(h, tmp.alloc(&d_users, (size_t)n));
-  CK(h, tmp.alloc(&d_xq, (size_t)n * KP));
-  CK(h, tmp.alloc(&d_valid, (size_t)n));
-  CK(h, tmp.alloc(&d_cand, (size_t)n * lists * pass_max));
-  CK(h, tmp.alloc(&d_oi, (size_t)n * topk));
-  CK(h, tmp.alloc(&d_os, (size_t)n * topk));
-  CK(h, tmp.alloc(&d_oc, (size_t)n));
-  CK(h, cudaMemcpyAsync(d_users, users, sizeof(int) * n, cudaMemcpyHostToDevice, st));
-  if (item_mask) {
-    CK(h, tmp.alloc(&d_mask, (size_t)h->I.n));
-    CK(h, cudaMemcpyAsync(d_mask, item_mask, (size_t)h->I.n, cudaMemcpyHostToDevice, st));
+  v0.push_back((int)vsrc.size());
+  std::vector<long long> rel((size_t)n_queries + 1);
+  for (int j = 0; j <= n_queries; ++j) rel[j] = q_ptr[j] - q_ptr[0];
+  const int nvec = (int)vsrc.size();
+  const size_t nv1 = nvec > 0 ? (size_t)nvec : 1;
+  int *d_q0 = nullptr, *d_v0 = nullptr, *d_vq = nullptr, *d_vsrc = nullptr;
+  long long* d_qptr = nullptr;
+  float* d_qfc = nullptr;
+  ScoreIdx* d_cand = nullptr;
+  if (bins) CK(h, tmp.alloc(&d_q0, q0.size()));
+  CK(h, tmp.alloc(&d_v0, v0.size()));
+  CK(h, tmp.alloc(&d_vq, nv1));
+  CK(h, tmp.alloc(&d_vsrc, nv1));
+  CK(h, tmp.alloc(&d_qptr, rel.size()));
+  CK(h, tmp.alloc(&d_qfc, nv1 * KP));
+  if (bins) CK(h, cudaMemcpyAsync(d_q0, q0.data(), sizeof(int) * q0.size(), cudaMemcpyHostToDevice, st));
+  CK(h, cudaMemcpyAsync(d_v0, v0.data(), sizeof(int) * v0.size(), cudaMemcpyHostToDevice, st));
+  CK(h, cudaMemcpyAsync(d_qptr, rel.data(), sizeof(long long) * rel.size(), cudaMemcpyHostToDevice, st));
+  if (nvec > 0) {
+    CK(h, cudaMemcpyAsync(d_vq, vq.data(), sizeof(int) * nvec, cudaMemcpyHostToDevice, st));
+    CK(h, cudaMemcpyAsync(d_vsrc, vsrc.data(), sizeof(int) * nvec, cudaMemcpyHostToDevice, st));
+    const int rc = score_launch(h, copy_rows_kernel, dim3(nvec), dim3(64), 0, 0, d_qf_all, KP, (const int*)d_vsrc, d_qfc);
+    if (rc) return rc;
   }
-  if (item_weight) {
-    CK(h, tmp.alloc(&d_weight, (size_t)h->I.n));
-    CK(h, cudaMemcpyAsync(d_weight, item_weight, sizeof(double) * (size_t)h->I.n, cudaMemcpyHostToDevice, st));
-  }
-  if (topk > TK_MAXK) CK(h, tmp.alloc(&d_bound, (size_t)n));
-  gather_rows_kernel<<<n, 64, 0, st>>>(h->U.F, KP, d_users, n, h->U.perm, h->U.deg, h->U.n, d_xq, d_valid);
-  SCORE_LAUNCHED(h, 0);
-  for (int done = 0; done < topk; done += TK_MAXK) {
-    const int pk = topk - done < TK_MAXK ? topk - done : TK_MAXK;
-    if (done > 0) h->st.last_score_path |= PIO_ALS_PATH_MULTI_PASS;
-    // grid.y is limited to 65535 query groups per launch
-    for (int g0 = 0; g0 < ngroups; g0 += 32768) {
-      const int ng = ngroups - g0 < 32768 ? ngroups - g0 : 32768;
-      const int q0 = g0 * SB_QB;
-      const int nq = n - q0 < ng * SB_QB ? n - q0 : ng * SB_QB;
-      if (blocked) {
-        const size_t smem = db_smem_bytes(KP, pk);
-        const int brc = launch_dot_blocked(h, dim3(gx, ng), smem, d_xq + (size_t)q0 * KP, d_valid + q0, nq, d_mask, d_weight, pk,
-                                           d_cand + (size_t)q0 * lists * pk);
-        if (brc) return brc;
-      } else {
-        score_dot_topk_batched_kernel<<<dim3(gx, ng), SB_THREADS, sb_smem, st>>>(
-            h->I.F, h->I.n_internal, KP, d_xq + (size_t)q0 * KP, d_valid + q0, nq, h->I.cand_ext, d_mask, d_weight,
-            (done > 0) ? d_bound + q0 : nullptr, pk, d_cand + (size_t)q0 * lists * pk);
-        SCORE_LAUNCHED(h, PIO_ALS_PATH_DOT_BATCHED);
-      }
-    }
-    // the candidate lists of a query are [lists][pk] entries, stored with stride pk
-    topk_merge_kernel<<<n, TK_THREADS, 0, st>>>(d_cand, lists * pk, pk, topk, done, d_oi, d_os, d_oc, d_bound);
-    SCORE_LAUNCHED(h, 0);
-  }
-  CK(h, cudaMemcpyAsync(out_items, d_oi, sizeof(int) * (size_t)n * topk, cudaMemcpyDeviceToHost, st));
-  CK(h, cudaMemcpyAsync(out_scores, d_os, sizeof(float) * (size_t)n * topk, cudaMemcpyDeviceToHost, st));
-  if (out_count) CK(h, cudaMemcpyAsync(out_count, d_oc, sizeof(int) * (size_t)n, cudaMemcpyDeviceToHost, st));
-  CK(h, cudaStreamSynchronize(st));
-  return PIO_ALS_OK;
+  CK(h, tmp.alloc(&d_cand, (size_t)n_queries * p.lists * p.pass_k));
+  MergeOut o;
+  int rc = alloc_results(h, tmp, n_queries, topk, p.passes > 1, &o);
+  if (rc) return rc;
+  const CosQueries q{d_qfc, d_q0, d_v0, (int)q0.size() - 1, d_vq, d_qptr, d_qid, (flags & PIO_ALS_SIM_KEEP_QUERY_ITEMS) ? 1 : 0};
+  rc = run_passes(h, p, n_queries, topk, d_cand, o, [&](const Chunk& c) { return launch_cos(h, p, c, q, f); });
+  if (rc) return rc;
+  return deliver(h, o, n_queries, topk, out_items, out_scores, out_count);
 }
 
-namespace pio {
-// one similar() query with mask / weights already on the device; results to HOST out arrays (topk entries)
-static int similar_one(pio_als_handle* h, const int32_t* query_items, int nq, int topk, const uint8_t* d_mask,
-                       const double* d_weight, int flags, int32_t* out_items, float* out_scores, int32_t* out_count) {
+// S5: one similar() query with mask / weights already on the device; results to HOST out arrays (topk entries)
+static int similar_one(pio_als_handle* h, const int32_t* query_items, int nq, int topk, const DevFilter& f, int flags,
+                       int32_t* out_items, float* out_scores, int32_t* out_count) {
   for (int t = 0; t < topk; ++t) { out_items[t] = -1; out_scores[t] = 0.f; }
   if (out_count) *out_count = 0;
   if (nq == 0) return PIO_ALS_OK;
@@ -2215,8 +2255,9 @@ static int similar_one(pio_als_handle* h, const int32_t* query_items, int nq, in
   CK(h, tmp.alloc(&d_qf, (size_t)nq * KP));
   CK(h, tmp.alloc(&d_valid, (size_t)nq));
   CK(h, cudaMemcpyAsync(d_q, query_items, sizeof(int) * nq, cudaMemcpyHostToDevice, st));
-  gather_rows_kernel<<<nq, 64, 0, st>>>(h->I.F, KP, d_q, nq, h->I.perm, h->I.deg, h->I.n, d_qf, d_valid);
-  SCORE_LAUNCHED(h, 0);
+  int rc = score_launch(h, gather_rows_kernel, dim3(nq), dim3(64), 0, 0, h->I.F, KP, (const int*)d_q, nq, h->I.perm,
+                        h->I.deg, h->I.n, d_qf, d_valid);
+  if (rc) return rc;
   std::vector<uint8_t> valid(nq);
   CK(h, cudaMemcpyAsync(valid.data(), d_valid, (size_t)nq, cudaMemcpyDeviceToHost, st));
   CK(h, cudaStreamSynchronize(st));
@@ -2224,60 +2265,76 @@ static int similar_one(pio_als_handle* h, const int32_t* query_items, int nq, in
   std::vector<int> keep;
   for (int q = 0; q < nq; ++q)
     if (valid[q]) keep.push_back(q);
-  if (keep.empty()) return PIO_ALS_OK;
+  const int nqv = (int)keep.size();
+  const ScorePlan p = plan_similar_query(score_env(h), nqv, nq, topk);
+  if (p.route == ROUTE_NONE) return PIO_ALS_OK;
   float* d_qc = nullptr;
   CK(h, tmp.alloc(&d_qc, keep.size() * (size_t)KP));
   for (size_t j = 0; j < keep.size(); ++j)
     CK(h, cudaMemcpyAsync(d_qc + j * KP, d_qf + (size_t)keep[j] * KP, sizeof(float) * KP, cudaMemcpyDeviceToDevice, st));
-  const int pass_max = topk < TK_MAXK ? topk : TK_MAXK;
-  // batched kernel (query vectors resident in shared memory) unless the query is too large for it
-  const int nqv = (int)keep.size();
-  const int nqp = (nqv + SC_G - 1) / SC_G * SC_G;
-  constexpr int SC_WARPS = SB_THREADS / 32;   // one candidate pool per warp
-  const size_t sc_smem = sizeof(double) * ((size_t)KP * nqp + nqp) + sizeof(float) * (size_t)SB_THREADS * (KP + 4) +
-                         (sizeof(double) + sizeof(int)) * (size_t)SC_WARPS * pass_max + sizeof(int) * (size_t)nq + 16;
-  const bool batched = sc_smem <= 100 * 1024;
-  int ntiles = (h->I.n_internal + TK_TILE - 1) / TK_TILE;
-  if (batched) {
-    const int nt = (h->I.n_internal + SB_THREADS - 1) / SB_THREADS;
-    ntiles = 2 * h->sm_count < (nt + 7) / 8 ? 2 * h->sm_count : (nt + 7) / 8;   // = CTAs (>= 8 tiles each)
-    ENSURE_SMEM(h, score_cos_topk_batched_kernel, sc_smem);
-  }
-  ScoreIdx *d_cand = nullptr, *d_bound = nullptr;
-  int *d_oi = nullptr, *d_oc = nullptr;
-  float* d_os = nullptr;
-  const int npools = batched ? ntiles * SC_WARPS : ntiles;   // candidate lists of pass_k entries left for the merge
-  CK(h, tmp.alloc(&d_cand, (size_t)npools * pass_max));
-  CK(h, tmp.alloc(&d_oi, (size_t)topk));
-  CK(h, tmp.alloc(&d_os, (size_t)topk));
-  CK(h, tmp.alloc(&d_oc, 1));
-  if (topk > TK_MAXK) CK(h, tmp.alloc(&d_bound, 1));
-  for (int done = 0; done < topk; done += TK_MAXK) {
-    const int pk = topk - done < TK_MAXK ? topk - done : TK_MAXK;
-    const ScoreIdx* bnd = done > 0 ? d_bound : nullptr;
-    if (done > 0) h->st.last_score_path |= PIO_ALS_PATH_MULTI_PASS;
-    if (batched) {
-      score_cos_topk_batched_kernel<<<ntiles, SB_THREADS, sc_smem, st>>>(h->I.F, h->I.n_internal, KP, k, d_qc, d_q, nq, nqv,
-                                                                         h->I.cand_ext, d_mask, d_weight, bnd, keep_query, pk,
-                                                                         d_cand);
-      SCORE_LAUNCHED(h, PIO_ALS_PATH_COS_BATCHED);
-    } else {
-      score_cos_topk_kernel<<<ntiles, TK_THREADS, 0, st>>>(h->I.F, h->I.n_internal, KP, k, d_qc, d_q, nq, nqv, h->I.cand_ext,
-                                                           d_mask, d_weight, bnd, keep_query, pk, d_cand);
-      SCORE_LAUNCHED(h, PIO_ALS_PATH_COS_FALLBACK);
-    }
-    topk_merge_kernel<<<1, TK_THREADS, 0, st>>>(d_cand, npools * pk, pk, topk, done, d_oi, d_os, d_oc, d_bound);
-    SCORE_LAUNCHED(h, 0);
-  }
-  CK(h, cudaMemcpyAsync(out_items, d_oi, sizeof(int) * topk, cudaMemcpyDeviceToHost, st));
-  CK(h, cudaMemcpyAsync(out_scores, d_os, sizeof(float) * topk, cudaMemcpyDeviceToHost, st));
+  ScoreIdx* d_cand = nullptr;
+  CK(h, tmp.alloc(&d_cand, (size_t)p.lists * p.pass_k));
+  MergeOut o;
+  rc = alloc_results(h, tmp, 1, topk, p.passes > 1, &o);
+  if (rc) return rc;
+  rc = run_passes(h, p, 1, topk, d_cand, o, [&](const Chunk& c) {
+    return score_launch(h, p.kernel == PIO_ALS_PATH_COS_BATCHED ? score_cos_topk_batched_kernel : score_cos_topk_kernel,
+                        c.grid, dim3(p.threads), p.smem, p.kernel, h->I.F, h->I.n_internal, KP, k, (const float*)d_qc,
+                        (const int*)d_q, nq, nqv, h->I.cand_ext, f.mask, f.weight, c.bound, keep_query, c.pk, c.cand);
+  });
+  if (rc) return rc;
   int cnt = 0;
-  CK(h, cudaMemcpyAsync(&cnt, d_oc, sizeof(int), cudaMemcpyDeviceToHost, st));
-  CK(h, cudaStreamSynchronize(st));
+  rc = deliver(h, o, 1, topk, out_items, out_scores, &cnt);
+  if (rc) return rc;
   if (out_count) *out_count = cnt;
   return PIO_ALS_OK;
 }
 }  // namespace pio
+
+extern "C" {
+
+// Scoring passes: at most TK_MAXK results per pass; a query asking for more runs further passes, each bounded by the last
+// result of the one before (topk.cuh below_bound).
+int pio_als_recommend(pio_als_handle* h, const int32_t* users, int n, int topk, const uint8_t* item_mask,
+                      const double* item_weight, int32_t* out_items, float* out_scores, int32_t* out_count) {
+  if (!h) return PIO_ALS_ERR_ARG;
+  std::lock_guard<std::mutex> lk(h->mu);
+  h->st.last_score_path = 0;   // also for a call that launches nothing
+  if (n < 0 || topk < 1) return fail(h, PIO_ALS_ERR_ARG, "topk must be >= 1 and n >= 0");
+  if (n == 0) return PIO_ALS_OK;
+  if (!users || !out_items || !out_scores) return fail(h, PIO_ALS_ERR_ARG, "null argument");
+  if (!h->U.F || !h->I.F || !h->I.cand_ext) return fail(h, PIO_ALS_ERR_STATE, "no model");
+  CK(h, cudaSetDevice(h->cfg.device));
+  const ScorePlan p = plan_recommend(score_env(h), n, topk);
+  if (p.route == ROUTE_ONE)   // the serving case: one query, one launch
+    return serve_one(h, p, false, users, 1, topk, item_mask, item_weight, 0, out_items, out_scores, out_count);
+  if (p.route == ROUTE_ARENA)   // a few queries
+    return recommend_small(h, p, users, n, topk, item_mask, item_weight, out_items, out_scores, out_count);
+  cudaStream_t st = h->stream;
+  const int KP = h->KP;
+  Scratch tmp(h);
+  int* d_users = nullptr;
+  float* d_xq = nullptr;
+  uint8_t* d_valid = nullptr;
+  ScoreIdx* d_cand = nullptr;
+  CK(h, tmp.alloc(&d_users, (size_t)n));
+  CK(h, tmp.alloc(&d_xq, (size_t)n * KP));
+  CK(h, tmp.alloc(&d_valid, (size_t)n));
+  CK(h, tmp.alloc(&d_cand, (size_t)n * p.lists * p.pass_k));
+  MergeOut o;
+  int rc = alloc_results(h, tmp, n, topk, p.passes > 1, &o);
+  if (rc) return rc;
+  CK(h, cudaMemcpyAsync(d_users, users, sizeof(int) * n, cudaMemcpyHostToDevice, st));
+  DevFilter f;
+  rc = upload_filter(h, item_mask, item_weight, &tmp, 0, &f);
+  if (rc) return rc;
+  rc = score_launch(h, gather_rows_kernel, dim3(n), dim3(64), 0, 0, h->U.F, KP, (const int*)d_users, n, h->U.perm, h->U.deg,
+                    h->U.n, d_xq, d_valid);
+  if (rc) return rc;
+  rc = run_passes(h, p, n, topk, d_cand, o, [&](const Chunk& c) { return launch_dot(h, p, c, d_xq, d_valid, f); });
+  if (rc) return rc;
+  return deliver(h, o, n, topk, out_items, out_scores, out_count);
+}
 
 int pio_als_similar_batch(pio_als_handle* h, const int64_t* q_ptr, const int32_t* q_items, int n_queries, int topk,
                           const uint8_t* item_mask, const double* item_weight, int flags, int32_t* out_items,
@@ -2293,192 +2350,47 @@ int pio_als_similar_batch(pio_als_handle* h, const int64_t* q_ptr, const int32_t
       return fail(h, PIO_ALS_ERR_ARG, "q_ptr must be non-decreasing offsets into q_items");
   if (!h->I.F || !h->I.cand_ext) return fail(h, PIO_ALS_ERR_STATE, "no model");
   CK(h, cudaSetDevice(h->cfg.device));
-  if (n_queries == 1 && serve_one_ok(h, (int)std::min<long long>(q_ptr[1] - q_ptr[0], 1 << 20), topk))   // the serving case
-    return serve_one(h, true, q_items + q_ptr[0], (int)(q_ptr[1] - q_ptr[0]), topk, item_mask, item_weight, flags, out_items,
-                     out_scores, out_count);
-  if (n_queries == 1 && q_ptr[1] - q_ptr[0] >= 1 && q_ptr[1] - q_ptr[0] <= SM_NV && topk <= TK_MAXK)
-    return similar_small(h, q_items + q_ptr[0], (int)(q_ptr[1] - q_ptr[0]), topk, item_mask, item_weight, flags, out_items,
-                         out_scores, out_count);
-  Scratch tmp(h);
-  uint8_t* d_mask = nullptr;
-  double* d_weight = nullptr;
-  if (item_mask) {
-    CK(h, tmp.alloc(&d_mask, (size_t)h->I.n));
-    CK(h, cudaMemcpyAsync(d_mask, item_mask, (size_t)h->I.n, cudaMemcpyHostToDevice, h->stream));
-  }
-  if (item_weight) {
-    CK(h, tmp.alloc(&d_weight, (size_t)h->I.n));
-    CK(h, cudaMemcpyAsync(d_weight, item_weight, sizeof(double) * (size_t)h->I.n, cudaMemcpyHostToDevice, h->stream));
-  }
-  cudaStream_t st = h->stream;
-  const int KP = h->KP, k = h->cfg.rank;
+  const ScoreEnv env = score_env(h);
   const long long total = q_ptr[n_queries] - q_ptr[0];
-  bool fast = n_queries > 1 && total > 0 && total < (1ll << 31);
-  std::vector<int> gvec0, vq, vsrc;
-  if (fast) {
+  const ScorePlan p = plan_similar(env, n_queries, q_ptr[1] - q_ptr[0], total, topk);
+  if (p.route == ROUTE_ONE)   // the serving case
+    return serve_one(h, p, true, q_items + q_ptr[0], (int)(q_ptr[1] - q_ptr[0]), topk, item_mask, item_weight, flags,
+                     out_items, out_scores, out_count);
+  if (p.route == ROUTE_ARENA)
+    return similar_small(h, p, q_items + q_ptr[0], (int)(q_ptr[1] - q_ptr[0]), topk, item_mask, item_weight, flags,
+                         out_items, out_scores, out_count);
+  cudaStream_t st = h->stream;
+  Scratch tmp(h);
+  DevFilter f;
+  int rc = upload_filter(h, item_mask, item_weight, &tmp, 0, &f);
+  if (rc) return rc;
+  if (p.route == ROUTE_BATCH) {
     // all query item vectors in one gather; which of them own a factor decides the vector list of every query
     int* d_qid = nullptr;
     float* d_qf_all = nullptr;
     uint8_t* d_valid = nullptr;
     CK(h, tmp.alloc(&d_qid, (size_t)total));
-    CK(h, tmp.alloc(&d_qf_all, (size_t)total * KP));
+    CK(h, tmp.alloc(&d_qf_all, (size_t)total * h->KP));
     CK(h, tmp.alloc(&d_valid, (size_t)total));
     CK(h, cudaMemcpyAsync(d_qid, q_items + q_ptr[0], sizeof(int) * total, cudaMemcpyHostToDevice, st));
-    gather_rows_kernel<<<(unsigned)total, 64, 0, st>>>(h->I.F, KP, d_qid, (int)total, h->I.perm, h->I.deg, h->I.n, d_qf_all, d_valid);
-    SCORE_LAUNCHED(h, 0);
+    rc = score_launch(h, gather_rows_kernel, dim3((unsigned)total), dim3(64), 0, 0, h->I.F, h->KP, (const int*)d_qid,
+                      (int)total, h->I.perm, h->I.deg, h->I.n, d_qf_all, d_valid);
+    if (rc) return rc;
     std::vector<uint8_t> valid((size_t)total);
     CK(h, cudaMemcpyAsync(valid.data(), d_valid, (size_t)total, cudaMemcpyDeviceToHost, st));
     CK(h, cudaStreamSynchronize(st));
-    // blocked kernel: bins of <= CB_QPW consecutive queries and <= DB_QW query vectors per warp (rank <= 64, topk <= DB_MAXK)
-    if (h->score_blocked && KP <= 64 && topk <= DB_MAXK) {
-      std::vector<int> bin_q0, bin_v0, bvq, bvsrc;
-      bool ok = true;
-      int bq = 0, bv = 0;      // queries / vectors in the open bin
-      bin_q0.push_back(0);
-      bin_v0.push_back(0);
-      for (int j = 0; j < n_queries && ok; ++j) {
-        int nvq = 0;
-        for (long long t = q_ptr[j]; t < q_ptr[j + 1]; ++t) nvq += valid[(size_t)(t - q_ptr[0])] ? 1 : 0;
-        if (nvq > DB_QW) { ok = false; break; }
-        if (bq == CB_QPW || bv + nvq > DB_QW) {
-          bin_q0.push_back(j);
-          bin_v0.push_back((int)bvsrc.size());
-          bq = bv = 0;
-        }
-        for (long long t = q_ptr[j]; t < q_ptr[j + 1]; ++t)
-          if (valid[(size_t)(t - q_ptr[0])]) {
-            bvsrc.push_back((int)(t - q_ptr[0]));
-            bvq.push_back(j);
-          }
-        ++bq;
-        bv += nvq;
-      }
-      if (ok) {
-        bin_q0.push_back(n_queries);
-        bin_v0.push_back((int)bvsrc.size());
-        const int n_bins = (int)bin_q0.size() - 1, nvec = (int)bvsrc.size();
-        const int ngroups = (n_bins + DB_WPR - 1) / DB_WPR;
-        int *d_bq0 = nullptr, *d_bv0 = nullptr, *d_vq = nullptr, *d_vsrc = nullptr, *d_oi = nullptr, *d_oc = nullptr;
-        long long* d_qptr = nullptr;
-        float *d_qfc = nullptr, *d_os = nullptr;
-        ScoreIdx* d_cand = nullptr;
-        std::vector<long long> rel((size_t)n_queries + 1);
-        for (int j = 0; j <= n_queries; ++j) rel[j] = q_ptr[j] - q_ptr[0];
-        CK(h, tmp.alloc(&d_bq0, bin_q0.size()));
-        CK(h, tmp.alloc(&d_bv0, bin_v0.size()));
-        CK(h, tmp.alloc(&d_vq, (size_t)(nvec > 0 ? nvec : 1)));
-        CK(h, tmp.alloc(&d_vsrc, (size_t)(nvec > 0 ? nvec : 1)));
-        CK(h, tmp.alloc(&d_qptr, rel.size()));
-        CK(h, tmp.alloc(&d_qfc, (size_t)(nvec > 0 ? nvec : 1) * KP));
-        CK(h, cudaMemcpyAsync(d_bq0, bin_q0.data(), sizeof(int) * bin_q0.size(), cudaMemcpyHostToDevice, st));
-        CK(h, cudaMemcpyAsync(d_bv0, bin_v0.data(), sizeof(int) * bin_v0.size(), cudaMemcpyHostToDevice, st));
-        CK(h, cudaMemcpyAsync(d_qptr, rel.data(), sizeof(long long) * rel.size(), cudaMemcpyHostToDevice, st));
-        if (nvec > 0) {
-          CK(h, cudaMemcpyAsync(d_vq, bvq.data(), sizeof(int) * nvec, cudaMemcpyHostToDevice, st));
-          CK(h, cudaMemcpyAsync(d_vsrc, bvsrc.data(), sizeof(int) * nvec, cudaMemcpyHostToDevice, st));
-          copy_rows_kernel<<<nvec, 64, 0, st>>>(d_qf_all, KP, d_vsrc, d_qfc);
-          SCORE_LAUNCHED(h, 0);
-        }
-        const int nsteps = (h->I.n_internal + DB_RINGS * DB_ROWS - 1) / (DB_RINGS * DB_ROWS);
-        int gx = (h->sm_count + ngroups - 1) / ngroups;
-        if (gx > (nsteps + 7) / 8) gx = (nsteps + 7) / 8;
-        if (gx < 1) gx = 1;
-        const int lists = gx * DB_RINGS;
-        CK(h, tmp.alloc(&d_cand, (size_t)n_queries * lists * topk));
-        CK(h, tmp.alloc(&d_oi, (size_t)n_queries * topk));
-        CK(h, tmp.alloc(&d_os, (size_t)n_queries * topk));
-        CK(h, tmp.alloc(&d_oc, (size_t)n_queries));
-        const int keep_query = (flags & PIO_ALS_SIM_KEEP_QUERY_ITEMS) ? 1 : 0;
-        const size_t smem = db_smem_bytes(KP, topk);
-        for (int g0 = 0; g0 < ngroups; g0 += 32768) {
-          const int ng = ngroups - g0 < 32768 ? ngroups - g0 : 32768;
-          const int brc = launch_cos_blocked(h, dim3(gx, ng), smem, d_qfc, d_bq0 + (size_t)g0 * DB_WPR, d_bv0 + (size_t)g0 * DB_WPR,
-                                             n_bins - g0 * DB_WPR, d_vq, d_qptr, d_qid, d_mask, d_weight, keep_query, topk, d_cand);
-          if (brc) return brc;
-        }
-        topk_merge_kernel<<<n_queries, TK_THREADS, 0, st>>>(d_cand, lists * topk, topk, topk, 0, d_oi, d_os, d_oc, nullptr);
-        SCORE_LAUNCHED(h, 0);
-        CK(h, cudaMemcpyAsync(out_items, d_oi, sizeof(int) * (size_t)n_queries * topk, cudaMemcpyDeviceToHost, st));
-        CK(h, cudaMemcpyAsync(out_scores, d_os, sizeof(float) * (size_t)n_queries * topk, cudaMemcpyDeviceToHost, st));
-        if (out_count) CK(h, cudaMemcpyAsync(out_count, d_oc, sizeof(int) * (size_t)n_queries, cudaMemcpyDeviceToHost, st));
-        CK(h, cudaStreamSynchronize(st));
-        return PIO_ALS_OK;
-      }
-    }
-    const int ngroups = (n_queries + SM_QG - 1) / SM_QG;
-    gvec0.assign((size_t)ngroups + 1, 0);
-    for (int g = 0; g < ngroups && fast; ++g) {
-      gvec0[g] = (int)vsrc.size();
-      for (int j = g * SM_QG; j < (g + 1) * SM_QG && j < n_queries; ++j)
-        for (long long t = q_ptr[j]; t < q_ptr[j + 1]; ++t)
-          if (valid[(size_t)(t - q_ptr[0])]) {
-            vsrc.push_back((int)(t - q_ptr[0]));
-            vq.push_back(j - g * SM_QG);
-          }
-      if ((int)vsrc.size() - gvec0[g] > SM_NV) fast = false;   // a group with too many query vectors: one query at a time
-    }
-    gvec0[ngroups] = (int)vsrc.size();
-    if (fast) {
-      const int nvec = (int)vsrc.size();
-      int *d_gvec0 = nullptr, *d_vq = nullptr, *d_vsrc = nullptr, *d_oi = nullptr, *d_oc = nullptr;
-      long long* d_qptr = nullptr;
-      float *d_qfc = nullptr, *d_os = nullptr;
-      ScoreIdx *d_cand = nullptr, *d_bound = nullptr;
-      std::vector<long long> rel((size_t)n_queries + 1);
-      for (int j = 0; j <= n_queries; ++j) rel[j] = q_ptr[j] - q_ptr[0];
-      CK(h, tmp.alloc(&d_gvec0, gvec0.size()));
-      CK(h, tmp.alloc(&d_vq, (size_t)(nvec > 0 ? nvec : 1)));
-      CK(h, tmp.alloc(&d_vsrc, (size_t)(nvec > 0 ? nvec : 1)));
-      CK(h, tmp.alloc(&d_qptr, rel.size()));
-      CK(h, tmp.alloc(&d_qfc, (size_t)(nvec > 0 ? nvec : 1) * KP));
-      CK(h, cudaMemcpyAsync(d_gvec0, gvec0.data(), sizeof(int) * gvec0.size(), cudaMemcpyHostToDevice, st));
-      CK(h, cudaMemcpyAsync(d_qptr, rel.data(), sizeof(long long) * rel.size(), cudaMemcpyHostToDevice, st));
-      if (nvec > 0) {
-        CK(h, cudaMemcpyAsync(d_vq, vq.data(), sizeof(int) * nvec, cudaMemcpyHostToDevice, st));
-        CK(h, cudaMemcpyAsync(d_vsrc, vsrc.data(), sizeof(int) * nvec, cudaMemcpyHostToDevice, st));
-        copy_rows_kernel<<<nvec, 64, 0, st>>>(d_qf_all, KP, d_vsrc, d_qfc);
-        SCORE_LAUNCHED(h, 0);
-      }
-      const int pass_max = topk < TK_MAXK ? topk : TK_MAXK;
-      const int ntiles = (h->I.n_internal + SB_THREADS - 1) / SB_THREADS;
-      int gx = (2 * h->sm_count + ngroups - 1) / ngroups;
-      if (gx > (ntiles + 7) / 8) gx = (ntiles + 7) / 8;
-      if (gx < 1) gx = 1;
-      const size_t smem = sizeof(double) * ((size_t)KP * SM_NV + SM_NV) + sb_tile_bytes(KP) +
-                          (sizeof(double) + sizeof(int)) * (size_t)SM_QG * pass_max + sizeof(int) * (SM_NV + SM_QG * SM_QIDS) + 16;
-      ENSURE_SMEM(h, score_cos_topk_multi_kernel, smem);
-      CK(h, tmp.alloc(&d_cand, (size_t)n_queries * gx * pass_max));
-      CK(h, tmp.alloc(&d_oi, (size_t)n_queries * topk));
-      CK(h, tmp.alloc(&d_os, (size_t)n_queries * topk));
-      CK(h, tmp.alloc(&d_oc, (size_t)n_queries));
-      if (topk > TK_MAXK) CK(h, tmp.alloc(&d_bound, (size_t)n_queries));
-      const int keep_query = (flags & PIO_ALS_SIM_KEEP_QUERY_ITEMS) ? 1 : 0;
-      for (int done = 0; done < topk; done += TK_MAXK) {
-        const int pk = topk - done < TK_MAXK ? topk - done : TK_MAXK;
-        if (done > 0) h->st.last_score_path |= PIO_ALS_PATH_MULTI_PASS;
-        for (int g0 = 0; g0 < ngroups; g0 += 32768) {
-          const int ng = ngroups - g0 < 32768 ? ngroups - g0 : 32768;
-          const int qa = g0 * SM_QG;
-          const int nq = n_queries - qa < ng * SM_QG ? n_queries - qa : ng * SM_QG;
-          score_cos_topk_multi_kernel<<<dim3(gx, ng), SB_THREADS, smem, st>>>(
-              h->I.F, h->I.n_internal, KP, k, d_qfc, d_gvec0 + g0, d_vq, d_qptr + qa, d_qid, nq, h->I.cand_ext, d_mask,
-              d_weight, done > 0 ? d_bound + qa : nullptr, keep_query, pk, d_cand + (size_t)qa * gx * pk);
-          SCORE_LAUNCHED(h, PIO_ALS_PATH_COS_MULTI);
-        }
-        topk_merge_kernel<<<n_queries, TK_THREADS, 0, st>>>(d_cand, gx * pk, pk, topk, done, d_oi, d_os, d_oc, d_bound);
-        SCORE_LAUNCHED(h, 0);
-      }
-      CK(h, cudaMemcpyAsync(out_items, d_oi, sizeof(int) * (size_t)n_queries * topk, cudaMemcpyDeviceToHost, st));
-      CK(h, cudaMemcpyAsync(out_scores, d_os, sizeof(float) * (size_t)n_queries * topk, cudaMemcpyDeviceToHost, st));
-      if (out_count) CK(h, cudaMemcpyAsync(out_count, d_oc, sizeof(int) * (size_t)n_queries, cudaMemcpyDeviceToHost, st));
-      CK(h, cudaStreamSynchronize(st));
-      return PIO_ALS_OK;
-    }
+    std::vector<int> nvalid((size_t)n_queries, 0), q0;
+    for (int j = 0; j < n_queries; ++j)
+      for (long long t = q_ptr[j]; t < q_ptr[j + 1]; ++t) nvalid[j] += valid[(size_t)(t - q_ptr[0])] ? 1 : 0;
+    const ScorePlan b = plan_similar_batch(env, nvalid, topk, &q0);
+    if (b.route == ROUTE_BATCH)
+      return similar_groups(h, b, q0, q_ptr, n_queries, topk, valid, d_qf_all, d_qid, f, flags, tmp, out_items, out_scores,
+                            out_count);
   }
-  for (int j = 0; j < n_queries; ++j) {
+  for (int j = 0; j < n_queries; ++j) {   // S5: one query at a time
     int32_t cnt = 0;
-    const int rc = similar_one(h, q_items + q_ptr[j], (int)(q_ptr[j + 1] - q_ptr[j]), topk, d_mask, d_weight, flags,
-                               out_items + (size_t)j * topk, out_scores + (size_t)j * topk, &cnt);
+    rc = similar_one(h, q_items + q_ptr[j], (int)(q_ptr[j + 1] - q_ptr[j]), topk, f, flags, out_items + (size_t)j * topk,
+                     out_scores + (size_t)j * topk, &cnt);
     if (rc) return rc;
     if (out_count) out_count[j] = cnt;
   }

@@ -11,31 +11,26 @@
 // loops over Array[Double], so scores and rankings are bit-identical to the oracle -- and the compute bound of every
 // kernel here is the fp64 pipe (one DFMA per query vector x item x feature), not HBM.
 //
-// Kernels, by call shape (pio_als.cu picks; DESIGN.md 4.6):
+// Kernels, by call shape (the planner in score_plan.h picks, pio_als.cu launches; DESIGN.md 4.6):
 //   score_one_kernel                 one query = one launch: lookup, scan, selection, result into mapped host memory
 //   score_dot_blocked_kernel         batches of users   (rank <= 64, topk <= 32): two items x eight queries per thread
 //   score_cos_blocked_kernel         batches of similar queries (same limits): bins of <= 4 queries / <= 8 vectors per warp
 //   score_dot_topk_batched_kernel    first-generation batch kernels (one item per thread): rank 128, topk > 32, and
 //   score_cos_topk_multi_kernel        2..16 users / long similar queries on the three-launch serving path
-//   score_cos_topk_kernel            fallback for very large single queries
+//   score_cos_topk_batched_kernel    one long similar query, its vectors in shared memory
+//   score_cos_topk_kernel            fallback for single queries too large for that
 //   topk_merge_kernel                merges the per-CTA / per-warp candidate lists of a query; multi-pass bounds (topk > 128)
+// Block sizes, pool shapes and every kernel's dynamic shared memory (*_smem_bytes) are in topk_geometry.h.
 // Pools: WarpPool (entries in shared memory, cooperative worst-entry search) and SortedPool (sorted in the registers of a
 // warp: ballot-counted position + shuffle shift).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include "topk_geometry.h"
+
 namespace pio {
 
-constexpr int TK_THREADS = 256;
-constexpr int TK_ITEMS = 4;                       // items per thread
-constexpr int TK_TILE = TK_THREADS * TK_ITEMS;    // items per CTA
-constexpr int TK_MAXK = 128;                      // max supported topk
-
-struct ScoreIdx {
-  double s;
-  int i;
-};
 __device__ __forceinline__ bool better(double s1, int i1, double s2, int i2) {
   return (s1 > s2) || (s1 == s2 && i1 < i2);
 }
@@ -105,14 +100,6 @@ __device__ __forceinline__ void block_select_topk(double (&sc)[TK_ITEMS], int (&
 // keeps a top-k pool in shared memory for the whole scan; an item is offered to it only if it beats the pool's current
 // worst entry (rare after the first tiles), under a per-query lock - no per-tile block-wide selection rounds.
 // xq: [n_queries][kp] (zero padded), qvalid[q] == 0 -> no candidates.  cand: [n_queries][GX][topk], unsorted, i = -1 = empty.
-constexpr int SB_THREADS = 256;
-constexpr int SB_QB = 16;
-// staged tile [SB_THREADS][kp + 4] floats, large enough to be reused for the [SB_QB][SB_THREADS] fp64 score exchange + ids
-__host__ __device__ inline size_t sb_tile_bytes(int kp) {
-  const size_t a = sizeof(float) * (size_t)SB_THREADS * (kp + 4);
-  const size_t b = sizeof(double) * (size_t)SB_QB * SB_THREADS + sizeof(int) * SB_THREADS;
-  return a > b ? a : b;
-}
 
 __device__ __forceinline__ void sb_cp_async16(void* smem_dst, const void* gsrc) {
   const unsigned d = (unsigned)__cvta_generic_to_shared(smem_dst);
@@ -397,21 +384,6 @@ struct SortedPool {
 // pipe 31 % busy; rings of four warps (4 queries each) convert every row four times and the conversion pipe (F2F: 15.7
 // lanes/clk/SM) becomes co-critical (fp64 45 %, XU 44 %).  Same arithmetic and order as above -> bit-identical results.
 // For kp <= 64 and topk <= DB_MAXK; cand: [n_queries][gridDim.x * DB_RINGS][topk], unsorted, i = -1 = empty.
-constexpr int DB_QW = 8;                     // queries per warp
-constexpr int DB_WPR = SB_QB / DB_QW;        // warps per ring
-constexpr int DB_RINGS = 8;
-constexpr int DB_WARPS = DB_RINGS * DB_WPR;  // 16
-constexpr int DB_ROWS = 64;                  // rows per ring step (two per lane)
-constexpr int DB_STAGES = 1;                 // a ring waits for its own rows while the other seven compute
-constexpr int DB_MAXK = 32;
-struct alignas(16) DbPoolHdr {   // 32 bytes; the first 16 are read with one LDS.128 for the threshold test
-  double thr;
-  int cnt, wid, worst, pad[3];
-};
-__host__ __device__ inline size_t db_smem_bytes(int kp, int topk) {
-  return sizeof(double) * (size_t)kp * SB_QB + sizeof(float) * (size_t)DB_RINGS * DB_STAGES * DB_ROWS * (kp + 4) +
-         (size_t)DB_RINGS * SB_QB * (sizeof(DbPoolHdr) + (sizeof(double) + sizeof(int)) * (size_t)topk);
-}
 
 // The rare path of the scan (a score passed the threshold test): NOT inlined -- unrolled copies of the pool insertion
 // between the threshold tests of a step are tens of KB of code on the hot path (ncu on a first version: "no
@@ -596,7 +568,6 @@ score_dot_blocked_kernel(const float* __restrict__ Y, int n_items, const float* 
 // of bins (the two warps of every ring).  bin_q0 / bin_v0: first query / first vector of every bin (+ one end entry);
 // qf: the query vectors [n_vec][KP]; vq: global query of every vector; qid_ptr / qid: the id list of every query (all
 // of them are excluded from its results unless keep_query).  cand: [n_queries][gridDim.x * DB_RINGS][topk].
-constexpr int CB_QPW = 4;   // queries per warp
 
 __device__ __noinline__ void cb_insert(DbPoolHdr* hd, double* ps, int* pi, unsigned long long* cthr, bool w0, double s0,
                                        int e0, bool w1, double s1, int e1, int topk, const int* __restrict__ qid, int nid) {
@@ -822,7 +793,6 @@ score_cos_blocked_kernel(const float* __restrict__ Y, int n_items, int k, const 
 // (external) - every one of them is excluded from the candidates (ALSAlgorithm.scala:243-245).  score_i = sum over the
 // query vectors, in query order, of d / (sqrt(n1) * sqrt(n2)) with d, n1, n2 accumulated in fp64 in index order
 // (ALSAlgorithm.scala:220-234), kept only if > 0.  cand: [gridDim.x][warps][topk].
-constexpr int SC_G = 8;   // query vectors scored per pass over a staged row
 
 __global__ void __launch_bounds__(SB_THREADS, 2)
 score_cos_topk_batched_kernel(const float* __restrict__ Y, int n_items, int kp, int k,
@@ -943,9 +913,6 @@ score_cos_topk_batched_kernel(const float* __restrict__ Y, int n_items, int kp, 
 //   gvec0[g] .. gvec0[g+1] : vectors of group g in qf ([total vectors][kp], query order inside a query)
 //   vq[v]                  : query (0..SM_QG-1 inside the group) of vector v
 //   qid_ptr / qid          : all query item ids (external) of every query, for the exclusion rule
-constexpr int SM_QG = 8;    // queries per group = warps per CTA
-constexpr int SM_NV = 40;   // query vectors per group held in shared memory
-constexpr int SM_QIDS = 64; // query item ids per query held in shared memory (longer lists are read from global memory)
 
 __global__ void __launch_bounds__(SB_THREADS, 2)
 score_cos_topk_multi_kernel(const float* __restrict__ Y, int n_items, int kp, int k, const float* __restrict__ qf,
@@ -1221,17 +1188,10 @@ topk_merge_kernel(const ScoreIdx* __restrict__ cand, int n_cand, int topk, int o
 // pools of a CTA are merged by rank counting; the last CTA to finish (device counter) merges the per-CTA lists and
 // writes the result straight into mapped host memory, followed by a sequence flag the host polls.  Arithmetic and
 // tie-breaking are those of the batched kernels above (fp64 in index order, better()): results are bit-identical.
-constexpr int S1_THREADS = 256;
-constexpr int S1_STAGES = 3;
-constexpr int S1_MAXNV = 8;
 struct OneQuery {
   int nq;
   int ids[S1_MAXNV];   // external ids (COS: the query items; dot: ids[0] = the user)
 };
-__host__ __device__ inline size_t s1_smem_bytes(int kp, int nvp, int topk) {
-  return sizeof(double) * ((size_t)kp * nvp + S1_MAXNV) + sizeof(float) * (size_t)S1_STAGES * S1_THREADS * (kp + 4) +
-         (sizeof(double) + sizeof(int)) * (size_t)(S1_THREADS / 32) * topk + 128;
-}
 // n_lists lists of topk candidates each, every list best first and padded with i = -1 -> the best topk overall.
 // Only candidates at least as good as the topk-th best list head can make it: those few are collected in `surv` (shared
 // memory, capacity cap) and ordered by rank counting.  All S1_THREADS threads call; returns the number of results.

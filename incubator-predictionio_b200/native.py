@@ -75,7 +75,8 @@ NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-
 
 def build(force: bool = False, verbose: bool = False) -> Path:
     """nvcc cross-compile of csrc/pio_als.cu for sm_90a (H100) into the in-tree libpio_als.so."""
-    srcs = sorted(CSRC.glob("*.cu")) + sorted(CSRC.glob("*.cuh")) + [REPO_ROOT / "include" / "pio_als.h"]
+    srcs = (sorted(CSRC.glob("*.cu")) + sorted(CSRC.glob("*.cuh")) + sorted(CSRC.glob("*.h")) +
+            [REPO_ROOT / "include" / "pio_als.h"])
     if LIB_PATH.exists() and not force and all(LIB_PATH.stat().st_mtime >= s.stat().st_mtime for s in srcs):
         return LIB_PATH
     cmd = ["nvcc", *NVCC_FLAGS, "-o", str(LIB_PATH), str(CSRC / "pio_als.cu")]

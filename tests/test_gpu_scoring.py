@@ -2,7 +2,7 @@
 
 pio_als.h promises that recommend / similar / similar_batch return results identical to the fp64 reference on every path,
 ties going to the smaller item id.  Each case below compares ids, scores (as bits) and counts with scoring_ref and asserts
-pio_als_stats.last_score_path, so it provably ran the kernels it names.  The dispatch (pio_als.cu, DESIGN.md 4.6):
+pio_als_stats.last_score_path, so it provably ran the kernels it names.  The dispatch (csrc/score_plan.h, DESIGN.md 4.6):
 
   R1 recommend, n == 1, KP <= 64, topk <= 128            score_one           S1 one query of 1..8 ids, KP <= 64, topk <= 128
   R2 n <= 16, topk <= 128                                dot_batched         S2 one query of 1..40 ids, topk <= 128
@@ -24,8 +24,8 @@ import scoring_ref
 
 pytestmark = pytest.mark.gpu
 
-# dispatch constants of topk.cuh / pio_als.cu; tests/test_scoring_thresholds.py checks them against the sources and that
-# the ladders below straddle each one
+# dispatch constants of topk_geometry.h / score_plan.h; tests/test_scoring_plan.py checks them, and the planner's rules,
+# against the sources, and that the ladders below straddle each one
 TK_MAXK, DB_MAXK, SB_QB, S1_MAXNV, SM_NV, SM_QG, SM_QIDS, DB_QW = 128, 32, 16, 8, 40, 8, 64, 8
 CB_QPW, DB_WPR = 4, 2
 SB_THREADS, SC_G, S5_SMEM_LIMIT, GROUP_CHUNK = 256, 8, 100 * 1024, 32768
