@@ -1,7 +1,8 @@
 // pio_als.cu -- C-ABI implementation (see include/pio_als.h for the reference interfaces each
 // entry point replaces).  Host orchestration only; all arithmetic is in the CUDA kernels of
-// als_kernels.cuh / sort_scan.cuh / topk.cuh.  No CPU fallback: without a usable sm_90 device
-// every computing entry point returns PIO_ALS_ERR_CUDA.
+// als_kernels.cuh / sort_scan.cuh / topk.cuh.  Which kernels a half-step or a scoring call runs, and with
+// what geometry, is planned by solve_plan.h and score_plan.h; this file executes the plans.  No CPU
+// fallback: without a usable sm_90 device every computing entry point returns PIO_ALS_ERR_CUDA.
 #include "../../include/pio_als.h"
 
 #include <cuda_runtime.h>
@@ -44,17 +45,11 @@
 #include "sort_scan.cuh"
 #include "topk.cuh"
 #include "score_plan.h"
+#include "solve_plan.h"
 #include "ids_encode.cuh"
 #include "cooc.cuh"
 
 namespace pio {
-
-constexpr int HEAVY_T = 4096;     // rows with more ratings than this are cut into parts (als_finish_kernel solves them)
-constexpr int HEAVY_T_TC = 8192;  // same threshold when the tensor-core path handles the shorter rows
-constexpr int TC_TILE_ROWS = 1 << 20;  // split mode: rows whose normal equations are buffered at once (9.1 KB per row)
-constexpr int PART = 2016;        // ratings per part (multiple of every CH and of the tensor-core stage size 24)
-constexpr int PAIR_SEG_T = 1024;  // pair kernel (als_pair_kernel.cuh): rows with more ratings than this are cut into parts ...
-constexpr int PAIR_PART = 512;    // ... of this many ratings: two-level summation keeps long rows inside the parity bound
 
 static thread_local std::string g_create_error;
 
@@ -384,10 +379,7 @@ struct Side {
   float* F = nullptr;        // [n_internal][KP]
   int* cand_ext = nullptr;   // [n_internal]
   int n_active = 0, n_heavy = 0;
-  bool use_tc = false;       // this side's short rows go through the tensor-core kernel (decided from GLOBAL counts: every rank agrees)
-  int heavy_t = 0;           // rows with more ratings than this are cut into parts
-  int part_len = 0;          // ratings per part
-  bool use_pair = false;     // rows and parts of this side run on the pair kernel (rank 33..64, mma.sync + lockstep solve)
+  SidePlan plan;             // kernel, heavy-row threshold and part length of this side (solve_plan.h)
   // parts of the n_heavy longest local rows
   long long* part_beg = nullptr;
   long long* part_end = nullptr;
@@ -423,17 +415,12 @@ struct pio_als_handle {
   long long* d_timing = nullptr;  // PIO_ALS_TC_TIMING=1: per-warp cycle counters of the last tensor-core launch
   float* d_dbg = nullptr;     // PIO_ALS_TC_DEBUG=1: A/b dump of the last tensor-core half-step
   size_t dbg_rows = 0;
-  bool use_tc = false;        // rank in 33..64 and PIO_ALS_TC != 0
-  bool use_mma = true;        // PIO_ALS_MMA=0: FP32 kernel instead of the mma.sync kernels for rank 33..64
-  bool use_pair = true;       // PIO_ALS_MMA=1: round-1 one-warp-per-row mma.sync kernel instead of the pair kernel
-  int pair_seg_t = PAIR_SEG_T, pair_part = PAIR_PART;   // PIO_ALS_SEG_T / PIO_ALS_PART
-  int pair_warps = 4;         // PIO_ALS_PAIR_WARPS: warps per CTA of the pair kernel (1, 2, 4, 6 or 12)
+  SolveSwitches sw;           // the solve's environment switches (solve_plan.h)
   // half-step pipeline (pair-kernel sides): long rows (parts + finish) run on `aux` next to the whole rows on `stream`;
-  // the destination rows are cut into n_pieces local ranges and the all-gather of a finished range runs on `comm_st`
-  // while the next range is solved (world_size > 1)
+  // the destination rows are cut into sw.n_pieces local ranges and the all-gather of a finished range runs on
+  // `comm_st` while the next range is solved (world_size > 1)
   cudaStream_t aux = nullptr, comm_st = nullptr;
   cudaEvent_t ev_start = nullptr, ev_heavy = nullptr, ev_piece[8] = {}, ev_comm = nullptr;
-  int n_pieces = 1;           // PIO_ALS_PIECES (1..8); default 4 when world_size > 1
   bool pieces_done = false;   // the last launch_solve recorded ev_piece[] / ev_heavy (pair path)
   // low-latency serving (few queries, topk <= 128): a persistent device arena and a mapped pinned host arena -- no
   // allocation, no staging copies, results written by the merge kernel straight into host memory
@@ -449,10 +436,8 @@ struct pio_als_handle {
   bool serve_fused = true;                 // PIO_ALS_SERVE_FUSED=0: single queries take the three-launch path
   bool score_blocked = true;               // PIO_ALS_SCORE_BLOCKED=0: batched recommend on the one-item-per-thread kernel
   bool serve_trace = false;                // PIO_ALS_SERVE_TRACE=1: per-phase device timestamps of every fused call on stderr
-  bool tc_split = false;      // PIO_ALS_TC_SPLIT=1: the tensor-core kernel only accumulates, a second kernel solves (measured: no gain)
-  float* tc_out = nullptr;    // split mode: normal equations of one tile of rows ([rows][ASLOT + KP])
+  float* tc_out = nullptr;    // wgmma split mode: normal equations of one tile of rows ([rows][ASLOT + KP])
   size_t tc_out_rows = 0;
-  double tc_min_deg = 0.0;    // PIO_ALS_TC_MIN_DEG: only sides whose rows average at least this many ratings use it
   bool have_ratings = false, have_init = false, trained = false;
   ncclComm_t comm = nullptr;
   std::string err;
@@ -595,20 +580,10 @@ static int build_side(pio_als_handle* h, Side& row, const Side& col, const int* 
   }
   tmark(h, "  side: ptr + extract csr");
   CK(h, cudaMemsetAsync(h->d_counts, 0, 2 * sizeof(int), st));
-  // kernel choice from global numbers only (ratings after dedup / rows of this side), so that every rank of a sharded
-  // run and the single-GPU run take the same path for the same row
-  row.use_tc = h->use_tc && h->KP == 64 && row.n > 0 && (double)nnz_global / (double)row.n >= h->tc_min_deg;
-  row.use_pair = !row.use_tc && h->KP == 64 && h->use_mma && h->use_pair;
-  // one warp (mma kernels) or one A slot (wgmma kernel) carries a whole row.  Pair kernel: rows up to 1024
-  // ratings stay whole, longer rows become 512-rating parts of the same kernel (two-level summation); round-1 mma /
-  // wgmma kernels: rows up to 8192 ratings whole, longer rows as 2016-rating parts on the FP32 kernel; FP32 kernel
-  // (other ranks): cut at 4096
-  // rank 65..128: every row is a work-list row (FP32 Gramian kernel -> partial normal equations -> lockstep finish kernel)
-  row.heavy_t = h->KP == 128 ? 0 : row.use_pair ? h->pair_seg_t : (row.use_tc || (h->KP == 64 && h->use_mma)) ? HEAVY_T_TC : HEAVY_T;
-  row.part_len = row.use_pair ? h->pair_part : PART;
+  row.plan = plan_side(h->sw, h->KP, row.n, nnz_global);
   local_rows_kernel<<<nblk(row.R + 1, 256), 256, 0, st>>>(ptr_full, rk * row.R, row.R, be[0], row.inv, row.deg,
                                                            row.npos, h->cfg.implicit_prefs, row.ptr, row.nreg,
-                                                           h->d_counts, row.heavy_t);
+                                                           h->d_counts, row.plan.heavy_t);
   LAUNCHED(h);
   int counts[2];
   CK(h, cudaMemcpyAsync(counts, h->d_counts, sizeof counts, cudaMemcpyDeviceToHost, st));
@@ -623,11 +598,12 @@ static int build_side(pio_als_handle* h, Side& row, const Side& col, const int* 
     CK(h, cudaStreamSynchronize(st));
     std::vector<long long> pb, pe;
     std::vector<int> rpp((size_t)row.n_heavy + 1);
+    const int part_len = row.plan.part_len;
     for (int r = 0; r < row.n_heavy; ++r) {
       rpp[r] = (int)pb.size();
-      for (long long b = hp[r]; b < hp[r + 1]; b += row.part_len) {
+      for (long long b = hp[r]; b < hp[r + 1]; b += part_len) {
         pb.push_back(b);
-        pe.push_back(b + row.part_len < hp[r + 1] ? b + row.part_len : hp[r + 1]);
+        pe.push_back(b + part_len < hp[r + 1] ? b + part_len : hp[r + 1]);
       }
     }
     rpp[row.n_heavy] = (int)pb.size();
@@ -968,315 +944,237 @@ static int init_hash(pio_als_handle* h) {
 }
 
 // ---- solve dispatch ---------------------------------------------------------------------------
-template <class Cfg, bool IMPLICIT>
-static cudaError_t launch_solve_one(pio_als_handle* h, const SolveParams& p, int grid, cudaStream_t st) {
-  static bool attr_set[64] = {};
-  int dev = h->cfg.device;
-  auto kern = als_solve_kernel<Cfg, IMPLICIT>;
-  const size_t smem = Cfg::smem_bytes();
-  if (dev < 64 && !attr_set[dev]) {
-    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (e != cudaSuccess) return e;
-    attr_set[dev] = true;
-  }
-  kern<<<grid, Cfg::NT, smem, st>>>(p);
-  LAUNCHED(h);
-  ++h->st.solve_launches;
-  return cudaGetLastError();
-}
-
-// Gramians on wgmma (als_tc_kernel.cuh): persistent, one CTA per SM, rows assigned statically.  A = role partition.
-// Split mode (PIO_ALS_TC_SPLIT=1, off by default): the kernel only accumulates and stores the normal equations of a
-// tile of rows; a second kernel solves them with every warp of the SM (the one-warp 64x64 Cholesky is latency-bound,
-// so more solver warps per SM can help where the fused solves do not overlap the MMAs well).
-template <class A>
-static cudaError_t launch_tc(pio_als_handle* h, Side& dst, const SolveParams& p, bool imp, int nlight) {
-  cudaError_t e = cudaSuccess;
-  static bool attr_set[64] = {};
-  if (h->cfg.device < 64 && !attr_set[h->cfg.device]) {
-    if ((e = cudaFuncSetAttribute(A::kernel(true), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)A::kSmem)) != cudaSuccess) return e;
-    if ((e = cudaFuncSetAttribute(A::kernel(false), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)A::kSmem)) != cudaSuccess) return e;
-    if ((e = cudaFuncSetAttribute(A::solver(true), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)A::kSolveSmem)) != cudaSuccess) return e;
-    if ((e = cudaFuncSetAttribute(A::solver(false), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)A::kSolveSmem)) != cudaSuccess) return e;
-    attr_set[h->cfg.device] = true;
-  }
-  typename A::Params tp;
-  tp.dbg = nullptr;
-  tp.timing = nullptr;
-  tp.out = nullptr;
-  tp.out_row0 = 0;
-  if (getenv("PIO_ALS_TC_TIMING")) {
-    if (!h->d_timing && (e = cudaMalloc((void**)&h->d_timing, (size_t)h->sm_count * 16 * 8 * sizeof(long long))) != cudaSuccess) return e;
-    cudaMemsetAsync(h->d_timing, 0, (size_t)h->sm_count * 16 * 8 * sizeof(long long), h->stream);
-    tp.timing = h->d_timing;
-  }
-  if (getenv("PIO_ALS_TC_DEBUG")) {
-    if (h->dbg_rows < (size_t)dst.R) {
-      if (h->d_dbg) cudaFree(h->d_dbg);
-      if ((e = cudaMalloc((void**)&h->d_dbg, (size_t)dst.R * A::kRowFloats * sizeof(float))) != cudaSuccess) return e;
-      h->dbg_rows = dst.R;
-    }
-    cudaMemsetAsync(h->d_dbg, 0, (size_t)dst.R * A::kRowFloats * sizeof(float), h->stream);
-    tp.dbg = h->d_dbg;
-  }
-  const int tile = h->tc_split ? TC_TILE_ROWS : nlight;
-  if (h->tc_split) {
-    const size_t need = (size_t)(nlight < tile ? nlight : tile);
-    if (h->tc_out_rows < need) {
-      if (h->tc_out) cudaFree(h->tc_out);
-      h->tc_out = nullptr;
-      h->tc_out_rows = 0;
-      if ((e = cudaMalloc((void**)&h->tc_out, need * A::kRowFloats * sizeof(float))) != cudaSuccess) return e;
-      h->tc_out_rows = need;
-    }
-  }
-  for (int t0 = p.row_begin; t0 < p.row_end; t0 += tile) {
-    SolveParams q = p;
-    q.row_begin = t0;
-    q.row_end = t0 + tile < p.row_end ? t0 + tile : p.row_end;
-    const int nrows = q.row_end - q.row_begin;
-    tp.sp = q;
-    tp.out = h->tc_split ? h->tc_out : nullptr;
-    tp.out_row0 = t0;
-    int grid = (nrows + A::kPerCta - 1) / A::kPerCta;
-    if (grid > h->sm_count) grid = h->sm_count;
-    A::kernel(imp)<<<grid, A::kThreads, A::kSmem, h->stream>>>(tp);
-    LAUNCHED(h);
-    ++h->st.solve_launches;
-    if ((e = cudaGetLastError()) != cudaSuccess) return e;
-    if (h->tc_split) {
-      int sgrid = (nrows + A::kSolveWarps - 1) / A::kSolveWarps;
-      if (sgrid > 4 * h->sm_count) sgrid = 4 * h->sm_count;
-      A::solver(imp)<<<sgrid, A::kSolveWarps * 32, A::kSolveSmem, h->stream>>>(q, h->tc_out, t0);
-      LAUNCHED(h);
-      ++h->st.solve_launches;
-      if ((e = cudaGetLastError()) != cudaSuccess) return e;
-    }
-  }
-  return e;
-}
-
-template <int WARPS>
-static cudaError_t launch_pair_w(pio_als_handle* h, Side& dst, const SolveParams& p0, bool imp) {
-  cudaError_t e = cudaSuccess;
-  static bool attr_set[64] = {};
-  const size_t smem = pr::smem_bytes(WARPS), fsmem = pr::smem_bytes(1);
-  if (h->cfg.device < 64 && !attr_set[h->cfg.device]) {
-    struct { const void* f; size_t sm; } ks[4] = {{(const void*)pr::als_solve_pair_kernel<true, WARPS>, smem},
-                                                 {(const void*)pr::als_solve_pair_kernel<false, WARPS>, smem},
-                                                 {(const void*)pr::als_finish_pair_kernel<true>, fsmem},
-                                                 {(const void*)pr::als_finish_pair_kernel<false>, fsmem}};
-    for (auto& kf : ks) {
-      if ((e = cudaFuncSetAttribute(kf.f, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kf.sm)) != cudaSuccess) return e;
-      if ((e = cudaFuncSetAttribute(kf.f, cudaFuncAttributePreferredSharedMemoryCarveout, 100)) != cudaSuccess) return e;
-    }
-    attr_set[h->cfg.device] = true;
-  }
-  const int max_ctas = (12 / WARPS) * h->sm_count;
-  auto grid_for = [&](int items) {
-    const int npairs = (items + 1) / 2;
-    const int g = (npairs + WARPS - 1) / WARPS;
-    return g < max_ctas ? g : max_ctas;
-  };
-  auto sk = imp ? pr::als_solve_pair_kernel<true, WARPS> : pr::als_solve_pair_kernel<false, WARPS>;
-  cudaEventRecord(h->ev_start, h->stream);
-  if (dst.n_heavy > 0) {
-    // long rows on the auxiliary stream: parts, then the finish kernel.  Launched first: the kernels are persistent
-    // (one full wave), so the CTAs of the whole-row launch below move in as the part CTAs retire and the finish
-    // kernel overlaps the whole-row kernel instead of waiting behind it.
-    if (!dst.partial) {
-      if ((e = cudaMallocAsync((void**)&dst.partial, sizeof(float) * (size_t)dst.n_parts * pr::PART_FLOATS, h->stream)) != cudaSuccess) return e;
-      cudaEventRecord(h->ev_start, h->stream);
-    }
-    cudaStreamWaitEvent(h->aux, h->ev_start, 0);
-    SolveParams pp = p0;
-    pp.wl_beg = dst.part_beg;
-    pp.wl_end = dst.part_end;
-    pp.partial = dst.partial;
-    pp.n_items = dst.n_parts;
-    pp.row_begin = 0;
-    pp.row_end = dst.n_heavy;
-    sk<<<grid_for(dst.n_parts), 32 * WARPS, smem, h->aux>>>(pp, dst.n_parts);
-    LAUNCHED(h);
-    ++h->st.solve_launches;
-    if ((e = cudaGetLastError()) != cudaSuccess) return e;
-    auto fk = imp ? pr::als_finish_pair_kernel<true> : pr::als_finish_pair_kernel<false>;
-    int fgrid = (dst.n_heavy + 1) / 2;
-    if (fgrid > 12 * h->sm_count) fgrid = 12 * h->sm_count;
-    fk<<<fgrid, 32, fsmem, h->aux>>>(pp, dst.row_part_ptr, dst.n_heavy);
-    LAUNCHED(h);
-    ++h->st.solve_launches;
-    if ((e = cudaGetLastError()) != cudaSuccess) return e;
-  }
-  cudaEventRecord(h->ev_heavy, h->aux);
-  // whole rows, one launch per piece of the local row range (the all-gather of a piece starts when its rows are done)
-  const int C = h->n_pieces;
-  for (int c = 0; c < C; ++c) {
-    const long long plo = (long long)dst.R * c / C, phi = (long long)dst.R * (c + 1) / C;
-    const int lo = plo > dst.n_heavy ? (int)plo : dst.n_heavy;
-    const int hi = phi < dst.n_active ? (int)phi : dst.n_active;
-    if (hi > lo) {
-      SolveParams p = p0;
-      p.row_begin = lo;
-      p.row_end = hi;
-      sk<<<grid_for(hi - lo), 32 * WARPS, smem, h->stream>>>(p, hi - lo);
-      LAUNCHED(h);
-      ++h->st.solve_launches;
-      if ((e = cudaGetLastError()) != cudaSuccess) return e;
-    }
-    cudaEventRecord(h->ev_piece[c], h->stream);
-  }
-  cudaStreamWaitEvent(h->stream, h->ev_heavy, 0);   // the half-step ends when both streams are done
-  h->pieces_done = true;
-  return e;
-}
-
-// Rank 33..64, pair kernel (als_pair_kernel.cuh): persistent CTAs of pair_warps independent warps, twelve warps per
-// SM.  Long rows first (their 512-rating parts as work items, then the finish kernel), then the rows that stay whole.
-static cudaError_t launch_pair(pio_als_handle* h, Side& dst, const SolveParams& p0, bool imp) {
-  switch (h->pair_warps) {
-    case 1: return launch_pair_w<1>(h, dst, p0, imp);
-    case 2: return launch_pair_w<2>(h, dst, p0, imp);
-    case 6: return launch_pair_w<6>(h, dst, p0, imp);
-    case 12: return launch_pair_w<12>(h, dst, p0, imp);
-    default: return launch_pair_w<4>(h, dst, p0, imp);
-  }
-}
-
-template <class Cfg>
-static cudaError_t launch_solve_cfg(pio_als_handle* h, Side& dst, const Side& src) {
-  SolveParams p;
-  p.ptr = dst.ptr;
-  p.idx = dst.idx;
-  p.val = dst.val;
-  p.src = src.F;
-  p.dst = dst.F;
-  p.yty = h->yty;
-  p.nreg = dst.nreg;
-  p.fail = h->d_fail;
-  p.lambda = (float)h->cfg.lambda;
-  p.alpha = (float)h->cfg.alpha;
-  p.k = h->cfg.rank;
-  p.dst_row_offset = h->cfg.world_rank * dst.R;
-  const bool imp = h->cfg.implicit_prefs != 0;
-  cudaError_t e = cudaSuccess;
-  p.wl_beg = nullptr;
-  p.wl_end = nullptr;
-  p.partial = nullptr;
-  p.n_items = 0;
-  if (dst.use_pair && Cfg::KP == 64) return launch_pair(h, dst, p, imp);
-  if (Cfg::LS_PARTIAL) {
-    // rank 65..128: rows in tiles; per tile one Gramian launch over the tile's parts and one lockstep finish launch
-    constexpr int TILE_ROWS = 32768;
-    const int nrows = dst.n_heavy;   // == n_active (heavy_t = 0)
-    if (nrows == 0) return cudaSuccess;
-    const std::vector<int>& rpp = dst.h_row_part_ptr;
-    if (!dst.partial) {
-      int mx = 0;
-      for (int r0 = 0; r0 < nrows; r0 += TILE_ROWS) {
-        const int r1 = r0 + TILE_ROWS < nrows ? r0 + TILE_ROWS : nrows;
-        mx = rpp[r1] - rpp[r0] > mx ? rpp[r1] - rpp[r0] : mx;
-      }
-      if ((e = cudaMallocAsync((void**)&dst.partial, sizeof(float) * (size_t)mx * Cfg::PART_FLOATS, h->stream)) != cudaSuccess) return e;
-    }
-    static bool fattr[64] = {};
-    const size_t fsmem = sizeof(float) * (size_t)FIN128_FLOATS * FIN128_WARPS;
-    if (h->cfg.device < 64 && !fattr[h->cfg.device]) {
-      if ((e = cudaFuncSetAttribute(als_finish_ls128_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)fsmem)) != cudaSuccess) return e;
-      if ((e = cudaFuncSetAttribute(als_finish_ls128_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)fsmem)) != cudaSuccess) return e;
-      fattr[h->cfg.device] = true;
-    }
-    for (int r0 = 0; r0 < nrows; r0 += TILE_ROWS) {
-      const int r1 = r0 + TILE_ROWS < nrows ? r0 + TILE_ROWS : nrows;
-      const int part0 = rpp[r0], np = rpp[r1] - rpp[r0];
-      SolveParams pp = p;
-      pp.wl_beg = dst.part_beg + part0;
-      pp.wl_end = dst.part_end + part0;
-      pp.partial = dst.partial;
-      pp.n_items = np;
-      pp.row_begin = 0;
-      pp.row_end = nrows;
-      const int grid = (np + Cfg::NG - 1) / Cfg::NG;
-      e = imp ? launch_solve_one<Cfg, true>(h, pp, grid, h->stream) : launch_solve_one<Cfg, false>(h, pp, grid, h->stream);
-      if (e != cudaSuccess) return e;
-      int fgrid = (r1 - r0 + FIN128_WARPS - 1) / FIN128_WARPS;
-      if (fgrid > h->sm_count) fgrid = h->sm_count;
-      if (imp) als_finish_ls128_kernel<true><<<fgrid, 32 * FIN128_WARPS, fsmem, h->stream>>>(pp, dst.row_part_ptr, r0, r1 - r0, part0);
-      else als_finish_ls128_kernel<false><<<fgrid, 32 * FIN128_WARPS, fsmem, h->stream>>>(pp, dst.row_part_ptr, r0, r1 - r0, part0);
-      LAUNCHED(h);
-      ++h->st.solve_launches;
-      if ((e = cudaGetLastError()) != cudaSuccess) return e;
-    }
-    return e;
-  }
-  // very long rows: their parts run as ordinary light batch items that emit partial normal equations
-  if (dst.n_heavy > 0) {
-    if (!dst.partial) {
-      if ((e = cudaMallocAsync((void**)&dst.partial, sizeof(float) * (size_t)dst.n_parts * (Cfg::SLOT + Cfg::KP), h->stream)) != cudaSuccess) return e;
-    }
-    SolveParams pp = p;
-    pp.wl_beg = dst.part_beg;
-    pp.wl_end = dst.part_end;
-    pp.partial = dst.partial;
-    pp.n_items = dst.n_parts;
-    pp.row_begin = 0;
-    pp.row_end = dst.n_heavy;
-    const int grid = (dst.n_parts + Cfg::NG - 1) / Cfg::NG;
-    e = imp ? launch_solve_one<Cfg, true>(h, pp, grid, h->stream) : launch_solve_one<Cfg, false>(h, pp, grid, h->stream);
-    if (e != cudaSuccess) return e;
-    // finish: sum the parts of every heavy row in fixed order, then Cholesky
-    {
-      static bool fattr[64] = {};
-      const size_t fsmem = sizeof(float) * 4 * (Cfg::SLOT + 4 * Cfg::KP);
-      auto fk = imp ? als_finish_kernel<Cfg, true> : als_finish_kernel<Cfg, false>;
-      if (h->cfg.device < 64 && !fattr[h->cfg.device]) {
-        if ((e = cudaFuncSetAttribute(als_finish_kernel<Cfg, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)fsmem)) != cudaSuccess) return e;
-        if ((e = cudaFuncSetAttribute(als_finish_kernel<Cfg, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)fsmem)) != cudaSuccess) return e;
-        fattr[h->cfg.device] = true;
-      }
-      const int fgrid = Cfg::WARP_CHOL ? (dst.n_heavy + 3) / 4 : dst.n_heavy;
-      fk<<<fgrid, Cfg::WARP_CHOL ? 128 : Cfg::NT, fsmem, h->stream>>>(pp, dst.row_part_ptr, dst.n_heavy);
-      LAUNCHED(h);
-      ++h->st.solve_launches;
-      if ((e = cudaGetLastError()) != cudaSuccess) return e;
-    }
-  }
-  const int nlight = dst.n_active - dst.n_heavy;
-  if (nlight > 0) {
-    p.row_begin = dst.n_heavy;
-    p.row_end = dst.n_active;
-    if (dst.use_tc && Cfg::KP == 64) {
-      e = launch_tc<tc::Api>(h, dst, p, imp, nlight);
-      if (e != cudaSuccess) return e;
-    } else if (Cfg::KP == 64 && h->use_mma) {
-      // short rows of rank 33..64: one warp per row, mma.sync Gramian (als_mma_kernel.cuh)
-      static bool mattr[64] = {};
-      auto mk = imp ? mm::als_solve_mma_kernel<true> : mm::als_solve_mma_kernel<false>;
-      if (h->cfg.device < 64 && !mattr[h->cfg.device]) {
-        if ((e = cudaFuncSetAttribute(mm::als_solve_mma_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)mm::SMEM_BYTES)) != cudaSuccess) return e;
-        if ((e = cudaFuncSetAttribute(mm::als_solve_mma_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)mm::SMEM_BYTES)) != cudaSuccess) return e;
-        mattr[h->cfg.device] = true;
-      }
-      const int grid = (nlight + mm::WARPS - 1) / mm::WARPS;
-      mk<<<grid, mm::NT, mm::SMEM_BYTES, h->stream>>>(p);
-      LAUNCHED(h);
-      ++h->st.solve_launches;
-      if ((e = cudaGetLastError()) != cudaSuccess) return e;
-    } else {
-      const int grid = (nlight + Cfg::NG - 1) / Cfg::NG;
-      e = imp ? launch_solve_one<Cfg, true>(h, p, grid, h->stream) : launch_solve_one<Cfg, false>(h, p, grid, h->stream);
-      if (e != cudaSuccess) return e;
-    }
-  }
-  return e;
-}
-
+// solve_plan.h decides which kernels a half-step runs and with what geometry; launch_solve_cfg executes that plan.
 using Cfg16 = SolveCfg<16, 4, 25, 8>;
 using Cfg32 = SolveCfg<32, 8, 25, 4>;
 using Cfg64 = SolveCfg<64, 8, 7, 8>;
 using Cfg128 = SolveCfg<128, 8, 2, 9>;
 
-static cudaError_t launch_solve(pio_als_handle* h, Side& dst, const Side& src) {
+// the planner's copy of each kernel's launch geometry
+static_assert(fp32_rows_per_cta(16) == Cfg16::NG && fp32_rows_per_cta(32) == Cfg32::NG &&
+              fp32_rows_per_cta(64) == Cfg64::NG && fp32_rows_per_cta(128) == Cfg128::NG, "SolveCfg::NG");
+static_assert(Cfg16::WARP_CHOL && Cfg32::WARP_CHOL && Cfg64::WARP_CHOL && Cfg128::LS_PARTIAL,
+              "als_finish_kernel runs one warp per row below KP 128, and KP 128 takes the LS128 route");
+static_assert(MMA_ROWS_PER_CTA == mm::WARPS, "mm::WARPS");
+static_assert(TC_ROWS_PER_CTA == tc::Api::kPerCta && TC_SOLVE_ROWS_PER_CTA == tc::Api::kSolveWarps, "tc::Api");
+static_assert(LS128_FINISH_ROWS_PER_CTA == FIN128_WARPS, "FIN128_WARPS");
+// a part boundary never splits a chunk of any kernel or a wgmma stage; the pair part length stays a multiple of its chunk
+static_assert(PART % Cfg16::CH == 0 && PART % Cfg32::CH == 0 && PART % Cfg64::CH == 0 && PART % Cfg128::CH == 0 &&
+              PART % mm::CH == 0 && PART % tc::STAGE_RATINGS == 0, "PART");
+static_assert(PAIR_PART % pr::CH == 0 && pr::CH == 8, "PAIR_PART and PIO_ALS_PART round to multiples of pr::CH");
+
+// cudaFuncSetAttribute(MaxDynamicSharedMemorySize) SETS a kernel's limit on the current device, it does not raise it.  A
+// kernel launched from several call sites therefore needs one record of the limit in place, shared by all handles and
+// threads of the process: this one only ever raises it, per kernel and device.  carveout: also ask once for the
+// largest shared-memory carveout.
+static int ensure_dyn_smem(pio_als_handle* h, const void* kernel, size_t bytes, bool carveout = false) {
+  struct Rec {
+    size_t bytes = 0;
+    bool carveout = false;
+  };
+  static std::mutex mu;
+  static std::map<std::pair<const void*, int>, Rec> recs;
+  std::lock_guard<std::mutex> lk(mu);
+  Rec& r = recs[std::make_pair(kernel, h->cfg.device)];
+  if (r.bytes < bytes) {
+    CK(h, cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes));
+    r.bytes = bytes;
+  }
+  if (carveout && !r.carveout) {
+    CK(h, cudaFuncSetAttribute(kernel, cudaFuncAttributePreferredSharedMemoryCarveout, 100));
+    r.carveout = true;
+  }
+  return PIO_ALS_OK;
+}
+
+// Every launch of a half-step's solve goes through here: raise the kernel's dynamic shared-memory limit, launch on `st`,
+// count the launch and fail on a launch error.
+template <typename... KArgs, typename... Args>
+static int solve_launch(pio_als_handle* h, void (*kernel)(KArgs...), int grid, int block, size_t smem, bool carveout,
+                        cudaStream_t st, Args... args) {
+  const int rc = ensure_dyn_smem(h, (const void*)kernel, smem, carveout);
+  if (rc) return rc;
+  kernel<<<grid, block, smem, st>>>(args...);
+  LAUNCHED(h);
+  ++h->st.solve_launches;
+  CK(h, cudaGetLastError());
+  return PIO_ALS_OK;
+}
+
+// the pair kernel with PIO_ALS_PAIR_WARPS warps per CTA
+static void (*pair_kernel(int warps, bool imp))(const SolveParams, int) {
+  switch (warps) {
+    case 1: return imp ? pr::als_solve_pair_kernel<true, 1> : pr::als_solve_pair_kernel<false, 1>;
+    case 2: return imp ? pr::als_solve_pair_kernel<true, 2> : pr::als_solve_pair_kernel<false, 2>;
+    case 6: return imp ? pr::als_solve_pair_kernel<true, 6> : pr::als_solve_pair_kernel<false, 6>;
+    case 12: return imp ? pr::als_solve_pair_kernel<true, 12> : pr::als_solve_pair_kernel<false, 12>;
+    default: return imp ? pr::als_solve_pair_kernel<true, 4> : pr::als_solve_pair_kernel<false, 4>;
+  }
+}
+
+// Buffers of the wgmma kernel, before its first launch of a half-step: the PIO_ALS_TC_TIMING / PIO_ALS_TC_DEBUG dumps
+// and, in split mode (PIO_ALS_TC_SPLIT=1, off by default), the normal equations of one tile of rows, which a second
+// kernel solves with every warp of the SM (the one-warp 64x64 Cholesky is latency-bound, so more solver warps per SM
+// can help where the fused solves do not overlap the MMAs well).
+static int tc_buffers(pio_als_handle* h, const Side& dst, tc::Api::Params* tp) {
+  using A = tc::Api;
+  tp->dbg = nullptr;
+  tp->timing = nullptr;
+  tp->out = nullptr;
+  tp->out_row0 = 0;
+  if (h->sw.tc_timing) {
+    if (!h->d_timing) CK(h, cudaMalloc((void**)&h->d_timing, (size_t)h->sm_count * 16 * 8 * sizeof(long long)));
+    cudaMemsetAsync(h->d_timing, 0, (size_t)h->sm_count * 16 * 8 * sizeof(long long), h->stream);
+    tp->timing = h->d_timing;
+  }
+  if (h->sw.tc_debug) {
+    if (h->dbg_rows < (size_t)dst.R) {
+      if (h->d_dbg) cudaFree(h->d_dbg);
+      CK(h, cudaMalloc((void**)&h->d_dbg, (size_t)dst.R * A::kRowFloats * sizeof(float)));
+      h->dbg_rows = dst.R;
+    }
+    cudaMemsetAsync(h->d_dbg, 0, (size_t)dst.R * A::kRowFloats * sizeof(float), h->stream);
+    tp->dbg = h->d_dbg;
+  }
+  if (h->sw.tc_split) {
+    const int nlight = dst.n_active - dst.n_heavy;
+    const size_t need = (size_t)(nlight < TC_TILE_ROWS ? nlight : TC_TILE_ROWS);
+    if (h->tc_out_rows < need) {
+      if (h->tc_out) cudaFree(h->tc_out);
+      h->tc_out = nullptr;
+      h->tc_out_rows = 0;
+      CK(h, cudaMalloc((void**)&h->tc_out, need * A::kRowFloats * sizeof(float)));
+      h->tc_out_rows = need;
+    }
+  }
+  return PIO_ALS_OK;
+}
+
+template <class Cfg>
+static int launch_solve_cfg(pio_als_handle* h, Side& dst, const Side& src) {
+  SolveParams p0;
+  p0.ptr = dst.ptr;
+  p0.idx = dst.idx;
+  p0.val = dst.val;
+  p0.src = src.F;
+  p0.dst = dst.F;
+  p0.yty = h->yty;
+  p0.nreg = dst.nreg;
+  p0.fail = h->d_fail;
+  p0.lambda = (float)h->cfg.lambda;
+  p0.alpha = (float)h->cfg.alpha;
+  p0.k = h->cfg.rank;
+  p0.dst_row_offset = h->cfg.world_rank * dst.R;
+  p0.wl_beg = nullptr;
+  p0.wl_end = nullptr;
+  p0.partial = nullptr;
+  p0.n_items = 0;
+  const bool imp = h->cfg.implicit_prefs != 0;
+  const SolvePlan plan = plan_half_step(h->sw, dst.plan, Cfg::KP, h->sm_count, dst.R, dst.n_active, dst.n_heavy,
+                                        dst.n_parts, dst.h_row_part_ptr);
+  const bool pair = dst.plan.kernel == SOLVE_PAIR;
+  if (pair) cudaEventRecord(h->ev_start, h->stream);
+  if (plan.partial_parts > 0 && !dst.partial) {
+    const size_t floats = pair ? pr::PART_FLOATS : Cfg::PART_FLOATS;
+    CK(h, cudaMallocAsync((void**)&dst.partial, sizeof(float) * (size_t)plan.partial_parts * floats, h->stream));
+    if (pair) cudaEventRecord(h->ev_start, h->stream);
+  }
+  if (plan.n_aux > 0) cudaStreamWaitEvent(h->aux, h->ev_start, 0);
+  // pair path: ev_heavy once the long rows are launched on aux, ev_piece[c] once the rows of piece c are launched (the
+  // all-gather of a piece starts when its rows are done)
+  size_t next_piece = 0;
+  auto record_events = [&](int issued) {
+    if (pair && issued == plan.n_aux) cudaEventRecord(h->ev_heavy, h->aux);
+    for (; next_piece < plan.piece_after.size() && plan.piece_after[next_piece] == issued; ++next_piece)
+      cudaEventRecord(h->ev_piece[next_piece], h->stream);
+  };
+  record_events(0);
+  const int warps = h->sw.pair_warps;
+  tc::Api::Params tp;
+  bool tc_ready = false;
+  for (size_t i = 0; i < plan.launches.size(); ++i) {
+    const SolveLaunch& L = plan.launches[i];
+    const cudaStream_t st = L.aux ? h->aux : h->stream;
+    const int nrows = L.row_end - L.row_begin;
+    SolveParams p = p0;
+    if (L.stage == STAGE_ROWS || L.stage == STAGE_TC_SOLVE) {
+      p.row_begin = L.row_begin;
+      p.row_end = L.row_end;
+    } else {   // work-list stages: parts [wl_off, wl_off + wl_count) of the heavy rows
+      p.wl_beg = dst.part_beg + L.wl_off;
+      p.wl_end = dst.part_end + L.wl_off;
+      p.partial = dst.partial;
+      p.n_items = L.wl_count;
+      p.row_begin = 0;
+      p.row_end = dst.n_heavy;
+    }
+    auto fp32 = [&] {
+      return solve_launch(h, imp ? als_solve_kernel<Cfg, true> : als_solve_kernel<Cfg, false>, L.grid, Cfg::NT,
+                          Cfg::smem_bytes(), false, st, p);
+    };
+    auto pair_items = [&](int n_items) {
+      return solve_launch(h, pair_kernel(warps, imp), L.grid, 32 * warps, pr::smem_bytes(warps), true, st, p, n_items);
+    };
+    int rc = PIO_ALS_OK;
+    switch (L.stage) {
+      case STAGE_PARTS:
+        rc = pair ? pair_items(L.wl_count) : fp32();
+        break;
+      case STAGE_FINISH:
+        rc = pair ? solve_launch(h, imp ? pr::als_finish_pair_kernel<true> : pr::als_finish_pair_kernel<false>, L.grid,
+                                 32, pr::smem_bytes(1), true, st, p, dst.row_part_ptr, nrows)
+                  : solve_launch(h, imp ? als_finish_kernel<Cfg, true> : als_finish_kernel<Cfg, false>, L.grid,
+                                 32 * FINISH_ROWS_PER_CTA, sizeof(float) * 4 * (Cfg::SLOT + 4 * Cfg::KP), false, st, p,
+                                 dst.row_part_ptr, nrows);
+        break;
+      case STAGE_LS128_TILE:
+        rc = fp32();
+        break;
+      case STAGE_LS128_FINISH:
+        rc = solve_launch(h, imp ? als_finish_ls128_kernel<true> : als_finish_ls128_kernel<false>, L.grid,
+                          32 * FIN128_WARPS, sizeof(float) * (size_t)FIN128_FLOATS * FIN128_WARPS, false, st, p,
+                          dst.row_part_ptr, L.row_begin, nrows, L.wl_off);
+        break;
+      case STAGE_ROWS:
+        switch (dst.plan.kernel) {
+          case SOLVE_PAIR:
+            rc = pair_items(nrows);
+            break;
+          case SOLVE_MMA:
+            rc = solve_launch(h, imp ? mm::als_solve_mma_kernel<true> : mm::als_solve_mma_kernel<false>, L.grid, mm::NT,
+                              mm::SMEM_BYTES, false, st, p);
+            break;
+          case SOLVE_WGMMA:
+            if (!tc_ready) {
+              rc = tc_buffers(h, dst, &tp);
+              if (rc) return rc;
+              tc_ready = true;
+            }
+            tp.sp = p;
+            tp.out = h->sw.tc_split ? h->tc_out : nullptr;
+            tp.out_row0 = L.row_begin;
+            rc = solve_launch(h, tc::Api::kernel(imp), L.grid, tc::Api::kThreads, tc::Api::kSmem, false, st, tp);
+            break;
+          default:
+            rc = fp32();
+        }
+        break;
+      case STAGE_TC_SOLVE:
+        rc = solve_launch(h, tc::Api::solver(imp), L.grid, 32 * tc::Api::kSolveWarps, tc::Api::kSolveSmem, false, st, p,
+                          (const float*)h->tc_out, L.row_begin);
+        break;
+    }
+    if (rc) return rc;
+    record_events((int)i + 1);
+  }
+  if (pair) {
+    cudaStreamWaitEvent(h->stream, h->ev_heavy, 0);   // the half-step ends when both streams are done
+    h->pieces_done = true;
+  }
+  return PIO_ALS_OK;
+}
+
+static int launch_solve(pio_als_handle* h, Side& dst, const Side& src) {
   switch (h->KP) {
     case 16: return launch_solve_cfg<Cfg16>(h, dst, src);
     case 32: return launch_solve_cfg<Cfg32>(h, dst, src);
@@ -1361,7 +1259,8 @@ static int half_step(pio_als_handle* h, Side& dst, const Side& src, bool more) {
     cudaEventRecord(e.a, st);
     h->pieces_done = false;
     if (h->gram_side == &dst) h->gram_side = nullptr;
-    CK(h, launch_solve(h, dst, src));
+    const int rc = launch_solve(h, dst, src);
+    if (rc) return rc;
     cudaEventRecord(e.b, st);
   }
   const bool prep = implicit && more;
@@ -1370,11 +1269,11 @@ static int half_step(pio_als_handle* h, Side& dst, const Side& src, bool more) {
     NcclApi& nc = nccl_api();
     const int W = h->cfg.world_size, me = h->cfg.world_rank;
     const EvPair e = next_ev(h, EV_COMM);
-    if (h->pieces_done && h->n_pieces > 1) {
+    if (h->pieces_done && h->sw.n_pieces > 1) {
       // all-gather piece by piece on the communication stream: piece c = local rows [R c / C, R (c + 1) / C) of every
       // rank, exchanged as soon as its rows are solved (grouped send/recv: NVSwitch gives every pair full bandwidth)
       cudaStream_t sc = h->comm_st;
-      const int C = h->n_pieces;
+      const int C = h->sw.n_pieces;
       bool first = true;
       for (int c = 0; c < C; ++c) {
         const long long lo = (long long)dst.R * c / C, hi = (long long)dst.R * (c + 1) / C;
@@ -1502,35 +1401,11 @@ static int create_common(pio_als_handle* h) {
       if (cudaEventCreateWithFlags(evs[i], cudaEventDisableTiming) != cudaSuccess) return fail(nullptr, PIO_ALS_ERR_CUDA, "cudaEventCreate");
     for (int i = 0; i < 8; ++i)
       if (cudaEventCreateWithFlags(&h->ev_piece[i], cudaEventDisableTiming) != cudaSuccess) return fail(nullptr, PIO_ALS_ERR_CUDA, "cudaEventCreate");
-    h->n_pieces = h->cfg.world_size > 1 ? 4 : 1;
     if (const char* v = getenv("PIO_ALS_SERVE_FUSED")) h->serve_fused = atoi(v) != 0;
     if (const char* v = getenv("PIO_ALS_SERVE_TRACE")) h->serve_trace = atoi(v) != 0;
     if (const char* v = getenv("PIO_ALS_SCORE_BLOCKED")) h->score_blocked = atoi(v) != 0;
-    if (const char* v = getenv("PIO_ALS_PIECES")) {
-      const int n = atoi(v);
-      if (n >= 1 && n <= 8) h->n_pieces = n;
-    }
   }
-  {
-    // Rank 33..64 kernel selection.  Default: the pair kernel (als_pair_kernel.cuh: mma.sync 3xTF32 Gramian, two rows per
-    // warp, lockstep Cholesky) for every side -- every warp gathers, accumulates and solves, so it needs no producer
-    // warps -- and, with rows above 1024 ratings summed in two levels, it stays inside the parity bound on long rows.
-    // PIO_ALS_TC=1: the wgmma Gramian kernel (als_tc_kernel.cuh) for
-    // every side (PIO_ALS_TC_MIN_DEG=n: only sides averaging >= n ratings per row); PIO_ALS_MMA=1: the round-1
-    // one-warp-per-row mma.sync kernel; PIO_ALS_MMA=0: the FP32 CUDA-core kernel.
-    const char* env = getenv("PIO_ALS_TC");
-    h->use_tc = h->KP == 64 && env && env[0] == '1';
-    h->tc_min_deg = 0.0;
-    if (const char* md = getenv("PIO_ALS_TC_MIN_DEG")) h->tc_min_deg = atof(md);
-    if (const char* sp = getenv("PIO_ALS_TC_SPLIT")) h->tc_split = sp[0] == '1';
-    if (const char* mm_ = getenv("PIO_ALS_MMA")) {
-      h->use_mma = mm_[0] != '0';
-      h->use_pair = mm_[0] != '1';
-    }
-    if (const char* v = getenv("PIO_ALS_PAIR_WARPS")) h->pair_warps = atoi(v);
-    if (const char* v = getenv("PIO_ALS_SEG_T")) h->pair_seg_t = atoi(v) > 0 ? atoi(v) : PAIR_SEG_T;
-    if (const char* v = getenv("PIO_ALS_PART")) h->pair_part = atoi(v) >= 8 ? (atoi(v) + 7) / 8 * 8 : PAIR_PART;
-  }
+  h->sw = read_solve_switches(getenv, h->KP, h->cfg.world_size);
   h->gram_blocks = GRAM_GROUPS * h->sm_count;   // a sharded run gives every rank whole groups: one CTA per SM at 8 GPUs
   if (cudaMallocAsync((void**)&h->yty, sizeof(float) * h->KP * h->KP, h->stream) != cudaSuccess ||
       cudaMallocAsync((void**)&h->gram_partial, sizeof(double) * (size_t)h->gram_blocks * h->KP * h->KP, h->stream) != cudaSuccess ||
@@ -1760,10 +1635,9 @@ int pio_als_get_phase_ms(pio_als_handle* h, double out[8]) {
   if (!h || !out) return PIO_ALS_ERR_ARG;
   std::lock_guard<std::mutex> lk(h->mu);
   for (int i = 0; i < 8; ++i) out[i] = h->phase_ms[i];
-  // kernel of the rows below the heavy-row threshold: 0 = FP32 (als_solve_kernel), 1 = wgmma, 2 = mma.sync
-  const bool mma = h->KP == 64 && h->use_mma;
-  out[4] = h->I.use_tc ? 1.0 : h->I.use_pair ? 3.0 : (mma ? 2.0 : 0.0);
-  out[5] = h->U.use_tc ? 1.0 : h->U.use_pair ? 3.0 : (mma ? 2.0 : 0.0);
+  // kernel of the rows below the heavy-row threshold: 0 = FP32 (als_solve_kernel), 1 = wgmma, 2 = mma.sync, 3 = pair
+  out[4] = phase_code(h->I.plan.kernel);
+  out[5] = phase_code(h->U.plan.kernel);
   return PIO_ALS_OK;
 }
 
@@ -1846,20 +1720,6 @@ struct ArenaLayout {
     return at;
   }
 };
-
-// cudaFuncSetAttribute(MaxDynamicSharedMemorySize) SETS a kernel's limit on the current device, it does not raise it.  A
-// kernel launched from several call sites therefore needs one record of the limit in place, shared by all handles and
-// threads of the process: this one only ever raises it, per kernel and device.
-static int ensure_dyn_smem(pio_als_handle* h, const void* kernel, size_t bytes) {
-  static std::mutex mu;
-  static std::map<std::pair<const void*, int>, size_t> limit;
-  std::lock_guard<std::mutex> lk(mu);
-  size_t& cur = limit[std::make_pair(kernel, h->cfg.device)];
-  if (cur >= bytes) return PIO_ALS_OK;
-  CK(h, cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes));
-  cur = bytes;
-  return PIO_ALS_OK;
-}
 
 // Every launch of a scoring call goes through here: raise the kernel's dynamic shared-memory limit when it takes any,
 // launch on the handle's stream, count the launch, record which scoring kernel ran (path: its PIO_ALS_PATH_* bit, 0 for

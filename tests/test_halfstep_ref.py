@@ -76,9 +76,10 @@ def test_backward_error_measures(implicit):
     assert H.half_step(i, u, r, ni, u0, lam, implicit, alpha, cand=x).eta[row] >= 1e-5
 
 
-def test_degree_ladder_straddles_every_threshold():
-    """Moving a row-length threshold in the CUDA sources without moving the GPU tests' degree ladder fails here."""
-    host, tc = G.source_constants("pio_als.cu"), G.source_constants("als_tc_kernel.cuh")
+def test_degree_ladder_straddles_every_planner_threshold():
+    """Moving a row-length threshold in the solve planner (solve_plan.h) or the CUDA sources without moving the GPU
+    tests' degree ladder fails here."""
+    host, tc = G.source_constants("solve_plan.h"), G.source_constants("als_tc_kernel.cuh")
     assert G.HEAVY == {"pair": host["PAIR_SEG_T"], "mma": host["HEAVY_T_TC"], "wgmma": host["HEAVY_T_TC"],
                        "fp32": host["HEAVY_T"]}
     ladder = set(G.DEGREE_LADDER)
@@ -94,5 +95,5 @@ def test_degree_ladder_straddles_every_threshold():
     assert max(ladder) > host["HEAVY_T_TC"] + host["PART"]              # several parts on every path
     assert set(range(1, 10)) <= ladder and {15, 16, 17} <= ladder
     # the rank 65..128 case has more active rows on one side than one tile of the work-list launch
-    assert G.SCALE_ROWS > host["TILE_ROWS"]
+    assert G.SCALE_ROWS > host["LS128_TILE_ROWS"]
     assert max(G.SCALE_HEAVY) > 2 * host["PART"]
