@@ -233,6 +233,53 @@ PIO_API int pio_als_synth_ratings_device(int device, int32_t n_users, int32_t n_
 PIO_API int pio_ids_encode(int device, const uint8_t* bytes, const int64_t* offsets, int64_t n, int32_t* out_index,
                            int64_t* out_first, int32_t* out_n_unique);
 
+/* Event file scan: PEventStore.find (data/src/main/scala/org/apache/predictionio/data/store/PEventStore.scala:59-119)
+ * over text in the `pio import` / `pio export` JSON-lines format (tools/src/main/scala/org/apache/predictionio/tools/
+ * imprt/FileToEvents.scala:93-103), producing event columns instead of Event objects (DESIGN.md 3.1).
+ * Strings are NUL-terminated UTF-8. */
+#define PIO_EVENTS_TARGET_ANY 0      /* targetEntityType not restricted */
+#define PIO_EVENTS_TARGET_ABSENT 1   /* targetEntityType must be absent (Some(None)) */
+#define PIO_EVENTS_TARGET_EQUALS 2   /* targetEntityType must equal target_entity_type (Some(Some(x))) */
+#define PIO_EVENTS_MIN_EVENT_BYTES 64 /* no matched line is shorter: n_bytes / 64 + 1 events always fit */
+#define PIO_EVENTS_HAS_VALUE 1       /* out_flags bits */
+#define PIO_EVENTS_HAS_TARGET 2
+
+typedef struct pio_events_filter {
+  const char* entity_type;             /* NULL = any entity type */
+  const char* const* event_names;      /* an event's output code is the index of its name here; NULL = any event
+                                          name (code -1), as eventNames = None in find */
+  int32_t n_event_names;               /* with event_names != NULL, 0 = an empty list: no event matches */
+  int32_t target_entity_type_mode;     /* PIO_EVENTS_TARGET_* */
+  const char* target_entity_type;      /* for PIO_EVENTS_TARGET_EQUALS */
+  const char* property;                /* numeric property to extract (DataMap.get(name, Double)); NULL = none */
+  int32_t has_start, has_until;        /* eventTime >= start_us, eventTime < until_us (half-open, as in find) */
+  int64_t start_us, until_us;          /* microseconds since 1970-01-01T00:00:00Z */
+} pio_events_filter;
+
+/* text[0 .. n_bytes): complete lines, ended by "\n", "\r\n" or a lone "\r" (the last one may lack its terminator); HOST
+ * buffers.  Lines are numbered from 0, blank ones included; a line that is empty after stripping spaces and tabs is
+ * no event.  Every line is either parsed on the device -- exactly as Event.from_json(json.loads(line)) and find's
+ * filter would take it -- or listed as a fallback line for the caller to parse (anything outside the accepted grammar,
+ * DESIGN.md 3.1; falling back is always correct).
+ * Per matched event, in line order (capacity entries, capacity >= n_bytes / PIO_EVENTS_MIN_EVENT_BYTES + 1):
+ *   out_line (line index), out_code (event-name index), out_value + out_flags & PIO_EVENTS_HAS_VALUE (the property as
+ *   a double; a property value that is not a number exact in double makes the line a fallback line), out_time_us,
+ *   out_flags & PIO_EVENTS_HAS_TARGET (targetEntityId present), and the decoded entityId / targetEntityId bytes:
+ *   event e's id is out_eid_bytes[out_eid_off[e] .. out_eid_off[e + 1]) (offsets: capacity + 1 entries; bytes: n_bytes
+ *   suffice, decoded ids are never longer than their JSON text).
+ * Fallback lines, in line order: out_fb_line, and the line's bytes text[out_fb_begin .. out_fb_end) without the
+ *   terminator.  *out_n_fallback is the number of fallback lines; when it exceeds fb_capacity only the first
+ *   fb_capacity were written: call again with room for all of them.
+ * *out_n_lines = number of lines.  PIO_ALS_ERR_ARG for a bad filter or sizes; PIO_ALS_ERR_CUDA without a device.
+ * Device memory is bounded by the device chunk (64 MB), not by n_bytes; the copy of one chunk overlaps the scan of the
+ * one before. */
+PIO_API int pio_events_scan(int device, const uint8_t* text, int64_t n_bytes, const pio_events_filter* filter,
+                            int64_t capacity, int64_t* out_line, int32_t* out_code, double* out_value,
+                            uint8_t* out_flags, int64_t* out_time_us, uint8_t* out_eid_bytes, int64_t* out_eid_off,
+                            uint8_t* out_tid_bytes, int64_t* out_tid_off, int64_t* out_n_events, int64_t fb_capacity,
+                            int64_t* out_fb_line, int64_t* out_fb_begin, int64_t* out_fb_end, int64_t* out_n_fallback,
+                            int64_t* out_n_lines);
+
 /* Item co-occurrence of the similarproduct template's CooccurrenceAlgorithm.trainCooccurrence
  * (examples/scala-parallel-similarproduct/multi-events-multi-algos/src/main/scala/CooccurrenceAlgorithm.scala:72-105):
  * (user, item) view events (indices, HOST) -> distinct -> for every user all item pairs -> count per pair -> for every item the

@@ -47,6 +47,7 @@
 #include "score_plan.h"
 #include "solve_plan.h"
 #include "ids_encode.cuh"
+#include "events_scan.cuh"
 #include "cooc.cuh"
 
 namespace pio {
@@ -2607,6 +2608,326 @@ int pio_ids_encode(int device, const uint8_t* bytes, const int64_t* offsets, int
   const int64_t nuniq = (int64_t)last_ex + last_flag;
   if (out_first) CK0(cudaMemcpy(out_first, d_first, 8 * (size_t)nuniq, cudaMemcpyDeviceToHost));
   *out_n_unique = (int32_t)nuniq;
+  return PIO_ALS_OK;
+}
+
+// ---- event file scan (PEventStore.findColumns; events_scan.cuh) --------------------------------------------------------
+// Where the time of the last pio_events_scan on this thread went, summed over its chunks (pio_events_debug_timing).
+struct EvTiming {
+  double h2d_ms, kernel_ms, d2h_ms, stage_ms;   // device times (CUDA events); stage: host copy into pinned memory
+  int64_t chunks;
+};
+static thread_local EvTiming g_ev_timing;
+static_assert(PIO_EVENTS_MIN_EVENT_BYTES <= ev::MIN_MATCHED_BYTES, "capacity bound of pio_events_scan");
+
+// End of the device chunk that starts at b: after the last terminator in [b, b + cap), never between the "\r" and "\n"
+// of a CRLF; b when [b, b + cap) holds no usable terminator (the line at b is longer than a chunk).
+static int64_t ev_cut(const uint8_t* t, int64_t n, int64_t b, int64_t cap) {
+  if (n - b <= cap) return n;
+  const int64_t lim = b + cap;
+  for (int64_t p = lim - 1; p >= b; --p) {
+    if (t[p] == '\n') return p + 1;
+    if (t[p] == '\r' && t[p + 1] != '\n') return p + 1;   // p + 1 <= lim < n
+  }
+  return b;
+}
+
+int pio_events_scan(int device, const uint8_t* text, int64_t n_bytes, const pio_events_filter* f, int64_t capacity,
+                    int64_t* out_line, int32_t* out_code, double* out_value, uint8_t* out_flags, int64_t* out_time_us,
+                    uint8_t* out_eid_bytes, int64_t* out_eid_off, uint8_t* out_tid_bytes, int64_t* out_tid_off,
+                    int64_t* out_n_events, int64_t fb_capacity, int64_t* out_fb_line, int64_t* out_fb_begin,
+                    int64_t* out_fb_end, int64_t* out_n_fallback, int64_t* out_n_lines) {
+  if (n_bytes < 0 || (n_bytes > 0 && !text) || !f || capacity < n_bytes / PIO_EVENTS_MIN_EVENT_BYTES + 1 ||
+      fb_capacity < 0 || !out_line || !out_code || !out_value || !out_flags || !out_time_us || !out_eid_bytes ||
+      !out_eid_off || !out_tid_bytes || !out_tid_off || !out_n_events || (fb_capacity > 0 && (!out_fb_line ||
+      !out_fb_begin || !out_fb_end)) || !out_n_fallback || !out_n_lines)
+    return fail(nullptr, PIO_ALS_ERR_ARG, "bad pio_events_scan arguments");
+  if (f->n_event_names < 0 || (f->n_event_names > 0 && !f->event_names))
+    return fail(nullptr, PIO_ALS_ERR_ARG, "bad event name list");
+  for (int k = 0; k < f->n_event_names; ++k)
+    if (!f->event_names[k]) return fail(nullptr, PIO_ALS_ERR_ARG, "event name %d is NULL", k);
+  if (f->target_entity_type_mode < PIO_EVENTS_TARGET_ANY || f->target_entity_type_mode > PIO_EVENTS_TARGET_EQUALS ||
+      (f->target_entity_type_mode == PIO_EVENTS_TARGET_EQUALS && !f->target_entity_type))
+    return fail(nullptr, PIO_ALS_ERR_ARG, "bad target_entity_type_mode / target_entity_type");
+  *out_n_events = *out_n_fallback = *out_n_lines = 0;
+  out_eid_off[0] = out_tid_off[0] = 0;
+  if (n_bytes == 0) return PIO_ALS_OK;
+  CK0(cudaSetDevice(device));
+
+  // the filter's strings, packed: entity type | target entity type | property | names...
+  std::vector<uint8_t> fbytes;
+  auto put = [&](const char* s) -> int {
+    const size_t at = fbytes.size();
+    fbytes.insert(fbytes.end(), s, s + strlen(s));
+    return (int)at;
+  };
+  const int at_et = f->entity_type ? put(f->entity_type) : 0;
+  const int len_et = f->entity_type ? (int)(fbytes.size() - at_et) : -1;
+  const int at_tt = f->target_entity_type_mode == PIO_EVENTS_TARGET_EQUALS ? put(f->target_entity_type) : 0;
+  const int len_tt = (int)fbytes.size() - at_tt;
+  const int at_pr = f->property ? put(f->property) : 0;
+  const int len_pr = f->property ? (int)(fbytes.size() - at_pr) : -1;
+  std::vector<int> noff(1, (int)fbytes.size());
+  for (int k = 0; k < f->n_event_names; ++k) {
+    put(f->event_names[k]);
+    noff.push_back((int)fbytes.size());
+  }
+
+  int64_t cap = 64ll << 20;   // device chunk; PIO_EVENTS_DEVICE_CHUNK (bytes) lets tests straddle its boundaries
+  if (const char* c = getenv("PIO_EVENTS_DEVICE_CHUNK")) {
+    const long long v = atoll(c);
+    if (v >= 1 && v <= (1ll << 30)) cap = v;
+  }
+  if (cap > n_bytes) cap = n_bytes;
+
+  std::vector<void*> owned, pinned;
+  cudaStream_t streams[2] = {nullptr, nullptr};
+  // copy begin / end per staging slot, then on the scan stream: kernels before and after the line count, and the
+  // device-to-host copies (pio_events_debug_timing)
+  cudaEvent_t evs[10] = {};
+  cudaEvent_t *h2d_begin = evs, *copied = evs + 2, &k0 = evs[4], &k1 = evs[5], &k2 = evs[6], &k3 = evs[7],
+              &d0 = evs[8], &d1 = evs[9];
+  struct Guard {
+    std::vector<void*>& d;
+    std::vector<void*>& p;
+    cudaStream_t* s;
+    cudaEvent_t* e;
+    ~Guard() {
+      for (int k = 0; k < 2; ++k)
+        if (s[k]) cudaStreamSynchronize(s[k]);
+      for (void* q : d) cudaFree(q);
+      for (void* q : p) cudaFreeHost(q);
+      for (int k = 0; k < 2; ++k)
+        if (s[k]) cudaStreamDestroy(s[k]);
+      for (int k = 0; k < 10; ++k)
+        if (e[k]) cudaEventDestroy(e[k]);
+    }
+  } guard{owned, pinned, streams, evs};
+  auto A = [&](void** p, size_t bytes_) -> cudaError_t {
+    cudaError_t e = cudaMalloc(p, bytes_ ? bytes_ : 1);
+    if (e == cudaSuccess) owned.push_back(*p);
+    return e;
+  };
+  auto P = [&](void** p, size_t bytes_) -> cudaError_t {
+    cudaError_t e = cudaHostAlloc(p, bytes_ ? bytes_ : 1, cudaHostAllocDefault);
+    if (e == cudaSuccess) pinned.push_back(*p);
+    return e;
+  };
+  for (int k = 0; k < 2; ++k) CK0(cudaStreamCreateWithFlags(&streams[k], cudaStreamNonBlocking));
+  for (cudaEvent_t& e : evs) CK0(cudaEventCreate(&e));
+  EvTiming& tm = g_ev_timing;
+  tm = EvTiming{};
+  bool use_smem = true;   // PIO_EVENTS_SMEM=0: the parse reads its lines from global memory (A/B measurements)
+  if (const char* c = getenv("PIO_EVENTS_SMEM")) use_smem = atoi(c) != 0;
+  if (use_smem)
+    CK0(cudaFuncSetAttribute(ev_parse_smem_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, EV_SMEM_BYTES));
+  cudaStream_t ex = streams[0], cp = streams[1];   // scan, host-to-device copies
+  uint8_t *d_text[2] = {nullptr, nullptr}, *stage[2] = {nullptr, nullptr}, *d_scratch = nullptr, *d_fbytes = nullptr;
+  uint32_t *d_flag = nullptr, *d_lid = nullptr, *d_tot = nullptr, *h_tot = nullptr;
+  int* d_noff = nullptr;
+  for (int k = 0; k < 2; ++k) {
+    CK0(A((void**)&d_text[k], (size_t)cap));
+    CK0(P((void**)&stage[k], (size_t)cap));
+  }
+  CK0(A((void**)&d_scratch, (size_t)cap));
+  CK0(A((void**)&d_flag, 4 * (size_t)cap));
+  CK0(A((void**)&d_lid, 4 * (size_t)cap));
+  CK0(A((void**)&d_fbytes, fbytes.size()));
+  CK0(A((void**)&d_noff, sizeof(int) * noff.size()));
+  CK0(A((void**)&d_tot, 4 * sizeof(uint32_t)));
+  CK0(P((void**)&h_tot, 8 * sizeof(uint32_t)));
+  if (!fbytes.empty()) CK0(cudaMemcpy(d_fbytes, fbytes.data(), fbytes.size(), cudaMemcpyHostToDevice));
+  CK0(cudaMemcpy(d_noff, noff.data(), sizeof(int) * noff.size(), cudaMemcpyHostToDevice));
+  ev::Filter df;
+  df.entity_type = d_fbytes + at_et;
+  df.entity_type_len = len_et;
+  df.names = d_fbytes;
+  df.name_off = d_noff;
+  df.n_names = f->event_names ? f->n_event_names : -1;   // NULL: any name; an empty list: none
+  df.target_mode = f->target_entity_type_mode;
+  df.target = d_fbytes + at_tt;
+  df.target_len = len_tt;
+  df.prop = d_fbytes + at_pr;
+  df.prop_len = len_pr;
+  df.has_start = f->has_start != 0;
+  df.has_until = f->has_until != 0;
+  df.start_us = f->start_us;
+  df.until_us = f->until_us;
+
+  EvBase base{0, 0, 0, 0};
+  int64_t n_ev = 0, n_fb = 0;   // n_fb counts every fallback line, also those beyond fb_capacity
+  // lines longer than a chunk, found while cutting the next chunk: written after the current chunk's fallback lines so
+  // that the fallback list stays in line order
+  std::vector<int64_t> oversized;
+  auto flush_oversized = [&]() {
+    for (size_t k = 0; k < oversized.size(); k += 3) {
+      if (n_fb < fb_capacity)
+        out_fb_line[n_fb] = oversized[k], out_fb_begin[n_fb] = oversized[k + 1], out_fb_end[n_fb] = oversized[k + 2];
+      ++n_fb;
+    }
+    oversized.clear();
+  };
+  // stage a chunk: host copy into pinned memory, then an asynchronous copy on cp.  The loop below calls it for chunk
+  // k + 1 after it has launched the parse of chunk k, so that both copies run while the device parses.
+  auto prefetch = [&](int slot, int64_t b, int64_t e) -> int {
+    const auto h0 = std::chrono::steady_clock::now();
+    memcpy(stage[slot], text + b, (size_t)(e - b));
+    tm.stage_ms += std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - h0).count();
+    CK0(cudaEventRecord(h2d_begin[slot], cp));
+    CK0(cudaMemcpyAsync(d_text[slot], stage[slot], (size_t)(e - b), cudaMemcpyHostToDevice, cp));
+    CK0(cudaEventRecord(copied[slot], cp));
+    return PIO_ALS_OK;
+  };
+  auto ms = [](cudaEvent_t a, cudaEvent_t b) {
+    float v = 0.f;
+    cudaEventElapsedTime(&v, a, b);
+    return (double)v;
+  };
+  // the next chunk [b, e) at or after pos; lines longer than a chunk become fallback lines on the way
+  auto next_chunk = [&](int64_t pos, int64_t* b, int64_t* e) {
+    for (;;) {
+      if (pos >= n_bytes) {
+        *b = *e = n_bytes;
+        return;
+      }
+      const int64_t c = ev_cut(text, n_bytes, pos, cap);
+      if (c > pos) {
+        *b = pos, *e = c;
+        return;
+      }
+      int64_t q = pos;   // a line longer than a chunk: the host parses it
+      while (q < n_bytes && text[q] != '\n' && text[q] != '\r') ++q;
+      oversized.insert(oversized.end(), {base.line, pos, q});
+      ++base.line;
+      if (q < n_bytes && text[q] == '\r' && q + 1 < n_bytes && text[q + 1] == '\n') ++q;
+      pos = q < n_bytes ? q + 1 : q;
+    }
+  };
+
+  int64_t cb, ce;
+  next_chunk(0, &cb, &ce);
+  flush_oversized();
+  if (cb < ce && prefetch(0, cb, ce) != PIO_ALS_OK) return PIO_ALS_ERR_CUDA;
+  for (int slot = 0; cb < ce; slot ^= 1) {
+    const long long L = ce - cb;
+    base.byte = cb;
+    CK0(cudaStreamWaitEvent(ex, copied[slot], 0));
+    const uint8_t* t = d_text[slot];
+    CK0(cudaEventRecord(k0, ex));
+    ev_start_flag_kernel<<<nblk(L, EV_THREADS), EV_THREADS, 0, ex>>>(t, L, d_flag);
+    CK0(scan_exclusive_u32(d_flag, d_lid, (size_t)L, ex, nullptr));
+    CK0(cudaMemcpyAsync(h_tot + 4, d_flag + L - 1, 4, cudaMemcpyDeviceToHost, ex));
+    CK0(cudaMemcpyAsync(h_tot + 5, d_lid + L - 1, 4, cudaMemcpyDeviceToHost, ex));
+    CK0(cudaEventRecord(k1, ex));
+    CK0(cudaStreamSynchronize(ex));
+    const long long nl = (long long)h_tot[4] + h_tot[5];
+    const EvBase here = base;
+    base.line += nl;
+
+    std::vector<void*> chunk_mem;
+    struct ChunkGuard {
+      std::vector<void*>& v;
+      cudaStream_t s;
+      ~ChunkGuard() { for (void* q : v) cudaFreeAsync(q, s); }
+    } chunk_guard{chunk_mem, ex};
+    auto CA = [&](void** p, size_t bytes_) -> cudaError_t {
+      cudaError_t e = cudaMallocAsync(p, bytes_ ? bytes_ : 1, ex);
+      if (e == cudaSuccess) chunk_mem.push_back(*p);
+      return e;
+    };
+    uint32_t* starts = nullptr;
+    EvLines Ls;
+    EvOut o;
+    const size_t nls = (size_t)nl;
+    CK0(CA((void**)&starts, 4 * (nls + 1)));
+    uint32_t** u32s[8] = {&Ls.is_match, &Ls.is_fb, &Ls.eid_len, &Ls.tid_len, &Ls.match_pos, &Ls.fb_pos, &Ls.eid_pos,
+                          &Ls.tid_pos};
+    for (uint32_t** p : u32s) CK0(CA((void**)p, 4 * nls));
+    CK0(CA((void**)&Ls.code, 4 * nls));
+    CK0(CA((void**)&Ls.value, 8 * nls));
+    CK0(CA((void**)&Ls.time_us, 8 * nls));
+    CK0(CA((void**)&Ls.flags, nls));
+    CK0(CA((void**)&o.line, 8 * nls));
+    CK0(CA((void**)&o.code, 4 * nls));
+    CK0(CA((void**)&o.value, 8 * nls));
+    CK0(CA((void**)&o.flags, nls));
+    CK0(CA((void**)&o.time_us, 8 * nls));
+    CK0(CA((void**)&o.eid_off, 8 * nls));
+    CK0(CA((void**)&o.tid_off, 8 * nls));
+    CK0(CA((void**)&o.fb_line, 8 * nls));
+    CK0(CA((void**)&o.fb_begin, 8 * nls));
+    CK0(CA((void**)&o.fb_end, 8 * nls));
+    CK0(CA((void**)&o.eid_bytes, (size_t)L));
+    CK0(CA((void**)&o.tid_bytes, (size_t)L));
+    CK0(cudaEventRecord(k2, ex));
+    ev_start_scatter_kernel<<<nblk(L, EV_THREADS), EV_THREADS, 0, ex>>>(d_flag, d_lid, L, nl, starts);
+    if (use_smem)
+      ev_parse_smem_kernel<<<nblk(nl, EV_THREADS), EV_THREADS, EV_SMEM_BYTES, ex>>>(t, starts, nl, df, d_scratch, Ls);
+    else
+      ev_parse_kernel<<<nblk(nl, EV_THREADS), EV_THREADS, 0, ex>>>(t, starts, nl, df, d_scratch, Ls);
+    CK0(cudaGetLastError());
+    CK0(scan_exclusive_u32(Ls.is_match, Ls.match_pos, nls, ex, nullptr));
+    CK0(scan_exclusive_u32(Ls.is_fb, Ls.fb_pos, nls, ex, nullptr));
+    CK0(scan_exclusive_u32(Ls.eid_len, Ls.eid_pos, nls, ex, nullptr));
+    CK0(scan_exclusive_u32(Ls.tid_len, Ls.tid_pos, nls, ex, nullptr));
+    EvBase cb_{here.line, here.byte, base.eid, base.tid};
+    ev_compact_kernel<<<nblk(nl, EV_THREADS), EV_THREADS, 0, ex>>>(t, starts, nl, cb_, d_scratch, Ls, o);
+    ev_totals_kernel<<<1, 1, 0, ex>>>(Ls, nl, d_tot);
+    CK0(cudaGetLastError());
+    CK0(cudaEventRecord(k3, ex));
+    CK0(cudaMemcpyAsync(h_tot, d_tot, 4 * sizeof(uint32_t), cudaMemcpyDeviceToHost, ex));
+    // find and stage the next chunk while this one is parsed (oversized lines before it belong after this chunk's
+    // lines, so their line numbers are assigned only now that this chunk's line count is known)
+    int64_t nb, ne;
+    next_chunk(ce, &nb, &ne);
+    if (nb < ne && prefetch(slot ^ 1, nb, ne) != PIO_ALS_OK) return PIO_ALS_ERR_CUDA;
+    CK0(cudaStreamSynchronize(ex));
+    const int64_t nm = h_tot[0], nf = h_tot[1], eb = h_tot[2], tb = h_tot[3];
+    if (n_ev + nm > capacity) return fail(nullptr, PIO_ALS_ERR_ARG, "more matched events than capacity");
+    CK0(cudaEventRecord(d0, ex));
+    CK0(cudaMemcpyAsync(out_line + n_ev, o.line, 8 * nm, cudaMemcpyDeviceToHost, ex));
+    CK0(cudaMemcpyAsync(out_code + n_ev, o.code, 4 * nm, cudaMemcpyDeviceToHost, ex));
+    CK0(cudaMemcpyAsync(out_value + n_ev, o.value, 8 * nm, cudaMemcpyDeviceToHost, ex));
+    CK0(cudaMemcpyAsync(out_flags + n_ev, o.flags, nm, cudaMemcpyDeviceToHost, ex));
+    CK0(cudaMemcpyAsync(out_time_us + n_ev, o.time_us, 8 * nm, cudaMemcpyDeviceToHost, ex));
+    CK0(cudaMemcpyAsync(out_eid_off + n_ev, o.eid_off, 8 * nm, cudaMemcpyDeviceToHost, ex));
+    CK0(cudaMemcpyAsync(out_tid_off + n_ev, o.tid_off, 8 * nm, cudaMemcpyDeviceToHost, ex));
+    CK0(cudaMemcpyAsync(out_eid_bytes + base.eid, o.eid_bytes, eb, cudaMemcpyDeviceToHost, ex));
+    CK0(cudaMemcpyAsync(out_tid_bytes + base.tid, o.tid_bytes, tb, cudaMemcpyDeviceToHost, ex));
+    const int64_t room = fb_capacity - n_fb, nfc = nf < room ? nf : (room > 0 ? room : 0);
+    if (nfc > 0) {
+      CK0(cudaMemcpyAsync(out_fb_line + n_fb, o.fb_line, 8 * nfc, cudaMemcpyDeviceToHost, ex));
+      CK0(cudaMemcpyAsync(out_fb_begin + n_fb, o.fb_begin, 8 * nfc, cudaMemcpyDeviceToHost, ex));
+      CK0(cudaMemcpyAsync(out_fb_end + n_fb, o.fb_end, 8 * nfc, cudaMemcpyDeviceToHost, ex));
+    }
+    CK0(cudaEventRecord(d1, ex));
+    CK0(cudaStreamSynchronize(ex));
+    tm.h2d_ms += ms(h2d_begin[slot], copied[slot]);
+    tm.kernel_ms += ms(k0, k1) + ms(k2, k3);
+    tm.d2h_ms += ms(d0, d1);
+    ++tm.chunks;
+    n_ev += nm;
+    n_fb += nf;
+    base.eid += eb;
+    base.tid += tb;
+    flush_oversized();
+    cb = nb, ce = ne;
+  }
+  out_eid_off[n_ev] = base.eid;
+  out_tid_off[n_ev] = base.tid;
+  *out_n_events = n_ev;
+  *out_n_fallback = n_fb;
+  *out_n_lines = base.line;
+  return PIO_ALS_OK;
+}
+
+/* debug only (not in pio_als.h): out[0] host-to-device copy, out[1] kernels, out[2] device-to-host copy (device ms),
+ * out[3] host copy into pinned staging (wall ms), out[4] device chunks -- of the last pio_events_scan on this thread.
+ * Used by tools/events_bench.py. */
+__attribute__((visibility("default"))) int pio_events_debug_timing(double out[5]) {
+  if (!out) return PIO_ALS_ERR_ARG;
+  const EvTiming& t = g_ev_timing;
+  out[0] = t.h2d_ms, out[1] = t.kernel_ms, out[2] = t.d2h_ms, out[3] = t.stage_ms, out[4] = (double)t.chunks;
   return PIO_ALS_OK;
 }
 

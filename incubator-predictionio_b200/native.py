@@ -32,6 +32,7 @@ EXPORTED_SYMBOLS = [
     "pio_als_set_init", "pio_als_run", "pio_als_get_factors", "pio_als_train", "pio_als_recommend",
     "pio_als_similar", "pio_als_similar_batch", "pio_als_model_import", "pio_als_save", "pio_als_load", "pio_als_get_stats", "pio_als_get_phase_ms",
     "pio_als_synth_ratings_device", "pio_nb_train", "pio_nb_predict", "pio_ids_encode", "pio_cooc_train",
+    "pio_events_scan",
 ]
 
 
@@ -379,6 +380,77 @@ def ids_encode(strings, device=0):
     if rc != 0:
         raise NativeError(rc, lib().pio_als_last_error(None).decode())
     return idx, first[:nu.value]
+
+
+EVENTS_TARGET_ANY, EVENTS_TARGET_ABSENT, EVENTS_TARGET_EQUALS = 0, 1, 2
+EVENTS_MIN_EVENT_BYTES = 64
+EVENTS_HAS_VALUE, EVENTS_HAS_TARGET = 1, 2
+
+
+class EventsFilter(C.Structure):
+    _fields_ = [
+        ("entity_type", C.c_char_p), ("event_names", C.POINTER(C.c_char_p)), ("n_event_names", C.c_int32),
+        ("target_entity_type_mode", C.c_int32), ("target_entity_type", C.c_char_p), ("property", C.c_char_p),
+        ("has_start", C.c_int32), ("has_until", C.c_int32), ("start_us", C.c_int64), ("until_us", C.c_int64),
+    ]
+
+
+def events_scan(text, entity_type=None, event_names=None, target_mode=EVENTS_TARGET_ANY, target_entity_type=None,
+                prop=None, start_us=None, until_us=None, device=0):
+    """pio_events_scan over one buffer of complete JSON lines (bytes / uint8 array).  Returns a dict of numpy columns:
+    line, code, value, flags, time_us, eid_bytes/eid_off, tid_bytes/tid_off (matched events, line order), fb_line,
+    fb_begin, fb_end (lines the caller parses) and n_lines."""
+    buf = np.frombuffer(text, np.uint8) if isinstance(text, (bytes, bytearray, memoryview)) else \
+        np.ascontiguousarray(text, np.uint8)
+    n = int(buf.shape[0])
+    names = [] if event_names is None else [x.encode("utf-8") for x in event_names]
+    f = EventsFilter()
+    keep = (C.c_char_p * max(len(names), 1))(*names)
+    f.entity_type = None if entity_type is None else entity_type.encode("utf-8")
+    f.event_names = None if event_names is None else keep   # None: any name; []: no event matches (as in find)
+    f.n_event_names = len(names)
+    f.target_entity_type_mode = int(target_mode)
+    f.target_entity_type = None if target_entity_type is None else target_entity_type.encode("utf-8")
+    f.property = None if prop is None else prop.encode("utf-8")
+    f.has_start, f.start_us = (0, 0) if start_us is None else (1, int(start_us))
+    f.has_until, f.until_us = (0, 0) if until_us is None else (1, int(until_us))
+    cap = n // EVENTS_MIN_EVENT_BYTES + 1
+    out = dict(line=np.empty(cap, np.int64), code=np.empty(cap, np.int32), value=np.empty(cap, np.float64),
+               flags=np.empty(cap, np.uint8), time_us=np.empty(cap, np.int64), eid_bytes=np.empty(max(n, 1), np.uint8),
+               eid_off=np.empty(cap + 1, np.int64), tid_bytes=np.empty(max(n, 1), np.uint8),
+               tid_off=np.empty(cap + 1, np.int64))
+    fb_cap = max(1024, n // 4096)
+    n_ev, n_fb, n_lines = C.c_int64(0), C.c_int64(0), C.c_int64(0)
+    while True:
+        fb = [np.empty(fb_cap, np.int64) for _ in range(3)]
+        rc = lib().pio_events_scan(
+            C.c_int(device), _ptr(buf, C.c_uint8) if n else None, C.c_int64(n), C.byref(f), C.c_int64(cap),
+            *[_ptr(out[k], t) for k, t in (("line", C.c_int64), ("code", C.c_int32), ("value", C.c_double),
+                                           ("flags", C.c_uint8), ("time_us", C.c_int64), ("eid_bytes", C.c_uint8),
+                                           ("eid_off", C.c_int64), ("tid_bytes", C.c_uint8), ("tid_off", C.c_int64))],
+            C.byref(n_ev), C.c_int64(fb_cap), *[_ptr(a, C.c_int64) for a in fb], C.byref(n_fb), C.byref(n_lines))
+        if rc != 0:
+            raise NativeError(rc, lib().pio_als_last_error(None).decode())
+        if n_fb.value <= fb_cap:
+            break
+        fb_cap = n_fb.value     # more fallback lines than room: once more with room for all of them
+    m = n_ev.value
+    res = {k: out[k][:m] for k in ("line", "code", "value", "flags", "time_us")}
+    res["eid_off"], res["tid_off"] = out["eid_off"][:m + 1], out["tid_off"][:m + 1]
+    res["eid_bytes"], res["tid_bytes"] = out["eid_bytes"][:res["eid_off"][-1]], out["tid_bytes"][:res["tid_off"][-1]]
+    res["fb_line"], res["fb_begin"], res["fb_end"] = (a[:n_fb.value] for a in fb)
+    res["n_lines"] = n_lines.value
+    return res
+
+
+def events_scan_timing() -> dict:
+    """Where the last events_scan on this thread spent its time (milliseconds, summed over its device chunks):
+    host-to-device copy, kernels, device-to-host copy (CUDA events), and the host copy into pinned staging."""
+    out = (C.c_double * 5)()
+    rc = lib().pio_events_debug_timing(out)
+    if rc != 0:
+        raise NativeError(rc, "pio_events_debug_timing")
+    return {"h2d_ms": out[0], "kernel_ms": out[1], "d2h_ms": out[2], "stage_ms": out[3], "chunks": int(out[4])}
 
 
 def cooc_train(user, item, n_users, n_items, topn, device=0):

@@ -10,8 +10,10 @@ Mirrors (reference paths relative to the repository root):
 The storage *engine* (JDBC/HBase/ES backends, Event Server) is out of scope (SURVEY 8 / section 2 rows
 11-15): events live in one JSON-lines file per app in the `pio import` / `pio export` format
 (tools/src/main/scala/org/apache/predictionio/tools/imprt/FileToEvents.scala:93-103) under
-$PIO_EVENTDATA_DIR (default ./pio_eventdata).  `find` returns a list of Event (the RDD stand-in)
-or, for the bulk path, numpy column arrays.
+$PIO_EVENTDATA_DIR (default ./pio_eventdata).  `find` returns a list of Event (the RDD stand-in).
+`findColumns` is the bulk path: the same events as numpy columns (`EventColumns`), scanned on the GPU
+(`native.events_scan`, DESIGN.md 3.1); the lines the device scanner does not accept are parsed here by the
+code `find` uses and merged in file order.
 """
 from __future__ import annotations
 
@@ -397,6 +399,15 @@ class PEventStore:
         return out
 
     @staticmethod
+    def findColumns(appName: str, entityType: Optional[str] = None, eventNames: Optional[Sequence[str]] = None,
+                    targetEntityType=_UNSET, property: Optional[str] = None, startTime=None, untilTime=None,
+                    channelName: Optional[str] = None, sc=None, chunk_bytes: int = None) -> "EventColumns":
+        """The events `find` returns for the same filter, as columns (EventColumns), scanned on the GPU with the
+        numeric `property` extracted.  Raises what `find` raises on the first bad line.  Needs the CUDA library."""
+        return _find_columns(appName, entityType, eventNames, targetEntityType, property, startTime, untilTime,
+                             channelName, sc, chunk_bytes or FIND_COLUMNS_CHUNK)
+
+    @staticmethod
     def aggregateProperties(appName: str, entityType: str, channelName: Optional[str] = None, startTime=None,
                             untilTime=None, required: Optional[Sequence[str]] = None, sc=None
                             ) -> List[Tuple[str, PropertyMap]]:
@@ -408,6 +419,183 @@ class PEventStore:
                 continue
             out.append((k, pm))
         return out
+
+
+_EPOCH = _dt.datetime(1970, 1, 1, tzinfo=_dt.timezone.utc)
+_ONE_US = _dt.timedelta(microseconds=1)
+
+
+def time_us(t: _dt.datetime) -> int:
+    """An aware datetime as integer microseconds since the epoch."""
+    return (t - _EPOCH) // _ONE_US
+
+
+def take_strings(buf: np.ndarray, off: np.ndarray, idx) -> Tuple[np.ndarray, np.ndarray]:
+    """Rows `idx` of a (bytes, offsets[n + 1]) string column, as a new column."""
+    idx = np.asarray(idx, np.int64)
+    lens = (off[1:] - off[:-1])[idx]
+    new_off = np.zeros(idx.shape[0] + 1, np.int64)
+    np.cumsum(lens, out=new_off[1:])
+    row = np.repeat(np.arange(idx.shape[0]), lens)
+    src = off[:-1][idx][row] + (np.arange(new_off[-1], dtype=np.int64) - new_off[:-1][row])
+    return buf[src], new_off
+
+
+def concat_strings(cols: Sequence[Tuple[np.ndarray, np.ndarray]]) -> Tuple[np.ndarray, np.ndarray]:
+    bufs = [b for b, _ in cols]
+    offs, base = [np.zeros(1, np.int64)], 0
+    for b, o in cols:
+        offs.append(o[1:] + base)
+        base += int(o[-1])
+    return (np.concatenate(bufs) if bufs else np.zeros(0, np.uint8)), np.concatenate(offs)
+
+
+def string_list(col: Tuple[np.ndarray, np.ndarray]) -> List[str]:
+    """The strings of a column (ids of lone surrogates come back as they went in: `surrogatepass`)."""
+    buf, off = col
+    raw = buf.tobytes()
+    return [raw[off[k]:off[k + 1]].decode("utf-8", "surrogatepass") for k in range(off.shape[0] - 1)]
+
+
+@dataclass
+class EventColumns:
+    """The matched events of PEventStore.findColumns, in file order, as columns.  `entityId` / `targetEntityId` are
+    (UTF-8 bytes uint8[], offsets int64[n + 1]) pairs, the input `native.ids_encode` takes; a targetEntityId that is
+    absent is an empty string with has_target False.  `value` is float(property) where has_value; `bad_value` maps the
+    event number of a property that is present but null or not convertible by float() to its raw value, so that a
+    caller reading it raises exactly what DataMap.get(name, float) raises."""
+    code: np.ndarray             # int32: index of the event name in eventNames (-1 when eventNames is None)
+    value: np.ndarray            # float64
+    has_value: np.ndarray        # bool
+    time_us: np.ndarray          # int64, microseconds since 1970-01-01T00:00:00Z
+    entityId: Tuple[np.ndarray, np.ndarray]
+    targetEntityId: Tuple[np.ndarray, np.ndarray]
+    has_target: np.ndarray       # bool
+    bad_value: Dict[int, Any] = field(default_factory=dict)
+    n_fallback: int = 0          # lines parsed on the host
+
+    def __len__(self) -> int:
+        return int(self.code.shape[0])
+
+    def take(self, idx) -> "EventColumns":
+        """The events `idx` (ascending event numbers keep file order)."""
+        idx = np.asarray(idx, np.int64)
+        pos = {int(k): j for j, k in enumerate(idx)} if self.bad_value else {}
+        return EventColumns(self.code[idx], self.value[idx], self.has_value[idx], self.time_us[idx],
+                            take_strings(*self.entityId, idx), take_strings(*self.targetEntityId, idx),
+                            self.has_target[idx], {pos[k]: v for k, v in self.bad_value.items() if k in pos},
+                            self.n_fallback)
+
+
+def _host_columns(lines, names, appName, entityType, eventNames, targetEntityType, prop, startTime, untilTime):
+    """Fallback lines (line index, bytes): the code `find` runs, producing column entries."""
+    rows = []
+    for ln, raw in lines:
+        text = raw.decode("utf-8").strip()
+        if not text:
+            continue
+        e = Event.from_json(json.loads(text))
+        if startTime is not None and e.eventTime < _parse_time(startTime):
+            continue
+        if untilTime is not None and e.eventTime >= _parse_time(untilTime):
+            continue
+        if entityType is not None and e.entityType != entityType:
+            continue
+        if names is not None and e.event not in names:
+            continue
+        if targetEntityType is not _UNSET and e.targetEntityType != targetEntityType:
+            continue
+        has, v, bad = False, 0.0, _UNSET
+        if prop is not None and e.properties.contains(prop):
+            raw_v = e.properties.fields[prop]
+            try:
+                v, has = e.properties.get(prop, float), True
+            except Exception:
+                bad = raw_v
+        code = -1 if eventNames is None else list(eventNames).index(e.event)
+        rows.append((ln, code, v, has, time_us(e.eventTime), e.entityId, e.targetEntityId, bad))
+    return rows
+
+
+def _columns_from_rows(rows) -> Tuple[Dict[str, np.ndarray], Dict[int, Any]]:
+    enc = lambda s: s.encode("utf-8", "surrogatepass")  # noqa: E731
+    eids = [enc(r[5]) for r in rows]
+    tids = [b"" if r[6] is None else enc(r[6]) for r in rows]
+    col = dict(line=np.array([r[0] for r in rows], np.int64), code=np.array([r[1] for r in rows], np.int32),
+               value=np.array([r[2] for r in rows], np.float64), has_value=np.array([r[3] for r in rows], bool),
+               time_us=np.array([r[4] for r in rows], np.int64), has_target=np.array([r[6] is not None for r in rows], bool))
+    for key, ids in (("eid", eids), ("tid", tids)):
+        off = np.zeros(len(ids) + 1, np.int64)
+        np.cumsum([len(b) for b in ids], out=off[1:])
+        col[key] = (np.frombuffer(b"".join(ids), np.uint8).copy(), off)
+    return col, {j: r[7] for j, r in enumerate(rows) if r[7] is not _UNSET}
+
+
+FIND_COLUMNS_CHUNK = 256 << 20
+
+
+def _find_columns(appName, entityType=None, eventNames=None, targetEntityType=_UNSET, property=None, startTime=None,
+                  untilTime=None, channelName=None, sc=None, chunk_bytes=FIND_COLUMNS_CHUNK) -> EventColumns:
+    from . import native
+    p = app_file(appName, channelName)
+    if not p.exists():
+        raise FileNotFoundError(f"Invalid app name {appName}: no event data at {p}")  # Common.appNameToId
+    names = None if eventNames is None else set(eventNames)
+    if targetEntityType is _UNSET:
+        mode, tet = native.EVENTS_TARGET_ANY, None
+    elif targetEntityType is None:
+        mode, tet = native.EVENTS_TARGET_ABSENT, None
+    else:
+        mode, tet = native.EVENTS_TARGET_EQUALS, targetEntityType
+    s_us = None if startTime is None else time_us(_parse_time(startTime))
+    u_us = None if untilTime is None else time_us(_parse_time(untilTime))
+    device = getattr(sc, "device", 0) or 0
+    parts, host_lines, line_base = [], [], 0
+    with open(p, "rb") as fh:
+        carry = b""
+        while True:
+            data = fh.read(chunk_bytes)
+            buf = carry + data                    # no copy while the carry is empty
+            cut = len(buf)
+            if data:
+                cut = buf.rfind(b"\n") + 1        # complete lines only; a chunk without "\n" grows
+                if cut == 0:
+                    carry = buf
+                    continue
+                carry = buf[cut:]
+            if cut:
+                view = memoryview(buf)[:cut]      # the scan reads the piece in place
+                r = native.events_scan(view, entityType, eventNames, mode, tet, property, s_us, u_us, device)
+                r["line"] += line_base
+                parts.append(r)
+                host_lines.extend((int(ln) + line_base, bytes(view[b:e])) for ln, b, e in
+                                  zip(r["fb_line"], r["fb_begin"], r["fb_end"]))
+                line_base += r["n_lines"]
+            if not data:
+                break
+    rows = _host_columns(host_lines, names, appName, entityType, eventNames, targetEntityType, property, startTime,
+                         untilTime)
+    dev = dict(line=np.concatenate([r["line"] for r in parts]) if parts else np.zeros(0, np.int64))
+    for k, t in (("code", np.int32), ("value", np.float64), ("time_us", np.int64)):
+        dev[k] = np.concatenate([r[k] for r in parts]).astype(t, copy=False) if parts else np.zeros(0, t)
+    flags = np.concatenate([r["flags"] for r in parts]) if parts else np.zeros(0, np.uint8)
+    dev["has_value"] = (flags & native.EVENTS_HAS_VALUE) != 0
+    dev["has_target"] = (flags & native.EVENTS_HAS_TARGET) != 0
+    dev["eid"] = concat_strings([(r["eid_bytes"], r["eid_off"]) for r in parts])
+    dev["tid"] = concat_strings([(r["tid_bytes"], r["tid_off"]) for r in parts])
+    if not rows:
+        return EventColumns(dev["code"], dev["value"], dev["has_value"], dev["time_us"], dev["eid"], dev["tid"],
+                            dev["has_target"])
+    host, bad = _columns_from_rows(rows)
+    nd = dev["line"].shape[0]
+    order = np.argsort(np.concatenate([dev["line"], host["line"]]), kind="stable")   # merge in line order
+    cat = {k: np.concatenate([dev[k], host[k]])[order] for k in ("code", "value", "has_value", "time_us", "has_target")}
+    eid = take_strings(*concat_strings([dev["eid"], host["eid"]]), order)
+    tid = take_strings(*concat_strings([dev["tid"], host["tid"]]), order)
+    where = np.empty(order.shape[0], np.int64)
+    where[order] = np.arange(order.shape[0])
+    return EventColumns(cat["code"], cat["value"], cat["has_value"], cat["time_us"], eid, tid, cat["has_target"],
+                        {int(where[nd + j]): v for j, v in bad.items()}, len(host_lines))
 
 
 class LEventStore:

@@ -10,14 +10,15 @@ import json
 import os
 from dataclasses import dataclass, field
 from pathlib import Path
-from typing import List, Optional, Set
+from typing import List, Optional, Set, Tuple
 
 import numpy as np
 
+from .. import native
 from ..controller import (Engine, EngineFactory, LServing, PAlgorithm, Params, PDataSource, PersistentModel,
                           PPreparator, SanityCheck)
 from ..mllib import ALS, MatrixFactorizationModel
-from ..storage import BiMap, PEventStore
+from ..storage import BiMap, DataMap, PEventStore, string_list, take_strings
 
 
 @dataclass
@@ -62,15 +63,50 @@ class DataSourceParams(Params):
     evalParams: Optional[DataSourceEvalParams] = None
 
 
+@dataclass
+class RatingColumns:
+    """The ratings as columns: user / item ids as (UTF-8 bytes, offsets[n + 1]) pairs, as native.ids_encode takes them;
+    has_item is False where the event had no targetEntityId (Rating.item None)."""
+    user: Tuple[np.ndarray, np.ndarray]
+    item: Tuple[np.ndarray, np.ndarray]
+    rating: np.ndarray        # float64
+    has_item: np.ndarray      # bool
+
+    def __len__(self) -> int:
+        return int(self.rating.shape[0])
+
+    def take(self, idx) -> "RatingColumns":
+        return RatingColumns(take_strings(*self.user, idx), take_strings(*self.item, idx), self.rating[idx],
+                             self.has_item[idx])
+
+    def to_ratings(self) -> List[Rating]:
+        items = string_list(self.item)
+        return [Rating(u, it if h else None, v) for u, it, h, v in
+                zip(string_list(self.user), items, self.has_item.tolist(), self.rating.tolist())]
+
+
 class TrainingData(SanityCheck):
-    def __init__(self, ratings: List[Rating]):
-        self.ratings = ratings
+    """Ratings as a list of Rating, or as RatingColumns (the list is then built on first use of `.ratings`)."""
+
+    def __init__(self, ratings: Optional[List[Rating]] = None, columns: Optional[RatingColumns] = None):
+        self._ratings = ratings
+        self.columns = columns
+
+    @property
+    def ratings(self) -> List[Rating]:
+        if self._ratings is None:
+            self._ratings = self.columns.to_ratings()
+        return self._ratings
+
+    def __len__(self) -> int:
+        return len(self.columns) if self._ratings is None else len(self._ratings)
 
     def sanityCheck(self):
         pass
 
     def __repr__(self):
-        return f"ratings: [{len(self.ratings)}] ({self.ratings[:2]}...)"
+        head = self.columns.take(np.arange(min(2, len(self)))).to_ratings() if self._ratings is None else self._ratings[:2]
+        return f"ratings: [{len(self)}] ({head}...)"
 
 
 PreparedData = TrainingData
@@ -80,42 +116,44 @@ class DataSource(PDataSource):
     def __init__(self, dsp: DataSourceParams):
         self.dsp = dsp
 
+    def getRatingColumns(self, sc) -> RatingColumns:
+        """The rate and buy events as RatingColumns, scanned on the GPU (PEventStore.findColumns)."""
+        cols = PEventStore.findColumns(appName=self.dsp.appName, entityType="user", eventNames=["rate", "buy"],
+                                       targetEntityType="item", property="rating", sc=sc)
+        is_rate = cols.code == 0
+        unusable = np.flatnonzero(is_rate & ~cols.has_value)
+        if unusable.size:   # the first rate event without a usable rating raises what e.properties.get(...) raises
+            k = int(unusable[0])
+            DataMap({"rating": cols.bad_value[k]} if k in cols.bad_value else {}).get("rating", float)
+        value = np.where(is_rate, cols.value, 4.0)  # map buy event to rating value of 4
+        return RatingColumns(cols.entityId, cols.targetEntityId, value, cols.has_target)
+
     def getRatings(self, sc) -> List[Rating]:
-        events = PEventStore.find(appName=self.dsp.appName, entityType="user", eventNames=["rate", "buy"],
-                                  targetEntityType="item", sc=sc)
-        out = []
-        for e in events:
-            if e.event == "rate":
-                v = e.properties.get("rating", float)
-            elif e.event == "buy":
-                v = 4.0  # map buy event to rating value of 4
-            else:
-                raise Exception(f"Unexpected event {e} is read.")
-            out.append(Rating(e.entityId, e.targetEntityId, v))
-        return out
+        return self.getRatingColumns(sc).to_ratings()
 
     def readTraining(self, sc) -> TrainingData:
-        return TrainingData(self.getRatings(sc))
+        return TrainingData(columns=self.getRatingColumns(sc))
 
     def readEval(self, sc):
         assert self.dsp.evalParams is not None, "Must specify evalParams"
         ep = self.dsp.evalParams
-        ratings = list(enumerate(self.getRatings(sc)))  # zipWithUniqueId
+        cols = self.getRatingColumns(sc)
+        fold_of = np.arange(len(cols)) % ep.kFold  # zipWithUniqueId, then i % kFold
         folds = []
         for idx in range(ep.kFold):
-            train = [r for i, r in ratings if i % ep.kFold != idx]
-            test = [r for i, r in ratings if i % ep.kFold == idx]
+            train = cols.take(np.flatnonzero(fold_of != idx))
+            test = cols.take(np.flatnonzero(fold_of == idx)).to_ratings()
             by_user = {}
             for r in test:
                 by_user.setdefault(r.user, []).append(r)
-            folds.append((TrainingData(train), None,
+            folds.append((TrainingData(columns=train), None,
                           [(Query(u, ep.queryNum, set()), ActualResult(rs)) for u, rs in by_user.items()]))
         return folds
 
 
 class Preparator(PPreparator):
     def prepare(self, sc, trainingData: TrainingData) -> PreparedData:
-        return PreparedData(trainingData.ratings)
+        return PreparedData(trainingData._ratings, trainingData.columns)
 
 
 @dataclass
@@ -170,15 +208,26 @@ class ALSAlgorithm(PAlgorithm):
 
     def train(self, sc, data: PreparedData) -> ALSModel:
         # MLLib ALS cannot handle empty training data (ALSAlgorithm.scala:54-57)
-        if not data.ratings:
+        if not len(data):
             raise ValueError("requirement failed: RDD[Rating] in PreparedData cannot be empty. Please check if "
                              "DataSource generates TrainingData and Preparator generates PreparedData correctly.")
-        userStringIntMap = BiMap.stringInt(r.user for r in data.ratings)
-        itemStringIntMap = BiMap.stringInt(r.item for r in data.ratings)
-        n = len(data.ratings)
-        u = np.fromiter((userStringIntMap(r.user) for r in data.ratings), np.int32, n)
-        i = np.fromiter((itemStringIntMap(r.item) for r in data.ratings), np.int32, n)
-        v = np.fromiter((r.rating for r in data.ratings), np.float32, n)
+        cols = data.columns
+        if cols is not None and data._ratings is None and cols.has_item.all():
+            # BiMap.stringInt on the GPU: indices in first-occurrence order, the maps built from the distinct ids only
+            dev = getattr(sc, "device", 0) or 0
+            u, ufirst = native.ids_encode(cols.user, dev)
+            i, ifirst = native.ids_encode(cols.item, dev)
+            userStringIntMap = BiMap({s: k for k, s in enumerate(string_list(take_strings(*cols.user, ufirst)))})
+            itemStringIntMap = BiMap({s: k for k, s in enumerate(string_list(take_strings(*cols.item, ifirst)))})
+            v = cols.rating.astype(np.float32)
+            n = len(cols)
+        else:
+            userStringIntMap = BiMap.stringInt(r.user for r in data.ratings)
+            itemStringIntMap = BiMap.stringInt(r.item for r in data.ratings)
+            n = len(data.ratings)
+            u = np.fromiter((userStringIntMap(r.user) for r in data.ratings), np.int32, n)
+            i = np.fromiter((itemStringIntMap(r.item) for r in data.ratings), np.int32, n)
+            v = np.fromiter((r.rating for r in data.ratings), np.float32, n)
         seed = sc.agree_seed(self.ap.seed) if hasattr(sc, "agree_seed") else (self.ap.seed or 0)
         als = ALS()
         als.setUserBlocks(-1).setProductBlocks(-1).setRank(self.ap.rank).setIterations(self.ap.numIterations)
