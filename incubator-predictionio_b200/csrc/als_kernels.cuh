@@ -45,6 +45,9 @@ struct SolveParams {
   int row_begin;         // local rows [row_begin, row_end) are covered by this launch
   int row_end;
   int dst_row_offset;    // internal id of local row 0
+  // pair kernel (rank 33..64): [0] max |src| (abs_max_kernel, every half-step), [1] max |rating| (ingest), as float
+  // bits -- together they fix the power-of-two scale of its FP16 split
+  const unsigned* absmax;
   // optional work list (parts of very long rows): item i covers ratings [wl_beg[i], wl_end[i]); its Gramian
   // blocks and right-hand side go to partial[i * (SLOT + KP)] instead of being solved in this kernel
   const long long* wl_beg;

@@ -1,25 +1,28 @@
 // als_pair_kernel.cuh -- rank 33..64 half-step, second generation: every warp is an independent worker that
 // accumulates the Gramians of TWO destination rows one after the other on the warp-level tensor-core path (mma.sync
-// m16n8k8 TF32, three passes hi*hi + lo*hi + hi*lo = fp32-class products) and then solves both normal equations at once
-// with the lockstep Cholesky of als_lockstep.cuh (16 lanes per matrix).
+// m16n8k16 FP16 with fp32 accumulation, three passes hi*hi + lo*hi + hi*lo of a scaled hi/lo split = fp32-class
+// products) and then solves both normal equations at once with the lockstep Cholesky of als_lockstep.cuh (16 lanes
+// per matrix).
 //
 // Differences to the round-1 kernel (als_mma_kernel.cuh: four warps per CTA, one row each):
-//   * no CTA-wide barrier: a warp stages its own eight gathered rows per chunk (cp.async, 3-deep ring, 72-float row
-//     stride so that the fragment LDS.32 are conflict-free) and synchronises with __syncwarp only; warps of unrelated
-//     rows no longer wait for each other;
-//   * the right-hand side is accumulated from the fragment registers (16 FMA per chunk, quad-reduced once per row)
-//     instead of a second pass over the staged rows (24 LDS + 16 FMA per chunk);
+//   * no CTA-wide barrier: a warp stages its own eight gathered rows per chunk (cp.async, 4-deep ring, 64-float rows
+//     with the features XOR-swizzled so that the fragment LDS.32 are conflict-free) and synchronises with __syncwarp
+//     only; warps of unrelated rows no longer wait for each other;
+//   * the right-hand side is accumulated from the fragment registers (16 FMA per 8 ratings, quad-reduced once per
+//     row) instead of a second pass over the staged rows (24 LDS + 16 FMA per chunk);
 //   * the solve costs ~1.8 k instead of ~6.4 k warp instructions per row and its 64-step pivot chain is shared by
 //     the two matrices;
 //   * work-list mode: an item may be a PART of a long row; its partial normal equation goes to global memory in the
 //     slot layout and als_finish_pair_kernel adds the parts of a row in fixed order and solves.  Cutting rows above
 //     1024 ratings into 512-rating parts is a two-level summation: the per-chunk round-to-nearest accumulation stays
 //     short, which keeps the kernel inside the 1e-4 parity bound on rows of thousands of ratings (round 1: 1.1e-4).
-// Per-row arithmetic depends on the row alone (sharded runs stay bit-identical).
+// Per-row arithmetic depends on the row and on the half-step's scale exponent alone (sharded runs stay bit-identical:
+// every rank derives the exponent from the same replicated source matrix and the same global rating maximum).
 //
 // Replaces, per destination row: NormalEquation.add + CholeskySolver.solve of Spark 2.4 ml.recommendation.ALS
 // (SURVEY.md section 8(c) items 5-6), reached from examples/scala-parallel-recommendation/.../ALSAlgorithm.scala:76-86.
 #pragma once
+#include <cuda_fp16.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
 
@@ -30,9 +33,9 @@ namespace pio {
 namespace pr {
 
 constexpr int KP = 64;
-constexpr int CH = 8;                     // ratings per chunk = K of one mma
-constexpr int RSTR = 72;                  // floats per staged source row (64 + 8 pad)
-constexpr int NSTAGE = 3;
+constexpr int CH = 8;                     // ratings per staged chunk (one cp.async stage); a loop step takes two = K 16
+constexpr int RSTR = KP;                  // floats per staged source row (features XOR-swizzled by 8 * row)
+constexpr int NSTAGE = 4;                 // two stages consumed per step, two in flight
 constexpr int STAGE = CH * RSTR;          // floats per stage
 constexpr int NTILE = 20;                 // 16x8 accumulator tiles covering the lower triangle of 64x64
 using LL = LsLayout<KP>;
@@ -40,6 +43,7 @@ constexpr int SLOT_STRIDE = LL::STRIDE;   // 2096 floats: the second matrix star
 constexpr int VSTR = 80;                  // per-matrix stride of the small vectors (== 16 mod 32)
 constexpr int PART_FLOATS = LL::SIZE + KP;   // one partial normal equation in global memory: slot + right-hand side
 static_assert(NSTAGE * STAGE <= SLOT_STRIDE, "the staging ring lives in the second slot");
+static_assert(NSTAGE % 2 == 0, "a loop step consumes two stages");
 // per-warp shared memory (floats): two slots (the ring aliases slot 1), b vectors, pivot lines, rating ring
 constexpr int W_BVEC = 2 * SLOT_STRIDE;
 constexpr int W_COL = W_BVEC + 2 * VSTR;
@@ -47,73 +51,108 @@ constexpr int W_MVAL = W_COL + 2 * VSTR;
 constexpr int W_FLOATS = W_MVAL + NSTAGE * CH + 8;
 constexpr size_t smem_bytes(int warps) { return sizeof(float) * (size_t)W_FLOATS * warps; }
 
-__device__ __forceinline__ void mma_tf32(float (&d)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
-  asm volatile(
-      "mma.sync.aligned.m16n8k8.row.col.f32.tf32.tf32.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};\n"
-      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
-      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
+// The FP16 split needs every value below the f16 range: the values X sqrt(c1) (implicit) or X (explicit) of a
+// half-step are multiplied by s = 2^e, with e chosen so that max |X sqrt(c1)| s < 2^15.  hi = f16(v) is then finite
+// and lo = f16(v - hi) stays a normal f16 down to max / 2^18 (below that its absolute error is under 2^-25 of the
+// largest value).  e is clamped so that 2^-2e, which takes the scale out of the accumulators, is a normal float; an
+// all-zero source gives e = 0.
+__device__ __forceinline__ int split_exponent(float vmax) {
+  if (!(vmax > 0.f)) return 0;
+  if (isinf(vmax)) return -63;
+  int x;
+  frexpf(vmax, &x);                       // vmax < 2^x
+  const int e = 15 - x;
+  return e < -63 ? -63 : e > 63 ? 63 : e;
+}
+__device__ __forceinline__ float pow2f(int e) { return __int_as_float((127 + e) << 23); }   // -126 <= e <= 127
+
+// max |x[0 .. n)| as float bits, atomicMax-ed into *out (which the caller zeroes): the bound of the FP16 split scale
+// (source factors, every half-step) and the rating maximum (once per ingest).  NaNs are ignored.
+__global__ void __launch_bounds__(256) abs_max_kernel(const float* __restrict__ x, long long n, unsigned* out) {
+  float m = 0.f;
+  const long long stride = (long long)gridDim.x * blockDim.x;
+  const long long i0 = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  long long tail = 0;
+  if ((reinterpret_cast<uintptr_t>(x) & 15) == 0) {
+    const long long n4 = n >> 2;
+    for (long long i = i0; i < n4; i += stride) {
+      const float4 v = __ldg(reinterpret_cast<const float4*>(x) + i);
+      m = fmaxf(m, fmaxf(fmaxf(fabsf(v.x), fabsf(v.y)), fmaxf(fabsf(v.z), fabsf(v.w))));
+    }
+    tail = 4 * n4;
+  }
+  for (long long i = tail + i0; i < n; i += stride) m = fmaxf(m, fabsf(__ldg(x + i)));
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
+  if ((threadIdx.x & 31) == 0) atomicMax(out, __float_as_uint(m));   // non-negative floats order like their bits
 }
 
-// First mma of a chain: C = 0 as an immediate (no registers to clear)
-__device__ __forceinline__ void mma_tf32_z(float (&d)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
-  asm volatile(
-      "mma.sync.aligned.m16n8k8.row.col.f32.tf32.tf32.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%10,%10,%10,%10};\n"
-      : "=f"(d[0]), "=f"(d[1]), "=f"(d[2]), "=f"(d[3])
-      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1), "f"(0.f));
-}
-
-// B fragment as one 64-bit register pair
+// D (+)= A B, m16n8k16, f16 inputs, f32 accumulation.  The B fragment is one 64-bit register pair.
 __device__ __forceinline__ uint64_t pack2(uint32_t x, uint32_t y) {
   uint64_t r;
   asm("mov.b64 %0, {%1, %2};" : "=l"(r) : "r"(x), "r"(y));
   return r;
 }
-__device__ __forceinline__ void mma_tf32_p(float (&d)[4], const uint32_t (&a)[4], uint64_t b) {
+__device__ __forceinline__ void mma_f16_p(float (&d)[4], const uint32_t (&a)[4], uint64_t b) {
   asm volatile(
       "{\n .reg .b32 b0, b1;\n mov.b64 {b0, b1}, %8;\n"
-      "mma.sync.aligned.m16n8k8.row.col.f32.tf32.tf32.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {b0,b1}, {%0,%1,%2,%3};\n}\n"
+      "mma.sync.aligned.m16n8k16.row.col.f32.f16.f16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {b0,b1}, {%0,%1,%2,%3};\n}\n"
       : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
       : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b));
 }
-__device__ __forceinline__ void mma_tf32_zp(float (&d)[4], const uint32_t (&a)[4], uint64_t b) {
+// First mma of a chain: C = 0 as an immediate (no registers to clear)
+__device__ __forceinline__ void mma_f16_zp(float (&d)[4], const uint32_t (&a)[4], uint64_t b) {
   asm volatile(
       "{\n .reg .b32 b0, b1;\n mov.b64 {b0, b1}, %4;\n"
-      "mma.sync.aligned.m16n8k8.row.col.f32.tf32.tf32.f32 {%0,%1,%2,%3}, {%5,%6,%7,%8}, {b0,b1}, {%9,%9,%9,%9};\n}\n"
+      "mma.sync.aligned.m16n8k16.row.col.f32.f16.f16.f32 {%0,%1,%2,%3}, {%5,%6,%7,%8}, {b0,b1}, {%9,%9,%9,%9};\n}\n"
       : "=f"(d[0]), "=f"(d[1]), "=f"(d[2]), "=f"(d[3])
       : "l"(b), "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "f"(0.f));
 }
 
+// hi/lo split of the pair (a, b) (k, k + 1 of one fragment register): hi = f16(a), f16(b); lo = f16 of the exact
+// fp32 remainders.  The intrinsics keep the compiler from contracting the scale multiply into the subtraction.
+__device__ __forceinline__ void split2(float a, float b, uint32_t& hi, uint32_t& lo) {
+  const __half2 h = __floats2half2_rn(a, b);          // .x (low 16 bits) = a
+  const float2 hf = __half22float2(h);
+  const __half2 l = __floats2half2_rn(__fsub_rn(a, hf.x), __fsub_rn(b, hf.y));
+  hi = *reinterpret_cast<const uint32_t*>(&h);
+  lo = *reinterpret_cast<const uint32_t*>(&l);
+}
+
 // Accumulates sum c1 y y^T (lower triangle, slot layout) and b of ratings [beg, end) into `slot` / `bv`.
 template <bool IMPLICIT>
-__device__ __forceinline__ void accumulate_row(const SolveParams& p, long long beg, long long end, float* ring,
-                                               float* mval, float* slot, float* bv) {
+__device__ __forceinline__ void accumulate_row(const SolveParams& p, long long beg, long long end, float s, float unscale,
+                                               float* ring, float* mval, float* slot, float* bv) {
   const int lane = threadIdx.x & 31;
   const int g = lane >> 2, t = lane & 3;
-  const int nchunks = (int)((end - beg + CH - 1) / CH);
+  const int nchunks = 2 * (int)((end - beg + 2 * CH - 1) / (2 * CH));   // whole steps; the last chunk may be all zero
   const int prow = lane >> 4, psl = lane & 15;     // staging: piece j of this lane = (staged row 2 j + prow, 16-byte slot psl)
 
-  int nidx[4];
+  // metadata of the two chunks of a step: lane l holds the index of rating l & 15 and (l < 16) its value
+  int nidx;
   float nval;
-  auto prefetch_meta = [&](int c) {
-    const long long e0 = beg + (long long)c * CH;
-#pragma unroll
-    for (int j = 0; j < 4; ++j) {
-      const long long e = e0 + 2 * j + prow;
-      nidx[j] = (c < nchunks && e < end) ? __ldg(p.idx + e) : -1;
-    }
-    nval = 0.f;
-    if (lane < CH && c < nchunks && e0 + lane < end) nval = __ldg(p.val + e0 + lane);
+  auto prefetch_meta = [&](int c) {   // c even
+    const long long e = beg + (long long)c * CH + (lane & 15);
+    nidx = (c < nchunks && e < end) ? __ldg(p.idx + e) : -1;
+    nval = (lane < 2 * CH && c < nchunks && e < end) ? __ldg(p.val + e) : 0.f;
   };
-  auto issue = [&](int c) {   // uses the metadata prefetched for chunk c; rows past the end are zero-filled
+  // staged row r holds feature f at r * RSTR + (f ^ 8 r): 16-byte pieces stay whole, and the fragment loads of rows
+  // t and t + 4 at features 16 i + g (+ 8) hit 32 different banks
+  auto issue = [&](int c) {   // chunks c, c + 1 from the metadata prefetched for them; rows past the end are zero-filled
     if (c < nchunks) {
-      float* sbuf = ring + (c % NSTAGE) * STAGE;
 #pragma unroll
-      for (int j = 0; j < 4; ++j) {
-        float4* d4 = reinterpret_cast<float4*>(sbuf + (2 * j + prow) * RSTR + psl * 4);
-        if (nidx[j] >= 0) cp_async16(d4, p.src + (size_t)nidx[j] * KP + psl * 4);
-        else *d4 = make_float4(0.f, 0.f, 0.f, 0.f);
+      for (int h = 0; h < 2; ++h) {
+        float* sbuf = ring + ((c + h) % NSTAGE) * STAGE;
+#pragma unroll
+        for (int j = 0; j < 4; ++j) {
+          const int r = 2 * j + prow;
+          const int src = __shfl_sync(0xffffffffu, nidx, CH * h + r);
+          float4* d4 = reinterpret_cast<float4*>(sbuf + r * RSTR + ((psl * 4) ^ (8 * r)));
+          if (src >= 0) cp_async16(d4, p.src + (size_t)src * KP + psl * 4);
+          else *d4 = make_float4(0.f, 0.f, 0.f, 0.f);
+        }
       }
-      if (lane < CH) mval[(c % NSTAGE) * CH + lane] = nval;
+      if (lane < 2 * CH) mval[(c % NSTAGE) * CH + lane] = nval;
     }
     cp_async_commit();
   };
@@ -127,61 +166,61 @@ __device__ __forceinline__ void accumulate_row(const SolveParams& p, long long b
 #pragma unroll
   for (int i = 0; i < 4; ++i) pb[i][0] = pb[i][1] = 0.f;
 
+  // the fragment columns of this lane: feature 16 i + 8 e + g of staged row t sits at column g + xo[(2 i + e) & 3] +
+  // 32 ((2 i + e) >> 2), of staged row t + 4 at column g + xo[(2 i + e) & 3] + 32 (1 - ((2 i + e) >> 2))
+  int xo[4];
+#pragma unroll
+  for (int q = 0; q < 4; ++q) xo[q] = g + 8 * (q ^ t);
+
   prefetch_meta(0);
   issue(0);
-  prefetch_meta(1);
-  issue(1);
   prefetch_meta(2);
 
 #pragma unroll 1
-  for (int c = 0; c < nchunks; ++c) {
-    cp_async_wait<1>();
+  for (int c = 0; c < nchunks; c += 2) {
+    cp_async_wait<0>();
     __syncwarp();
     issue(c + 2);
-    prefetch_meta(c + 3);
-    const float* X = ring + (c % NSTAGE) * STAGE;
+    prefetch_meta(c + 4);
+    const float* XA = ring + (c % NSTAGE) * STAGE + t * RSTR;   // stage A = chunk c (k 0..7), row t
+    const float* XB = XA + STAGE;                                // stage B = chunk c + 1 (k 8..15)
     const float* mv = mval + (c % NSTAGE) * CH;
-    const float r0 = mv[t], r1 = mv[t + 4];
-    float sc0 = 1.f, sc1 = 1.f, wb0 = r0, wb1 = r1;
-    if (IMPLICIT) {
-      const float c0 = p.alpha * fabsf(r0), c1 = p.alpha * fabsf(r1);
-      sc0 = sqrtf(c0);
-      sc1 = sqrtf(c1);
-      wb0 = r0 > 0.f ? 1.f + c0 : 0.f;
-      wb1 = r1 > 0.f ? 1.f + c1 : 0.f;
+    float wb[4], sc[4];       // ratings t, t + 4 of stage A, then of stage B
+    {
+      const float r[4] = {mv[t], mv[t + 4], mv[CH + t], mv[CH + t + 4]};
+#pragma unroll
+      for (int q = 0; q < 4; ++q) {
+        wb[q] = r[q];
+        sc[q] = s;
+        if (IMPLICIT) {
+          const float c1 = p.alpha * fabsf(r[q]);
+          sc[q] = __fmul_rn(sqrtf(c1), s);
+          wb[q] = r[q] > 0.f ? 1.f + c1 : 0.f;
+        }
+      }
     }
-    // fragments: v[i][0..3] = X[t][16i+g], X[t][16i+8+g], X[t+4][16i+g], X[t+4][16i+8+g]: the same registers are the A
-    // fragment of m-tile i and the B fragments of n-tiles 2i, 2i+1
+    // f16x2 fragments of m-tile i: register 0 = feature 16i+g, 1 = 16i+8+g of stage A, 2 and 3 the same of stage B;
+    // each holds ratings (t, t + 4).  The same registers are the A fragment of m-tile i and, as pairs (0, 2) and
+    // (1, 3), the B fragments of n-tiles 2i and 2i+1.
     uint32_t hi[4][4], lo[4][4];
 #pragma unroll
     for (int i = 0; i < 4; ++i) {
-      float v[4];
-      v[0] = X[t * RSTR + 16 * i + g];
-      v[1] = X[t * RSTR + 16 * i + 8 + g];
-      v[2] = X[(t + 4) * RSTR + 16 * i + g];
-      v[3] = X[(t + 4) * RSTR + 16 * i + 8 + g];
-      pb[i][0] = fmaf(wb0, v[0], pb[i][0]);
-      pb[i][1] = fmaf(wb0, v[1], pb[i][1]);
-      pb[i][0] = fmaf(wb1, v[2], pb[i][0]);
-      pb[i][1] = fmaf(wb1, v[3], pb[i][1]);
-      if (IMPLICIT) {
-        v[0] *= sc0; v[1] *= sc0; v[2] *= sc1; v[3] *= sc1;
-      }
 #pragma unroll
-      for (int e = 0; e < 4; ++e) {
-        // Veltkamp split: h = the 11 leading bits of v rounded to nearest (exactly a TF32 value), v - h exact; three
-        // FMA-pipe instructions instead of the ALU sequence cvt.rna.tf32 expands to.  |v - h| <= 2^-11 |v|;
-        // the dropped lo*lo term is 2^-22.
-        // (intrinsics: the compiler must not contract c - (c - v) into FMAs, which would return v itself)
-        const float c = __fmul_rn(v[e], 8193.f);       // 2^13 + 1
-        const float h = __fsub_rn(c, __fsub_rn(c, v[e]));
-        hi[i][e] = __float_as_uint(h);
-        lo[i][e] = __float_as_uint(__fsub_rn(v[e], h));
+      for (int e = 0; e < 2; ++e) {
+        const int q = 2 * i + e;
+        const int c0 = xo[q & 3] + 32 * (q >> 2), c4 = 4 * RSTR + xo[q & 3] + 32 * (1 - (q >> 2));
+        const float a0 = XA[c0], a4 = XA[c4], b0 = XB[c0], b4 = XB[c4];
+        pb[i][e] = fmaf(wb[0], a0, pb[i][e]);
+        pb[i][e] = fmaf(wb[1], a4, pb[i][e]);
+        pb[i][e] = fmaf(wb[2], b0, pb[i][e]);
+        pb[i][e] = fmaf(wb[3], b4, pb[i][e]);
+        split2(__fmul_rn(a0, sc[0]), __fmul_rn(a4, sc[1]), hi[i][e], lo[i][e]);
+        split2(__fmul_rn(b0, sc[2]), __fmul_rn(b4, sc[3]), hi[i][e + 2], lo[i][e + 2]);
       }
     }
     // D(16i.., 8j..) += A_i B_j for the tiles on or below the diagonal: j <= 2i+1.  The tensor core adds with
-    // truncation: only the 8 products of one chunk are summed inside it (small terms first), the running sum over
-    // the chunks is a round-to-nearest FADD in registers.
+    // truncation: only the 16 products of one step are summed inside it (small terms first), the running sum over
+    // the steps is a round-to-nearest FADD in registers.
     // n-tile j outermost: its B fragments (two registers each, hi and lo) are formed once and serve every m-tile
     // i >= j/2 below it -- SASS wants the pair in adjacent registers, so each use of a fresh pair costs two MOVs.
 #pragma unroll
@@ -193,9 +232,9 @@ __device__ __forceinline__ void accumulate_row(const SolveParams& p, long long b
       for (int i = bi; i < 4; ++i) {
         const int tile = i * (i + 1) + j;               // tiles of m-tile i start at sum_{i' < i} (2 i' + 2) = i (i + 1)
         float d[4];
-        mma_tf32_zp(d, lo[i], bh);
-        mma_tf32_p(d, hi[i], bl);
-        mma_tf32_p(d, hi[i], bh);
+        mma_f16_zp(d, lo[i], bh);
+        mma_f16_p(d, hi[i], bl);
+        mma_f16_p(d, hi[i], bh);
         acc[tile][0] += d[0];
         acc[tile][1] += d[1];
         acc[tile][2] += d[2];
@@ -216,7 +255,7 @@ __device__ __forceinline__ void accumulate_row(const SolveParams& p, long long b
       v += __shfl_xor_sync(0xffffffffu, v, 2);
       if (t == 0) bv[16 * i + 8 * e + g] = v;
     }
-  // ---- accumulators -> slot layout ----------------------------------------------------------------------------------------
+  // ---- accumulators -> slot layout, the scale s^2 taken out (exact: a power of two) ---------------------------------------
   {
     int tile = 0;
 #pragma unroll
@@ -225,16 +264,18 @@ __device__ __forceinline__ void accumulate_row(const SolveParams& p, long long b
       for (int j = 0; j <= 2 * i + 1; ++j, ++tile) {
         const int cb = j >> 1;
         const int cc = 8 * (j & 1) + 2 * t;           // column inside the 16-wide block (even)
+        const float d0 = acc[tile][0] * unscale, d1 = acc[tile][1] * unscale;
+        const float d2 = acc[tile][2] * unscale, d3 = acc[tile][3] * unscale;
         if (cb < i) {
           // off-diagonal block: two 8-byte stores (rows g and g + 8 of the block)
-          *reinterpret_cast<float2*>(slot + LL::offd(i, cb, g, cc)) = make_float2(acc[tile][0], acc[tile][1]);
-          *reinterpret_cast<float2*>(slot + LL::offd(i, cb, g + 8, cc)) = make_float2(acc[tile][2], acc[tile][3]);
+          *reinterpret_cast<float2*>(slot + LL::offd(i, cb, g, cc)) = make_float2(d0, d1);
+          *reinterpret_cast<float2*>(slot + LL::offd(i, cb, g + 8, cc)) = make_float2(d2, d3);
         } else {
           // diagonal block: packed triangle, keep c <= r
-          if (cc <= g) slot[LL::diag(i, g, cc)] = acc[tile][0];
-          if (cc + 1 <= g) slot[LL::diag(i, g, cc + 1)] = acc[tile][1];
-          if (cc <= g + 8) slot[LL::diag(i, g + 8, cc)] = acc[tile][2];
-          if (cc + 1 <= g + 8) slot[LL::diag(i, g + 8, cc + 1)] = acc[tile][3];
+          if (cc <= g) slot[LL::diag(i, g, cc)] = d0;
+          if (cc + 1 <= g) slot[LL::diag(i, g, cc + 1)] = d1;
+          if (cc <= g + 8) slot[LL::diag(i, g + 8, cc)] = d2;
+          if (cc + 1 <= g + 8) slot[LL::diag(i, g + 8, cc + 1)] = d3;
         }
       }
     }
@@ -272,6 +313,9 @@ __global__ void __launch_bounds__(32 * WARPS, 12 / WARPS) als_solve_pair_kernel(
   const int lane = threadIdx.x & 31;
   const int grp = lane >> 4;
   const int npairs = (n_items + 1) >> 1;
+  const float c1_root_max = IMPLICIT ? sqrtf(p.alpha * __uint_as_float(__ldg(p.absmax + 1))) : 1.f;
+  const int e = split_exponent(__uint_as_float(__ldg(p.absmax)) * c1_root_max);
+  const float s = pow2f(e), unscale = pow2f(-2 * e);
 
 #pragma unroll 1
   for (int base = blockIdx.x * WARPS; base < npairs; base += gridDim.x * WARPS) {
@@ -298,7 +342,7 @@ __global__ void __launch_bounds__(32 * WARPS, 12 / WARPS) als_solve_pair_kernel(
           if (h) row1 = r;
           else row0 = r;
         }
-        accumulate_row<IMPLICIT>(p, beg, end, ring, mval, slot, bv);
+        accumulate_row<IMPLICIT>(p, beg, end, s, unscale, ring, mval, slot, bv);
         if (p.partial) {
           // part of a long row: emit the partial normal equation (slot layout + b); als_finish_pair_kernel sums and solves
           float* out = p.partial + (size_t)item * PART_FLOATS;

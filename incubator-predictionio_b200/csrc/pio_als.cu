@@ -15,6 +15,7 @@
 #include <string.h>
 
 #include <chrono>
+#include <algorithm>
 #include <deque>
 #include <exception>
 #include <map>
@@ -413,6 +414,8 @@ struct pio_als_handle {
   int gram_blocks = 0;
   int* d_fail = nullptr;
   int* d_counts = nullptr;
+  // pair kernel FP16 split scale: [0] max |source factors| of the current half-step, [1] max |rating| (ingest); float bits
+  unsigned* d_absmax = nullptr;
   long long* d_timing = nullptr;  // PIO_ALS_TC_TIMING=1: per-warp cycle counters of the last tensor-core launch
   float* d_dbg = nullptr;     // PIO_ALS_TC_DEBUG=1: A/b dump of the last tensor-core half-step
   size_t dbg_rows = 0;
@@ -843,20 +846,27 @@ static int ingest_device(pio_als_handle* h, const int* d_user, const int* d_item
     degree_kernel<<<nblk(n2, 256), 256, 0, st>>>(cu, ci, cr, n2, U.deg, I.deg, U.npos, I.npos);
     LAUNCHED(h);
   }
+  // max |rating| (sharded: over all ranks): bounds sqrt(c1) in the pair kernel's FP16 split scale
+  CK(h, cudaMemsetAsync(h->d_absmax + 1, 0, sizeof(unsigned), st));
+  if (n2 > 0) {
+    pr::abs_max_kernel<<<std::min(nblk(n2, 256), 4u * h->sm_count), 256, 0, st>>>(cr, n2, h->d_absmax + 1);
+    LAUNCHED(h);
+  }
   long long n2_global = n2;
   if (sharded) {
     NcclApi& nc = nccl_api();   // only multi-GPU jobs touch NCCL (a single-GPU process must not load libnccl at all)
     long long* d_n = nullptr;
     CK(h, tmp.alloc(&d_n, 1));
     CK(h, cudaMemcpyAsync(d_n, &n2, sizeof(long long), cudaMemcpyHostToDevice, st));
-    if (nc.GroupStart() != ncclSuccess) return fail(h, PIO_ALS_ERR_COMM, "ncclGroupStart failed");   // one launch for the five
+    if (nc.GroupStart() != ncclSuccess) return fail(h, PIO_ALS_ERR_COMM, "ncclGroupStart failed");   // one launch for the six
     for (Side* s : {&U, &I}) {
       if (nc.AllReduce(s->deg, s->deg, (size_t)s->n, ncclUint32, ncclSum, h->comm, st) != ncclSuccess ||
           nc.AllReduce(s->npos, s->npos, (size_t)s->n, ncclUint32, ncclSum, h->comm, st) != ncclSuccess)
         return fail(h, PIO_ALS_ERR_COMM, "ncclAllReduce (degrees) failed");
     }
-    if (nc.AllReduce(d_n, d_n, 1, ncclInt64, ncclSum, h->comm, st) != ncclSuccess)
-      return fail(h, PIO_ALS_ERR_COMM, "ncclAllReduce (nnz) failed");
+    if (nc.AllReduce(d_n, d_n, 1, ncclInt64, ncclSum, h->comm, st) != ncclSuccess ||
+        nc.AllReduce(h->d_absmax + 1, h->d_absmax + 1, 1, ncclUint32, ncclMax, h->comm, st) != ncclSuccess)
+      return fail(h, PIO_ALS_ERR_COMM, "ncclAllReduce (nnz, rating maximum) failed");
     if (nc.GroupEnd() != ncclSuccess) return fail(h, PIO_ALS_ERR_COMM, "ncclGroupEnd failed");
     CK(h, cudaMemcpyAsync(&n2_global, d_n, sizeof(long long), cudaMemcpyDeviceToHost, st));
     CK(h, cudaStreamSynchronize(st));
@@ -1066,6 +1076,7 @@ static int launch_solve_cfg(pio_als_handle* h, Side& dst, const Side& src) {
   p0.alpha = (float)h->cfg.alpha;
   p0.k = h->cfg.rank;
   p0.dst_row_offset = h->cfg.world_rank * dst.R;
+  p0.absmax = h->d_absmax;
   p0.wl_beg = nullptr;
   p0.wl_end = nullptr;
   p0.partial = nullptr;
@@ -1260,6 +1271,13 @@ static int half_step(pio_als_handle* h, Side& dst, const Side& src, bool more) {
     cudaEventRecord(e.a, st);
     h->pieces_done = false;
     if (h->gram_side == &dst) h->gram_side = nullptr;
+    if (dst.plan.kernel == SOLVE_PAIR) {
+      // max |source factors| over the full replica (the same on every rank): the pair kernel's FP16 split scale
+      const long long n = (long long)src.n_internal * h->KP;
+      CK(h, cudaMemsetAsync(h->d_absmax, 0, sizeof(unsigned), st));
+      pr::abs_max_kernel<<<4 * h->sm_count, 256, 0, st>>>(src.F, n, h->d_absmax);
+      LAUNCHED(h);
+    }
     const int rc = launch_solve(h, dst, src);
     if (rc) return rc;
     cudaEventRecord(e.b, st);
@@ -1412,7 +1430,8 @@ static int create_common(pio_als_handle* h) {
       cudaMallocAsync((void**)&h->gram_partial, sizeof(double) * (size_t)h->gram_blocks * h->KP * h->KP, h->stream) != cudaSuccess ||
       cudaMallocAsync((void**)&h->gram_gsum, sizeof(double) * (size_t)GRAM_GROUPS * h->KP * h->KP, h->stream) != cudaSuccess ||
       cudaMallocAsync((void**)&h->d_fail, sizeof(int), h->stream) != cudaSuccess ||
-      cudaMallocAsync((void**)&h->d_counts, 4 * sizeof(int), h->stream) != cudaSuccess)
+      cudaMallocAsync((void**)&h->d_counts, 4 * sizeof(int), h->stream) != cudaSuccess ||
+      cudaMallocAsync((void**)&h->d_absmax, 2 * sizeof(unsigned), h->stream) != cudaSuccess)
     return fail(nullptr, PIO_ALS_ERR_CUDA, "device allocation failed");
   cudaMemsetAsync(h->yty, 0, sizeof(float) * h->KP * h->KP, h->stream);
   cudaMemsetAsync(h->d_fail, 0, sizeof(int), h->stream);
@@ -1460,6 +1479,7 @@ void pio_als_destroy(pio_als_handle* h) {
     dfree(h, h->gram_gsum);
     dfree(h, h->d_fail);
     dfree(h, h->d_counts);
+    dfree(h, h->d_absmax);
     cudaStreamSynchronize(h->stream);
     if (h->tc_out) cudaFree(h->tc_out);
     if (h->d_dbg) cudaFree(h->d_dbg);
