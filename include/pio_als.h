@@ -280,6 +280,45 @@ PIO_API int pio_events_scan(int device, const uint8_t* text, int64_t n_bytes, co
                             int64_t* out_fb_line, int64_t* out_fb_begin, int64_t* out_fb_end, int64_t* out_n_fallback,
                             int64_t* out_n_lines);
 
+/* Keyed event scan: pio_events_scan (same filter, chunking, pinned staging, fallback protocol and capacity bound) that
+ * also reads the top-level keys keys[0 .. n_keys) of each matched event's `properties` (DESIGN.md 3.2); what
+ * PEventStore.aggregatePropertyColumns folds.  Keys are compared with the JSON keys after unescaping.
+ * Per matched event e, next to everything pio_events_scan writes:
+ *   out_present[e] bit q : key q is in `properties` (a null value counts; absent or null `properties` has no keys)
+ *   out_number[e] bit q  : its value is a JSON number exact in double (integer <= 2^53 in magnitude, or Clinger's fast
+ *                          path), in out_num[e * n_keys + q] (0 otherwise)
+ *   token slot e * n_keys + q: the value's raw JSON token, out_tok_bytes[out_tok_off[slot] .. out_tok_off[slot + 1]):
+ *                          a string with its quotes, an array, an object, true / false / null, an integer, or a number
+ *                          off the fast path; empty for an absent key and for a fraction / exponent number on the fast
+ *                          path (out_num holds it).  out_tok_off: capacity * n_keys + 1 entries; out_tok_bytes: n_bytes.
+ * A tracked key twice in one `properties` object makes the line a fallback line; a number off the fast path does not.
+ * PIO_ALS_ERR_ARG for n_keys outside 1..8, a NULL, empty or repeated key, or filter->property != NULL. */
+PIO_API int pio_events_scan_keys(int device, const uint8_t* text, int64_t n_bytes, const pio_events_filter* filter,
+                                 const char* const* keys, int n_keys, int64_t capacity, int64_t* out_line,
+                                 int32_t* out_code, double* out_value, uint8_t* out_flags, int64_t* out_time_us,
+                                 uint8_t* out_eid_bytes, int64_t* out_eid_off, uint8_t* out_tid_bytes,
+                                 int64_t* out_tid_off, uint8_t* out_present, uint8_t* out_number, double* out_num,
+                                 uint8_t* out_tok_bytes, int64_t* out_tok_off, int64_t* out_n_events,
+                                 int64_t fb_capacity, int64_t* out_fb_line, int64_t* out_fb_begin, int64_t* out_fb_end,
+                                 int64_t* out_n_fallback, int64_t* out_n_lines);
+
+/* LEventAggregator's $set / $unset / $delete fold (data/src/main/scala/org/apache/predictionio/data/storage/
+ * LEventAggregator.scala) restricted to tracked keys, over n events in file order (HOST buffers): entity ids as bytes +
+ * n + 1 offsets (eid_off[0] == 0), code[e] 0 = $set / 1 = $unset / 2 = $delete, time_us[e], and present[e] (bit q: key
+ * q is in the event's properties; unused when n_keys == 0).  Events of one entity are taken in (time, file order).
+ * Per distinct entity, in order of first occurrence among the events (capacity n):
+ *   out_first_event   index of its first event (its id)
+ *   out_exists        1 when its last $set comes after its last $delete (the aggregate exists)
+ *   out_first_us / out_last_us   min / max time over all its events, also those before a $delete
+ *   out_winner[g * n_keys + q]   the $set whose value key q holds, or -1 when the key is absent: the last event among
+ *                                {$delete, $set with q present, $unset with q present} when that is a $set
+ * *out_n_entities = number of entities.  Deterministic.  PIO_ALS_ERR_ARG for n_keys outside 0..8, a code outside
+ * 0..2, n >= 2^31 or missing buffers. */
+PIO_API int pio_events_fold(int device, const uint8_t* eid_bytes, const int64_t* eid_off, const int32_t* code,
+                            const int64_t* time_us, const uint8_t* present, int64_t n, int n_keys,
+                            int64_t* out_first_event, uint8_t* out_exists, int64_t* out_first_us, int64_t* out_last_us,
+                            int64_t* out_winner, int64_t* out_n_entities);
+
 /* Item co-occurrence of the similarproduct template's CooccurrenceAlgorithm.trainCooccurrence
  * (examples/scala-parallel-similarproduct/multi-events-multi-algos/src/main/scala/CooccurrenceAlgorithm.scala:72-105):
  * (user, item) view events (indices, HOST) -> distinct -> for every user all item pairs -> count per pair -> for every item the

@@ -363,8 +363,32 @@ PIO_EV_HD bool int_id_ok(const uint8_t* s, const Span& sp) {   // str(int(token)
   return !(sp.e - sp.b == 2 && s[sp.b] == '-' && s[sp.b + 1] == '0');
 }
 
-// One line, terminator removed.  scratch: at least n bytes (decoded ids land at its start).
-PIO_EV_HD Result parse_line(const uint8_t* s, int n, const Filter& f, uint8_t* scratch) {
+// Keyed parse (parse_line_keys): the top-level keys of `properties` it reports, compared after unescaping.  The list is
+// an argument of its own rather than a Filter field, so that Filter keeps its layout.
+constexpr int MAX_KEYS = 8;
+
+struct KeyList {
+  const uint8_t* names;   // key q = names[off[q] .. off[q + 1])
+  const int* off;
+  int n;                  // 1 .. MAX_KEYS
+};
+
+// per key q of a MATCHED line (all zero otherwise)
+struct KeyValues {
+  uint32_t present;       // bit q: the key is in `properties` (a null value counts)
+  uint32_t number;        // bit q: the value is a JSON number exact in double, in num[q]
+  double num[MAX_KEYS];
+  int tok_b[MAX_KEYS];    // the value's raw JSON token at [tok_b, tok_e) of the line; empty for an absent key and for a
+  int tok_e[MAX_KEYS];    // fractional / exponent number on the fast path (num[q] is the value); an integer keeps its
+                          // token as well, so the host can tell 5 from 5.0
+};
+
+// One line, terminator removed.  scratch: at least n bytes (decoded ids land at its start).  KEYS == false is
+// parse_line; KEYS == true also fills *kv for the keys of *kl (Filter::prop_len must be < 0 then).  A tracked key twice
+// in one `properties` object makes the line FALLBACK; a number off the fast path does not (the host decodes its token).
+template <bool KEYS>
+PIO_EV_HD Result parse_line_t(const uint8_t* s, int n, const Filter& f, uint8_t* scratch, const KeyList* kl,
+                              KeyValues* kv) {
   Result r;
   r.outcome = FALLBACK;
   r.code = -1;
@@ -384,6 +408,13 @@ PIO_EV_HD Result parse_line(const uint8_t* s, int n, const Filter& f, uint8_t* s
 
   Span sp[N_SLOTS];
   for (int k = 0; k < N_SLOTS; ++k) sp[k].kind = K_ABSENT, sp[k].b = sp[k].e = 0, sp[k].esc = 0;
+  Span ksp[KEYS ? MAX_KEYS : 1];   // the tracked keys' values; `pending` = N_SLOTS + q while key q's value is read
+  if constexpr (KEYS) {
+    for (int q = 0; q < MAX_KEYS; ++q) ksp[q].kind = K_ABSENT, ksp[q].b = ksp[q].e = 0, ksp[q].esc = 0;
+  }
+  (void)ksp;
+  int kopen = -1;   // a tracked key whose value is a container (at depth 3) still open: its token ends where it closes
+  (void)kopen;
   enum { ST_VALUE, ST_VALUE_OR_END, ST_AFTER, ST_KEY_OR_END, ST_KEY, ST_COLON };
   int st = ST_VALUE, depth = 0, pending = -1;
   uint64_t arr = 0;   // bit d - 1: the container at depth d is an array
@@ -398,6 +429,9 @@ PIO_EV_HD Result parse_line(const uint8_t* s, int n, const Filter& f, uint8_t* s
     const uint8_t c = s[i];
     if (st == ST_VALUE || st == ST_VALUE_OR_END) {
       if (st == ST_VALUE_OR_END && c == ']') {
+        if constexpr (KEYS) {
+          if (depth == 3 && kopen >= 0) ksp[kopen].e = i + 1, kopen = -1;
+        }
         --depth;
         ++i;
         st = ST_AFTER;
@@ -436,7 +470,13 @@ PIO_EV_HD Result parse_line(const uint8_t* s, int n, const Filter& f, uint8_t* s
         return r;   // NaN, Infinity, bare words, stray punctuation, bytes >= 0x80
       }
       v.e = i;
-      if (pending >= 0) sp[pending] = v;
+      if constexpr (KEYS) {
+        if (pending >= N_SLOTS && (v.kind == K_OBJ || v.kind == K_ARR)) kopen = pending - N_SLOTS;
+        if (pending >= N_SLOTS) ksp[pending - N_SLOTS] = v;
+        else if (pending >= 0) sp[pending] = v;
+      } else {
+        if (pending >= 0) sp[pending] = v;
+      }
       pending = -1;
       continue;
     }
@@ -445,6 +485,9 @@ PIO_EV_HD Result parse_line(const uint8_t* s, int n, const Filter& f, uint8_t* s
       if (c == ',') {
         st = is_arr ? ST_VALUE : ST_KEY;
       } else if (c == (is_arr ? ']' : '}')) {
+        if constexpr (KEYS) {
+          if (depth == 3 && kopen >= 0) ksp[kopen].e = i + 1, kopen = -1;
+        }
         if (--depth < 2) in_props = false;
         st = ST_AFTER;
       } else {
@@ -454,6 +497,9 @@ PIO_EV_HD Result parse_line(const uint8_t* s, int n, const Filter& f, uint8_t* s
       continue;
     }
     if (st == ST_KEY_OR_END && c == '}') {
+      if constexpr (KEYS) {
+        if (depth == 3 && kopen >= 0) ksp[kopen].e = i + 1, kopen = -1;
+      }
       if (--depth < 2) in_props = false;
       ++i;
       st = ST_AFTER;
@@ -473,6 +519,17 @@ PIO_EV_HD Result parse_line(const uint8_t* s, int n, const Filter& f, uint8_t* s
       if (slot >= 0) {
         if (sp[slot].kind != K_ABSENT) return r;   // a key the parse reads, twice at its level
         sp[slot].kind = K_NULL;                     // placeholder: seen
+      }
+      if constexpr (KEYS) {
+        if (depth == 2 && in_props) {
+          for (int q = 0; q < kl->n; ++q) {
+            if (!str_eq(s, k, kl->names + kl->off[q], kl->off[q + 1] - kl->off[q], scratch)) continue;
+            if (ksp[q].kind != K_ABSENT) return r;   // a tracked key twice in `properties`
+            ksp[q].kind = K_NULL;
+            slot = N_SLOTS + q;
+            break;
+          }
+        }
       }
       pending = slot;
       st = ST_COLON;
@@ -544,8 +601,35 @@ PIO_EV_HD Result parse_line(const uint8_t* s, int n, const Filter& f, uint8_t* s
     for (int k = 0; k < r.tid_len; ++k) scratch[r.eid_len + k] = s[ti.b + k];
     r.has_target = 1;
   }
+  if constexpr (KEYS) {
+    for (int q = 0; q < kl->n; ++q) {
+      const Span& v = ksp[q];
+      if (v.kind == K_ABSENT) continue;
+      kv->present |= 1u << q;
+      if ((v.kind == K_INT || v.kind == K_NUM) && number_value(s, v, &kv->num[q])) {
+        kv->number |= 1u << q;
+        if (v.kind == K_NUM) continue;
+      } else {
+        kv->num[q] = 0.0;
+      }
+      kv->tok_b[q] = v.b;
+      kv->tok_e[q] = v.e;
+    }
+  }
   r.outcome = MATCHED;
   return r;
+}
+
+PIO_EV_HD Result parse_line(const uint8_t* s, int n, const Filter& f, uint8_t* scratch) {
+  return parse_line_t<false>(s, n, f, scratch, nullptr, nullptr);
+}
+
+// *kv is cleared first, so that a line that is not MATCHED reports no keys
+PIO_EV_HD Result parse_line_keys(const uint8_t* s, int n, const Filter& f, const KeyList& kl, uint8_t* scratch,
+                                 KeyValues* kv) {
+  kv->present = kv->number = 0;
+  for (int q = 0; q < MAX_KEYS; ++q) kv->num[q] = 0.0, kv->tok_b[q] = kv->tok_e[q] = 0;
+  return parse_line_t<true>(s, n, f, scratch, &kl, kv);
 }
 
 }  // namespace ev

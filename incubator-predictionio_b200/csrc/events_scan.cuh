@@ -9,6 +9,9 @@
 //                          chunk-sized scratch at the line's own offset (decoded ids are never longer than the line)
 //   scan_exclusive_u32 x4  output slots of the matched and fallback lines and of their id bytes
 //   ev_compact_kernel      matched events and their id bytes, fallback lines, in line order
+// The keyed scan (pio_events_scan_keys) runs the same kernels with KEYS = true: the parse also reports the tracked
+// `properties` keys of each line (event_line.h parse_line_keys), one more scan places their token bytes, and the compaction
+// copies present / number masks, numbers and token bytes next to the ids.  KEYS = false is the plain scan, unchanged.
 // Output order comes from the scans alone: no atomics, the result is deterministic.  A chunk is < 2^31 bytes, so every
 // per-chunk count fits the 32-bit scan.
 #pragma once
@@ -70,6 +73,24 @@ struct EvLines {            // per line of the chunk
   uint8_t* flags;           // bit 0: has value, bit 1: has target id
 };
 
+// the tracked keys of the keyed scan: per line of the chunk, then per matched event (unused when KEYS == false)
+struct EvKeys {
+  ev::KeyList list;         // device copy of the key names
+  uint8_t* present;         // per line: KeyValues::present / number
+  uint8_t* number;
+  double* num;              // per line x list.n
+  uint32_t* tok_b;          // per line x list.n, token range relative to the line start
+  uint32_t* tok_e;
+  uint32_t* tok_len;        // per line: token bytes of a matched line; then its exclusive scan in tok_pos
+  uint32_t* tok_pos;
+  long long tok_base;       // token bytes of the call before this chunk
+  uint8_t* o_present;       // per matched event
+  uint8_t* o_number;
+  double* o_num;            // per matched event x list.n
+  long long* o_tok_off;     // per matched event x list.n: start of the token in the caller's token column
+  uint8_t* o_tok;
+};
+
 __device__ __forceinline__ void ev_store(const EvLines& L, long long j, const ev::Result& r) {
   const bool m = r.outcome == ev::MATCHED;
   L.is_match[j] = m;
@@ -82,15 +103,44 @@ __device__ __forceinline__ void ev_store(const EvLines& L, long long j, const ev
   L.flags[j] = (uint8_t)(r.has_value | (r.has_target << 1));
 }
 
+__device__ __forceinline__ void ev_store_keys(const EvKeys& K, long long j, const ev::Result& r, const ev::KeyValues& kv) {
+  const int nk = K.list.n;
+  uint32_t len = 0;
+  K.present[j] = (uint8_t)kv.present;
+  K.number[j] = (uint8_t)kv.number;
+  for (int q = 0; q < nk; ++q) {
+    K.num[j * nk + q] = kv.num[q];
+    K.tok_b[j * nk + q] = (uint32_t)kv.tok_b[q];
+    K.tok_e[j * nk + q] = (uint32_t)kv.tok_e[q];
+    len += (uint32_t)(kv.tok_e[q] - kv.tok_b[q]);
+  }
+  K.tok_len[j] = r.outcome == ev::MATCHED ? len : 0u;
+}
+
+// the parse of one line, stored
+template <bool KEYS>
+__device__ __forceinline__ void ev_parse_store(const uint8_t* line, int n, const ev::Filter& f, uint8_t* scratch,
+                                               const EvLines& L, const EvKeys& K, long long j) {
+  if constexpr (KEYS) {
+    ev::KeyValues kv;
+    const ev::Result r = ev::parse_line_keys(line, n, f, K.list, scratch, &kv);
+    ev_store(L, j, r);
+    ev_store_keys(K, j, r, kv);
+  } else {
+    ev_store(L, j, ev::parse_line(line, n, f, scratch));
+  }
+}
+
 // one line per thread, read from global memory
+template <bool KEYS>
 __global__ void __launch_bounds__(EV_THREADS)
 ev_parse_kernel(const uint8_t* __restrict__ t, const uint32_t* __restrict__ starts, long long nl, const ev::Filter f,
-                uint8_t* __restrict__ scratch, EvLines L) {
+                uint8_t* __restrict__ scratch, EvLines L, const EvKeys K) {
   const long long j = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (j >= nl) return;
   uint32_t b, e;
   ev_line_range(t, starts, j, &b, &e);
-  ev_store(L, j, ev::parse_line(t + b, (int)(e - b), f, scratch + b));
+  ev_parse_store<KEYS>(t + b, (int)(e - b), f, scratch + b, L, K, j);
 }
 
 // The same parse with the block's lines first copied into shared memory by the whole block in coalesced 16-byte loads
@@ -98,9 +148,10 @@ ev_parse_kernel(const uint8_t* __restrict__ t, const uint32_t* __restrict__ star
 // reads global memory like ev_parse_kernel.  `t` must be 16-byte aligned.
 constexpr int EV_SMEM_BYTES = 64 * 1024;
 
+template <bool KEYS>
 __global__ void __launch_bounds__(EV_THREADS)
 ev_parse_smem_kernel(const uint8_t* __restrict__ t, const uint32_t* __restrict__ starts, long long nl,
-                     const ev::Filter f, uint8_t* __restrict__ scratch, EvLines L) {
+                     const ev::Filter f, uint8_t* __restrict__ scratch, EvLines L, const EvKeys K) {
   extern __shared__ __align__(16) uint8_t ev_sm[];
   const long long j0 = (long long)blockIdx.x * blockDim.x;
   const long long j1 = j0 + blockDim.x < nl ? j0 + blockDim.x : nl;
@@ -118,7 +169,7 @@ ev_parse_smem_kernel(const uint8_t* __restrict__ t, const uint32_t* __restrict__
   if (j >= nl) return;
   uint32_t b, e;
   ev_line_range(t, starts, j, &b, &e);
-  ev_store(L, j, ev::parse_line(staged ? ev_sm + (b - a0) : t + b, (int)(e - b), f, scratch + b));
+  ev_parse_store<KEYS>(staged ? ev_sm + (b - a0) : t + b, (int)(e - b), f, scratch + b, L, K, j);
 }
 
 struct EvOut {              // device output of one chunk, indexed by the chunk's match / fallback / byte slots
@@ -141,9 +192,10 @@ struct EvBase {
   long long line, byte, eid, tid;
 };
 
+template <bool KEYS>
 __global__ void __launch_bounds__(EV_THREADS)
 ev_compact_kernel(const uint8_t* __restrict__ t, const uint32_t* __restrict__ starts, long long nl, const EvBase base,
-                  const uint8_t* __restrict__ scratch, const EvLines L, EvOut o) {
+                  const uint8_t* __restrict__ scratch, const EvLines L, EvOut o, const EvKeys K) {
   const long long j = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (j >= nl) return;
   if (L.is_match[j]) {
@@ -158,6 +210,18 @@ ev_compact_kernel(const uint8_t* __restrict__ t, const uint32_t* __restrict__ st
     o.tid_off[k] = base.tid + pt;
     for (uint32_t q = 0; q < ne; ++q) o.eid_bytes[pe + q] = scratch[b + q];
     for (uint32_t q = 0; q < nt; ++q) o.tid_bytes[pt + q] = scratch[b + ne + q];
+    if constexpr (KEYS) {   // token bytes straight from the text, in line order like the ids
+      const int nk = K.list.n;
+      K.o_present[k] = K.present[j];
+      K.o_number[k] = K.number[j];
+      uint32_t at = K.tok_pos[j];
+      for (int q = 0; q < nk; ++q) {
+        const uint32_t tb = K.tok_b[j * nk + q], te = K.tok_e[j * nk + q];
+        K.o_num[(long long)k * nk + q] = K.num[j * nk + q];
+        K.o_tok_off[(long long)k * nk + q] = K.tok_base + at;
+        for (uint32_t c = tb; c < te; ++c) K.o_tok[at++] = t[b + c];
+      }
+    }
   } else if (L.is_fb[j]) {
     const uint32_t k = L.fb_pos[j];
     uint32_t b, e;

@@ -49,6 +49,7 @@
 #include "solve_plan.h"
 #include "ids_encode.cuh"
 #include "events_scan.cuh"
+#include "events_fold.cuh"
 #include "cooc.cuh"
 
 namespace pio {
@@ -2566,41 +2567,33 @@ int pio_als_synth_ratings_device(int device, int32_t n_users, int32_t n_items, i
 }
 
 // ---- string ids -> dense indices (BiMap.stringInt) ---------------------------------------------------------------------
-int pio_ids_encode(int device, const uint8_t* bytes, const int64_t* offsets, int64_t n, int32_t* out_index,
-                   int64_t* out_first, int32_t* out_n_unique) {
-  if (n < 0 || !offsets || !out_index || !out_n_unique || (n > 0 && !bytes && offsets[n] > offsets[0]))
-    return fail(nullptr, PIO_ALS_ERR_ARG, "bad pio_ids_encode arguments");
-  *out_n_unique = 0;
-  if (n == 0) return PIO_ALS_OK;
-  if (n >= (1ll << 32)) return fail(nullptr, PIO_ALS_ERR_ARG, "n must be < 2^32");
-  if (offsets[0] != 0) return fail(nullptr, PIO_ALS_ERR_ARG, "offsets[0] must be 0");
-  CK0(cudaSetDevice(device));
-  const size_t nb = (size_t)offsets[n];
-  uint8_t* d_bytes = nullptr;
-  long long *d_off = nullptr, *d_first = nullptr;
+// The pipeline of ids_encode.cuh over n strings already on the device, on stream st (pio_ids_encode, pio_events_fold):
+// d_index[e] = dense index of string e in order of first occurrence; d_first (nullable, n entries) [id] = position of
+// the first occurrence of id; *n_unique.  0 < n < 2^32.
+static int ids_encode_device(const uint8_t* d_bytes, const long long* d_off, int64_t n, cudaStream_t st, int* d_index,
+                             long long* d_first, int64_t* n_unique) {
   uint64_t *ka = nullptr, *kb = nullptr;
   uint32_t *va = nullptr, *vb = nullptr, *f1 = nullptr, *f2 = nullptr, *run_start = nullptr, *head = nullptr, *ishead = nullptr,
            *firstpos = nullptr, *isfirst = nullptr;
-  int* d_out = nullptr;
   std::vector<void*> owned;
   auto A = [&](void** p, size_t bytes_) -> cudaError_t {
     cudaError_t e = cudaMalloc(p, bytes_ ? bytes_ : 1);
     if (e == cudaSuccess) owned.push_back(*p);
     return e;
   };
-  struct Guard { std::vector<void*>& v; ~Guard() { for (void* q : v) cudaFree(q); } } guard{owned};
-  CK0(A((void**)&d_bytes, nb));
-  CK0(A((void**)&d_off, sizeof(long long) * (n + 1)));
+  struct Guard {
+    std::vector<void*>& v;
+    cudaStream_t s;
+    ~Guard() {
+      cudaStreamSynchronize(s);
+      for (void* q : v) cudaFree(q);
+    }
+  } guard{owned, st};
   CK0(A((void**)&ka, 8 * (size_t)n)); CK0(A((void**)&kb, 8 * (size_t)n));
   CK0(A((void**)&va, 4 * (size_t)n)); CK0(A((void**)&vb, 4 * (size_t)n));
   CK0(A((void**)&f1, 4 * (size_t)n)); CK0(A((void**)&f2, 4 * (size_t)n));
   CK0(A((void**)&run_start, 4 * (size_t)n)); CK0(A((void**)&head, 4 * (size_t)n)); CK0(A((void**)&ishead, 4 * (size_t)n));
   CK0(A((void**)&firstpos, 4 * (size_t)n)); CK0(A((void**)&isfirst, 4 * (size_t)n));
-  CK0(A((void**)&d_out, 4 * (size_t)n));
-  CK0(A((void**)&d_first, 8 * (size_t)n));
-  cudaStream_t st = 0;
-  CK0(cudaMemcpyAsync(d_bytes, bytes, nb, cudaMemcpyHostToDevice, st));
-  CK0(cudaMemcpyAsync(d_off, offsets, sizeof(long long) * (n + 1), cudaMemcpyHostToDevice, st));
   uint64_t mask = ~0ull;
   if (const char* hb = getenv("PIO_IDS_HASH_BITS")) {   // tests: a short hash makes different strings collide on purpose
     const int b = atoi(hb);
@@ -2622,10 +2615,44 @@ int pio_ids_encode(int device, const uint8_t* bytes, const int64_t* offsets, int
   CK0(cudaMemsetAsync(isfirst, 0, 4 * (size_t)n, st));
   ids_firstpos_kernel<<<nblk(n, 256), 256, 0, st>>>(vs, ishead, f2, n, firstpos, isfirst);
   CK0(scan_exclusive_u32(isfirst, isfirst, (size_t)n, st, nullptr));       // ids by first occurrence
-  ids_assign_kernel<<<nblk(n, 256), 256, 0, st>>>(vs, head, isfirst, n, d_out, out_first ? d_first : nullptr);
-  CK0(cudaMemcpyAsync(out_index, d_out, 4 * (size_t)n, cudaMemcpyDeviceToHost, st));
+  ids_assign_kernel<<<nblk(n, 256), 256, 0, st>>>(vs, head, isfirst, n, d_index, d_first);
+  CK0(cudaGetLastError());
   CK0(cudaStreamSynchronize(st));
-  const int64_t nuniq = (int64_t)last_ex + last_flag;
+  *n_unique = (int64_t)last_ex + last_flag;
+  return PIO_ALS_OK;
+}
+
+int pio_ids_encode(int device, const uint8_t* bytes, const int64_t* offsets, int64_t n, int32_t* out_index,
+                   int64_t* out_first, int32_t* out_n_unique) {
+  if (n < 0 || !offsets || !out_index || !out_n_unique || (n > 0 && !bytes && offsets[n] > offsets[0]))
+    return fail(nullptr, PIO_ALS_ERR_ARG, "bad pio_ids_encode arguments");
+  *out_n_unique = 0;
+  if (n == 0) return PIO_ALS_OK;
+  if (n >= (1ll << 32)) return fail(nullptr, PIO_ALS_ERR_ARG, "n must be < 2^32");
+  if (offsets[0] != 0) return fail(nullptr, PIO_ALS_ERR_ARG, "offsets[0] must be 0");
+  CK0(cudaSetDevice(device));
+  const size_t nb = (size_t)offsets[n];
+  uint8_t* d_bytes = nullptr;
+  long long *d_off = nullptr, *d_first = nullptr;
+  int* d_out = nullptr;
+  std::vector<void*> owned;
+  auto A = [&](void** p, size_t bytes_) -> cudaError_t {
+    cudaError_t e = cudaMalloc(p, bytes_ ? bytes_ : 1);
+    if (e == cudaSuccess) owned.push_back(*p);
+    return e;
+  };
+  struct Guard { std::vector<void*>& v; ~Guard() { for (void* q : v) cudaFree(q); } } guard{owned};
+  CK0(A((void**)&d_bytes, nb));
+  CK0(A((void**)&d_off, sizeof(long long) * (n + 1)));
+  CK0(A((void**)&d_out, 4 * (size_t)n));
+  CK0(A((void**)&d_first, 8 * (size_t)n));
+  cudaStream_t st = 0;
+  CK0(cudaMemcpyAsync(d_bytes, bytes, nb, cudaMemcpyHostToDevice, st));
+  CK0(cudaMemcpyAsync(d_off, offsets, sizeof(long long) * (n + 1), cudaMemcpyHostToDevice, st));
+  int64_t nuniq = 0;
+  const int rc = ids_encode_device(d_bytes, d_off, n, st, d_out, out_first ? d_first : nullptr, &nuniq);
+  if (rc != PIO_ALS_OK) return rc;
+  CK0(cudaMemcpy(out_index, d_out, 4 * (size_t)n, cudaMemcpyDeviceToHost));
   if (out_first) CK0(cudaMemcpy(out_first, d_first, 8 * (size_t)nuniq, cudaMemcpyDeviceToHost));
   *out_n_unique = (int32_t)nuniq;
   return PIO_ALS_OK;
@@ -2652,11 +2679,24 @@ static int64_t ev_cut(const uint8_t* t, int64_t n, int64_t b, int64_t cap) {
   return b;
 }
 
-int pio_events_scan(int device, const uint8_t* text, int64_t n_bytes, const pio_events_filter* f, int64_t capacity,
-                    int64_t* out_line, int32_t* out_code, double* out_value, uint8_t* out_flags, int64_t* out_time_us,
-                    uint8_t* out_eid_bytes, int64_t* out_eid_off, uint8_t* out_tid_bytes, int64_t* out_tid_off,
-                    int64_t* out_n_events, int64_t fb_capacity, int64_t* out_fb_line, int64_t* out_fb_begin,
-                    int64_t* out_fb_end, int64_t* out_n_fallback, int64_t* out_n_lines) {
+// the tracked keys of pio_events_scan_keys and where their columns go (host buffers)
+struct EvKeyArgs {
+  const char* const* keys;
+  int n;
+  uint8_t* out_present;
+  uint8_t* out_number;
+  double* out_num;
+  uint8_t* out_tok_bytes;
+  int64_t* out_tok_off;
+};
+
+// pio_events_scan (ka == nullptr) and pio_events_scan_keys: one chunk loop, the kernels instantiated with KEYS = ka != 0
+static int events_scan_impl(int device, const uint8_t* text, int64_t n_bytes, const pio_events_filter* f,
+                            int64_t capacity, int64_t* out_line, int32_t* out_code, double* out_value, uint8_t* out_flags,
+                            int64_t* out_time_us, uint8_t* out_eid_bytes, int64_t* out_eid_off, uint8_t* out_tid_bytes,
+                            int64_t* out_tid_off, int64_t* out_n_events, int64_t fb_capacity, int64_t* out_fb_line,
+                            int64_t* out_fb_begin, int64_t* out_fb_end, int64_t* out_n_fallback, int64_t* out_n_lines,
+                            const EvKeyArgs* ka) {
   if (n_bytes < 0 || (n_bytes > 0 && !text) || !f || capacity < n_bytes / PIO_EVENTS_MIN_EVENT_BYTES + 1 ||
       fb_capacity < 0 || !out_line || !out_code || !out_value || !out_flags || !out_time_us || !out_eid_bytes ||
       !out_eid_off || !out_tid_bytes || !out_tid_off || !out_n_events || (fb_capacity > 0 && (!out_fb_line ||
@@ -2669,8 +2709,10 @@ int pio_events_scan(int device, const uint8_t* text, int64_t n_bytes, const pio_
   if (f->target_entity_type_mode < PIO_EVENTS_TARGET_ANY || f->target_entity_type_mode > PIO_EVENTS_TARGET_EQUALS ||
       (f->target_entity_type_mode == PIO_EVENTS_TARGET_EQUALS && !f->target_entity_type))
     return fail(nullptr, PIO_ALS_ERR_ARG, "bad target_entity_type_mode / target_entity_type");
+  const int nk = ka ? ka->n : 0;
   *out_n_events = *out_n_fallback = *out_n_lines = 0;
   out_eid_off[0] = out_tid_off[0] = 0;
+  if (ka) ka->out_tok_off[0] = 0;
   if (n_bytes == 0) return PIO_ALS_OK;
   CK0(cudaSetDevice(device));
 
@@ -2691,6 +2733,11 @@ int pio_events_scan(int device, const uint8_t* text, int64_t n_bytes, const pio_
   for (int k = 0; k < f->n_event_names; ++k) {
     put(f->event_names[k]);
     noff.push_back((int)fbytes.size());
+  }
+  std::vector<int> koff(1, (int)fbytes.size());   // then the tracked keys
+  for (int q = 0; q < nk; ++q) {
+    put(ka->keys[q]);
+    koff.push_back((int)fbytes.size());
   }
 
   int64_t cap = 64ll << 20;   // device chunk; PIO_EVENTS_DEVICE_CHUNK (bytes) lets tests straddle its boundaries
@@ -2740,11 +2787,12 @@ int pio_events_scan(int device, const uint8_t* text, int64_t n_bytes, const pio_
   bool use_smem = true;   // PIO_EVENTS_SMEM=0: the parse reads its lines from global memory (A/B measurements)
   if (const char* c = getenv("PIO_EVENTS_SMEM")) use_smem = atoi(c) != 0;
   if (use_smem)
-    CK0(cudaFuncSetAttribute(ev_parse_smem_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, EV_SMEM_BYTES));
+    CK0(cudaFuncSetAttribute(ka ? ev_parse_smem_kernel<true> : ev_parse_smem_kernel<false>,
+                             cudaFuncAttributeMaxDynamicSharedMemorySize, EV_SMEM_BYTES));
   cudaStream_t ex = streams[0], cp = streams[1];   // scan, host-to-device copies
   uint8_t *d_text[2] = {nullptr, nullptr}, *stage[2] = {nullptr, nullptr}, *d_scratch = nullptr, *d_fbytes = nullptr;
   uint32_t *d_flag = nullptr, *d_lid = nullptr, *d_tot = nullptr, *h_tot = nullptr;
-  int* d_noff = nullptr;
+  int *d_noff = nullptr, *d_koff = nullptr;
   for (int k = 0; k < 2; ++k) {
     CK0(A((void**)&d_text[k], (size_t)cap));
     CK0(P((void**)&stage[k], (size_t)cap));
@@ -2758,6 +2806,8 @@ int pio_events_scan(int device, const uint8_t* text, int64_t n_bytes, const pio_
   CK0(P((void**)&h_tot, 8 * sizeof(uint32_t)));
   if (!fbytes.empty()) CK0(cudaMemcpy(d_fbytes, fbytes.data(), fbytes.size(), cudaMemcpyHostToDevice));
   CK0(cudaMemcpy(d_noff, noff.data(), sizeof(int) * noff.size(), cudaMemcpyHostToDevice));
+  CK0(A((void**)&d_koff, sizeof(int) * koff.size()));
+  CK0(cudaMemcpy(d_koff, koff.data(), sizeof(int) * koff.size(), cudaMemcpyHostToDevice));
   ev::Filter df;
   df.entity_type = d_fbytes + at_et;
   df.entity_type_len = len_et;
@@ -2774,8 +2824,13 @@ int pio_events_scan(int device, const uint8_t* text, int64_t n_bytes, const pio_
   df.start_us = f->start_us;
   df.until_us = f->until_us;
 
+  EvKeys K{};
+  K.list.names = d_fbytes;
+  K.list.off = d_koff;
+  K.list.n = nk;
+
   EvBase base{0, 0, 0, 0};
-  int64_t n_ev = 0, n_fb = 0;   // n_fb counts every fallback line, also those beyond fb_capacity
+  int64_t n_ev = 0, n_fb = 0, n_tok = 0;   // n_tok: token bytes so far   // n_fb counts every fallback line, also those beyond fb_capacity
   // lines longer than a chunk, found while cutting the next chunk: written after the current chunk's fallback lines so
   // that the fallback list stays in line order
   std::vector<int64_t> oversized;
@@ -2879,23 +2934,52 @@ int pio_events_scan(int device, const uint8_t* text, int64_t n_bytes, const pio_
     CK0(CA((void**)&o.fb_end, 8 * nls));
     CK0(CA((void**)&o.eid_bytes, (size_t)L));
     CK0(CA((void**)&o.tid_bytes, (size_t)L));
+    if (ka) {
+      const size_t nlk = nls * (size_t)nk;
+      CK0(CA((void**)&K.present, nls));
+      CK0(CA((void**)&K.number, nls));
+      CK0(CA((void**)&K.num, 8 * nlk));
+      CK0(CA((void**)&K.tok_b, 4 * nlk));
+      CK0(CA((void**)&K.tok_e, 4 * nlk));
+      CK0(CA((void**)&K.tok_len, 4 * nls));
+      CK0(CA((void**)&K.tok_pos, 4 * nls));
+      CK0(CA((void**)&K.o_present, nls));
+      CK0(CA((void**)&K.o_number, nls));
+      CK0(CA((void**)&K.o_num, 8 * nlk));
+      CK0(CA((void**)&K.o_tok_off, 8 * nlk));
+      CK0(CA((void**)&K.o_tok, (size_t)L));   // tokens are disjoint pieces of the chunk's text
+      K.tok_base = n_tok;
+    }
     CK0(cudaEventRecord(k2, ex));
     ev_start_scatter_kernel<<<nblk(L, EV_THREADS), EV_THREADS, 0, ex>>>(d_flag, d_lid, L, nl, starts);
-    if (use_smem)
-      ev_parse_smem_kernel<<<nblk(nl, EV_THREADS), EV_THREADS, EV_SMEM_BYTES, ex>>>(t, starts, nl, df, d_scratch, Ls);
+    const unsigned gl = nblk(nl, EV_THREADS);
+    if (use_smem && ka)
+      ev_parse_smem_kernel<true><<<gl, EV_THREADS, EV_SMEM_BYTES, ex>>>(t, starts, nl, df, d_scratch, Ls, K);
+    else if (use_smem)
+      ev_parse_smem_kernel<false><<<gl, EV_THREADS, EV_SMEM_BYTES, ex>>>(t, starts, nl, df, d_scratch, Ls, K);
+    else if (ka)
+      ev_parse_kernel<true><<<gl, EV_THREADS, 0, ex>>>(t, starts, nl, df, d_scratch, Ls, K);
     else
-      ev_parse_kernel<<<nblk(nl, EV_THREADS), EV_THREADS, 0, ex>>>(t, starts, nl, df, d_scratch, Ls);
+      ev_parse_kernel<false><<<gl, EV_THREADS, 0, ex>>>(t, starts, nl, df, d_scratch, Ls, K);
     CK0(cudaGetLastError());
     CK0(scan_exclusive_u32(Ls.is_match, Ls.match_pos, nls, ex, nullptr));
     CK0(scan_exclusive_u32(Ls.is_fb, Ls.fb_pos, nls, ex, nullptr));
     CK0(scan_exclusive_u32(Ls.eid_len, Ls.eid_pos, nls, ex, nullptr));
     CK0(scan_exclusive_u32(Ls.tid_len, Ls.tid_pos, nls, ex, nullptr));
+    if (ka) CK0(scan_exclusive_u32(K.tok_len, K.tok_pos, nls, ex, nullptr));
     EvBase cb_{here.line, here.byte, base.eid, base.tid};
-    ev_compact_kernel<<<nblk(nl, EV_THREADS), EV_THREADS, 0, ex>>>(t, starts, nl, cb_, d_scratch, Ls, o);
+    if (ka)
+      ev_compact_kernel<true><<<gl, EV_THREADS, 0, ex>>>(t, starts, nl, cb_, d_scratch, Ls, o, K);
+    else
+      ev_compact_kernel<false><<<gl, EV_THREADS, 0, ex>>>(t, starts, nl, cb_, d_scratch, Ls, o, K);
     ev_totals_kernel<<<1, 1, 0, ex>>>(Ls, nl, d_tot);
     CK0(cudaGetLastError());
     CK0(cudaEventRecord(k3, ex));
     CK0(cudaMemcpyAsync(h_tot, d_tot, 4 * sizeof(uint32_t), cudaMemcpyDeviceToHost, ex));
+    if (ka) {   // token bytes of the chunk: last exclusive position + last length
+      CK0(cudaMemcpyAsync(h_tot + 6, K.tok_pos + nl - 1, 4, cudaMemcpyDeviceToHost, ex));
+      CK0(cudaMemcpyAsync(h_tot + 7, K.tok_len + nl - 1, 4, cudaMemcpyDeviceToHost, ex));
+    }
     // find and stage the next chunk while this one is parsed (oversized lines before it belong after this chunk's
     // lines, so their line numbers are assigned only now that this chunk's line count is known)
     int64_t nb, ne;
@@ -2914,6 +2998,15 @@ int pio_events_scan(int device, const uint8_t* text, int64_t n_bytes, const pio_
     CK0(cudaMemcpyAsync(out_tid_off + n_ev, o.tid_off, 8 * nm, cudaMemcpyDeviceToHost, ex));
     CK0(cudaMemcpyAsync(out_eid_bytes + base.eid, o.eid_bytes, eb, cudaMemcpyDeviceToHost, ex));
     CK0(cudaMemcpyAsync(out_tid_bytes + base.tid, o.tid_bytes, tb, cudaMemcpyDeviceToHost, ex));
+    int64_t tk = 0;
+    if (ka) {
+      tk = (int64_t)h_tot[6] + h_tot[7];
+      CK0(cudaMemcpyAsync(ka->out_present + n_ev, K.o_present, nm, cudaMemcpyDeviceToHost, ex));
+      CK0(cudaMemcpyAsync(ka->out_number + n_ev, K.o_number, nm, cudaMemcpyDeviceToHost, ex));
+      CK0(cudaMemcpyAsync(ka->out_num + n_ev * nk, K.o_num, 8 * nm * nk, cudaMemcpyDeviceToHost, ex));
+      CK0(cudaMemcpyAsync(ka->out_tok_off + n_ev * nk, K.o_tok_off, 8 * nm * nk, cudaMemcpyDeviceToHost, ex));
+      CK0(cudaMemcpyAsync(ka->out_tok_bytes + n_tok, K.o_tok, tk, cudaMemcpyDeviceToHost, ex));
+    }
     const int64_t room = fb_capacity - n_fb, nfc = nf < room ? nf : (room > 0 ? room : 0);
     if (nfc > 0) {
       CK0(cudaMemcpyAsync(out_fb_line + n_fb, o.fb_line, 8 * nfc, cudaMemcpyDeviceToHost, ex));
@@ -2930,14 +3023,136 @@ int pio_events_scan(int device, const uint8_t* text, int64_t n_bytes, const pio_
     n_fb += nf;
     base.eid += eb;
     base.tid += tb;
+    n_tok += tk;
     flush_oversized();
     cb = nb, ce = ne;
   }
   out_eid_off[n_ev] = base.eid;
   out_tid_off[n_ev] = base.tid;
+  if (ka) ka->out_tok_off[n_ev * nk] = n_tok;
   *out_n_events = n_ev;
   *out_n_fallback = n_fb;
   *out_n_lines = base.line;
+  return PIO_ALS_OK;
+}
+
+int pio_events_scan(int device, const uint8_t* text, int64_t n_bytes, const pio_events_filter* f, int64_t capacity,
+                    int64_t* out_line, int32_t* out_code, double* out_value, uint8_t* out_flags, int64_t* out_time_us,
+                    uint8_t* out_eid_bytes, int64_t* out_eid_off, uint8_t* out_tid_bytes, int64_t* out_tid_off,
+                    int64_t* out_n_events, int64_t fb_capacity, int64_t* out_fb_line, int64_t* out_fb_begin,
+                    int64_t* out_fb_end, int64_t* out_n_fallback, int64_t* out_n_lines) {
+  return events_scan_impl(device, text, n_bytes, f, capacity, out_line, out_code, out_value, out_flags, out_time_us,
+                          out_eid_bytes, out_eid_off, out_tid_bytes, out_tid_off, out_n_events, fb_capacity, out_fb_line,
+                          out_fb_begin, out_fb_end, out_n_fallback, out_n_lines, nullptr);
+}
+
+int pio_events_scan_keys(int device, const uint8_t* text, int64_t n_bytes, const pio_events_filter* f,
+                         const char* const* keys, int n_keys, int64_t capacity, int64_t* out_line, int32_t* out_code,
+                         double* out_value, uint8_t* out_flags, int64_t* out_time_us, uint8_t* out_eid_bytes,
+                         int64_t* out_eid_off, uint8_t* out_tid_bytes, int64_t* out_tid_off, uint8_t* out_present,
+                         uint8_t* out_number, double* out_num, uint8_t* out_tok_bytes, int64_t* out_tok_off,
+                         int64_t* out_n_events, int64_t fb_capacity, int64_t* out_fb_line, int64_t* out_fb_begin,
+                         int64_t* out_fb_end, int64_t* out_n_fallback, int64_t* out_n_lines) {
+  if (n_keys < 1 || n_keys > ev::MAX_KEYS || !keys || !out_present || !out_number || !out_num || !out_tok_bytes ||
+      !out_tok_off)
+    return fail(nullptr, PIO_ALS_ERR_ARG, "bad pio_events_scan_keys arguments (n_keys must be 1..%d)", ev::MAX_KEYS);
+  if (!f || f->property)
+    return fail(nullptr, PIO_ALS_ERR_ARG, "pio_events_scan_keys: filter->property must be NULL");
+  for (int q = 0; q < n_keys; ++q) {
+    if (!keys[q] || !keys[q][0]) return fail(nullptr, PIO_ALS_ERR_ARG, "key %d is NULL or empty", q);
+    for (int p = 0; p < q; ++p)
+      if (!strcmp(keys[p], keys[q])) return fail(nullptr, PIO_ALS_ERR_ARG, "key %d repeats key %d", q, p);
+  }
+  const EvKeyArgs ka{keys, n_keys, out_present, out_number, out_num, out_tok_bytes, out_tok_off};
+  return events_scan_impl(device, text, n_bytes, f, capacity, out_line, out_code, out_value, out_flags, out_time_us,
+                          out_eid_bytes, out_eid_off, out_tid_bytes, out_tid_off, out_n_events, fb_capacity, out_fb_line,
+                          out_fb_begin, out_fb_end, out_n_fallback, out_n_lines, &ka);
+}
+
+// ---- $set / $unset / $delete fold (PEventStore.aggregatePropertyColumns; events_fold.cuh) -----------------------------
+int pio_events_fold(int device, const uint8_t* eid_bytes, const int64_t* eid_off, const int32_t* code,
+                    const int64_t* time_us, const uint8_t* present, int64_t n, int n_keys, int64_t* out_first_event,
+                    uint8_t* out_exists, int64_t* out_first_us, int64_t* out_last_us, int64_t* out_winner,
+                    int64_t* out_n_entities) {
+  if (n < 0 || n_keys < 0 || n_keys > ev::MAX_KEYS || !eid_off || !out_n_entities || (n > 0 && (!code || !time_us ||
+      !out_first_event || !out_exists || !out_first_us || !out_last_us || (n_keys > 0 && (!present || !out_winner)) ||
+      (!eid_bytes && eid_off[n] > eid_off[0]))))
+    return fail(nullptr, PIO_ALS_ERR_ARG, "bad pio_events_fold arguments (n_keys must be 0..%d)", ev::MAX_KEYS);
+  *out_n_entities = 0;
+  if (n == 0) return PIO_ALS_OK;
+  if (n >= (1ll << 31)) return fail(nullptr, PIO_ALS_ERR_ARG, "n must be < 2^31");
+  if (eid_off[0] != 0) return fail(nullptr, PIO_ALS_ERR_ARG, "eid_off[0] must be 0");
+  for (int64_t e = 0; e < n; ++e)
+    if (code[e] < FOLD_SET || code[e] > FOLD_DELETE)
+      return fail(nullptr, PIO_ALS_ERR_ARG, "code[%lld] = %d is not 0 ($set), 1 ($unset) or 2 ($delete)", (long long)e,
+                  code[e]);
+  CK0(cudaSetDevice(device));
+  const size_t nb = (size_t)eid_off[n], nn = (size_t)n, nk = (size_t)n_keys;
+  std::vector<void*> owned;
+  auto A = [&](void** p, size_t bytes_) -> cudaError_t {
+    cudaError_t e = cudaMalloc(p, bytes_ ? bytes_ : 1);
+    if (e == cudaSuccess) owned.push_back(*p);
+    return e;
+  };
+  struct Guard { std::vector<void*>& v; ~Guard() { for (void* q : v) cudaFree(q); } } guard{owned};
+  uint8_t *d_bytes = nullptr, *d_present = nullptr, *d_exists = nullptr;
+  long long *d_off = nullptr, *d_time = nullptr, *d_first = nullptr, *d_fus = nullptr, *d_lus = nullptr, *d_win = nullptr;
+  int32_t* d_code = nullptr;
+  int *d_ent = nullptr, *seg_first = nullptr, *seg_last = nullptr, *last_set = nullptr, *last_del = nullptr, *win = nullptr;
+  uint64_t *ka = nullptr, *kb = nullptr;
+  uint32_t *va = nullptr, *vb = nullptr;
+  CK0(A((void**)&d_bytes, nb));
+  CK0(A((void**)&d_off, 8 * (nn + 1)));
+  CK0(A((void**)&d_code, 4 * nn));
+  CK0(A((void**)&d_time, 8 * nn));
+  CK0(A((void**)&d_present, nn));
+  CK0(A((void**)&d_ent, 4 * nn));
+  CK0(A((void**)&d_first, 8 * nn));
+  CK0(A((void**)&ka, 8 * nn)); CK0(A((void**)&kb, 8 * nn));
+  CK0(A((void**)&va, 4 * nn)); CK0(A((void**)&vb, 4 * nn));
+  cudaStream_t st = 0;
+  CK0(cudaMemcpyAsync(d_bytes, eid_bytes, nb, cudaMemcpyHostToDevice, st));
+  CK0(cudaMemcpyAsync(d_off, eid_off, 8 * (nn + 1), cudaMemcpyHostToDevice, st));
+  CK0(cudaMemcpyAsync(d_code, code, 4 * nn, cudaMemcpyHostToDevice, st));
+  CK0(cudaMemcpyAsync(d_time, time_us, 8 * nn, cudaMemcpyHostToDevice, st));
+  if (n_keys) CK0(cudaMemcpyAsync(d_present, present, nn, cudaMemcpyHostToDevice, st));
+  int64_t n_ent = 0;
+  const int rc = ids_encode_device(d_bytes, d_off, n, st, d_ent, d_first, &n_ent);
+  if (rc != PIO_ALS_OK) return rc;
+  const size_t ne = (size_t)n_ent;
+  CK0(A((void**)&seg_first, 4 * ne)); CK0(A((void**)&seg_last, 4 * ne));
+  CK0(A((void**)&last_set, 4 * ne)); CK0(A((void**)&last_del, 4 * ne));
+  CK0(A((void**)&win, 4 * ne * nk));
+  CK0(A((void**)&d_exists, ne));
+  CK0(A((void**)&d_fus, 8 * ne)); CK0(A((void**)&d_lus, 8 * ne));
+  CK0(A((void**)&d_win, 8 * ne * nk));
+  CK0(cudaMemsetAsync(last_set, 0xFF, 4 * ne, st));   // -1: none
+  CK0(cudaMemsetAsync(last_del, 0xFF, 4 * ne, st));
+  if (nk) CK0(cudaMemsetAsync(win, 0xFF, 4 * ne * nk, st));
+  // (entity, time, line): stable by time, then stable by entity
+  fold_time_key_kernel<<<nblk(n, 256), 256, 0, st>>>(d_time, n, ka, va);
+  bool in_b = false;
+  CK0(radix_sort_pairs(ka, va, kb, vb, nn, 64, st, &in_b, nullptr));
+  uint64_t* k1 = in_b ? kb : ka;   // sorted by time; the other pair is free
+  uint32_t* v1 = in_b ? vb : va;
+  uint64_t* k2 = in_b ? ka : kb;
+  uint32_t* v2 = in_b ? va : vb;
+  fold_entity_key_kernel<<<nblk(n, 256), 256, 0, st>>>(v1, d_ent, n, k1);
+  CK0(radix_sort_pairs(k1, v1, k2, v2, nn, ceil_log2((uint64_t)n_ent), st, &in_b, nullptr));
+  const uint64_t* ks = in_b ? k2 : k1;
+  const uint32_t* vs = in_b ? v2 : v1;
+  fold_reduce_kernel<<<nblk(n, 256), 256, 0, st>>>(ks, vs, d_code, d_present, n_keys, n, seg_first, seg_last, last_set,
+                                                   last_del, win);
+  fold_finish_kernel<<<nblk(n_ent, 256), 256, 0, st>>>(vs, d_code, d_time, seg_first, seg_last, last_set, last_del, win,
+                                                       n_keys, n_ent, d_exists, d_fus, d_lus, d_win);
+  CK0(cudaGetLastError());
+  CK0(cudaMemcpyAsync(out_first_event, d_first, 8 * ne, cudaMemcpyDeviceToHost, st));
+  CK0(cudaMemcpyAsync(out_exists, d_exists, ne, cudaMemcpyDeviceToHost, st));
+  CK0(cudaMemcpyAsync(out_first_us, d_fus, 8 * ne, cudaMemcpyDeviceToHost, st));
+  CK0(cudaMemcpyAsync(out_last_us, d_lus, 8 * ne, cudaMemcpyDeviceToHost, st));
+  if (nk) CK0(cudaMemcpyAsync(out_winner, d_win, 8 * ne * nk, cudaMemcpyDeviceToHost, st));
+  CK0(cudaStreamSynchronize(st));
+  *out_n_entities = n_ent;
   return PIO_ALS_OK;
 }
 

@@ -32,7 +32,7 @@ EXPORTED_SYMBOLS = [
     "pio_als_set_init", "pio_als_run", "pio_als_get_factors", "pio_als_train", "pio_als_recommend",
     "pio_als_similar", "pio_als_similar_batch", "pio_als_model_import", "pio_als_save", "pio_als_load", "pio_als_get_stats", "pio_als_get_phase_ms",
     "pio_als_synth_ratings_device", "pio_nb_train", "pio_nb_predict", "pio_ids_encode", "pio_cooc_train",
-    "pio_events_scan",
+    "pio_events_scan", "pio_events_scan_keys", "pio_events_fold",
 ]
 
 
@@ -395,11 +395,29 @@ class EventsFilter(C.Structure):
     ]
 
 
+EVENTS_MAX_KEYS = 8
+
+
 def events_scan(text, entity_type=None, event_names=None, target_mode=EVENTS_TARGET_ANY, target_entity_type=None,
                 prop=None, start_us=None, until_us=None, device=0):
     """pio_events_scan over one buffer of complete JSON lines (bytes / uint8 array).  Returns a dict of numpy columns:
     line, code, value, flags, time_us, eid_bytes/eid_off, tid_bytes/tid_off (matched events, line order), fb_line,
     fb_begin, fb_end (lines the caller parses) and n_lines."""
+    return _events_scan(text, entity_type, event_names, target_mode, target_entity_type, prop, start_us, until_us,
+                        device, None)
+
+
+def events_scan_keys(text, keys, entity_type=None, event_names=None, target_mode=EVENTS_TARGET_ANY,
+                     target_entity_type=None, start_us=None, until_us=None, device=0):
+    """pio_events_scan_keys: events_scan's columns plus, per matched event, the top-level `properties` keys `keys`:
+    present / number (uint8 bit masks, bit q = keys[q]), num (float64 [n, n_keys]) and the raw JSON tokens as a string
+    column tok_bytes / tok_off with n_keys slots per event (slot e * n_keys + q)."""
+    return _events_scan(text, entity_type, event_names, target_mode, target_entity_type, None, start_us, until_us,
+                        device, list(keys))
+
+
+def _events_scan(text, entity_type, event_names, target_mode, target_entity_type, prop, start_us, until_us, device,
+                 keys):
     buf = np.frombuffer(text, np.uint8) if isinstance(text, (bytes, bytearray, memoryview)) else \
         np.ascontiguousarray(text, np.uint8)
     n = int(buf.shape[0])
@@ -419,16 +437,28 @@ def events_scan(text, entity_type=None, event_names=None, target_mode=EVENTS_TAR
                flags=np.empty(cap, np.uint8), time_us=np.empty(cap, np.int64), eid_bytes=np.empty(max(n, 1), np.uint8),
                eid_off=np.empty(cap + 1, np.int64), tid_bytes=np.empty(max(n, 1), np.uint8),
                tid_off=np.empty(cap + 1, np.int64))
+    cols = [("line", C.c_int64), ("code", C.c_int32), ("value", C.c_double), ("flags", C.c_uint8),
+            ("time_us", C.c_int64), ("eid_bytes", C.c_uint8), ("eid_off", C.c_int64), ("tid_bytes", C.c_uint8),
+            ("tid_off", C.c_int64)]
+    nk = 0 if keys is None else len(keys)
+    if keys is not None:
+        kb = [k.encode("utf-8") if isinstance(k, str) else k for k in keys]
+        kp = (C.c_char_p * max(nk, 1))(*kb)
+        out.update(present=np.empty(cap, np.uint8), number=np.empty(cap, np.uint8), num=np.empty((cap, max(nk, 1))),
+                   tok_bytes=np.empty(max(n, 1), np.uint8), tok_off=np.empty(cap * max(nk, 1) + 1, np.int64))
+        cols += [("present", C.c_uint8), ("number", C.c_uint8), ("num", C.c_double), ("tok_bytes", C.c_uint8),
+                 ("tok_off", C.c_int64)]
     fb_cap = max(1024, n // 4096)
     n_ev, n_fb, n_lines = C.c_int64(0), C.c_int64(0), C.c_int64(0)
     while True:
         fb = [np.empty(fb_cap, np.int64) for _ in range(3)]
-        rc = lib().pio_events_scan(
-            C.c_int(device), _ptr(buf, C.c_uint8) if n else None, C.c_int64(n), C.byref(f), C.c_int64(cap),
-            *[_ptr(out[k], t) for k, t in (("line", C.c_int64), ("code", C.c_int32), ("value", C.c_double),
-                                           ("flags", C.c_uint8), ("time_us", C.c_int64), ("eid_bytes", C.c_uint8),
-                                           ("eid_off", C.c_int64), ("tid_bytes", C.c_uint8), ("tid_off", C.c_int64))],
-            C.byref(n_ev), C.c_int64(fb_cap), *[_ptr(a, C.c_int64) for a in fb], C.byref(n_fb), C.byref(n_lines))
+        head = (C.c_int(device), _ptr(buf, C.c_uint8) if n else None, C.c_int64(n), C.byref(f))
+        tail = (C.byref(n_ev), C.c_int64(fb_cap), *[_ptr(a, C.c_int64) for a in fb], C.byref(n_fb), C.byref(n_lines))
+        if keys is None:
+            rc = lib().pio_events_scan(*head, C.c_int64(cap), *[_ptr(out[k], t) for k, t in cols], *tail)
+        else:
+            rc = lib().pio_events_scan_keys(*head, kp, C.c_int(nk), C.c_int64(cap),
+                                            *[_ptr(out[k], t) for k, t in cols], *tail)
         if rc != 0:
             raise NativeError(rc, lib().pio_als_last_error(None).decode())
         if n_fb.value <= fb_cap:
@@ -440,7 +470,36 @@ def events_scan(text, entity_type=None, event_names=None, target_mode=EVENTS_TAR
     res["eid_bytes"], res["tid_bytes"] = out["eid_bytes"][:res["eid_off"][-1]], out["tid_bytes"][:res["tid_off"][-1]]
     res["fb_line"], res["fb_begin"], res["fb_end"] = (a[:n_fb.value] for a in fb)
     res["n_lines"] = n_lines.value
+    if keys is not None:
+        res["present"], res["number"], res["num"] = out["present"][:m], out["number"][:m], out["num"][:m, :nk]
+        res["tok_off"] = out["tok_off"][:m * nk + 1]
+        res["tok_bytes"] = out["tok_bytes"][:res["tok_off"][-1]]
     return res
+
+
+def events_fold(eid, code, time_us, present=None, n_keys=0, device=0):
+    """pio_events_fold: LEventAggregator's fold of $set (code 0) / $unset (1) / $delete (2) events in file order, per
+    entity in order of first occurrence.  eid: (bytes uint8[], offsets int64[n + 1]).  Returns a dict: first_event,
+    exists (bool), first_us, last_us, winner (int64 [n_entities, n_keys], -1 = key absent)."""
+    buf = np.ascontiguousarray(eid[0], np.uint8)
+    off = np.ascontiguousarray(eid[1], np.int64)
+    code = np.ascontiguousarray(code, np.int32)
+    time_us = np.ascontiguousarray(time_us, np.int64)
+    n = int(code.shape[0])
+    pm = None if present is None else np.ascontiguousarray(present, np.uint8)
+    first, exists = np.empty(max(n, 1), np.int64), np.empty(max(n, 1), np.uint8)
+    fus, lus = np.empty(max(n, 1), np.int64), np.empty(max(n, 1), np.int64)
+    win = np.empty((max(n, 1), max(int(n_keys), 1)), np.int64)
+    ne = C.c_int64(0)
+    rc = lib().pio_events_fold(C.c_int(device), _ptr(buf, C.c_uint8) if buf.size else None, _ptr(off, C.c_int64),
+                               _ptr(code, C.c_int32), _ptr(time_us, C.c_int64), _ptr(pm, C.c_uint8), C.c_int64(n),
+                               C.c_int(int(n_keys)), _ptr(first, C.c_int64), _ptr(exists, C.c_uint8), _ptr(fus, C.c_int64),
+                               _ptr(lus, C.c_int64), _ptr(win, C.c_int64), C.byref(ne))
+    if rc != 0:
+        raise NativeError(rc, lib().pio_als_last_error(None).decode())
+    g = ne.value
+    return dict(first_event=first[:g], exists=exists[:g].astype(bool), first_us=fus[:g], last_us=lus[:g],
+                winner=win[:g, :int(n_keys)])
 
 
 def events_scan_timing() -> dict:

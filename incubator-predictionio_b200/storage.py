@@ -408,6 +408,18 @@ class PEventStore:
                              channelName, sc, chunk_bytes or FIND_COLUMNS_CHUNK)
 
     @staticmethod
+    def aggregatePropertyColumns(appName: str, entityType: str, keys: Sequence[str],
+                                 required: Optional[Sequence[str]] = None, startTime=None, untilTime=None,
+                                 channelName: Optional[str] = None, sc=None, chunk_bytes: int = None
+                                 ) -> "PropertyColumns":
+        """aggregateProperties restricted to the properties `keys`, as columns (PropertyColumns): the same entities in
+        the same order, `required` applied.  The $set / $unset / $delete events are scanned on the GPU
+        (native.events_scan_keys) and folded there (native.events_fold); raises what `find` raises on the first bad
+        line.  At most 8 keys and required keys together.  Needs the CUDA library."""
+        return _aggregate_property_columns(appName, entityType, keys, required, startTime, untilTime, channelName, sc,
+                                           chunk_bytes or FIND_COLUMNS_CHUNK)
+
+    @staticmethod
     def aggregateProperties(appName: str, entityType: str, channelName: Optional[str] = None, startTime=None,
                             untilTime=None, required: Optional[Sequence[str]] = None, sc=None
                             ) -> List[Tuple[str, PropertyMap]]:
@@ -487,9 +499,8 @@ class EventColumns:
                             self.n_fallback)
 
 
-def _host_columns(lines, names, appName, entityType, eventNames, targetEntityType, prop, startTime, untilTime):
-    """Fallback lines (line index, bytes): the code `find` runs, producing column entries."""
-    rows = []
+def _host_events(lines, names, entityType, targetEntityType, startTime, untilTime) -> Iterator[Tuple[int, Event]]:
+    """Fallback lines (line index, bytes) through the code `find` runs: the matched events with their line index."""
     for ln, raw in lines:
         text = raw.decode("utf-8").strip()
         if not text:
@@ -505,6 +516,13 @@ def _host_columns(lines, names, appName, entityType, eventNames, targetEntityTyp
             continue
         if targetEntityType is not _UNSET and e.targetEntityType != targetEntityType:
             continue
+        yield ln, e
+
+
+def _host_columns(lines, names, appName, entityType, eventNames, targetEntityType, prop, startTime, untilTime):
+    """Fallback lines (line index, bytes): the code `find` runs, producing column entries."""
+    rows = []
+    for ln, e in _host_events(lines, names, entityType, targetEntityType, startTime, untilTime):
         has, v, bad = False, 0.0, _UNSET
         if prop is not None and e.properties.contains(prop):
             raw_v = e.properties.fields[prop]
@@ -534,22 +552,13 @@ def _columns_from_rows(rows) -> Tuple[Dict[str, np.ndarray], Dict[int, Any]]:
 FIND_COLUMNS_CHUNK = 256 << 20
 
 
-def _find_columns(appName, entityType=None, eventNames=None, targetEntityType=_UNSET, property=None, startTime=None,
-                  untilTime=None, channelName=None, sc=None, chunk_bytes=FIND_COLUMNS_CHUNK) -> EventColumns:
-    from . import native
+def _scan_file(appName, channelName, scan, chunk_bytes):
+    """The app's event file, read in pieces of complete lines (about chunk_bytes each) that `scan` (a native.events_scan
+    call on a memoryview) reads in place.  Returns the scan results with file-wide line numbers, and the fallback lines
+    as (line index, bytes) in line order."""
     p = app_file(appName, channelName)
     if not p.exists():
         raise FileNotFoundError(f"Invalid app name {appName}: no event data at {p}")  # Common.appNameToId
-    names = None if eventNames is None else set(eventNames)
-    if targetEntityType is _UNSET:
-        mode, tet = native.EVENTS_TARGET_ANY, None
-    elif targetEntityType is None:
-        mode, tet = native.EVENTS_TARGET_ABSENT, None
-    else:
-        mode, tet = native.EVENTS_TARGET_EQUALS, targetEntityType
-    s_us = None if startTime is None else time_us(_parse_time(startTime))
-    u_us = None if untilTime is None else time_us(_parse_time(untilTime))
-    device = getattr(sc, "device", 0) or 0
     parts, host_lines, line_base = [], [], 0
     with open(p, "rb") as fh:
         carry = b""
@@ -565,7 +574,7 @@ def _find_columns(appName, entityType=None, eventNames=None, targetEntityType=_U
                 carry = buf[cut:]
             if cut:
                 view = memoryview(buf)[:cut]      # the scan reads the piece in place
-                r = native.events_scan(view, entityType, eventNames, mode, tet, property, s_us, u_us, device)
+                r = scan(view)
                 r["line"] += line_base
                 parts.append(r)
                 host_lines.extend((int(ln) + line_base, bytes(view[b:e])) for ln, b, e in
@@ -573,6 +582,30 @@ def _find_columns(appName, entityType=None, eventNames=None, targetEntityType=_U
                 line_base += r["n_lines"]
             if not data:
                 break
+    return parts, host_lines
+
+
+def _scan_args(startTime, untilTime, sc):
+    s_us = None if startTime is None else time_us(_parse_time(startTime))
+    u_us = None if untilTime is None else time_us(_parse_time(untilTime))
+    return s_us, u_us, getattr(sc, "device", 0) or 0
+
+
+def _find_columns(appName, entityType=None, eventNames=None, targetEntityType=_UNSET, property=None, startTime=None,
+                  untilTime=None, channelName=None, sc=None, chunk_bytes=FIND_COLUMNS_CHUNK) -> EventColumns:
+    from . import native
+    names = None if eventNames is None else set(eventNames)
+    if targetEntityType is _UNSET:
+        mode, tet = native.EVENTS_TARGET_ANY, None
+    elif targetEntityType is None:
+        mode, tet = native.EVENTS_TARGET_ABSENT, None
+    else:
+        mode, tet = native.EVENTS_TARGET_EQUALS, targetEntityType
+    s_us, u_us, device = _scan_args(startTime, untilTime, sc)
+    parts, host_lines = _scan_file(
+        appName, channelName,
+        lambda view: native.events_scan(view, entityType, eventNames, mode, tet, property, s_us, u_us, device),
+        chunk_bytes)
     rows = _host_columns(host_lines, names, appName, entityType, eventNames, targetEntityType, property, startTime,
                          untilTime)
     dev = dict(line=np.concatenate([r["line"] for r in parts]) if parts else np.zeros(0, np.int64))
@@ -596,6 +629,214 @@ def _find_columns(appName, entityType=None, eventNames=None, targetEntityType=_U
     where[order] = np.arange(order.shape[0])
     return EventColumns(cat["code"], cat["value"], cat["has_value"], cat["time_us"], eid, tid, cat["has_target"],
                         {int(where[nd + j]): v for j, v in bad.items()}, len(host_lines))
+
+
+def require_values(cols: EventColumns, which: np.ndarray, name: str) -> None:
+    """For the events `which` (bool mask) that must carry a number `name`: the first one without a usable value raises
+    what DataMap.get(name, float) raises on it (absent, null, or not convertible by float())."""
+    unusable = np.flatnonzero(which & ~cols.has_value)
+    if unusable.size:
+        k = int(unusable[0])
+        DataMap({name: cols.bad_value[k]} if k in cols.bad_value else {}).get(name, float)
+
+
+@dataclass
+class PropertyColumns:
+    """aggregateProperties restricted to some keys (PEventStore.aggregatePropertyColumns), one row per entity in the
+    order aggregateProperties lists them.  `entityId` is a (UTF-8 bytes, offsets) column; first_us / last_us are
+    time_us(firstUpdated / lastUpdated).  Per key q of `keys`: present[:, q] (the key is in the PropertyMap, a null
+    value included), has_number[:, q] / number[:, q] (the value is a JSON number and number = float(value); False for
+    an integer beyond 2^53 and for a number the device scan could not convert exactly), and `value` / `values` give
+    the Python value itself."""
+    keys: List[str]
+    entityId: Tuple[np.ndarray, np.ndarray]
+    first_us: np.ndarray          # int64
+    last_us: np.ndarray           # int64
+    present: np.ndarray           # bool [n, n_keys]
+    has_number: np.ndarray        # bool [n, n_keys]
+    number: np.ndarray            # float64 [n, n_keys]
+    token: Tuple[np.ndarray, np.ndarray]   # raw JSON token of (row i, key q) at slot i * n_keys + q; empty: see `value`
+    host_value: Dict[Tuple[int, int], Any] = field(default_factory=dict)   # values read from lines parsed on the host
+    n_fallback: int = 0           # lines parsed on the host
+
+    def __len__(self) -> int:
+        return int(self.first_us.shape[0])
+
+    def entity_ids(self) -> List[str]:
+        return string_list(self.entityId)
+
+    def values(self, key: str) -> List[Any]:
+        """The Python value of `key` for every row (None where absent): json.loads of its token, the number, or the
+        value of a line parsed on the host."""
+        q, nk = self.keys.index(key), len(self.keys)
+        buf, off = self.token
+        raw = buf.tobytes()
+        out = []
+        for i in range(len(self)):
+            if not self.present[i, q]:
+                out.append(None)
+            elif (i, q) in self.host_value:
+                out.append(self.host_value[(i, q)])
+            else:
+                b, e = off[i * nk + q], off[i * nk + q + 1]
+                out.append(json.loads(raw[b:e]) if e > b else float(self.number[i, q]))
+        return out
+
+    def value(self, i: int, key: str):
+        q, nk = self.keys.index(key), len(self.keys)
+        if not self.present[i, q]:
+            return None
+        if (i, q) in self.host_value:
+            return self.host_value[(i, q)]
+        buf, off = self.token
+        b, e = off[i * nk + q], off[i * nk + q + 1]
+        return json.loads(buf[b:e].tobytes()) if e > b else float(self.number[i, q])
+
+
+def _as_number(v) -> Tuple[bool, float]:
+    """(has_number, number) of a value parsed on the host, as the device reports them: a float, or an integer exact in
+    double."""
+    if isinstance(v, float):
+        return True, v
+    if isinstance(v, int) and not isinstance(v, bool) and abs(v) <= 2 ** 53:
+        return True, float(v)
+    return False, 0.0
+
+
+FOLD_EVENTS = ["$set", "$unset", "$delete"]   # event codes 0 / 1 / 2 of native.events_fold
+
+
+def _aggregate_property_columns(appName, entityType, keys, required, startTime, untilTime, channelName, sc,
+                                chunk_bytes) -> PropertyColumns:
+    from . import native
+    keys = list(keys)
+    required = list(required or [])
+    scan_keys = keys + [r for r in dict.fromkeys(required) if r not in keys]
+    if not 1 <= len(scan_keys) <= native.EVENTS_MAX_KEYS or len(set(keys)) != len(keys) or not all(scan_keys):
+        raise ValueError(f"aggregatePropertyColumns: 1 to {native.EVENTS_MAX_KEYS} distinct non-empty keys "
+                         f"(required ones included), got {scan_keys}")
+    nk = len(scan_keys)
+    s_us, u_us, device = _scan_args(startTime, untilTime, sc)
+    parts, host_lines = _scan_file(
+        appName, channelName,
+        lambda view: native.events_scan_keys(view, scan_keys, entityType, FOLD_EVENTS, native.EVENTS_TARGET_ANY, None,
+                                             s_us, u_us, device),
+        chunk_bytes)
+    cat = lambda k, t: np.concatenate([r[k] for r in parts]).astype(t, copy=False) if parts else np.zeros(0, t)  # noqa: E731
+    d_line, d_code, d_time, d_present = cat("line", np.int64), cat("code", np.int32), cat("time_us", np.int64), \
+        cat("present", np.uint8)
+    d_number = cat("number", np.uint8)
+    d_num = np.concatenate([r["num"] for r in parts]) if parts else np.zeros((0, nk))
+    d_eid = concat_strings([(r["eid_bytes"], r["eid_off"]) for r in parts])
+    d_tok = concat_strings([(r["tok_bytes"], r["tok_off"]) for r in parts])
+    # fallback lines: the code find runs, merged by line index
+    enc = lambda x: x.encode("utf-8", "surrogatepass")  # noqa: E731
+    h_line, h_code, h_time, h_present, h_eid, h_vals = [], [], [], [], [], []
+    for ln, e in _host_events(host_lines, set(FOLD_EVENTS), entityType, _UNSET, startTime, untilTime):
+        f = e.properties.fields
+        h_line.append(ln)
+        h_code.append(FOLD_EVENTS.index(e.event))
+        h_time.append(time_us(e.eventTime))
+        h_present.append(sum(1 << q for q, k in enumerate(scan_keys) if k in f))
+        h_eid.append(enc(e.entityId))
+        h_vals.append({q: f[k] for q, k in enumerate(scan_keys) if k in f})
+    nd = d_line.shape[0]
+    if h_line:
+        h_off = np.zeros(len(h_eid) + 1, np.int64)
+        np.cumsum([len(b) for b in h_eid], out=h_off[1:])
+        order = np.argsort(np.concatenate([d_line, np.array(h_line, np.int64)]), kind="stable")
+        code = np.concatenate([d_code, np.array(h_code, np.int32)])[order]
+        t_us = np.concatenate([d_time, np.array(h_time, np.int64)])[order]
+        present = np.concatenate([d_present, np.array(h_present, np.uint8)])[order]
+        eid = take_strings(*concat_strings([d_eid, (np.frombuffer(b"".join(h_eid), np.uint8).copy(), h_off)]), order)
+    else:
+        order, code, t_us, present, eid = np.arange(nd), d_code, d_time, d_present, d_eid
+    f = native.events_fold(eid, code, t_us, present, nk, device)
+    win = f["winner"]
+    keep = f["exists"] & (win[:, len(keys):] >= 0).all(axis=1)   # required keys: present, even if null
+    keep &= (win[:, [scan_keys.index(r) for r in required if r in keys]] >= 0).all(axis=1)
+    rows = np.flatnonzero(keep)
+    win = win[rows][:, :len(keys)]
+    n, k = rows.shape[0], len(keys)
+    present_k = win >= 0
+    src = np.where(present_k, order[np.maximum(win, 0)], -1)      # event in the scan (< nd) or fallback row (>= nd)
+    dev = present_k & (src < nd)
+    ds = np.where(dev, src, 0)
+    has_number = dev & (((d_number[ds] if nd else np.zeros_like(ds, np.uint8)) >> np.arange(k)) & 1).astype(bool)
+    number = np.where(has_number, d_num[ds, np.arange(k)] if nd else 0.0, 0.0)
+    slots = np.where(dev, ds * nk + np.arange(k), 0).reshape(-1)
+    tb, to = take_strings(*d_tok, slots) if nd else (np.zeros(0, np.uint8), np.zeros(n * k + 1, np.int64))
+    lens = np.where(dev.reshape(-1), to[1:] - to[:-1], 0)          # only winners scanned on the device carry tokens
+    keep_b = np.repeat(dev.reshape(-1), to[1:] - to[:-1])
+    tok_off = np.zeros(n * k + 1, np.int64)
+    np.cumsum(lens, out=tok_off[1:])
+    host_value = {}
+    for i, q in zip(*np.nonzero(present_k & ~dev)):
+        v = h_vals[int(src[i, q]) - nd][int(q)]
+        host_value[(int(i), int(q))] = v
+        has_number[i, q], number[i, q] = _as_number(v)
+    return PropertyColumns(keys, take_strings(*eid, f["first_event"][rows]), f["first_us"][rows], f["last_us"][rows],
+                           present_k, has_number, number, (tb[keep_b], tok_off), host_value, len(host_lines))
+
+
+def event_millis(t_us) -> np.ndarray:
+    """int(e.eventTime.timestamp() * 1000) of every event: (time_us / 10^6) * 1000 in float64, truncated toward zero
+    (not time_us // 1000, which differs for negative times and for some microsecond values)."""
+    t = np.asarray(t_us, np.int64)
+    ms = np.trunc(t.astype(np.float64) / 1e6 * 1000.0).astype(np.int64)
+    for k in np.flatnonzero(np.abs(t) > 2 ** 53):   # float64(t) would round first; Python divides the integers exactly
+        ms[k] = int(int(t[k]) / 10 ** 6 * 1000)
+    return ms
+
+
+def index_in(keys: Tuple[np.ndarray, np.ndarray], ids: Tuple[np.ndarray, np.ndarray], device: int = 0) -> np.ndarray:
+    """BiMap(keys -> position).getOrElse(id, -1) for every id, with one native.ids_encode over keys ++ ids: the n distinct
+    keys take codes 0 .. n - 1, and an id with a code >= n is not among them."""
+    from . import native
+    n = keys[1].shape[0] - 1
+    code, _ = native.ids_encode(concat_strings([keys, ids]), device)
+    out = code[n:].astype(np.int32)
+    out[out >= n] = -1
+    return out
+
+
+@dataclass
+class EntityEventColumns:
+    """What a template DataSource reads as columns: the aggregated users and items (PropertyColumns, items with a
+    "categories" key) and the user-to-item events (EventColumns, `code` = index of the event name).  The BiMaps and
+    event indices the algorithms need are computed once and kept."""
+    users: PropertyColumns
+    items: PropertyColumns
+    events: EventColumns
+    device: int = 0
+    _cache: Dict[str, Any] = field(default_factory=dict, repr=False)
+
+    def _once(self, key, make):
+        if key not in self._cache:
+            self._cache[key] = make()
+        return self._cache[key]
+
+    def millis(self) -> np.ndarray:
+        return self._once("t", lambda: event_millis(self.events.time_us))
+
+    def user_map(self) -> BiMap:
+        return self._once("um", lambda: BiMap({k: j for j, k in enumerate(self.users.entity_ids())}))
+
+    def item_map(self) -> BiMap:
+        return self._once("im", lambda: BiMap({k: j for j, k in enumerate(self.items.entity_ids())}))
+
+    def categories(self) -> List[Any]:
+        """pm.getOpt("categories") of every item: its JSON value, None when absent or null."""
+        return self._once("cat", lambda: self.items.values("categories"))
+
+    def event_users(self) -> np.ndarray:
+        """userMap.getOrElse(e.user, -1) per event."""
+        return self._once("eu", lambda: index_in(self.users.entityId, self.events.entityId, self.device))
+
+    def event_items(self) -> np.ndarray:
+        """itemMap.getOrElse(e.item, -1) per event (-1 also without a targetEntityId)."""
+        return self._once("ei", lambda: np.where(self.events.has_target, index_in(
+            self.items.entityId, self.events.targetEntityId, self.device), -1).astype(np.int32))
 
 
 class LEventStore:

@@ -13,7 +13,7 @@ import numpy as np
 
 from ..controller import Engine, EngineFactory, IdentityPreparator, LFirstServing, P2LAlgorithm, Params, PDataSource
 from ..mllib import NaiveBayes, NaiveBayesModel
-from ..storage import PEventStore
+from ..storage import DataMap, PEventStore
 
 
 @dataclass
@@ -43,12 +43,17 @@ class DataSource(PDataSource):
         self.dsp = dsp
 
     def readTraining(self, sc) -> TrainingData:
-        rows = PEventStore.aggregateProperties(self.dsp.appName, "user", required=["plan", "attr0", "attr1", "attr2"],
-                                               sc=sc)
-        labels = np.array([pm.get("plan", float) for _, pm in rows], np.float64)
-        feats = np.array([[pm.get("attr0", float), pm.get("attr1", float), pm.get("attr2", float)] for _, pm in rows],
-                         np.float32).reshape(-1, 3)
-        return TrainingData(labels, feats)
+        """plan -> label, attr0..2 -> features of every user that has all four, scanned and folded on the GPU
+        (PEventStore.aggregatePropertyColumns).  Numbers come straight from the number columns; any other value goes
+        through DataMap.get(name, float), in the order the host path reads them: every plan first, then the attributes
+        row by row, so the first bad value raises the same exception."""
+        keys = ["plan", "attr0", "attr1", "attr2"]
+        pc = PEventStore.aggregatePropertyColumns(self.dsp.appName, "user", keys, required=keys, sc=sc)
+        x = pc.number.copy()
+        for i, q in [(i, 0) for i in np.flatnonzero(~pc.has_number[:, 0])] + \
+                [(i, q + 1) for i, q in np.argwhere(~pc.has_number[:, 1:])]:
+            x[i, q] = DataMap({keys[q]: pc.value(int(i), keys[q])}).get(keys[q], float)
+        return TrainingData(x[:, 0].astype(np.float64), x[:, 1:].astype(np.float32).reshape(-1, 3))
 
 
 @dataclass

@@ -18,7 +18,7 @@ import numpy as np
 from ..controller import (Engine, EngineFactory, LFirstServing, P2LAlgorithm, Params, PDataSource, PersistentModel,
                           IdentityPreparator)
 from ..mllib import ALS, MatrixFactorizationModel
-from ..storage import BiMap, LEventStore, PEventStore
+from ..storage import BiMap, EntityEventColumns, LEventStore, PEventStore, require_values, string_list
 
 
 @dataclass
@@ -66,9 +66,54 @@ class DataSourceParams(Params):
     appName: str
 
 
+RATE, BUY = 0, 1   # event codes of the columns (eventNames order)
+
+
 class TrainingData:
-    def __init__(self, users, items, rateEvents, buyEvents):
-        self.users, self.items, self.rateEvents, self.buyEvents = users, items, rateEvents, buyEvents
+    """users / items / rateEvents / buyEvents as dicts and lists, or as EntityEventColumns (`columns`); the dicts and
+    lists are then built on first use, and ECommAlgorithm trains from the columns."""
+
+    def __init__(self, users=None, items=None, rateEvents=None, buyEvents=None,
+                 columns: Optional[EntityEventColumns] = None):
+        self._users, self._items, self._rateEvents, self._buyEvents = users, items, rateEvents, buyEvents
+        self.columns = columns
+
+    @property
+    def users(self):
+        if self._users is None:
+            self._users = {k: True for k in self.columns.users.entity_ids()}
+        return self._users
+
+    @property
+    def items(self):
+        if self._items is None:
+            c = self.columns
+            self._items = {k: Item(v) for k, v in zip(c.items.entity_ids(), c.categories())}
+        return self._items
+
+    def _events(self):
+        ev = self.columns.events
+        users, items, t = string_list(ev.entityId), string_list(ev.targetEntityId), self.columns.millis().tolist()
+        rates, buys = [], []
+        for k, (code, has, v) in enumerate(zip(ev.code.tolist(), ev.has_target.tolist(), ev.value.tolist())):
+            item = items[k] if has else None
+            if code == RATE:
+                rates.append(RateEvent(users[k], item, v, t[k]))
+            else:
+                buys.append(BuyEvent(users[k], item, t[k]))
+        self._rateEvents, self._buyEvents = rates, buys
+
+    @property
+    def rateEvents(self):
+        if self._rateEvents is None:
+            self._events()
+        return self._rateEvents
+
+    @property
+    def buyEvents(self):
+        if self._buyEvents is None:
+            self._events()
+        return self._buyEvents
 
 
 PreparedData = TrainingData
@@ -79,19 +124,16 @@ class DataSource(PDataSource):
         self.dsp = dsp
 
     def readTraining(self, sc) -> TrainingData:
-        users = {k: True for k, _ in PEventStore.aggregateProperties(self.dsp.appName, "user", sc=sc)}
-        items = {k: Item(pm.getOpt("categories"))
-                 for k, pm in PEventStore.aggregateProperties(self.dsp.appName, "item", sc=sc)}
-        evs = PEventStore.find(self.dsp.appName, entityType="user", eventNames=["rate", "buy"],
-                               targetEntityType="item", sc=sc)
-        rates, buys = [], []
-        for e in evs:
-            t = int(e.eventTime.timestamp() * 1000)
-            if e.event == "rate":
-                rates.append(RateEvent(e.entityId, e.targetEntityId, e.properties.get("rating", float), t))
-            else:
-                buys.append(BuyEvent(e.entityId, e.targetEntityId, t))
-        return TrainingData(users, items, rates, buys)
+        """The users, the items with their categories, and the rate / buy events, scanned and folded on the GPU
+        (PEventStore.aggregatePropertyColumns, PEventStore.findColumns).  A rate event without a usable rating raises
+        what e.properties.get("rating", float) raises."""
+        app = self.dsp.appName
+        users = PEventStore.aggregatePropertyColumns(app, "user", ["categories"], sc=sc)   # only the ids are used
+        items = PEventStore.aggregatePropertyColumns(app, "item", ["categories"], sc=sc)
+        evs = PEventStore.findColumns(app, entityType="user", eventNames=["rate", "buy"], targetEntityType="item",
+                                      property="rating", sc=sc)
+        require_values(evs, evs.code == RATE, "rating")
+        return TrainingData(columns=EntityEventColumns(users, items, evs, getattr(sc, "device", 0) or 0))
 
 
 @dataclass
@@ -143,30 +185,46 @@ class ECommAlgorithm(P2LAlgorithm):
         self.ap = ap
 
     def train(self, sc, data: PreparedData) -> ECommModel:
-        for name, coll in (("rateEvents", data.rateEvents), ("users", data.users), ("items", data.items)):
-            if not coll:
+        c = data.columns if data._users is None and data._rateEvents is None else None   # None: built from lists
+        sizes = None if c is None else (int((c.events.code == RATE).sum()), len(c.users), len(c.items))
+        for k, (name, coll) in enumerate((("rateEvents", lambda: data.rateEvents), ("users", lambda: data.users),
+                                          ("items", lambda: data.items))):
+            if not (coll() if c is None else sizes[k]):
                 raise ValueError(f"requirement failed: {name} in PreparedData cannot be empty.")
-        userMap = BiMap.stringInt(data.users.keys())
-        itemMap = BiMap.stringInt(data.items.keys())
-        us, its, vs, ts = [], [], [], []
-        for r in data.rateEvents:  # genMLlibRating: drop unknown ids; latest rating of a pair wins (on the GPU)
-            u, i = userMap.getOrElse(r.user, -1), itemMap.getOrElse(r.item, -1)
-            if u != -1 and i != -1:
-                us.append(u); its.append(i); vs.append(r.rating); ts.append(r.t)
-        if not us:
+        if c is None:
+            userMap = BiMap.stringInt(data.users.keys())
+            itemMap = BiMap.stringInt(data.items.keys())
+            us, its, vs, ts = [], [], [], []
+            for r in data.rateEvents:  # genMLlibRating: drop unknown ids; latest rating of a pair wins (on the GPU)
+                u, i = userMap.getOrElse(r.user, -1), itemMap.getOrElse(r.item, -1)
+                if u != -1 and i != -1:
+                    us.append(u); its.append(i); vs.append(r.rating); ts.append(r.t)
+            coo = (np.array(us, np.int32), np.array(its, np.int32), np.array(vs, np.float32), np.array(ts, np.int64))
+        else:
+            userMap, itemMap = c.user_map(), c.item_map()
+            eu, ei = c.event_users(), c.event_items()
+            keep = (c.events.code == RATE) & (eu >= 0) & (ei >= 0)
+            coo = (eu[keep], ei[keep], c.events.value[keep].astype(np.float32), c.millis()[keep])
+        if not coo[0].size:
             raise ValueError("requirement failed: mllibRatings cannot be empty. Please check if your events contain "
                              "valid user and item ID.")
-        coo = (np.array(us, np.int32), np.array(its, np.int32), np.array(vs, np.float32), np.array(ts, np.int64))
         seed = sc.agree_seed(self.ap.seed) if hasattr(sc, "agree_seed") else (self.ap.seed or 0)
         kw = dict(rank=self.ap.rank, iterations=self.ap.numIterations, lambda_=self.ap.lambda_, blocks=-1, seed=seed,
                   dedup="keep_last", n_users=userMap.size, n_products=itemMap.size, sc=sc)
         m = ALS.trainImplicit(coo, alpha=1.0, **kw) if self.ap.implicitPrefs else ALS.train(coo, **kw)
-        items = {itemMap(k): v for k, v in data.items.items()}
         popular: Dict[int, int] = {}
-        for b in data.buyEvents:  # trainDefault
-            u, i = userMap.getOrElse(b.user, -1), itemMap.getOrElse(b.item, -1)
-            if u != -1 and i != -1:
-                popular[i] = popular.get(i, 0) + 1
+        if c is None:
+            items = {itemMap(k): v for k, v in data.items.items()}
+            for b in data.buyEvents:  # trainDefault
+                u, i = userMap.getOrElse(b.user, -1), itemMap.getOrElse(b.item, -1)
+                if u != -1 and i != -1:
+                    popular[i] = popular.get(i, 0) + 1
+        else:
+            items = {k: Item(v) for k, v in enumerate(c.categories())}
+            bought = ei[(c.events.code == BUY) & (eu >= 0) & (ei >= 0)]
+            counts = np.bincount(bought, minlength=itemMap.size)
+            _, first = np.unique(bought, return_index=True)   # in order of the first buy, as the loop above fills it
+            popular = {int(i): int(counts[i]) for i in bought[np.sort(first)]}
         return ECommModel(m, userMap, itemMap, items, popular)
 
     # -- serving -------------------------------------------------------------------------------

@@ -18,7 +18,7 @@ from .. import native
 from ..controller import (Engine, EngineFactory, LServing, PAlgorithm, Params, PDataSource, PersistentModel,
                           PPreparator, SanityCheck)
 from ..mllib import ALS, MatrixFactorizationModel
-from ..storage import BiMap, DataMap, PEventStore, string_list, take_strings
+from ..storage import BiMap, PEventStore, require_values, string_list, take_strings
 
 
 @dataclass
@@ -121,10 +121,7 @@ class DataSource(PDataSource):
         cols = PEventStore.findColumns(appName=self.dsp.appName, entityType="user", eventNames=["rate", "buy"],
                                        targetEntityType="item", property="rating", sc=sc)
         is_rate = cols.code == 0
-        unusable = np.flatnonzero(is_rate & ~cols.has_value)
-        if unusable.size:   # the first rate event without a usable rating raises what e.properties.get(...) raises
-            k = int(unusable[0])
-            DataMap({"rating": cols.bad_value[k]} if k in cols.bad_value else {}).get("rating", float)
+        require_values(cols, is_rate, "rating")   # what e.properties.get("rating", float) raises on the first bad one
         value = np.where(is_rate, cols.value, 4.0)  # map buy event to rating value of 4
         return RatingColumns(cols.entityId, cols.targetEntityId, value, cols.has_target)
 

@@ -18,7 +18,7 @@ import numpy as np
 from ..controller import (Engine, EngineFactory, LServing, P2LAlgorithm, Params, PDataSource, PersistentModel,
                           PPreparator)
 from ..mllib import ALS, MatrixFactorizationModel
-from ..storage import BiMap, PEventStore
+from ..storage import BiMap, EntityEventColumns, PEventStore, string_list, take_strings
 
 
 @dataclass
@@ -72,13 +72,63 @@ class LikeEvent:
     like: bool
 
 
+VIEW, LIKE, DISLIKE = 0, 1, 2   # event codes of the columns (eventNames order)
+
+
 class TrainingData:
-    def __init__(self, users: Dict[str, User], items: Dict[str, Item], viewEvents: List[ViewEvent],
-                 likeEvents: List[LikeEvent]):
-        self.users, self.items, self.viewEvents, self.likeEvents = users, items, viewEvents, likeEvents
+    """users / items / viewEvents / likeEvents as dicts and lists, or as EntityEventColumns (`columns`); the dicts and
+    lists are then built on first use, and the algorithms train from the columns."""
+
+    def __init__(self, users: Optional[Dict[str, User]] = None, items: Optional[Dict[str, Item]] = None,
+                 viewEvents: Optional[List[ViewEvent]] = None, likeEvents: Optional[List[LikeEvent]] = None,
+                 columns: Optional[EntityEventColumns] = None):
+        self._users, self._items, self._viewEvents, self._likeEvents = users, items, viewEvents, likeEvents
+        self.columns = columns
+
+    @property
+    def users(self) -> Dict[str, User]:
+        if self._users is None:
+            self._users = {k: User() for k in self.columns.users.entity_ids()}
+        return self._users
+
+    @property
+    def items(self) -> Dict[str, Item]:
+        if self._items is None:
+            c = self.columns
+            self._items = {k: Item(categories=v) for k, v in zip(c.items.entity_ids(), c.categories())}
+        return self._items
+
+    def _events(self):
+        ev = self.columns.events
+        users, items, t = string_list(ev.entityId), string_list(ev.targetEntityId), self.columns.millis().tolist()
+        views, likes = [], []
+        for k, (code, has) in enumerate(zip(ev.code.tolist(), ev.has_target.tolist())):
+            item = items[k] if has else None
+            if code == VIEW:
+                views.append(ViewEvent(users[k], item, t[k]))
+            else:
+                likes.append(LikeEvent(users[k], item, t[k], code == LIKE))
+        self._viewEvents, self._likeEvents = views, likes
+
+    @property
+    def viewEvents(self) -> List[ViewEvent]:
+        if self._viewEvents is None:
+            self._events()
+        return self._viewEvents
+
+    @property
+    def likeEvents(self) -> List[LikeEvent]:
+        if self._likeEvents is None:
+            self._events()
+        return self._likeEvents
 
 
 PreparedData = TrainingData
+
+
+def _columns(data: TrainingData) -> Optional[EntityEventColumns]:
+    """The columns an algorithm trains from, or None when `data` was built from lists (the host path)."""
+    return data.columns if data._users is None and data._viewEvents is None else None
 
 
 class DataSource(PDataSource):
@@ -86,19 +136,14 @@ class DataSource(PDataSource):
         self.dsp = dsp
 
     def readTraining(self, sc) -> TrainingData:
-        users = {k: User() for k, _ in PEventStore.aggregateProperties(self.dsp.appName, "user", sc=sc)}
-        items = {k: Item(categories=pm.getOpt("categories"))
-                 for k, pm in PEventStore.aggregateProperties(self.dsp.appName, "item", sc=sc)}
-        evs = PEventStore.find(self.dsp.appName, entityType="user", eventNames=["view", "like", "dislike"],
-                               targetEntityType="item", sc=sc)
-        views, likes = [], []
-        for e in evs:
-            t = int(e.eventTime.timestamp() * 1000)
-            if e.event == "view":
-                views.append(ViewEvent(e.entityId, e.targetEntityId, t))
-            else:
-                likes.append(LikeEvent(e.entityId, e.targetEntityId, t, e.event == "like"))
-        return TrainingData(users, items, views, likes)
+        """The users, the items with their categories, and the view / like / dislike events, scanned and folded on the
+        GPU (PEventStore.aggregatePropertyColumns, PEventStore.findColumns)."""
+        app = self.dsp.appName
+        users = PEventStore.aggregatePropertyColumns(app, "user", ["categories"], sc=sc)   # only the ids are used
+        items = PEventStore.aggregatePropertyColumns(app, "item", ["categories"], sc=sc)
+        evs = PEventStore.findColumns(app, entityType="user", eventNames=["view", "like", "dislike"],
+                                      targetEntityType="item", sc=sc)
+        return TrainingData(columns=EntityEventColumns(users, items, evs, getattr(sc, "device", 0) or 0))
 
 
 class Preparator(PPreparator):
@@ -145,6 +190,11 @@ class ALSModel(PersistentModel):
         return cls(mf, BiMap(json.loads((d / "itemStringIntMap.json").read_text())), items)
 
 
+def _item_index(c: EntityEventColumns) -> Dict[int, Item]:
+    """{itemMap(k): Item(categories)} of the columns: item k of the map is row k of the aggregated items."""
+    return {k: Item(categories=v) for k, v in enumerate(c.categories())}
+
+
 def candidate_mask(n_items: int, items: Dict[int, Item], queryList: Set[int], query: Query,
                    itemStringIntMap: BiMap) -> np.ndarray:
     """isCandidateItem (ALSAlgorithm.scala:237-263) as an exclusion mask (1 = not a candidate); the query items
@@ -185,15 +235,28 @@ class ALSAlgorithm(P2LAlgorithm):
                 its.append(i)
         return np.array(us, np.int32), np.array(its, np.int32), np.ones(len(us), np.float32)
 
+    def _columns_ratings(self, c: EntityEventColumns):
+        """_ratings from the columns: view events of known users and items, in event order."""
+        u, i = c.event_users(), c.event_items()
+        keep = (c.events.code == VIEW) & (u >= 0) & (i >= 0)
+        return u[keep], i[keep], np.ones(int(keep.sum()), np.float32)
+
     def train(self, sc, data: PreparedData) -> ALSModel:
-        for name, coll in (("viewEvents", data.viewEvents), ("users", data.users), ("items", data.items)):
-            if not coll:
+        c = _columns(data)
+        sizes = None if c is None else (int((c.events.code == VIEW).sum()), len(c.users), len(c.items))
+        for k, (name, coll) in enumerate((("viewEvents", lambda: data.viewEvents), ("users", lambda: data.users),
+                                          ("items", lambda: data.items))):
+            if not (coll() if c is None else sizes[k]):
                 raise ValueError(f"requirement failed: {name} in PreparedData cannot be empty. Please check if "
                                  "DataSource generates TrainingData and Preprator generates PreparedData correctly.")
-        userMap = BiMap.stringInt(data.users.keys())
-        itemMap = BiMap.stringInt(data.items.keys())
-        items = {itemMap(k): v for k, v in data.items.items()}
-        u, i, v = self._ratings(data, userMap, itemMap)
+        if c is None:
+            userMap = BiMap.stringInt(data.users.keys())
+            itemMap = BiMap.stringInt(data.items.keys())
+            items = {itemMap(k): v for k, v in data.items.items()}
+            u, i, v = self._ratings(data, userMap, itemMap)
+        else:
+            userMap, itemMap, items = c.user_map(), c.item_map(), _item_index(c)
+            u, i, v = self._columns_ratings(c)
         if u.size == 0:
             raise ValueError("requirement failed: mllibRatings cannot be empty. Please check if your events contain "
                              "valid user and item ID.")
@@ -231,13 +294,23 @@ class LikeAlgorithm(ALSAlgorithm):
                 ts.append(r.t)
         return np.array(us, np.int32), np.array(its, np.int32), np.array(vs, np.float32), np.array(ts, np.int64)
 
+    def _columns_ratings(self, c: EntityEventColumns):
+        u, i, code = c.event_users(), c.event_items(), c.events.code
+        keep = (code != VIEW) & (u >= 0) & (i >= 0)
+        return u[keep], i[keep], np.where(code[keep] == LIKE, 1.0, -1.0).astype(np.float32), c.millis()[keep]
+
     def train(self, sc, data):
-        if not data.likeEvents:
+        c = _columns(data)
+        if not (data.likeEvents if c is None else (c.events.code != VIEW).any()):
             raise ValueError("requirement failed: likeEvents in PreparedData cannot be empty.")
-        userMap = BiMap.stringInt(data.users.keys())
-        itemMap = BiMap.stringInt(data.items.keys())
-        items = {itemMap(k): v for k, v in data.items.items()}
-        u, i, v, ts = self._ratings(data, userMap, itemMap)
+        if c is None:
+            userMap = BiMap.stringInt(data.users.keys())
+            itemMap = BiMap.stringInt(data.items.keys())
+            items = {itemMap(k): v for k, v in data.items.items()}
+            u, i, v, ts = self._ratings(data, userMap, itemMap)
+        else:
+            userMap, itemMap, items = c.user_map(), c.item_map(), _item_index(c)
+            u, i, v, ts = self._columns_ratings(c)
         if u.size == 0:
             raise ValueError("requirement failed: mllibRatings cannot be empty.")
         seed = sc.agree_seed(self.ap.seed) if hasattr(sc, "agree_seed") else (self.ap.seed or 0)
@@ -275,18 +348,27 @@ class CooccurrenceAlgorithm(P2LAlgorithm):
 
     def train(self, sc, data) -> CooccurrenceModel:
         from .. import native
-        itemMap = BiMap.stringInt(data.items.keys())
-        userMap = BiMap.stringInt(e.user for e in data.viewEvents)     # only to index the users of the view events
-        us, its = [], []
-        for e in data.viewEvents:
-            i = itemMap.getOrElse(e.item, -1)
-            if i != -1:
-                us.append(userMap(e.user))
-                its.append(i)
-        items = {itemMap(k): v for k, v in data.items.items()}
+        c = _columns(data)
+        if c is None:
+            itemMap = BiMap.stringInt(data.items.keys())
+            userMap = BiMap.stringInt(e.user for e in data.viewEvents)     # only to index the users of the view events
+            us, its = [], []
+            for e in data.viewEvents:
+                i = itemMap.getOrElse(e.item, -1)
+                if i != -1:
+                    us.append(userMap(e.user))
+                    its.append(i)
+            items = {itemMap(k): v for k, v in data.items.items()}
+            n_users = userMap.size
+        else:   # the users numbered over all view events, as BiMap.stringInt(e.user for e in data.viewEvents)
+            itemMap, items = c.item_map(), _item_index(c)
+            views = np.flatnonzero(c.events.code == VIEW)
+            vu, first = native.ids_encode(take_strings(*c.events.entityId, views), c.device)
+            vi = c.event_items()[views]
+            us, its, n_users = vu[vi >= 0], vi[vi >= 0], first.shape[0]
         n_items = itemMap.size
-        if us:
-            ti, tc, tn = native.cooc_train(np.array(us, np.int32), np.array(its, np.int32), max(userMap.size, 1), n_items,
+        if len(us):
+            ti, tc, tn = native.cooc_train(np.array(us, np.int32), np.array(its, np.int32), max(n_users, 1), n_items,
                                            self.ap.n, device=getattr(sc, "device", 0))
         else:
             ti = np.full((n_items, self.ap.n), -1, np.int32)
