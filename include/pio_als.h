@@ -319,6 +319,52 @@ PIO_API int pio_events_fold(int device, const uint8_t* eid_bytes, const int64_t*
                             int64_t* out_first_event, uint8_t* out_exists, int64_t* out_first_us, int64_t* out_last_us,
                             int64_t* out_winner, int64_t* out_n_entities);
 
+/* Event index: LEventStore.findByEntity (data/src/main/scala/org/apache/predictionio/data/store/LEventStore.scala:76)
+ * for one view -- a `find` filter (entity type, event names, target entity type) -- of an append-only event file, kept
+ * on the device (DESIGN.md 3.3).  Per matched event it holds the hash of the decoded entityId, eventTime, the byte
+ * offset and length of the event's line in the file, and the id bytes, in two runs (main, delta) ordered by
+ * (hash, eventTime descending, offset ascending).  An append is sorted and merged into delta; delta is merged into main
+ * once it holds more than 1 / PIO_EVENTS_INDEX_MERGE_DIVISOR of main's entries.  HOST buffers throughout. */
+#define PIO_EVENTS_INDEX_MERGE_DIVISOR 16
+
+typedef struct pio_events_index pio_events_index;
+
+typedef struct pio_events_index_stats {
+  int64_t n_main, n_delta;   /* entries in each run */
+  int64_t n_merges;          /* delta -> main merges so far */
+  double scan_ms, sort_ms, merge_ms;   /* the last append / add_host: chunk loop, sort + merge into delta, delta -> main
+                                          merge (0 when none); wall milliseconds, device work included */
+} pio_events_index_stats;
+
+/* An empty index of `view` on `device` (the filter's strings are copied).  PIO_ALS_ERR_ARG for a view with `property`
+ * set or with time bounds. */
+PIO_API int pio_events_index_create(int device, const pio_events_filter* view, pio_events_index** out);
+
+/* Adds the events of text[0 .. n_bytes): complete lines as pio_events_scan takes them, whose first byte is at
+ * `base_offset` in the file; every offset must be larger than those already indexed.  The matched events stay on the
+ * device.  Fallback lines are reported as pio_events_scan reports them (byte ranges relative to text, line order);
+ * when *out_n_fallback exceeds fb_capacity nothing was added: call again with room for all of them.  The caller parses
+ * the fallback lines and adds the matching ones with pio_events_index_add_host. */
+PIO_API int pio_events_index_append(pio_events_index* ix, const uint8_t* text, int64_t n_bytes, int64_t base_offset,
+                                    int64_t fb_capacity, int64_t* out_fb_begin, int64_t* out_fb_end,
+                                    int64_t* out_n_fallback);
+
+/* Adds n events parsed by the caller: entityId k = id_bytes[id_off[k] .. id_off[k + 1]) (id_off[0] == 0), its
+ * eventTime, and its line's byte offset and length in the file. */
+PIO_API int pio_events_index_add_host(pio_events_index* ix, const uint8_t* id_bytes, const int64_t* id_off,
+                                      const int64_t* time_us, const int64_t* offset, const int32_t* length, int64_t n);
+
+/* For each of n ids (id k = id_bytes[id_off[k] .. id_off[k + 1])): out_count[k] = its events, at most `limit` (limit < 0:
+ * all).  *out_total = the sum.  When *out_total <= capacity, id k's events are at out_offset / out_len
+ * [sum(out_count[0 .. k)) ..), as (line offset, line length), latest eventTime first and in file order among equal
+ * times; otherwise nothing is written there: call again with capacity >= *out_total. */
+PIO_API int pio_events_index_lookup(pio_events_index* ix, const uint8_t* id_bytes, const int64_t* id_off, int32_t n,
+                                    int64_t limit, int64_t capacity, int64_t* out_count, int64_t* out_total,
+                                    int64_t* out_offset, int32_t* out_len);
+
+PIO_API int pio_events_index_get_stats(const pio_events_index* ix, pio_events_index_stats* out);
+PIO_API int pio_events_index_destroy(pio_events_index* ix);
+
 /* Item co-occurrence of the similarproduct template's CooccurrenceAlgorithm.trainCooccurrence
  * (examples/scala-parallel-similarproduct/multi-events-multi-algos/src/main/scala/CooccurrenceAlgorithm.scala:72-105):
  * (user, item) view events (indices, HOST) -> distinct -> for every user all item pairs -> count per pair -> for every item the

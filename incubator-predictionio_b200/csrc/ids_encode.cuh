@@ -16,24 +16,41 @@
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
+#include <stdlib.h>
 
 #include "sort_scan.cuh"
 
 namespace pio {
 
-__global__ void ids_hash_kernel(const uint8_t* __restrict__ bytes, const long long* __restrict__ off, long long n,
-                                uint64_t* __restrict__ keys, uint32_t* __restrict__ pay, uint64_t mask) {
-  const long long e = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-  if (e >= n) return;
-  uint64_t hsh = 0xcbf29ce484222325ull;   // FNV-1a, then a splitmix64 finaliser
-  for (long long b = off[e]; b < off[e + 1]; ++b) {
-    hsh ^= (uint64_t)bytes[b];
+// The 64-bit hash of the string p[0 .. n): FNV-1a, then a splitmix64 finaliser; & mask (all ones unless
+// PIO_IDS_HASH_BITS shortens it, ids_hash_mask).  ids_encode and the event index (events_index.cuh) both hash with it.
+__device__ __forceinline__ uint64_t ids_hash(const uint8_t* p, long long n, uint64_t mask) {
+  uint64_t hsh = 0xcbf29ce484222325ull;
+  for (long long b = 0; b < n; ++b) {
+    hsh ^= (uint64_t)p[b];
     hsh *= 0x100000001b3ull;
   }
   hsh ^= hsh >> 30; hsh *= 0xBF58476D1CE4E5B9ull;
   hsh ^= hsh >> 27; hsh *= 0x94D049BB133111EBull;
   hsh ^= hsh >> 31;
-  keys[e] = hsh & mask;   // mask = all ones; PIO_IDS_HASH_BITS (tests) shortens the hash to force collisions
+  return hsh & mask;
+}
+
+// tests: PIO_IDS_HASH_BITS = b (1 <= b < 64) keeps the low b bits of the hash, so that different strings collide on
+// purpose
+inline uint64_t ids_hash_mask() {
+  if (const char* hb = getenv("PIO_IDS_HASH_BITS")) {
+    const int b = atoi(hb);
+    if (b >= 1 && b < 64) return (1ull << b) - 1ull;
+  }
+  return ~0ull;
+}
+
+__global__ void ids_hash_kernel(const uint8_t* __restrict__ bytes, const long long* __restrict__ off, long long n,
+                                uint64_t* __restrict__ keys, uint32_t* __restrict__ pay, uint64_t mask) {
+  const long long e = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (e >= n) return;
+  keys[e] = ids_hash(bytes + off[e], off[e + 1] - off[e], mask);
   pay[e] = (uint32_t)e;
 }
 

@@ -50,6 +50,7 @@
 #include "ids_encode.cuh"
 #include "events_scan.cuh"
 #include "events_fold.cuh"
+#include "events_index.cuh"
 #include "cooc.cuh"
 
 namespace pio {
@@ -2594,12 +2595,7 @@ static int ids_encode_device(const uint8_t* d_bytes, const long long* d_off, int
   CK0(A((void**)&f1, 4 * (size_t)n)); CK0(A((void**)&f2, 4 * (size_t)n));
   CK0(A((void**)&run_start, 4 * (size_t)n)); CK0(A((void**)&head, 4 * (size_t)n)); CK0(A((void**)&ishead, 4 * (size_t)n));
   CK0(A((void**)&firstpos, 4 * (size_t)n)); CK0(A((void**)&isfirst, 4 * (size_t)n));
-  uint64_t mask = ~0ull;
-  if (const char* hb = getenv("PIO_IDS_HASH_BITS")) {   // tests: a short hash makes different strings collide on purpose
-    const int b = atoi(hb);
-    if (b >= 1 && b < 64) mask = (1ull << b) - 1ull;
-  }
-  ids_hash_kernel<<<nblk(n, 256), 256, 0, st>>>(d_bytes, d_off, n, ka, va, mask);
+  ids_hash_kernel<<<nblk(n, 256), 256, 0, st>>>(d_bytes, d_off, n, ka, va, ids_hash_mask());
   bool in_b = false;
   CK0(radix_sort_pairs(ka, va, kb, vb, (size_t)n, 64, st, &in_b, nullptr));
   const uint64_t* ks = in_b ? kb : ka;
@@ -2690,17 +2686,89 @@ struct EvKeyArgs {
   int64_t* out_tok_off;
 };
 
+// ---- event index (pio_events_index_*; events_index.cuh) --------------------------------------------------------------
+static void eix_free(EixRun& r) {
+  void* ps[7] = {r.hash, r.time_us, r.off, r.len, r.id_off, r.id_len, r.arena};
+  for (void* q : ps) cudaFree(q);
+  r = EixRun{};
+}
+
+// device arrays of a run for n entries and `bytes` arena bytes (bytes < 0: no arena); nothing is copied
+static cudaError_t eix_alloc(EixRun& r, long long n, long long bytes) {
+  const size_t m = n > 0 ? (size_t)n : 1;
+  cudaError_t e;
+  if ((e = cudaMalloc((void**)&r.hash, 8 * m)) != cudaSuccess) return e;
+  if ((e = cudaMalloc((void**)&r.time_us, 8 * m)) != cudaSuccess) return e;
+  if ((e = cudaMalloc((void**)&r.off, 8 * m)) != cudaSuccess) return e;
+  if ((e = cudaMalloc((void**)&r.len, 4 * m)) != cudaSuccess) return e;
+  if ((e = cudaMalloc((void**)&r.id_off, 8 * m)) != cudaSuccess) return e;
+  if ((e = cudaMalloc((void**)&r.id_len, 4 * m)) != cudaSuccess) return e;
+  return bytes < 0 ? cudaSuccess : cudaMalloc((void**)&r.arena, bytes > 0 ? (size_t)bytes : 1);
+}
+
+// The entries of one append in file order, grown chunk by chunk: the chunk loop of events_scan_impl puts a chunk's
+// matched events here instead of copying them to the host.  The arena is the scan's entityId column.
+struct EixBatch {
+  EixRun r;
+  long long cap_n = 0, cap_bytes = 0;
+  long long file_base = 0;   // file offset of the scanned text's first byte
+  uint64_t mask = ~0ull;
+};
+
+static int eix_reserve(EixBatch* b, long long n, long long bytes, cudaStream_t st) {
+  if (n <= b->cap_n && bytes <= b->cap_bytes) return PIO_ALS_OK;
+  const long long cn = n > 2 * b->cap_n ? n : 2 * b->cap_n, cb = bytes > 2 * b->cap_bytes ? bytes : 2 * b->cap_bytes;
+  EixRun g;
+  const cudaError_t e = eix_alloc(g, cn, cb);
+  if (e != cudaSuccess) {
+    eix_free(g);
+    return fail(nullptr, PIO_ALS_ERR_CUDA, "event index: %s", cudaGetErrorString(e));
+  }
+  const EixRun& r = b->r;
+  const size_t m = (size_t)r.n;
+  CK0(cudaMemcpyAsync(g.hash, r.hash, 8 * m, cudaMemcpyDeviceToDevice, st));
+  CK0(cudaMemcpyAsync(g.time_us, r.time_us, 8 * m, cudaMemcpyDeviceToDevice, st));
+  CK0(cudaMemcpyAsync(g.off, r.off, 8 * m, cudaMemcpyDeviceToDevice, st));
+  CK0(cudaMemcpyAsync(g.len, r.len, 4 * m, cudaMemcpyDeviceToDevice, st));
+  CK0(cudaMemcpyAsync(g.id_off, r.id_off, 8 * m, cudaMemcpyDeviceToDevice, st));
+  CK0(cudaMemcpyAsync(g.id_len, r.id_len, 4 * m, cudaMemcpyDeviceToDevice, st));
+  CK0(cudaMemcpyAsync(g.arena, r.arena, (size_t)r.arena_bytes, cudaMemcpyDeviceToDevice, st));
+  CK0(cudaStreamSynchronize(st));
+  g.n = r.n;
+  g.arena_bytes = r.arena_bytes;
+  eix_free(b->r);
+  b->r = g;
+  b->cap_n = cn, b->cap_bytes = cb;
+  return PIO_ALS_OK;
+}
+
+// one chunk's nm matched events (o, line order) and their eb id bytes, which start at eid_base in the call's id column
+static int eix_take_chunk(EixBatch* b, const EvOut& o, const uint8_t* t, const uint32_t* starts, const EvBase& here,
+                          long long eid_base, int64_t nm, int64_t eb, cudaStream_t st) {
+  if (nm == 0) return PIO_ALS_OK;
+  const int rc = eix_reserve(b, b->r.n + nm, eid_base + eb, st);
+  if (rc != PIO_ALS_OK) return rc;
+  CK0(cudaMemcpyAsync(b->r.arena + eid_base, o.eid_bytes, (size_t)eb, cudaMemcpyDeviceToDevice, st));
+  eix_take_kernel<<<nblk(nm, 256), 256, 0, st>>>(o, t, starts, nm, here.line, b->file_base + here.byte, eid_base + eb,
+                                                 b->mask, b->r, b->r.n);
+  CK0(cudaGetLastError());
+  b->r.n += nm;
+  b->r.arena_bytes = eid_base + eb;
+  return PIO_ALS_OK;
+}
+
 // pio_events_scan (ka == nullptr) and pio_events_scan_keys: one chunk loop, the kernels instantiated with KEYS = ka != 0
 static int events_scan_impl(int device, const uint8_t* text, int64_t n_bytes, const pio_events_filter* f,
                             int64_t capacity, int64_t* out_line, int32_t* out_code, double* out_value, uint8_t* out_flags,
                             int64_t* out_time_us, uint8_t* out_eid_bytes, int64_t* out_eid_off, uint8_t* out_tid_bytes,
                             int64_t* out_tid_off, int64_t* out_n_events, int64_t fb_capacity, int64_t* out_fb_line,
                             int64_t* out_fb_begin, int64_t* out_fb_end, int64_t* out_n_fallback, int64_t* out_n_lines,
-                            const EvKeyArgs* ka) {
-  if (n_bytes < 0 || (n_bytes > 0 && !text) || !f || capacity < n_bytes / PIO_EVENTS_MIN_EVENT_BYTES + 1 ||
-      fb_capacity < 0 || !out_line || !out_code || !out_value || !out_flags || !out_time_us || !out_eid_bytes ||
-      !out_eid_off || !out_tid_bytes || !out_tid_off || !out_n_events || (fb_capacity > 0 && (!out_fb_line ||
-      !out_fb_begin || !out_fb_end)) || !out_n_fallback || !out_n_lines)
+                            const EvKeyArgs* ka, EixBatch* sink = nullptr) {
+  const bool cols = sink == nullptr;   // host columns; with a sink the matched events stay on the device
+  if (n_bytes < 0 || (n_bytes > 0 && !text) || !f || fb_capacity < 0 || (cols && (capacity < n_bytes /
+      PIO_EVENTS_MIN_EVENT_BYTES + 1 || !out_line || !out_code || !out_value || !out_flags || !out_time_us ||
+      !out_eid_bytes || !out_eid_off || !out_tid_bytes || !out_tid_off || !out_n_events)) || (fb_capacity > 0 &&
+      (!out_fb_line || !out_fb_begin || !out_fb_end)) || !out_n_fallback || !out_n_lines)
     return fail(nullptr, PIO_ALS_ERR_ARG, "bad pio_events_scan arguments");
   if (f->n_event_names < 0 || (f->n_event_names > 0 && !f->event_names))
     return fail(nullptr, PIO_ALS_ERR_ARG, "bad event name list");
@@ -2710,8 +2778,8 @@ static int events_scan_impl(int device, const uint8_t* text, int64_t n_bytes, co
       (f->target_entity_type_mode == PIO_EVENTS_TARGET_EQUALS && !f->target_entity_type))
     return fail(nullptr, PIO_ALS_ERR_ARG, "bad target_entity_type_mode / target_entity_type");
   const int nk = ka ? ka->n : 0;
-  *out_n_events = *out_n_fallback = *out_n_lines = 0;
-  out_eid_off[0] = out_tid_off[0] = 0;
+  *out_n_fallback = *out_n_lines = 0;
+  if (cols) *out_n_events = 0, out_eid_off[0] = out_tid_off[0] = 0;
   if (ka) ka->out_tok_off[0] = 0;
   if (n_bytes == 0) return PIO_ALS_OK;
   CK0(cudaSetDevice(device));
@@ -2987,17 +3055,22 @@ static int events_scan_impl(int device, const uint8_t* text, int64_t n_bytes, co
     if (nb < ne && prefetch(slot ^ 1, nb, ne) != PIO_ALS_OK) return PIO_ALS_ERR_CUDA;
     CK0(cudaStreamSynchronize(ex));
     const int64_t nm = h_tot[0], nf = h_tot[1], eb = h_tot[2], tb = h_tot[3];
-    if (n_ev + nm > capacity) return fail(nullptr, PIO_ALS_ERR_ARG, "more matched events than capacity");
+    if (cols && n_ev + nm > capacity) return fail(nullptr, PIO_ALS_ERR_ARG, "more matched events than capacity");
     CK0(cudaEventRecord(d0, ex));
-    CK0(cudaMemcpyAsync(out_line + n_ev, o.line, 8 * nm, cudaMemcpyDeviceToHost, ex));
-    CK0(cudaMemcpyAsync(out_code + n_ev, o.code, 4 * nm, cudaMemcpyDeviceToHost, ex));
-    CK0(cudaMemcpyAsync(out_value + n_ev, o.value, 8 * nm, cudaMemcpyDeviceToHost, ex));
-    CK0(cudaMemcpyAsync(out_flags + n_ev, o.flags, nm, cudaMemcpyDeviceToHost, ex));
-    CK0(cudaMemcpyAsync(out_time_us + n_ev, o.time_us, 8 * nm, cudaMemcpyDeviceToHost, ex));
-    CK0(cudaMemcpyAsync(out_eid_off + n_ev, o.eid_off, 8 * nm, cudaMemcpyDeviceToHost, ex));
-    CK0(cudaMemcpyAsync(out_tid_off + n_ev, o.tid_off, 8 * nm, cudaMemcpyDeviceToHost, ex));
-    CK0(cudaMemcpyAsync(out_eid_bytes + base.eid, o.eid_bytes, eb, cudaMemcpyDeviceToHost, ex));
-    CK0(cudaMemcpyAsync(out_tid_bytes + base.tid, o.tid_bytes, tb, cudaMemcpyDeviceToHost, ex));
+    if (sink) {
+      const int rc = eix_take_chunk(sink, o, t, starts, here, base.eid, nm, eb, ex);
+      if (rc != PIO_ALS_OK) return rc;
+    } else {
+      CK0(cudaMemcpyAsync(out_line + n_ev, o.line, 8 * nm, cudaMemcpyDeviceToHost, ex));
+      CK0(cudaMemcpyAsync(out_code + n_ev, o.code, 4 * nm, cudaMemcpyDeviceToHost, ex));
+      CK0(cudaMemcpyAsync(out_value + n_ev, o.value, 8 * nm, cudaMemcpyDeviceToHost, ex));
+      CK0(cudaMemcpyAsync(out_flags + n_ev, o.flags, nm, cudaMemcpyDeviceToHost, ex));
+      CK0(cudaMemcpyAsync(out_time_us + n_ev, o.time_us, 8 * nm, cudaMemcpyDeviceToHost, ex));
+      CK0(cudaMemcpyAsync(out_eid_off + n_ev, o.eid_off, 8 * nm, cudaMemcpyDeviceToHost, ex));
+      CK0(cudaMemcpyAsync(out_tid_off + n_ev, o.tid_off, 8 * nm, cudaMemcpyDeviceToHost, ex));
+      CK0(cudaMemcpyAsync(out_eid_bytes + base.eid, o.eid_bytes, eb, cudaMemcpyDeviceToHost, ex));
+      CK0(cudaMemcpyAsync(out_tid_bytes + base.tid, o.tid_bytes, tb, cudaMemcpyDeviceToHost, ex));
+    }
     int64_t tk = 0;
     if (ka) {
       tk = (int64_t)h_tot[6] + h_tot[7];
@@ -3027,10 +3100,8 @@ static int events_scan_impl(int device, const uint8_t* text, int64_t n_bytes, co
     flush_oversized();
     cb = nb, ce = ne;
   }
-  out_eid_off[n_ev] = base.eid;
-  out_tid_off[n_ev] = base.tid;
+  if (cols) out_eid_off[n_ev] = base.eid, out_tid_off[n_ev] = base.tid, *out_n_events = n_ev;
   if (ka) ka->out_tok_off[n_ev * nk] = n_tok;
-  *out_n_events = n_ev;
   *out_n_fallback = n_fb;
   *out_n_lines = base.line;
   return PIO_ALS_OK;
@@ -3153,6 +3224,297 @@ int pio_events_fold(int device, const uint8_t* eid_bytes, const int64_t* eid_off
   if (nk) CK0(cudaMemcpyAsync(out_winner, d_win, 8 * ne * nk, cudaMemcpyDeviceToHost, st));
   CK0(cudaStreamSynchronize(st));
   *out_n_entities = n_ent;
+  return PIO_ALS_OK;
+}
+
+}  // extern "C"
+
+// ---- event index (LEventStore.findByEntity for one view; events_index.cuh) ---------------------------------------------
+struct pio_events_index {
+  int device = 0;
+  uint64_t mask = ~0ull;                 // ids_hash_mask() when the index was created: build and lookup hash alike
+  cudaStream_t st = nullptr;
+  std::string entity_type, target;       // the view's strings, owned
+  std::vector<std::string> names;
+  std::vector<const char*> name_ptrs;
+  pio_events_filter view{};
+  pio::EixRun main, delta;
+  pio_events_index_stats stats{};
+  // lookup scratch, grown as needed: query ids, counts, positions, results
+  uint8_t* q_bytes = nullptr;
+  long long* q_off = nullptr;
+  uint32_t *count = nullptr, *pos = nullptr;
+  long long* r_off = nullptr;
+  int32_t* r_len = nullptr;
+  size_t cap_qb = 0, cap_qo = 0, cap_count = 0, cap_pos = 0, cap_roff = 0, cap_rlen = 0;
+};
+
+namespace pio {
+using Clock = std::chrono::steady_clock;
+static double ms_since(Clock::time_point t0) {
+  return std::chrono::duration<double, std::milli>(Clock::now() - t0).count();
+}
+
+// batch b (entries in file order) -> a run in (hash, time descending, offset ascending) order; b's arena moves into it
+static int eix_sort(pio_events_index* ix, EixBatch& b, EixRun* out) {
+  const long long n = b.r.n;
+  const cudaStream_t st = ix->st;
+  std::vector<void*> owned;
+  struct Guard { std::vector<void*>& v; ~Guard() { for (void* q : v) cudaFree(q); } } guard{owned};
+  auto A = [&](void** p, size_t bytes_) -> cudaError_t {
+    cudaError_t e = cudaMalloc(p, bytes_ ? bytes_ : 1);
+    if (e == cudaSuccess) owned.push_back(*p);
+    return e;
+  };
+  uint64_t *ka = nullptr, *kb = nullptr;
+  uint32_t *va = nullptr, *vb = nullptr;
+  CK0(A((void**)&ka, 8 * (size_t)n)); CK0(A((void**)&kb, 8 * (size_t)n));
+  CK0(A((void**)&va, 4 * (size_t)n)); CK0(A((void**)&vb, 4 * (size_t)n));
+  eix_time_key_kernel<<<nblk(n, 256), 256, 0, st>>>(b.r.time_us, n, ka, va);
+  bool in_b = false;
+  CK0(radix_sort_pairs(ka, va, kb, vb, (size_t)n, 64, st, &in_b, nullptr));
+  uint64_t* k1 = in_b ? kb : ka;   // by time; the other pair is free
+  uint32_t* v1 = in_b ? vb : va;
+  uint64_t* k2 = in_b ? ka : kb;
+  uint32_t* v2 = in_b ? va : vb;
+  eix_hash_key_kernel<<<nblk(n, 256), 256, 0, st>>>(v1, b.r.hash, n, k1);
+  CK0(radix_sort_pairs(k1, v1, k2, v2, (size_t)n, 64 - __builtin_clzll(ix->mask), st, &in_b, nullptr));
+  EixRun r;
+  const cudaError_t e = eix_alloc(r, n, -1);
+  if (e != cudaSuccess) {
+    eix_free(r);
+    return fail(nullptr, PIO_ALS_ERR_CUDA, "event index: %s", cudaGetErrorString(e));
+  }
+  r.n = n;
+  eix_gather_kernel<<<nblk(n, 256), 256, 0, st>>>(b.r, in_b ? v2 : v1, r);
+  r.arena = b.r.arena, r.arena_bytes = b.r.arena_bytes;
+  b.r.arena = nullptr;
+  const cudaError_t e2 = cudaStreamSynchronize(st);
+  eix_free(b.r);
+  if (e2 != cudaSuccess || (e2 == cudaSuccess && cudaGetLastError() != cudaSuccess)) {
+    eix_free(r);
+    return fail(nullptr, PIO_ALS_ERR_CUDA, "event index sort: %s", cudaGetErrorString(e2));
+  }
+  *out = r;
+  return PIO_ALS_OK;
+}
+
+// *a = merge(*a, *b); both are consumed
+static int eix_merge(pio_events_index* ix, EixRun* a, EixRun* b) {
+  if (b->n == 0 || a->n == 0) {
+    EixRun& keep = a->n == 0 ? *b : *a;
+    EixRun& drop = a->n == 0 ? *a : *b;
+    eix_free(drop);
+    *a = keep;
+    if (&keep == b) *b = EixRun{};
+    return PIO_ALS_OK;
+  }
+  EixRun r;
+  const long long n = a->n + b->n;
+  const cudaError_t e = eix_alloc(r, n, a->arena_bytes + b->arena_bytes);
+  if (e != cudaSuccess) {
+    eix_free(r);
+    return fail(nullptr, PIO_ALS_ERR_CUDA, "event index merge: %s", cudaGetErrorString(e));
+  }
+  r.n = n;
+  r.arena_bytes = a->arena_bytes + b->arena_bytes;
+  CK0(cudaMemcpyAsync(r.arena, a->arena, (size_t)a->arena_bytes, cudaMemcpyDeviceToDevice, ix->st));
+  CK0(cudaMemcpyAsync(r.arena + a->arena_bytes, b->arena, (size_t)b->arena_bytes, cudaMemcpyDeviceToDevice, ix->st));
+  eix_merge_kernel<<<nblk(n, EIX_MERGE_SPAN), EIX_MERGE_THREADS, 0, ix->st>>>(*a, *b, r);
+  CK0(cudaGetLastError());
+  CK0(cudaStreamSynchronize(ix->st));
+  eix_free(*a);
+  eix_free(*b);
+  *a = r;
+  return PIO_ALS_OK;
+}
+
+// sorts a batch into delta, and merges delta into main once it is past 1 / PIO_EVENTS_INDEX_MERGE_DIVISOR of main
+static int eix_add_batch(pio_events_index* ix, EixBatch& b) {
+  if (b.r.n == 0) return PIO_ALS_OK;
+  const auto t0 = Clock::now();
+  EixRun r;
+  int rc = eix_sort(ix, b, &r);
+  if (rc == PIO_ALS_OK) rc = eix_merge(ix, &ix->delta, &r);
+  ix->stats.sort_ms = ms_since(t0);
+  if (rc != PIO_ALS_OK) return rc;
+  if (ix->delta.n * PIO_EVENTS_INDEX_MERGE_DIVISOR > ix->main.n) {
+    const auto t1 = Clock::now();
+    rc = eix_merge(ix, &ix->main, &ix->delta);
+    ix->stats.merge_ms = ms_since(t1);
+    ++ix->stats.n_merges;
+  }
+  ix->stats.n_main = ix->main.n;
+  ix->stats.n_delta = ix->delta.n;
+  return rc;
+}
+
+// a lookup buffer of at least n elements (contents are not kept)
+template <typename T>
+static cudaError_t eix_grow(T** p, size_t* cap, size_t n) {
+  if (n <= *cap) return cudaSuccess;
+  const size_t c = n > 2 * *cap ? n : 2 * *cap;
+  cudaFree(*p);
+  *p = nullptr;
+  *cap = 0;
+  const cudaError_t e = cudaMalloc((void**)p, c * sizeof(T));
+  if (e == cudaSuccess) *cap = c;
+  return e;
+}
+}  // namespace pio
+
+extern "C" {
+
+int pio_events_index_create(int device, const pio_events_filter* view, pio_events_index** out) {
+  if (!view || !out) return fail(nullptr, PIO_ALS_ERR_ARG, "bad pio_events_index_create arguments");
+  *out = nullptr;
+  if (view->property || view->has_start || view->has_until)
+    return fail(nullptr, PIO_ALS_ERR_ARG, "an event index view has no property and no time bounds");
+  if (view->n_event_names < 0 || (view->n_event_names > 0 && !view->event_names))
+    return fail(nullptr, PIO_ALS_ERR_ARG, "bad event name list");
+  for (int k = 0; k < view->n_event_names; ++k)
+    if (!view->event_names[k]) return fail(nullptr, PIO_ALS_ERR_ARG, "event name %d is NULL", k);
+  if (view->target_entity_type_mode < PIO_EVENTS_TARGET_ANY || view->target_entity_type_mode > PIO_EVENTS_TARGET_EQUALS ||
+      (view->target_entity_type_mode == PIO_EVENTS_TARGET_EQUALS && !view->target_entity_type))
+    return fail(nullptr, PIO_ALS_ERR_ARG, "bad target_entity_type_mode / target_entity_type");
+  CK0(cudaSetDevice(device));
+  auto* ix = new pio_events_index;
+  ix->device = device;
+  ix->mask = ids_hash_mask();
+  if (view->entity_type) ix->entity_type = view->entity_type;
+  if (view->target_entity_type_mode == PIO_EVENTS_TARGET_EQUALS) ix->target = view->target_entity_type;
+  for (int k = 0; k < view->n_event_names; ++k) ix->names.emplace_back(view->event_names[k]);
+  for (const std::string& nm : ix->names) ix->name_ptrs.push_back(nm.c_str());
+  ix->view.entity_type = view->entity_type ? ix->entity_type.c_str() : nullptr;
+  ix->view.event_names = view->event_names ? (ix->name_ptrs.empty() ? &ix->view.entity_type : ix->name_ptrs.data())
+                                           : nullptr;   // an empty list stays non-NULL: no event matches
+  ix->view.n_event_names = view->n_event_names;
+  ix->view.target_entity_type_mode = view->target_entity_type_mode;
+  ix->view.target_entity_type = view->target_entity_type_mode == PIO_EVENTS_TARGET_EQUALS ? ix->target.c_str() : nullptr;
+  const cudaError_t e = cudaStreamCreateWithFlags(&ix->st, cudaStreamNonBlocking);
+  if (e != cudaSuccess) {
+    delete ix;
+    return fail(nullptr, PIO_ALS_ERR_CUDA, "cudaStreamCreate: %s", cudaGetErrorString(e));
+  }
+  *out = ix;
+  return PIO_ALS_OK;
+}
+
+int pio_events_index_append(pio_events_index* ix, const uint8_t* text, int64_t n_bytes, int64_t base_offset,
+                            int64_t fb_capacity, int64_t* out_fb_begin, int64_t* out_fb_end, int64_t* out_n_fallback) {
+  if (!ix || n_bytes < 0 || (n_bytes > 0 && !text) || base_offset < 0 || fb_capacity < 0 || !out_n_fallback ||
+      (fb_capacity > 0 && (!out_fb_begin || !out_fb_end)))
+    return fail(nullptr, PIO_ALS_ERR_ARG, "bad pio_events_index_append arguments");
+  *out_n_fallback = 0;
+  ix->stats.scan_ms = ix->stats.sort_ms = ix->stats.merge_ms = 0;
+  if (n_bytes == 0) return PIO_ALS_OK;
+  CK0(cudaSetDevice(ix->device));
+  EixBatch b;
+  b.file_base = base_offset;
+  b.mask = ix->mask;
+  struct Guard { EixRun& r; ~Guard() { eix_free(r); } } guard{b.r};
+  std::vector<int64_t> fb_line((size_t)(fb_capacity > 0 ? fb_capacity : 1));
+  int64_t n_lines = 0;
+  const auto t0 = Clock::now();
+  const int rc = events_scan_impl(ix->device, text, n_bytes, &ix->view, 0, nullptr, nullptr, nullptr, nullptr, nullptr,
+                                  nullptr, nullptr, nullptr, nullptr, nullptr, fb_capacity, fb_line.data(), out_fb_begin,
+                                  out_fb_end, out_n_fallback, &n_lines, nullptr, &b);
+  ix->stats.scan_ms = ms_since(t0);
+  if (rc != PIO_ALS_OK) return rc;
+  if (*out_n_fallback > fb_capacity) return PIO_ALS_OK;   // nothing added; the caller asks again with more room
+  return eix_add_batch(ix, b);
+}
+
+int pio_events_index_add_host(pio_events_index* ix, const uint8_t* id_bytes, const int64_t* id_off,
+                              const int64_t* time_us, const int64_t* offset, const int32_t* length, int64_t n) {
+  if (!ix || n < 0 || (n > 0 && (!id_off || !time_us || !offset || !length || id_off[0] != 0 ||
+                                 (!id_bytes && id_off[n] > 0))))
+    return fail(nullptr, PIO_ALS_ERR_ARG, "bad pio_events_index_add_host arguments");
+  if (n >= (1ll << 32)) return fail(nullptr, PIO_ALS_ERR_ARG, "n must be < 2^32");
+  for (int64_t k = 0; k < n; ++k)
+    if (id_off[k + 1] < id_off[k] || length[k] < 0 || (k > 0 && offset[k] <= offset[k - 1]))
+      return fail(nullptr, PIO_ALS_ERR_ARG, "event %lld: id offsets must not decrease and line offsets must increase",
+                  (long long)k);
+  ix->stats.scan_ms = ix->stats.sort_ms = ix->stats.merge_ms = 0;
+  if (n == 0) return PIO_ALS_OK;
+  CK0(cudaSetDevice(ix->device));
+  EixBatch b;
+  struct Guard { EixRun& r; ~Guard() { eix_free(r); } } guard{b.r};
+  const cudaError_t e = eix_alloc(b.r, n, id_off[n]);
+  if (e != cudaSuccess) return fail(nullptr, PIO_ALS_ERR_CUDA, "event index: %s", cudaGetErrorString(e));
+  b.r.n = n;
+  b.r.arena_bytes = id_off[n];
+  std::vector<int32_t> id_len((size_t)n);
+  for (int64_t k = 0; k < n; ++k) id_len[k] = (int32_t)(id_off[k + 1] - id_off[k]);
+  const size_t m = (size_t)n;
+  CK0(cudaMemcpyAsync(b.r.arena, id_bytes, (size_t)id_off[n], cudaMemcpyHostToDevice, ix->st));
+  CK0(cudaMemcpyAsync(b.r.id_off, id_off, 8 * m, cudaMemcpyHostToDevice, ix->st));
+  CK0(cudaMemcpyAsync(b.r.id_len, id_len.data(), 4 * m, cudaMemcpyHostToDevice, ix->st));
+  CK0(cudaMemcpyAsync(b.r.time_us, time_us, 8 * m, cudaMemcpyHostToDevice, ix->st));
+  CK0(cudaMemcpyAsync(b.r.off, offset, 8 * m, cudaMemcpyHostToDevice, ix->st));
+  CK0(cudaMemcpyAsync(b.r.len, length, 4 * m, cudaMemcpyHostToDevice, ix->st));
+  eix_hash_kernel<<<nblk(n, 256), 256, 0, ix->st>>>(b.r, ix->mask);
+  CK0(cudaGetLastError());
+  return eix_add_batch(ix, b);
+}
+
+int pio_events_index_lookup(pio_events_index* ix, const uint8_t* id_bytes, const int64_t* id_off, int32_t n,
+                            int64_t limit, int64_t capacity, int64_t* out_count, int64_t* out_total,
+                            int64_t* out_offset, int32_t* out_len) {
+  if (!ix || n < 0 || capacity < 0 || !out_total || (n > 0 && (!id_off || !out_count || id_off[0] != 0 ||
+      (!id_bytes && id_off[n] > 0))) || (capacity > 0 && (!out_offset || !out_len)))
+    return fail(nullptr, PIO_ALS_ERR_ARG, "bad pio_events_index_lookup arguments");
+  *out_total = 0;
+  if (n == 0) return PIO_ALS_OK;
+  CK0(cudaSetDevice(ix->device));
+  const cudaStream_t st = ix->st;
+  const size_t nb = (size_t)id_off[n], nq = (size_t)n;
+  CK0(eix_grow(&ix->q_bytes, &ix->cap_qb, nb ? nb : 1));
+  CK0(eix_grow(&ix->q_off, &ix->cap_qo, nq + 1));
+  CK0(eix_grow(&ix->count, &ix->cap_count, nq));
+  CK0(eix_grow(&ix->pos, &ix->cap_pos, nq));
+  CK0(cudaMemcpyAsync(ix->q_bytes, id_bytes, nb, cudaMemcpyHostToDevice, st));
+  CK0(cudaMemcpyAsync(ix->q_off, id_off, 8 * (nq + 1), cudaMemcpyHostToDevice, st));
+  const unsigned grid = nblk(n, EIX_LOOKUP_WARPS);
+  eix_count_kernel<<<grid, 32 * EIX_LOOKUP_WARPS, 0, st>>>(ix->main, ix->delta, ix->q_bytes, ix->q_off, n, ix->mask,
+                                                            limit, ix->count);
+  CK0(cudaGetLastError());
+  CK0(scan_exclusive_u32(ix->count, ix->pos, nq, st, nullptr));
+  std::vector<uint32_t> cnt(nq);
+  CK0(cudaMemcpyAsync(cnt.data(), ix->count, 4 * nq, cudaMemcpyDeviceToHost, st));
+  CK0(cudaStreamSynchronize(st));
+  int64_t total = 0;
+  for (size_t k = 0; k < nq; ++k) total += out_count[k] = cnt[k];
+  *out_total = total;
+  if (total == 0 || total > capacity) return PIO_ALS_OK;
+  if (total >= (1ll << 32)) return fail(nullptr, PIO_ALS_ERR_ARG, "more than 2^32-1 events in one lookup");
+  CK0(eix_grow(&ix->r_off, &ix->cap_roff, (size_t)total));
+  CK0(eix_grow(&ix->r_len, &ix->cap_rlen, (size_t)total));
+  eix_write_kernel<<<grid, 32 * EIX_LOOKUP_WARPS, 0, st>>>(ix->main, ix->delta, ix->q_bytes, ix->q_off, n, ix->mask,
+                                                            ix->count, ix->pos, ix->r_off, ix->r_len);
+  CK0(cudaGetLastError());
+  CK0(cudaMemcpyAsync(out_offset, ix->r_off, 8 * (size_t)total, cudaMemcpyDeviceToHost, st));
+  CK0(cudaMemcpyAsync(out_len, ix->r_len, 4 * (size_t)total, cudaMemcpyDeviceToHost, st));
+  CK0(cudaStreamSynchronize(st));
+  return PIO_ALS_OK;
+}
+
+int pio_events_index_get_stats(const pio_events_index* ix, pio_events_index_stats* out) {
+  if (!ix || !out) return fail(nullptr, PIO_ALS_ERR_ARG, "bad pio_events_index_get_stats arguments");
+  *out = ix->stats;
+  return PIO_ALS_OK;
+}
+
+int pio_events_index_destroy(pio_events_index* ix) {
+  if (!ix) return PIO_ALS_OK;
+  cudaSetDevice(ix->device);
+  if (ix->st) cudaStreamSynchronize(ix->st);
+  eix_free(ix->main);
+  eix_free(ix->delta);
+  void* ps[6] = {ix->q_bytes, ix->q_off, ix->count, ix->pos, ix->r_off, ix->r_len};
+  for (void* q : ps) cudaFree(q);
+  if (ix->st) cudaStreamDestroy(ix->st);
+  delete ix;
   return PIO_ALS_OK;
 }
 

@@ -32,7 +32,9 @@ EXPORTED_SYMBOLS = [
     "pio_als_set_init", "pio_als_run", "pio_als_get_factors", "pio_als_train", "pio_als_recommend",
     "pio_als_similar", "pio_als_similar_batch", "pio_als_model_import", "pio_als_save", "pio_als_load", "pio_als_get_stats", "pio_als_get_phase_ms",
     "pio_als_synth_ratings_device", "pio_nb_train", "pio_nb_predict", "pio_ids_encode", "pio_cooc_train",
-    "pio_events_scan", "pio_events_scan_keys", "pio_events_fold",
+    "pio_events_scan", "pio_events_scan_keys", "pio_events_fold", "pio_events_index_create",
+    "pio_events_index_append", "pio_events_index_add_host", "pio_events_index_lookup", "pio_events_index_get_stats",
+    "pio_events_index_destroy",
 ]
 
 
@@ -111,6 +113,10 @@ def lib():
         L.pio_als_similar.argtypes = [vp, vp, ci, ci, vp, vp, ci, vp, vp, vp]
         L.pio_als_similar_batch.restype = ci
         L.pio_als_similar_batch.argtypes = [vp, vp, vp, ci, ci, vp, vp, ci, vp, vp, vp]
+        i64 = C.c_int64
+        L.pio_events_index_lookup.restype = ci
+        L.pio_events_index_lookup.argtypes = [vp, vp, vp, C.c_int32, i64, i64, vp, vp, vp, vp]
+        L.pio_events_index_destroy.argtypes = [vp]
         for name in EXPORTED_SYMBOLS:
             getattr(L, name)  # AttributeError if the ABI is incomplete
         _lib = L
@@ -421,17 +427,7 @@ def _events_scan(text, entity_type, event_names, target_mode, target_entity_type
     buf = np.frombuffer(text, np.uint8) if isinstance(text, (bytes, bytearray, memoryview)) else \
         np.ascontiguousarray(text, np.uint8)
     n = int(buf.shape[0])
-    names = [] if event_names is None else [x.encode("utf-8") for x in event_names]
-    f = EventsFilter()
-    keep = (C.c_char_p * max(len(names), 1))(*names)
-    f.entity_type = None if entity_type is None else entity_type.encode("utf-8")
-    f.event_names = None if event_names is None else keep   # None: any name; []: no event matches (as in find)
-    f.n_event_names = len(names)
-    f.target_entity_type_mode = int(target_mode)
-    f.target_entity_type = None if target_entity_type is None else target_entity_type.encode("utf-8")
-    f.property = None if prop is None else prop.encode("utf-8")
-    f.has_start, f.start_us = (0, 0) if start_us is None else (1, int(start_us))
-    f.has_until, f.until_us = (0, 0) if until_us is None else (1, int(until_us))
+    f, keep = _events_filter(entity_type, event_names, target_mode, target_entity_type, prop, start_us, until_us)
     cap = n // EVENTS_MIN_EVENT_BYTES + 1
     out = dict(line=np.empty(cap, np.int64), code=np.empty(cap, np.int32), value=np.empty(cap, np.float64),
                flags=np.empty(cap, np.uint8), time_us=np.empty(cap, np.int64), eid_bytes=np.empty(max(n, 1), np.uint8),
@@ -500,6 +496,111 @@ def events_fold(eid, code, time_us, present=None, n_keys=0, device=0):
     g = ne.value
     return dict(first_event=first[:g], exists=exists[:g].astype(bool), first_us=fus[:g], last_us=lus[:g],
                 winner=win[:g, :int(n_keys)])
+
+
+class EventsIndexStats(C.Structure):
+    _fields_ = [("n_main", C.c_int64), ("n_delta", C.c_int64), ("n_merges", C.c_int64), ("scan_ms", C.c_double),
+                ("sort_ms", C.c_double), ("merge_ms", C.c_double)]
+
+
+def _events_filter(entity_type, event_names, target_mode, target_entity_type, prop, start_us, until_us):
+    """A pio_events_filter, and the ctypes objects its pointers refer to (keep both alive together)."""
+    names = [] if event_names is None else [x.encode("utf-8") for x in event_names]
+    f = EventsFilter()
+    keep = (C.c_char_p * max(len(names), 1))(*names)
+    f.entity_type = None if entity_type is None else entity_type.encode("utf-8")
+    f.event_names = None if event_names is None else keep   # None: any name; []: no event matches (as in find)
+    f.n_event_names = len(names)
+    f.target_entity_type_mode = int(target_mode)
+    f.target_entity_type = None if target_entity_type is None else target_entity_type.encode("utf-8")
+    f.property = None if prop is None else prop.encode("utf-8")
+    f.has_start, f.start_us = (0, 0) if start_us is None else (1, int(start_us))
+    f.has_until, f.until_us = (0, 0) if until_us is None else (1, int(until_us))
+    return f, keep
+
+
+class EventsIndex:
+    """pio_events_index: the events of one view (entity type, event names, target entity type) of an append-only event
+    file on the device, looked up by entityId in LEventStore.findByEntity's order (latest first, file order among equal
+    times).  Lines are given by byte offset and length in the file."""
+
+    def __init__(self, entity_type, event_names, target_mode=EVENTS_TARGET_ANY, target_entity_type=None, device=0):
+        self._h = C.c_void_p()
+        f, keep = _events_filter(entity_type, event_names, target_mode, target_entity_type, None, None, None)
+        self._check(lib().pio_events_index_create(C.c_int(device), C.byref(f), C.byref(self._h)))
+
+    def _check(self, rc):
+        if rc != 0:
+            raise NativeError(rc, lib().pio_als_last_error(None).decode())
+
+    def close(self):
+        if self._h:
+            lib().pio_events_index_destroy(self._h)
+            self._h = C.c_void_p()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    def append(self, text, base_offset: int):
+        """Indexes the complete lines `text` (bytes / memoryview), whose first byte is at `base_offset` in the file.
+        Returns the fallback lines as (begin, end) file offsets, in line order: the caller parses them and adds the
+        matching ones with add_host."""
+        buf = np.frombuffer(text, np.uint8)
+        n = int(buf.shape[0])
+        fb_cap = max(1024, n // 4096)
+        n_fb = C.c_int64(0)
+        while True:
+            fb = [np.empty(fb_cap, np.int64) for _ in range(2)]
+            self._check(lib().pio_events_index_append(self._h, _ptr(buf, C.c_uint8) if n else None, C.c_int64(n),
+                                                      C.c_int64(base_offset), C.c_int64(fb_cap),
+                                                      *[_ptr(a, C.c_int64) for a in fb], C.byref(n_fb)))
+            if n_fb.value <= fb_cap:
+                break
+            fb_cap = n_fb.value     # nothing was added: once more with room for every fallback line
+        return fb[0][:n_fb.value] + base_offset, fb[1][:n_fb.value] + base_offset
+
+    def add_host(self, ids, time_us, offset, length):
+        """Events parsed on the host, in file order: entityId strings, eventTime (us), line offset and length."""
+        enc = [x.encode("utf-8", "surrogatepass") for x in ids]
+        off = np.zeros(len(enc) + 1, np.int64)
+        np.cumsum([len(b) for b in enc], out=off[1:])
+        buf = np.frombuffer(b"".join(enc), np.uint8)
+        t, o, ln = (np.ascontiguousarray(a, d) for a, d in ((time_us, np.int64), (offset, np.int64), (length, np.int32)))
+        self._check(lib().pio_events_index_add_host(self._h, _ptr(buf, C.c_uint8) if buf.size else None,
+                                                    _ptr(off, C.c_int64), _ptr(t, C.c_int64), _ptr(o, C.c_int64),
+                                                    _ptr(ln, C.c_int32), C.c_int64(len(enc))))
+
+    def lookup(self, ids, limit=None):
+        """For each entityId of `ids` (str): (offsets int64[], lengths int32[]) of its lines, latest first, at most
+        `limit` (None or negative: all)."""
+        enc = [x.encode("utf-8", "surrogatepass") for x in ids]
+        n = len(enc)
+        off = np.zeros(n + 1, np.int64)
+        np.cumsum([len(b) for b in enc], out=off[1:])
+        buf = np.frombuffer(b"".join(enc), np.uint8)
+        lim = -1 if limit is None else int(limit)
+        count = np.zeros(max(n, 1), np.int64)
+        total = C.c_int64(0)
+        cap = max(16, 16 * n if lim < 0 else lim * n)
+        while True:
+            ro, rl = np.empty(cap, np.int64), np.empty(cap, np.int32)
+            self._check(lib().pio_events_index_lookup(self._h, buf.ctypes.data if buf.size else None, off.ctypes.data,
+                                                      n, lim, cap, count.ctypes.data, C.addressof(total),
+                                                      ro.ctypes.data, rl.ctypes.data))
+            if total.value <= cap:
+                break
+            cap = total.value       # the result did not fit: ask again with room for all of it
+        pos = np.zeros(n + 1, np.int64)
+        np.cumsum(count[:n], out=pos[1:])
+        return [(ro[pos[k]:pos[k + 1]], rl[pos[k]:pos[k + 1]]) for k in range(n)]
+
+    def stats(self) -> dict:
+        st = EventsIndexStats()
+        self._check(lib().pio_events_index_get_stats(self._h, C.byref(st)))
+        return {name: getattr(st, name) for name, _ in EventsIndexStats._fields_}
 
 
 def events_scan_timing() -> dict:

@@ -20,6 +20,7 @@ from __future__ import annotations
 import datetime as _dt
 import json
 import os
+import threading
 from dataclasses import dataclass, field
 from pathlib import Path
 from typing import Any, Dict, Iterable, Iterator, List, Optional, Sequence, Tuple
@@ -552,6 +553,27 @@ def _columns_from_rows(rows) -> Tuple[Dict[str, np.ndarray], Dict[int, Any]]:
 FIND_COLUMNS_CHUNK = 256 << 20
 
 
+def _line_pieces(fh, chunk_bytes) -> Iterator[Tuple[int, memoryview, bool]]:
+    """The rest of the open binary file fh in pieces of about chunk_bytes, each cut after a "\n" (a piece without one
+    grows): (file offset, bytes, complete).  Only the last piece, the bytes after the last "\n", has complete False; it
+    is not yielded when empty."""
+    pos, carry = fh.tell(), b""
+    while True:
+        data = fh.read(chunk_bytes)
+        buf = carry + data                        # no copy while the carry is empty
+        if not data:
+            if buf:
+                yield pos, memoryview(buf), False
+            return
+        cut = buf.rfind(b"\n") + 1
+        if cut == 0:
+            carry = buf
+            continue
+        yield pos, memoryview(buf)[:cut], True    # read in place
+        pos += cut
+        carry = buf[cut:]
+
+
 def _scan_file(appName, channelName, scan, chunk_bytes):
     """The app's event file, read in pieces of complete lines (about chunk_bytes each) that `scan` (a native.events_scan
     call on a memoryview) reads in place.  Returns the scan results with file-wide line numbers, and the fallback lines
@@ -561,27 +583,13 @@ def _scan_file(appName, channelName, scan, chunk_bytes):
         raise FileNotFoundError(f"Invalid app name {appName}: no event data at {p}")  # Common.appNameToId
     parts, host_lines, line_base = [], [], 0
     with open(p, "rb") as fh:
-        carry = b""
-        while True:
-            data = fh.read(chunk_bytes)
-            buf = carry + data                    # no copy while the carry is empty
-            cut = len(buf)
-            if data:
-                cut = buf.rfind(b"\n") + 1        # complete lines only; a chunk without "\n" grows
-                if cut == 0:
-                    carry = buf
-                    continue
-                carry = buf[cut:]
-            if cut:
-                view = memoryview(buf)[:cut]      # the scan reads the piece in place
-                r = scan(view)
-                r["line"] += line_base
-                parts.append(r)
-                host_lines.extend((int(ln) + line_base, bytes(view[b:e])) for ln, b, e in
-                                  zip(r["fb_line"], r["fb_begin"], r["fb_end"]))
-                line_base += r["n_lines"]
-            if not data:
-                break
+        for _, view, _ in _line_pieces(fh, chunk_bytes):
+            r = scan(view)
+            r["line"] += line_base
+            parts.append(r)
+            host_lines.extend((int(ln) + line_base, bytes(view[b:e])) for ln, b, e in
+                              zip(r["fb_line"], r["fb_begin"], r["fb_end"]))
+            line_base += r["n_lines"]
     return parts, host_lines
 
 
@@ -591,16 +599,21 @@ def _scan_args(startTime, untilTime, sc):
     return s_us, u_us, getattr(sc, "device", 0) or 0
 
 
+def _target_filter(targetEntityType):
+    """find's targetEntityType argument as the native filter's (mode, target entity type)."""
+    from . import native
+    if targetEntityType is _UNSET:
+        return native.EVENTS_TARGET_ANY, None
+    if targetEntityType is None:
+        return native.EVENTS_TARGET_ABSENT, None
+    return native.EVENTS_TARGET_EQUALS, targetEntityType
+
+
 def _find_columns(appName, entityType=None, eventNames=None, targetEntityType=_UNSET, property=None, startTime=None,
                   untilTime=None, channelName=None, sc=None, chunk_bytes=FIND_COLUMNS_CHUNK) -> EventColumns:
     from . import native
     names = None if eventNames is None else set(eventNames)
-    if targetEntityType is _UNSET:
-        mode, tet = native.EVENTS_TARGET_ANY, None
-    elif targetEntityType is None:
-        mode, tet = native.EVENTS_TARGET_ABSENT, None
-    else:
-        mode, tet = native.EVENTS_TARGET_EQUALS, targetEntityType
+    mode, tet = _target_filter(targetEntityType)
     s_us, u_us, device = _scan_args(startTime, untilTime, sc)
     parts, host_lines = _scan_file(
         appName, channelName,
@@ -851,3 +864,133 @@ class LEventStore:
                                targetEntityType, targetEntityId)
         evs.sort(key=lambda e: e.eventTime, reverse=latest)
         return evs if limit is None or limit < 0 else evs[:limit]
+
+    @staticmethod
+    def entityIndex(appName: str, entityType: str, eventNames: Optional[Sequence[str]] = None, targetEntityType=_UNSET,
+                    channelName: Optional[str] = None, device: int = 0) -> "EntityEventIndex":
+        """findByEntity for one view (entityType, eventNames, targetEntityType) served from an event index on the GPU
+        (EntityEventIndex).  Built on its first find.  Needs the CUDA library."""
+        return EntityEventIndex(appName, entityType, eventNames, targetEntityType, channelName, device)
+
+
+_INDEX_CHECK_BYTES = 4096
+
+
+class EntityEventIndex:
+    """LEventStore.findByEntity for one view -- entityType, eventNames, targetEntityType -- of an app's event file, from
+    an index of its events by entityId kept on the GPU (native.EventsIndex, DESIGN.md 3.3).  `find(entityId, limit)`
+    returns exactly the list findByEntity(appName, entityType, entityId, channelName, eventNames, targetEntityType,
+    limit=limit, latest=True) returns at that moment, the same exception included.
+
+    Every find first brings the index up to date with the file.  The file store is append-only: import_events appends,
+    delete_app_data unlinks.  What this relies on: a file that still has the indexed file's (st_dev, st_ino), is at
+    least as long, and still ends the indexed bytes with the same last 4 KB, holds the indexed bytes unchanged.  Such a
+    file is brought up to date by indexing its new complete lines (up to the last "\n"); any other file is indexed
+    from scratch.  Bytes after the last "\n" are parsed on the host on every find.  A missing file raises what find
+    raises and drops the index.  Calls are serialised by a lock."""
+
+    def __init__(self, appName: str, entityType: str, eventNames: Optional[Sequence[str]] = None,
+                 targetEntityType=_UNSET, channelName: Optional[str] = None, device: int = 0):
+        self.appName, self.channelName, self.device = appName, channelName, device
+        self.entityType = entityType
+        self.eventNames = None if eventNames is None else list(eventNames)
+        self.targetEntityType = targetEntityType
+        self._lock = threading.Lock()
+        self._ix = None
+        self._file: Optional[Tuple[int, int]] = None   # (st_dev, st_ino) of the indexed file
+        self._length = 0                                # bytes indexed: complete lines
+        self._end = b""                                 # their last <= 4 KB
+        self._bad: Optional[Tuple[int, bytes]] = None   # first line of the indexed bytes that find cannot parse
+
+    def close(self) -> None:
+        with self._lock:
+            self._drop()
+
+    def stats(self) -> Dict[str, Any]:
+        """The native index's run sizes, merge count and last append's times (empty before the first find)."""
+        with self._lock:
+            return {} if self._ix is None else self._ix.stats()
+
+    def find(self, entityId: str, limit: Optional[int] = None) -> List[Event]:
+        return self.find_many([entityId], limit)[0]
+
+    def find_many(self, entityIds: Sequence[str], limit: Optional[int] = None) -> List[List[Event]]:
+        """find for every id of entityIds, with one lookup on the device."""
+        with self._lock:
+            p = app_file(self.appName, self.channelName)
+            try:
+                fh = open(p, "rb")
+            except FileNotFoundError:
+                self._drop()
+                raise FileNotFoundError(f"Invalid app name {self.appName}: no event data at {p}") from None  # as find
+            with fh:
+                tail = self._update(fh)
+                if self._bad is not None:   # find raises on the first line it cannot parse
+                    list(self._host_events([self._bad]))
+                tail_events = [e for _, e in self._host_events(tail)]
+                hits = self._ix.lookup(list(entityIds), limit)
+                fd, out = fh.fileno(), []
+                for eid, (offs, lens) in zip(entityIds, hits):
+                    evs = [Event.from_json(json.loads(os.pread(fd, int(n), int(o)).decode("utf-8").strip()))
+                           for o, n in zip(offs, lens)]
+                    more = [e for e in tail_events if e.entityId == eid]
+                    if more:   # stable: at equal times the indexed events, which come first in the file, stay first
+                        evs = sorted(evs + more, key=lambda e: e.eventTime, reverse=True)
+                    out.append(evs if limit is None or limit < 0 else evs[:limit])
+                return out
+
+    def _drop(self) -> None:
+        if self._ix is not None:
+            self._ix.close()
+        self._ix, self._file, self._length, self._end, self._bad = None, None, 0, b"", None
+
+    def _host_events(self, lines) -> Iterator[Tuple[int, Event]]:
+        names = None if self.eventNames is None else set(self.eventNames)
+        return _host_events(lines, names, self.entityType, self.targetEntityType, None, None)
+
+    def _update(self, fh) -> List[Tuple[int, bytes]]:
+        """Indexes what the file has gained (everything, when it is not the indexed file any more); returns the lines
+        after the last "\n" as (offset, bytes)."""
+        from . import native
+        st = os.fstat(fh.fileno())
+        if self._ix is not None:
+            k = len(self._end)
+            if (st.st_dev, st.st_ino) != self._file or st.st_size < self._length or \
+                    os.pread(fh.fileno(), k, self._length - k) != self._end:
+                self._drop()
+        if self._ix is None:
+            mode, tet = _target_filter(self.targetEntityType)
+            self._ix = native.EventsIndex(self.entityType, self.eventNames, mode, tet, self.device)
+            self._file = (st.st_dev, st.st_ino)
+        fh.seek(self._length)
+        # read() allocates the size it is asked for: ask for about what is new, not a whole piece
+        for base, view, complete in _line_pieces(fh, min(FIND_COLUMNS_CHUNK, st.st_size - self._length + 1)):
+            if not complete:   # no "\n" in it: only lone "\r" can end its lines
+                lines, at = [], base
+                for piece in bytes(view).split(b"\r"):
+                    lines.append((at, piece))
+                    at += len(piece) + 1
+                return lines
+            self._append(base, view)
+        return []
+
+    def _append(self, base: int, view: memoryview) -> None:
+        fb_begin, fb_end = self._ix.append(view, base)
+        ids, t_us, offs, lens = [], [], [], []
+        for b, e in zip(fb_begin.tolist(), fb_end.tolist()):
+            raw = bytes(view[b - base:e - base])
+            try:
+                evs = list(self._host_events([(b, raw)]))
+            except Exception:
+                if self._bad is None:
+                    self._bad = (b, raw)
+                continue
+            for _, ev in evs:
+                ids.append(ev.entityId)
+                t_us.append(time_us(ev.eventTime))
+                offs.append(b)
+                lens.append(e - b)
+        if ids:
+            self._ix.add_host(ids, t_us, offs, lens)
+        self._length = base + len(view)
+        self._end = (self._end + bytes(view[-_INDEX_CHECK_BYTES:]))[-_INDEX_CHECK_BYTES:]

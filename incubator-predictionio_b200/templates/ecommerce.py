@@ -18,7 +18,8 @@ import numpy as np
 from ..controller import (Engine, EngineFactory, LFirstServing, P2LAlgorithm, Params, PDataSource, PersistentModel,
                           IdentityPreparator)
 from ..mllib import ALS, MatrixFactorizationModel
-from ..storage import BiMap, EntityEventColumns, LEventStore, PEventStore, require_values, string_list
+from ..storage import (BiMap, EntityEventColumns, EntityEventIndex, LEventStore, PEventStore, require_values,
+                       string_list)
 
 
 @dataclass
@@ -183,6 +184,18 @@ class ECommModel(PersistentModel):
 class ECommAlgorithm(P2LAlgorithm):
     def __init__(self, ap: ECommAlgorithmParams):
         self.ap = ap
+        self._indexes: Dict[str, EntityEventIndex] = {}
+
+    def _index(self, view: str) -> EntityEventIndex:
+        """The event index behind one of the serving lookups, created on first use: "seen" (user, seenEvents, item),
+        "similar" (user, similarEvents, item) or "constraint" (constraint, [$set], any target)."""
+        if view not in self._indexes:
+            ap = self.ap
+            kw = {"seen": dict(entityType="user", eventNames=ap.seenEvents, targetEntityType="item"),
+                  "similar": dict(entityType="user", eventNames=ap.similarEvents, targetEntityType="item"),
+                  "constraint": dict(entityType="constraint", eventNames=["$set"])}[view]
+            self._indexes[view] = LEventStore.entityIndex(ap.appName, **kw)
+        return self._indexes[view]
 
     def train(self, sc, data: PreparedData) -> ECommModel:
         c = data.columns if data._users is None and data._rateEvents is None else None   # None: built from lists
@@ -231,13 +244,10 @@ class ECommAlgorithm(P2LAlgorithm):
     def genBlackList(self, query: Query) -> Set[str]:
         seen: Set[str] = set()
         if self.ap.unseenOnly:
-            seen = {e.targetEntityId for e in LEventStore.findByEntity(self.ap.appName, "user", query.user,
-                                                                     eventNames=self.ap.seenEvents,
-                                                                     targetEntityType="item")}
+            seen = {e.targetEntityId for e in self._index("seen").find(query.user)}
         unavailable: Set[str] = set()
         try:
-            cons = LEventStore.findByEntity(self.ap.appName, "constraint", "unavailableItems", eventNames=["$set"],
-                                            limit=1, latest=True)
+            cons = self._index("constraint").find("unavailableItems", limit=1)
             if cons:
                 unavailable = set(cons[0].properties.get("items"))
         except FileNotFoundError:
@@ -245,9 +255,7 @@ class ECommAlgorithm(P2LAlgorithm):
         return set(query.blackList or ()) | seen | unavailable
 
     def getRecentItems(self, query: Query) -> Set[str]:
-        return {e.targetEntityId for e in LEventStore.findByEntity(self.ap.appName, "user", query.user,
-                                                                  eventNames=self.ap.similarEvents,
-                                                                  targetEntityType="item", limit=10, latest=True)}
+        return {e.targetEntityId for e in self._index("similar").find(query.user, limit=10)}
 
     def _mask(self, model: ECommModel, query: Query, blackList: Set[int]) -> np.ndarray:
         n = len(model.mf.productHas)
@@ -270,8 +278,7 @@ class ECommAlgorithm(P2LAlgorithm):
         """Latest `$set` of the constraint entity "weightedItems": [{"items": [...], "weight": w}, ...]
         (adjust-score/src/main/scala/ECommAlgorithm.scala:402-429); Nil when the event does not exist."""
         try:
-            cons = LEventStore.findByEntity(self.ap.appName, "constraint", "weightedItems", eventNames=["$set"],
-                                            limit=1, latest=True)
+            cons = self._index("constraint").find("weightedItems", limit=1)
         except FileNotFoundError:
             return []
         if not cons:
