@@ -16,6 +16,7 @@
 
 #include <chrono>
 #include <algorithm>
+#include <array>
 #include <deque>
 #include <exception>
 #include <map>
@@ -497,22 +498,67 @@ static void dfree(pio_als_handle* h, T*& p) {
   p = nullptr;
 }
 
-// Device temporaries of one API call: released (stream-ordered) on every exit path, including the early error returns
-// of CK().
+// Device temporaries of one API call, or of one chunk of an event scan, on stream s: released (stream-ordered) on every
+// exit path, including the early error returns of CK() and CK0().
 struct Scratch {
-  pio_als_handle* h;
+  cudaStream_t s;
   std::vector<void*> ptrs;
-  explicit Scratch(pio_als_handle* h_) : h(h_) {}
+  explicit Scratch(cudaStream_t s_) : s(s_) {}
   Scratch(const Scratch&) = delete;
   Scratch& operator=(const Scratch&) = delete;
   template <class T>
   cudaError_t alloc(T** p, size_t n) {
-    const cudaError_t e = dalloc(h, p, n);
+    const cudaError_t e = cudaMallocAsync((void**)p, (n ? n : 1) * sizeof(T), s);
     if (e == cudaSuccess) ptrs.push_back((void*)*p);
     return e;
   }
   ~Scratch() {
-    for (void* q : ptrs) cudaFreeAsync(q, h->stream);
+    for (void* q : ptrs) cudaFreeAsync(q, s);
+  }
+};
+
+// Everything a synchronous call without a handle holds until it returns: device memory (cudaMalloc), pinned host memory
+// (cudaHostAlloc), and the streams and events it creates.  On every exit path, including the early error returns of
+// CK0(), the stream it was given and the streams it created are drained first, so that nothing is freed under a
+// running kernel or copy; then everything is released.
+struct CallMem {
+  std::vector<cudaStream_t> drain, streams;
+  std::vector<cudaEvent_t> events;
+  std::vector<void*> dev, pinned;
+  CallMem() = default;
+  explicit CallMem(cudaStream_t st) : drain{st} {}
+  CallMem(const CallMem&) = delete;
+  CallMem& operator=(const CallMem&) = delete;
+  template <class T>
+  cudaError_t device(T** p, size_t n) {
+    const size_t bytes = n * sizeof(T);
+    const cudaError_t e = cudaMalloc((void**)p, bytes ? bytes : 1);
+    if (e == cudaSuccess) dev.push_back((void*)*p);
+    return e;
+  }
+  template <class T>
+  cudaError_t host(T** p, size_t n) {
+    const size_t bytes = n * sizeof(T);
+    const cudaError_t e = cudaHostAlloc((void**)p, bytes ? bytes : 1, cudaHostAllocDefault);
+    if (e == cudaSuccess) pinned.push_back((void*)*p);
+    return e;
+  }
+  cudaError_t stream(cudaStream_t* s) {
+    const cudaError_t e = cudaStreamCreateWithFlags(s, cudaStreamNonBlocking);
+    if (e == cudaSuccess) drain.push_back(*s), streams.push_back(*s);
+    return e;
+  }
+  cudaError_t event(cudaEvent_t* ev) {
+    const cudaError_t e = cudaEventCreate(ev);
+    if (e == cudaSuccess) events.push_back(*ev);
+    return e;
+  }
+  ~CallMem() {
+    for (cudaStream_t s : drain) cudaStreamSynchronize(s);
+    for (void* q : dev) cudaFree(q);
+    for (void* q : pinned) cudaFreeHost(q);
+    for (cudaStream_t s : streams) cudaStreamDestroy(s);
+    for (cudaEvent_t e : events) cudaEventDestroy(e);
   }
 };
 
@@ -545,7 +591,7 @@ static int build_side(pio_als_handle* h, Side& row, const Side& col, const int* 
   // nnz_global = ratings after dedup over all ranks (kernel choice must agree on every rank)
   cudaStream_t st = h->stream;
   const int W = h->cfg.world_size, rk = h->cfg.world_rank;
-  Scratch tmp(h);
+  Scratch tmp(h->stream);
   uint64_t *ka = nullptr, *kb = nullptr;
   uint32_t *va = nullptr, *vb = nullptr;
   CK(h, tmp.alloc(&ka, (size_t)nnz));
@@ -630,7 +676,7 @@ static int build_side(pio_als_handle* h, Side& row, const Side& col, const int* 
 
 static int rank_rows(pio_als_handle* h, Side& s) {
   cudaStream_t st = h->stream;
-  Scratch tmp(h);
+  Scratch tmp(h->stream);
   uint64_t *ka = nullptr, *kb = nullptr;
   uint32_t *va = nullptr, *vb = nullptr;
   CK(h, tmp.alloc(&ka, (size_t)s.n));
@@ -663,7 +709,7 @@ static int exchange_events(pio_als_handle* h, Scratch& keep, uint64_t* ka, uint3
   cudaStream_t st = h->stream;
   NcclApi& nc = nccl_api();
   const int W = h->cfg.world_size, me = h->cfg.world_rank;
-  Scratch tmp(h);
+  Scratch tmp(h->stream);
   bool in_b = false;
   if (n > 0) CK(h, radix_sort_pairs(ka, va, kb, vb, (size_t)n, ceil_log2((uint64_t)W), st, &in_b, &h->st.kernel_launches));
   const uint64_t* ks = in_b ? kb : ka;
@@ -766,7 +812,7 @@ static int ingest_device(pio_als_handle* h, const int* d_user, const int* d_item
   if (bad) return fail(h, PIO_ALS_ERR_ARG, "%d ratings have a user/item index out of range", bad);
 
   mark("validate");
-  Scratch tmp(h);   // everything temporary: released on every exit path, including the CK() early returns
+  Scratch tmp(h->stream);   // everything temporary: released on every exit path, including the CK() early returns
   // 0. sharded + dedup: first bring all events of a user to one rank (user mod W), keeping the event order
   const int* su = d_user;
   const int* si = d_item;
@@ -774,7 +820,7 @@ static int ingest_device(pio_als_handle* h, const int* d_user, const int* d_item
   const long long* sts = d_ts;
   long long ns = nnz;
   if (sharded && dedup != PIO_ALS_DEDUP_NONE) {
-    Scratch xs(h);
+    Scratch xs(h->stream);
     uint64_t *ka = nullptr, *kb = nullptr;
     uint32_t *va = nullptr, *vb = nullptr;
     CK(h, xs.alloc(&ka, (size_t)nnz)); CK(h, xs.alloc(&kb, (size_t)nnz));
@@ -798,7 +844,7 @@ static int ingest_device(pio_als_handle* h, const int* d_user, const int* d_item
   const float* cr = sr;
   long long n2 = ns;
   if (dedup != PIO_ALS_DEDUP_NONE && ns > 0) {
-    Scratch ds(h);
+    Scratch ds(h->stream);
     uint64_t *ka = nullptr, *kb = nullptr;
     uint32_t *va = nullptr, *vb = nullptr;
     CK(h, ds.alloc(&ka, (size_t)ns)); CK(h, ds.alloc(&kb, (size_t)ns));
@@ -896,7 +942,7 @@ static int ingest_device(pio_als_handle* h, const int* d_user, const int* d_item
   } else {
     struct { Side* row; Side* col; const int* rowext; const int* colext; } jobs[2] = {{&U, &I, cu, ci}, {&I, &U, ci, cu}};
     for (auto& j : jobs) {
-      Scratch xs(h), recv(h);
+      Scratch xs(h->stream), recv(h->stream);
       uint64_t *ka = nullptr, *kb = nullptr;
       uint32_t *va = nullptr, *vb = nullptr;
       CK(h, xs.alloc(&ka, (size_t)n2)); CK(h, xs.alloc(&kb, (size_t)n2));
@@ -1523,7 +1569,7 @@ static int set_ratings_impl(pio_als_handle* h, const int32_t* user, const int32_
   cudaEventRecord(a, st);
   int rc;
   {
-    Scratch tmp(h);
+    Scratch tmp(h->stream);
     const int *du = user, *di = item;
     const float* dr = rating;
     const long long* dts = (const long long*)ts;
@@ -2130,7 +2176,7 @@ static int similar_one(pio_als_handle* h, const int32_t* query_items, int nq, in
   cudaStream_t st = h->stream;
   const int KP = h->KP, k = h->cfg.rank;
   const int keep_query = (flags & PIO_ALS_SIM_KEEP_QUERY_ITEMS) ? 1 : 0;
-  Scratch tmp(h);
+  Scratch tmp(h->stream);
   int* d_q = nullptr;
   float* d_qf = nullptr;
   uint8_t* d_valid = nullptr;
@@ -2195,7 +2241,7 @@ int pio_als_recommend(pio_als_handle* h, const int32_t* users, int n, int topk, 
     return recommend_small(h, p, users, n, topk, item_mask, item_weight, out_items, out_scores, out_count);
   cudaStream_t st = h->stream;
   const int KP = h->KP;
-  Scratch tmp(h);
+  Scratch tmp(h->stream);
   int* d_users = nullptr;
   float* d_xq = nullptr;
   uint8_t* d_valid = nullptr;
@@ -2243,7 +2289,7 @@ int pio_als_similar_batch(pio_als_handle* h, const int64_t* q_ptr, const int32_t
     return similar_small(h, p, q_items + q_ptr[0], (int)(q_ptr[1] - q_ptr[0]), topk, item_mask, item_weight, flags,
                          out_items, out_scores, out_count);
   cudaStream_t st = h->stream;
-  Scratch tmp(h);
+  Scratch tmp(h->stream);
   DevFilter f;
   int rc = upload_filter(h, item_mask, item_weight, &tmp, 0, &f);
   if (rc) return rc;
@@ -2366,7 +2412,7 @@ int pio_als_model_import(const pio_als_config* cfg_in, const float* user_factors
       CK(h, dalloc(h, &s.perm, j.n)); CK(h, dalloc(h, &s.inv, j.n)); CK(h, dalloc(h, &s.deg, j.n));
       CK(h, dalloc(h, &s.npos, j.n)); CK(h, dalloc(h, &s.cand_ext, j.n));
       CK(h, dalloc(h, &s.F, j.n * (size_t)h->KP));
-      Scratch tmp(h);
+      Scratch tmp(h->stream);
       uint8_t* dh = nullptr;
       float* dfac = nullptr;
       if (j.has) {
@@ -2508,12 +2554,13 @@ __attribute__((visibility("default"))) int pio_als_debug_lockstep(int device, in
                                                                   int* fail_out) {
   if ((N != 64 && N != 128) || n < 1 || !A || !b || !x) return PIO_ALS_ERR_ARG;
   CK0(cudaSetDevice(device));
+  CallMem tmp(0);
   float *dA = nullptr, *db = nullptr, *dx = nullptr;
   int* dfail = nullptr;
-  CK0(cudaMalloc((void**)&dA, sizeof(float) * (size_t)n * N * N));
-  CK0(cudaMalloc((void**)&db, sizeof(float) * (size_t)n * N));
-  CK0(cudaMalloc((void**)&dx, sizeof(float) * (size_t)n * N));
-  CK0(cudaMalloc((void**)&dfail, sizeof(int)));
+  CK0(tmp.device(&dA, (size_t)n * N * N));
+  CK0(tmp.device(&db, (size_t)n * N));
+  CK0(tmp.device(&dx, (size_t)n * N));
+  CK0(tmp.device(&dfail, 1));
   CK0(cudaMemset(dfail, 0, sizeof(int)));
   CK0(cudaMemcpy(dA, A, sizeof(float) * (size_t)n * N * N, cudaMemcpyHostToDevice));
   CK0(cudaMemcpy(db, b, sizeof(float) * (size_t)n * N, cudaMemcpyHostToDevice));
@@ -2525,8 +2572,8 @@ __attribute__((visibility("default"))) int pio_als_debug_lockstep(int device, in
   const int cap = pr_.multiProcessorCount * (N == 64 ? 12 : 6);
   if (grid > cap) grid = cap;
   cudaEvent_t e0, e1;
-  cudaEventCreate(&e0);
-  cudaEventCreate(&e1);
+  CK0(tmp.event(&e0));
+  CK0(tmp.event(&e1));
   if (N == 64) {
     CK0(cudaFuncSetAttribute(lockstep_probe_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     CK0(cudaFuncSetAttribute(lockstep_probe_kernel<64>, cudaFuncAttributePreferredSharedMemoryCarveout, 100));
@@ -2539,15 +2586,13 @@ __attribute__((visibility("default"))) int pio_als_debug_lockstep(int device, in
     lockstep_probe_kernel<128><<<grid, 32, smem>>>(dA, db, n, ridge, dx, reps < 1 ? 1 : reps, dfail);
   }
   cudaEventRecord(e1);
+  CK0(cudaGetLastError());
   CK0(cudaDeviceSynchronize());
   float ms = 0.f;
   cudaEventElapsedTime(&ms, e0, e1);
   if (ms_out) *ms_out = ms;
   CK0(cudaMemcpy(x, dx, sizeof(float) * (size_t)n * N, cudaMemcpyDeviceToHost));
   if (fail_out) CK0(cudaMemcpy(fail_out, dfail, sizeof(int), cudaMemcpyDeviceToHost));
-  cudaEventDestroy(e0);
-  cudaEventDestroy(e1);
-  cudaFree(dA); cudaFree(db); cudaFree(dx); cudaFree(dfail);
   return PIO_ALS_OK;
 }
 
@@ -2576,25 +2621,9 @@ static int ids_encode_device(const uint8_t* d_bytes, const long long* d_off, int
   uint64_t *ka = nullptr, *kb = nullptr;
   uint32_t *va = nullptr, *vb = nullptr, *f1 = nullptr, *f2 = nullptr, *run_start = nullptr, *head = nullptr, *ishead = nullptr,
            *firstpos = nullptr, *isfirst = nullptr;
-  std::vector<void*> owned;
-  auto A = [&](void** p, size_t bytes_) -> cudaError_t {
-    cudaError_t e = cudaMalloc(p, bytes_ ? bytes_ : 1);
-    if (e == cudaSuccess) owned.push_back(*p);
-    return e;
-  };
-  struct Guard {
-    std::vector<void*>& v;
-    cudaStream_t s;
-    ~Guard() {
-      cudaStreamSynchronize(s);
-      for (void* q : v) cudaFree(q);
-    }
-  } guard{owned, st};
-  CK0(A((void**)&ka, 8 * (size_t)n)); CK0(A((void**)&kb, 8 * (size_t)n));
-  CK0(A((void**)&va, 4 * (size_t)n)); CK0(A((void**)&vb, 4 * (size_t)n));
-  CK0(A((void**)&f1, 4 * (size_t)n)); CK0(A((void**)&f2, 4 * (size_t)n));
-  CK0(A((void**)&run_start, 4 * (size_t)n)); CK0(A((void**)&head, 4 * (size_t)n)); CK0(A((void**)&ishead, 4 * (size_t)n));
-  CK0(A((void**)&firstpos, 4 * (size_t)n)); CK0(A((void**)&isfirst, 4 * (size_t)n));
+  CallMem tmp(st);
+  for (uint64_t** p : {&ka, &kb}) CK0(tmp.device(p, (size_t)n));
+  for (uint32_t** p : {&va, &vb, &f1, &f2, &run_start, &head, &ishead, &firstpos, &isfirst}) CK0(tmp.device(p, (size_t)n));
   ids_hash_kernel<<<nblk(n, 256), 256, 0, st>>>(d_bytes, d_off, n, ka, va, ids_hash_mask());
   bool in_b = false;
   CK0(radix_sort_pairs(ka, va, kb, vb, (size_t)n, 64, st, &in_b, nullptr));
@@ -2631,18 +2660,12 @@ int pio_ids_encode(int device, const uint8_t* bytes, const int64_t* offsets, int
   uint8_t* d_bytes = nullptr;
   long long *d_off = nullptr, *d_first = nullptr;
   int* d_out = nullptr;
-  std::vector<void*> owned;
-  auto A = [&](void** p, size_t bytes_) -> cudaError_t {
-    cudaError_t e = cudaMalloc(p, bytes_ ? bytes_ : 1);
-    if (e == cudaSuccess) owned.push_back(*p);
-    return e;
-  };
-  struct Guard { std::vector<void*>& v; ~Guard() { for (void* q : v) cudaFree(q); } } guard{owned};
-  CK0(A((void**)&d_bytes, nb));
-  CK0(A((void**)&d_off, sizeof(long long) * (n + 1)));
-  CK0(A((void**)&d_out, 4 * (size_t)n));
-  CK0(A((void**)&d_first, 8 * (size_t)n));
   cudaStream_t st = 0;
+  CallMem tmp(st);
+  CK0(tmp.device(&d_bytes, nb));
+  CK0(tmp.device(&d_off, (size_t)n + 1));
+  CK0(tmp.device(&d_out, (size_t)n));
+  CK0(tmp.device(&d_first, (size_t)n));
   CK0(cudaMemcpyAsync(d_bytes, bytes, nb, cudaMemcpyHostToDevice, st));
   CK0(cudaMemcpyAsync(d_off, offsets, sizeof(long long) * (n + 1), cudaMemcpyHostToDevice, st));
   int64_t nuniq = 0;
@@ -2686,90 +2709,38 @@ struct EvKeyArgs {
   int64_t* out_tok_off;
 };
 
-// ---- event index (pio_events_index_*; events_index.cuh) --------------------------------------------------------------
-static void eix_free(EixRun& r) {
-  void* ps[7] = {r.hash, r.time_us, r.off, r.len, r.id_off, r.id_len, r.arena};
-  for (void* q : ps) cudaFree(q);
-  r = EixRun{};
-}
-
-// device arrays of a run for n entries and `bytes` arena bytes (bytes < 0: no arena); nothing is copied
-static cudaError_t eix_alloc(EixRun& r, long long n, long long bytes) {
-  const size_t m = n > 0 ? (size_t)n : 1;
-  cudaError_t e;
-  if ((e = cudaMalloc((void**)&r.hash, 8 * m)) != cudaSuccess) return e;
-  if ((e = cudaMalloc((void**)&r.time_us, 8 * m)) != cudaSuccess) return e;
-  if ((e = cudaMalloc((void**)&r.off, 8 * m)) != cudaSuccess) return e;
-  if ((e = cudaMalloc((void**)&r.len, 4 * m)) != cudaSuccess) return e;
-  if ((e = cudaMalloc((void**)&r.id_off, 8 * m)) != cudaSuccess) return e;
-  if ((e = cudaMalloc((void**)&r.id_len, 4 * m)) != cudaSuccess) return e;
-  return bytes < 0 ? cudaSuccess : cudaMalloc((void**)&r.arena, bytes > 0 ? (size_t)bytes : 1);
-}
-
-// The entries of one append in file order, grown chunk by chunk: the chunk loop of events_scan_impl puts a chunk's
-// matched events here instead of copying them to the host.  The arena is the scan's entityId column.
-struct EixBatch {
-  EixRun r;
-  long long cap_n = 0, cap_bytes = 0;
-  long long file_base = 0;   // file offset of the scanned text's first byte
-  uint64_t mask = ~0ull;
+// where pio_events_scan and pio_events_scan_keys put the matched events: host columns of `capacity` events, n taken
+struct EvHostCols {
+  int64_t capacity;
+  int64_t* line;
+  int32_t* code;
+  double* value;
+  uint8_t* flags;
+  int64_t* time_us;
+  uint8_t* eid_bytes;
+  int64_t* eid_off;
+  uint8_t* tid_bytes;
+  int64_t* tid_off;
+  int64_t n;
 };
 
-static int eix_reserve(EixBatch* b, long long n, long long bytes, cudaStream_t st) {
-  if (n <= b->cap_n && bytes <= b->cap_bytes) return PIO_ALS_OK;
-  const long long cn = n > 2 * b->cap_n ? n : 2 * b->cap_n, cb = bytes > 2 * b->cap_bytes ? bytes : 2 * b->cap_bytes;
-  EixRun g;
-  const cudaError_t e = eix_alloc(g, cn, cb);
-  if (e != cudaSuccess) {
-    eix_free(g);
-    return fail(nullptr, PIO_ALS_ERR_CUDA, "event index: %s", cudaGetErrorString(e));
-  }
-  const EixRun& r = b->r;
-  const size_t m = (size_t)r.n;
-  CK0(cudaMemcpyAsync(g.hash, r.hash, 8 * m, cudaMemcpyDeviceToDevice, st));
-  CK0(cudaMemcpyAsync(g.time_us, r.time_us, 8 * m, cudaMemcpyDeviceToDevice, st));
-  CK0(cudaMemcpyAsync(g.off, r.off, 8 * m, cudaMemcpyDeviceToDevice, st));
-  CK0(cudaMemcpyAsync(g.len, r.len, 4 * m, cudaMemcpyDeviceToDevice, st));
-  CK0(cudaMemcpyAsync(g.id_off, r.id_off, 8 * m, cudaMemcpyDeviceToDevice, st));
-  CK0(cudaMemcpyAsync(g.id_len, r.id_len, 4 * m, cudaMemcpyDeviceToDevice, st));
-  CK0(cudaMemcpyAsync(g.arena, r.arena, (size_t)r.arena_bytes, cudaMemcpyDeviceToDevice, st));
-  CK0(cudaStreamSynchronize(st));
-  g.n = r.n;
-  g.arena_bytes = r.arena_bytes;
-  eix_free(b->r);
-  b->r = g;
-  b->cap_n = cn, b->cap_bytes = cb;
-  return PIO_ALS_OK;
-}
+// the lines a scan leaves to the host, in line order: line number (line may be NULL) and byte range without the
+// terminator, for the first `capacity`; n counts every one
+struct EvFallback {
+  int64_t capacity;
+  int64_t* line;
+  int64_t* begin;
+  int64_t* end;
+  int64_t n;
+};
 
-// one chunk's nm matched events (o, line order) and their eb id bytes, which start at eid_base in the call's id column
-static int eix_take_chunk(EixBatch* b, const EvOut& o, const uint8_t* t, const uint32_t* starts, const EvBase& here,
-                          long long eid_base, int64_t nm, int64_t eb, cudaStream_t st) {
-  if (nm == 0) return PIO_ALS_OK;
-  const int rc = eix_reserve(b, b->r.n + nm, eid_base + eb, st);
-  if (rc != PIO_ALS_OK) return rc;
-  CK0(cudaMemcpyAsync(b->r.arena + eid_base, o.eid_bytes, (size_t)eb, cudaMemcpyDeviceToDevice, st));
-  eix_take_kernel<<<nblk(nm, 256), 256, 0, st>>>(o, t, starts, nm, here.line, b->file_base + here.byte, eid_base + eb,
-                                                 b->mask, b->r, b->r.n);
-  CK0(cudaGetLastError());
-  b->r.n += nm;
-  b->r.arena_bytes = eid_base + eb;
-  return PIO_ALS_OK;
-}
+// one parsed chunk: matched events, fallback lines, entityId, targetEntityId and token bytes
+struct EvTotals {
+  int64_t nm, nf, eb, tb, tk;
+};
 
-// pio_events_scan (ka == nullptr) and pio_events_scan_keys: one chunk loop, the kernels instantiated with KEYS = ka != 0
-static int events_scan_impl(int device, const uint8_t* text, int64_t n_bytes, const pio_events_filter* f,
-                            int64_t capacity, int64_t* out_line, int32_t* out_code, double* out_value, uint8_t* out_flags,
-                            int64_t* out_time_us, uint8_t* out_eid_bytes, int64_t* out_eid_off, uint8_t* out_tid_bytes,
-                            int64_t* out_tid_off, int64_t* out_n_events, int64_t fb_capacity, int64_t* out_fb_line,
-                            int64_t* out_fb_begin, int64_t* out_fb_end, int64_t* out_n_fallback, int64_t* out_n_lines,
-                            const EvKeyArgs* ka, EixBatch* sink = nullptr) {
-  const bool cols = sink == nullptr;   // host columns; with a sink the matched events stay on the device
-  if (n_bytes < 0 || (n_bytes > 0 && !text) || !f || fb_capacity < 0 || (cols && (capacity < n_bytes /
-      PIO_EVENTS_MIN_EVENT_BYTES + 1 || !out_line || !out_code || !out_value || !out_flags || !out_time_us ||
-      !out_eid_bytes || !out_eid_off || !out_tid_bytes || !out_tid_off || !out_n_events)) || (fb_capacity > 0 &&
-      (!out_fb_line || !out_fb_begin || !out_fb_end)) || !out_n_fallback || !out_n_lines)
-    return fail(nullptr, PIO_ALS_ERR_ARG, "bad pio_events_scan arguments");
+// the checks of a scan's filter or an index view, made before any CUDA call
+static int ev_check_filter(const pio_events_filter* f) {
   if (f->n_event_names < 0 || (f->n_event_names > 0 && !f->event_names))
     return fail(nullptr, PIO_ALS_ERR_ARG, "bad event name list");
   for (int k = 0; k < f->n_event_names; ++k)
@@ -2777,14 +2748,13 @@ static int events_scan_impl(int device, const uint8_t* text, int64_t n_bytes, co
   if (f->target_entity_type_mode < PIO_EVENTS_TARGET_ANY || f->target_entity_type_mode > PIO_EVENTS_TARGET_EQUALS ||
       (f->target_entity_type_mode == PIO_EVENTS_TARGET_EQUALS && !f->target_entity_type))
     return fail(nullptr, PIO_ALS_ERR_ARG, "bad target_entity_type_mode / target_entity_type");
-  const int nk = ka ? ka->n : 0;
-  *out_n_fallback = *out_n_lines = 0;
-  if (cols) *out_n_events = 0, out_eid_off[0] = out_tid_off[0] = 0;
-  if (ka) ka->out_tok_off[0] = 0;
-  if (n_bytes == 0) return PIO_ALS_OK;
-  CK0(cudaSetDevice(device));
+  return PIO_ALS_OK;
+}
 
-  // the filter's strings, packed: entity type | target entity type | property | names...
+// the filter's strings and the nk tracked keys on the device, in tmp: the parse kernels' filter and key list
+static int ev_upload_filter(const pio_events_filter* f, const char* const* keys, int nk, CallMem& tmp, ev::Filter* df,
+                            ev::KeyList* dk) {
+  // packed: entity type | target entity type | property | names... | keys...
   std::vector<uint8_t> fbytes;
   auto put = [&](const char* s) -> int {
     const size_t at = fbytes.size();
@@ -2802,12 +2772,165 @@ static int events_scan_impl(int device, const uint8_t* text, int64_t n_bytes, co
     put(f->event_names[k]);
     noff.push_back((int)fbytes.size());
   }
-  std::vector<int> koff(1, (int)fbytes.size());   // then the tracked keys
+  std::vector<int> koff(1, (int)fbytes.size());
   for (int q = 0; q < nk; ++q) {
-    put(ka->keys[q]);
+    put(keys[q]);
     koff.push_back((int)fbytes.size());
   }
+  uint8_t* d_fbytes = nullptr;
+  int *d_noff = nullptr, *d_koff = nullptr;
+  CK0(tmp.device(&d_fbytes, fbytes.size()));
+  CK0(tmp.device(&d_noff, noff.size()));
+  CK0(tmp.device(&d_koff, koff.size()));
+  if (!fbytes.empty()) CK0(cudaMemcpy(d_fbytes, fbytes.data(), fbytes.size(), cudaMemcpyHostToDevice));
+  CK0(cudaMemcpy(d_noff, noff.data(), sizeof(int) * noff.size(), cudaMemcpyHostToDevice));
+  CK0(cudaMemcpy(d_koff, koff.data(), sizeof(int) * koff.size(), cudaMemcpyHostToDevice));
+  df->entity_type = d_fbytes + at_et;
+  df->entity_type_len = len_et;
+  df->names = d_fbytes;
+  df->name_off = d_noff;
+  df->n_names = f->event_names ? f->n_event_names : -1;   // NULL: any name; an empty list: none
+  df->target_mode = f->target_entity_type_mode;
+  df->target = d_fbytes + at_tt;
+  df->target_len = len_tt;
+  df->prop = d_fbytes + at_pr;
+  df->prop_len = len_pr;
+  df->has_start = f->has_start != 0;
+  df->has_until = f->has_until != 0;
+  df->start_us = f->start_us;
+  df->until_us = f->until_us;
+  dk->names = d_fbytes;
+  dk->off = d_koff;
+  dk->n = nk;
+  return PIO_ALS_OK;
+}
 
+// the parse and compaction kernels of a scan with (keys) or without tracked keys; smem: the parse that stages its lines
+// in shared memory
+struct EvKernels {
+  decltype(&ev_parse_kernel<false>) parse;
+  decltype(&ev_compact_kernel<false>) compact;
+};
+static EvKernels ev_kernels(bool keys, bool smem) {
+  if (keys) return {smem ? ev_parse_smem_kernel<true> : ev_parse_kernel<true>, ev_compact_kernel<true>};
+  return {smem ? ev_parse_smem_kernel<false> : ev_parse_kernel<false>, ev_compact_kernel<false>};
+}
+
+// Delivery into host columns: a parsed chunk's matched events, and with ka their key columns, after those of the chunks
+// before it (here: its id bytes; K.tok_base: its token bytes).  The offset columns are closed after each chunk; the
+// next chunk's first event overwrites the closing entries with the same values.
+static int ev_take_host(EvHostCols& c, const EvKeyArgs* ka, const EvOut& o, const EvKeys& K, const EvBase& here,
+                        const EvTotals& tot, cudaStream_t st) {
+  const int64_t n = c.n, nm = tot.nm;
+  if (n + nm > c.capacity) return fail(nullptr, PIO_ALS_ERR_ARG, "more matched events than capacity");
+  CK0(cudaMemcpyAsync(c.line + n, o.line, 8 * nm, cudaMemcpyDeviceToHost, st));
+  CK0(cudaMemcpyAsync(c.code + n, o.code, 4 * nm, cudaMemcpyDeviceToHost, st));
+  CK0(cudaMemcpyAsync(c.value + n, o.value, 8 * nm, cudaMemcpyDeviceToHost, st));
+  CK0(cudaMemcpyAsync(c.flags + n, o.flags, nm, cudaMemcpyDeviceToHost, st));
+  CK0(cudaMemcpyAsync(c.time_us + n, o.time_us, 8 * nm, cudaMemcpyDeviceToHost, st));
+  CK0(cudaMemcpyAsync(c.eid_off + n, o.eid_off, 8 * nm, cudaMemcpyDeviceToHost, st));
+  CK0(cudaMemcpyAsync(c.tid_off + n, o.tid_off, 8 * nm, cudaMemcpyDeviceToHost, st));
+  CK0(cudaMemcpyAsync(c.eid_bytes + here.eid, o.eid_bytes, tot.eb, cudaMemcpyDeviceToHost, st));
+  CK0(cudaMemcpyAsync(c.tid_bytes + here.tid, o.tid_bytes, tot.tb, cudaMemcpyDeviceToHost, st));
+  c.n += nm;
+  c.eid_off[c.n] = here.eid + tot.eb, c.tid_off[c.n] = here.tid + tot.tb;
+  if (ka) {
+    const int nk = ka->n;
+    CK0(cudaMemcpyAsync(ka->out_present + n, K.o_present, nm, cudaMemcpyDeviceToHost, st));
+    CK0(cudaMemcpyAsync(ka->out_number + n, K.o_number, nm, cudaMemcpyDeviceToHost, st));
+    CK0(cudaMemcpyAsync(ka->out_num + n * nk, K.o_num, 8 * nm * nk, cudaMemcpyDeviceToHost, st));
+    CK0(cudaMemcpyAsync(ka->out_tok_off + n * nk, K.o_tok_off, 8 * nm * nk, cudaMemcpyDeviceToHost, st));
+    CK0(cudaMemcpyAsync(ka->out_tok_bytes + K.tok_base, K.o_tok, tot.tk, cudaMemcpyDeviceToHost, st));
+    ka->out_tok_off[c.n * nk] = K.tok_base + tot.tk;
+  }
+  return PIO_ALS_OK;
+}
+
+// ---- event index (pio_events_index_*; events_index.cuh) --------------------------------------------------------------
+// the entry columns of a run, n entries each, and their entry sizes (the arena, of arena_bytes, is apart)
+struct EixCol {
+  void** p;
+  size_t size;
+};
+static std::array<EixCol, 6> eix_cols(EixRun& r) {
+  return {{{(void**)&r.hash, sizeof *r.hash}, {(void**)&r.time_us, sizeof *r.time_us}, {(void**)&r.off, sizeof *r.off},
+           {(void**)&r.len, sizeof *r.len}, {(void**)&r.id_off, sizeof *r.id_off}, {(void**)&r.id_len, sizeof *r.id_len}}};
+}
+
+static void eix_free(EixRun& r) {
+  for (const EixCol& c : eix_cols(r)) cudaFree(*c.p);
+  cudaFree(r.arena);
+  r = EixRun{};
+}
+
+// device arrays of a run for n entries and `bytes` arena bytes (bytes < 0: no arena); nothing is copied
+static cudaError_t eix_alloc(EixRun& r, long long n, long long bytes) {
+  const size_t m = n > 0 ? (size_t)n : 1;
+  for (const EixCol& c : eix_cols(r)) {
+    const cudaError_t e = cudaMalloc(c.p, c.size * m);
+    if (e != cudaSuccess) return e;
+  }
+  return bytes < 0 ? cudaSuccess : cudaMalloc((void**)&r.arena, bytes > 0 ? (size_t)bytes : 1);
+}
+
+// The entries of one append in file order, grown chunk by chunk: ev_scan puts a chunk's matched events here instead of
+// copying them to the host.  The arena is the scan's entityId column.  The batch owns its run.
+struct EixBatch {
+  EixRun r;
+  long long cap_n = 0, cap_bytes = 0;
+  long long file_base = 0;   // file offset of the scanned text's first byte
+  uint64_t mask = ~0ull;
+  EixBatch() = default;
+  EixBatch(const EixBatch&) = delete;
+  EixBatch& operator=(const EixBatch&) = delete;
+  ~EixBatch() { eix_free(r); }
+};
+
+static int eix_reserve(EixBatch* b, long long n, long long bytes, cudaStream_t st) {
+  if (n <= b->cap_n && bytes <= b->cap_bytes) return PIO_ALS_OK;
+  const long long cn = n > 2 * b->cap_n ? n : 2 * b->cap_n, cb = bytes > 2 * b->cap_bytes ? bytes : 2 * b->cap_bytes;
+  EixRun g;
+  cudaError_t e = eix_alloc(g, cn, cb);
+  const auto to = eix_cols(g), from = eix_cols(b->r);
+  for (size_t k = 0; k < to.size() && e == cudaSuccess; ++k)
+    e = cudaMemcpyAsync(*to[k].p, *from[k].p, to[k].size * (size_t)b->r.n, cudaMemcpyDeviceToDevice, st);
+  if (e == cudaSuccess) e = cudaMemcpyAsync(g.arena, b->r.arena, (size_t)b->r.arena_bytes, cudaMemcpyDeviceToDevice, st);
+  if (e == cudaSuccess) e = cudaStreamSynchronize(st);
+  if (e != cudaSuccess) {
+    eix_free(g);
+    return fail(nullptr, PIO_ALS_ERR_CUDA, "event index: %s", cudaGetErrorString(e));
+  }
+  g.n = b->r.n;
+  g.arena_bytes = b->r.arena_bytes;
+  eix_free(b->r);
+  b->r = g;
+  b->cap_n = cn, b->cap_bytes = cb;
+  return PIO_ALS_OK;
+}
+
+// Delivery into an index batch: one chunk's nm matched events (o, line order) and their eb id bytes, which start at
+// eid_base in the call's id column
+static int eix_take_chunk(EixBatch* b, const EvOut& o, const uint8_t* t, const uint32_t* starts, const EvBase& here,
+                          long long eid_base, int64_t nm, int64_t eb, cudaStream_t st) {
+  if (nm == 0) return PIO_ALS_OK;
+  const int rc = eix_reserve(b, b->r.n + nm, eid_base + eb, st);
+  if (rc != PIO_ALS_OK) return rc;
+  CK0(cudaMemcpyAsync(b->r.arena + eid_base, o.eid_bytes, (size_t)eb, cudaMemcpyDeviceToDevice, st));
+  eix_take_kernel<<<nblk(nm, 256), 256, 0, st>>>(o, t, starts, nm, here.line, b->file_base + here.byte, eid_base + eb,
+                                                 b->mask, b->r, b->r.n);
+  CK0(cudaGetLastError());
+  b->r.n += nm;
+  b->r.arena_bytes = eid_base + eb;
+  return PIO_ALS_OK;
+}
+
+// The chunk loop of every event scan, over text[0, n_bytes) (n_bytes > 0, f checked): cuts the text into device chunks,
+// stages each through pinned memory on a copy stream, and parses, scans and compacts it on the scan stream.  Each
+// chunk's matched events are delivered to the host columns `cols` (with ka: and their key columns) or, when batch is
+// set, into that index batch.  Lines longer than a chunk and the lines the device leaves to the host go to *fb.
+static int ev_scan(int device, const uint8_t* text, int64_t n_bytes, const pio_events_filter* f, const EvKeyArgs* ka,
+                   EvHostCols* cols, EixBatch* batch, EvFallback* fb, int64_t* n_lines) {
+  CK0(cudaSetDevice(device));
   int64_t cap = 64ll << 20;   // device chunk; PIO_EVENTS_DEVICE_CHUNK (bytes) lets tests straddle its boundaries
   if (const char* c = getenv("PIO_EVENTS_DEVICE_CHUNK")) {
     const long long v = atoll(c);
@@ -2815,98 +2938,51 @@ static int events_scan_impl(int device, const uint8_t* text, int64_t n_bytes, co
   }
   if (cap > n_bytes) cap = n_bytes;
 
-  std::vector<void*> owned, pinned;
-  cudaStream_t streams[2] = {nullptr, nullptr};
+  CallMem tmp;
+  cudaStream_t ex = nullptr, cp = nullptr;   // scan, host-to-device copies
   // copy begin / end per staging slot, then on the scan stream: kernels before and after the line count, and the
   // device-to-host copies (pio_events_debug_timing)
   cudaEvent_t evs[10] = {};
   cudaEvent_t *h2d_begin = evs, *copied = evs + 2, &k0 = evs[4], &k1 = evs[5], &k2 = evs[6], &k3 = evs[7],
               &d0 = evs[8], &d1 = evs[9];
-  struct Guard {
-    std::vector<void*>& d;
-    std::vector<void*>& p;
-    cudaStream_t* s;
-    cudaEvent_t* e;
-    ~Guard() {
-      for (int k = 0; k < 2; ++k)
-        if (s[k]) cudaStreamSynchronize(s[k]);
-      for (void* q : d) cudaFree(q);
-      for (void* q : p) cudaFreeHost(q);
-      for (int k = 0; k < 2; ++k)
-        if (s[k]) cudaStreamDestroy(s[k]);
-      for (int k = 0; k < 10; ++k)
-        if (e[k]) cudaEventDestroy(e[k]);
-    }
-  } guard{owned, pinned, streams, evs};
-  auto A = [&](void** p, size_t bytes_) -> cudaError_t {
-    cudaError_t e = cudaMalloc(p, bytes_ ? bytes_ : 1);
-    if (e == cudaSuccess) owned.push_back(*p);
-    return e;
-  };
-  auto P = [&](void** p, size_t bytes_) -> cudaError_t {
-    cudaError_t e = cudaHostAlloc(p, bytes_ ? bytes_ : 1, cudaHostAllocDefault);
-    if (e == cudaSuccess) pinned.push_back(*p);
-    return e;
-  };
-  for (int k = 0; k < 2; ++k) CK0(cudaStreamCreateWithFlags(&streams[k], cudaStreamNonBlocking));
-  for (cudaEvent_t& e : evs) CK0(cudaEventCreate(&e));
+  CK0(tmp.stream(&ex));
+  CK0(tmp.stream(&cp));
+  for (cudaEvent_t& e : evs) CK0(tmp.event(&e));
   EvTiming& tm = g_ev_timing;
   tm = EvTiming{};
   bool use_smem = true;   // PIO_EVENTS_SMEM=0: the parse reads its lines from global memory (A/B measurements)
   if (const char* c = getenv("PIO_EVENTS_SMEM")) use_smem = atoi(c) != 0;
-  if (use_smem)
-    CK0(cudaFuncSetAttribute(ka ? ev_parse_smem_kernel<true> : ev_parse_smem_kernel<false>,
-                             cudaFuncAttributeMaxDynamicSharedMemorySize, EV_SMEM_BYTES));
-  cudaStream_t ex = streams[0], cp = streams[1];   // scan, host-to-device copies
-  uint8_t *d_text[2] = {nullptr, nullptr}, *stage[2] = {nullptr, nullptr}, *d_scratch = nullptr, *d_fbytes = nullptr;
+  const EvKernels kn = ev_kernels(ka != nullptr, use_smem);
+  if (use_smem) CK0(cudaFuncSetAttribute(kn.parse, cudaFuncAttributeMaxDynamicSharedMemorySize, EV_SMEM_BYTES));
+  uint8_t *d_text[2] = {nullptr, nullptr}, *stage[2] = {nullptr, nullptr}, *d_scratch = nullptr;
   uint32_t *d_flag = nullptr, *d_lid = nullptr, *d_tot = nullptr, *h_tot = nullptr;
-  int *d_noff = nullptr, *d_koff = nullptr;
   for (int k = 0; k < 2; ++k) {
-    CK0(A((void**)&d_text[k], (size_t)cap));
-    CK0(P((void**)&stage[k], (size_t)cap));
+    CK0(tmp.device(&d_text[k], (size_t)cap));
+    CK0(tmp.host(&stage[k], (size_t)cap));
   }
-  CK0(A((void**)&d_scratch, (size_t)cap));
-  CK0(A((void**)&d_flag, 4 * (size_t)cap));
-  CK0(A((void**)&d_lid, 4 * (size_t)cap));
-  CK0(A((void**)&d_fbytes, fbytes.size()));
-  CK0(A((void**)&d_noff, sizeof(int) * noff.size()));
-  CK0(A((void**)&d_tot, 4 * sizeof(uint32_t)));
-  CK0(P((void**)&h_tot, 8 * sizeof(uint32_t)));
-  if (!fbytes.empty()) CK0(cudaMemcpy(d_fbytes, fbytes.data(), fbytes.size(), cudaMemcpyHostToDevice));
-  CK0(cudaMemcpy(d_noff, noff.data(), sizeof(int) * noff.size(), cudaMemcpyHostToDevice));
-  CK0(A((void**)&d_koff, sizeof(int) * koff.size()));
-  CK0(cudaMemcpy(d_koff, koff.data(), sizeof(int) * koff.size(), cudaMemcpyHostToDevice));
+  CK0(tmp.device(&d_scratch, (size_t)cap));
+  CK0(tmp.device(&d_flag, (size_t)cap));
+  CK0(tmp.device(&d_lid, (size_t)cap));
+  CK0(tmp.device(&d_tot, 4));
+  CK0(tmp.host(&h_tot, 8));
   ev::Filter df;
-  df.entity_type = d_fbytes + at_et;
-  df.entity_type_len = len_et;
-  df.names = d_fbytes;
-  df.name_off = d_noff;
-  df.n_names = f->event_names ? f->n_event_names : -1;   // NULL: any name; an empty list: none
-  df.target_mode = f->target_entity_type_mode;
-  df.target = d_fbytes + at_tt;
-  df.target_len = len_tt;
-  df.prop = d_fbytes + at_pr;
-  df.prop_len = len_pr;
-  df.has_start = f->has_start != 0;
-  df.has_until = f->has_until != 0;
-  df.start_us = f->start_us;
-  df.until_us = f->until_us;
-
   EvKeys K{};
-  K.list.names = d_fbytes;
-  K.list.off = d_koff;
-  K.list.n = nk;
+  const int nk = ka ? ka->n : 0;
+  const int urc = ev_upload_filter(f, ka ? ka->keys : nullptr, nk, tmp, &df, &K.list);
+  if (urc != PIO_ALS_OK) return urc;
 
   EvBase base{0, 0, 0, 0};
-  int64_t n_ev = 0, n_fb = 0, n_tok = 0;   // n_tok: token bytes so far   // n_fb counts every fallback line, also those beyond fb_capacity
+  int64_t n_tok = 0;   // token bytes so far
   // lines longer than a chunk, found while cutting the next chunk: written after the current chunk's fallback lines so
   // that the fallback list stays in line order
   std::vector<int64_t> oversized;
   auto flush_oversized = [&]() {
     for (size_t k = 0; k < oversized.size(); k += 3) {
-      if (n_fb < fb_capacity)
-        out_fb_line[n_fb] = oversized[k], out_fb_begin[n_fb] = oversized[k + 1], out_fb_end[n_fb] = oversized[k + 2];
-      ++n_fb;
+      if (fb->n < fb->capacity) {
+        if (fb->line) fb->line[fb->n] = oversized[k];
+        fb->begin[fb->n] = oversized[k + 1], fb->end[fb->n] = oversized[k + 2];
+      }
+      ++fb->n;
     }
     oversized.clear();
   };
@@ -2964,82 +3040,61 @@ static int events_scan_impl(int device, const uint8_t* text, int64_t n_bytes, co
     CK0(cudaEventRecord(k1, ex));
     CK0(cudaStreamSynchronize(ex));
     const long long nl = (long long)h_tot[4] + h_tot[5];
-    const EvBase here = base;
+    const EvBase here = base;   // lines and text bytes before this chunk, and the call's id bytes
     base.line += nl;
 
-    std::vector<void*> chunk_mem;
-    struct ChunkGuard {
-      std::vector<void*>& v;
-      cudaStream_t s;
-      ~ChunkGuard() { for (void* q : v) cudaFreeAsync(q, s); }
-    } chunk_guard{chunk_mem, ex};
-    auto CA = [&](void** p, size_t bytes_) -> cudaError_t {
-      cudaError_t e = cudaMallocAsync(p, bytes_ ? bytes_ : 1, ex);
-      if (e == cudaSuccess) chunk_mem.push_back(*p);
-      return e;
-    };
+    Scratch chunk(ex);
     uint32_t* starts = nullptr;
     EvLines Ls;
     EvOut o;
     const size_t nls = (size_t)nl;
-    CK0(CA((void**)&starts, 4 * (nls + 1)));
-    uint32_t** u32s[8] = {&Ls.is_match, &Ls.is_fb, &Ls.eid_len, &Ls.tid_len, &Ls.match_pos, &Ls.fb_pos, &Ls.eid_pos,
-                          &Ls.tid_pos};
-    for (uint32_t** p : u32s) CK0(CA((void**)p, 4 * nls));
-    CK0(CA((void**)&Ls.code, 4 * nls));
-    CK0(CA((void**)&Ls.value, 8 * nls));
-    CK0(CA((void**)&Ls.time_us, 8 * nls));
-    CK0(CA((void**)&Ls.flags, nls));
-    CK0(CA((void**)&o.line, 8 * nls));
-    CK0(CA((void**)&o.code, 4 * nls));
-    CK0(CA((void**)&o.value, 8 * nls));
-    CK0(CA((void**)&o.flags, nls));
-    CK0(CA((void**)&o.time_us, 8 * nls));
-    CK0(CA((void**)&o.eid_off, 8 * nls));
-    CK0(CA((void**)&o.tid_off, 8 * nls));
-    CK0(CA((void**)&o.fb_line, 8 * nls));
-    CK0(CA((void**)&o.fb_begin, 8 * nls));
-    CK0(CA((void**)&o.fb_end, 8 * nls));
-    CK0(CA((void**)&o.eid_bytes, (size_t)L));
-    CK0(CA((void**)&o.tid_bytes, (size_t)L));
+    CK0(chunk.alloc(&starts, nls + 1));
+    for (uint32_t** p : {&Ls.is_match, &Ls.is_fb, &Ls.eid_len, &Ls.tid_len, &Ls.match_pos, &Ls.fb_pos, &Ls.eid_pos,
+                         &Ls.tid_pos})
+      CK0(chunk.alloc(p, nls));
+    CK0(chunk.alloc(&Ls.code, nls));
+    CK0(chunk.alloc(&Ls.value, nls));
+    CK0(chunk.alloc(&Ls.time_us, nls));
+    CK0(chunk.alloc(&Ls.flags, nls));
+    CK0(chunk.alloc(&o.line, nls));
+    CK0(chunk.alloc(&o.code, nls));
+    CK0(chunk.alloc(&o.value, nls));
+    CK0(chunk.alloc(&o.flags, nls));
+    CK0(chunk.alloc(&o.time_us, nls));
+    CK0(chunk.alloc(&o.eid_off, nls));
+    CK0(chunk.alloc(&o.tid_off, nls));
+    CK0(chunk.alloc(&o.fb_line, nls));
+    CK0(chunk.alloc(&o.fb_begin, nls));
+    CK0(chunk.alloc(&o.fb_end, nls));
+    CK0(chunk.alloc(&o.eid_bytes, (size_t)L));
+    CK0(chunk.alloc(&o.tid_bytes, (size_t)L));
     if (ka) {
       const size_t nlk = nls * (size_t)nk;
-      CK0(CA((void**)&K.present, nls));
-      CK0(CA((void**)&K.number, nls));
-      CK0(CA((void**)&K.num, 8 * nlk));
-      CK0(CA((void**)&K.tok_b, 4 * nlk));
-      CK0(CA((void**)&K.tok_e, 4 * nlk));
-      CK0(CA((void**)&K.tok_len, 4 * nls));
-      CK0(CA((void**)&K.tok_pos, 4 * nls));
-      CK0(CA((void**)&K.o_present, nls));
-      CK0(CA((void**)&K.o_number, nls));
-      CK0(CA((void**)&K.o_num, 8 * nlk));
-      CK0(CA((void**)&K.o_tok_off, 8 * nlk));
-      CK0(CA((void**)&K.o_tok, (size_t)L));   // tokens are disjoint pieces of the chunk's text
+      CK0(chunk.alloc(&K.present, nls));
+      CK0(chunk.alloc(&K.number, nls));
+      CK0(chunk.alloc(&K.num, nlk));
+      CK0(chunk.alloc(&K.tok_b, nlk));
+      CK0(chunk.alloc(&K.tok_e, nlk));
+      CK0(chunk.alloc(&K.tok_len, nls));
+      CK0(chunk.alloc(&K.tok_pos, nls));
+      CK0(chunk.alloc(&K.o_present, nls));
+      CK0(chunk.alloc(&K.o_number, nls));
+      CK0(chunk.alloc(&K.o_num, nlk));
+      CK0(chunk.alloc(&K.o_tok_off, nlk));
+      CK0(chunk.alloc(&K.o_tok, (size_t)L));   // tokens are disjoint pieces of the chunk's text
       K.tok_base = n_tok;
     }
     CK0(cudaEventRecord(k2, ex));
     ev_start_scatter_kernel<<<nblk(L, EV_THREADS), EV_THREADS, 0, ex>>>(d_flag, d_lid, L, nl, starts);
     const unsigned gl = nblk(nl, EV_THREADS);
-    if (use_smem && ka)
-      ev_parse_smem_kernel<true><<<gl, EV_THREADS, EV_SMEM_BYTES, ex>>>(t, starts, nl, df, d_scratch, Ls, K);
-    else if (use_smem)
-      ev_parse_smem_kernel<false><<<gl, EV_THREADS, EV_SMEM_BYTES, ex>>>(t, starts, nl, df, d_scratch, Ls, K);
-    else if (ka)
-      ev_parse_kernel<true><<<gl, EV_THREADS, 0, ex>>>(t, starts, nl, df, d_scratch, Ls, K);
-    else
-      ev_parse_kernel<false><<<gl, EV_THREADS, 0, ex>>>(t, starts, nl, df, d_scratch, Ls, K);
+    kn.parse<<<gl, EV_THREADS, use_smem ? EV_SMEM_BYTES : 0, ex>>>(t, starts, nl, df, d_scratch, Ls, K);
     CK0(cudaGetLastError());
     CK0(scan_exclusive_u32(Ls.is_match, Ls.match_pos, nls, ex, nullptr));
     CK0(scan_exclusive_u32(Ls.is_fb, Ls.fb_pos, nls, ex, nullptr));
     CK0(scan_exclusive_u32(Ls.eid_len, Ls.eid_pos, nls, ex, nullptr));
     CK0(scan_exclusive_u32(Ls.tid_len, Ls.tid_pos, nls, ex, nullptr));
     if (ka) CK0(scan_exclusive_u32(K.tok_len, K.tok_pos, nls, ex, nullptr));
-    EvBase cb_{here.line, here.byte, base.eid, base.tid};
-    if (ka)
-      ev_compact_kernel<true><<<gl, EV_THREADS, 0, ex>>>(t, starts, nl, cb_, d_scratch, Ls, o, K);
-    else
-      ev_compact_kernel<false><<<gl, EV_THREADS, 0, ex>>>(t, starts, nl, cb_, d_scratch, Ls, o, K);
+    kn.compact<<<gl, EV_THREADS, 0, ex>>>(t, starts, nl, here, d_scratch, Ls, o, K);
     ev_totals_kernel<<<1, 1, 0, ex>>>(Ls, nl, d_tot);
     CK0(cudaGetLastError());
     CK0(cudaEventRecord(k3, ex));
@@ -3054,37 +3109,16 @@ static int events_scan_impl(int device, const uint8_t* text, int64_t n_bytes, co
     next_chunk(ce, &nb, &ne);
     if (nb < ne && prefetch(slot ^ 1, nb, ne) != PIO_ALS_OK) return PIO_ALS_ERR_CUDA;
     CK0(cudaStreamSynchronize(ex));
-    const int64_t nm = h_tot[0], nf = h_tot[1], eb = h_tot[2], tb = h_tot[3];
-    if (cols && n_ev + nm > capacity) return fail(nullptr, PIO_ALS_ERR_ARG, "more matched events than capacity");
+    const EvTotals tot{h_tot[0], h_tot[1], h_tot[2], h_tot[3], ka ? (int64_t)h_tot[6] + h_tot[7] : 0};
     CK0(cudaEventRecord(d0, ex));
-    if (sink) {
-      const int rc = eix_take_chunk(sink, o, t, starts, here, base.eid, nm, eb, ex);
-      if (rc != PIO_ALS_OK) return rc;
-    } else {
-      CK0(cudaMemcpyAsync(out_line + n_ev, o.line, 8 * nm, cudaMemcpyDeviceToHost, ex));
-      CK0(cudaMemcpyAsync(out_code + n_ev, o.code, 4 * nm, cudaMemcpyDeviceToHost, ex));
-      CK0(cudaMemcpyAsync(out_value + n_ev, o.value, 8 * nm, cudaMemcpyDeviceToHost, ex));
-      CK0(cudaMemcpyAsync(out_flags + n_ev, o.flags, nm, cudaMemcpyDeviceToHost, ex));
-      CK0(cudaMemcpyAsync(out_time_us + n_ev, o.time_us, 8 * nm, cudaMemcpyDeviceToHost, ex));
-      CK0(cudaMemcpyAsync(out_eid_off + n_ev, o.eid_off, 8 * nm, cudaMemcpyDeviceToHost, ex));
-      CK0(cudaMemcpyAsync(out_tid_off + n_ev, o.tid_off, 8 * nm, cudaMemcpyDeviceToHost, ex));
-      CK0(cudaMemcpyAsync(out_eid_bytes + base.eid, o.eid_bytes, eb, cudaMemcpyDeviceToHost, ex));
-      CK0(cudaMemcpyAsync(out_tid_bytes + base.tid, o.tid_bytes, tb, cudaMemcpyDeviceToHost, ex));
-    }
-    int64_t tk = 0;
-    if (ka) {
-      tk = (int64_t)h_tot[6] + h_tot[7];
-      CK0(cudaMemcpyAsync(ka->out_present + n_ev, K.o_present, nm, cudaMemcpyDeviceToHost, ex));
-      CK0(cudaMemcpyAsync(ka->out_number + n_ev, K.o_number, nm, cudaMemcpyDeviceToHost, ex));
-      CK0(cudaMemcpyAsync(ka->out_num + n_ev * nk, K.o_num, 8 * nm * nk, cudaMemcpyDeviceToHost, ex));
-      CK0(cudaMemcpyAsync(ka->out_tok_off + n_ev * nk, K.o_tok_off, 8 * nm * nk, cudaMemcpyDeviceToHost, ex));
-      CK0(cudaMemcpyAsync(ka->out_tok_bytes + n_tok, K.o_tok, tk, cudaMemcpyDeviceToHost, ex));
-    }
-    const int64_t room = fb_capacity - n_fb, nfc = nf < room ? nf : (room > 0 ? room : 0);
+    const int rc = batch ? eix_take_chunk(batch, o, t, starts, here, here.eid, tot.nm, tot.eb, ex)
+                         : ev_take_host(*cols, ka, o, K, here, tot, ex);
+    if (rc != PIO_ALS_OK) return rc;
+    const int64_t room = fb->capacity - fb->n, nfc = tot.nf < room ? tot.nf : (room > 0 ? room : 0);
     if (nfc > 0) {
-      CK0(cudaMemcpyAsync(out_fb_line + n_fb, o.fb_line, 8 * nfc, cudaMemcpyDeviceToHost, ex));
-      CK0(cudaMemcpyAsync(out_fb_begin + n_fb, o.fb_begin, 8 * nfc, cudaMemcpyDeviceToHost, ex));
-      CK0(cudaMemcpyAsync(out_fb_end + n_fb, o.fb_end, 8 * nfc, cudaMemcpyDeviceToHost, ex));
+      if (fb->line) CK0(cudaMemcpyAsync(fb->line + fb->n, o.fb_line, 8 * nfc, cudaMemcpyDeviceToHost, ex));
+      CK0(cudaMemcpyAsync(fb->begin + fb->n, o.fb_begin, 8 * nfc, cudaMemcpyDeviceToHost, ex));
+      CK0(cudaMemcpyAsync(fb->end + fb->n, o.fb_end, 8 * nfc, cudaMemcpyDeviceToHost, ex));
     }
     CK0(cudaEventRecord(d1, ex));
     CK0(cudaStreamSynchronize(ex));
@@ -3092,18 +3126,36 @@ static int events_scan_impl(int device, const uint8_t* text, int64_t n_bytes, co
     tm.kernel_ms += ms(k0, k1) + ms(k2, k3);
     tm.d2h_ms += ms(d0, d1);
     ++tm.chunks;
-    n_ev += nm;
-    n_fb += nf;
-    base.eid += eb;
-    base.tid += tb;
-    n_tok += tk;
+    fb->n += tot.nf;
+    base.eid += tot.eb;
+    base.tid += tot.tb;
+    n_tok += tot.tk;
     flush_oversized();
     cb = nb, ce = ne;
   }
-  if (cols) out_eid_off[n_ev] = base.eid, out_tid_off[n_ev] = base.tid, *out_n_events = n_ev;
-  if (ka) ka->out_tok_off[n_ev * nk] = n_tok;
-  *out_n_fallback = n_fb;
-  *out_n_lines = base.line;
+  if (n_lines) *n_lines = base.line;
+  return PIO_ALS_OK;
+}
+
+// pio_events_scan (ka == nullptr) and pio_events_scan_keys: the checks they share, then the chunk loop into host columns
+static int ev_scan_host(int device, const uint8_t* text, int64_t n_bytes, const pio_events_filter* f,
+                        const EvKeyArgs* ka, EvHostCols cols, int64_t* out_n_events, EvFallback fb,
+                        int64_t* out_n_fallback, int64_t* out_n_lines) {
+  if (n_bytes < 0 || (n_bytes > 0 && !text) || !f || fb.capacity < 0 || cols.capacity < n_bytes /
+      PIO_EVENTS_MIN_EVENT_BYTES + 1 || !cols.line || !cols.code || !cols.value || !cols.flags || !cols.time_us ||
+      !cols.eid_bytes || !cols.eid_off || !cols.tid_bytes || !cols.tid_off || !out_n_events || (fb.capacity > 0 &&
+      (!fb.line || !fb.begin || !fb.end)) || !out_n_fallback || !out_n_lines)
+    return fail(nullptr, PIO_ALS_ERR_ARG, "bad pio_events_scan arguments");
+  int rc = ev_check_filter(f);
+  if (rc != PIO_ALS_OK) return rc;
+  *out_n_fallback = *out_n_lines = *out_n_events = 0;
+  cols.eid_off[0] = cols.tid_off[0] = 0;
+  if (ka) ka->out_tok_off[0] = 0;
+  if (n_bytes == 0) return PIO_ALS_OK;
+  rc = ev_scan(device, text, n_bytes, f, ka, &cols, nullptr, &fb, out_n_lines);
+  if (rc != PIO_ALS_OK) return rc;
+  *out_n_events = cols.n;
+  *out_n_fallback = fb.n;
   return PIO_ALS_OK;
 }
 
@@ -3112,9 +3164,10 @@ int pio_events_scan(int device, const uint8_t* text, int64_t n_bytes, const pio_
                     uint8_t* out_eid_bytes, int64_t* out_eid_off, uint8_t* out_tid_bytes, int64_t* out_tid_off,
                     int64_t* out_n_events, int64_t fb_capacity, int64_t* out_fb_line, int64_t* out_fb_begin,
                     int64_t* out_fb_end, int64_t* out_n_fallback, int64_t* out_n_lines) {
-  return events_scan_impl(device, text, n_bytes, f, capacity, out_line, out_code, out_value, out_flags, out_time_us,
-                          out_eid_bytes, out_eid_off, out_tid_bytes, out_tid_off, out_n_events, fb_capacity, out_fb_line,
-                          out_fb_begin, out_fb_end, out_n_fallback, out_n_lines, nullptr);
+  const EvHostCols cols{capacity,      out_line,    out_code,      out_value,   out_flags, out_time_us,
+                        out_eid_bytes, out_eid_off, out_tid_bytes, out_tid_off, 0};
+  return ev_scan_host(device, text, n_bytes, f, nullptr, cols, out_n_events,
+                      EvFallback{fb_capacity, out_fb_line, out_fb_begin, out_fb_end, 0}, out_n_fallback, out_n_lines);
 }
 
 int pio_events_scan_keys(int device, const uint8_t* text, int64_t n_bytes, const pio_events_filter* f,
@@ -3135,9 +3188,10 @@ int pio_events_scan_keys(int device, const uint8_t* text, int64_t n_bytes, const
       if (!strcmp(keys[p], keys[q])) return fail(nullptr, PIO_ALS_ERR_ARG, "key %d repeats key %d", q, p);
   }
   const EvKeyArgs ka{keys, n_keys, out_present, out_number, out_num, out_tok_bytes, out_tok_off};
-  return events_scan_impl(device, text, n_bytes, f, capacity, out_line, out_code, out_value, out_flags, out_time_us,
-                          out_eid_bytes, out_eid_off, out_tid_bytes, out_tid_off, out_n_events, fb_capacity, out_fb_line,
-                          out_fb_begin, out_fb_end, out_n_fallback, out_n_lines, &ka);
+  const EvHostCols cols{capacity,      out_line,    out_code,      out_value,   out_flags, out_time_us,
+                        out_eid_bytes, out_eid_off, out_tid_bytes, out_tid_off, 0};
+  return ev_scan_host(device, text, n_bytes, f, &ka, cols, out_n_events,
+                      EvFallback{fb_capacity, out_fb_line, out_fb_begin, out_fb_end, 0}, out_n_fallback, out_n_lines);
 }
 
 // ---- $set / $unset / $delete fold (PEventStore.aggregatePropertyColumns; events_fold.cuh) -----------------------------
@@ -3159,29 +3213,23 @@ int pio_events_fold(int device, const uint8_t* eid_bytes, const int64_t* eid_off
                   code[e]);
   CK0(cudaSetDevice(device));
   const size_t nb = (size_t)eid_off[n], nn = (size_t)n, nk = (size_t)n_keys;
-  std::vector<void*> owned;
-  auto A = [&](void** p, size_t bytes_) -> cudaError_t {
-    cudaError_t e = cudaMalloc(p, bytes_ ? bytes_ : 1);
-    if (e == cudaSuccess) owned.push_back(*p);
-    return e;
-  };
-  struct Guard { std::vector<void*>& v; ~Guard() { for (void* q : v) cudaFree(q); } } guard{owned};
+  cudaStream_t st = 0;
+  CallMem tmp(st);
   uint8_t *d_bytes = nullptr, *d_present = nullptr, *d_exists = nullptr;
   long long *d_off = nullptr, *d_time = nullptr, *d_first = nullptr, *d_fus = nullptr, *d_lus = nullptr, *d_win = nullptr;
   int32_t* d_code = nullptr;
   int *d_ent = nullptr, *seg_first = nullptr, *seg_last = nullptr, *last_set = nullptr, *last_del = nullptr, *win = nullptr;
   uint64_t *ka = nullptr, *kb = nullptr;
   uint32_t *va = nullptr, *vb = nullptr;
-  CK0(A((void**)&d_bytes, nb));
-  CK0(A((void**)&d_off, 8 * (nn + 1)));
-  CK0(A((void**)&d_code, 4 * nn));
-  CK0(A((void**)&d_time, 8 * nn));
-  CK0(A((void**)&d_present, nn));
-  CK0(A((void**)&d_ent, 4 * nn));
-  CK0(A((void**)&d_first, 8 * nn));
-  CK0(A((void**)&ka, 8 * nn)); CK0(A((void**)&kb, 8 * nn));
-  CK0(A((void**)&va, 4 * nn)); CK0(A((void**)&vb, 4 * nn));
-  cudaStream_t st = 0;
+  CK0(tmp.device(&d_bytes, nb));
+  CK0(tmp.device(&d_off, nn + 1));
+  CK0(tmp.device(&d_code, nn));
+  CK0(tmp.device(&d_time, nn));
+  CK0(tmp.device(&d_present, nn));
+  CK0(tmp.device(&d_ent, nn));
+  CK0(tmp.device(&d_first, nn));
+  CK0(tmp.device(&ka, nn)); CK0(tmp.device(&kb, nn));
+  CK0(tmp.device(&va, nn)); CK0(tmp.device(&vb, nn));
   CK0(cudaMemcpyAsync(d_bytes, eid_bytes, nb, cudaMemcpyHostToDevice, st));
   CK0(cudaMemcpyAsync(d_off, eid_off, 8 * (nn + 1), cudaMemcpyHostToDevice, st));
   CK0(cudaMemcpyAsync(d_code, code, 4 * nn, cudaMemcpyHostToDevice, st));
@@ -3191,12 +3239,12 @@ int pio_events_fold(int device, const uint8_t* eid_bytes, const int64_t* eid_off
   const int rc = ids_encode_device(d_bytes, d_off, n, st, d_ent, d_first, &n_ent);
   if (rc != PIO_ALS_OK) return rc;
   const size_t ne = (size_t)n_ent;
-  CK0(A((void**)&seg_first, 4 * ne)); CK0(A((void**)&seg_last, 4 * ne));
-  CK0(A((void**)&last_set, 4 * ne)); CK0(A((void**)&last_del, 4 * ne));
-  CK0(A((void**)&win, 4 * ne * nk));
-  CK0(A((void**)&d_exists, ne));
-  CK0(A((void**)&d_fus, 8 * ne)); CK0(A((void**)&d_lus, 8 * ne));
-  CK0(A((void**)&d_win, 8 * ne * nk));
+  CK0(tmp.device(&seg_first, ne)); CK0(tmp.device(&seg_last, ne));
+  CK0(tmp.device(&last_set, ne)); CK0(tmp.device(&last_del, ne));
+  CK0(tmp.device(&win, ne * nk));
+  CK0(tmp.device(&d_exists, ne));
+  CK0(tmp.device(&d_fus, ne)); CK0(tmp.device(&d_lus, ne));
+  CK0(tmp.device(&d_win, ne * nk));
   CK0(cudaMemsetAsync(last_set, 0xFF, 4 * ne, st));   // -1: none
   CK0(cudaMemsetAsync(last_del, 0xFF, 4 * ne, st));
   if (nk) CK0(cudaMemsetAsync(win, 0xFF, 4 * ne * nk, st));
@@ -3259,17 +3307,11 @@ static double ms_since(Clock::time_point t0) {
 static int eix_sort(pio_events_index* ix, EixBatch& b, EixRun* out) {
   const long long n = b.r.n;
   const cudaStream_t st = ix->st;
-  std::vector<void*> owned;
-  struct Guard { std::vector<void*>& v; ~Guard() { for (void* q : v) cudaFree(q); } } guard{owned};
-  auto A = [&](void** p, size_t bytes_) -> cudaError_t {
-    cudaError_t e = cudaMalloc(p, bytes_ ? bytes_ : 1);
-    if (e == cudaSuccess) owned.push_back(*p);
-    return e;
-  };
+  CallMem tmp(st);
   uint64_t *ka = nullptr, *kb = nullptr;
   uint32_t *va = nullptr, *vb = nullptr;
-  CK0(A((void**)&ka, 8 * (size_t)n)); CK0(A((void**)&kb, 8 * (size_t)n));
-  CK0(A((void**)&va, 4 * (size_t)n)); CK0(A((void**)&vb, 4 * (size_t)n));
+  CK0(tmp.device(&ka, (size_t)n)); CK0(tmp.device(&kb, (size_t)n));
+  CK0(tmp.device(&va, (size_t)n)); CK0(tmp.device(&vb, (size_t)n));
   eix_time_key_kernel<<<nblk(n, 256), 256, 0, st>>>(b.r.time_us, n, ka, va);
   bool in_b = false;
   CK0(radix_sort_pairs(ka, va, kb, vb, (size_t)n, 64, st, &in_b, nullptr));
@@ -3289,9 +3331,10 @@ static int eix_sort(pio_events_index* ix, EixBatch& b, EixRun* out) {
   eix_gather_kernel<<<nblk(n, 256), 256, 0, st>>>(b.r, in_b ? v2 : v1, r);
   r.arena = b.r.arena, r.arena_bytes = b.r.arena_bytes;
   b.r.arena = nullptr;
-  const cudaError_t e2 = cudaStreamSynchronize(st);
+  cudaError_t e2 = cudaStreamSynchronize(st);
+  if (e2 == cudaSuccess) e2 = cudaGetLastError();
   eix_free(b.r);
-  if (e2 != cudaSuccess || (e2 == cudaSuccess && cudaGetLastError() != cudaSuccess)) {
+  if (e2 != cudaSuccess) {
     eix_free(r);
     return fail(nullptr, PIO_ALS_ERR_CUDA, "event index sort: %s", cudaGetErrorString(e2));
   }
@@ -3370,13 +3413,8 @@ int pio_events_index_create(int device, const pio_events_filter* view, pio_event
   *out = nullptr;
   if (view->property || view->has_start || view->has_until)
     return fail(nullptr, PIO_ALS_ERR_ARG, "an event index view has no property and no time bounds");
-  if (view->n_event_names < 0 || (view->n_event_names > 0 && !view->event_names))
-    return fail(nullptr, PIO_ALS_ERR_ARG, "bad event name list");
-  for (int k = 0; k < view->n_event_names; ++k)
-    if (!view->event_names[k]) return fail(nullptr, PIO_ALS_ERR_ARG, "event name %d is NULL", k);
-  if (view->target_entity_type_mode < PIO_EVENTS_TARGET_ANY || view->target_entity_type_mode > PIO_EVENTS_TARGET_EQUALS ||
-      (view->target_entity_type_mode == PIO_EVENTS_TARGET_EQUALS && !view->target_entity_type))
-    return fail(nullptr, PIO_ALS_ERR_ARG, "bad target_entity_type_mode / target_entity_type");
+  const int rc = ev_check_filter(view);
+  if (rc != PIO_ALS_OK) return rc;
   CK0(cudaSetDevice(device));
   auto* ix = new pio_events_index;
   ix->device = device;
@@ -3408,20 +3446,16 @@ int pio_events_index_append(pio_events_index* ix, const uint8_t* text, int64_t n
   *out_n_fallback = 0;
   ix->stats.scan_ms = ix->stats.sort_ms = ix->stats.merge_ms = 0;
   if (n_bytes == 0) return PIO_ALS_OK;
-  CK0(cudaSetDevice(ix->device));
   EixBatch b;
   b.file_base = base_offset;
   b.mask = ix->mask;
-  struct Guard { EixRun& r; ~Guard() { eix_free(r); } } guard{b.r};
-  std::vector<int64_t> fb_line((size_t)(fb_capacity > 0 ? fb_capacity : 1));
-  int64_t n_lines = 0;
+  EvFallback fb{fb_capacity, nullptr, out_fb_begin, out_fb_end, 0};
   const auto t0 = Clock::now();
-  const int rc = events_scan_impl(ix->device, text, n_bytes, &ix->view, 0, nullptr, nullptr, nullptr, nullptr, nullptr,
-                                  nullptr, nullptr, nullptr, nullptr, nullptr, fb_capacity, fb_line.data(), out_fb_begin,
-                                  out_fb_end, out_n_fallback, &n_lines, nullptr, &b);
+  const int rc = ev_scan(ix->device, text, n_bytes, &ix->view, nullptr, nullptr, &b, &fb, nullptr);
   ix->stats.scan_ms = ms_since(t0);
   if (rc != PIO_ALS_OK) return rc;
-  if (*out_n_fallback > fb_capacity) return PIO_ALS_OK;   // nothing added; the caller asks again with more room
+  *out_n_fallback = fb.n;
+  if (fb.n > fb_capacity) return PIO_ALS_OK;   // nothing added; the caller asks again with more room
   return eix_add_batch(ix, b);
 }
 
@@ -3439,20 +3473,17 @@ int pio_events_index_add_host(pio_events_index* ix, const uint8_t* id_bytes, con
   if (n == 0) return PIO_ALS_OK;
   CK0(cudaSetDevice(ix->device));
   EixBatch b;
-  struct Guard { EixRun& r; ~Guard() { eix_free(r); } } guard{b.r};
   const cudaError_t e = eix_alloc(b.r, n, id_off[n]);
   if (e != cudaSuccess) return fail(nullptr, PIO_ALS_ERR_CUDA, "event index: %s", cudaGetErrorString(e));
   b.r.n = n;
   b.r.arena_bytes = id_off[n];
   std::vector<int32_t> id_len((size_t)n);
   for (int64_t k = 0; k < n; ++k) id_len[k] = (int32_t)(id_off[k + 1] - id_off[k]);
-  const size_t m = (size_t)n;
   CK0(cudaMemcpyAsync(b.r.arena, id_bytes, (size_t)id_off[n], cudaMemcpyHostToDevice, ix->st));
-  CK0(cudaMemcpyAsync(b.r.id_off, id_off, 8 * m, cudaMemcpyHostToDevice, ix->st));
-  CK0(cudaMemcpyAsync(b.r.id_len, id_len.data(), 4 * m, cudaMemcpyHostToDevice, ix->st));
-  CK0(cudaMemcpyAsync(b.r.time_us, time_us, 8 * m, cudaMemcpyHostToDevice, ix->st));
-  CK0(cudaMemcpyAsync(b.r.off, offset, 8 * m, cudaMemcpyHostToDevice, ix->st));
-  CK0(cudaMemcpyAsync(b.r.len, length, 4 * m, cudaMemcpyHostToDevice, ix->st));
+  const void* from[6] = {nullptr, time_us, offset, length, id_off, id_len.data()};   // in eix_cols order; hashed below
+  const auto to = eix_cols(b.r);
+  for (size_t k = 1; k < to.size(); ++k)
+    CK0(cudaMemcpyAsync(*to[k].p, from[k], to[k].size * (size_t)n, cudaMemcpyHostToDevice, ix->st));
   eix_hash_kernel<<<nblk(n, 256), 256, 0, ix->st>>>(b.r, ix->mask);
   CK0(cudaGetLastError());
   return eix_add_batch(ix, b);
@@ -3541,21 +3572,15 @@ int pio_cooc_train(int device, const int32_t* user, const int32_t* item, int64_t
   const int bits_u = ceil_log2((uint64_t)n_users), bits_i = ceil_log2((uint64_t)n_items);
   if (2 * bits_i > 40) return fail(nullptr, PIO_ALS_ERR_ARG, "n_items too large for the pair keys (max 2^20 items)");
   const int bits_c = 64 - 2 * bits_i > 32 ? 32 : 64 - 2 * bits_i;
-  std::vector<void*> owned;
-  auto A = [&](void** p, size_t bytes_) -> cudaError_t {
-    cudaError_t e = cudaMalloc(p, bytes_ ? bytes_ : 1);
-    if (e == cudaSuccess) owned.push_back(*p);
-    return e;
-  };
-  struct Guard { std::vector<void*>& v; ~Guard() { for (void* q : v) cudaFree(q); } } guard{owned};
   cudaStream_t st = 0;
+  CallMem tmp(st);
   int *du = nullptr, *di = nullptr;
   uint64_t *ka = nullptr, *kb = nullptr, *dk = nullptr;
   uint32_t *va = nullptr, *vb = nullptr, *flag = nullptr, *rank = nullptr;
-  CK0(A((void**)&du, 4 * (size_t)n)); CK0(A((void**)&di, 4 * (size_t)n));
-  CK0(A((void**)&ka, 8 * (size_t)n)); CK0(A((void**)&kb, 8 * (size_t)n));
-  CK0(A((void**)&va, 4 * (size_t)n)); CK0(A((void**)&vb, 4 * (size_t)n));
-  CK0(A((void**)&flag, 4 * (size_t)n)); CK0(A((void**)&dk, 8 * (size_t)n)); CK0(A((void**)&rank, 4 * (size_t)n));
+  CK0(tmp.device(&du, (size_t)n)); CK0(tmp.device(&di, (size_t)n));
+  CK0(tmp.device(&ka, (size_t)n)); CK0(tmp.device(&kb, (size_t)n));
+  CK0(tmp.device(&va, (size_t)n)); CK0(tmp.device(&vb, (size_t)n));
+  CK0(tmp.device(&flag, (size_t)n)); CK0(tmp.device(&dk, (size_t)n)); CK0(tmp.device(&rank, (size_t)n));
   CK0(cudaMemcpyAsync(du, user, 4 * (size_t)n, cudaMemcpyHostToDevice, st));
   CK0(cudaMemcpyAsync(di, item, 4 * (size_t)n, cudaMemcpyHostToDevice, st));
   // 1. distinct (user, item), sorted by user then item
@@ -3586,9 +3611,9 @@ int pio_cooc_train(int device, const int32_t* user, const int32_t* item, int64_t
   if (np > 0) {
     uint64_t *pk = nullptr, *pk2 = nullptr, *rk = nullptr, *rk2 = nullptr;
     uint32_t *pp = nullptr, *pp2 = nullptr, *pf = nullptr, *ppos = nullptr, *rp = nullptr, *rp2 = nullptr;
-    CK0(A((void**)&pk, 8 * (size_t)np)); CK0(A((void**)&pk2, 8 * (size_t)np));
-    CK0(A((void**)&pp, 4 * (size_t)np)); CK0(A((void**)&pp2, 4 * (size_t)np));
-    CK0(A((void**)&pf, 4 * (size_t)np)); CK0(A((void**)&ppos, 4 * (size_t)np));
+    CK0(tmp.device(&pk, (size_t)np)); CK0(tmp.device(&pk2, (size_t)np));
+    CK0(tmp.device(&pp, (size_t)np)); CK0(tmp.device(&pp2, (size_t)np));
+    CK0(tmp.device(&pf, (size_t)np)); CK0(tmp.device(&ppos, (size_t)np));
     cooc_pairs_kernel<<<nblk(m, 256), 256, 0, st>>>(dk, rank, off, m, bits_i, pk, pp);
     bool pb_ = false;
     CK0(radix_sort_pairs(pk, pp, pk2, pp2, (size_t)np, 2 * bits_i, st, &pb_, nullptr));
@@ -3601,14 +3626,14 @@ int pio_cooc_train(int device, const int32_t* user, const int32_t* item, int64_t
     CK0(cudaStreamSynchronize(st));
     const long long C = (long long)cp + cf, n2 = 2 * C;
     // 3. both directions, ranked per item by (count desc, other item asc)
-    CK0(A((void**)&rk, 8 * (size_t)n2)); CK0(A((void**)&rk2, 8 * (size_t)n2));
-    CK0(A((void**)&rp, 4 * (size_t)n2)); CK0(A((void**)&rp2, 4 * (size_t)n2));
+    CK0(tmp.device(&rk, (size_t)n2)); CK0(tmp.device(&rk2, (size_t)n2));
+    CK0(tmp.device(&rp, (size_t)n2)); CK0(tmp.device(&rp2, (size_t)n2));
     cooc_runs_kernel<<<nblk(np, 256), 256, 0, st>>>(pks, pf, ppos, np, bits_i, bits_c, rk, rp);
     bool rb = false;
     CK0(radix_sort_pairs(rk, rp, rk2, rp2, (size_t)n2, 2 * bits_i + bits_c, st, &rb, nullptr));
     int *d_oi = nullptr, *d_oc = nullptr, *d_on = nullptr;
-    CK0(A((void**)&d_oi, 4 * (size_t)n_items * topn)); CK0(A((void**)&d_oc, 4 * (size_t)n_items * topn));
-    CK0(A((void**)&d_on, 4 * (size_t)n_items));
+    CK0(tmp.device(&d_oi, (size_t)n_items * topn)); CK0(tmp.device(&d_oc, (size_t)n_items * topn));
+    CK0(tmp.device(&d_on, (size_t)n_items));
     CK0(cudaMemsetAsync(d_oi, 0xff, 4 * (size_t)n_items * topn, st));
     CK0(cudaMemsetAsync(d_oc, 0, 4 * (size_t)n_items * topn, st));
     CK0(cudaMemsetAsync(d_on, 0, 4 * (size_t)n_items, st));
@@ -3634,23 +3659,24 @@ int pio_nb_train(int device, const int32_t* label, const float* x, int64_t n, in
   CK0(cudaSetDevice(device));
   for (int64_t r = 0; r < n; ++r)
     if (label[r] < 0 || label[r] >= n_class) return fail(nullptr, PIO_ALS_ERR_ARG, "label out of range at row %lld", (long long)r);
+  CallMem tmp(0);
   int* dl = nullptr;
   float* dx = nullptr;
   double *dp = nullptr, *dout = nullptr;
   const int nb = 296;
-  CK0(cudaMalloc((void**)&dl, sizeof(int) * n));
-  CK0(cudaMalloc((void**)&dx, sizeof(float) * n * n_feat));
-  CK0(cudaMalloc((void**)&dp, sizeof(double) * (size_t)nb * width));
-  CK0(cudaMalloc((void**)&dout, sizeof(double) * width));
+  CK0(tmp.device(&dl, (size_t)n));
+  CK0(tmp.device(&dx, (size_t)n * n_feat));
+  CK0(tmp.device(&dp, (size_t)nb * width));
+  CK0(tmp.device(&dout, (size_t)width));
   CK0(cudaMemcpy(dl, label, sizeof(int) * n, cudaMemcpyHostToDevice));
   CK0(cudaMemcpy(dx, x, sizeof(float) * n * n_feat, cudaMemcpyHostToDevice));
   const size_t smem = sizeof(double) * 8 * width;
   CK0(cudaFuncSetAttribute(nb_partial_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   nb_partial_kernel<<<nb, 256, smem>>>(dl, dx, n, n_feat, n_class, dp);
   nb_reduce_kernel<<<nblk(width, 128), 128>>>(dp, nb, width, dout);
+  CK0(cudaGetLastError());
   std::vector<double> acc(width);
   CK0(cudaMemcpy(acc.data(), dout, sizeof(double) * width, cudaMemcpyDeviceToHost));
-  cudaFree(dl); cudaFree(dx); cudaFree(dp); cudaFree(dout);
   // MLlib multinomial: pi_c = log(n_c + l) - log(N + C l); theta_cj = log(s_cj + l) - log(sum_j s_cj + F l)
   const double logden = log((double)n + n_class * lambda);
   for (int c = 0; c < n_class; ++c) {
@@ -3667,19 +3693,20 @@ int pio_nb_predict(int device, const float* x, int64_t n, int n_feat, int n_clas
                    int32_t* out_label) {
   if (!x || !pi || !theta || !out_label || n <= 0) return fail(nullptr, PIO_ALS_ERR_ARG, "bad NaiveBayes arguments");
   CK0(cudaSetDevice(device));
+  CallMem tmp(0);
   float* dx = nullptr;
   double *dpi = nullptr, *dth = nullptr;
   int* dout = nullptr;
-  CK0(cudaMalloc((void**)&dx, sizeof(float) * n * n_feat));
-  CK0(cudaMalloc((void**)&dpi, sizeof(double) * n_class));
-  CK0(cudaMalloc((void**)&dth, sizeof(double) * n_class * n_feat));
-  CK0(cudaMalloc((void**)&dout, sizeof(int) * n));
+  CK0(tmp.device(&dx, (size_t)n * n_feat));
+  CK0(tmp.device(&dpi, (size_t)n_class));
+  CK0(tmp.device(&dth, (size_t)n_class * n_feat));
+  CK0(tmp.device(&dout, (size_t)n));
   CK0(cudaMemcpy(dx, x, sizeof(float) * n * n_feat, cudaMemcpyHostToDevice));
   CK0(cudaMemcpy(dpi, pi, sizeof(double) * n_class, cudaMemcpyHostToDevice));
   CK0(cudaMemcpy(dth, theta, sizeof(double) * n_class * n_feat, cudaMemcpyHostToDevice));
   nb_predict_kernel<<<nblk(n, 256), 256>>>(dx, n, n_feat, n_class, dpi, dth, dout);
+  CK0(cudaGetLastError());
   CK0(cudaMemcpy(out_label, dout, sizeof(int) * n, cudaMemcpyDeviceToHost));
-  cudaFree(dx); cudaFree(dpi); cudaFree(dth); cudaFree(dout);
   return PIO_ALS_OK;
 }
 
