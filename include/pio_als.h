@@ -319,6 +319,54 @@ PIO_API int pio_events_fold(int device, const uint8_t* eid_bytes, const int64_t*
                             int64_t* out_first_event, uint8_t* out_exists, int64_t* out_first_us, int64_t* out_last_us,
                             int64_t* out_winner, int64_t* out_n_entities);
 
+/* Whole-map event scan: pio_events_scan (same filter, chunking, pinned staging, fallback protocol and capacity bound)
+ * that also reads every top-level key of each matched event's `properties`, in object order (DESIGN.md 3.4); what
+ * PEventStore.aggregatePropertyMaps folds.  Per matched event e, next to everything pio_events_scan writes:
+ *   out_utc_offset[e]   eventTime's UTC offset in minutes (0 for "Z" or no offset)
+ *   out_prop_off[e]     its records are out_prop_off[e] .. out_prop_off[e + 1) (capacity + 1 entries); none for absent,
+ *                       null or {} properties
+ * Per record r, one per key in object order (a key twice in one object gives two records):
+ *   the key, unescaped to UTF-8: out_key_bytes[out_key_off[r] .. out_key_off[r + 1])
+ *   the value's raw JSON token: out_tok_bytes[out_tok_off[r] .. out_tok_off[r + 1]) (numbers too: the caller decodes)
+ * rec_capacity >= n_bytes / PIO_EVENTS_MIN_RECORD_BYTES + 1 (a record takes at least `"":0` of line text);
+ * out_key_off / out_tok_off: rec_capacity + 1 entries; out_key_bytes / out_tok_bytes: n_bytes each.
+ * *out_n_records = number of records.  PIO_ALS_ERR_ARG for a bad filter or sizes, or filter->property != NULL. */
+#define PIO_EVENTS_MIN_RECORD_BYTES 4
+PIO_API int pio_events_scan_props(int device, const uint8_t* text, int64_t n_bytes, const pio_events_filter* filter,
+                                  int64_t capacity, int64_t* out_line, int32_t* out_code, double* out_value,
+                                  uint8_t* out_flags, int64_t* out_time_us, uint8_t* out_eid_bytes, int64_t* out_eid_off,
+                                  uint8_t* out_tid_bytes, int64_t* out_tid_off, int16_t* out_utc_offset,
+                                  int64_t* out_prop_off, int64_t rec_capacity, uint8_t* out_key_bytes,
+                                  int64_t* out_key_off, uint8_t* out_tok_bytes, int64_t* out_tok_off,
+                                  int64_t* out_n_events, int64_t* out_n_records, int64_t fb_capacity,
+                                  int64_t* out_fb_line, int64_t* out_fb_begin, int64_t* out_fb_end,
+                                  int64_t* out_n_fallback, int64_t* out_n_lines);
+
+/* LEventAggregator's $set / $unset / $delete fold of every key (DESIGN.md 3.4), over n events in file order (HOST
+ * buffers): entity ids as bytes + n + 1 offsets (eid_off[0] == 0), code[e] 0 = $set / 1 = $unset / 2 = $delete,
+ * time_us[e], and the records of event e, prop_off[e] .. prop_off[e + 1) (prop_off[0] == 0), one per key of its
+ * properties in object order, whose keys are key_bytes[key_off[r] .. key_off[r + 1]).  Events of one entity are taken in
+ * (time, file order); records of a $delete are ignored.
+ * Per distinct entity g, in order of first occurrence among the events (capacity n, out_win_off n + 1):
+ *   out_first_event        index of its first event (its id)
+ *   out_exists             1 when its last $set comes after its last $delete (the PropertyMap exists)
+ *   out_first_time_event   the event that gives firstUpdated: the first in (time, file order)
+ *   out_last_time_event    the event that gives lastUpdated: the first in file order among those at the latest time
+ *   out_win_rec[out_win_off[g] .. out_win_off[g + 1])   the record holding the value of each key of the PropertyMap, in
+ *                          the map's order; out_win_key[w] its key code (capacity prop_off[n] each)
+ * A key k is present when the last $set record with k comes after remover(k) = max(the last $delete, the last $unset
+ * with k); that record holds its value, and its place in the map is that of the first $set record with k after
+ * remover(k): (event, index in the object).  Key codes number distinct keys in order of first occurrence among the
+ * records; out_key_first[c] is the first record of code c (capacity prop_off[n]).  *out_n_entities, *out_n_keys: the
+ * numbers of entities and key codes.  Deterministic.  PIO_ALS_ERR_ARG for a code outside 0..2, decreasing prop_off,
+ * n or prop_off[n] >= 2^31, or missing buffers. */
+PIO_API int pio_events_fold_props(int device, const uint8_t* eid_bytes, const int64_t* eid_off, const int32_t* code,
+                                  const int64_t* time_us, const int64_t* prop_off, int64_t n, const uint8_t* key_bytes,
+                                  const int64_t* key_off, int64_t* out_first_event, uint8_t* out_exists,
+                                  int64_t* out_first_time_event, int64_t* out_last_time_event, int64_t* out_win_off,
+                                  int64_t* out_win_rec, int32_t* out_win_key, int64_t* out_key_first,
+                                  int64_t* out_n_entities, int64_t* out_n_keys);
+
 /* Event index: LEventStore.findByEntity (data/src/main/scala/org/apache/predictionio/data/store/LEventStore.scala:76)
  * for one view -- a `find` filter (entity type, event names, target entity type) -- of an append-only event file, kept
  * on the device (DESIGN.md 3.3).  Per matched event it holds the hash of the decoded entityId, eventTime, the byte

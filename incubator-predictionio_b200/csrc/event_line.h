@@ -299,8 +299,10 @@ PIO_EV_HD int two(const uint8_t* t, int i) {
   return is_digit(t[i]) && is_digit(t[i + 1]) ? (t[i] - '0') * 10 + (t[i + 1] - '0') : -1;
 }
 
-// YYYY-MM-DDTHH:MM:SS[.f{1,6}][Z|+HH:MM|-HH:MM] -> microseconds since the epoch (UTC when there is no offset)
-PIO_EV_HD bool parse_time(const uint8_t* t, int n, int64_t* us) {
+// YYYY-MM-DDTHH:MM:SS[.f{1,6}][Z|+HH:MM|-HH:MM] -> microseconds since the epoch (UTC when there is no offset), and with
+// OFF the UTC offset in minutes
+template <bool OFF>
+PIO_EV_HD bool parse_time_t(const uint8_t* t, int n, int64_t* us, int* off) {
   if (n < 19 || t[4] != '-' || t[7] != '-' || t[10] != 'T' || t[13] != ':' || t[16] != ':') return false;
   const int y0 = two(t, 0), y1 = two(t, 2), mo = two(t, 5), d = two(t, 8), h = two(t, 11), mi = two(t, 14), sec = two(t, 17);
   if (y0 < 0 || y1 < 0 || mo < 0 || d < 0 || h < 0 || mi < 0 || sec < 0) return false;
@@ -338,8 +340,11 @@ PIO_EV_HD bool parse_time(const uint8_t* t, int n, int64_t* us) {
   if (p != n) return false;
   const int64_t secs = days_from_civil(y, mo, d) * 86400 + h * 3600 + mi * 60 + sec - (int64_t)off_min * 60;
   *us = secs * 1000000 + frac;
+  if constexpr (OFF) *off = off_min;
   return true;
 }
+
+PIO_EV_HD bool parse_time(const uint8_t* t, int n, int64_t* us) { return parse_time_t<false>(t, n, us, nullptr); }
 
 PIO_EV_HD bool key_is(const uint8_t* s, const Span& k, const char* name, int len, uint8_t* tmp) {
   return str_eq(s, k, (const uint8_t*)name, len, tmp);
@@ -383,12 +388,22 @@ struct KeyValues {
                           // token as well, so the host can tell 5 from 5.0
 };
 
+// Whole-map parse (parse_line_props): every top-level key of `properties`, for a MATCHED line (all zero otherwise).
+// The keys themselves are read by a second walk over the validated object (next_prop).
+struct PropsInfo {
+  int n_keys;             // top-level keys of `properties`: 0 for absent, null or {}
+  int b, e;               // the `properties` object at [b, e) of the line (empty when it has no keys)
+  int utc_off;            // eventTime's UTC offset in minutes (0 for Z or none)
+};
+
 // One line, terminator removed.  scratch: at least n bytes (decoded ids land at its start).  KEYS == false is
 // parse_line; KEYS == true also fills *kv for the keys of *kl (Filter::prop_len must be < 0 then).  A tracked key twice
 // in one `properties` object makes the line FALLBACK; a number off the fast path does not (the host decodes its token).
-template <bool KEYS>
+// ALL == true (KEYS false) fills *pi instead; it takes every key, so no key makes a line FALLBACK, duplicates included.
+template <bool KEYS, bool ALL = false>
 PIO_EV_HD Result parse_line_t(const uint8_t* s, int n, const Filter& f, uint8_t* scratch, const KeyList* kl,
-                              KeyValues* kv) {
+                              KeyValues* kv, PropsInfo* pi = nullptr) {
+  static_assert(!(KEYS && ALL), "one mode at a time");
   Result r;
   r.outcome = FALLBACK;
   r.code = -1;
@@ -415,6 +430,8 @@ PIO_EV_HD Result parse_line_t(const uint8_t* s, int n, const Filter& f, uint8_t*
   (void)ksp;
   int kopen = -1;   // a tracked key whose value is a container (at depth 3) still open: its token ends where it closes
   (void)kopen;
+  int pkeys = 0, pend = 0;   // ALL: keys of `properties` so far, and where it closes
+  (void)pkeys, (void)pend;
   enum { ST_VALUE, ST_VALUE_OR_END, ST_AFTER, ST_KEY_OR_END, ST_KEY, ST_COLON };
   int st = ST_VALUE, depth = 0, pending = -1;
   uint64_t arr = 0;   // bit d - 1: the container at depth d is an array
@@ -488,6 +505,9 @@ PIO_EV_HD Result parse_line_t(const uint8_t* s, int n, const Filter& f, uint8_t*
         if constexpr (KEYS) {
           if (depth == 3 && kopen >= 0) ksp[kopen].e = i + 1, kopen = -1;
         }
+        if constexpr (ALL) {
+          if (depth == 2 && in_props) pend = i + 1;
+        }
         if (--depth < 2) in_props = false;
         st = ST_AFTER;
       } else {
@@ -499,6 +519,9 @@ PIO_EV_HD Result parse_line_t(const uint8_t* s, int n, const Filter& f, uint8_t*
     if (st == ST_KEY_OR_END && c == '}') {
       if constexpr (KEYS) {
         if (depth == 3 && kopen >= 0) ksp[kopen].e = i + 1, kopen = -1;
+      }
+      if constexpr (ALL) {
+        if (depth == 2 && in_props) pend = i + 1;
       }
       if (--depth < 2) in_props = false;
       ++i;
@@ -531,6 +554,9 @@ PIO_EV_HD Result parse_line_t(const uint8_t* s, int n, const Filter& f, uint8_t*
           }
         }
       }
+      if constexpr (ALL) {
+        if (depth == 2 && in_props) ++pkeys;
+      }
       pending = slot;
       st = ST_COLON;
       continue;
@@ -553,9 +579,15 @@ PIO_EV_HD Result parse_line_t(const uint8_t* s, int n, const Filter& f, uint8_t*
   const uint8_t pk = sp[S_PROPS].kind;
   if (pk != K_ABSENT && pk != K_NULL && pk != K_OBJ) return r;
   if (sp[S_TIME].kind != K_STR) return r;   // absent = now() on the host
+  int utc_off = 0;
+  (void)utc_off;
   {
     const int tn = decode_string(s, sp[S_TIME].b, sp[S_TIME].e, scratch);
-    if (!parse_time(scratch, tn, &r.time_us)) return r;
+    if constexpr (ALL) {
+      if (!parse_time_t<true>(scratch, tn, &r.time_us, &utc_off)) return r;
+    } else {
+      if (!parse_time(scratch, tn, &r.time_us)) return r;
+    }
   }
 
   // PEventStore.find's filter
@@ -616,6 +648,10 @@ PIO_EV_HD Result parse_line_t(const uint8_t* s, int n, const Filter& f, uint8_t*
       kv->tok_e[q] = v.e;
     }
   }
+  if constexpr (ALL) {
+    pi->utc_off = utc_off;
+    if (pk == K_OBJ && pkeys > 0) pi->n_keys = pkeys, pi->b = sp[S_PROPS].b, pi->e = pend;
+  }
   r.outcome = MATCHED;
   return r;
 }
@@ -630,6 +666,82 @@ PIO_EV_HD Result parse_line_keys(const uint8_t* s, int n, const Filter& f, const
   kv->present = kv->number = 0;
   for (int q = 0; q < MAX_KEYS; ++q) kv->num[q] = 0.0, kv->tok_b[q] = kv->tok_e[q] = 0;
   return parse_line_t<true>(s, n, f, scratch, &kl, kv);
+}
+
+// *pi is cleared first, so that a line that is not MATCHED reports no keys
+PIO_EV_HD Result parse_line_props(const uint8_t* s, int n, const Filter& f, uint8_t* scratch, PropsInfo* pi) {
+  pi->n_keys = pi->b = pi->e = pi->utc_off = 0;
+  return parse_line_t<false, true>(s, n, f, scratch, nullptr, nullptr, pi);
+}
+
+// ---- the second walk: one record per key of a MATCHED line's `properties` object, in object order -------------------
+struct PropRec {
+  int kb, ke;       // the key's string token, quotes included
+  int vb, ve;       // the value's raw JSON token
+};
+
+// the end of the validated JSON value at s[i]
+PIO_EV_HD int skip_value(const uint8_t* s, int n, int i) {
+  uint8_t esc;
+  const uint8_t c = s[i];
+  if (c == '"') return scan_string(s, n, i, &esc);
+  if (c != '{' && c != '[') {   // number, true, false, null
+    while (i < n && s[i] != ',' && s[i] != '}' && s[i] != ']' && !is_ws(s[i])) ++i;
+    return i;
+  }
+  int d = 0;
+  for (;;) {
+    const uint8_t x = s[i];
+    if (x == '"') {
+      i = scan_string(s, n, i, &esc);
+      continue;
+    }
+    if (x == '{' || x == '[') ++d;
+    else if ((x == '}' || x == ']') && --d == 0) return i + 1;
+    ++i;
+  }
+}
+
+// *at: just after the object's "{" or after the previous value (PropsInfo::b + 1 to start); the object ends before e.
+// Fills *r and advances *at; false at the closing "}".
+PIO_EV_HD bool next_prop(const uint8_t* s, int e, int* at, PropRec* r) {
+  int i = *at;
+  while (is_ws(s[i]) || s[i] == ',') ++i;
+  if (s[i] == '}') return false;
+  uint8_t esc;
+  r->kb = i;
+  i = scan_string(s, e, i, &esc);
+  r->ke = i;
+  while (is_ws(s[i]) || s[i] == ':') ++i;
+  r->vb = i;
+  i = skip_value(s, e, i);
+  r->ve = i;
+  *at = i;
+  return true;
+}
+
+// the number of bytes decode_string writes for the validated string token [b, e)
+PIO_EV_HD int decoded_len(const uint8_t* s, int b, int e) {
+  int i = b + 1, o = 0;
+  const int end = e - 1;
+  while (i < end) {
+    if (s[i] != '\\') {
+      ++o, ++i;
+      continue;
+    }
+    if (s[i + 1] != 'u') {
+      ++o, i += 2;
+      continue;
+    }
+    const int u = hex4(s, e, i + 2);
+    i += 6;
+    if (u >= 0xD800 && u <= 0xDBFF) {
+      o += 4, i += 6;
+      continue;
+    }
+    o += u < 0x80 ? 1 : u < 0x800 ? 2 : 3;
+  }
+  return o;
 }
 
 }  // namespace ev

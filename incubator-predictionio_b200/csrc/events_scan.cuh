@@ -12,6 +12,10 @@
 // The keyed scan (pio_events_scan_keys) runs the same kernels with KEYS = true: the parse also reports the tracked
 // `properties` keys of each line (event_line.h parse_line_keys), one more scan places their token bytes, and the compaction
 // copies present / number masks, numbers and token bytes next to the ids.  KEYS = false is the plain scan, unchanged.
+// The whole-map scan (pio_events_scan_props) runs them with ALL = true: the parse counts the keys of `properties` and
+// notes where the object lies and eventTime's UTC offset (parse_line_props); a scan places each line's records;
+// ev_props_emit_kernel walks each object once more and writes one record per key, two more scans place the decoded
+// key bytes and the value tokens, and ev_props_copy_kernel copies them.
 // Output order comes from the scans alone: no atomics, the result is deterministic.  A chunk is < 2^31 bytes, so every
 // per-chunk count fits the 32-bit scan.
 #pragma once
@@ -117,11 +121,36 @@ __device__ __forceinline__ void ev_store_keys(const EvKeys& K, long long j, cons
   K.tok_len[j] = r.outcome == ev::MATCHED ? len : 0u;
 }
 
+// the whole-map scan (pio_events_scan_props): per line of the chunk, then per matched event (unused otherwise)
+struct EvProps {
+  uint32_t* n_rec;          // per line: top-level keys of `properties` of a matched line; then its exclusive scan in rec_pos
+  uint32_t* rec_pos;
+  uint32_t* obj_b;          // per line: the `properties` object, relative to the line start (PropsInfo::b)
+  uint32_t* obj_e;
+  int16_t* utc_off;         // per line: eventTime's UTC offset in minutes
+  long long rec_base;       // records of the call before this chunk
+  int16_t* o_utc_off;       // per matched event
+  long long* o_prop_off;    // per matched event: its first record in the caller's record columns
+};
+
+__device__ __forceinline__ void ev_store_props(const EvProps& P, long long j, const ev::Result& r, const ev::PropsInfo& pi) {
+  const bool m = r.outcome == ev::MATCHED;
+  P.n_rec[j] = m ? (uint32_t)pi.n_keys : 0u;
+  P.obj_b[j] = (uint32_t)pi.b;
+  P.obj_e[j] = (uint32_t)pi.e;
+  P.utc_off[j] = (int16_t)pi.utc_off;
+}
+
 // the parse of one line, stored
-template <bool KEYS>
+template <bool KEYS, bool ALL>
 __device__ __forceinline__ void ev_parse_store(const uint8_t* line, int n, const ev::Filter& f, uint8_t* scratch,
-                                               const EvLines& L, const EvKeys& K, long long j) {
-  if constexpr (KEYS) {
+                                               const EvLines& L, const EvKeys& K, const EvProps& P, long long j) {
+  if constexpr (ALL) {
+    ev::PropsInfo pi;
+    const ev::Result r = ev::parse_line_props(line, n, f, scratch, &pi);
+    ev_store(L, j, r);
+    ev_store_props(P, j, r, pi);
+  } else if constexpr (KEYS) {
     ev::KeyValues kv;
     const ev::Result r = ev::parse_line_keys(line, n, f, K.list, scratch, &kv);
     ev_store(L, j, r);
@@ -132,15 +161,15 @@ __device__ __forceinline__ void ev_parse_store(const uint8_t* line, int n, const
 }
 
 // one line per thread, read from global memory
-template <bool KEYS>
+template <bool KEYS, bool ALL = false>
 __global__ void __launch_bounds__(EV_THREADS)
 ev_parse_kernel(const uint8_t* __restrict__ t, const uint32_t* __restrict__ starts, long long nl, const ev::Filter f,
-                uint8_t* __restrict__ scratch, EvLines L, const EvKeys K) {
+                uint8_t* __restrict__ scratch, EvLines L, const EvKeys K, const EvProps P) {
   const long long j = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (j >= nl) return;
   uint32_t b, e;
   ev_line_range(t, starts, j, &b, &e);
-  ev_parse_store<KEYS>(t + b, (int)(e - b), f, scratch + b, L, K, j);
+  ev_parse_store<KEYS, ALL>(t + b, (int)(e - b), f, scratch + b, L, K, P, j);
 }
 
 // The same parse with the block's lines first copied into shared memory by the whole block in coalesced 16-byte loads
@@ -148,10 +177,10 @@ ev_parse_kernel(const uint8_t* __restrict__ t, const uint32_t* __restrict__ star
 // reads global memory like ev_parse_kernel.  `t` must be 16-byte aligned.
 constexpr int EV_SMEM_BYTES = 64 * 1024;
 
-template <bool KEYS>
+template <bool KEYS, bool ALL = false>
 __global__ void __launch_bounds__(EV_THREADS)
 ev_parse_smem_kernel(const uint8_t* __restrict__ t, const uint32_t* __restrict__ starts, long long nl,
-                     const ev::Filter f, uint8_t* __restrict__ scratch, EvLines L, const EvKeys K) {
+                     const ev::Filter f, uint8_t* __restrict__ scratch, EvLines L, const EvKeys K, const EvProps P) {
   extern __shared__ __align__(16) uint8_t ev_sm[];
   const long long j0 = (long long)blockIdx.x * blockDim.x;
   const long long j1 = j0 + blockDim.x < nl ? j0 + blockDim.x : nl;
@@ -169,7 +198,7 @@ ev_parse_smem_kernel(const uint8_t* __restrict__ t, const uint32_t* __restrict__
   if (j >= nl) return;
   uint32_t b, e;
   ev_line_range(t, starts, j, &b, &e);
-  ev_parse_store<KEYS>(staged ? ev_sm + (b - a0) : t + b, (int)(e - b), f, scratch + b, L, K, j);
+  ev_parse_store<KEYS, ALL>(staged ? ev_sm + (b - a0) : t + b, (int)(e - b), f, scratch + b, L, K, P, j);
 }
 
 struct EvOut {              // device output of one chunk, indexed by the chunk's match / fallback / byte slots
@@ -192,10 +221,10 @@ struct EvBase {
   long long line, byte, eid, tid;
 };
 
-template <bool KEYS>
+template <bool KEYS, bool ALL = false>
 __global__ void __launch_bounds__(EV_THREADS)
 ev_compact_kernel(const uint8_t* __restrict__ t, const uint32_t* __restrict__ starts, long long nl, const EvBase base,
-                  const uint8_t* __restrict__ scratch, const EvLines L, EvOut o, const EvKeys K) {
+                  const uint8_t* __restrict__ scratch, const EvLines L, EvOut o, const EvKeys K, const EvProps P) {
   const long long j = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (j >= nl) return;
   if (L.is_match[j]) {
@@ -222,6 +251,10 @@ ev_compact_kernel(const uint8_t* __restrict__ t, const uint32_t* __restrict__ st
         for (uint32_t c = tb; c < te; ++c) K.o_tok[at++] = t[b + c];
       }
     }
+    if constexpr (ALL) {
+      P.o_utc_off[k] = P.utc_off[j];
+      P.o_prop_off[k] = P.rec_base + P.rec_pos[j];
+    }
   } else if (L.is_fb[j]) {
     const uint32_t k = L.fb_pos[j];
     uint32_t b, e;
@@ -239,6 +272,58 @@ __global__ void ev_totals_kernel(const EvLines L, long long nl, uint32_t* __rest
   out[1] = L.fb_pos[j] + L.is_fb[j];
   out[2] = L.eid_pos[j] + L.eid_len[j];
   out[3] = L.tid_pos[j] + L.tid_len[j];
+}
+
+// ---- records of the whole-map scan: one per top-level key of a matched event's `properties`, in line and object order
+// (the next_prop walk of event_line.h over the object the parse validated).  Key and token ranges are chunk offsets.
+struct EvRecs {
+  uint32_t* kb;             // key string token [kb, ke), quotes included
+  uint32_t* ke;
+  uint32_t* vb;             // value token [vb, vb + v_len)
+  uint32_t* k_len;          // decoded key bytes; then the exclusive scans in k_pos / v_pos
+  uint32_t* v_len;
+  uint32_t* k_pos;
+  uint32_t* v_pos;
+};
+
+__global__ void __launch_bounds__(EV_THREADS)
+ev_props_emit_kernel(const uint8_t* __restrict__ t, const uint32_t* __restrict__ starts, long long nl, const EvProps P,
+                     EvRecs R) {
+  const long long j = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (j >= nl || P.n_rec[j] == 0) return;
+  const uint32_t b = starts[j];
+  const uint8_t* s = t + b;
+  uint32_t r = P.rec_pos[j];
+  int at = (int)P.obj_b[j] + 1;
+  ev::PropRec pr;
+  while (ev::next_prop(s, (int)P.obj_e[j], &at, &pr)) {
+    R.kb[r] = b + pr.kb;
+    R.ke[r] = b + pr.ke;
+    R.vb[r] = b + pr.vb;
+    R.k_len[r] = (uint32_t)ev::decoded_len(s, pr.kb, pr.ke);
+    R.v_len[r] = (uint32_t)(pr.ve - pr.vb);
+    ++r;
+  }
+}
+
+// one record per thread: the decoded key and the raw token, at their scanned positions
+__global__ void __launch_bounds__(EV_THREADS)
+ev_props_copy_kernel(const uint8_t* __restrict__ t, long long nr, const EvRecs R, long long key_base, long long tok_base,
+                     long long* __restrict__ o_key_off, uint8_t* __restrict__ o_key, long long* __restrict__ o_tok_off,
+                     uint8_t* __restrict__ o_tok) {
+  const long long r = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (r >= nr) return;
+  const uint32_t kp = R.k_pos[r], vp = R.v_pos[r], vb = R.vb[r], vn = R.v_len[r];
+  ev::decode_string(t, (int)R.kb[r], (int)R.ke[r], o_key + kp);
+  for (uint32_t c = 0; c < vn; ++c) o_tok[vp + c] = t[vb + c];
+  o_key_off[r] = key_base + kp;
+  o_tok_off[r] = tok_base + vp;
+}
+
+// key bytes and token bytes of the chunk's nr > 0 records
+__global__ void ev_props_totals_kernel(const EvRecs R, long long nr, uint32_t* __restrict__ out) {
+  out[0] = R.k_pos[nr - 1] + R.k_len[nr - 1];
+  out[1] = R.v_pos[nr - 1] + R.v_len[nr - 1];
 }
 
 }  // namespace pio

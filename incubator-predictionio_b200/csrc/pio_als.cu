@@ -2734,9 +2734,22 @@ struct EvFallback {
   int64_t n;
 };
 
-// one parsed chunk: matched events, fallback lines, entityId, targetEntityId and token bytes
+// where pio_events_scan_props puts the UTC offsets and records of the matched events (host buffers; capacities are
+// rec_capacity records and byte_capacity key / token bytes), and the records and bytes taken so far
+struct EvPropArgs {
+  int16_t* out_utc_off;     // per event
+  int64_t* out_prop_off;    // per event, and the closing entry
+  int64_t rec_capacity, byte_capacity;
+  uint8_t* out_key_bytes;
+  int64_t* out_key_off;     // per record, and the closing entry
+  uint8_t* out_tok_bytes;
+  int64_t* out_tok_off;
+  int64_t n_rec, n_key, n_tok;
+};
+
+// one parsed chunk: matched events, fallback lines, entityId, targetEntityId and token bytes, records
 struct EvTotals {
-  int64_t nm, nf, eb, tb, tk;
+  int64_t nm, nf, eb, tb, tk, nr;
 };
 
 // the checks of a scan's filter or an index view, made before any CUDA call
@@ -2811,8 +2824,10 @@ struct EvKernels {
   decltype(&ev_parse_kernel<false>) parse;
   decltype(&ev_compact_kernel<false>) compact;
 };
-static EvKernels ev_kernels(bool keys, bool smem) {
+static EvKernels ev_kernels(bool keys, bool all, bool smem) {
   if (keys) return {smem ? ev_parse_smem_kernel<true> : ev_parse_kernel<true>, ev_compact_kernel<true>};
+  if (all)
+    return {smem ? ev_parse_smem_kernel<false, true> : ev_parse_kernel<false, true>, ev_compact_kernel<false, true>};
   return {smem ? ev_parse_smem_kernel<false> : ev_parse_kernel<false>, ev_compact_kernel<false>};
 }
 
@@ -2843,6 +2858,54 @@ static int ev_take_host(EvHostCols& c, const EvKeyArgs* ka, const EvOut& o, cons
     CK0(cudaMemcpyAsync(ka->out_tok_bytes + K.tok_base, K.o_tok, tot.tk, cudaMemcpyDeviceToHost, st));
     ka->out_tok_off[c.n * nk] = K.tok_base + tot.tk;
   }
+  return PIO_ALS_OK;
+}
+
+// Delivery of the whole-map scan: ev_take_host's columns, each event's UTC offset and first record, and the chunk's
+// tot.nr records (per line: P.n_rec at P.rec_pos), walked out of the text t, their decoded keys and raw value tokens
+// placed by two scans and copied to the host after the records of the chunks before it.
+static int ev_take_props(EvHostCols& c, EvPropArgs* pa, const EvOut& o, const EvKeys& K, const EvProps& P,
+                         const uint8_t* t, const uint32_t* starts, long long nl, const EvBase& here, const EvTotals& tot,
+                         cudaStream_t st) {
+  const int64_t n = c.n, nm = tot.nm, nr = tot.nr;
+  if (pa->n_rec + nr > pa->rec_capacity) return fail(nullptr, PIO_ALS_ERR_ARG, "more records than rec_capacity");
+  const int rc = ev_take_host(c, nullptr, o, K, here, tot, st);
+  if (rc != PIO_ALS_OK) return rc;
+  CK0(cudaMemcpyAsync(pa->out_utc_off + n, P.o_utc_off, 2 * nm, cudaMemcpyDeviceToHost, st));
+  CK0(cudaMemcpyAsync(pa->out_prop_off + n, P.o_prop_off, 8 * nm, cudaMemcpyDeviceToHost, st));
+  pa->out_prop_off[c.n] = pa->n_rec + nr;
+  if (nr == 0) return PIO_ALS_OK;
+  Scratch sc(st);
+  EvRecs R;
+  for (uint32_t** p : {&R.kb, &R.ke, &R.vb, &R.k_len, &R.v_len, &R.k_pos, &R.v_pos}) CK0(sc.alloc(p, (size_t)nr));
+  uint32_t* d_tot = nullptr;
+  CK0(sc.alloc(&d_tot, 2));
+  ev_props_emit_kernel<<<nblk(nl, EV_THREADS), EV_THREADS, 0, st>>>(t, starts, nl, P, R);
+  CK0(cudaGetLastError());
+  CK0(scan_exclusive_u32(R.k_len, R.k_pos, (size_t)nr, st, nullptr));
+  CK0(scan_exclusive_u32(R.v_len, R.v_pos, (size_t)nr, st, nullptr));
+  ev_props_totals_kernel<<<1, 1, 0, st>>>(R, nr, d_tot);
+  uint32_t h_tot[2];
+  CK0(cudaMemcpyAsync(h_tot, d_tot, sizeof h_tot, cudaMemcpyDeviceToHost, st));
+  CK0(cudaStreamSynchronize(st));
+  const int64_t kb = h_tot[0], vb = h_tot[1];
+  if (pa->n_key + kb > pa->byte_capacity || pa->n_tok + vb > pa->byte_capacity)
+    return fail(nullptr, PIO_ALS_ERR_ARG, "more key or token bytes than n_bytes");
+  uint8_t *o_key = nullptr, *o_tok = nullptr;
+  long long *o_key_off = nullptr, *o_tok_off = nullptr;
+  CK0(sc.alloc(&o_key, (size_t)kb));
+  CK0(sc.alloc(&o_tok, (size_t)vb));
+  CK0(sc.alloc(&o_key_off, (size_t)nr));
+  CK0(sc.alloc(&o_tok_off, (size_t)nr));
+  ev_props_copy_kernel<<<nblk(nr, EV_THREADS), EV_THREADS, 0, st>>>(t, nr, R, pa->n_key, pa->n_tok, o_key_off, o_key,
+                                                                    o_tok_off, o_tok);
+  CK0(cudaGetLastError());
+  CK0(cudaMemcpyAsync(pa->out_key_off + pa->n_rec, o_key_off, 8 * nr, cudaMemcpyDeviceToHost, st));
+  CK0(cudaMemcpyAsync(pa->out_tok_off + pa->n_rec, o_tok_off, 8 * nr, cudaMemcpyDeviceToHost, st));
+  CK0(cudaMemcpyAsync(pa->out_key_bytes + pa->n_key, o_key, (size_t)kb, cudaMemcpyDeviceToHost, st));
+  CK0(cudaMemcpyAsync(pa->out_tok_bytes + pa->n_tok, o_tok, (size_t)vb, cudaMemcpyDeviceToHost, st));
+  pa->n_rec += nr, pa->n_key += kb, pa->n_tok += vb;
+  pa->out_key_off[pa->n_rec] = pa->n_key, pa->out_tok_off[pa->n_rec] = pa->n_tok;
   return PIO_ALS_OK;
 }
 
@@ -2927,9 +2990,10 @@ static int eix_take_chunk(EixBatch* b, const EvOut& o, const uint8_t* t, const u
 // The chunk loop of every event scan, over text[0, n_bytes) (n_bytes > 0, f checked): cuts the text into device chunks,
 // stages each through pinned memory on a copy stream, and parses, scans and compacts it on the scan stream.  Each
 // chunk's matched events are delivered to the host columns `cols` (with ka: and their key columns) or, when batch is
-// set, into that index batch.  Lines longer than a chunk and the lines the device leaves to the host go to *fb.
+// set, into that index batch; with pa, the host columns and every key of `properties` as records (ka is then NULL).
+// Lines longer than a chunk and the lines the device leaves to the host go to *fb.
 static int ev_scan(int device, const uint8_t* text, int64_t n_bytes, const pio_events_filter* f, const EvKeyArgs* ka,
-                   EvHostCols* cols, EixBatch* batch, EvFallback* fb, int64_t* n_lines) {
+                   EvPropArgs* pa, EvHostCols* cols, EixBatch* batch, EvFallback* fb, int64_t* n_lines) {
   CK0(cudaSetDevice(device));
   int64_t cap = 64ll << 20;   // device chunk; PIO_EVENTS_DEVICE_CHUNK (bytes) lets tests straddle its boundaries
   if (const char* c = getenv("PIO_EVENTS_DEVICE_CHUNK")) {
@@ -2952,7 +3016,7 @@ static int ev_scan(int device, const uint8_t* text, int64_t n_bytes, const pio_e
   tm = EvTiming{};
   bool use_smem = true;   // PIO_EVENTS_SMEM=0: the parse reads its lines from global memory (A/B measurements)
   if (const char* c = getenv("PIO_EVENTS_SMEM")) use_smem = atoi(c) != 0;
-  const EvKernels kn = ev_kernels(ka != nullptr, use_smem);
+  const EvKernels kn = ev_kernels(ka != nullptr, pa != nullptr, use_smem);
   if (use_smem) CK0(cudaFuncSetAttribute(kn.parse, cudaFuncAttributeMaxDynamicSharedMemorySize, EV_SMEM_BYTES));
   uint8_t *d_text[2] = {nullptr, nullptr}, *stage[2] = {nullptr, nullptr}, *d_scratch = nullptr;
   uint32_t *d_flag = nullptr, *d_lid = nullptr, *d_tot = nullptr, *h_tot = nullptr;
@@ -2967,6 +3031,7 @@ static int ev_scan(int device, const uint8_t* text, int64_t n_bytes, const pio_e
   CK0(tmp.host(&h_tot, 8));
   ev::Filter df;
   EvKeys K{};
+  EvProps P{};
   const int nk = ka ? ka->n : 0;
   const int urc = ev_upload_filter(f, ka ? ka->keys : nullptr, nk, tmp, &df, &K.list);
   if (urc != PIO_ALS_OK) return urc;
@@ -3084,17 +3149,25 @@ static int ev_scan(int device, const uint8_t* text, int64_t n_bytes, const pio_e
       CK0(chunk.alloc(&K.o_tok, (size_t)L));   // tokens are disjoint pieces of the chunk's text
       K.tok_base = n_tok;
     }
+    if (pa) {
+      for (uint32_t** p : {&P.n_rec, &P.rec_pos, &P.obj_b, &P.obj_e}) CK0(chunk.alloc(p, nls));
+      CK0(chunk.alloc(&P.utc_off, nls));
+      CK0(chunk.alloc(&P.o_utc_off, nls));
+      CK0(chunk.alloc(&P.o_prop_off, nls));
+      P.rec_base = pa->n_rec;
+    }
     CK0(cudaEventRecord(k2, ex));
     ev_start_scatter_kernel<<<nblk(L, EV_THREADS), EV_THREADS, 0, ex>>>(d_flag, d_lid, L, nl, starts);
     const unsigned gl = nblk(nl, EV_THREADS);
-    kn.parse<<<gl, EV_THREADS, use_smem ? EV_SMEM_BYTES : 0, ex>>>(t, starts, nl, df, d_scratch, Ls, K);
+    kn.parse<<<gl, EV_THREADS, use_smem ? EV_SMEM_BYTES : 0, ex>>>(t, starts, nl, df, d_scratch, Ls, K, P);
     CK0(cudaGetLastError());
     CK0(scan_exclusive_u32(Ls.is_match, Ls.match_pos, nls, ex, nullptr));
     CK0(scan_exclusive_u32(Ls.is_fb, Ls.fb_pos, nls, ex, nullptr));
     CK0(scan_exclusive_u32(Ls.eid_len, Ls.eid_pos, nls, ex, nullptr));
     CK0(scan_exclusive_u32(Ls.tid_len, Ls.tid_pos, nls, ex, nullptr));
     if (ka) CK0(scan_exclusive_u32(K.tok_len, K.tok_pos, nls, ex, nullptr));
-    kn.compact<<<gl, EV_THREADS, 0, ex>>>(t, starts, nl, here, d_scratch, Ls, o, K);
+    if (pa) CK0(scan_exclusive_u32(P.n_rec, P.rec_pos, nls, ex, nullptr));
+    kn.compact<<<gl, EV_THREADS, 0, ex>>>(t, starts, nl, here, d_scratch, Ls, o, K, P);
     ev_totals_kernel<<<1, 1, 0, ex>>>(Ls, nl, d_tot);
     CK0(cudaGetLastError());
     CK0(cudaEventRecord(k3, ex));
@@ -3103,15 +3176,21 @@ static int ev_scan(int device, const uint8_t* text, int64_t n_bytes, const pio_e
       CK0(cudaMemcpyAsync(h_tot + 6, K.tok_pos + nl - 1, 4, cudaMemcpyDeviceToHost, ex));
       CK0(cudaMemcpyAsync(h_tot + 7, K.tok_len + nl - 1, 4, cudaMemcpyDeviceToHost, ex));
     }
+    if (pa) {   // records of the chunk, the same way
+      CK0(cudaMemcpyAsync(h_tot + 6, P.rec_pos + nl - 1, 4, cudaMemcpyDeviceToHost, ex));
+      CK0(cudaMemcpyAsync(h_tot + 7, P.n_rec + nl - 1, 4, cudaMemcpyDeviceToHost, ex));
+    }
     // find and stage the next chunk while this one is parsed (oversized lines before it belong after this chunk's
     // lines, so their line numbers are assigned only now that this chunk's line count is known)
     int64_t nb, ne;
     next_chunk(ce, &nb, &ne);
     if (nb < ne && prefetch(slot ^ 1, nb, ne) != PIO_ALS_OK) return PIO_ALS_ERR_CUDA;
     CK0(cudaStreamSynchronize(ex));
-    const EvTotals tot{h_tot[0], h_tot[1], h_tot[2], h_tot[3], ka ? (int64_t)h_tot[6] + h_tot[7] : 0};
+    const int64_t last = (int64_t)h_tot[6] + h_tot[7];
+    const EvTotals tot{h_tot[0], h_tot[1], h_tot[2], h_tot[3], ka ? last : 0, pa ? last : 0};
     CK0(cudaEventRecord(d0, ex));
     const int rc = batch ? eix_take_chunk(batch, o, t, starts, here, here.eid, tot.nm, tot.eb, ex)
+                   : pa  ? ev_take_props(*cols, pa, o, K, P, t, starts, nl, here, tot, ex)
                          : ev_take_host(*cols, ka, o, K, here, tot, ex);
     if (rc != PIO_ALS_OK) return rc;
     const int64_t room = fb->capacity - fb->n, nfc = tot.nf < room ? tot.nf : (room > 0 ? room : 0);
@@ -3137,9 +3216,10 @@ static int ev_scan(int device, const uint8_t* text, int64_t n_bytes, const pio_e
   return PIO_ALS_OK;
 }
 
-// pio_events_scan (ka == nullptr) and pio_events_scan_keys: the checks they share, then the chunk loop into host columns
+// pio_events_scan (ka, pa == nullptr), pio_events_scan_keys (ka) and pio_events_scan_props (pa): the checks they share,
+// then the chunk loop into host columns
 static int ev_scan_host(int device, const uint8_t* text, int64_t n_bytes, const pio_events_filter* f,
-                        const EvKeyArgs* ka, EvHostCols cols, int64_t* out_n_events, EvFallback fb,
+                        const EvKeyArgs* ka, EvPropArgs* pa, EvHostCols cols, int64_t* out_n_events, EvFallback fb,
                         int64_t* out_n_fallback, int64_t* out_n_lines) {
   if (n_bytes < 0 || (n_bytes > 0 && !text) || !f || fb.capacity < 0 || cols.capacity < n_bytes /
       PIO_EVENTS_MIN_EVENT_BYTES + 1 || !cols.line || !cols.code || !cols.value || !cols.flags || !cols.time_us ||
@@ -3151,8 +3231,9 @@ static int ev_scan_host(int device, const uint8_t* text, int64_t n_bytes, const 
   *out_n_fallback = *out_n_lines = *out_n_events = 0;
   cols.eid_off[0] = cols.tid_off[0] = 0;
   if (ka) ka->out_tok_off[0] = 0;
+  if (pa) pa->out_prop_off[0] = pa->out_key_off[0] = pa->out_tok_off[0] = 0;
   if (n_bytes == 0) return PIO_ALS_OK;
-  rc = ev_scan(device, text, n_bytes, f, ka, &cols, nullptr, &fb, out_n_lines);
+  rc = ev_scan(device, text, n_bytes, f, ka, pa, &cols, nullptr, &fb, out_n_lines);
   if (rc != PIO_ALS_OK) return rc;
   *out_n_events = cols.n;
   *out_n_fallback = fb.n;
@@ -3166,7 +3247,7 @@ int pio_events_scan(int device, const uint8_t* text, int64_t n_bytes, const pio_
                     int64_t* out_fb_end, int64_t* out_n_fallback, int64_t* out_n_lines) {
   const EvHostCols cols{capacity,      out_line,    out_code,      out_value,   out_flags, out_time_us,
                         out_eid_bytes, out_eid_off, out_tid_bytes, out_tid_off, 0};
-  return ev_scan_host(device, text, n_bytes, f, nullptr, cols, out_n_events,
+  return ev_scan_host(device, text, n_bytes, f, nullptr, nullptr, cols, out_n_events,
                       EvFallback{fb_capacity, out_fb_line, out_fb_begin, out_fb_end, 0}, out_n_fallback, out_n_lines);
 }
 
@@ -3190,8 +3271,31 @@ int pio_events_scan_keys(int device, const uint8_t* text, int64_t n_bytes, const
   const EvKeyArgs ka{keys, n_keys, out_present, out_number, out_num, out_tok_bytes, out_tok_off};
   const EvHostCols cols{capacity,      out_line,    out_code,      out_value,   out_flags, out_time_us,
                         out_eid_bytes, out_eid_off, out_tid_bytes, out_tid_off, 0};
-  return ev_scan_host(device, text, n_bytes, f, &ka, cols, out_n_events,
+  return ev_scan_host(device, text, n_bytes, f, &ka, nullptr, cols, out_n_events,
                       EvFallback{fb_capacity, out_fb_line, out_fb_begin, out_fb_end, 0}, out_n_fallback, out_n_lines);
+}
+
+int pio_events_scan_props(int device, const uint8_t* text, int64_t n_bytes, const pio_events_filter* f,
+                          int64_t capacity, int64_t* out_line, int32_t* out_code, double* out_value, uint8_t* out_flags,
+                          int64_t* out_time_us, uint8_t* out_eid_bytes, int64_t* out_eid_off, uint8_t* out_tid_bytes,
+                          int64_t* out_tid_off, int16_t* out_utc_offset, int64_t* out_prop_off, int64_t rec_capacity,
+                          uint8_t* out_key_bytes, int64_t* out_key_off, uint8_t* out_tok_bytes, int64_t* out_tok_off,
+                          int64_t* out_n_events, int64_t* out_n_records, int64_t fb_capacity, int64_t* out_fb_line,
+                          int64_t* out_fb_begin, int64_t* out_fb_end, int64_t* out_n_fallback, int64_t* out_n_lines) {
+  if (n_bytes < 0 || !out_utc_offset || !out_prop_off || rec_capacity < n_bytes / PIO_EVENTS_MIN_RECORD_BYTES + 1 ||
+      !out_key_bytes || !out_key_off || !out_tok_bytes || !out_tok_off || !out_n_records)
+    return fail(nullptr, PIO_ALS_ERR_ARG, "bad pio_events_scan_props arguments");
+  if (!f || f->property) return fail(nullptr, PIO_ALS_ERR_ARG, "pio_events_scan_props: filter->property must be NULL");
+  *out_n_records = 0;
+  EvPropArgs pa{out_utc_offset, out_prop_off, rec_capacity, n_bytes, out_key_bytes, out_key_off, out_tok_bytes,
+                out_tok_off, 0, 0, 0};
+  const EvHostCols cols{capacity,      out_line,    out_code,      out_value,   out_flags, out_time_us,
+                        out_eid_bytes, out_eid_off, out_tid_bytes, out_tid_off, 0};
+  const int rc = ev_scan_host(device, text, n_bytes, f, nullptr, &pa, cols, out_n_events,
+                              EvFallback{fb_capacity, out_fb_line, out_fb_begin, out_fb_end, 0}, out_n_fallback,
+                              out_n_lines);
+  if (rc == PIO_ALS_OK) *out_n_records = pa.n_rec;
+  return rc;
 }
 
 // ---- $set / $unset / $delete fold (PEventStore.aggregatePropertyColumns; events_fold.cuh) -----------------------------
@@ -3272,6 +3376,190 @@ int pio_events_fold(int device, const uint8_t* eid_bytes, const int64_t* eid_off
   if (nk) CK0(cudaMemcpyAsync(out_winner, d_win, 8 * ne * nk, cudaMemcpyDeviceToHost, st));
   CK0(cudaStreamSynchronize(st));
   *out_n_entities = n_ent;
+  return PIO_ALS_OK;
+}
+
+// ---- the fold of every key (PEventStore.aggregatePropertyMaps; events_fold.cuh) ----------------------------------------
+int pio_events_fold_props(int device, const uint8_t* eid_bytes, const int64_t* eid_off, const int32_t* code,
+                          const int64_t* time_us, const int64_t* prop_off, int64_t n, const uint8_t* key_bytes,
+                          const int64_t* key_off, int64_t* out_first_event, uint8_t* out_exists,
+                          int64_t* out_first_time_event, int64_t* out_last_time_event, int64_t* out_win_off,
+                          int64_t* out_win_rec, int32_t* out_win_key, int64_t* out_key_first, int64_t* out_n_entities,
+                          int64_t* out_n_keys) {
+  if (n < 0 || !eid_off || !prop_off || !out_n_entities || !out_n_keys ||
+      (n > 0 && (!code || !time_us || !out_first_event || !out_exists || !out_first_time_event ||
+                 !out_last_time_event || !out_win_off || (!eid_bytes && eid_off[n] > eid_off[0]))))
+    return fail(nullptr, PIO_ALS_ERR_ARG, "bad pio_events_fold_props arguments");
+  *out_n_entities = *out_n_keys = 0;
+  if (n == 0) return PIO_ALS_OK;
+  if (n >= (1ll << 31)) return fail(nullptr, PIO_ALS_ERR_ARG, "n must be < 2^31");
+  if (eid_off[0] != 0 || prop_off[0] != 0) return fail(nullptr, PIO_ALS_ERR_ARG, "eid_off[0] and prop_off[0] must be 0");
+  int64_t max_keys = 0;   // records of the largest event: the bits of an index in one object
+  for (int64_t e = 0; e < n; ++e) {
+    if (code[e] < FOLD_SET || code[e] > FOLD_DELETE)
+      return fail(nullptr, PIO_ALS_ERR_ARG, "code[%lld] = %d is not 0 ($set), 1 ($unset) or 2 ($delete)", (long long)e,
+                  code[e]);
+    if (prop_off[e + 1] < prop_off[e]) return fail(nullptr, PIO_ALS_ERR_ARG, "prop_off must not decrease");
+    max_keys = std::max(max_keys, prop_off[e + 1] - prop_off[e]);
+  }
+  const int64_t nr = prop_off[n];
+  if (nr >= (1ll << 31)) return fail(nullptr, PIO_ALS_ERR_ARG, "prop_off[n] must be < 2^31");
+  if (nr > 0 && (!key_off || !out_win_rec || !out_win_key || !out_key_first || key_off[0] != 0 ||
+                 (!key_bytes && key_off[nr] > 0)))
+    return fail(nullptr, PIO_ALS_ERR_ARG, "bad pio_events_fold_props record arguments");
+  CK0(cudaSetDevice(device));
+  const size_t nb = (size_t)eid_off[n], nn = (size_t)n;
+  cudaStream_t st = 0;
+  CallMem tmp(st);
+  uint8_t *d_bytes = nullptr, *d_exists = nullptr;
+  long long *d_off = nullptr, *d_time = nullptr, *d_first = nullptr, *d_fev = nullptr, *d_lev = nullptr,
+            *d_woff = nullptr, *d_prop = nullptr;
+  int32_t* d_code = nullptr;
+  int *d_ent = nullptr, *seg_first = nullptr, *seg_last = nullptr, *last_set = nullptr, *last_del = nullptr,
+      *last_time = nullptr;
+  uint64_t *ka = nullptr, *kb = nullptr;
+  uint32_t *va = nullptr, *vb = nullptr, *rank = nullptr;
+  CK0(tmp.device(&d_bytes, nb));
+  CK0(tmp.device(&d_off, nn + 1));
+  CK0(tmp.device(&d_code, nn));
+  CK0(tmp.device(&d_time, nn));
+  CK0(tmp.device(&d_prop, nn + 1));
+  CK0(tmp.device(&d_ent, nn));
+  CK0(tmp.device(&d_first, nn));
+  CK0(tmp.device(&rank, nn));
+  CK0(tmp.device(&ka, nn)); CK0(tmp.device(&kb, nn));
+  CK0(tmp.device(&va, nn)); CK0(tmp.device(&vb, nn));
+  CK0(cudaMemcpyAsync(d_bytes, eid_bytes, nb, cudaMemcpyHostToDevice, st));
+  CK0(cudaMemcpyAsync(d_off, eid_off, 8 * (nn + 1), cudaMemcpyHostToDevice, st));
+  CK0(cudaMemcpyAsync(d_code, code, 4 * nn, cudaMemcpyHostToDevice, st));
+  CK0(cudaMemcpyAsync(d_time, time_us, 8 * nn, cudaMemcpyHostToDevice, st));
+  CK0(cudaMemcpyAsync(d_prop, prop_off, 8 * (nn + 1), cudaMemcpyHostToDevice, st));
+  int64_t n_ent = 0;
+  int rc = ids_encode_device(d_bytes, d_off, n, st, d_ent, d_first, &n_ent);
+  if (rc != PIO_ALS_OK) return rc;
+  const size_t ne = (size_t)n_ent;
+  CK0(tmp.device(&seg_first, ne)); CK0(tmp.device(&seg_last, ne));
+  CK0(tmp.device(&last_set, ne)); CK0(tmp.device(&last_del, ne)); CK0(tmp.device(&last_time, ne));
+  CK0(tmp.device(&d_exists, ne));
+  CK0(tmp.device(&d_fev, ne)); CK0(tmp.device(&d_lev, ne));
+  CK0(tmp.device(&d_woff, ne + 1));
+  CK0(cudaMemsetAsync(last_set, 0xFF, 4 * ne, st));   // -1: none
+  CK0(cudaMemsetAsync(last_del, 0xFF, 4 * ne, st));
+  // (entity, time, line), as pio_events_fold
+  fold_time_key_kernel<<<nblk(n, 256), 256, 0, st>>>(d_time, n, ka, va);
+  bool in_b = false;
+  CK0(radix_sort_pairs(ka, va, kb, vb, nn, 64, st, &in_b, nullptr));
+  uint64_t* k1 = in_b ? kb : ka;
+  uint32_t* v1 = in_b ? vb : va;
+  uint64_t* k2 = in_b ? ka : kb;
+  uint32_t* v2 = in_b ? va : vb;
+  fold_entity_key_kernel<<<nblk(n, 256), 256, 0, st>>>(v1, d_ent, n, k1);
+  CK0(radix_sort_pairs(k1, v1, k2, v2, nn, ceil_log2((uint64_t)n_ent), st, &in_b, nullptr));
+  const uint64_t* ks = in_b ? k2 : k1;
+  const uint32_t* vs = in_b ? v2 : v1;
+  fold_reduce_kernel<<<nblk(n, 256), 256, 0, st>>>(ks, vs, d_code, nullptr, 0, n, seg_first, seg_last, last_set,
+                                                   last_del, nullptr);
+  fold_last_time_kernel<<<nblk(n, 256), 256, 0, st>>>(ks, vs, d_time, seg_last, n, last_time);
+  fold_rank_kernel<<<nblk(n, 256), 256, 0, st>>>(vs, n, rank);
+  CK0(cudaGetLastError());
+
+  uint32_t* count = nullptr;   // winners per entity, then their exclusive scan: the CSR
+  CK0(tmp.device(&count, ne + 1));
+  CK0(cudaMemsetAsync(count, 0, 4 * (ne + 1), st));
+  int64_t n_kc = 0, nw = 0;
+  if (nr > 0) {
+    const size_t nrs = (size_t)nr;
+    uint8_t* d_kbytes = nullptr;
+    long long *d_koff = nullptr, *d_kfirst = nullptr, *d_wrec = nullptr;
+    int *kcode = nullptr, *seg_unset = nullptr, *seg_set = nullptr, *seg_place = nullptr, *d_wkey = nullptr;
+    uint64_t *ra = nullptr, *rb = nullptr;
+    uint32_t *rva = nullptr, *rvb = nullptr, *rec_ev = nullptr, *head = nullptr, *seg_id = nullptr;
+    CK0(tmp.device(&d_kbytes, (size_t)key_off[nr]));
+    CK0(tmp.device(&d_koff, nrs + 1));
+    CK0(tmp.device(&kcode, nrs));
+    CK0(tmp.device(&d_kfirst, nrs));
+    CK0(tmp.device(&rec_ev, nrs));
+    CK0(tmp.device(&head, nrs)); CK0(tmp.device(&seg_id, nrs));
+    CK0(tmp.device(&ra, nrs)); CK0(tmp.device(&rb, nrs));
+    CK0(tmp.device(&rva, nrs)); CK0(tmp.device(&rvb, nrs));
+    CK0(cudaMemcpyAsync(d_kbytes, key_bytes, (size_t)key_off[nr], cudaMemcpyHostToDevice, st));
+    CK0(cudaMemcpyAsync(d_koff, key_off, 8 * (nrs + 1), cudaMemcpyHostToDevice, st));
+    rc = ids_encode_device(d_kbytes, d_koff, nr, st, kcode, d_kfirst, &n_kc);   // key codes
+    if (rc != PIO_ALS_OK) return rc;
+    const int kbits = ceil_log2((uint64_t)n_kc), ebits = ceil_log2((uint64_t)n_ent);
+    fold_rec_event_kernel<<<nblk(n, 256), 256, 0, st>>>(d_prop, n, rec_ev);
+    // (entity, key, time, line, index in the object): stable by sorted event position, then by (entity, key)
+    fold_rec_rank_key_kernel<<<nblk(nr, 256), 256, 0, st>>>(rec_ev, rank, nr, ra, rva);
+    CK0(radix_sort_pairs(ra, rva, rb, rvb, nrs, ceil_log2((uint64_t)n), st, &in_b, nullptr));
+    uint64_t* r1 = in_b ? rb : ra;
+    uint32_t* p1 = in_b ? rvb : rva;
+    uint64_t* r2 = in_b ? ra : rb;
+    uint32_t* p2 = in_b ? rva : rvb;
+    fold_rec_key_kernel<<<nblk(nr, 256), 256, 0, st>>>(p1, rec_ev, d_ent, kcode, kbits, nr, r1);
+    CK0(radix_sort_pairs(r1, p1, r2, p2, nrs, ebits + kbits, st, &in_b, nullptr));
+    const uint64_t* rk = in_b ? r2 : r1;
+    const uint32_t* rp = in_b ? p2 : p1;
+    fold_seg_flag_kernel<<<nblk(nr, 256), 256, 0, st>>>(rk, nr, head);
+    CK0(scan_exclusive_u32(head, seg_id, nrs, st, nullptr));
+    uint32_t last[2] = {0, 0};
+    CK0(cudaMemcpyAsync(last, seg_id + nr - 1, 4, cudaMemcpyDeviceToHost, st));
+    CK0(cudaMemcpyAsync(last + 1, head + nr - 1, 4, cudaMemcpyDeviceToHost, st));
+    CK0(cudaStreamSynchronize(st));
+    const int64_t n_seg = (int64_t)last[0] + last[1];
+    const size_t nsg = (size_t)n_seg;
+    uint32_t *present = nullptr, *w_pos = nullptr;
+    CK0(tmp.device(&seg_unset, nsg)); CK0(tmp.device(&seg_set, nsg)); CK0(tmp.device(&seg_place, nsg));
+    CK0(tmp.device(&present, nsg)); CK0(tmp.device(&w_pos, nsg));
+    CK0(cudaMemsetAsync(seg_unset, 0xFF, 4 * nsg, st));
+    CK0(cudaMemsetAsync(seg_set, 0xFF, 4 * nsg, st));
+    CK0(cudaMemsetAsync(seg_place, 0x7F, 4 * nsg, st));   // 0x7F7F7F7F: above every position
+    fold_props_last_kernel<<<nblk(nr, 256), 256, 0, st>>>(rp, rec_ev, rank, d_code, head, seg_id, nr, seg_unset,
+                                                          seg_set);
+    fold_props_place_kernel<<<nblk(nr, 256), 256, 0, st>>>(rp, rec_ev, rank, d_code, d_ent, last_del, head, seg_id,
+                                                           seg_unset, nr, seg_place);
+    fold_props_present_kernel<<<nblk(n_seg, 256), 256, 0, st>>>(rp, rec_ev, rank, d_ent, last_del, seg_unset, seg_set,
+                                                                n_seg, present);
+    CK0(cudaGetLastError());
+    CK0(scan_exclusive_u32(present, w_pos, nsg, st, nullptr));
+    CK0(cudaMemcpyAsync(last, w_pos + n_seg - 1, 4, cudaMemcpyDeviceToHost, st));
+    CK0(cudaMemcpyAsync(last + 1, present + n_seg - 1, 4, cudaMemcpyDeviceToHost, st));
+    CK0(cudaStreamSynchronize(st));
+    nw = (int64_t)last[0] + last[1];
+    if (nw > 0) {
+      // the winners in dict order: the sorted record buffers are free again
+      const int ibits = ceil_log2((uint64_t)max_keys);
+      uint64_t* wk = const_cast<uint64_t*>(rk) == ra ? rb : ra;
+      uint32_t* wv = const_cast<uint32_t*>(rp) == rva ? rvb : rva;
+      fold_props_winner_kernel<<<nblk(n_seg, 256), 256, 0, st>>>(rp, rec_ev, rank, d_prop, present, w_pos, seg_set,
+                                                                 seg_place, ibits, n_seg, wk, wv);
+      uint64_t* wk2 = wk == ra ? rb : ra;   // rk / rp are no longer read
+      uint32_t* wv2 = wv == rva ? rvb : rva;
+      CK0(radix_sort_pairs(wk, wv, wk2, wv2, (size_t)nw, ceil_log2((uint64_t)n) + ibits, st, &in_b, nullptr));
+      const uint32_t* ws = in_b ? wv2 : wv;
+      CK0(tmp.device(&d_wrec, (size_t)nw));
+      CK0(tmp.device(&d_wkey, (size_t)nw));
+      fold_props_out_kernel<<<nblk(nw, 256), 256, 0, st>>>(ws, rec_ev, d_ent, kcode, nw, count, d_wrec, d_wkey);
+      CK0(cudaGetLastError());
+      CK0(cudaMemcpyAsync(out_win_rec, d_wrec, 8 * (size_t)nw, cudaMemcpyDeviceToHost, st));
+      CK0(cudaMemcpyAsync(out_win_key, d_wkey, 4 * (size_t)nw, cudaMemcpyDeviceToHost, st));
+    }
+    CK0(cudaMemcpyAsync(out_key_first, d_kfirst, 8 * (size_t)n_kc, cudaMemcpyDeviceToHost, st));
+    CK0(cudaStreamSynchronize(st));
+  }
+  uint32_t* w_off = nullptr;
+  CK0(tmp.device(&w_off, ne + 1));
+  CK0(scan_exclusive_u32(count, w_off, ne + 1, st, nullptr));
+  fold_props_finish_kernel<<<nblk(n_ent + 1, 256), 256, 0, st>>>(vs, seg_first, last_time, last_set, last_del, w_off,
+                                                                 n_ent, d_exists, d_fev, d_lev, d_woff);
+  CK0(cudaGetLastError());
+  CK0(cudaMemcpyAsync(out_first_event, d_first, 8 * ne, cudaMemcpyDeviceToHost, st));
+  CK0(cudaMemcpyAsync(out_exists, d_exists, ne, cudaMemcpyDeviceToHost, st));
+  CK0(cudaMemcpyAsync(out_first_time_event, d_fev, 8 * ne, cudaMemcpyDeviceToHost, st));
+  CK0(cudaMemcpyAsync(out_last_time_event, d_lev, 8 * ne, cudaMemcpyDeviceToHost, st));
+  CK0(cudaMemcpyAsync(out_win_off, d_woff, 8 * (ne + 1), cudaMemcpyDeviceToHost, st));
+  CK0(cudaStreamSynchronize(st));
+  *out_n_entities = n_ent;
+  *out_n_keys = n_kc;
   return PIO_ALS_OK;
 }
 
@@ -3451,7 +3739,7 @@ int pio_events_index_append(pio_events_index* ix, const uint8_t* text, int64_t n
   b.mask = ix->mask;
   EvFallback fb{fb_capacity, nullptr, out_fb_begin, out_fb_end, 0};
   const auto t0 = Clock::now();
-  const int rc = ev_scan(ix->device, text, n_bytes, &ix->view, nullptr, nullptr, &b, &fb, nullptr);
+  const int rc = ev_scan(ix->device, text, n_bytes, &ix->view, nullptr, nullptr, nullptr, &b, &fb, nullptr);
   ix->stats.scan_ms = ms_since(t0);
   if (rc != PIO_ALS_OK) return rc;
   *out_n_fallback = fb.n;

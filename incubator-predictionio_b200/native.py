@@ -32,7 +32,8 @@ EXPORTED_SYMBOLS = [
     "pio_als_set_init", "pio_als_run", "pio_als_get_factors", "pio_als_train", "pio_als_recommend",
     "pio_als_similar", "pio_als_similar_batch", "pio_als_model_import", "pio_als_save", "pio_als_load", "pio_als_get_stats", "pio_als_get_phase_ms",
     "pio_als_synth_ratings_device", "pio_nb_train", "pio_nb_predict", "pio_ids_encode", "pio_cooc_train",
-    "pio_events_scan", "pio_events_scan_keys", "pio_events_fold", "pio_events_index_create",
+    "pio_events_scan", "pio_events_scan_keys", "pio_events_fold", "pio_events_scan_props", "pio_events_fold_props",
+    "pio_events_index_create",
     "pio_events_index_append", "pio_events_index_add_host", "pio_events_index_lookup", "pio_events_index_get_stats",
     "pio_events_index_destroy",
 ]
@@ -471,6 +472,90 @@ def _events_scan(text, entity_type, event_names, target_mode, target_entity_type
         res["tok_off"] = out["tok_off"][:m * nk + 1]
         res["tok_bytes"] = out["tok_bytes"][:res["tok_off"][-1]]
     return res
+
+
+EVENTS_MIN_RECORD_BYTES = 4
+
+
+def events_scan_props(text, entity_type=None, event_names=None, target_mode=EVENTS_TARGET_ANY, target_entity_type=None,
+                      start_us=None, until_us=None, device=0):
+    """pio_events_scan_props: events_scan's columns plus, per matched event, utc_off (eventTime's UTC offset in minutes,
+    int16) and prop_off (int64 [n + 1]: its records), and per record r, one per top-level key of `properties` in object
+    order: the decoded key key_bytes[key_off[r]:key_off[r + 1]] and the raw JSON token of its value
+    tok_bytes[tok_off[r]:tok_off[r + 1]]."""
+    buf = np.frombuffer(text, np.uint8) if isinstance(text, (bytes, bytearray, memoryview)) else \
+        np.ascontiguousarray(text, np.uint8)
+    n = int(buf.shape[0])
+    f, keep = _events_filter(entity_type, event_names, target_mode, target_entity_type, None, start_us, until_us)
+    cap = n // EVENTS_MIN_EVENT_BYTES + 1
+    rcap = n // EVENTS_MIN_RECORD_BYTES + 1
+    out = dict(line=np.empty(cap, np.int64), code=np.empty(cap, np.int32), value=np.empty(cap, np.float64),
+               flags=np.empty(cap, np.uint8), time_us=np.empty(cap, np.int64), eid_bytes=np.empty(max(n, 1), np.uint8),
+               eid_off=np.empty(cap + 1, np.int64), tid_bytes=np.empty(max(n, 1), np.uint8),
+               tid_off=np.empty(cap + 1, np.int64), utc_off=np.empty(cap, np.int16), prop_off=np.empty(cap + 1, np.int64))
+    rec = dict(key_bytes=np.empty(max(n, 1), np.uint8), key_off=np.empty(rcap + 1, np.int64),
+               tok_bytes=np.empty(max(n, 1), np.uint8), tok_off=np.empty(rcap + 1, np.int64))
+    fb_cap = max(1024, n // 4096)
+    n_ev, n_rec, n_fb, n_lines = C.c_int64(0), C.c_int64(0), C.c_int64(0), C.c_int64(0)
+    while True:
+        fb = [np.empty(fb_cap, np.int64) for _ in range(3)]
+        rc = lib().pio_events_scan_props(
+            C.c_int(device), _ptr(buf, C.c_uint8) if n else None, C.c_int64(n), C.byref(f), C.c_int64(cap),
+            *[C.c_void_p(_addr(out[k])) for k in ("line", "code", "value", "flags", "time_us", "eid_bytes", "eid_off",
+                                                  "tid_bytes", "tid_off", "utc_off", "prop_off")],
+            C.c_int64(rcap), *[C.c_void_p(_addr(rec[k])) for k in ("key_bytes", "key_off", "tok_bytes", "tok_off")],
+            C.byref(n_ev), C.byref(n_rec), C.c_int64(fb_cap), *[_ptr(a, C.c_int64) for a in fb], C.byref(n_fb),
+            C.byref(n_lines))
+        if rc != 0:
+            raise NativeError(rc, lib().pio_als_last_error(None).decode())
+        if n_fb.value <= fb_cap:
+            break
+        fb_cap = n_fb.value     # more fallback lines than room: once more with room for all of them
+    m, nr = n_ev.value, n_rec.value
+    res = {k: out[k][:m] for k in ("line", "code", "value", "flags", "time_us", "utc_off")}
+    for k in ("eid", "tid"):
+        res[k + "_off"] = out[k + "_off"][:m + 1]
+        res[k + "_bytes"] = out[k + "_bytes"][:res[k + "_off"][-1]]
+    res["prop_off"] = out["prop_off"][:m + 1]
+    for k in ("key", "tok"):
+        res[k + "_off"] = rec[k + "_off"][:nr + 1]
+        res[k + "_bytes"] = rec[k + "_bytes"][:res[k + "_off"][-1]]
+    res["fb_line"], res["fb_begin"], res["fb_end"] = (a[:n_fb.value] for a in fb)
+    res["n_lines"] = n_lines.value
+    return res
+
+
+def events_fold_props(eid, code, time_us, prop_off, keys, device=0):
+    """pio_events_fold_props: LEventAggregator's fold of every key, over $set (code 0) / $unset (1) / $delete (2)
+    events in file order whose records (one per key of `properties`, object order) are prop_off[e]:prop_off[e + 1] of
+    keys = (bytes uint8[], offsets int64[n_records + 1]).  eid: (bytes, offsets).  Returns, per entity in order of first
+    occurrence: first_event, exists (bool), first_time_event / last_time_event (the events giving firstUpdated /
+    lastUpdated), win_off (int64 [n_entities + 1]) over win_rec (the record holding each key's value, in the map's
+    order) and win_key (its key code); and key_first (the first record of each key code)."""
+    buf, off = np.ascontiguousarray(eid[0], np.uint8), np.ascontiguousarray(eid[1], np.int64)
+    kbuf, koff = np.ascontiguousarray(keys[0], np.uint8), np.ascontiguousarray(keys[1], np.int64)
+    code = np.ascontiguousarray(code, np.int32)
+    time_us = np.ascontiguousarray(time_us, np.int64)
+    prop_off = np.ascontiguousarray(prop_off, np.int64)
+    n = int(code.shape[0])
+    nr = int(prop_off[-1]) if prop_off.size else 0
+    first, exists = np.empty(max(n, 1), np.int64), np.empty(max(n, 1), np.uint8)
+    fev, lev, woff = np.empty(max(n, 1), np.int64), np.empty(max(n, 1), np.int64), np.empty(n + 1, np.int64)
+    wrec, wkey, kfirst = np.empty(max(nr, 1), np.int64), np.empty(max(nr, 1), np.int32), np.empty(max(nr, 1), np.int64)
+    ne, nk = C.c_int64(0), C.c_int64(0)
+    rc = lib().pio_events_fold_props(
+        C.c_int(device), _ptr(buf, C.c_uint8) if buf.size else None, _ptr(off, C.c_int64), _ptr(code, C.c_int32),
+        _ptr(time_us, C.c_int64), _ptr(prop_off, C.c_int64), C.c_int64(n), _ptr(kbuf, C.c_uint8) if kbuf.size else None,
+        _ptr(koff, C.c_int64), _ptr(first, C.c_int64), _ptr(exists, C.c_uint8), _ptr(fev, C.c_int64),
+        _ptr(lev, C.c_int64), _ptr(woff, C.c_int64), _ptr(wrec, C.c_int64), _ptr(wkey, C.c_int32),
+        _ptr(kfirst, C.c_int64), C.byref(ne), C.byref(nk))
+    if rc != 0:
+        raise NativeError(rc, lib().pio_als_last_error(None).decode())
+    g = ne.value
+    w_off = woff[:g + 1] if g else np.zeros(1, np.int64)
+    nw = int(w_off[-1])
+    return dict(first_event=first[:g], exists=exists[:g].astype(bool), first_time_event=fev[:g],
+                last_time_event=lev[:g], win_off=w_off, win_rec=wrec[:nw], win_key=wkey[:nw], key_first=kfirst[:nk.value])
 
 
 def events_fold(eid, code, time_us, present=None, n_keys=0, device=0):

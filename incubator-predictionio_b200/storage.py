@@ -421,6 +421,18 @@ class PEventStore:
                                            chunk_bytes or FIND_COLUMNS_CHUNK)
 
     @staticmethod
+    def aggregatePropertyMaps(appName: str, entityType: str, channelName: Optional[str] = None, startTime=None,
+                              untilTime=None, required: Optional[Sequence[str]] = None, sc=None,
+                              chunk_bytes: int = None) -> List[Tuple[str, PropertyMap]]:
+        """What aggregateProperties returns -- the same entities in the same order, every key of each PropertyMap in
+        the same order with the same Python values, firstUpdated / lastUpdated with their UTC offsets -- computed on the
+        GPU: the $set / $unset / $delete events are scanned with every key of `properties` (native.events_scan_props)
+        and folded there (native.events_fold_props); the host decodes the winning values only.  Raises what
+        aggregateProperties raises on the first bad line.  Needs the CUDA library."""
+        return _aggregate_property_maps(appName, entityType, channelName, startTime, untilTime, required, sc,
+                                        chunk_bytes or FIND_COLUMNS_CHUNK)
+
+    @staticmethod
     def aggregateProperties(appName: str, entityType: str, channelName: Optional[str] = None, startTime=None,
                             untilTime=None, required: Optional[Sequence[str]] = None, sc=None
                             ) -> List[Tuple[str, PropertyMap]]:
@@ -790,6 +802,108 @@ def _aggregate_property_columns(appName, entityType, keys, required, startTime, 
         has_number[i, q], number[i, q] = _as_number(v)
     return PropertyColumns(keys, take_strings(*eid, f["first_event"][rows]), f["first_us"][rows], f["last_us"][rows],
                            present_k, has_number, number, (tb[keep_b], tok_off), host_value, len(host_lines))
+
+
+_LOCAL_EPOCH = _dt.datetime(1970, 1, 1)
+
+
+def _event_datetime(t_us: int, utc_off: int) -> _dt.datetime:
+    """The aware datetime _parse_time makes of an eventTime at t_us written with a UTC offset of utc_off minutes (built
+    from the local time, which is always in datetime's range)."""
+    local = _LOCAL_EPOCH + _dt.timedelta(microseconds=t_us + utc_off * 60_000_000)
+    return local.replace(tzinfo=_dt.timezone(_dt.timedelta(minutes=utc_off)))   # offset 0 is timezone.utc itself
+
+
+def _json_array(col: Tuple[np.ndarray, np.ndarray]) -> bytes:
+    """The JSON tokens of a string column as one JSON array, "[t0,t1,...]", built without a Python loop."""
+    buf, off = col
+    n = off.shape[0] - 1
+    out = np.full(int(off[-1]) + max(n, 1) + 1, ord(","), np.uint8)
+    out[0], out[-1] = ord("["), ord("]")
+    if n:
+        row = np.repeat(np.arange(n, dtype=np.int64), off[1:] - off[:-1])
+        out[np.arange(off[-1], dtype=np.int64) + row + 1] = buf
+    return out.tobytes()
+
+
+def _aggregate_property_maps(appName, entityType, channelName, startTime, untilTime, required, sc,
+                             chunk_bytes) -> List[Tuple[str, PropertyMap]]:
+    from . import native
+    s_us, u_us, device = _scan_args(startTime, untilTime, sc)
+    parts, host_lines = _scan_file(
+        appName, channelName,
+        lambda view: native.events_scan_props(view, entityType, FOLD_EVENTS, native.EVENTS_TARGET_ANY, None, s_us,
+                                              u_us, device),
+        chunk_bytes)
+    cat = lambda k, t: np.concatenate([r[k] for r in parts]).astype(t, copy=False) if parts else np.zeros(0, t)  # noqa: E731
+    d_line, d_code, d_time, d_utc = cat("line", np.int64), cat("code", np.int32), cat("time_us", np.int64), \
+        cat("utc_off", np.int16)
+    d_eid = concat_strings([(r["eid_bytes"], r["eid_off"]) for r in parts])
+    d_keys = concat_strings([(r["key_bytes"], r["key_off"]) for r in parts])
+    d_toks = concat_strings([(r["tok_bytes"], r["tok_off"]) for r in parts])
+    d_prop, base = [], 0
+    for r in parts:
+        d_prop.append(r["prop_off"][:-1] + base)
+        base += int(r["prop_off"][-1])
+    d_prop = np.concatenate(d_prop + [np.array([base], np.int64)])
+    nd, nrd = d_line.shape[0], base
+    # fallback lines: the code find runs, merged by line index; their keys become records whose values stay Python objects
+    enc = lambda x: x.encode("utf-8", "surrogatepass")  # noqa: E731
+    h_line, h_code, h_time, h_eid, h_dt, h_items = [], [], [], [], [], []
+    for ln, e in _host_events(host_lines, set(FOLD_EVENTS), entityType, _UNSET, startTime, untilTime):
+        h_line.append(ln)
+        h_code.append(FOLD_EVENTS.index(e.event))
+        h_time.append(time_us(e.eventTime))
+        h_eid.append(enc(e.entityId))
+        h_dt.append(e.eventTime)
+        h_items.append(list(e.properties.fields.items()))
+    h_vals = [v for items in h_items for _, v in items]
+    rec_perm = None   # the fold's records -> records of the scan (< nrd) and of the fallback lines (>= nrd)
+    if h_line:
+        col = lambda bs: (np.frombuffer(b"".join(bs), np.uint8).copy(),  # noqa: E731
+                          np.concatenate([[0], np.cumsum([len(b) for b in bs], dtype=np.int64)]).astype(np.int64))
+        h_cnt = np.array([len(items) for items in h_items], np.int64)
+        order = np.argsort(np.concatenate([d_line, np.array(h_line, np.int64)]), kind="stable")
+        code = np.concatenate([d_code, np.array(h_code, np.int32)])[order]
+        t_us = np.concatenate([d_time, np.array(h_time, np.int64)])[order]
+        eid = take_strings(*concat_strings([d_eid, col(h_eid)]), order)
+        start = np.concatenate([d_prop[:-1], nrd + np.cumsum(h_cnt) - h_cnt])[order]
+        lens = np.concatenate([np.diff(d_prop), h_cnt])[order]
+        prop_off = np.zeros(order.shape[0] + 1, np.int64)
+        np.cumsum(lens, out=prop_off[1:])
+        rec_perm = np.repeat(start - prop_off[:-1], lens) + np.arange(prop_off[-1], dtype=np.int64)
+        keys = take_strings(*concat_strings([d_keys, col([enc(k) for items in h_items for k, _ in items])]), rec_perm)
+    else:
+        order, code, t_us, eid, prop_off, keys = np.arange(nd), d_code, d_time, d_eid, d_prop, d_keys
+    f = native.events_fold_props(eid, code, t_us, prop_off, keys, device)
+
+    # the winning values: one json.loads of the scanned tokens, the fallback lines' values as they are
+    rec = f["win_rec"] if rec_perm is None else rec_perm[f["win_rec"]]
+    dev = rec < nrd
+    vals = json.loads(_json_array(take_strings(*d_toks, rec[dev]))) if nrd else []
+    if not dev.all():
+        it = iter(vals)
+        vals = [next(it) if d else h_vals[int(r) - nrd] for d, r in zip(dev.tolist(), rec.tolist())]
+    kraw, koff = keys[0].tobytes(), keys[1]
+    key_names = [kraw[koff[r]:koff[r + 1]].decode("utf-8", "surrogatepass") for r in f["key_first"].tolist()]
+    names = [key_names[c] for c in f["win_key"].tolist()]
+
+    def when(m):   # the datetime of event m of the fold
+        src = int(order[m])
+        return _event_datetime(int(d_time[src]), int(d_utc[src])) if src < nd else h_dt[src - nd]
+
+    rows = np.flatnonzero(f["exists"])
+    ids = string_list(take_strings(*eid, f["first_event"][rows]))
+    w_off = f["win_off"].tolist()
+    fev, lev = f["first_time_event"].tolist(), f["last_time_event"].tolist()
+    out = []
+    for k, g in zip(ids, rows.tolist()):
+        a, b = w_off[g], w_off[g + 1]
+        fields = dict(zip(names[a:b], vals[a:b]))
+        if required is not None and not all(r in fields for r in required):
+            continue
+        out.append((k, PropertyMap(fields, when(fev[g]), when(lev[g]))))
+    return out
 
 
 def event_millis(t_us) -> np.ndarray:
