@@ -592,21 +592,20 @@ static int build_side(pio_als_handle* h, Side& row, const Side& col, const int* 
   cudaStream_t st = h->stream;
   const int W = h->cfg.world_size, rk = h->cfg.world_rank;
   Scratch tmp(h->stream);
-  uint64_t *ka = nullptr, *kb = nullptr;
-  uint32_t *va = nullptr, *vb = nullptr;
-  CK(h, tmp.alloc(&ka, (size_t)nnz));
-  CK(h, tmp.alloc(&kb, (size_t)nnz));
-  CK(h, tmp.alloc(&va, (size_t)nnz));
-  CK(h, tmp.alloc(&vb, (size_t)nnz));
-  bool in_b = false;
+  SortBufs sb;
+  for (int i : {0, 1}) {
+    CK(h, tmp.alloc(&sb.k[i], (size_t)nnz));
+    CK(h, tmp.alloc(&sb.v[i], (size_t)nnz));
+  }
   if (nnz > 0) {
-    make_keys_int_kernel<<<nblk(nnz, 256), 256, 0, st>>>(rowext, colext, nnz, row.perm, col.rpos, col.bits, ka, va);
+    make_keys_int_kernel<<<nblk(nnz, 256), 256, 0, st>>>(rowext, colext, nnz, row.perm, col.rpos, col.bits, sb.keys(),
+                                                         sb.vals());
     LAUNCHED(h);
-    CK(h, radix_sort_pairs(ka, va, kb, vb, (size_t)nnz, row.bits + col.bits, st, &in_b, &h->st.kernel_launches));
+    CK(h, radix_sort_pairs(sb, (size_t)nnz, row.bits + col.bits, st, &h->st.kernel_launches));
   }
   tmark(h, "  side: keys + radix sort");
-  const uint64_t* ks = in_b ? kb : ka;
-  const uint32_t* vs = in_b ? vb : va;
+  const uint64_t* ks = sb.keys();
+  const uint32_t* vs = sb.vals();
   long long* ptr_full = nullptr;
   CK(h, tmp.alloc(&ptr_full, (size_t)row.n_internal + 1));
   CK(h, cudaMemsetAsync(ptr_full, 0, sizeof(long long) * ((size_t)row.n_internal + 1), st));
@@ -677,19 +676,17 @@ static int build_side(pio_als_handle* h, Side& row, const Side& col, const int* 
 static int rank_rows(pio_als_handle* h, Side& s) {
   cudaStream_t st = h->stream;
   Scratch tmp(h->stream);
-  uint64_t *ka = nullptr, *kb = nullptr;
-  uint32_t *va = nullptr, *vb = nullptr;
-  CK(h, tmp.alloc(&ka, (size_t)s.n));
-  CK(h, tmp.alloc(&kb, (size_t)s.n));
-  CK(h, tmp.alloc(&va, (size_t)s.n));
-  CK(h, tmp.alloc(&vb, (size_t)s.n));
-  degree_keys_kernel<<<nblk(s.n, 256), 256, 0, st>>>(s.deg, s.n, ka, va);
+  SortBufs sb;
+  for (int i : {0, 1}) {
+    CK(h, tmp.alloc(&sb.k[i], (size_t)s.n));
+    CK(h, tmp.alloc(&sb.v[i], (size_t)s.n));
+  }
+  degree_keys_kernel<<<nblk(s.n, 256), 256, 0, st>>>(s.deg, s.n, sb.keys(), sb.vals());
   LAUNCHED(h);
-  bool in_b = false;
-  CK(h, radix_sort_pairs(ka, va, kb, vb, (size_t)s.n, 32, st, &in_b, &h->st.kernel_launches));
+  CK(h, radix_sort_pairs(sb, (size_t)s.n, 32, st, &h->st.kernel_launches));
   fill_int_kernel<<<nblk(s.n_internal, 256), 256, 0, st>>>(s.inv, s.n_internal, -1);
   LAUNCHED(h);
-  assign_internal_kernel<<<nblk(s.n, 256), 256, 0, st>>>(in_b ? vb : va, s.n, h->cfg.world_size, s.R, s.perm, s.inv,
+  assign_internal_kernel<<<nblk(s.n, 256), 256, 0, st>>>(sb.vals(), s.n, h->cfg.world_size, s.R, s.perm, s.inv,
                                                          s.rpos, s.p2i);
   LAUNCHED(h);
   return PIO_ALS_OK;
@@ -697,23 +694,22 @@ static int rank_rows(pio_als_handle* h, Side& s) {
 
 // ---- sharded ingest: all-to-all exchange of event arrays ------------------------------------------------------------
 // The n events on this rank go to the ranks named by the sort keys (destination rank, payload = event index; built by the
-// caller in ka/va).  Events keep their order per destination and arrive concatenated in source-rank order, so a global
-// event order (rank r's slice precedes rank r + 1's) survives.  The received arrays are allocated in `keep`.
+// caller in sb's live half).  Events keep their order per destination and arrive concatenated in source-rank order, so a
+// global event order (rank r's slice precedes rank r + 1's) survives.  The received arrays are allocated in `keep`.
 struct XArr {
   const void* in;
   void** out;
   size_t elem;
 };
-static int exchange_events(pio_als_handle* h, Scratch& keep, uint64_t* ka, uint32_t* va, uint64_t* kb, uint32_t* vb,
-                           long long n, XArr* arrs, int na, long long* n_out) {
+static int exchange_events(pio_als_handle* h, Scratch& keep, SortBufs& sb, long long n, XArr* arrs, int na,
+                           long long* n_out) {
   cudaStream_t st = h->stream;
   NcclApi& nc = nccl_api();
   const int W = h->cfg.world_size, me = h->cfg.world_rank;
   Scratch tmp(h->stream);
-  bool in_b = false;
-  if (n > 0) CK(h, radix_sort_pairs(ka, va, kb, vb, (size_t)n, ceil_log2((uint64_t)W), st, &in_b, &h->st.kernel_launches));
-  const uint64_t* ks = in_b ? kb : ka;
-  const uint32_t* vs = in_b ? vb : va;
+  if (n > 0) CK(h, radix_sort_pairs(sb, (size_t)n, ceil_log2((uint64_t)W), st, &h->st.kernel_launches));
+  const uint64_t* ks = sb.keys();
+  const uint32_t* vs = sb.vals();
   long long *d_off = nullptr, *d_cnt = nullptr, *d_all = nullptr;
   CK(h, tmp.alloc(&d_off, (size_t)W + 1));
   CK(h, tmp.alloc(&d_cnt, (size_t)W));
@@ -821,18 +817,19 @@ static int ingest_device(pio_als_handle* h, const int* d_user, const int* d_item
   long long ns = nnz;
   if (sharded && dedup != PIO_ALS_DEDUP_NONE) {
     Scratch xs(h->stream);
-    uint64_t *ka = nullptr, *kb = nullptr;
-    uint32_t *va = nullptr, *vb = nullptr;
-    CK(h, xs.alloc(&ka, (size_t)nnz)); CK(h, xs.alloc(&kb, (size_t)nnz));
-    CK(h, xs.alloc(&va, (size_t)nnz)); CK(h, xs.alloc(&vb, (size_t)nnz));
+    SortBufs sb;
+    for (int i : {0, 1}) {
+      CK(h, xs.alloc(&sb.k[i], (size_t)nnz));
+      CK(h, xs.alloc(&sb.v[i], (size_t)nnz));
+    }
     if (nnz > 0) {
-      dest_mod_kernel<<<nblk(nnz, 256), 256, 0, st>>>(d_user, nnz, W, ka, va);
+      dest_mod_kernel<<<nblk(nnz, 256), 256, 0, st>>>(d_user, nnz, W, sb.keys(), sb.vals());
       LAUNCHED(h);
     }
     void *xu = nullptr, *xi = nullptr, *xr = nullptr, *xt = nullptr;
     XArr arrs[4] = {{d_user, &xu, 4}, {d_item, &xi, 4}, {d_rating, &xr, 4},
                     {dedup == PIO_ALS_DEDUP_KEEP_LAST ? (const void*)d_ts : nullptr, &xt, 8}};
-    int rc = exchange_events(h, tmp, ka, va, kb, vb, nnz, arrs, 4, &ns);
+    int rc = exchange_events(h, tmp, sb, nnz, arrs, 4, &ns);
     if (rc) return rc;
     su = (const int*)xu; si = (const int*)xi; sr = (const float*)xr; sts = (const long long*)xt;
   }
@@ -845,17 +842,17 @@ static int ingest_device(pio_als_handle* h, const int* d_user, const int* d_item
   long long n2 = ns;
   if (dedup != PIO_ALS_DEDUP_NONE && ns > 0) {
     Scratch ds(h->stream);
-    uint64_t *ka = nullptr, *kb = nullptr;
-    uint32_t *va = nullptr, *vb = nullptr;
-    CK(h, ds.alloc(&ka, (size_t)ns)); CK(h, ds.alloc(&kb, (size_t)ns));
-    CK(h, ds.alloc(&va, (size_t)ns)); CK(h, ds.alloc(&vb, (size_t)ns));
+    SortBufs sb;
+    for (int i : {0, 1}) {
+      CK(h, ds.alloc(&sb.k[i], (size_t)ns));
+      CK(h, ds.alloc(&sb.v[i], (size_t)ns));
+    }
     const int bu = ceil_log2((uint64_t)U.n), bi = ceil_log2((uint64_t)I.n);
-    make_keys_ext_kernel<<<nblk(ns, 256), 256, 0, st>>>(su, si, ns, bi, ka, va);
+    make_keys_ext_kernel<<<nblk(ns, 256), 256, 0, st>>>(su, si, ns, bi, sb.keys(), sb.vals());
     LAUNCHED(h);
-    bool in_b = false;
-    CK(h, radix_sort_pairs(ka, va, kb, vb, (size_t)ns, bu + bi, st, &in_b, &h->st.kernel_launches));
-    const uint64_t* ks = in_b ? kb : ka;
-    const uint32_t* vs = in_b ? vb : va;
+    CK(h, radix_sort_pairs(sb, (size_t)ns, bu + bi, st, &h->st.kernel_launches));
+    const uint64_t* ks = sb.keys();
+    const uint32_t* vs = sb.vals();
     uint32_t* flag = nullptr;
     CK(h, ds.alloc(&flag, (size_t)ns));
     head_flags_kernel<<<nblk(ns, 256), 256, 0, st>>>(ks, ns, flag);
@@ -943,18 +940,19 @@ static int ingest_device(pio_als_handle* h, const int* d_user, const int* d_item
     struct { Side* row; Side* col; const int* rowext; const int* colext; } jobs[2] = {{&U, &I, cu, ci}, {&I, &U, ci, cu}};
     for (auto& j : jobs) {
       Scratch xs(h->stream), recv(h->stream);
-      uint64_t *ka = nullptr, *kb = nullptr;
-      uint32_t *va = nullptr, *vb = nullptr;
-      CK(h, xs.alloc(&ka, (size_t)n2)); CK(h, xs.alloc(&kb, (size_t)n2));
-      CK(h, xs.alloc(&va, (size_t)n2)); CK(h, xs.alloc(&vb, (size_t)n2));
+      SortBufs sb;
+      for (int i : {0, 1}) {
+        CK(h, xs.alloc(&sb.k[i], (size_t)n2));
+        CK(h, xs.alloc(&sb.v[i], (size_t)n2));
+      }
       if (n2 > 0) {
-        dest_owner_kernel<<<nblk(n2, 256), 256, 0, st>>>(j.rowext, n2, j.row->perm, j.row->R, ka, va);
+        dest_owner_kernel<<<nblk(n2, 256), 256, 0, st>>>(j.rowext, n2, j.row->perm, j.row->R, sb.keys(), sb.vals());
         LAUNCHED(h);
       }
       void *xrow = nullptr, *xcol = nullptr, *xr = nullptr;
       XArr arrs[3] = {{j.rowext, &xrow, 4}, {j.colext, &xcol, 4}, {cr, &xr, 4}};
       long long ne = 0;
-      rc = exchange_events(h, recv, ka, va, kb, vb, n2, arrs, 3, &ne);
+      rc = exchange_events(h, recv, sb, n2, arrs, 3, &ne);
       if (rc) return rc;
       mark("exchange by row owner");
       rc = build_side(h, *j.row, *j.col, (const int*)xrow, (const int*)xcol, (const float*)xr, ne, n2_global);
@@ -2618,17 +2616,17 @@ int pio_als_synth_ratings_device(int device, int32_t n_users, int32_t n_items, i
 // the first occurrence of id; *n_unique.  0 < n < 2^32.
 static int ids_encode_device(const uint8_t* d_bytes, const long long* d_off, int64_t n, cudaStream_t st, int* d_index,
                              long long* d_first, int64_t* n_unique) {
-  uint64_t *ka = nullptr, *kb = nullptr;
-  uint32_t *va = nullptr, *vb = nullptr, *f1 = nullptr, *f2 = nullptr, *run_start = nullptr, *head = nullptr, *ishead = nullptr,
-           *firstpos = nullptr, *isfirst = nullptr;
+  SortBufs sb;
+  uint32_t *f1 = nullptr, *f2 = nullptr, *run_start = nullptr, *head = nullptr, *ishead = nullptr, *firstpos = nullptr,
+           *isfirst = nullptr;
   CallMem tmp(st);
-  for (uint64_t** p : {&ka, &kb}) CK0(tmp.device(p, (size_t)n));
-  for (uint32_t** p : {&va, &vb, &f1, &f2, &run_start, &head, &ishead, &firstpos, &isfirst}) CK0(tmp.device(p, (size_t)n));
-  ids_hash_kernel<<<nblk(n, 256), 256, 0, st>>>(d_bytes, d_off, n, ka, va, ids_hash_mask());
-  bool in_b = false;
-  CK0(radix_sort_pairs(ka, va, kb, vb, (size_t)n, 64, st, &in_b, nullptr));
-  const uint64_t* ks = in_b ? kb : ka;
-  const uint32_t* vs = in_b ? vb : va;
+  for (uint64_t** p : {&sb.k[0], &sb.k[1]}) CK0(tmp.device(p, (size_t)n));
+  for (uint32_t** p : {&sb.v[0], &sb.v[1], &f1, &f2, &run_start, &head, &ishead, &firstpos, &isfirst})
+    CK0(tmp.device(p, (size_t)n));
+  ids_hash_kernel<<<nblk(n, 256), 256, 0, st>>>(d_bytes, d_off, n, sb.keys(), sb.vals(), ids_hash_mask());
+  CK0(radix_sort_pairs(sb, (size_t)n, 64, st, nullptr));
+  const uint64_t* ks = sb.keys();
+  const uint32_t* vs = sb.vals();
   ids_runflag_kernel<<<nblk(n, 256), 256, 0, st>>>(ks, n, f1);
   CK0(scan_exclusive_u32(f1, f1, (size_t)n, st, nullptr));                 // f1 = run ids
   ids_runstart_kernel<<<nblk(n, 256), 256, 0, st>>>(ks, f1, n, run_start);
@@ -2647,6 +2645,22 @@ static int ids_encode_device(const uint8_t* d_bytes, const long long* d_off, int
   return PIO_ALS_OK;
 }
 
+// ids_encode_device over the host string column (bytes, offsets[0..n]), uploaded on st: *d_index and, when d_first is
+// not null, *d_first (n entries each) are allocated in tmp.  0 < n < 2^32, offsets[0] == 0.
+static int ids_encode_host(CallMem& tmp, cudaStream_t st, const uint8_t* bytes, const int64_t* offsets, int64_t n,
+                           int** d_index, long long** d_first, int64_t* n_unique) {
+  const size_t nb = (size_t)offsets[n];
+  uint8_t* d_bytes = nullptr;
+  long long* d_off = nullptr;
+  CK0(tmp.device(&d_bytes, nb));
+  CK0(tmp.device(&d_off, (size_t)n + 1));
+  CK0(tmp.device(d_index, (size_t)n));
+  if (d_first) CK0(tmp.device(d_first, (size_t)n));
+  CK0(cudaMemcpyAsync(d_bytes, bytes, nb, cudaMemcpyHostToDevice, st));
+  CK0(cudaMemcpyAsync(d_off, offsets, sizeof(long long) * ((size_t)n + 1), cudaMemcpyHostToDevice, st));
+  return ids_encode_device(d_bytes, d_off, n, st, *d_index, d_first ? *d_first : nullptr, n_unique);
+}
+
 int pio_ids_encode(int device, const uint8_t* bytes, const int64_t* offsets, int64_t n, int32_t* out_index,
                    int64_t* out_first, int32_t* out_n_unique) {
   if (n < 0 || !offsets || !out_index || !out_n_unique || (n > 0 && !bytes && offsets[n] > offsets[0]))
@@ -2656,20 +2670,12 @@ int pio_ids_encode(int device, const uint8_t* bytes, const int64_t* offsets, int
   if (n >= (1ll << 32)) return fail(nullptr, PIO_ALS_ERR_ARG, "n must be < 2^32");
   if (offsets[0] != 0) return fail(nullptr, PIO_ALS_ERR_ARG, "offsets[0] must be 0");
   CK0(cudaSetDevice(device));
-  const size_t nb = (size_t)offsets[n];
-  uint8_t* d_bytes = nullptr;
-  long long *d_off = nullptr, *d_first = nullptr;
+  long long* d_first = nullptr;
   int* d_out = nullptr;
   cudaStream_t st = 0;
   CallMem tmp(st);
-  CK0(tmp.device(&d_bytes, nb));
-  CK0(tmp.device(&d_off, (size_t)n + 1));
-  CK0(tmp.device(&d_out, (size_t)n));
-  CK0(tmp.device(&d_first, (size_t)n));
-  CK0(cudaMemcpyAsync(d_bytes, bytes, nb, cudaMemcpyHostToDevice, st));
-  CK0(cudaMemcpyAsync(d_off, offsets, sizeof(long long) * (n + 1), cudaMemcpyHostToDevice, st));
   int64_t nuniq = 0;
-  const int rc = ids_encode_device(d_bytes, d_off, n, st, d_out, out_first ? d_first : nullptr, &nuniq);
+  const int rc = ids_encode_host(tmp, st, bytes, offsets, n, &d_out, out_first ? &d_first : nullptr, &nuniq);
   if (rc != PIO_ALS_OK) return rc;
   CK0(cudaMemcpy(out_index, d_out, 4 * (size_t)n, cudaMemcpyDeviceToHost));
   if (out_first) CK0(cudaMemcpy(out_first, d_first, 8 * (size_t)nuniq, cudaMemcpyDeviceToHost));
@@ -3299,6 +3305,65 @@ int pio_events_scan_props(int device, const uint8_t* text, int64_t n_bytes, cons
 }
 
 // ---- $set / $unset / $delete fold (PEventStore.aggregatePropertyColumns; events_fold.cuh) -----------------------------
+// PIO_ALS_OK, or the error both folds report for code[e] outside $set / $unset / $delete
+static int fold_check_code(const int32_t* code, int64_t e) {
+  if (code[e] >= FOLD_SET && code[e] <= FOLD_DELETE) return PIO_ALS_OK;
+  return fail(nullptr, PIO_ALS_ERR_ARG, "code[%lld] = %d is not 0 ($set), 1 ($unset) or 2 ($delete)", (long long)e,
+              code[e]);
+}
+
+// What both folds do before they diverge, for n > 0 checked events: upload them, number their entities, order them by
+// (entity, time, line) and reduce that order per entity (fold_reduce_kernel). Device arrays are owned by the caller's
+// CallMem.
+struct FoldOrder {
+  int32_t* code = nullptr;      // [n]
+  long long* time = nullptr;    // [n] eventTime, us
+  int* ent = nullptr;           // [n] entity of each event, numbered in order of first occurrence
+  long long* first = nullptr;   // [n_ent] first event of each entity
+  int64_t n_ent = 0;
+  SortBufs sorted;              // live half: entity keys and event indices in (entity, time, line) order
+  int *seg_first = nullptr, *seg_last = nullptr, *last_set = nullptr, *last_del = nullptr;   // [n_ent], see the kernel
+  int* win = nullptr;           // [n_ent x n_keys] last toucher of each tracked key; null when n_keys == 0
+};
+
+static int fold_order(CallMem& tmp, cudaStream_t st, const uint8_t* eid_bytes, const int64_t* eid_off,
+                      const int32_t* code, const int64_t* time_us, const uint8_t* present, int64_t n, int n_keys,
+                      FoldOrder* o) {
+  const size_t nn = (size_t)n, nk = (size_t)n_keys;
+  uint8_t* d_present = nullptr;
+  CK0(tmp.device(&o->code, nn));
+  CK0(tmp.device(&o->time, nn));
+  for (int i : {0, 1}) {
+    CK0(tmp.device(&o->sorted.k[i], nn));
+    CK0(tmp.device(&o->sorted.v[i], nn));
+  }
+  CK0(cudaMemcpyAsync(o->code, code, 4 * nn, cudaMemcpyHostToDevice, st));
+  CK0(cudaMemcpyAsync(o->time, time_us, 8 * nn, cudaMemcpyHostToDevice, st));
+  if (nk) {
+    CK0(tmp.device(&d_present, nn));
+    CK0(cudaMemcpyAsync(d_present, present, nn, cudaMemcpyHostToDevice, st));
+  }
+  const int rc = ids_encode_host(tmp, st, eid_bytes, eid_off, n, &o->ent, &o->first, &o->n_ent);
+  if (rc != PIO_ALS_OK) return rc;
+  const size_t ne = (size_t)o->n_ent;
+  for (int** p : {&o->seg_first, &o->seg_last, &o->last_set, &o->last_del}) CK0(tmp.device(p, ne));
+  CK0(cudaMemsetAsync(o->last_set, 0xFF, 4 * ne, st));   // -1: none
+  CK0(cudaMemsetAsync(o->last_del, 0xFF, 4 * ne, st));
+  if (nk) {
+    CK0(tmp.device(&o->win, ne * nk));
+    CK0(cudaMemsetAsync(o->win, 0xFF, 4 * ne * nk, st));
+  }
+  // stable by time, then stable by entity
+  SortBufs& s = o->sorted;
+  fold_time_key_kernel<<<nblk(n, 256), 256, 0, st>>>(o->time, n, s.keys(), s.vals());
+  CK0(radix_sort_pairs(s, nn, 64, st, nullptr));
+  fold_entity_key_kernel<<<nblk(n, 256), 256, 0, st>>>(s.vals(), o->ent, n, s.keys());
+  CK0(radix_sort_pairs(s, nn, ceil_log2((uint64_t)o->n_ent), st, nullptr));
+  fold_reduce_kernel<<<nblk(n, 256), 256, 0, st>>>(s.keys(), s.vals(), o->code, d_present, n_keys, n, o->seg_first,
+                                                   o->seg_last, o->last_set, o->last_del, o->win);
+  return PIO_ALS_OK;
+}
+
 int pio_events_fold(int device, const uint8_t* eid_bytes, const int64_t* eid_off, const int32_t* code,
                     const int64_t* time_us, const uint8_t* present, int64_t n, int n_keys, int64_t* out_first_event,
                     uint8_t* out_exists, int64_t* out_first_us, int64_t* out_last_us, int64_t* out_winner,
@@ -3312,70 +3377,30 @@ int pio_events_fold(int device, const uint8_t* eid_bytes, const int64_t* eid_off
   if (n >= (1ll << 31)) return fail(nullptr, PIO_ALS_ERR_ARG, "n must be < 2^31");
   if (eid_off[0] != 0) return fail(nullptr, PIO_ALS_ERR_ARG, "eid_off[0] must be 0");
   for (int64_t e = 0; e < n; ++e)
-    if (code[e] < FOLD_SET || code[e] > FOLD_DELETE)
-      return fail(nullptr, PIO_ALS_ERR_ARG, "code[%lld] = %d is not 0 ($set), 1 ($unset) or 2 ($delete)", (long long)e,
-                  code[e]);
+    if (const int rc = fold_check_code(code, e)) return rc;
   CK0(cudaSetDevice(device));
-  const size_t nb = (size_t)eid_off[n], nn = (size_t)n, nk = (size_t)n_keys;
   cudaStream_t st = 0;
   CallMem tmp(st);
-  uint8_t *d_bytes = nullptr, *d_present = nullptr, *d_exists = nullptr;
-  long long *d_off = nullptr, *d_time = nullptr, *d_first = nullptr, *d_fus = nullptr, *d_lus = nullptr, *d_win = nullptr;
-  int32_t* d_code = nullptr;
-  int *d_ent = nullptr, *seg_first = nullptr, *seg_last = nullptr, *last_set = nullptr, *last_del = nullptr, *win = nullptr;
-  uint64_t *ka = nullptr, *kb = nullptr;
-  uint32_t *va = nullptr, *vb = nullptr;
-  CK0(tmp.device(&d_bytes, nb));
-  CK0(tmp.device(&d_off, nn + 1));
-  CK0(tmp.device(&d_code, nn));
-  CK0(tmp.device(&d_time, nn));
-  CK0(tmp.device(&d_present, nn));
-  CK0(tmp.device(&d_ent, nn));
-  CK0(tmp.device(&d_first, nn));
-  CK0(tmp.device(&ka, nn)); CK0(tmp.device(&kb, nn));
-  CK0(tmp.device(&va, nn)); CK0(tmp.device(&vb, nn));
-  CK0(cudaMemcpyAsync(d_bytes, eid_bytes, nb, cudaMemcpyHostToDevice, st));
-  CK0(cudaMemcpyAsync(d_off, eid_off, 8 * (nn + 1), cudaMemcpyHostToDevice, st));
-  CK0(cudaMemcpyAsync(d_code, code, 4 * nn, cudaMemcpyHostToDevice, st));
-  CK0(cudaMemcpyAsync(d_time, time_us, 8 * nn, cudaMemcpyHostToDevice, st));
-  if (n_keys) CK0(cudaMemcpyAsync(d_present, present, nn, cudaMemcpyHostToDevice, st));
-  int64_t n_ent = 0;
-  const int rc = ids_encode_device(d_bytes, d_off, n, st, d_ent, d_first, &n_ent);
+  FoldOrder o;
+  const int rc = fold_order(tmp, st, eid_bytes, eid_off, code, time_us, present, n, n_keys, &o);
   if (rc != PIO_ALS_OK) return rc;
-  const size_t ne = (size_t)n_ent;
-  CK0(tmp.device(&seg_first, ne)); CK0(tmp.device(&seg_last, ne));
-  CK0(tmp.device(&last_set, ne)); CK0(tmp.device(&last_del, ne));
-  CK0(tmp.device(&win, ne * nk));
+  const size_t ne = (size_t)o.n_ent, nk = (size_t)n_keys;
+  uint8_t* d_exists = nullptr;
+  long long *d_fus = nullptr, *d_lus = nullptr, *d_win = nullptr;
   CK0(tmp.device(&d_exists, ne));
   CK0(tmp.device(&d_fus, ne)); CK0(tmp.device(&d_lus, ne));
   CK0(tmp.device(&d_win, ne * nk));
-  CK0(cudaMemsetAsync(last_set, 0xFF, 4 * ne, st));   // -1: none
-  CK0(cudaMemsetAsync(last_del, 0xFF, 4 * ne, st));
-  if (nk) CK0(cudaMemsetAsync(win, 0xFF, 4 * ne * nk, st));
-  // (entity, time, line): stable by time, then stable by entity
-  fold_time_key_kernel<<<nblk(n, 256), 256, 0, st>>>(d_time, n, ka, va);
-  bool in_b = false;
-  CK0(radix_sort_pairs(ka, va, kb, vb, nn, 64, st, &in_b, nullptr));
-  uint64_t* k1 = in_b ? kb : ka;   // sorted by time; the other pair is free
-  uint32_t* v1 = in_b ? vb : va;
-  uint64_t* k2 = in_b ? ka : kb;
-  uint32_t* v2 = in_b ? va : vb;
-  fold_entity_key_kernel<<<nblk(n, 256), 256, 0, st>>>(v1, d_ent, n, k1);
-  CK0(radix_sort_pairs(k1, v1, k2, v2, nn, ceil_log2((uint64_t)n_ent), st, &in_b, nullptr));
-  const uint64_t* ks = in_b ? k2 : k1;
-  const uint32_t* vs = in_b ? v2 : v1;
-  fold_reduce_kernel<<<nblk(n, 256), 256, 0, st>>>(ks, vs, d_code, d_present, n_keys, n, seg_first, seg_last, last_set,
-                                                   last_del, win);
-  fold_finish_kernel<<<nblk(n_ent, 256), 256, 0, st>>>(vs, d_code, d_time, seg_first, seg_last, last_set, last_del, win,
-                                                       n_keys, n_ent, d_exists, d_fus, d_lus, d_win);
+  fold_finish_kernel<<<nblk(o.n_ent, 256), 256, 0, st>>>(o.sorted.vals(), o.code, o.time, o.seg_first, o.seg_last,
+                                                         o.last_set, o.last_del, o.win, n_keys, o.n_ent, d_exists,
+                                                         d_fus, d_lus, d_win);
   CK0(cudaGetLastError());
-  CK0(cudaMemcpyAsync(out_first_event, d_first, 8 * ne, cudaMemcpyDeviceToHost, st));
+  CK0(cudaMemcpyAsync(out_first_event, o.first, 8 * ne, cudaMemcpyDeviceToHost, st));
   CK0(cudaMemcpyAsync(out_exists, d_exists, ne, cudaMemcpyDeviceToHost, st));
   CK0(cudaMemcpyAsync(out_first_us, d_fus, 8 * ne, cudaMemcpyDeviceToHost, st));
   CK0(cudaMemcpyAsync(out_last_us, d_lus, 8 * ne, cudaMemcpyDeviceToHost, st));
   if (nk) CK0(cudaMemcpyAsync(out_winner, d_win, 8 * ne * nk, cudaMemcpyDeviceToHost, st));
   CK0(cudaStreamSynchronize(st));
-  *out_n_entities = n_ent;
+  *out_n_entities = o.n_ent;
   return PIO_ALS_OK;
 }
 
@@ -3396,9 +3421,7 @@ int pio_events_fold_props(int device, const uint8_t* eid_bytes, const int64_t* e
   if (eid_off[0] != 0 || prop_off[0] != 0) return fail(nullptr, PIO_ALS_ERR_ARG, "eid_off[0] and prop_off[0] must be 0");
   int64_t max_keys = 0;   // records of the largest event: the bits of an index in one object
   for (int64_t e = 0; e < n; ++e) {
-    if (code[e] < FOLD_SET || code[e] > FOLD_DELETE)
-      return fail(nullptr, PIO_ALS_ERR_ARG, "code[%lld] = %d is not 0 ($set), 1 ($unset) or 2 ($delete)", (long long)e,
-                  code[e]);
+    if (const int rc = fold_check_code(code, e)) return rc;
     if (prop_off[e + 1] < prop_off[e]) return fail(nullptr, PIO_ALS_ERR_ARG, "prop_off must not decrease");
     max_keys = std::max(max_keys, prop_off[e + 1] - prop_off[e]);
   }
@@ -3408,58 +3431,27 @@ int pio_events_fold_props(int device, const uint8_t* eid_bytes, const int64_t* e
                  (!key_bytes && key_off[nr] > 0)))
     return fail(nullptr, PIO_ALS_ERR_ARG, "bad pio_events_fold_props record arguments");
   CK0(cudaSetDevice(device));
-  const size_t nb = (size_t)eid_off[n], nn = (size_t)n;
+  const size_t nn = (size_t)n;
   cudaStream_t st = 0;
   CallMem tmp(st);
-  uint8_t *d_bytes = nullptr, *d_exists = nullptr;
-  long long *d_off = nullptr, *d_time = nullptr, *d_first = nullptr, *d_fev = nullptr, *d_lev = nullptr,
-            *d_woff = nullptr, *d_prop = nullptr;
-  int32_t* d_code = nullptr;
-  int *d_ent = nullptr, *seg_first = nullptr, *seg_last = nullptr, *last_set = nullptr, *last_del = nullptr,
-      *last_time = nullptr;
-  uint64_t *ka = nullptr, *kb = nullptr;
-  uint32_t *va = nullptr, *vb = nullptr, *rank = nullptr;
-  CK0(tmp.device(&d_bytes, nb));
-  CK0(tmp.device(&d_off, nn + 1));
-  CK0(tmp.device(&d_code, nn));
-  CK0(tmp.device(&d_time, nn));
+  uint8_t* d_exists = nullptr;
+  long long *d_fev = nullptr, *d_lev = nullptr, *d_woff = nullptr, *d_prop = nullptr;
+  int* last_time = nullptr;
+  uint32_t* rank = nullptr;
   CK0(tmp.device(&d_prop, nn + 1));
-  CK0(tmp.device(&d_ent, nn));
-  CK0(tmp.device(&d_first, nn));
   CK0(tmp.device(&rank, nn));
-  CK0(tmp.device(&ka, nn)); CK0(tmp.device(&kb, nn));
-  CK0(tmp.device(&va, nn)); CK0(tmp.device(&vb, nn));
-  CK0(cudaMemcpyAsync(d_bytes, eid_bytes, nb, cudaMemcpyHostToDevice, st));
-  CK0(cudaMemcpyAsync(d_off, eid_off, 8 * (nn + 1), cudaMemcpyHostToDevice, st));
-  CK0(cudaMemcpyAsync(d_code, code, 4 * nn, cudaMemcpyHostToDevice, st));
-  CK0(cudaMemcpyAsync(d_time, time_us, 8 * nn, cudaMemcpyHostToDevice, st));
   CK0(cudaMemcpyAsync(d_prop, prop_off, 8 * (nn + 1), cudaMemcpyHostToDevice, st));
-  int64_t n_ent = 0;
-  int rc = ids_encode_device(d_bytes, d_off, n, st, d_ent, d_first, &n_ent);
+  FoldOrder o;
+  int rc = fold_order(tmp, st, eid_bytes, eid_off, code, time_us, nullptr, n, 0, &o);
   if (rc != PIO_ALS_OK) return rc;
+  const int64_t n_ent = o.n_ent;
   const size_t ne = (size_t)n_ent;
-  CK0(tmp.device(&seg_first, ne)); CK0(tmp.device(&seg_last, ne));
-  CK0(tmp.device(&last_set, ne)); CK0(tmp.device(&last_del, ne)); CK0(tmp.device(&last_time, ne));
+  CK0(tmp.device(&last_time, ne));
   CK0(tmp.device(&d_exists, ne));
   CK0(tmp.device(&d_fev, ne)); CK0(tmp.device(&d_lev, ne));
   CK0(tmp.device(&d_woff, ne + 1));
-  CK0(cudaMemsetAsync(last_set, 0xFF, 4 * ne, st));   // -1: none
-  CK0(cudaMemsetAsync(last_del, 0xFF, 4 * ne, st));
-  // (entity, time, line), as pio_events_fold
-  fold_time_key_kernel<<<nblk(n, 256), 256, 0, st>>>(d_time, n, ka, va);
-  bool in_b = false;
-  CK0(radix_sort_pairs(ka, va, kb, vb, nn, 64, st, &in_b, nullptr));
-  uint64_t* k1 = in_b ? kb : ka;
-  uint32_t* v1 = in_b ? vb : va;
-  uint64_t* k2 = in_b ? ka : kb;
-  uint32_t* v2 = in_b ? va : vb;
-  fold_entity_key_kernel<<<nblk(n, 256), 256, 0, st>>>(v1, d_ent, n, k1);
-  CK0(radix_sort_pairs(k1, v1, k2, v2, nn, ceil_log2((uint64_t)n_ent), st, &in_b, nullptr));
-  const uint64_t* ks = in_b ? k2 : k1;
-  const uint32_t* vs = in_b ? v2 : v1;
-  fold_reduce_kernel<<<nblk(n, 256), 256, 0, st>>>(ks, vs, d_code, nullptr, 0, n, seg_first, seg_last, last_set,
-                                                   last_del, nullptr);
-  fold_last_time_kernel<<<nblk(n, 256), 256, 0, st>>>(ks, vs, d_time, seg_last, n, last_time);
+  const uint32_t* vs = o.sorted.vals();
+  fold_last_time_kernel<<<nblk(n, 256), 256, 0, st>>>(o.sorted.keys(), vs, o.time, o.seg_last, n, last_time);
   fold_rank_kernel<<<nblk(n, 256), 256, 0, st>>>(vs, n, rank);
   CK0(cudaGetLastError());
 
@@ -3469,36 +3461,27 @@ int pio_events_fold_props(int device, const uint8_t* eid_bytes, const int64_t* e
   int64_t n_kc = 0, nw = 0;
   if (nr > 0) {
     const size_t nrs = (size_t)nr;
-    uint8_t* d_kbytes = nullptr;
-    long long *d_koff = nullptr, *d_kfirst = nullptr, *d_wrec = nullptr;
+    long long *d_kfirst = nullptr, *d_wrec = nullptr;
     int *kcode = nullptr, *seg_unset = nullptr, *seg_set = nullptr, *seg_place = nullptr, *d_wkey = nullptr;
-    uint64_t *ra = nullptr, *rb = nullptr;
-    uint32_t *rva = nullptr, *rvb = nullptr, *rec_ev = nullptr, *head = nullptr, *seg_id = nullptr;
-    CK0(tmp.device(&d_kbytes, (size_t)key_off[nr]));
-    CK0(tmp.device(&d_koff, nrs + 1));
-    CK0(tmp.device(&kcode, nrs));
-    CK0(tmp.device(&d_kfirst, nrs));
+    uint32_t *rec_ev = nullptr, *head = nullptr, *seg_id = nullptr;
+    SortBufs r;
     CK0(tmp.device(&rec_ev, nrs));
     CK0(tmp.device(&head, nrs)); CK0(tmp.device(&seg_id, nrs));
-    CK0(tmp.device(&ra, nrs)); CK0(tmp.device(&rb, nrs));
-    CK0(tmp.device(&rva, nrs)); CK0(tmp.device(&rvb, nrs));
-    CK0(cudaMemcpyAsync(d_kbytes, key_bytes, (size_t)key_off[nr], cudaMemcpyHostToDevice, st));
-    CK0(cudaMemcpyAsync(d_koff, key_off, 8 * (nrs + 1), cudaMemcpyHostToDevice, st));
-    rc = ids_encode_device(d_kbytes, d_koff, nr, st, kcode, d_kfirst, &n_kc);   // key codes
+    for (int i : {0, 1}) {
+      CK0(tmp.device(&r.k[i], nrs));
+      CK0(tmp.device(&r.v[i], nrs));
+    }
+    rc = ids_encode_host(tmp, st, key_bytes, key_off, nr, &kcode, &d_kfirst, &n_kc);   // key codes
     if (rc != PIO_ALS_OK) return rc;
     const int kbits = ceil_log2((uint64_t)n_kc), ebits = ceil_log2((uint64_t)n_ent);
     fold_rec_event_kernel<<<nblk(n, 256), 256, 0, st>>>(d_prop, n, rec_ev);
     // (entity, key, time, line, index in the object): stable by sorted event position, then by (entity, key)
-    fold_rec_rank_key_kernel<<<nblk(nr, 256), 256, 0, st>>>(rec_ev, rank, nr, ra, rva);
-    CK0(radix_sort_pairs(ra, rva, rb, rvb, nrs, ceil_log2((uint64_t)n), st, &in_b, nullptr));
-    uint64_t* r1 = in_b ? rb : ra;
-    uint32_t* p1 = in_b ? rvb : rva;
-    uint64_t* r2 = in_b ? ra : rb;
-    uint32_t* p2 = in_b ? rva : rvb;
-    fold_rec_key_kernel<<<nblk(nr, 256), 256, 0, st>>>(p1, rec_ev, d_ent, kcode, kbits, nr, r1);
-    CK0(radix_sort_pairs(r1, p1, r2, p2, nrs, ebits + kbits, st, &in_b, nullptr));
-    const uint64_t* rk = in_b ? r2 : r1;
-    const uint32_t* rp = in_b ? p2 : p1;
+    fold_rec_rank_key_kernel<<<nblk(nr, 256), 256, 0, st>>>(rec_ev, rank, nr, r.keys(), r.vals());
+    CK0(radix_sort_pairs(r, nrs, ceil_log2((uint64_t)n), st, nullptr));
+    fold_rec_key_kernel<<<nblk(nr, 256), 256, 0, st>>>(r.vals(), rec_ev, o.ent, kcode, kbits, nr, r.keys());
+    CK0(radix_sort_pairs(r, nrs, ebits + kbits, st, nullptr));
+    const uint64_t* rk = r.keys();
+    const uint32_t* rp = r.vals();
     fold_seg_flag_kernel<<<nblk(nr, 256), 256, 0, st>>>(rk, nr, head);
     CK0(scan_exclusive_u32(head, seg_id, nrs, st, nullptr));
     uint32_t last[2] = {0, 0};
@@ -3513,12 +3496,12 @@ int pio_events_fold_props(int device, const uint8_t* eid_bytes, const int64_t* e
     CK0(cudaMemsetAsync(seg_unset, 0xFF, 4 * nsg, st));
     CK0(cudaMemsetAsync(seg_set, 0xFF, 4 * nsg, st));
     CK0(cudaMemsetAsync(seg_place, 0x7F, 4 * nsg, st));   // 0x7F7F7F7F: above every position
-    fold_props_last_kernel<<<nblk(nr, 256), 256, 0, st>>>(rp, rec_ev, rank, d_code, head, seg_id, nr, seg_unset,
+    fold_props_last_kernel<<<nblk(nr, 256), 256, 0, st>>>(rp, rec_ev, rank, o.code, head, seg_id, nr, seg_unset,
                                                           seg_set);
-    fold_props_place_kernel<<<nblk(nr, 256), 256, 0, st>>>(rp, rec_ev, rank, d_code, d_ent, last_del, head, seg_id,
+    fold_props_place_kernel<<<nblk(nr, 256), 256, 0, st>>>(rp, rec_ev, rank, o.code, o.ent, o.last_del, head, seg_id,
                                                            seg_unset, nr, seg_place);
-    fold_props_present_kernel<<<nblk(n_seg, 256), 256, 0, st>>>(rp, rec_ev, rank, d_ent, last_del, seg_unset, seg_set,
-                                                                n_seg, present);
+    fold_props_present_kernel<<<nblk(n_seg, 256), 256, 0, st>>>(rp, rec_ev, rank, o.ent, o.last_del, seg_unset,
+                                                                seg_set, n_seg, present);
     CK0(cudaGetLastError());
     CK0(scan_exclusive_u32(present, w_pos, nsg, st, nullptr));
     CK0(cudaMemcpyAsync(last, w_pos + n_seg - 1, 4, cudaMemcpyDeviceToHost, st));
@@ -3526,19 +3509,17 @@ int pio_events_fold_props(int device, const uint8_t* eid_bytes, const int64_t* e
     CK0(cudaStreamSynchronize(st));
     nw = (int64_t)last[0] + last[1];
     if (nw > 0) {
-      // the winners in dict order: the sorted record buffers are free again
+      // the winners in dict order, keyed into the spare record half; then they are the data to sort, and the sorted
+      // records (rk / rp) are no longer read
       const int ibits = ceil_log2((uint64_t)max_keys);
-      uint64_t* wk = const_cast<uint64_t*>(rk) == ra ? rb : ra;
-      uint32_t* wv = const_cast<uint32_t*>(rp) == rva ? rvb : rva;
       fold_props_winner_kernel<<<nblk(n_seg, 256), 256, 0, st>>>(rp, rec_ev, rank, d_prop, present, w_pos, seg_set,
-                                                                 seg_place, ibits, n_seg, wk, wv);
-      uint64_t* wk2 = wk == ra ? rb : ra;   // rk / rp are no longer read
-      uint32_t* wv2 = wv == rva ? rvb : rva;
-      CK0(radix_sort_pairs(wk, wv, wk2, wv2, (size_t)nw, ceil_log2((uint64_t)n) + ibits, st, &in_b, nullptr));
-      const uint32_t* ws = in_b ? wv2 : wv;
+                                                                 seg_place, ibits, n_seg, r.spare_keys(),
+                                                                 r.spare_vals());
+      r.flip();
+      CK0(radix_sort_pairs(r, (size_t)nw, ceil_log2((uint64_t)n) + ibits, st, nullptr));
       CK0(tmp.device(&d_wrec, (size_t)nw));
       CK0(tmp.device(&d_wkey, (size_t)nw));
-      fold_props_out_kernel<<<nblk(nw, 256), 256, 0, st>>>(ws, rec_ev, d_ent, kcode, nw, count, d_wrec, d_wkey);
+      fold_props_out_kernel<<<nblk(nw, 256), 256, 0, st>>>(r.vals(), rec_ev, o.ent, kcode, nw, count, d_wrec, d_wkey);
       CK0(cudaGetLastError());
       CK0(cudaMemcpyAsync(out_win_rec, d_wrec, 8 * (size_t)nw, cudaMemcpyDeviceToHost, st));
       CK0(cudaMemcpyAsync(out_win_key, d_wkey, 4 * (size_t)nw, cudaMemcpyDeviceToHost, st));
@@ -3549,10 +3530,10 @@ int pio_events_fold_props(int device, const uint8_t* eid_bytes, const int64_t* e
   uint32_t* w_off = nullptr;
   CK0(tmp.device(&w_off, ne + 1));
   CK0(scan_exclusive_u32(count, w_off, ne + 1, st, nullptr));
-  fold_props_finish_kernel<<<nblk(n_ent + 1, 256), 256, 0, st>>>(vs, seg_first, last_time, last_set, last_del, w_off,
-                                                                 n_ent, d_exists, d_fev, d_lev, d_woff);
+  fold_props_finish_kernel<<<nblk(n_ent + 1, 256), 256, 0, st>>>(vs, o.seg_first, last_time, o.last_set, o.last_del,
+                                                                 w_off, n_ent, d_exists, d_fev, d_lev, d_woff);
   CK0(cudaGetLastError());
-  CK0(cudaMemcpyAsync(out_first_event, d_first, 8 * ne, cudaMemcpyDeviceToHost, st));
+  CK0(cudaMemcpyAsync(out_first_event, o.first, 8 * ne, cudaMemcpyDeviceToHost, st));
   CK0(cudaMemcpyAsync(out_exists, d_exists, ne, cudaMemcpyDeviceToHost, st));
   CK0(cudaMemcpyAsync(out_first_time_event, d_fev, 8 * ne, cudaMemcpyDeviceToHost, st));
   CK0(cudaMemcpyAsync(out_last_time_event, d_lev, 8 * ne, cudaMemcpyDeviceToHost, st));
@@ -3596,19 +3577,15 @@ static int eix_sort(pio_events_index* ix, EixBatch& b, EixRun* out) {
   const long long n = b.r.n;
   const cudaStream_t st = ix->st;
   CallMem tmp(st);
-  uint64_t *ka = nullptr, *kb = nullptr;
-  uint32_t *va = nullptr, *vb = nullptr;
-  CK0(tmp.device(&ka, (size_t)n)); CK0(tmp.device(&kb, (size_t)n));
-  CK0(tmp.device(&va, (size_t)n)); CK0(tmp.device(&vb, (size_t)n));
-  eix_time_key_kernel<<<nblk(n, 256), 256, 0, st>>>(b.r.time_us, n, ka, va);
-  bool in_b = false;
-  CK0(radix_sort_pairs(ka, va, kb, vb, (size_t)n, 64, st, &in_b, nullptr));
-  uint64_t* k1 = in_b ? kb : ka;   // by time; the other pair is free
-  uint32_t* v1 = in_b ? vb : va;
-  uint64_t* k2 = in_b ? ka : kb;
-  uint32_t* v2 = in_b ? va : vb;
-  eix_hash_key_kernel<<<nblk(n, 256), 256, 0, st>>>(v1, b.r.hash, n, k1);
-  CK0(radix_sort_pairs(k1, v1, k2, v2, (size_t)n, 64 - __builtin_clzll(ix->mask), st, &in_b, nullptr));
+  SortBufs sb;
+  for (int i : {0, 1}) {
+    CK0(tmp.device(&sb.k[i], (size_t)n));
+    CK0(tmp.device(&sb.v[i], (size_t)n));
+  }
+  eix_time_key_kernel<<<nblk(n, 256), 256, 0, st>>>(b.r.time_us, n, sb.keys(), sb.vals());
+  CK0(radix_sort_pairs(sb, (size_t)n, 64, st, nullptr));
+  eix_hash_key_kernel<<<nblk(n, 256), 256, 0, st>>>(sb.vals(), b.r.hash, n, sb.keys());
+  CK0(radix_sort_pairs(sb, (size_t)n, 64 - __builtin_clzll(ix->mask), st, nullptr));
   EixRun r;
   const cudaError_t e = eix_alloc(r, n, -1);
   if (e != cudaSuccess) {
@@ -3616,7 +3593,7 @@ static int eix_sort(pio_events_index* ix, EixBatch& b, EixRun* out) {
     return fail(nullptr, PIO_ALS_ERR_CUDA, "event index: %s", cudaGetErrorString(e));
   }
   r.n = n;
-  eix_gather_kernel<<<nblk(n, 256), 256, 0, st>>>(b.r, in_b ? v2 : v1, r);
+  eix_gather_kernel<<<nblk(n, 256), 256, 0, st>>>(b.r, sb.vals(), r);
   r.arena = b.r.arena, r.arena_bytes = b.r.arena_bytes;
   b.r.arena = nullptr;
   cudaError_t e2 = cudaStreamSynchronize(st);
@@ -3863,23 +3840,25 @@ int pio_cooc_train(int device, const int32_t* user, const int32_t* item, int64_t
   cudaStream_t st = 0;
   CallMem tmp(st);
   int *du = nullptr, *di = nullptr;
-  uint64_t *ka = nullptr, *kb = nullptr, *dk = nullptr;
-  uint32_t *va = nullptr, *vb = nullptr, *flag = nullptr, *rank = nullptr;
+  uint64_t* dk = nullptr;
+  uint32_t *flag = nullptr, *rank = nullptr;
+  SortBufs sb;
   CK0(tmp.device(&du, (size_t)n)); CK0(tmp.device(&di, (size_t)n));
-  CK0(tmp.device(&ka, (size_t)n)); CK0(tmp.device(&kb, (size_t)n));
-  CK0(tmp.device(&va, (size_t)n)); CK0(tmp.device(&vb, (size_t)n));
+  for (int i : {0, 1}) {
+    CK0(tmp.device(&sb.k[i], (size_t)n));
+    CK0(tmp.device(&sb.v[i], (size_t)n));
+  }
   CK0(tmp.device(&flag, (size_t)n)); CK0(tmp.device(&dk, (size_t)n)); CK0(tmp.device(&rank, (size_t)n));
   CK0(cudaMemcpyAsync(du, user, 4 * (size_t)n, cudaMemcpyHostToDevice, st));
   CK0(cudaMemcpyAsync(di, item, 4 * (size_t)n, cudaMemcpyHostToDevice, st));
   // 1. distinct (user, item), sorted by user then item
-  cooc_keys_kernel<<<nblk(n, 256), 256, 0, st>>>(du, di, n, bits_i, ka, va);
-  bool in_b = false;
-  CK0(radix_sort_pairs(ka, va, kb, vb, (size_t)n, bits_u + bits_i, st, &in_b, nullptr));
-  const uint64_t* ks = in_b ? kb : ka;
+  cooc_keys_kernel<<<nblk(n, 256), 256, 0, st>>>(du, di, n, bits_i, sb.keys(), sb.vals());
+  CK0(radix_sort_pairs(sb, (size_t)n, bits_u + bits_i, st, nullptr));
+  const uint64_t* ks = sb.keys();
   cooc_head_kernel<<<nblk(n, 256), 256, 0, st>>>(ks, n, flag);
   uint32_t lf = 0, lp = 0;
   CK0(cudaMemcpyAsync(&lf, flag + n - 1, 4, cudaMemcpyDeviceToHost, st));
-  uint32_t* pos = in_b ? va : vb;   // the payload buffer that is free now
+  uint32_t* pos = sb.spare_vals();
   CK0(scan_exclusive_u32(flag, pos, (size_t)n, st, nullptr));
   CK0(cudaMemcpyAsync(&lp, pos + n - 1, 4, cudaMemcpyDeviceToHost, st));
   CK0(cudaStreamSynchronize(st));
@@ -3897,15 +3876,16 @@ int pio_cooc_train(int device, const int32_t* user, const int32_t* item, int64_t
   if (np >= (1ll << 31)) return fail(nullptr, PIO_ALS_ERR_ARG, "more than 2^31-1 co-occurrence pairs (%lld)", np);
   std::vector<int> h_item((size_t)n_items * topn, -1), h_cnt((size_t)n_items * topn, 0), h_n((size_t)n_items, 0);
   if (np > 0) {
-    uint64_t *pk = nullptr, *pk2 = nullptr, *rk = nullptr, *rk2 = nullptr;
-    uint32_t *pp = nullptr, *pp2 = nullptr, *pf = nullptr, *ppos = nullptr, *rp = nullptr, *rp2 = nullptr;
-    CK0(tmp.device(&pk, (size_t)np)); CK0(tmp.device(&pk2, (size_t)np));
-    CK0(tmp.device(&pp, (size_t)np)); CK0(tmp.device(&pp2, (size_t)np));
+    SortBufs ps, rs;
+    uint32_t *pf = nullptr, *ppos = nullptr;
+    for (int i : {0, 1}) {
+      CK0(tmp.device(&ps.k[i], (size_t)np));
+      CK0(tmp.device(&ps.v[i], (size_t)np));
+    }
     CK0(tmp.device(&pf, (size_t)np)); CK0(tmp.device(&ppos, (size_t)np));
-    cooc_pairs_kernel<<<nblk(m, 256), 256, 0, st>>>(dk, rank, off, m, bits_i, pk, pp);
-    bool pb_ = false;
-    CK0(radix_sort_pairs(pk, pp, pk2, pp2, (size_t)np, 2 * bits_i, st, &pb_, nullptr));
-    const uint64_t* pks = pb_ ? pk2 : pk;
+    cooc_pairs_kernel<<<nblk(m, 256), 256, 0, st>>>(dk, rank, off, m, bits_i, ps.keys(), ps.vals());
+    CK0(radix_sort_pairs(ps, (size_t)np, 2 * bits_i, st, nullptr));
+    const uint64_t* pks = ps.keys();
     cooc_head_kernel<<<nblk(np, 256), 256, 0, st>>>(pks, np, pf);
     uint32_t cf = 0, cp = 0;
     CK0(cudaMemcpyAsync(&cf, pf + np - 1, 4, cudaMemcpyDeviceToHost, st));
@@ -3914,18 +3894,19 @@ int pio_cooc_train(int device, const int32_t* user, const int32_t* item, int64_t
     CK0(cudaStreamSynchronize(st));
     const long long C = (long long)cp + cf, n2 = 2 * C;
     // 3. both directions, ranked per item by (count desc, other item asc)
-    CK0(tmp.device(&rk, (size_t)n2)); CK0(tmp.device(&rk2, (size_t)n2));
-    CK0(tmp.device(&rp, (size_t)n2)); CK0(tmp.device(&rp2, (size_t)n2));
-    cooc_runs_kernel<<<nblk(np, 256), 256, 0, st>>>(pks, pf, ppos, np, bits_i, bits_c, rk, rp);
-    bool rb = false;
-    CK0(radix_sort_pairs(rk, rp, rk2, rp2, (size_t)n2, 2 * bits_i + bits_c, st, &rb, nullptr));
+    for (int i : {0, 1}) {
+      CK0(tmp.device(&rs.k[i], (size_t)n2));
+      CK0(tmp.device(&rs.v[i], (size_t)n2));
+    }
+    cooc_runs_kernel<<<nblk(np, 256), 256, 0, st>>>(pks, pf, ppos, np, bits_i, bits_c, rs.keys(), rs.vals());
+    CK0(radix_sort_pairs(rs, (size_t)n2, 2 * bits_i + bits_c, st, nullptr));
     int *d_oi = nullptr, *d_oc = nullptr, *d_on = nullptr;
     CK0(tmp.device(&d_oi, (size_t)n_items * topn)); CK0(tmp.device(&d_oc, (size_t)n_items * topn));
     CK0(tmp.device(&d_on, (size_t)n_items));
     CK0(cudaMemsetAsync(d_oi, 0xff, 4 * (size_t)n_items * topn, st));
     CK0(cudaMemsetAsync(d_oc, 0, 4 * (size_t)n_items * topn, st));
     CK0(cudaMemsetAsync(d_on, 0, 4 * (size_t)n_items, st));
-    cooc_take_kernel<<<nblk(n2, 256), 256, 0, st>>>(rb ? rk2 : rk, rb ? rp2 : rp, n2, bits_i, bits_c, topn, d_oi, d_oc, d_on);
+    cooc_take_kernel<<<nblk(n2, 256), 256, 0, st>>>(rs.keys(), rs.vals(), n2, bits_i, bits_c, topn, d_oi, d_oc, d_on);
     CK0(cudaMemcpyAsync(h_item.data(), d_oi, 4 * h_item.size(), cudaMemcpyDeviceToHost, st));
     CK0(cudaMemcpyAsync(h_cnt.data(), d_oc, 4 * h_cnt.size(), cudaMemcpyDeviceToHost, st));
     CK0(cudaMemcpyAsync(h_n.data(), d_on, 4 * h_n.size(), cudaMemcpyDeviceToHost, st));

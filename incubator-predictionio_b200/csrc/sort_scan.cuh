@@ -203,35 +203,41 @@ rs_scatter_kernel(const uint64_t* __restrict__ kin, const uint32_t* __restrict__
 
 constexpr size_t RS_SCATTER_SMEM = (size_t)RS_TILE * (sizeof(uint64_t) + sizeof(uint32_t));   // 48 KB
 
-// Sorts by key bits [0, nbits). Buffers a = input (clobbered), b = scratch. *result_in_b tells
-// where the sorted data ended up.
-inline cudaError_t radix_sort_pairs(uint64_t* ka, uint32_t* va, uint64_t* kb, uint32_t* vb, size_t n,
-                                    int nbits, cudaStream_t st, bool* result_in_b, int64_t* launches) {
-  *result_in_b = false;
+// The two halves of a sort's ping-pong, each a key buffer with its payload buffer. The caller allocates both halves
+// (all four buffers hold n elements) and fills the live one; radix_sort_pairs sorts the live half and leaves `live`
+// naming the half that holds the result. The other half is spare: free for the caller to reuse.
+struct SortBufs {
+  uint64_t* k[2] = {nullptr, nullptr};
+  uint32_t* v[2] = {nullptr, nullptr};
+  int live = 0;
+  uint64_t* keys() const { return k[live]; }
+  uint32_t* vals() const { return v[live]; }
+  uint64_t* spare_keys() const { return k[live ^ 1]; }
+  uint32_t* spare_vals() const { return v[live ^ 1]; }
+  void flip() { live ^= 1; }   // the spare half becomes live: for data the caller writes there
+};
+
+// Stable sort of the live half by key bits [0, nbits); the spare half is clobbered.
+inline cudaError_t radix_sort_pairs(SortBufs& b, size_t n, int nbits, cudaStream_t st, int64_t* launches) {
   if (n == 0) return cudaSuccess;
   const unsigned nblocks = (unsigned)((n + RS_TILE - 1) / RS_TILE);
   uint32_t* hist = nullptr;
   cudaError_t e = cudaMallocAsync((void**)&hist, (size_t)256 * nblocks * sizeof(uint32_t), st);
   if (e != cudaSuccess) return e;
   e = cudaFuncSetAttribute(rs_scatter_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)RS_SCATTER_SMEM);
-  if (e != cudaSuccess) return e;
-  bool in_b = false;
-  for (int shift = 0; shift < nbits; shift += 8) {
-    uint64_t* ki = in_b ? kb : ka;
-    uint32_t* vi = in_b ? vb : va;
-    uint64_t* ko = in_b ? ka : kb;
-    uint32_t* vo = in_b ? va : vb;
-    rs_hist_kernel<<<nblocks, RS_THREADS, 0, st>>>(ki, n, shift, hist, nblocks);
+  for (int shift = 0; e == cudaSuccess && shift < nbits; shift += 8) {
+    rs_hist_kernel<<<nblocks, RS_THREADS, 0, st>>>(b.keys(), n, shift, hist, nblocks);
     if (launches) ++*launches;
     e = scan_exclusive_u32(hist, hist, (size_t)256 * nblocks, st, launches);
-    if (e != cudaSuccess) return e;
-    rs_scatter_kernel<<<nblocks, RS_THREADS, RS_SCATTER_SMEM, st>>>(ki, vi, ko, vo, n, shift, hist, nblocks);
+    if (e != cudaSuccess) break;
+    rs_scatter_kernel<<<nblocks, RS_THREADS, RS_SCATTER_SMEM, st>>>(b.keys(), b.vals(), b.spare_keys(), b.spare_vals(),
+                                                                    n, shift, hist, nblocks);
     if (launches) ++*launches;
-    in_b = !in_b;
+    b.flip();
   }
-  e = cudaFreeAsync(hist, st);
+  const cudaError_t ef = cudaFreeAsync(hist, st);
   if (e != cudaSuccess) return e;
-  *result_in_b = in_b;
+  if (ef != cudaSuccess) return ef;
   return cudaGetLastError();
 }
 

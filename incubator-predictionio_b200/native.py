@@ -135,15 +135,26 @@ def _addr(a):
     return None if a is None else a.ctypes.data
 
 
+def _check(rc, h=None):
+    """Raises NativeError for a nonzero status, with the library's last error message (of handle h, if given)."""
+    if rc != 0:
+        raise NativeError(rc, lib().pio_als_last_error(h).decode())
+
+
+def _str_column(enc):
+    """A string column (bytes uint8[], offsets int64[n + 1]) from a list of already-encoded bytes."""
+    off = np.zeros(len(enc) + 1, np.int64)
+    off[1:] = np.cumsum([len(b) for b in enc], dtype=np.int64)
+    return np.frombuffer(b"".join(enc), np.uint8), off
+
+
 def device_count() -> int:
     return int(lib().pio_als_device_count())
 
 
 def nccl_unique_id() -> bytes:
     buf = (C.c_uint8 * 128)()
-    rc = lib().pio_als_nccl_unique_id(buf)
-    if rc != 0:
-        raise NativeError(rc, lib().pio_als_last_error(None).decode())
+    _check(lib().pio_als_nccl_unique_id(buf))
     return bytes(buf)
 
 
@@ -165,9 +176,7 @@ class NativeALS:
         cfg.lambda_, cfg.alpha, cfg.seed = float(lam), float(alpha), int(seed)
         if nccl_id is not None:
             cfg.nccl_id[:] = list(nccl_id)
-        rc = lib().pio_als_create(C.byref(cfg), C.byref(self._h))
-        if rc != 0:
-            raise NativeError(rc, lib().pio_als_last_error(None).decode())
+        _check(lib().pio_als_create(C.byref(cfg), C.byref(self._h)))
 
     # -- lifecycle --------------------------------------------------------------------------
     def close(self):
@@ -182,8 +191,7 @@ class NativeALS:
             pass
 
     def _check(self, rc):
-        if rc != 0:
-            raise NativeError(rc, lib().pio_als_last_error(self._h).decode())
+        _check(rc, self._h)
 
     # -- training ---------------------------------------------------------------------------
     def set_ratings(self, user, item, rating, dedup=DEDUP_NONE, ts=None):
@@ -312,9 +320,7 @@ class NativeALS:
     @classmethod
     def load(cls, path: str, device: int = 0) -> "NativeALS":
         h = C.c_void_p()
-        rc = lib().pio_als_load(str(path).encode(), C.c_int(device), C.byref(h))
-        if rc != 0:
-            raise NativeError(rc, lib().pio_als_last_error(None).decode())
+        _check(lib().pio_als_load(str(path).encode(), C.c_int(device), C.byref(h)))
         # read the header for the shape
         hdr = np.fromfile(path, dtype=np.int32, count=8)
         return cls(rank=int(hdr[3]), n_users=int(hdr[5]), n_items=int(hdr[6]), _handle=h)
@@ -334,10 +340,8 @@ class NativeALS:
         uh = None if user_has is None else np.ascontiguousarray(user_has, np.uint8)
         ih = None if item_has is None else np.ascontiguousarray(item_has, np.uint8)
         h = C.c_void_p()
-        rc = lib().pio_als_model_import(C.byref(cfg), _ptr(uf, C.c_float), _ptr(itf, C.c_float), _ptr(uh, C.c_uint8),
-                                        _ptr(ih, C.c_uint8), C.byref(h))
-        if rc != 0:
-            raise NativeError(rc, lib().pio_als_last_error(None).decode())
+        _check(lib().pio_als_model_import(C.byref(cfg), _ptr(uf, C.c_float), _ptr(itf, C.c_float), _ptr(uh, C.c_uint8),
+                                          _ptr(ih, C.c_uint8), C.byref(h)))
         return cls(rank=int(k), n_users=max(int(nu), 1), n_items=int(ni), _handle=h)
 
     def stats(self) -> dict:
@@ -358,11 +362,9 @@ class NativeALS:
 
 
 def synth_ratings_device(device, n_users, n_items, nnz, seed, implicit, start, d_user, d_item, d_rating):
-    rc = lib().pio_als_synth_ratings_device(C.c_int(device), C.c_int32(n_users), C.c_int32(n_items), C.c_int64(nnz),
-                                            C.c_int64(seed), C.c_int(int(implicit)), C.c_int64(start),
-                                            C.c_void_p(d_user), C.c_void_p(d_item), C.c_void_p(d_rating))
-    if rc != 0:
-        raise NativeError(rc, lib().pio_als_last_error(None).decode())
+    _check(lib().pio_als_synth_ratings_device(C.c_int(device), C.c_int32(n_users), C.c_int32(n_items), C.c_int64(nnz),
+                                              C.c_int64(seed), C.c_int(int(implicit)), C.c_int64(start),
+                                              C.c_void_p(d_user), C.c_void_p(d_item), C.c_void_p(d_rating)))
 
 
 def ids_encode(strings, device=0):
@@ -373,19 +375,13 @@ def ids_encode(strings, device=0):
         buf = np.ascontiguousarray(buf, np.uint8)
         off = np.ascontiguousarray(off, np.int64)
     else:
-        enc = [s if isinstance(s, (bytes, bytearray)) else str(s).encode("utf-8") for s in strings]
-        off = np.zeros(len(enc) + 1, np.int64)
-        if enc:
-            off[1:] = np.cumsum([len(b) for b in enc])
-        buf = np.frombuffer(b"".join(enc), np.uint8) if enc else np.zeros(0, np.uint8)
+        buf, off = _str_column([s if isinstance(s, (bytes, bytearray)) else str(s).encode("utf-8") for s in strings])
     n = off.shape[0] - 1
     idx = np.empty(n, np.int32)
     first = np.empty(max(n, 1), np.int64)
     nu = C.c_int32(0)
-    rc = lib().pio_ids_encode(C.c_int(device), _ptr(buf, C.c_uint8) if buf.size else None, _ptr(off, C.c_int64),
-                              C.c_int64(n), _ptr(idx, C.c_int32), _ptr(first, C.c_int64), C.byref(nu))
-    if rc != 0:
-        raise NativeError(rc, lib().pio_als_last_error(None).decode())
+    _check(lib().pio_ids_encode(C.c_int(device), _ptr(buf, C.c_uint8) if buf.size else None, _ptr(off, C.c_int64),
+                                C.c_int64(n), _ptr(idx, C.c_int32), _ptr(first, C.c_int64), C.byref(nu)))
     return idx, first[:nu.value]
 
 
@@ -425,52 +421,24 @@ def events_scan_keys(text, keys, entity_type=None, event_names=None, target_mode
 
 def _events_scan(text, entity_type, event_names, target_mode, target_entity_type, prop, start_us, until_us, device,
                  keys):
-    buf = np.frombuffer(text, np.uint8) if isinstance(text, (bytes, bytearray, memoryview)) else \
-        np.ascontiguousarray(text, np.uint8)
-    n = int(buf.shape[0])
-    f, keep = _events_filter(entity_type, event_names, target_mode, target_entity_type, prop, start_us, until_us)
-    cap = n // EVENTS_MIN_EVENT_BYTES + 1
-    out = dict(line=np.empty(cap, np.int64), code=np.empty(cap, np.int32), value=np.empty(cap, np.float64),
-               flags=np.empty(cap, np.uint8), time_us=np.empty(cap, np.int64), eid_bytes=np.empty(max(n, 1), np.uint8),
-               eid_off=np.empty(cap + 1, np.int64), tid_bytes=np.empty(max(n, 1), np.uint8),
-               tid_off=np.empty(cap + 1, np.int64))
-    cols = [("line", C.c_int64), ("code", C.c_int32), ("value", C.c_double), ("flags", C.c_uint8),
-            ("time_us", C.c_int64), ("eid_bytes", C.c_uint8), ("eid_off", C.c_int64), ("tid_bytes", C.c_uint8),
-            ("tid_off", C.c_int64)]
-    nk = 0 if keys is None else len(keys)
-    if keys is not None:
-        kb = [k.encode("utf-8") if isinstance(k, str) else k for k in keys]
-        kp = (C.c_char_p * max(nk, 1))(*kb)
-        out.update(present=np.empty(cap, np.uint8), number=np.empty(cap, np.uint8), num=np.empty((cap, max(nk, 1))),
-                   tok_bytes=np.empty(max(n, 1), np.uint8), tok_off=np.empty(cap * max(nk, 1) + 1, np.int64))
-        cols += [("present", C.c_uint8), ("number", C.c_uint8), ("num", C.c_double), ("tok_bytes", C.c_uint8),
-                 ("tok_off", C.c_int64)]
-    fb_cap = max(1024, n // 4096)
-    n_ev, n_fb, n_lines = C.c_int64(0), C.c_int64(0), C.c_int64(0)
-    while True:
-        fb = [np.empty(fb_cap, np.int64) for _ in range(3)]
-        head = (C.c_int(device), _ptr(buf, C.c_uint8) if n else None, C.c_int64(n), C.byref(f))
-        tail = (C.byref(n_ev), C.c_int64(fb_cap), *[_ptr(a, C.c_int64) for a in fb], C.byref(n_fb), C.byref(n_lines))
-        if keys is None:
-            rc = lib().pio_events_scan(*head, C.c_int64(cap), *[_ptr(out[k], t) for k, t in cols], *tail)
-        else:
-            rc = lib().pio_events_scan_keys(*head, kp, C.c_int(nk), C.c_int64(cap),
-                                            *[_ptr(out[k], t) for k, t in cols], *tail)
-        if rc != 0:
-            raise NativeError(rc, lib().pio_als_last_error(None).decode())
-        if n_fb.value <= fb_cap:
-            break
-        fb_cap = n_fb.value     # more fallback lines than room: once more with room for all of them
-    m = n_ev.value
-    res = {k: out[k][:m] for k in ("line", "code", "value", "flags", "time_us")}
-    res["eid_off"], res["tid_off"] = out["eid_off"][:m + 1], out["tid_off"][:m + 1]
-    res["eid_bytes"], res["tid_bytes"] = out["eid_bytes"][:res["eid_off"][-1]], out["tid_bytes"][:res["tid_off"][-1]]
-    res["fb_line"], res["fb_begin"], res["fb_end"] = (a[:n_fb.value] for a in fb)
-    res["n_lines"] = n_lines.value
-    if keys is not None:
-        res["present"], res["number"], res["num"] = out["present"][:m], out["number"][:m], out["num"][:m, :nk]
-        res["tok_off"] = out["tok_off"][:m * nk + 1]
-        res["tok_bytes"] = out["tok_bytes"][:res["tok_off"][-1]]
+    """pio_events_scan (keys None) or pio_events_scan_keys, with any filter (the ABI refuses a keyed scan with prop)."""
+    filt = (entity_type, event_names, target_mode, target_entity_type, prop, start_us, until_us)
+    if keys is None:
+        return _scan(text, filt, device, lambda n, cap: {},
+                     lambda head, base, out, tail: lib().pio_events_scan(*head, *base, *tail))[0]
+    kb = [k.encode("utf-8") if isinstance(k, str) else k for k in keys]
+    nk = len(kb)
+    kp = (C.c_char_p * max(nk, 1))(*kb)
+    res, out = _scan(
+        text, filt, device,
+        lambda n, cap: dict(present=np.empty(cap, np.uint8), number=np.empty(cap, np.uint8),
+                            num=np.empty((cap, max(nk, 1))), tok_bytes=np.empty(max(n, 1), np.uint8),
+                            tok_off=np.empty(cap * max(nk, 1) + 1, np.int64)),
+        lambda head, base, out, tail: lib().pio_events_scan_keys(
+            *head, kp, C.c_int(nk), *base, *_addrs(out, "present", "number", "num", "tok_bytes", "tok_off"), *tail))
+    m = len(res["line"])
+    res["present"], res["number"], res["num"] = out["present"][:m], out["number"][:m], out["num"][:m, :nk]
+    _take_strings(res, out, "tok", m * nk)
     return res
 
 
@@ -483,46 +451,73 @@ def events_scan_props(text, entity_type=None, event_names=None, target_mode=EVEN
     int16) and prop_off (int64 [n + 1]: its records), and per record r, one per top-level key of `properties` in object
     order: the decoded key key_bytes[key_off[r]:key_off[r + 1]] and the raw JSON token of its value
     tok_bytes[tok_off[r]:tok_off[r + 1]]."""
+    rcap, n_rec = C.c_int64(0), C.c_int64(0)
+
+    def cols(n, cap):
+        rcap.value = n // EVENTS_MIN_RECORD_BYTES + 1
+        return dict(utc_off=np.empty(cap, np.int16), prop_off=np.empty(cap + 1, np.int64),
+                    key_bytes=np.empty(max(n, 1), np.uint8), key_off=np.empty(rcap.value + 1, np.int64),
+                    tok_bytes=np.empty(max(n, 1), np.uint8), tok_off=np.empty(rcap.value + 1, np.int64))
+
+    res, out = _scan(
+        text, (entity_type, event_names, target_mode, target_entity_type, None, start_us, until_us), device, cols,
+        lambda head, base, out, tail: lib().pio_events_scan_props(
+            *head, *base, *_addrs(out, "utc_off", "prop_off"), rcap,
+            *_addrs(out, "key_bytes", "key_off", "tok_bytes", "tok_off"), tail[0], C.byref(n_rec), *tail[1:]))
+    m = len(res["line"])
+    res["utc_off"], res["prop_off"] = out["utc_off"][:m], out["prop_off"][:m + 1]
+    for k in ("key", "tok"):
+        _take_strings(res, out, k, n_rec.value)
+    return res
+
+
+_SCAN_COLS = (("line", np.int64), ("code", np.int32), ("value", np.float64), ("flags", np.uint8),
+              ("time_us", np.int64))
+
+
+def _scan(text, filt, device, extra_cols, call):
+    """What every event scan marshals: the text buffer, the filter (filt: _events_filter's arguments), the base columns,
+    the second call with room for every fallback line, and the slicing of the base results.  extra_cols(n_bytes, cap)
+    gives the scan's own output arrays; call(head, base, out, tail) makes its ABI call, where head is (device, text,
+    n_bytes, filter), base is (capacity, the base columns), out holds every output array and tail is (n_events,
+    fallback capacity, the three fallback columns, n_fallback, n_lines).  Returns the dict of base results and `out`,
+    from which the caller slices its own columns."""
     buf = np.frombuffer(text, np.uint8) if isinstance(text, (bytes, bytearray, memoryview)) else \
         np.ascontiguousarray(text, np.uint8)
     n = int(buf.shape[0])
-    f, keep = _events_filter(entity_type, event_names, target_mode, target_entity_type, None, start_us, until_us)
+    f, keep = _events_filter(*filt)
     cap = n // EVENTS_MIN_EVENT_BYTES + 1
-    rcap = n // EVENTS_MIN_RECORD_BYTES + 1
-    out = dict(line=np.empty(cap, np.int64), code=np.empty(cap, np.int32), value=np.empty(cap, np.float64),
-               flags=np.empty(cap, np.uint8), time_us=np.empty(cap, np.int64), eid_bytes=np.empty(max(n, 1), np.uint8),
-               eid_off=np.empty(cap + 1, np.int64), tid_bytes=np.empty(max(n, 1), np.uint8),
-               tid_off=np.empty(cap + 1, np.int64), utc_off=np.empty(cap, np.int16), prop_off=np.empty(cap + 1, np.int64))
-    rec = dict(key_bytes=np.empty(max(n, 1), np.uint8), key_off=np.empty(rcap + 1, np.int64),
-               tok_bytes=np.empty(max(n, 1), np.uint8), tok_off=np.empty(rcap + 1, np.int64))
+    out = {k: np.empty(cap, t) for k, t in _SCAN_COLS}
+    out.update(eid_bytes=np.empty(max(n, 1), np.uint8), eid_off=np.empty(cap + 1, np.int64),
+               tid_bytes=np.empty(max(n, 1), np.uint8), tid_off=np.empty(cap + 1, np.int64), **extra_cols(n, cap))
+    head = (C.c_int(device), _ptr(buf, C.c_uint8) if n else None, C.c_int64(n), C.byref(f))
+    base = (C.c_int64(cap), *_addrs(out, *[k for k, _ in _SCAN_COLS], "eid_bytes", "eid_off", "tid_bytes", "tid_off"))
     fb_cap = max(1024, n // 4096)
-    n_ev, n_rec, n_fb, n_lines = C.c_int64(0), C.c_int64(0), C.c_int64(0), C.c_int64(0)
+    n_ev, n_fb, n_lines = C.c_int64(0), C.c_int64(0), C.c_int64(0)
     while True:
         fb = [np.empty(fb_cap, np.int64) for _ in range(3)]
-        rc = lib().pio_events_scan_props(
-            C.c_int(device), _ptr(buf, C.c_uint8) if n else None, C.c_int64(n), C.byref(f), C.c_int64(cap),
-            *[C.c_void_p(_addr(out[k])) for k in ("line", "code", "value", "flags", "time_us", "eid_bytes", "eid_off",
-                                                  "tid_bytes", "tid_off", "utc_off", "prop_off")],
-            C.c_int64(rcap), *[C.c_void_p(_addr(rec[k])) for k in ("key_bytes", "key_off", "tok_bytes", "tok_off")],
-            C.byref(n_ev), C.byref(n_rec), C.c_int64(fb_cap), *[_ptr(a, C.c_int64) for a in fb], C.byref(n_fb),
-            C.byref(n_lines))
-        if rc != 0:
-            raise NativeError(rc, lib().pio_als_last_error(None).decode())
+        _check(call(head, base, out, (C.byref(n_ev), C.c_int64(fb_cap), *[_ptr(a, C.c_int64) for a in fb],
+                                      C.byref(n_fb), C.byref(n_lines))))
         if n_fb.value <= fb_cap:
             break
         fb_cap = n_fb.value     # more fallback lines than room: once more with room for all of them
-    m, nr = n_ev.value, n_rec.value
-    res = {k: out[k][:m] for k in ("line", "code", "value", "flags", "time_us", "utc_off")}
+    m = n_ev.value
+    res = {k: out[k][:m] for k, _ in _SCAN_COLS}
     for k in ("eid", "tid"):
-        res[k + "_off"] = out[k + "_off"][:m + 1]
-        res[k + "_bytes"] = out[k + "_bytes"][:res[k + "_off"][-1]]
-    res["prop_off"] = out["prop_off"][:m + 1]
-    for k in ("key", "tok"):
-        res[k + "_off"] = rec[k + "_off"][:nr + 1]
-        res[k + "_bytes"] = rec[k + "_bytes"][:res[k + "_off"][-1]]
+        _take_strings(res, out, k, m)
     res["fb_line"], res["fb_begin"], res["fb_end"] = (a[:n_fb.value] for a in fb)
     res["n_lines"] = n_lines.value
-    return res
+    return res, out
+
+
+def _addrs(out, *keys):
+    return [C.c_void_p(_addr(out[k])) for k in keys]
+
+
+def _take_strings(res, out, name, count):
+    """res[name_off], res[name_bytes]: the first `count` strings of the string column out[name_bytes / name_off]."""
+    res[name + "_off"] = out[name + "_off"][:count + 1]
+    res[name + "_bytes"] = out[name + "_bytes"][:res[name + "_off"][-1]]
 
 
 def events_fold_props(eid, code, time_us, prop_off, keys, device=0):
@@ -543,14 +538,12 @@ def events_fold_props(eid, code, time_us, prop_off, keys, device=0):
     fev, lev, woff = np.empty(max(n, 1), np.int64), np.empty(max(n, 1), np.int64), np.empty(n + 1, np.int64)
     wrec, wkey, kfirst = np.empty(max(nr, 1), np.int64), np.empty(max(nr, 1), np.int32), np.empty(max(nr, 1), np.int64)
     ne, nk = C.c_int64(0), C.c_int64(0)
-    rc = lib().pio_events_fold_props(
+    _check(lib().pio_events_fold_props(
         C.c_int(device), _ptr(buf, C.c_uint8) if buf.size else None, _ptr(off, C.c_int64), _ptr(code, C.c_int32),
         _ptr(time_us, C.c_int64), _ptr(prop_off, C.c_int64), C.c_int64(n), _ptr(kbuf, C.c_uint8) if kbuf.size else None,
         _ptr(koff, C.c_int64), _ptr(first, C.c_int64), _ptr(exists, C.c_uint8), _ptr(fev, C.c_int64),
         _ptr(lev, C.c_int64), _ptr(woff, C.c_int64), _ptr(wrec, C.c_int64), _ptr(wkey, C.c_int32),
-        _ptr(kfirst, C.c_int64), C.byref(ne), C.byref(nk))
-    if rc != 0:
-        raise NativeError(rc, lib().pio_als_last_error(None).decode())
+        _ptr(kfirst, C.c_int64), C.byref(ne), C.byref(nk)))
     g = ne.value
     w_off = woff[:g + 1] if g else np.zeros(1, np.int64)
     nw = int(w_off[-1])
@@ -572,12 +565,10 @@ def events_fold(eid, code, time_us, present=None, n_keys=0, device=0):
     fus, lus = np.empty(max(n, 1), np.int64), np.empty(max(n, 1), np.int64)
     win = np.empty((max(n, 1), max(int(n_keys), 1)), np.int64)
     ne = C.c_int64(0)
-    rc = lib().pio_events_fold(C.c_int(device), _ptr(buf, C.c_uint8) if buf.size else None, _ptr(off, C.c_int64),
-                               _ptr(code, C.c_int32), _ptr(time_us, C.c_int64), _ptr(pm, C.c_uint8), C.c_int64(n),
-                               C.c_int(int(n_keys)), _ptr(first, C.c_int64), _ptr(exists, C.c_uint8), _ptr(fus, C.c_int64),
-                               _ptr(lus, C.c_int64), _ptr(win, C.c_int64), C.byref(ne))
-    if rc != 0:
-        raise NativeError(rc, lib().pio_als_last_error(None).decode())
+    _check(lib().pio_events_fold(C.c_int(device), _ptr(buf, C.c_uint8) if buf.size else None, _ptr(off, C.c_int64),
+                                 _ptr(code, C.c_int32), _ptr(time_us, C.c_int64), _ptr(pm, C.c_uint8), C.c_int64(n),
+                                 C.c_int(int(n_keys)), _ptr(first, C.c_int64), _ptr(exists, C.c_uint8), _ptr(fus, C.c_int64),
+                                 _ptr(lus, C.c_int64), _ptr(win, C.c_int64), C.byref(ne)))
     g = ne.value
     return dict(first_event=first[:g], exists=exists[:g].astype(bool), first_us=fus[:g], last_us=lus[:g],
                 winner=win[:g, :int(n_keys)])
@@ -615,8 +606,7 @@ class EventsIndex:
         self._check(lib().pio_events_index_create(C.c_int(device), C.byref(f), C.byref(self._h)))
 
     def _check(self, rc):
-        if rc != 0:
-            raise NativeError(rc, lib().pio_als_last_error(None).decode())
+        _check(rc)
 
     def close(self):
         if self._h:
@@ -650,9 +640,7 @@ class EventsIndex:
     def add_host(self, ids, time_us, offset, length):
         """Events parsed on the host, in file order: entityId strings, eventTime (us), line offset and length."""
         enc = [x.encode("utf-8", "surrogatepass") for x in ids]
-        off = np.zeros(len(enc) + 1, np.int64)
-        np.cumsum([len(b) for b in enc], out=off[1:])
-        buf = np.frombuffer(b"".join(enc), np.uint8)
+        buf, off = _str_column(enc)
         t, o, ln = (np.ascontiguousarray(a, d) for a, d in ((time_us, np.int64), (offset, np.int64), (length, np.int32)))
         self._check(lib().pio_events_index_add_host(self._h, _ptr(buf, C.c_uint8) if buf.size else None,
                                                     _ptr(off, C.c_int64), _ptr(t, C.c_int64), _ptr(o, C.c_int64),
@@ -661,11 +649,8 @@ class EventsIndex:
     def lookup(self, ids, limit=None):
         """For each entityId of `ids` (str): (offsets int64[], lengths int32[]) of its lines, latest first, at most
         `limit` (None or negative: all)."""
-        enc = [x.encode("utf-8", "surrogatepass") for x in ids]
-        n = len(enc)
-        off = np.zeros(n + 1, np.int64)
-        np.cumsum([len(b) for b in enc], out=off[1:])
-        buf = np.frombuffer(b"".join(enc), np.uint8)
+        buf, off = _str_column([x.encode("utf-8", "surrogatepass") for x in ids])
+        n = off.shape[0] - 1
         lim = -1 if limit is None else int(limit)
         count = np.zeros(max(n, 1), np.int64)
         total = C.c_int64(0)
@@ -705,11 +690,9 @@ def cooc_train(user, item, n_users, n_items, topn, device=0):
     oi = np.full((n_items, topn), -1, np.int32)
     oc = np.zeros((n_items, topn), np.int32)
     on = np.zeros(n_items, np.int32)
-    rc = lib().pio_cooc_train(C.c_int(device), _ptr(user, C.c_int32), _ptr(item, C.c_int32), C.c_int64(user.shape[0]),
-                              C.c_int32(n_users), C.c_int32(n_items), C.c_int(topn), _ptr(oi, C.c_int32),
-                              _ptr(oc, C.c_int32), _ptr(on, C.c_int32))
-    if rc != 0:
-        raise NativeError(rc, lib().pio_als_last_error(None).decode())
+    _check(lib().pio_cooc_train(C.c_int(device), _ptr(user, C.c_int32), _ptr(item, C.c_int32), C.c_int64(user.shape[0]),
+                                C.c_int32(n_users), C.c_int32(n_items), C.c_int(topn), _ptr(oi, C.c_int32),
+                                _ptr(oc, C.c_int32), _ptr(on, C.c_int32)))
     return oi, oc, on
 
 
@@ -719,10 +702,8 @@ def nb_train(label, x, n_class, lam, device=0):
     n, f = x.shape
     pi = np.zeros(n_class, np.float64)
     theta = np.zeros((n_class, f), np.float64)
-    rc = lib().pio_nb_train(C.c_int(device), _ptr(label, C.c_int32), _ptr(x, C.c_float), C.c_int64(n), C.c_int(f),
-                            C.c_int(n_class), C.c_double(lam), _ptr(pi, C.c_double), _ptr(theta, C.c_double))
-    if rc != 0:
-        raise NativeError(rc, lib().pio_als_last_error(None).decode())
+    _check(lib().pio_nb_train(C.c_int(device), _ptr(label, C.c_int32), _ptr(x, C.c_float), C.c_int64(n), C.c_int(f),
+                              C.c_int(n_class), C.c_double(lam), _ptr(pi, C.c_double), _ptr(theta, C.c_double)))
     return pi, theta
 
 
@@ -732,8 +713,6 @@ def nb_predict(x, pi, theta, device=0):
     theta = np.ascontiguousarray(theta, np.float64)
     n, f = x.shape
     out = np.zeros(n, np.int32)
-    rc = lib().pio_nb_predict(C.c_int(device), _ptr(x, C.c_float), C.c_int64(n), C.c_int(f), C.c_int(pi.shape[0]),
-                              _ptr(pi, C.c_double), _ptr(theta, C.c_double), _ptr(out, C.c_int32))
-    if rc != 0:
-        raise NativeError(rc, lib().pio_als_last_error(None).decode())
+    _check(lib().pio_nb_predict(C.c_int(device), _ptr(x, C.c_float), C.c_int64(n), C.c_int(f), C.c_int(pi.shape[0]),
+                                _ptr(pi, C.c_double), _ptr(theta, C.c_double), _ptr(out, C.c_int32)))
     return out

@@ -466,13 +466,18 @@ def take_strings(buf: np.ndarray, off: np.ndarray, idx) -> Tuple[np.ndarray, np.
     return buf[src], new_off
 
 
+def _concat_offsets(offs: Sequence[np.ndarray]) -> np.ndarray:
+    """Offset columns (each starting at 0) one after the other, each rebased to end where the previous one ends."""
+    out, base = [np.zeros(1, np.int64)], 0
+    for o in offs:
+        out.append(o[1:] + base)
+        base += int(o[-1])
+    return np.concatenate(out)
+
+
 def concat_strings(cols: Sequence[Tuple[np.ndarray, np.ndarray]]) -> Tuple[np.ndarray, np.ndarray]:
     bufs = [b for b, _ in cols]
-    offs, base = [np.zeros(1, np.int64)], 0
-    for b, o in cols:
-        offs.append(o[1:] + base)
-        base += int(o[-1])
-    return (np.concatenate(bufs) if bufs else np.zeros(0, np.uint8)), np.concatenate(offs)
+    return (np.concatenate(bufs) if bufs else np.zeros(0, np.uint8)), _concat_offsets([o for _, o in cols])
 
 
 def string_list(col: Tuple[np.ndarray, np.ndarray]) -> List[str]:
@@ -549,16 +554,13 @@ def _host_columns(lines, names, appName, entityType, eventNames, targetEntityTyp
 
 
 def _columns_from_rows(rows) -> Tuple[Dict[str, np.ndarray], Dict[int, Any]]:
+    from . import native
     enc = lambda s: s.encode("utf-8", "surrogatepass")  # noqa: E731
-    eids = [enc(r[5]) for r in rows]
-    tids = [b"" if r[6] is None else enc(r[6]) for r in rows]
     col = dict(line=np.array([r[0] for r in rows], np.int64), code=np.array([r[1] for r in rows], np.int32),
                value=np.array([r[2] for r in rows], np.float64), has_value=np.array([r[3] for r in rows], bool),
-               time_us=np.array([r[4] for r in rows], np.int64), has_target=np.array([r[6] is not None for r in rows], bool))
-    for key, ids in (("eid", eids), ("tid", tids)):
-        off = np.zeros(len(ids) + 1, np.int64)
-        np.cumsum([len(b) for b in ids], out=off[1:])
-        col[key] = (np.frombuffer(b"".join(ids), np.uint8).copy(), off)
+               time_us=np.array([r[4] for r in rows], np.int64), has_target=np.array([r[6] is not None for r in rows], bool),
+               eid=native._str_column([enc(r[5]) for r in rows]),
+               tid=native._str_column([b"" if r[6] is None else enc(r[6]) for r in rows]))
     return col, {j: r[7] for j, r in enumerate(rows) if r[7] is not _UNSET}
 
 
@@ -605,6 +607,27 @@ def _scan_file(appName, channelName, scan, chunk_bytes):
     return parts, host_lines
 
 
+def _concat_parts(parts, numeric, strings=(), offsets=()) -> Dict[str, Any]:
+    """_scan_file's per-piece results as whole-file columns: the numeric columns ({name: dtype}) concatenated, each
+    string column (name_bytes, name_off) as one (bytes, offsets) column, and each offsets-only column rebased."""
+    out = {k: np.concatenate([r[k] for r in parts]) if parts else np.zeros(0, t) for k, t in numeric.items()}
+    out.update({k: concat_strings([(r[k + "_bytes"], r[k + "_off"]) for r in parts]) for k in strings})
+    out.update({k: _concat_offsets([r[k] for r in parts]) for k in offsets})
+    return out
+
+
+def _merge_by_line(dev, host) -> Tuple[Dict[str, Any], np.ndarray]:
+    """The columns of the device scan and of the fallback lines parsed on the host, merged in line order.  `host` has
+    "line" and the columns to merge: numeric arrays or (bytes, offsets) string columns, each named as in `dev`.  Returns
+    the merged columns and `order`: merged row j is row order[j] of dev followed by host.  Without fallback rows, `dev`
+    comes back as it is, with order = arange(n)."""
+    if host["line"].shape[0] == 0:
+        return dev, np.arange(dev["line"].shape[0])
+    order = np.argsort(np.concatenate([dev["line"], host["line"]]), kind="stable")
+    return {k: take_strings(*concat_strings([dev[k], h]), order) if isinstance(h, tuple) else
+            np.concatenate([dev[k], h])[order] for k, h in host.items() if k != "line"}, order
+
+
 def _scan_args(startTime, untilTime, sc):
     s_us = None if startTime is None else time_us(_parse_time(startTime))
     u_us = None if untilTime is None else time_us(_parse_time(untilTime))
@@ -633,27 +656,19 @@ def _find_columns(appName, entityType=None, eventNames=None, targetEntityType=_U
         chunk_bytes)
     rows = _host_columns(host_lines, names, appName, entityType, eventNames, targetEntityType, property, startTime,
                          untilTime)
-    dev = dict(line=np.concatenate([r["line"] for r in parts]) if parts else np.zeros(0, np.int64))
-    for k, t in (("code", np.int32), ("value", np.float64), ("time_us", np.int64)):
-        dev[k] = np.concatenate([r[k] for r in parts]).astype(t, copy=False) if parts else np.zeros(0, t)
-    flags = np.concatenate([r["flags"] for r in parts]) if parts else np.zeros(0, np.uint8)
-    dev["has_value"] = (flags & native.EVENTS_HAS_VALUE) != 0
-    dev["has_target"] = (flags & native.EVENTS_HAS_TARGET) != 0
-    dev["eid"] = concat_strings([(r["eid_bytes"], r["eid_off"]) for r in parts])
-    dev["tid"] = concat_strings([(r["tid_bytes"], r["tid_off"]) for r in parts])
-    if not rows:
-        return EventColumns(dev["code"], dev["value"], dev["has_value"], dev["time_us"], dev["eid"], dev["tid"],
-                            dev["has_target"])
+    d = _concat_parts(parts, dict(line=np.int64, code=np.int32, value=np.float64, time_us=np.int64, flags=np.uint8),
+                      ("eid", "tid"))
+    d["has_value"] = (d["flags"] & native.EVENTS_HAS_VALUE) != 0
+    d["has_target"] = (d["flags"] & native.EVENTS_HAS_TARGET) != 0
     host, bad = _columns_from_rows(rows)
-    nd = dev["line"].shape[0]
-    order = np.argsort(np.concatenate([dev["line"], host["line"]]), kind="stable")   # merge in line order
-    cat = {k: np.concatenate([dev[k], host[k]])[order] for k in ("code", "value", "has_value", "time_us", "has_target")}
-    eid = take_strings(*concat_strings([dev["eid"], host["eid"]]), order)
-    tid = take_strings(*concat_strings([dev["tid"], host["tid"]]), order)
-    where = np.empty(order.shape[0], np.int64)
-    where[order] = np.arange(order.shape[0])
-    return EventColumns(cat["code"], cat["value"], cat["has_value"], cat["time_us"], eid, tid, cat["has_target"],
-                        {int(where[nd + j]): v for j, v in bad.items()}, len(host_lines))
+    c, order = _merge_by_line(d, host)
+    bad_value = {}
+    if bad:   # keyed by the merged event number
+        where = np.empty(order.shape[0], np.int64)
+        where[order] = np.arange(order.shape[0])
+        bad_value = {int(where[d["line"].shape[0] + j]): v for j, v in bad.items()}
+    return EventColumns(c["code"], c["value"], c["has_value"], c["time_us"], c["eid"], c["tid"], c["has_target"],
+                        bad_value, len(host_lines) if rows else 0)
 
 
 def require_values(cols: EventColumns, which: np.ndarray, name: str) -> None:
@@ -747,13 +762,9 @@ def _aggregate_property_columns(appName, entityType, keys, required, startTime, 
         lambda view: native.events_scan_keys(view, scan_keys, entityType, FOLD_EVENTS, native.EVENTS_TARGET_ANY, None,
                                              s_us, u_us, device),
         chunk_bytes)
-    cat = lambda k, t: np.concatenate([r[k] for r in parts]).astype(t, copy=False) if parts else np.zeros(0, t)  # noqa: E731
-    d_line, d_code, d_time, d_present = cat("line", np.int64), cat("code", np.int32), cat("time_us", np.int64), \
-        cat("present", np.uint8)
-    d_number = cat("number", np.uint8)
-    d_num = np.concatenate([r["num"] for r in parts]) if parts else np.zeros((0, nk))
-    d_eid = concat_strings([(r["eid_bytes"], r["eid_off"]) for r in parts])
-    d_tok = concat_strings([(r["tok_bytes"], r["tok_off"]) for r in parts])
+    d = _concat_parts(parts, dict(line=np.int64, code=np.int32, time_us=np.int64, present=np.uint8, number=np.uint8,
+                                  num=np.float64), ("eid", "tok"))
+    d_number, d_num, d_tok = d["number"], d["num"], d["tok"]
     # fallback lines: the code find runs, merged by line index
     enc = lambda x: x.encode("utf-8", "surrogatepass")  # noqa: E731
     h_line, h_code, h_time, h_present, h_eid, h_vals = [], [], [], [], [], []
@@ -765,18 +776,12 @@ def _aggregate_property_columns(appName, entityType, keys, required, startTime, 
         h_present.append(sum(1 << q for q, k in enumerate(scan_keys) if k in f))
         h_eid.append(enc(e.entityId))
         h_vals.append({q: f[k] for q, k in enumerate(scan_keys) if k in f})
-    nd = d_line.shape[0]
-    if h_line:
-        h_off = np.zeros(len(h_eid) + 1, np.int64)
-        np.cumsum([len(b) for b in h_eid], out=h_off[1:])
-        order = np.argsort(np.concatenate([d_line, np.array(h_line, np.int64)]), kind="stable")
-        code = np.concatenate([d_code, np.array(h_code, np.int32)])[order]
-        t_us = np.concatenate([d_time, np.array(h_time, np.int64)])[order]
-        present = np.concatenate([d_present, np.array(h_present, np.uint8)])[order]
-        eid = take_strings(*concat_strings([d_eid, (np.frombuffer(b"".join(h_eid), np.uint8).copy(), h_off)]), order)
-    else:
-        order, code, t_us, present, eid = np.arange(nd), d_code, d_time, d_present, d_eid
-    f = native.events_fold(eid, code, t_us, present, nk, device)
+    nd = d["line"].shape[0]
+    c, order = _merge_by_line(d, dict(line=np.array(h_line, np.int64), code=np.array(h_code, np.int32),
+                                      time_us=np.array(h_time, np.int64), present=np.array(h_present, np.uint8),
+                                      eid=native._str_column(h_eid)))
+    eid = c["eid"]
+    f = native.events_fold(eid, c["code"], c["time_us"], c["present"], nk, device)
     win = f["winner"]
     keep = f["exists"] & (win[:, len(keys):] >= 0).all(axis=1)   # required keys: present, even if null
     keep &= (win[:, [scan_keys.index(r) for r in required if r in keys]] >= 0).all(axis=1)
@@ -835,18 +840,10 @@ def _aggregate_property_maps(appName, entityType, channelName, startTime, untilT
         lambda view: native.events_scan_props(view, entityType, FOLD_EVENTS, native.EVENTS_TARGET_ANY, None, s_us,
                                               u_us, device),
         chunk_bytes)
-    cat = lambda k, t: np.concatenate([r[k] for r in parts]).astype(t, copy=False) if parts else np.zeros(0, t)  # noqa: E731
-    d_line, d_code, d_time, d_utc = cat("line", np.int64), cat("code", np.int32), cat("time_us", np.int64), \
-        cat("utc_off", np.int16)
-    d_eid = concat_strings([(r["eid_bytes"], r["eid_off"]) for r in parts])
-    d_keys = concat_strings([(r["key_bytes"], r["key_off"]) for r in parts])
-    d_toks = concat_strings([(r["tok_bytes"], r["tok_off"]) for r in parts])
-    d_prop, base = [], 0
-    for r in parts:
-        d_prop.append(r["prop_off"][:-1] + base)
-        base += int(r["prop_off"][-1])
-    d_prop = np.concatenate(d_prop + [np.array([base], np.int64)])
-    nd, nrd = d_line.shape[0], base
+    d = _concat_parts(parts, dict(line=np.int64, code=np.int32, time_us=np.int64, utc_off=np.int16),
+                      ("eid", "key", "tok"), ("prop_off",))
+    d_time, d_utc, d_toks, d_prop = d["time_us"], d["utc_off"], d["tok"], d["prop_off"]
+    nd, nrd = d["line"].shape[0], int(d_prop[-1])
     # fallback lines: the code find runs, merged by line index; their keys become records whose values stay Python objects
     enc = lambda x: x.encode("utf-8", "surrogatepass")  # noqa: E731
     h_line, h_code, h_time, h_eid, h_dt, h_items = [], [], [], [], [], []
@@ -858,24 +855,21 @@ def _aggregate_property_maps(appName, entityType, channelName, startTime, untilT
         h_dt.append(e.eventTime)
         h_items.append(list(e.properties.fields.items()))
     h_vals = [v for items in h_items for _, v in items]
+    h_cnt = np.array([len(items) for items in h_items], np.int64)
+    # each event's records (first record, count) travel with it through the merge
+    d["rec_start"], d["rec_len"] = d_prop[:-1], np.diff(d_prop)
+    c, order = _merge_by_line(d, dict(line=np.array(h_line, np.int64), code=np.array(h_code, np.int32),
+                                      time_us=np.array(h_time, np.int64), eid=native._str_column(h_eid),
+                                      rec_start=nrd + np.cumsum(h_cnt) - h_cnt, rec_len=h_cnt))
+    eid, prop_off, keys = c["eid"], d_prop, d["key"]
     rec_perm = None   # the fold's records -> records of the scan (< nrd) and of the fallback lines (>= nrd)
     if h_line:
-        col = lambda bs: (np.frombuffer(b"".join(bs), np.uint8).copy(),  # noqa: E731
-                          np.concatenate([[0], np.cumsum([len(b) for b in bs], dtype=np.int64)]).astype(np.int64))
-        h_cnt = np.array([len(items) for items in h_items], np.int64)
-        order = np.argsort(np.concatenate([d_line, np.array(h_line, np.int64)]), kind="stable")
-        code = np.concatenate([d_code, np.array(h_code, np.int32)])[order]
-        t_us = np.concatenate([d_time, np.array(h_time, np.int64)])[order]
-        eid = take_strings(*concat_strings([d_eid, col(h_eid)]), order)
-        start = np.concatenate([d_prop[:-1], nrd + np.cumsum(h_cnt) - h_cnt])[order]
-        lens = np.concatenate([np.diff(d_prop), h_cnt])[order]
         prop_off = np.zeros(order.shape[0] + 1, np.int64)
-        np.cumsum(lens, out=prop_off[1:])
-        rec_perm = np.repeat(start - prop_off[:-1], lens) + np.arange(prop_off[-1], dtype=np.int64)
-        keys = take_strings(*concat_strings([d_keys, col([enc(k) for items in h_items for k, _ in items])]), rec_perm)
-    else:
-        order, code, t_us, eid, prop_off, keys = np.arange(nd), d_code, d_time, d_eid, d_prop, d_keys
-    f = native.events_fold_props(eid, code, t_us, prop_off, keys, device)
+        np.cumsum(c["rec_len"], out=prop_off[1:])
+        rec_perm = np.repeat(c["rec_start"] - prop_off[:-1], c["rec_len"]) + np.arange(prop_off[-1], dtype=np.int64)
+        keys = take_strings(*concat_strings([keys, native._str_column([enc(k) for items in h_items for k, _ in items])]),
+                            rec_perm)
+    f = native.events_fold_props(eid, c["code"], c["time_us"], prop_off, keys, device)
 
     # the winning values: one json.loads of the scanned tokens, the fallback lines' values as they are
     rec = f["win_rec"] if rec_perm is None else rec_perm[f["win_rec"]]
