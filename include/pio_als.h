@@ -33,6 +33,8 @@
  *       examples/scala-parallel-recommendation/blacklist-items/src/main/scala/ALSModel.scala:63-100
  *   pio_nb_train / pio_nb_predict replace NaiveBayes.train / model.predict
  *       examples/scala-parallel-classification/add-algorithm/src/main/scala/NaiveBayesAlgorithm.scala:41-57
+ *   pio_rf_train / pio_rf_predict replace RandomForest.trainClassifier / model.predict
+ *       examples/scala-parallel-classification/add-algorithm/src/main/scala/RandomForestAlgorithm.scala:46-70
  */
 #ifndef PIO_ALS_H_
 #define PIO_ALS_H_
@@ -429,6 +431,49 @@ PIO_API int pio_nb_train(int device, const int32_t* label, const float* x, int64
                          int n_class, double lambda, double* pi, double* theta);
 PIO_API int pio_nb_predict(int device, const float* x, int64_t n, int n_feat, int n_class,
                            const double* pi, const double* theta, int32_t* out_label);
+
+/* MLlib 2.4 RandomForest.trainClassifier with continuous features (classification template, RandomForestAlgorithm
+ *   examples/scala-parallel-classification/add-algorithm/src/main/scala/RandomForestAlgorithm.scala:46-70).
+ * The rules, and which of them are this project's choices, are stated in tests/forest_ref.py and DESIGN.md 4.10: every
+ * random draw (split sample, bootstrap, feature subsets) is a pure function of (seed, stream, tree, index), counts are
+ * integers, and the forest does not depend on the device, launch order or how trees are grouped.
+ * Limits of this implementation (PIO_ALS_ERR_ARG): num_classes <= 64, max_bins <= 65536, n < 2^31.  Arguments, labels
+ * and features are checked on the host before any device work; a label < 0 or >= num_classes fails with the message
+ * of MLlib's GiniAggregator / EntropyAggregator, a non-finite label or feature is rejected. */
+#define PIO_RF_GINI 0
+#define PIO_RF_ENTROPY 1
+
+typedef struct pio_rf_params {
+  int32_t num_classes;                  /* >= 2 */
+  int32_t num_trees;                    /* >= 1 */
+  int32_t max_depth;                    /* 0 .. 30 */
+  int32_t max_bins;                     /* >= 2 */
+  int32_t impurity;                     /* PIO_RF_GINI / PIO_RF_ENTROPY */
+  int32_t reserved0;
+  const char* feature_subset_strategy;  /* auto | all | sqrt | log2 | onethird | integer k > 0 | fraction in (0, 1] */
+  int64_t seed;
+} pio_rf_params;
+
+typedef struct pio_rf_forest pio_rf_forest;   /* a trained forest, host memory only */
+
+/* label: n class labels (class = trunc(label)); x: n x n_feat row-major fp64 (HOST buffers). */
+PIO_API int pio_rf_train(int device, const pio_rf_params* params, const double* label, const double* x, int64_t n,
+                         int32_t n_feat, pio_rf_forest** out);
+/* The forest's size: trees and nodes over all trees (after MLlib's pruning of equal leaf pairs). */
+PIO_API int pio_rf_forest_size(const pio_rf_forest* f, int32_t* n_trees, int64_t* n_nodes);
+/* Flat per-node arrays, trees one after the other, each in preorder: tree_off [n_trees + 1] (first node of each tree),
+ * and per node: feature (-1 at a leaf), threshold (x[feature] <= threshold goes left; 0 at a leaf), left / right
+ * (indices into these arrays, -1 at a leaf), prediction (class), impurity, gain (0 at a leaf) and count (the node's
+ * bootstrap-weighted row count).  Any output pointer may be null. */
+PIO_API int pio_rf_forest_get(const pio_rf_forest* f, int32_t* tree_off, int32_t* feature, double* threshold,
+                              int32_t* left, int32_t* right, int32_t* prediction, double* impurity, double* gain,
+                              int64_t* count);
+PIO_API int pio_rf_forest_destroy(pio_rf_forest* f);
+/* The forest's majority vote (ties to the smaller class) for n rows x (n x n_feat fp64, HOST) into out (class index),
+ * from the flat arrays of pio_rf_forest_get. */
+PIO_API int pio_rf_predict(int device, int32_t n_trees, const int32_t* tree_off, int64_t n_nodes, const int32_t* feature,
+                           const double* threshold, const int32_t* left, const int32_t* right, const int32_t* prediction,
+                           int32_t num_classes, const double* x, int64_t n, int32_t n_feat, int32_t* out);
 
 #ifdef __cplusplus
 }

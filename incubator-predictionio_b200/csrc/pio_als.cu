@@ -53,6 +53,7 @@
 #include "events_fold.cuh"
 #include "events_index.cuh"
 #include "cooc.cuh"
+#include "forest.cuh"
 
 namespace pio {
 
@@ -3976,6 +3977,544 @@ int pio_nb_predict(int device, const float* x, int64_t n, int n_feat, int n_clas
   nb_predict_kernel<<<nblk(n, 256), 256>>>(dx, n, n_feat, n_class, dpi, dth, dout);
   CK0(cudaGetLastError());
   CK0(cudaMemcpy(out_label, dout, sizeof(int) * n, cudaMemcpyDeviceToHost));
+  return PIO_ALS_OK;
+}
+
+// ---- RandomForest (csrc/forest.cuh, csrc/forest_splits.h; rules: tests/forest_ref.py) ------------------------------
+struct pio_rf_forest {
+  int32_t n_trees = 0, n_class = 0;
+  std::vector<int32_t> tree_off, feature, left, right, prediction;
+  std::vector<double> threshold, impurity, gain;
+  std::vector<int64_t> count;
+};
+
+}  // extern "C"
+
+namespace pio {
+
+constexpr int64_t RF_NODE_BUDGET = 1ll << 30;   // node ids of one tree group (int32 per tree and row)
+constexpr int64_t RF_HIST_BUDGET = 1ll << 29;   // the global histogram of one chunk of a level's node slots
+constexpr int RF_SMEM = 96 * 1024;              // shared-memory histogram of one pass (two blocks per SM)
+
+// where the last pio_rf_train on this thread spent its time (wall ms; every phase ends in a stream synchronise)
+struct RfTiming {
+  double h2d = 0, split = 0, bin = 0, hist = 0, sel = 0, upd = 0;
+  int levels = 0, groups = 0;
+  double hist_l[RF_MAX_DEPTH + 1] = {}, sel_l[RF_MAX_DEPTH + 1] = {};
+};
+static thread_local RfTiming g_rf_timing;
+
+struct RfRec {
+  bool leaf;
+  int feature;
+  double thr, imp, gain;
+  int pred;
+  int64_t count;
+};
+using RfTree = std::map<int64_t, RfRec>;
+
+// a double as the error messages print it: the shortest %g that reads back, '.0' on an integral value
+static std::string rf_fmt(double v) {
+  char b[64];
+  for (int p = 1; p <= 17; ++p) {
+    snprintf(b, sizeof b, "%.*g", p, v);
+    if (strtod(b, nullptr) == v) break;
+  }
+  std::string s(b);
+  if (s.find_first_of(".en") == std::string::npos) s += ".0";
+  return s;
+}
+
+static int rf_check(const pio_rf_params* p, const double* label, const double* x, int64_t n, int F) {
+  const int C = p->num_classes;
+  if (C < 2)
+    return fail(nullptr, PIO_ALS_ERR_ARG, "DecisionTree Strategy for Classification must have numClasses >= 2, but "
+                "numClasses = %d.", C);
+  if (C > RF_MAX_CLASSES)
+    return fail(nullptr, PIO_ALS_ERR_ARG, "numClasses = %d: at most %d classes are supported.", C, RF_MAX_CLASSES);
+  if (p->num_trees < 1)
+    return fail(nullptr, PIO_ALS_ERR_ARG, "RandomForest requires numTrees > 0, but was given numTrees = %d.",
+                p->num_trees);
+  if (rf_subset_size(p->feature_subset_strategy, F > 1 ? F : 1, p->num_trees) == 0)
+    return fail(nullptr, PIO_ALS_ERR_ARG, "RandomForest given invalid featureSubsetStrategy: %s. Supported values: "
+                "auto, all, onethird, sqrt, log2, (0.0-1.0], [1-n].",
+                p->feature_subset_strategy ? p->feature_subset_strategy : "null");
+  if (p->max_depth < 0)
+    return fail(nullptr, PIO_ALS_ERR_ARG, "DecisionTree Strategy given invalid maxDepth parameter: %d.  Valid values "
+                "are integers >= 0.", p->max_depth);
+  if (p->max_depth > RF_MAX_DEPTH)
+    return fail(nullptr, PIO_ALS_ERR_ARG, "DecisionTree currently only supports maxDepth <= 30, but was given maxDepth "
+                "= %d.", p->max_depth);
+  if (p->max_bins < 2)
+    return fail(nullptr, PIO_ALS_ERR_ARG, "DecisionTree Strategy given invalid maxBins parameter: %d.  Valid values are "
+                "integers >= 2.", p->max_bins);
+  if (p->max_bins > RF_MAX_BINS)
+    return fail(nullptr, PIO_ALS_ERR_ARG, "maxBins = %d: at most %d bins are supported.", p->max_bins, RF_MAX_BINS);
+  if (p->impurity != RF_GINI && p->impurity != RF_ENTROPY)
+    return fail(nullptr, PIO_ALS_ERR_ARG, "unknown impurity code %d", p->impurity);
+  if (n < 1 || F < 1) return fail(nullptr, PIO_ALS_ERR_ARG, "RandomForest requires at least one row and one feature.");
+  if (n >= (1ll << 31)) return fail(nullptr, PIO_ALS_ERR_ARG, "at most 2^31 - 1 rows are supported.");
+  if (!label || !x) return fail(nullptr, PIO_ALS_ERR_ARG, "bad pio_rf_train arguments");
+  for (int64_t r = 0; r < n; ++r) {
+    if (!isfinite(label[r]))
+      return fail(nullptr, PIO_ALS_ERR_ARG, "label of row %lld is not finite (%s).", (long long)r,
+                  rf_fmt(label[r]).c_str());
+    for (int f = 0; f < F; ++f)
+      if (!isfinite(x[r * F + f]))
+        return fail(nullptr, PIO_ALS_ERR_ARG, "feature %d of row %lld is not finite (%s).", f, (long long)r,
+                    rf_fmt(x[r * F + f]).c_str());
+  }
+  const char* agg = p->impurity == RF_GINI ? "GiniAggregator" : "EntropyAggregator";
+  for (int64_t r = 0; r < n; ++r) {
+    if (label[r] >= C)
+      return fail(nullptr, PIO_ALS_ERR_ARG, "%s given label %s but requires label < numClasses (= %d).", agg,
+                  rf_fmt(label[r]).c_str(), C);
+    if (label[r] < 0)
+      return fail(nullptr, PIO_ALS_ERR_ARG, "%s given label %sbut requires label is non-negative.", agg,
+                  rf_fmt(label[r]).c_str());
+  }
+  return PIO_ALS_OK;
+}
+
+static double rf_ms(std::chrono::steady_clock::time_point& t0) {
+  const auto t = std::chrono::steady_clock::now();
+  const double ms = std::chrono::duration<double, std::milli>(t - t0).count();
+  t0 = t;
+  return ms;
+}
+
+// LearningNode.toNode(prune = true): an internal node whose two children end as leaves with the same prediction becomes
+// a leaf; returns the node's prediction
+static int rf_prune(RfTree& t, int64_t i) {
+  RfRec& r = t[i];
+  if (r.leaf) return r.pred;
+  const int a = rf_prune(t, 2 * i), b = rf_prune(t, 2 * i + 1);
+  if (t[2 * i].leaf && t[2 * i + 1].leaf && a == b) r.leaf = true, r.pred = a, r.feature = -1, r.thr = 0.0, r.gain = 0.0;
+  return r.pred;
+}
+// preorder: the node, its left subtree, its right subtree; returns the node's index in the flat arrays
+static int32_t rf_emit(const RfTree& t, int64_t i, pio_rf_forest* o) {
+  const RfRec& r = t.at(i);
+  const int32_t me = (int32_t)o->feature.size();
+  o->feature.push_back(r.leaf ? -1 : r.feature);
+  o->threshold.push_back(r.leaf ? 0.0 : r.thr);
+  o->left.push_back(-1);
+  o->right.push_back(-1);
+  o->prediction.push_back(r.pred);
+  o->impurity.push_back(r.imp);
+  o->gain.push_back(r.leaf ? 0.0 : r.gain);
+  o->count.push_back(r.count);
+  if (!r.leaf) {
+    const int32_t l = rf_emit(t, 2 * i, o);
+    o->left[me] = l;
+    const int32_t rr = rf_emit(t, 2 * i + 1, o);
+    o->right[me] = rr;
+  }
+  return me;
+}
+
+struct RfCtx {
+  CallMem* tmp;
+  cudaStream_t st;
+  int sm;
+  const pio_rf_params* p;
+  int64_t n;
+  int F, K, C, NB;
+  const double* dx;
+  const uint8_t* dcls;
+  const double* dthr;
+  const int* doff;
+  const int* dnthr;
+  const std::vector<std::vector<double>>* thr;
+  pio_rf_forest* out;
+};
+
+// bin codes, then every tree group level by level
+template <typename BinT>
+static int rf_bin_and_grow(const RfCtx& c) {
+  CallMem& tmp = *c.tmp;
+  const cudaStream_t st = c.st;
+  const int64_t n = c.n;
+  const int F = c.F, K = c.K, C = c.C, NB = c.NB, T = c.p->num_trees, max_depth = c.p->max_depth;
+  const int64_t seed = c.p->seed;
+  RfTiming& tm = g_rf_timing;
+  auto t0 = std::chrono::steady_clock::now();
+  BinT* dbins = nullptr;
+  CK0(tmp.device(&dbins, (size_t)n * F));
+  std::vector<int> hoff(F + 1, 0);
+  for (int f = 0; f < F; ++f) hoff[f + 1] = hoff[f] + (int)(*c.thr)[f].size();
+  const size_t thr_bytes = sizeof(double) * (size_t)hoff[F];
+  const int staged = thr_bytes <= 48 * 1024 ? 1 : 0;
+  const unsigned bgrid = (unsigned)std::min<int64_t>(nblk(n * F, rf::THREADS), (int64_t)c.sm * 16);
+  rf::bin_kernel<BinT><<<bgrid, rf::THREADS, staged ? thr_bytes : 0, st>>>(c.dx, n, F, c.dthr, c.doff, staged, dbins);
+  CK0(cudaGetLastError());
+  CK0(cudaStreamSynchronize(st));
+  tm.bin = rf_ms(t0);
+
+  const char* env = getenv("PIO_RF_TREES_PER_PASS");
+  const auto groups = rf_plan_groups(T, n, RF_NODE_BUDGET, env ? atoi(env) : 0);
+  int gmax = 0;
+  for (const auto& g : groups) gmax = std::max(gmax, g.second - g.first);
+  int* dnode = nullptr;
+  uint64_t* dbag = nullptr;
+  CK0(tmp.device(&dnode, (size_t)n * gmax));
+  CK0(tmp.device(&dbag, (size_t)gmax));
+  rf::Cdf cdf;
+  rf_poisson_table(cdf.v);
+  const int64_t slot_bytes = (int64_t)K * NB * C * 8, smem_slot = (int64_t)K * NB * C * 4;
+  const int64_t chunk_max = std::max<int64_t>(1, RF_HIST_BUDGET / slot_bytes);
+  const int64_t pass_slots = RF_SMEM / smem_slot;
+  if (pass_slots >= 1) {
+    CK0(cudaFuncSetAttribute(rf::hist_kernel<BinT, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, RF_SMEM));
+  }
+  const unsigned ugrid = (unsigned)std::min<int64_t>(nblk(n * gmax, rf::THREADS), (int64_t)c.sm * 16);
+  tm.groups = (int)groups.size();
+  for (const auto& grp : groups) {
+    const int t_first = grp.first, G = grp.second - grp.first;
+    rf::root_kernel<<<ugrid, rf::THREADS, 0, st>>>(dnode, n, G);
+    std::vector<uint64_t> hbag(G);
+    for (int g = 0; g < G; ++g) hbag[g] = rf_stream(seed, RF_TAG_BAG, (uint64_t)(t_first + g));
+    CK0(cudaMemcpyAsync(dbag, hbag.data(), 8 * (size_t)G, cudaMemcpyHostToDevice, st));
+    std::vector<RfTree> trees(G);
+    std::vector<std::pair<int, int64_t>> active;
+    for (int g = 0; g < G; ++g) active.push_back({g, 1});
+    for (int level = 0; !active.empty(); ++level) {
+      const int64_t S = (int64_t)active.size();
+      if (S >= (1ll << 31) / std::max(K, C)) return fail(nullptr, PIO_ALS_ERR_ARG, "too many nodes in one level");
+      std::vector<int> hsub((size_t)S * K);
+      for (int64_t s = 0; s < S; ++s)
+        rf_node_subset(rf_stream(seed, RF_TAG_SUBSET, (uint64_t)(t_first + active[s].first)), active[s].second, F, K,
+                       &hsub[(size_t)s * K]);
+      Scratch lv(st);
+      int *dsub = nullptr, *dbest = nullptr;
+      double* dgain = nullptr;
+      long long *dleft = nullptr, *dtot = nullptr;
+      unsigned long long* dhist = nullptr;
+      const int64_t cap = std::min<int64_t>(S, chunk_max);
+      CK0(lv.alloc(&dsub, (size_t)S * K));
+      CK0(lv.alloc(&dbest, (size_t)S * 2));
+      CK0(lv.alloc(&dgain, (size_t)S));
+      CK0(lv.alloc(&dleft, (size_t)S * C));
+      CK0(lv.alloc(&dtot, (size_t)S * C));
+      CK0(lv.alloc(&dhist, (size_t)cap * K * NB * C));
+      CK0(cudaMemcpyAsync(dsub, hsub.data(), 4 * hsub.size(), cudaMemcpyHostToDevice, st));
+      CK0(cudaStreamSynchronize(st));
+      rf_ms(t0);
+      for (int64_t c0 = 0; c0 < S; c0 += cap) {
+        const int64_t c1 = std::min(S, c0 + cap);
+        CK0(cudaMemsetAsync(dhist, 0, (size_t)(c1 - c0) * slot_bytes, st));
+        rf::HistArgs a{c.dcls, dbins, dnode, T > 1 ? dbag : nullptr, dsub, dhist, n, F, G, K, NB, C,
+                       (int)c0, (int)c1, (int)c0, active[c0].first, active[c1 - 1].first, cdf};
+        if (pass_slots >= 1) {
+          const unsigned grid = (unsigned)std::min<int64_t>(nblk(n, rf::THREADS), (int64_t)c.sm * 2);
+          for (int64_t p0 = c0; p0 < c1; p0 += pass_slots) {
+            a.s0 = (int)p0;
+            a.s1 = (int)std::min(c1, p0 + pass_slots);
+            a.g0 = active[a.s0].first;
+            a.g1 = active[a.s1 - 1].first;
+            rf::hist_kernel<BinT, true><<<grid, rf::THREADS, (size_t)(a.s1 - a.s0) * smem_slot, st>>>(a);
+          }
+        } else {
+          const unsigned grid = (unsigned)std::min<int64_t>(nblk(n, rf::THREADS), (int64_t)c.sm * 8);
+          rf::hist_kernel<BinT, false><<<grid, rf::THREADS, 0, st>>>(a);
+        }
+        CK0(cudaGetLastError());
+        CK0(cudaStreamSynchronize(st));
+        const double hm = rf_ms(t0);
+        tm.hist += hm, tm.hist_l[level] += hm;
+        rf::SelArgs sa{dhist, dsub, c.dnthr, dgain, dbest, dleft, dtot, K, NB, C, c.p->impurity, (int)c0, (int)c0};
+        rf::select_kernel<<<(unsigned)(c1 - c0), rf::SEL_WARPS * 32, 0, st>>>(sa);
+        CK0(cudaGetLastError());
+        CK0(cudaStreamSynchronize(st));
+        const double sm_ = rf_ms(t0);
+        tm.sel += sm_, tm.sel_l[level] += sm_;
+      }
+      std::vector<double> hgain(S);
+      std::vector<int> hbest(2 * S);
+      std::vector<int64_t> hleft(S * C), htot(S * C);
+      CK0(cudaMemcpyAsync(hgain.data(), dgain, 8 * (size_t)S, cudaMemcpyDeviceToHost, st));
+      CK0(cudaMemcpyAsync(hbest.data(), dbest, 8 * (size_t)S, cudaMemcpyDeviceToHost, st));
+      CK0(cudaMemcpyAsync(hleft.data(), dleft, 8 * (size_t)S * C, cudaMemcpyDeviceToHost, st));
+      CK0(cudaMemcpyAsync(htot.data(), dtot, 8 * (size_t)S * C, cudaMemcpyDeviceToHost, st));
+      CK0(cudaStreamSynchronize(st));
+      // the level's decisions (tests/forest_ref.py train): leaves, splits, children and the next level's slots
+      std::vector<int4> upd(S);
+      std::vector<std::pair<int, int64_t>> next;
+      std::vector<int64_t> cc(C);
+      for (int64_t s = 0; s < S; ++s) {
+        const int g = active[s].first;
+        const int64_t i = active[s].second;
+        const int64_t* tot = &htot[s * C];
+        int64_t cnt = 0;
+        for (int k = 0; k < C; ++k) cnt += tot[k];
+        RfRec rec{true, -1, 0.0, rf_impurity(tot, C, c.p->impurity), 0.0, rf_argmax(tot, C), cnt};
+        const int kk = hbest[2 * s];
+        if (kk < 0 || !(hgain[s] > 0.0) || level == max_depth) {
+          trees[g][i] = rec;
+          upd[s] = make_int4(-1, 0, -1, -1);
+          continue;
+        }
+        const int f = hsub[(size_t)s * K + kk], j = hbest[2 * s + 1];
+        rec.leaf = false, rec.feature = f, rec.thr = (*c.thr)[f][j], rec.gain = hgain[s];
+        trees[g][i] = rec;
+        int child_slot[2];
+        for (int side = 0; side < 2; ++side) {
+          int64_t ccount = 0;
+          for (int k = 0; k < C; ++k) {
+            cc[k] = side == 0 ? hleft[s * C + k] : tot[k] - hleft[s * C + k];
+            ccount += cc[k];
+          }
+          const double ci = rf_impurity(cc.data(), C, c.p->impurity);
+          const int64_t child = 2 * i + side;
+          if (level + 1 == max_depth || ci == 0.0) {
+            trees[g][child] = RfRec{true, -1, 0.0, ci, 0.0, rf_argmax(cc.data(), C), ccount};
+            child_slot[side] = -1;
+          } else {
+            child_slot[side] = (int)next.size();
+            next.push_back({g, child});
+          }
+        }
+        upd[s] = make_int4(f, j, child_slot[0], child_slot[1]);
+      }
+      if (!next.empty()) {
+        int4* dupd = nullptr;
+        CK0(lv.alloc(&dupd, (size_t)S));
+        CK0(cudaMemcpyAsync(dupd, upd.data(), sizeof(int4) * (size_t)S, cudaMemcpyHostToDevice, st));
+        rf::update_kernel<BinT><<<ugrid, rf::THREADS, 0, st>>>(dnode, n, G, dbins, F, dupd);
+        CK0(cudaGetLastError());
+        CK0(cudaStreamSynchronize(st));
+        tm.upd += rf_ms(t0);
+      }
+      tm.levels = std::max(tm.levels, level + 1);
+      active.swap(next);
+    }
+    for (int g = 0; g < G; ++g) {
+      rf_prune(trees[g], 1);
+      rf_emit(trees[g], 1, c.out);
+      c.out->tree_off.push_back((int32_t)c.out->feature.size());
+    }
+  }
+  return PIO_ALS_OK;
+}
+
+}  // namespace pio
+
+extern "C" {
+
+int pio_rf_train(int device, const pio_rf_params* p, const double* label, const double* x, int64_t n, int32_t n_feat,
+                 pio_rf_forest** out) {
+  if (!p || !out) return fail(nullptr, PIO_ALS_ERR_ARG, "bad pio_rf_train arguments");
+  *out = nullptr;
+  const int rc = rf_check(p, label, x, n, n_feat);
+  if (rc != PIO_ALS_OK) return rc;
+  const int F = n_feat, C = p->num_classes, K = rf_subset_size(p->feature_subset_strategy, F, p->num_trees);
+  g_rf_timing = RfTiming();
+  RfTiming& tm = g_rf_timing;
+  auto t0 = std::chrono::steady_clock::now();
+  CK0(cudaSetDevice(device));
+  int sm = 0;
+  CK0(cudaDeviceGetAttribute(&sm, cudaDevAttrMultiProcessorCount, device));
+  std::vector<uint8_t> hcls((size_t)n);
+  for (int64_t r = 0; r < n; ++r) hcls[r] = (uint8_t)(int)trunc(label[r]);
+  CallMem tmp;
+  cudaStream_t st;
+  CK0(tmp.stream(&st));
+  double* dx = nullptr;
+  uint8_t* dcls = nullptr;
+  CK0(tmp.device(&dx, (size_t)n * F));
+  CK0(tmp.device(&dcls, (size_t)n));
+  rf_ms(t0);
+  CK0(cudaMemcpyAsync(dx, x, sizeof(double) * (size_t)n * F, cudaMemcpyHostToDevice, st));
+  CK0(cudaMemcpyAsync(dcls, hcls.data(), (size_t)n, cudaMemcpyHostToDevice, st));
+  CK0(cudaStreamSynchronize(st));
+  tm.h2d = rf_ms(t0);
+
+  // split sample, then per feature its sorted distinct values: thresholds on the host (findSplitsForContinuousFeature)
+  const double frac = rf_sample_fraction(n, p->max_bins);
+  uint32_t* rows = nullptr;
+  int64_t m = n;
+  if (frac < 1.0) {
+    uint32_t *flag = nullptr, *pos = nullptr;
+    CK0(tmp.device(&flag, (size_t)n));
+    CK0(tmp.device(&pos, (size_t)n));
+    rf::sample_flag_kernel<<<nblk(n, 256), 256, 0, st>>>(n, rf_stream(p->seed, RF_TAG_SAMPLE, 0), frac, flag);
+    CK0(scan_exclusive_u32(flag, pos, (size_t)n, st, nullptr));
+    uint32_t lf = 0, lp = 0;
+    CK0(cudaMemcpyAsync(&lf, flag + n - 1, 4, cudaMemcpyDeviceToHost, st));
+    CK0(cudaMemcpyAsync(&lp, pos + n - 1, 4, cudaMemcpyDeviceToHost, st));
+    CK0(cudaStreamSynchronize(st));
+    m = (int64_t)lp + lf;
+    CK0(tmp.device(&rows, (size_t)m));
+    rf::sample_compact_kernel<<<nblk(n, 256), 256, 0, st>>>(flag, pos, n, rows);
+    CK0(cudaGetLastError());
+  }
+  std::vector<std::vector<double>> thr(F);
+  if (m > 0) {
+    SortBufs sb;
+    uint32_t *head = nullptr, *rpos = nullptr, *rstart = nullptr;
+    uint64_t* rkey = nullptr;
+    for (int i : {0, 1}) {
+      CK0(tmp.device(&sb.k[i], (size_t)m));
+      CK0(tmp.device(&sb.v[i], (size_t)m));
+    }
+    CK0(tmp.device(&head, (size_t)m));
+    CK0(tmp.device(&rpos, (size_t)m));
+    CK0(tmp.device(&rkey, (size_t)m));
+    CK0(tmp.device(&rstart, (size_t)m));
+    std::vector<uint64_t> hk;
+    std::vector<uint32_t> hs;
+    std::vector<double> vals;
+    std::vector<int64_t> cnts;
+    for (int f = 0; f < F; ++f) {
+      sb.live = 0;
+      rf::sample_keys_kernel<<<nblk(m, 256), 256, 0, st>>>(dx, F, f, rows, m, sb.keys(), sb.vals());
+      CK0(radix_sort_pairs(sb, (size_t)m, 64, st, nullptr));
+      rf::run_head_kernel<<<nblk(m, 256), 256, 0, st>>>(sb.keys(), m, head);
+      CK0(scan_exclusive_u32(head, rpos, (size_t)m, st, nullptr));
+      rf::run_compact_kernel<<<nblk(m, 256), 256, 0, st>>>(sb.keys(), head, rpos, m, rkey, rstart);
+      CK0(cudaGetLastError());
+      uint32_t lh = 0, lp = 0;
+      CK0(cudaMemcpyAsync(&lh, head + m - 1, 4, cudaMemcpyDeviceToHost, st));
+      CK0(cudaMemcpyAsync(&lp, rpos + m - 1, 4, cudaMemcpyDeviceToHost, st));
+      CK0(cudaStreamSynchronize(st));
+      const int64_t runs = (int64_t)lp + lh;
+      hk.resize(runs);
+      hs.resize(runs);
+      CK0(cudaMemcpyAsync(hk.data(), rkey, 8 * (size_t)runs, cudaMemcpyDeviceToHost, st));
+      CK0(cudaMemcpyAsync(hs.data(), rstart, 4 * (size_t)runs, cudaMemcpyDeviceToHost, st));
+      CK0(cudaStreamSynchronize(st));
+      vals.resize(runs);
+      cnts.resize(runs);
+      for (int64_t i = 0; i < runs; ++i) {
+        const uint64_t b = (hk[i] >> 63) ? (hk[i] & ~(1ull << 63)) : ~hk[i];
+        memcpy(&vals[i], &b, 8);
+        cnts[i] = (i + 1 < runs ? (int64_t)hs[i + 1] : m) - (int64_t)hs[i];
+      }
+      rf_thresholds(vals.data(), cnts.data(), runs, std::min<int64_t>(p->max_bins, n), thr[f]);
+    }
+  }
+  std::vector<double> hthr;
+  std::vector<int> hoff(F + 1, 0), hnthr(F);
+  for (int f = 0; f < F; ++f) {
+    hthr.insert(hthr.end(), thr[f].begin(), thr[f].end());
+    hnthr[f] = (int)thr[f].size();
+    hoff[f + 1] = (int)hthr.size();
+  }
+  const int NB = *std::max_element(hnthr.begin(), hnthr.end()) + 1;
+  double* dthr = nullptr;
+  int *doff = nullptr, *dnthr = nullptr;
+  CK0(tmp.device(&dthr, hthr.size()));
+  CK0(tmp.device(&doff, (size_t)F + 1));
+  CK0(tmp.device(&dnthr, (size_t)F));
+  if (!hthr.empty())
+    CK0(cudaMemcpyAsync(dthr, hthr.data(), 8 * hthr.size(), cudaMemcpyHostToDevice, st));
+  CK0(cudaMemcpyAsync(doff, hoff.data(), 4 * hoff.size(), cudaMemcpyHostToDevice, st));
+  CK0(cudaMemcpyAsync(dnthr, hnthr.data(), 4 * hnthr.size(), cudaMemcpyHostToDevice, st));
+  CK0(cudaStreamSynchronize(st));
+  tm.split = rf_ms(t0);
+
+  pio_rf_forest* fo = new pio_rf_forest();
+  fo->n_trees = p->num_trees;
+  fo->n_class = C;
+  fo->tree_off.push_back(0);
+  RfCtx ctx{&tmp, st, sm, p, n, F, K, C, NB, dx, dcls, dthr, doff, dnthr, &thr, fo};
+  const int rc2 = NB <= 256 ? rf_bin_and_grow<uint8_t>(ctx) : rf_bin_and_grow<uint16_t>(ctx);
+  if (rc2 != PIO_ALS_OK) {
+    delete fo;
+    return rc2;
+  }
+  *out = fo;
+  return PIO_ALS_OK;
+}
+
+int pio_rf_forest_size(const pio_rf_forest* f, int32_t* n_trees, int64_t* n_nodes) {
+  if (!f) return fail(nullptr, PIO_ALS_ERR_ARG, "null forest");
+  if (n_trees) *n_trees = f->n_trees;
+  if (n_nodes) *n_nodes = (int64_t)f->feature.size();
+  return PIO_ALS_OK;
+}
+
+int pio_rf_forest_get(const pio_rf_forest* f, int32_t* tree_off, int32_t* feature, double* threshold, int32_t* left,
+                      int32_t* right, int32_t* prediction, double* impurity, double* gain, int64_t* count) {
+  if (!f) return fail(nullptr, PIO_ALS_ERR_ARG, "null forest");
+  auto put = [](auto* dst, const auto& v) {
+    if (dst && !v.empty()) memcpy(dst, v.data(), v.size() * sizeof(v[0]));
+  };
+  put(tree_off, f->tree_off);
+  put(feature, f->feature);
+  put(threshold, f->threshold);
+  put(left, f->left);
+  put(right, f->right);
+  put(prediction, f->prediction);
+  put(impurity, f->impurity);
+  put(gain, f->gain);
+  put(count, f->count);
+  return PIO_ALS_OK;
+}
+
+int pio_rf_forest_destroy(pio_rf_forest* f) {
+  delete f;
+  return PIO_ALS_OK;
+}
+
+int pio_rf_predict(int device, int32_t n_trees, const int32_t* tree_off, int64_t n_nodes, const int32_t* feature,
+                   const double* threshold, const int32_t* left, const int32_t* right, const int32_t* prediction,
+                   int32_t num_classes, const double* x, int64_t n, int32_t n_feat, int32_t* out) {
+  if (!tree_off || !feature || !threshold || !left || !right || !prediction || !out || n_trees < 1 || n_nodes < 1 ||
+      n_nodes >= (1ll << 31) || num_classes < 1 || num_classes > RF_MAX_CLASSES || n_feat < 1 || n < 0 || (n > 0 && !x))
+    return fail(nullptr, PIO_ALS_ERR_ARG, "bad pio_rf_predict arguments");
+  // a walk must end: children come after their parent (preorder) and stay in their tree
+  for (int32_t t = 0; t < n_trees; ++t) {
+    const int64_t a = tree_off[t], b = t + 1 < n_trees ? tree_off[t + 1] : n_nodes;
+    if (a < 0 || a >= b || b > n_nodes) return fail(nullptr, PIO_ALS_ERR_ARG, "bad tree offsets");
+    for (int64_t i = a; i < b; ++i) {
+      if (prediction[i] < 0 || prediction[i] >= num_classes) return fail(nullptr, PIO_ALS_ERR_ARG, "bad prediction");
+      if (feature[i] >= n_feat) return fail(nullptr, PIO_ALS_ERR_ARG, "node %lld uses feature %d of %d", (long long)i,
+                                            feature[i], n_feat);
+      if (feature[i] >= 0 && (left[i] <= i || left[i] >= b || right[i] <= i || right[i] >= b))
+        return fail(nullptr, PIO_ALS_ERR_ARG, "bad children at node %lld", (long long)i);
+    }
+  }
+  if (n == 0) return PIO_ALS_OK;
+  CK0(cudaSetDevice(device));
+  CallMem tmp;
+  cudaStream_t st;
+  CK0(tmp.stream(&st));
+  int *dto = nullptr, *df = nullptr, *dl = nullptr, *dr = nullptr, *dp = nullptr, *dout = nullptr;
+  double *dt = nullptr, *dx = nullptr;
+  CK0(tmp.device(&dto, (size_t)n_trees));
+  CK0(tmp.device(&df, (size_t)n_nodes));
+  CK0(tmp.device(&dl, (size_t)n_nodes));
+  CK0(tmp.device(&dr, (size_t)n_nodes));
+  CK0(tmp.device(&dp, (size_t)n_nodes));
+  CK0(tmp.device(&dt, (size_t)n_nodes));
+  CK0(tmp.device(&dx, (size_t)n * n_feat));
+  CK0(tmp.device(&dout, (size_t)n));
+  CK0(cudaMemcpyAsync(dto, tree_off, 4 * (size_t)n_trees, cudaMemcpyHostToDevice, st));
+  CK0(cudaMemcpyAsync(df, feature, 4 * (size_t)n_nodes, cudaMemcpyHostToDevice, st));
+  CK0(cudaMemcpyAsync(dl, left, 4 * (size_t)n_nodes, cudaMemcpyHostToDevice, st));
+  CK0(cudaMemcpyAsync(dr, right, 4 * (size_t)n_nodes, cudaMemcpyHostToDevice, st));
+  CK0(cudaMemcpyAsync(dp, prediction, 4 * (size_t)n_nodes, cudaMemcpyHostToDevice, st));
+  CK0(cudaMemcpyAsync(dt, threshold, 8 * (size_t)n_nodes, cudaMemcpyHostToDevice, st));
+  CK0(cudaMemcpyAsync(dx, x, 8 * (size_t)n * n_feat, cudaMemcpyHostToDevice, st));
+  rf::predict_kernel<<<nblk(n, 128), 128, sizeof(int) * 128 * (size_t)num_classes, st>>>(
+      dto, n_trees, df, dt, dl, dr, dp, num_classes, dx, n, n_feat, dout);
+  CK0(cudaGetLastError());
+  CK0(cudaMemcpyAsync(out, dout, 4 * (size_t)n, cudaMemcpyDeviceToHost, st));
+  CK0(cudaStreamSynchronize(st));
+  return PIO_ALS_OK;
+}
+
+/* debug only (not in pio_als.h): where the last pio_rf_train on this thread spent its time, wall ms of phases that each
+ * end in a stream synchronise: out[0] host-to-device copy, [1] split search, [2] binning, [3] histograms, [4] split
+ * selection, [5] node update, [6] levels, [7] tree groups, [8 + l] histograms of level l, [39 + l] selection of level l
+ * (l < 31).  Used by tools/forest_bench.py. */
+__attribute__((visibility("default"))) int pio_rf_debug_timing(double out[70]) {
+  if (!out) return PIO_ALS_ERR_ARG;
+  const RfTiming& t = g_rf_timing;
+  out[0] = t.h2d, out[1] = t.split, out[2] = t.bin, out[3] = t.hist, out[4] = t.sel, out[5] = t.upd;
+  out[6] = t.levels, out[7] = t.groups;
+  for (int l = 0; l <= RF_MAX_DEPTH; ++l) out[8 + l] = t.hist_l[l], out[39 + l] = t.sel_l[l];
   return PIO_ALS_OK;
 }
 

@@ -8,6 +8,8 @@ Same names and argument meaning as the MLlib API the templates call (SURVEY 8(b)
     MatrixFactorizationModel(rank, userFeatures, productFeatures): recommendProducts, predict
     NaiveBayes.train(labeledPoints, lambda) / NaiveBayesModel.predict
         (examples/scala-parallel-classification/add-algorithm/src/main/scala/NaiveBayesAlgorithm.scala:41-57)
+    RandomForest.trainClassifier(...) / RandomForestModel.predict
+        (examples/scala-parallel-classification/add-algorithm/src/main/scala/RandomForestAlgorithm.scala:46-70)
 
 Ratings are COO arrays (user:int32, product:int32, rating:float32) -- the RDD[Rating(Int,Int,Double)]
 the templates build at ALSAlgorithm.scala:62-65 -- and everything below is one call through the C ABI
@@ -180,3 +182,68 @@ class NaiveBayes:
         classes, idx = np.unique(labels, return_inverse=True)                     # sorted ascending, as MLlib
         pi, theta = native.nb_train(idx.astype(np.int32), x, classes.shape[0], lambda_, device)
         return NaiveBayesModel(classes, pi, theta, device)
+
+
+class RandomForestModel:
+    """A trained classification forest as flat per-node numpy arrays (native.rf_train's dict), so that a pickle of the
+    model is the model.  Trees are stored one after the other, each in preorder; `tree_off[t]` is tree t's root."""
+
+    def __init__(self, numClasses: int, nodes: dict, device: int = 0):
+        self.numClasses = int(numClasses)
+        self.nodes = {k: np.asarray(v) for k, v in nodes.items()}
+        self.device = device
+
+    @property
+    def numTrees(self) -> int:
+        return int(self.nodes["tree_off"].shape[0] - 1)
+
+    @property
+    def totalNumNodes(self) -> int:
+        return int(self.nodes["feature"].shape[0])
+
+    @property
+    def numNodes(self) -> np.ndarray:
+        """Nodes of each tree."""
+        return np.diff(self.nodes["tree_off"])
+
+    @property
+    def depth(self) -> np.ndarray:
+        """Depth of each tree (a single leaf: 0)."""
+        feat, left, right = self.nodes["feature"], self.nodes["left"], self.nodes["right"]
+        d = np.zeros(feat.shape[0], np.int32)
+        for i in range(feat.shape[0]):          # preorder: a parent comes before its children
+            if feat[i] >= 0:
+                d[left[i]] = d[right[i]] = d[i] + 1
+        off = self.nodes["tree_off"]
+        return np.array([int(d[off[t]:off[t + 1]].max()) for t in range(self.numTrees)], np.int32)
+
+    def predict(self, features) -> float:
+        return float(self.predictBatch(np.asarray(features, np.float64).reshape(1, -1))[0])
+
+    def predictBatch(self, x: np.ndarray) -> np.ndarray:
+        """The forest's majority vote per row, as float labels; on the device."""
+        return native.rf_predict(self.nodes, self.numClasses, np.asarray(x, np.float64), self.device).astype(np.float64)
+
+
+class RandomForest:
+    IMPURITIES = {"gini": native.RF_GINI, "entropy": native.RF_ENTROPY}
+
+    @staticmethod
+    def trainClassifier(labels, features, numClasses: int, categoricalFeaturesInfo, numTrees: int,
+                        featureSubsetStrategy: str, impurity: str, maxDepth: int, maxBins: int, seed: int = 0,
+                        device: int = 0) -> RandomForestModel:
+        """MLlib's 8-argument RandomForest.trainClassifier (continuous features only) plus an explicit seed; the rules are
+        those of tests/forest_ref.py.  labels: n float labels (class = trunc(label)); features: n x F, trained in fp64.
+        Bad arguments and labels raise ValueError with MLlib's messages before any device work."""
+        if impurity not in RandomForest.IMPURITIES:
+            raise ValueError(f"Did not recognize Impurity name: {impurity}")
+        if categoricalFeaturesInfo:
+            raise ValueError("categoricalFeaturesInfo must be empty: categorical features are not supported")
+        try:
+            nodes = native.rf_train(labels, features, numClasses, numTrees, featureSubsetStrategy,
+                                    RandomForest.IMPURITIES[impurity], maxDepth, maxBins, seed, device)
+        except native.NativeError as e:
+            if e.code != native.ERR_ARG:
+                raise
+            raise ValueError(native.lib().pio_als_last_error(None).decode()) from None
+        return RandomForestModel(numClasses, nodes, device)

@@ -35,7 +35,8 @@ EXPORTED_SYMBOLS = [
     "pio_events_scan", "pio_events_scan_keys", "pio_events_fold", "pio_events_scan_props", "pio_events_fold_props",
     "pio_events_index_create",
     "pio_events_index_append", "pio_events_index_add_host", "pio_events_index_lookup", "pio_events_index_get_stats",
-    "pio_events_index_destroy",
+    "pio_events_index_destroy", "pio_rf_train", "pio_rf_forest_size", "pio_rf_forest_get", "pio_rf_forest_destroy",
+    "pio_rf_predict",
 ]
 
 
@@ -705,6 +706,69 @@ def nb_train(label, x, n_class, lam, device=0):
     _check(lib().pio_nb_train(C.c_int(device), _ptr(label, C.c_int32), _ptr(x, C.c_float), C.c_int64(n), C.c_int(f),
                               C.c_int(n_class), C.c_double(lam), _ptr(pi, C.c_double), _ptr(theta, C.c_double)))
     return pi, theta
+
+
+RF_GINI, RF_ENTROPY = 0, 1
+RF_FOREST_INT = ("feature", "left", "right", "prediction")
+RF_FOREST_F64 = ("threshold", "impurity", "gain")
+
+
+class RfParams(C.Structure):
+    _fields_ = [("num_classes", C.c_int32), ("num_trees", C.c_int32), ("max_depth", C.c_int32),
+                ("max_bins", C.c_int32), ("impurity", C.c_int32), ("reserved0", C.c_int32),
+                ("feature_subset_strategy", C.c_char_p), ("seed", C.c_int64)]
+
+
+def rf_train(label, x, num_classes, num_trees, strategy, impurity, max_depth, max_bins, seed=0, device=0):
+    """pio_rf_train: a RandomForest classifier (impurity RF_GINI / RF_ENTROPY) as a dict of flat per-node arrays:
+    tree_off (int32 [num_trees + 1]), feature, left, right, prediction (int32), threshold, impurity, gain (float64) and
+    count (int64)."""
+    label = np.ascontiguousarray(label, np.float64)
+    x = np.ascontiguousarray(x, np.float64)
+    if x.ndim != 2 or label.shape != (x.shape[0],):
+        raise ValueError("x must be n x n_feat and label must have n entries")
+    p = RfParams(num_classes=int(num_classes), num_trees=int(num_trees), max_depth=int(max_depth),
+                 max_bins=int(max_bins), impurity=int(impurity), feature_subset_strategy=str(strategy).encode("utf-8"),
+                 seed=int(seed))
+    h = C.c_void_p()
+    _check(lib().pio_rf_train(C.c_int(device), C.byref(p), _ptr(label, C.c_double), _ptr(x, C.c_double),
+                              C.c_int64(x.shape[0]), C.c_int32(x.shape[1]), C.byref(h)))
+    try:
+        nt, nn = C.c_int32(0), C.c_int64(0)
+        _check(lib().pio_rf_forest_size(h, C.byref(nt), C.byref(nn)))
+        out = {"tree_off": np.empty(nt.value + 1, np.int32), "count": np.empty(nn.value, np.int64)}
+        out.update({k: np.empty(nn.value, np.int32) for k in RF_FOREST_INT})
+        out.update({k: np.empty(nn.value, np.float64) for k in RF_FOREST_F64})
+        _check(lib().pio_rf_forest_get(h, *_addrs(out, "tree_off", "feature", "threshold", "left", "right", "prediction",
+                                                  "impurity", "gain", "count")))
+    finally:
+        lib().pio_rf_forest_destroy(h)
+    return out
+
+
+def rf_predict(forest, num_classes, x, device=0):
+    """pio_rf_predict: the forest's vote (class index, int32 [n]) for the rows of x (n x n_feat)."""
+    x = np.ascontiguousarray(x, np.float64)
+    a = {k: np.ascontiguousarray(forest[k], np.int32) for k in ("tree_off", *RF_FOREST_INT)}
+    thr = np.ascontiguousarray(forest["threshold"], np.float64)
+    n = x.shape[0]
+    out = np.empty(n, np.int32)
+    vp = C.c_void_p
+    _check(lib().pio_rf_predict(C.c_int(device), C.c_int32(a["tree_off"].shape[0] - 1), vp(_addr(a["tree_off"])),
+                                C.c_int64(thr.shape[0]), vp(_addr(a["feature"])), vp(_addr(thr)), vp(_addr(a["left"])),
+                                vp(_addr(a["right"])), vp(_addr(a["prediction"])), C.c_int32(num_classes), vp(_addr(x)),
+                                C.c_int64(n), C.c_int32(x.shape[1]), vp(_addr(out))))
+    return out
+
+
+def rf_train_timing() -> dict:
+    """Where the last rf_train on this thread spent its time (wall ms of phases that each end in a device synchronise)."""
+    out = (C.c_double * 70)()
+    _check(lib().pio_rf_debug_timing(out))
+    levels = int(out[6])
+    return {"h2d_ms": out[0], "split_ms": out[1], "bin_ms": out[2], "hist_ms": out[3], "select_ms": out[4],
+            "update_ms": out[5], "levels": levels, "groups": int(out[7]),
+            "hist_level_ms": list(out[8:8 + levels]), "select_level_ms": list(out[39:39 + levels])}
 
 
 def nb_predict(x, pi, theta, device=0):
