@@ -647,11 +647,15 @@ als_finish_ls128_kernel(const SolveParams p, const int* __restrict__ row_part_pt
         if (o < LL::SIZE / 4) reinterpret_cast<float4*>(slot)[o] = s;
         else reinterpret_cast<float4*>(bv)[o - LL::SIZE / 4] = s;
       }
+      if (IMPLICIT) {
+        __syncwarp();
+        ls_add_yty<128>(slot, p.yty);
+      }
     }
     __syncthreads();
     if (have)
-      chol_lockstep<128, IMPLICIT>(slot, bv, p.yty, p.lambda * p.nreg[r], p.k, colbuf,
-                                   p.dst + (size_t)(p.dst_row_offset + r) * 128, true, p.fail);
+      chol_lockstep<128>(slot, bv, p.lambda * p.nreg[r], p.k, colbuf, p.dst + (size_t)(p.dst_row_offset + r) * 128, true,
+                         p.fail);
     __syncthreads();
   }
 }

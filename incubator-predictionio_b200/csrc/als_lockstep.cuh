@@ -49,16 +49,39 @@ __device__ __forceinline__ float ls_rsqrt(float x) {
   return r;
 }
 
-// Solves (A + [YtY] + ridge I) x = b for the matrix of this lane's group.
-//   slot   : this group's matrix in LsLayout<N> (lower triangle of sum c y y^T); destroyed (L is written over it)
+// slot += YtY on the lower triangle (yty: N x N row-major, global), by all 32 lanes.  Implicit feedback adds YtY once
+// per matrix where the slot is filled from parts, so that the solver's panel loads stay in shared memory.
+template <int N>
+__device__ __forceinline__ void ls_add_yty(float* __restrict__ slot, const float* __restrict__ yty) {
+  using LL = LsLayout<N>;
+  const int lane = threadIdx.x & 31;
+  for (int o = lane; o < LL::NOFF * 64; o += 32) {     // off-diagonal blocks, one 16-byte piece of a row per step
+    const int b = o >> 6, rr = (o >> 2) & 15, cg = o & 3;
+    int rb = 1;
+    while (rb * (rb + 1) / 2 <= b) ++rb;               // block b = rb (rb - 1) / 2 + cb
+    const int cb = b - rb * (rb - 1) / 2;
+    float4* d = reinterpret_cast<float4*>(slot + LL::offd_base(rb, cb) + rr * 16 + 4 * (cg ^ LL::swz(rr)));
+    const float4 y = __ldg(reinterpret_cast<const float4*>(yty + (size_t)(16 * rb + rr) * N + 16 * cb + 4 * cg));
+    float4 v = *d;
+    v.x += y.x; v.y += y.y; v.z += y.z; v.w += y.w;
+    *d = v;
+  }
+  for (int o = lane; o < LL::NBK * 256; o += 32) {     // diagonal blocks, c <= r
+    const int rb = o >> 8, rr = (o >> 4) & 15, cc = o & 15;
+    if (cc <= rr) slot[LL::diag(rb, rr, cc)] += __ldg(yty + (size_t)(16 * rb + rr) * N + 16 * rb + cc);
+  }
+}
+
+// Solves (A + ridge I) x = b for the matrix of this lane's group.
+//   slot   : this group's matrix in LsLayout<N> (lower triangle; implicit feedback: sum c y y^T + YtY); destroyed (L is
+//            written over it)
 //   bvec   : this group's right-hand side (N floats, shared memory)
-//   yty    : N x N row-major (global, implicit only); ridge = lambda * n; dimensions >= k get a unit diagonal
+//   ridge  : lambda * n; dimensions >= k get a unit diagonal
 //   colbuf : this group's pivot line, 2 x 32 floats of shared memory
 //   dst_row: N floats (global); written only if `valid` (a warp whose second matrix is a dummy still runs the code)
 // All 32 lanes must call it together.
-template <int N, bool IMPLICIT>
-__device__ __forceinline__ void chol_lockstep(float* __restrict__ slot, const float* __restrict__ bvec,
-                                              const float* __restrict__ yty, float ridge, int k,
+template <int N>
+__device__ __forceinline__ void chol_lockstep(float* __restrict__ slot, const float* __restrict__ bvec, float ridge, int k,
                                               float* __restrict__ colbuf, float* __restrict__ dst_row, bool valid,
                                               int* __restrict__ fail) {
   using LL = LsLayout<N>;
@@ -110,14 +133,6 @@ __device__ __forceinline__ void chol_lockstep(float* __restrict__ slot, const fl
         for (int cg = 0; cg < 4; ++cg) {
           const float4 v = *reinterpret_cast<const float4*>(rowp + 4 * (cg ^ sw));
           a[i][4 * cg + 0] = v.x; a[i][4 * cg + 1] = v.y; a[i][4 * cg + 2] = v.z; a[i][4 * cg + 3] = v.w;
-        }
-      }
-      if (IMPLICIT) {
-        const float4* yr = reinterpret_cast<const float4*>(yty + (size_t)r * N + 16 * p);
-#pragma unroll
-        for (int cg = 0; cg < 4; ++cg) {
-          const float4 v = __ldg(yr + cg);
-          a[i][4 * cg + 0] += v.x; a[i][4 * cg + 1] += v.y; a[i][4 * cg + 2] += v.z; a[i][4 * cg + 3] += v.w;
         }
       }
       if (i == sp) {

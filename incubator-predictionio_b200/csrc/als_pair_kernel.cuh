@@ -119,10 +119,12 @@ __device__ __forceinline__ void split2(float a, float b, uint32_t& hi, uint32_t&
   lo = *reinterpret_cast<const uint32_t*>(&l);
 }
 
-// Accumulates sum c1 y y^T (lower triangle, slot layout) and b of ratings [beg, end) into `slot` / `bv`.
+// Accumulates sum c1 y y^T (lower triangle, slot layout) and b of ratings [beg, end) into `slot` / `bv`; a non-null
+// `yty` (N x N row-major, global) is added to the lower triangle as the accumulators are written out.
 template <bool IMPLICIT>
 __device__ __forceinline__ void accumulate_row(const SolveParams& p, long long beg, long long end, float s, float unscale,
-                                               float* ring, float* mval, float* slot, float* bv) {
+                                               const float* __restrict__ yty, float* ring, float* mval, float* slot,
+                                               float* bv) {
   const int lane = threadIdx.x & 31;
   const int g = lane >> 2, t = lane & 3;
   const int nchunks = 2 * (int)((end - beg + 2 * CH - 1) / (2 * CH));   // whole steps; the last chunk may be all zero
@@ -255,8 +257,9 @@ __device__ __forceinline__ void accumulate_row(const SolveParams& p, long long b
       v += __shfl_xor_sync(0xffffffffu, v, 2);
       if (t == 0) bv[16 * i + 8 * e + g] = v;
     }
-  // ---- accumulators -> slot layout, the scale s^2 taken out (exact: a power of two) ---------------------------------------
+  // ---- accumulators -> slot layout, the scale s^2 taken out (exact: a power of two), YtY added ------------------------
   {
+    const float* yl = yty ? yty + g * KP + 2 * t : nullptr;   // YtY(16 i + g (+ 8), 8 j + 2 t (+ 1))
     int tile = 0;
 #pragma unroll
     for (int i = 0; i < 4; ++i) {
@@ -264,8 +267,14 @@ __device__ __forceinline__ void accumulate_row(const SolveParams& p, long long b
       for (int j = 0; j <= 2 * i + 1; ++j, ++tile) {
         const int cb = j >> 1;
         const int cc = 8 * (j & 1) + 2 * t;           // column inside the 16-wide block (even)
-        const float d0 = acc[tile][0] * unscale, d1 = acc[tile][1] * unscale;
-        const float d2 = acc[tile][2] * unscale, d3 = acc[tile][3] * unscale;
+        float d0 = acc[tile][0] * unscale, d1 = acc[tile][1] * unscale;
+        float d2 = acc[tile][2] * unscale, d3 = acc[tile][3] * unscale;
+        if (yl) {
+          const float2 y0 = __ldg(reinterpret_cast<const float2*>(yl + 16 * i * KP + 8 * j));
+          const float2 y1 = __ldg(reinterpret_cast<const float2*>(yl + (16 * i + 8) * KP + 8 * j));
+          d0 += y0.x; d1 += y0.y;
+          d2 += y1.x; d3 += y1.y;
+        }
         if (cb < i) {
           // off-diagonal block: two 8-byte stores (rows g and g + 8 of the block)
           *reinterpret_cast<float2*>(slot + LL::offd(i, cb, g, cc)) = make_float2(d0, d1);
@@ -342,7 +351,8 @@ __global__ void __launch_bounds__(32 * WARPS, 12 / WARPS) als_solve_pair_kernel(
           if (h) row1 = r;
           else row0 = r;
         }
-        accumulate_row<IMPLICIT>(p, beg, end, s, unscale, ring, mval, slot, bv);
+        // a part carries no YtY: the finish kernel adds it once to the sum of the parts
+        accumulate_row<IMPLICIT>(p, beg, end, s, unscale, IMPLICIT && !p.partial ? p.yty : nullptr, ring, mval, slot, bv);
         if (p.partial) {
           // part of a long row: emit the partial normal equation (slot layout + b); als_finish_pair_kernel sums and solves
           float* out = p.partial + (size_t)item * PART_FLOATS;
@@ -358,8 +368,8 @@ __global__ void __launch_bounds__(32 * WARPS, 12 / WARPS) als_solve_pair_kernel(
     if (pair < npairs) {
       const int myrow = grp ? row1 : row0;
       const int rr = myrow < 0 ? p.row_begin : myrow;
-      chol_lockstep<KP, IMPLICIT>(grp ? slot1 : slot0, bvec + grp * VSTR, p.yty, p.lambda * p.nreg[rr], p.k,
-                                  colbuf + grp * VSTR, p.dst + (size_t)(p.dst_row_offset + rr) * KP, myrow >= 0, p.fail);
+      chol_lockstep<KP>(grp ? slot1 : slot0, bvec + grp * VSTR, p.lambda * p.nreg[rr], p.k, colbuf + grp * VSTR,
+                        p.dst + (size_t)(p.dst_row_offset + rr) * KP, myrow >= 0, p.fail);
       __syncwarp();
     }
   }
@@ -398,12 +408,16 @@ __global__ void __launch_bounds__(32, 12) als_finish_pair_kernel(const SolvePara
         else reinterpret_cast<float4*>(bv)[o - LL::SIZE / 4] = s;
       }
       __syncwarp();
+      if (IMPLICIT) {
+        ls_add_yty<KP>(slot, p.yty);
+        __syncwarp();
+      }
     }
     const int myrow = 2 * pair + grp;
     const bool valid = myrow < n_rows;
     const int rr = valid ? myrow : 0;
-    chol_lockstep<KP, IMPLICIT>(smem + grp * SLOT_STRIDE, bvec + grp * VSTR, p.yty, p.lambda * p.nreg[rr], p.k,
-                                colbuf + grp * VSTR, p.dst + (size_t)(p.dst_row_offset + rr) * KP, valid, p.fail);
+    chol_lockstep<KP>(smem + grp * SLOT_STRIDE, bvec + grp * VSTR, p.lambda * p.nreg[rr], p.k, colbuf + grp * VSTR,
+                      p.dst + (size_t)(p.dst_row_offset + rr) * KP, valid, p.fail);
     __syncwarp();
   }
 }

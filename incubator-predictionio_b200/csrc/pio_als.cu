@@ -2540,8 +2540,8 @@ __global__ void __launch_bounds__(32) lockstep_probe_kernel(const float* __restr
       }
       __syncwarp();
       const int mine = base + grp;
-      chol_lockstep<N, false>(sm + grp * LL::STRIDE, bvec + grp * (N > 64 ? N : 80), nullptr, ridge, N, colbuf + grp * 80,
-                              x + (size_t)(mine < n ? mine : 0) * N, mine < n, fail);
+      chol_lockstep<N>(sm + grp * LL::STRIDE, bvec + grp * (N > 64 ? N : 80), ridge, N, colbuf + grp * 80,
+                       x + (size_t)(mine < n ? mine : 0) * N, mine < n, fail);
       __syncwarp();
     }
   }
