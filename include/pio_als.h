@@ -115,6 +115,10 @@ typedef struct pio_als_stats {
 #define PIO_ALS_PATH_COS_BATCHED 0x20  /* long single similar query, query vectors in shared memory */
 #define PIO_ALS_PATH_COS_FALLBACK 0x40 /* long single similar query too large for shared memory */
 #define PIO_ALS_PATH_MULTI_PASS 0x80   /* more than one pass of <= 128 results (topk > 128) */
+/* further bits of last_score_path that only the filtered calls set (pio_als_recommend_filtered /
+ * pio_als_similar_batch_filtered); the PIO_ALS_PATH_* kernels above are the same for filtered and plain calls */
+#define PIO_ALS_FPATH_FILTERED 0x100   /* a batch kernel ran with the per-query filter test at its pool insertion */
+#define PIO_ALS_FPATH_LISTED 0x200     /* white-listed queries were scored over their lists (score_listed_kernel) */
 
 PIO_API int pio_als_abi_version(void);
 /* number of visible sm_90 devices, or PIO_ALS_ERR_CUDA */
@@ -201,6 +205,39 @@ PIO_API int pio_als_similar(pio_als_handle* h, const int32_t* query_items, int n
 PIO_API int pio_als_similar_batch(pio_als_handle* h, const int64_t* q_ptr, const int32_t* q_items, int n_queries,
                                   int topk, const uint8_t* item_mask, const double* item_weight, int flags,
                                   int32_t* out_items, float* out_scores, int32_t* out_count);
+
+/* Per-query filters of a batch scoring call: what every template query carries (blackList, whiteList, categories, the
+ * user's seen items; examples/scala-parallel-similarproduct/multi-events-multi-algos/src/main/scala/ALSAlgorithm.scala:
+ * 236-262, examples/scala-parallel-ecommercerecommendation/train-with-rate-event/src/main/scala/ECommAlgorithm.scala:
+ * 527-575).  Every pointer is HOST memory and nullable. */
+typedef struct pio_als_query_filter {
+  const int64_t* ex_ptr;    /* n_queries + 1: query j excludes ex_items[ex_ptr[j] .. ex_ptr[j+1]) */
+  const int32_t* ex_items;  /* item ids in any order; duplicates, ids < 0 or >= n_items are ignored */
+  const uint8_t* has_wl;    /* n_queries: 1 = query j has a white list (an empty one means no candidate) */
+  const int64_t* wl_ptr;    /* n_queries + 1 */
+  const int32_t* wl_items;  /* same id rules as ex_items */
+  const int32_t* set_ix;    /* n_queries: row of item_sets that applies to query j, or -1 */
+  const uint8_t* item_sets; /* n_sets x n_items bytes, 1 = not a candidate (category filters; queries share rows) */
+  int32_t n_sets;
+} pio_als_query_filter;
+
+/* pio_als_recommend / pio_als_similar_batch with a filter per query.  Row j of the result is, bit for bit, what the
+ * unfiltered call returns for query j alone with the dense mask
+ *   item_mask | item_sets[set_ix[j]] | (ex list of j) | (complement of the wl list of j, if has_wl[j])
+ * and the same item_weight / flags.  f == NULL or a filter of null pointers is the unfiltered call.  Queries without a
+ * white list scan the item matrix in the batch kernels, which test a candidate against its query's set row and sorted
+ * exclusion list only when it is about to enter a top-k pool; white-listed queries are scored over their lists, at a
+ * cost that follows the list length (DESIGN.md 4.6).  ex_ptr / wl_ptr not non-decreasing, a missing list where its
+ * ptr array says one is read, set_ix outside [-1, n_sets), n_sets < 0 or rows without item_sets: PIO_ALS_ERR_ARG
+ * before any device work. */
+PIO_API int pio_als_recommend_filtered(pio_als_handle* h, const int32_t* users, int n, int topk,
+                                       const uint8_t* item_mask, const double* item_weight,
+                                       const pio_als_query_filter* f, int32_t* out_items, float* out_scores,
+                                       int32_t* out_count);
+PIO_API int pio_als_similar_batch_filtered(pio_als_handle* h, const int64_t* q_ptr, const int32_t* q_items,
+                                           int n_queries, int topk, const uint8_t* item_mask,
+                                           const double* item_weight, int flags, const pio_als_query_filter* f,
+                                           int32_t* out_items, float* out_scores, int32_t* out_count);
 
 /* A scoring handle from factors held by the caller (HOST, row-major n x rank; has flags nullable = every row owns a
  * factor): what ALSModel.apply / a P2LAlgorithm's driver-local Map[Int, Array[Double]] model becomes on the device

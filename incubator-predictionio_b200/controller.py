@@ -188,6 +188,11 @@ class BaseAlgorithm:
     def batchPredictBase(self, sc, model, qs):
         return self.batchPredict(model, qs)
 
+    def predictMany(self, model, queries) -> list:
+        """Predictions of many queries: element j equals predict(model, queries[j]).  Algorithms whose scoring runs on
+        the device override it with a few batched calls that carry every query's own filter."""
+        return [self.predict(model, q) for q in queries]
+
     def queryClass(self):
         """Type used to decode a JSON query (BaseAlgorithm.queryClass)."""
         hints = typing.get_type_hints(self.predict)

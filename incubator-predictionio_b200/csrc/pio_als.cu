@@ -1928,17 +1928,35 @@ static int run_passes(pio_als_handle* h, const ScorePlan& p, int n_queries, int 
   return PIO_ALS_OK;
 }
 
+// f(std::true_type / std::false_type): the filtered or the plain instantiation of a batch kernel
+template <class F>
+static int with_filt(bool filtered, F&& f) {
+  return filtered ? f(std::true_type()) : f(std::false_type());
+}
+// the per-query filter of chunk c: the call's filter, numbered from the chunk's first query
+static QueryFilterDev chunk_filter(const QueryFilterDev* qf, const Chunk& c) {
+  QueryFilterDev q;
+  if (qf) q = *qf;
+  q.qbase = c.q0;
+  return q;
+}
 // the recommend kernel of the plan for the users of chunk c (xq / valid: the gathered user vectors)
 static int launch_dot(pio_als_handle* h, const ScorePlan& p, const Chunk& c, const float* d_xq, const uint8_t* d_valid,
-                      const DevFilter& f) {
+                      const DevFilter& f, const QueryFilterDev* qf = nullptr) {
   const float* xq = d_xq + (size_t)c.q0 * h->KP;
-  if (p.kernel == PIO_ALS_PATH_DOT_BLOCKED)
-    return with_kp(h->KP, [&](auto kp) {
-      return score_launch(h, score_dot_blocked_kernel<decltype(kp)::value>, c.grid, dim3(p.threads), p.smem, p.kernel, h->I.F,
-                          h->I.n_internal, xq, d_valid + c.q0, c.nq, h->I.cand_ext, f.mask, f.weight, c.pk, c.cand);
-    });
-  return score_launch(h, score_dot_topk_batched_kernel, c.grid, dim3(p.threads), p.smem, p.kernel, h->I.F, h->I.n_internal,
-                      h->KP, xq, d_valid + c.q0, c.nq, h->I.cand_ext, f.mask, f.weight, c.bound, c.pk, c.cand);
+  const QueryFilterDev q = chunk_filter(qf, c);
+  return with_filt(p.filtered, [&](auto filt) {
+    constexpr bool FILT = decltype(filt)::value;
+    if (p.kernel == PIO_ALS_PATH_DOT_BLOCKED)
+      return with_kp(h->KP, [&](auto kp) {
+        return score_launch(h, score_dot_blocked_kernel<decltype(kp)::value, FILT>, c.grid, dim3(p.threads), p.smem,
+                            p.launch_bits(), h->I.F, h->I.n_internal, xq, d_valid + c.q0, c.nq, h->I.cand_ext, f.mask, f.weight,
+                            c.pk, c.cand, q);
+      });
+    return score_launch(h, score_dot_topk_batched_kernel<FILT>, c.grid, dim3(p.threads), p.smem, p.launch_bits(), h->I.F,
+                        h->I.n_internal, h->KP, xq, d_valid + c.q0, c.nq, h->I.cand_ext, f.mask, f.weight, c.bound, c.pk, c.cand,
+                        q);
+  });
 }
 
 // the query vectors of a similar batch on the device: the vectors (qf), the first query (q0, bins only) and the first
@@ -1954,16 +1972,22 @@ struct CosQueries {
   int keep;   // PIO_ALS_SIM_KEEP_QUERY_ITEMS
 };
 // the batch similar kernel of the plan for the bins / groups of chunk c
-static int launch_cos(pio_als_handle* h, const ScorePlan& p, const Chunk& c, const CosQueries& q, const DevFilter& f) {
-  if (p.kernel == PIO_ALS_PATH_COS_BLOCKED)
-    return with_kp(h->KP, [&](auto kp) {
-      return score_launch(h, score_cos_blocked_kernel<decltype(kp)::value>, c.grid, dim3(p.threads), p.smem, p.kernel, h->I.F,
-                          h->I.n_internal, h->cfg.rank, q.qf, q.q0 + (size_t)c.g0 * DB_WPR, q.v0 + (size_t)c.g0 * DB_WPR,
-                          q.n_bins - c.g0 * DB_WPR, q.vq, q.qptr, q.qid, h->I.cand_ext, f.mask, f.weight, q.keep, c.pk, c.cand);
-    });
-  return score_launch(h, score_cos_topk_multi_kernel, c.grid, dim3(p.threads), p.smem, p.kernel, h->I.F, h->I.n_internal,
-                      h->KP, h->cfg.rank, q.qf, q.v0 + c.g0, q.vq, q.qptr + c.q0, q.qid, c.nq, h->I.cand_ext, f.mask, f.weight,
-                      c.bound, q.keep, c.pk, c.cand);
+static int launch_cos(pio_als_handle* h, const ScorePlan& p, const Chunk& c, const CosQueries& q, const DevFilter& f,
+                      const QueryFilterDev* qf = nullptr) {
+  const QueryFilterDev qd = chunk_filter(qf, c);   // bins carry the call's query numbers: their chunks start at query 0
+  return with_filt(p.filtered, [&](auto filt) {
+    constexpr bool FILT = decltype(filt)::value;
+    if (p.kernel == PIO_ALS_PATH_COS_BLOCKED)
+      return with_kp(h->KP, [&](auto kp) {
+        return score_launch(h, score_cos_blocked_kernel<decltype(kp)::value, FILT>, c.grid, dim3(p.threads), p.smem,
+                            p.launch_bits(), h->I.F, h->I.n_internal, h->cfg.rank, q.qf, q.q0 + (size_t)c.g0 * DB_WPR,
+                            q.v0 + (size_t)c.g0 * DB_WPR, q.n_bins - c.g0 * DB_WPR, q.vq, q.qptr, q.qid, h->I.cand_ext, f.mask,
+                            f.weight, q.keep, c.pk, c.cand, qd);
+      });
+    return score_launch(h, score_cos_topk_multi_kernel<FILT>, c.grid, dim3(p.threads), p.smem, p.launch_bits(), h->I.F,
+                        h->I.n_internal, h->KP, h->cfg.rank, q.qf, q.v0 + c.g0, q.vq, q.qptr + c.q0, q.qid, c.nq, h->I.cand_ext,
+                        f.mask, f.weight, c.bound, q.keep, c.pk, c.cand, qd);
+  });
 }
 
 // R2: n <= SB_QB users, topk <= TK_MAXK, in the serving arenas: three launches and one synchronisation
@@ -2116,7 +2140,7 @@ static int serve_one(pio_als_handle* h, const ScorePlan& p, bool cos, const int3
 static int similar_groups(pio_als_handle* h, const ScorePlan& p, const std::vector<int>& q0, const int64_t* q_ptr,
                           int n_queries, int topk, const std::vector<uint8_t>& valid, const float* d_qf_all,
                           const int* d_qid, const DevFilter& f, int flags, Scratch& tmp, int32_t* out_items,
-                          float* out_scores, int32_t* out_count) {
+                          float* out_scores, int32_t* out_count, const QueryFilterDev* qf = nullptr) {
   cudaStream_t st = h->stream;
   const int KP = h->KP;
   const bool bins = p.kernel == PIO_ALS_PATH_COS_BLOCKED;
@@ -2161,7 +2185,7 @@ static int similar_groups(pio_als_handle* h, const ScorePlan& p, const std::vect
   int rc = alloc_results(h, tmp, n_queries, topk, p.passes > 1, &o);
   if (rc) return rc;
   const CosQueries q{d_qfc, d_q0, d_v0, (int)q0.size() - 1, d_vq, d_qptr, d_qid, (flags & PIO_ALS_SIM_KEEP_QUERY_ITEMS) ? 1 : 0};
-  rc = run_passes(h, p, n_queries, topk, d_cand, o, [&](const Chunk& c) { return launch_cos(h, p, c, q, f); });
+  rc = run_passes(h, p, n_queries, topk, d_cand, o, [&](const Chunk& c) { return launch_cos(h, p, c, q, f, qf); });
   if (rc) return rc;
   return deliver(h, o, n_queries, topk, out_items, out_scores, out_count);
 }
@@ -2215,6 +2239,305 @@ static int similar_one(pio_als_handle* h, const int32_t* query_items, int nq, in
   rc = deliver(h, o, 1, topk, out_items, out_scores, &cnt);
   if (rc) return rc;
   if (out_count) *out_count = cnt;
+  return PIO_ALS_OK;
+}
+
+// ---- filtered batch calls (pio_als_query_filter) -------------------------------------------------------------------------
+// one key per list entry: (query of the entry << 32) | item id; thread t finds its query in ptr (the last j with ptr[j] <= t)
+__global__ void qf_keys_kernel(const int* __restrict__ items, const long long* __restrict__ ptr, int nq, long long total,
+                               unsigned long long* __restrict__ keys) {
+  const long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (t >= total) return;
+  int lo = 0, hi = nq;
+  while (hi - lo > 1) {
+    const int mid = (lo + hi) >> 1;
+    if (ptr[mid] <= t) lo = mid;
+    else hi = mid;
+  }
+  keys[t] = ((unsigned long long)(unsigned)lo << 32) | (unsigned)items[t];
+}
+// item_sets rows (one byte per item) -> one bit per item, `words` 32-bit words per row
+__global__ void qf_pack_sets_kernel(const uint8_t* __restrict__ sets, int n_items, int words, long long n_words,
+                                    unsigned* __restrict__ bits) {
+  const long long w = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (w >= n_words) return;
+  const uint8_t* row = sets + (size_t)(w / words) * n_items;
+  const int i0 = (int)(w % words) * 32;
+  unsigned v = 0;
+  for (int b = 0; b < 32 && i0 + b < n_items; ++b)
+    if (row[i0 + b]) v |= 1u << b;
+  bits[w] = v;
+}
+
+// the argument rules of a filter for n queries (pio_als.h); nullptr = fine, else what is wrong
+static const char* query_filter_error(const pio_als_query_filter* f, int n) {
+  if (f->n_sets < 0) return "query filter: n_sets < 0";
+  const struct { const int64_t* ptr; const int32_t* items; const char* order; const char* missing; } lists[2] = {
+      {f->ex_ptr, f->ex_items, "query filter: ex_ptr must be non-negative and non-decreasing", "query filter: ex_ptr names entries but ex_items is NULL"},
+      {f->wl_ptr, f->wl_items, "query filter: wl_ptr must be non-negative and non-decreasing", "query filter: wl_ptr names entries but wl_items is NULL"}};
+  for (const auto& l : lists) {
+    if (!l.ptr) continue;
+    if (l.ptr[0] < 0) return l.order;
+    for (int j = 0; j < n; ++j)
+      if (l.ptr[j + 1] < l.ptr[j]) return l.order;
+    if (l.ptr[n] > l.ptr[0] && !l.items) return l.missing;
+  }
+  if (f->set_ix)
+    for (int j = 0; j < n; ++j) {
+      if (f->set_ix[j] < -1 || f->set_ix[j] >= f->n_sets) return "query filter: set_ix must be -1 or a row of item_sets";
+      if (f->set_ix[j] >= 0 && !f->item_sets) return "query filter: set_ix names a row but item_sets is NULL";
+    }
+  return nullptr;
+}
+
+// the lists ptr / items of the queries idx on the device, as sorted keys; the queries are renumbered 0 .. idx.size() - 1
+struct DevLists {
+  const unsigned long long* keys = nullptr;
+  long long* ptr = nullptr;
+};
+static int upload_lists(pio_als_handle* h, const int64_t* ptr, const int32_t* items, const std::vector<int>& idx, Scratch& tmp,
+                        DevLists* out) {
+  cudaStream_t st = h->stream;
+  const int n = (int)idx.size();
+  std::vector<long long> rel((size_t)n + 1, 0);
+  for (int i = 0; i < n; ++i) rel[i + 1] = rel[i] + (ptr ? ptr[idx[i] + 1] - ptr[idx[i]] : 0);
+  const long long total = rel[n];
+  CK(h, tmp.alloc(&out->ptr, rel.size()));
+  CK(h, cudaMemcpyAsync(out->ptr, rel.data(), sizeof(long long) * rel.size(), cudaMemcpyHostToDevice, st));
+  if (total == 0) return PIO_ALS_OK;
+  std::vector<int> flat((size_t)total);
+  for (int i = 0; i < n; ++i)
+    if (rel[i + 1] > rel[i]) memcpy(flat.data() + rel[i], items + ptr[idx[i]], sizeof(int) * (size_t)(rel[i + 1] - rel[i]));
+  int* d_items = nullptr;
+  SortBufs sb;
+  CK(h, tmp.alloc(&d_items, (size_t)total));
+  for (int b = 0; b < 2; ++b) {
+    CK(h, tmp.alloc(&sb.k[b], (size_t)total));
+    CK(h, tmp.alloc(&sb.v[b], (size_t)total));
+  }
+  CK(h, cudaMemcpyAsync(d_items, flat.data(), sizeof(int) * (size_t)total, cudaMemcpyHostToDevice, st));
+  const int rc = score_launch(h, qf_keys_kernel, dim3(nblk(total, 256)), dim3(256), 0, 0, (const int*)d_items,
+                              (const long long*)out->ptr, n, total, (unsigned long long*)sb.k[0]);
+  if (rc) return rc;
+  CK(h, cudaMemsetAsync(sb.v[0], 0, sizeof(uint32_t) * (size_t)total, st));   // the sort carries a payload; none is needed
+  CK(h, radix_sort_pairs(sb, (size_t)total, 32 + ceil_log2((uint64_t)n), st, &h->st.kernel_launches));
+  out->keys = (const unsigned long long*)sb.keys();
+  return PIO_ALS_OK;
+}
+
+// what every part of a filtered call shares on the device: the dense mask / weights and the set rows as bits
+struct CallFilter {
+  DevFilter dense;
+  unsigned* set_bits = nullptr;
+  int set_words = 0;
+};
+static int upload_call_filter(pio_als_handle* h, const uint8_t* item_mask, const double* item_weight,
+                              const pio_als_query_filter* f, Scratch& tmp, CallFilter* out) {
+  int rc = upload_filter(h, item_mask, item_weight, &tmp, 0, &out->dense);
+  if (rc) return rc;
+  if (!f->set_ix || f->n_sets == 0 || !f->item_sets) return PIO_ALS_OK;
+  const int n_items = h->I.n;
+  out->set_words = (n_items + 31) / 32;
+  const long long n_words = (long long)f->n_sets * out->set_words;
+  uint8_t* d_sets = nullptr;
+  CK(h, tmp.alloc(&d_sets, (size_t)f->n_sets * n_items));
+  CK(h, tmp.alloc(&out->set_bits, (size_t)n_words));
+  CK(h, cudaMemcpyAsync(d_sets, f->item_sets, (size_t)f->n_sets * n_items, cudaMemcpyHostToDevice, h->stream));
+  return score_launch(h, qf_pack_sets_kernel, dim3(nblk(n_words, 256)), dim3(256), 0, 0, (const uint8_t*)d_sets, n_items,
+                      out->set_words, n_words, out->set_bits);
+}
+// the exclusion lists and set rows of the queries idx (renumbered 0 .. idx.size() - 1)
+static int upload_part_filter(pio_als_handle* h, const pio_als_query_filter* f, const CallFilter& cf,
+                              const std::vector<int>& idx, Scratch& tmp, QueryFilterDev* out) {
+  if (f->ex_ptr) {
+    DevLists ex;
+    const int rc = upload_lists(h, f->ex_ptr, f->ex_items, idx, tmp, &ex);
+    if (rc) return rc;
+    out->ex = ex.keys;
+    out->ex_ptr = ex.ptr;
+  }
+  if (cf.set_bits) {
+    std::vector<int> six(idx.size());
+    for (size_t i = 0; i < idx.size(); ++i) six[i] = f->set_ix[idx[i]];
+    int* d_six = nullptr;
+    CK(h, tmp.alloc(&d_six, six.size()));
+    CK(h, cudaMemcpyAsync(d_six, six.data(), sizeof(int) * six.size(), cudaMemcpyHostToDevice, h->stream));
+    out->set_ix = d_six;
+    out->set_bits = cf.set_bits;
+    out->set_words = cf.set_words;
+  }
+  return PIO_ALS_OK;
+}
+
+// host rows of a part's results, and their way back to the rows idx of the caller's arrays
+struct PartOut {
+  std::vector<int32_t> items, count;
+  std::vector<float> scores;
+  PartOut(size_t n, int topk) : items(n * topk), count(n), scores(n * topk) {}
+  void scatter(const std::vector<int>& idx, int topk, int32_t* out_items, float* out_scores, int32_t* out_count) const {
+    for (size_t i = 0; i < idx.size(); ++i) {
+      memcpy(out_items + (size_t)idx[i] * topk, items.data() + i * topk, sizeof(int32_t) * topk);
+      memcpy(out_scores + (size_t)idx[i] * topk, scores.data() + i * topk, sizeof(float) * topk);
+      if (out_count) out_count[idx[i]] = count[i];
+    }
+  }
+};
+
+// the users idx of a filtered recommend call: scanned by R3 / R4 with the filter test, or (listed) scored over their
+// white lists
+static int recommend_part(pio_als_handle* h, const int32_t* users, const std::vector<int>& idx, bool listed, int topk,
+                          const pio_als_query_filter* f, const CallFilter& cf, int32_t* out_items, float* out_scores,
+                          int32_t* out_count) {
+  const int n = (int)idx.size();
+  if (n == 0) return PIO_ALS_OK;
+  cudaStream_t st = h->stream;
+  const int KP = h->KP;
+  Scratch tmp(st);
+  std::vector<int> sub((size_t)n);
+  for (int i = 0; i < n; ++i) sub[i] = users[idx[i]];
+  const ScorePlan p = listed ? plan_listed(n, topk) : plan_recommend_filtered(score_env(h), n, topk);
+  int* d_users = nullptr;
+  float* d_xq = nullptr;
+  uint8_t* d_valid = nullptr;
+  ScoreIdx* d_cand = nullptr;
+  CK(h, tmp.alloc(&d_users, (size_t)n));
+  CK(h, tmp.alloc(&d_xq, (size_t)n * KP));
+  CK(h, tmp.alloc(&d_valid, (size_t)n));
+  CK(h, tmp.alloc(&d_cand, (size_t)n * p.lists * p.pass_k));
+  MergeOut o;
+  int rc = alloc_results(h, tmp, n, topk, p.passes > 1, &o);
+  if (rc) return rc;
+  CK(h, cudaMemcpyAsync(d_users, sub.data(), sizeof(int) * n, cudaMemcpyHostToDevice, st));
+  rc = score_launch(h, gather_rows_kernel, dim3(n), dim3(64), 0, 0, h->U.F, KP, (const int*)d_users, n, h->U.perm, h->U.deg,
+                    h->U.n, d_xq, d_valid);
+  if (rc) return rc;
+  QueryFilterDev qf;
+  rc = upload_part_filter(h, f, cf, idx, tmp, &qf);
+  if (rc) return rc;
+  if (listed) {
+    DevLists wl;
+    rc = upload_lists(h, f->wl_ptr, f->wl_items, idx, tmp, &wl);
+    if (rc) return rc;
+    rc = run_passes(h, p, n, topk, d_cand, o, [&](const Chunk& c) {
+      return score_launch(h, score_listed_kernel<false>, c.grid, dim3(p.threads), p.smem, p.launch_bits(), h->I.F, KP, h->I.perm,
+                          h->I.deg, h->I.n, (const float*)d_xq, (const uint8_t*)d_valid, (const long long*)nullptr,
+                          (const int*)nullptr, wl.keys, (const long long*)wl.ptr, cf.dense.mask, cf.dense.weight, c.bound, 0, c.pk,
+                          c.cand, chunk_filter(&qf, c));
+    });
+  } else {
+    rc = run_passes(h, p, n, topk, d_cand, o,
+                    [&](const Chunk& c) { return launch_dot(h, p, c, d_xq, d_valid, cf.dense, &qf); });
+  }
+  if (rc) return rc;
+  PartOut po((size_t)n, topk);
+  rc = deliver(h, o, n, topk, po.items.data(), po.scores.data(), po.count.data());
+  if (rc) return rc;
+  po.scatter(idx, topk, out_items, out_scores, out_count);
+  return PIO_ALS_OK;
+}
+
+// the queries idx of a filtered similar call.  sp / flat: their id lists, renumbered and concatenated.
+static int similar_part(pio_als_handle* h, const std::vector<int64_t>& sp, const std::vector<int32_t>& flat,
+                        const std::vector<int>& idx, bool listed, int topk, const uint8_t* item_mask,
+                        const pio_als_query_filter* f, const CallFilter& cf, int flags, int32_t* out_items, float* out_scores,
+                        int32_t* out_count) {
+  const int n = (int)idx.size();
+  if (n == 0) return PIO_ALS_OK;
+  cudaStream_t st = h->stream;
+  const ScoreEnv env = score_env(h);
+  const long long total = sp[n];
+  Scratch tmp(st);
+  PartOut po((size_t)n, topk);
+  QueryFilterDev qf;
+  int rc = PIO_ALS_OK;
+  const ScorePlan first = listed ? plan_listed(n, topk) : plan_similar_filtered(n, total, topk);
+  bool done = false;
+  if (listed || first.route == ROUTE_BATCH) {
+    if (total >= (1ll << 31)) return fail(h, PIO_ALS_ERR_ARG, "white-listed queries with 2^31 or more query items in all");
+    rc = upload_part_filter(h, f, cf, idx, tmp, &qf);
+    if (rc) return rc;
+    // all query item vectors in one gather (zeros for an id without a factor)
+    int* d_qid = nullptr;
+    float* d_qf_all = nullptr;
+    uint8_t* d_valid = nullptr;
+    CK(h, tmp.alloc(&d_qid, (size_t)total));
+    CK(h, tmp.alloc(&d_qf_all, (size_t)total * h->KP));
+    CK(h, tmp.alloc(&d_valid, (size_t)total));
+    if (total > 0) {
+      CK(h, cudaMemcpyAsync(d_qid, flat.data(), sizeof(int) * total, cudaMemcpyHostToDevice, st));
+      rc = score_launch(h, gather_rows_kernel, dim3((unsigned)total), dim3(64), 0, 0, h->I.F, h->KP, (const int*)d_qid,
+                        (int)total, h->I.perm, h->I.deg, h->I.n, d_qf_all, d_valid);
+      if (rc) return rc;
+    }
+    if (listed) {
+      DevLists wl;
+      rc = upload_lists(h, f->wl_ptr, f->wl_items, idx, tmp, &wl);
+      if (rc) return rc;
+      std::vector<long long> rel(sp.begin(), sp.end());
+      long long* d_qptr = nullptr;
+      ScoreIdx* d_cand = nullptr;
+      CK(h, tmp.alloc(&d_qptr, rel.size()));
+      CK(h, cudaMemcpyAsync(d_qptr, rel.data(), sizeof(long long) * rel.size(), cudaMemcpyHostToDevice, st));
+      CK(h, tmp.alloc(&d_cand, (size_t)n * first.lists * first.pass_k));
+      MergeOut o;
+      rc = alloc_results(h, tmp, n, topk, first.passes > 1, &o);
+      if (rc) return rc;
+      const int keep = (flags & PIO_ALS_SIM_KEEP_QUERY_ITEMS) ? 1 : 0;
+      rc = run_passes(h, first, n, topk, d_cand, o, [&](const Chunk& c) {
+        return score_launch(h, score_listed_kernel<true>, c.grid, dim3(first.threads), first.smem, first.launch_bits(), h->I.F,
+                            h->KP, h->I.perm, h->I.deg, h->I.n, (const float*)d_qf_all, (const uint8_t*)nullptr,
+                            (const long long*)d_qptr, (const int*)d_qid, wl.keys, (const long long*)wl.ptr, cf.dense.mask,
+                            cf.dense.weight, c.bound, keep, c.pk, c.cand, chunk_filter(&qf, c));
+      });
+      if (rc) return rc;
+      rc = deliver(h, o, n, topk, po.items.data(), po.scores.data(), po.count.data());
+      if (rc) return rc;
+      done = true;
+    } else {
+      std::vector<uint8_t> valid((size_t)total);
+      CK(h, cudaMemcpyAsync(valid.data(), d_valid, (size_t)total, cudaMemcpyDeviceToHost, st));
+      CK(h, cudaStreamSynchronize(st));
+      std::vector<int> nvalid((size_t)n, 0), q0;
+      for (int j = 0; j < n; ++j)
+        for (long long t = sp[j]; t < sp[j + 1]; ++t) nvalid[j] += valid[(size_t)t] ? 1 : 0;
+      ScorePlan b = plan_similar_batch(env, nvalid, topk, &q0);
+      if (b.route == ROUTE_BATCH) {
+        b.filtered = true;
+        rc = similar_groups(h, b, q0, sp.data(), n, topk, valid, d_qf_all, d_qid, cf.dense, flags, tmp, po.items.data(),
+                            po.scores.data(), po.count.data(), &qf);
+        if (rc) return rc;
+        done = true;
+      }
+    }
+  }
+  if (!done) {
+    // S5, one query at a time: the kernels of long single queries take a dense mask, so the query's filter becomes one
+    const size_t ni = (size_t)h->I.n;
+    std::vector<uint8_t> m(ni);
+    uint8_t* d_m = nullptr;
+    CK(h, tmp.alloc(&d_m, ni));
+    for (int j = 0; j < n; ++j) {
+      const int qj = idx[j];
+      if (item_mask) memcpy(m.data(), item_mask, ni);
+      else memset(m.data(), 0, ni);
+      if (f->set_ix && f->set_ix[qj] >= 0) {
+        const uint8_t* row = f->item_sets + (size_t)f->set_ix[qj] * ni;
+        for (size_t i = 0; i < ni; ++i) m[i] |= row[i] ? 1 : 0;
+      }
+      if (f->ex_ptr)
+        for (int64_t t = f->ex_ptr[qj]; t < f->ex_ptr[qj + 1]; ++t)
+          if (f->ex_items[t] >= 0 && (size_t)f->ex_items[t] < ni) m[f->ex_items[t]] = 1;
+      CK(h, cudaMemcpyAsync(d_m, m.data(), ni, cudaMemcpyHostToDevice, st));
+      DevFilter fj;
+      fj.mask = d_m;
+      fj.weight = cf.dense.weight;
+      rc = similar_one(h, flat.data() + sp[j], (int)(sp[j + 1] - sp[j]), topk, fj, flags, po.items.data() + (size_t)j * topk,
+                       po.scores.data() + (size_t)j * topk, &po.count[j]);
+      if (rc) return rc;
+      CK(h, cudaStreamSynchronize(st));   // m is rewritten for the next query
+    }
+  }
+  po.scatter(idx, topk, out_items, out_scores, out_count);
   return PIO_ALS_OK;
 }
 }  // namespace pio
@@ -2336,6 +2659,72 @@ int pio_als_similar(pio_als_handle* h, const int32_t* query_items, int nq, int t
   }
   const int64_t ptr[2] = {0, nq};
   return pio_als_similar_batch(h, ptr, query_items, 1, topk, item_mask, item_weight, flags, out_items, out_scores, out_count);
+}
+
+// Filtered batch calls: the white-listed queries are scored over their lists, the others scanned with the per-query test
+// at the pool insertion (score_plan.h); both parts write the caller's rows.
+static bool no_query_filter(const pio_als_query_filter* f) { return !f || (!f->ex_ptr && !f->has_wl && !f->set_ix); }
+
+int pio_als_recommend_filtered(pio_als_handle* h, const int32_t* users, int n, int topk, const uint8_t* item_mask,
+                               const double* item_weight, const pio_als_query_filter* f, int32_t* out_items,
+                               float* out_scores, int32_t* out_count) {
+  if (!h) return PIO_ALS_ERR_ARG;
+  if (no_query_filter(f)) return pio_als_recommend(h, users, n, topk, item_mask, item_weight, out_items, out_scores, out_count);
+  std::lock_guard<std::mutex> lk(h->mu);
+  h->st.last_score_path = 0;
+  if (n < 0 || topk < 1) return fail(h, PIO_ALS_ERR_ARG, "topk must be >= 1 and n >= 0");
+  if (n == 0) return PIO_ALS_OK;
+  if (!users || !out_items || !out_scores) return fail(h, PIO_ALS_ERR_ARG, "null argument");
+  if (const char* what = query_filter_error(f, n)) return fail(h, PIO_ALS_ERR_ARG, "%s", what);
+  if (!h->U.F || !h->I.F || !h->I.cand_ext) return fail(h, PIO_ALS_ERR_STATE, "no model");
+  CK(h, cudaSetDevice(h->cfg.device));
+  std::vector<int> listed, scanned;
+  split_listed(f->has_wl, n, &listed, &scanned);
+  Scratch tmp(h->stream);
+  CallFilter cf;
+  int rc = upload_call_filter(h, item_mask, item_weight, f, tmp, &cf);
+  if (rc) return rc;
+  rc = recommend_part(h, users, scanned, false, topk, f, cf, out_items, out_scores, out_count);
+  if (rc) return rc;
+  return recommend_part(h, users, listed, true, topk, f, cf, out_items, out_scores, out_count);
+}
+
+int pio_als_similar_batch_filtered(pio_als_handle* h, const int64_t* q_ptr, const int32_t* q_items, int n_queries, int topk,
+                                   const uint8_t* item_mask, const double* item_weight, int flags,
+                                   const pio_als_query_filter* f, int32_t* out_items, float* out_scores, int32_t* out_count) {
+  if (!h) return PIO_ALS_ERR_ARG;
+  if (no_query_filter(f))
+    return pio_als_similar_batch(h, q_ptr, q_items, n_queries, topk, item_mask, item_weight, flags, out_items, out_scores,
+                                 out_count);
+  std::lock_guard<std::mutex> lk(h->mu);
+  h->st.last_score_path = 0;
+  if (n_queries < 0 || topk < 1) return fail(h, PIO_ALS_ERR_ARG, "topk must be >= 1 and n_queries >= 0");
+  if (n_queries == 0) return PIO_ALS_OK;
+  if (!q_ptr || !out_items || !out_scores) return fail(h, PIO_ALS_ERR_ARG, "null argument");
+  for (int j = 0; j < n_queries; ++j)
+    if (q_ptr[j + 1] < q_ptr[j] || (q_ptr[j + 1] > q_ptr[j] && !q_items))
+      return fail(h, PIO_ALS_ERR_ARG, "q_ptr must be non-decreasing offsets into q_items");
+  if (const char* what = query_filter_error(f, n_queries)) return fail(h, PIO_ALS_ERR_ARG, "%s", what);
+  if (!h->I.F || !h->I.cand_ext) return fail(h, PIO_ALS_ERR_STATE, "no model");
+  CK(h, cudaSetDevice(h->cfg.device));
+  std::vector<int> listed, scanned;
+  split_listed(f->has_wl, n_queries, &listed, &scanned);
+  Scratch tmp(h->stream);
+  CallFilter cf;
+  int rc = upload_call_filter(h, item_mask, item_weight, f, tmp, &cf);
+  if (rc) return rc;
+  const std::vector<int>* parts[2] = {&scanned, &listed};
+  for (int part = 0; part < 2; ++part) {
+    const std::vector<int>& idx = *parts[part];
+    std::vector<int64_t> sp(idx.size() + 1, 0);
+    for (size_t i = 0; i < idx.size(); ++i) sp[i + 1] = sp[i] + (q_ptr[idx[i] + 1] - q_ptr[idx[i]]);
+    std::vector<int32_t> flat((size_t)sp[idx.size()]);
+    for (size_t i = 0; i < idx.size(); ++i)
+      if (sp[i + 1] > sp[i]) memcpy(flat.data() + sp[i], q_items + q_ptr[idx[i]], sizeof(int32_t) * (size_t)(sp[i + 1] - sp[i]));
+    rc = similar_part(h, sp, flat, idx, part == 1, topk, item_mask, f, cf, flags, out_items, out_scores, out_count);
+    if (rc) return rc;
+  }
+  return PIO_ALS_OK;
 }
 
 // ---- persistence ------------------------------------------------------------------------------

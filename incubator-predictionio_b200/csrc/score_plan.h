@@ -9,6 +9,12 @@
 //                                                                   S5 the rest, one query at a time: cos_batched if
 //                                                                      its shared memory fits 100 KB, else cos_fallback
 //
+// Filtered calls (pio_als_recommend_filtered / pio_als_similar_batch_filtered): the queries with a white list take the
+// listed route (L: score_listed, one CTA per query, any rank and topk); the others are scanned by the batch kernels in
+// their filtered instantiation -- R3 / R4 whatever the number of users (plan_recommend_filtered), S3 / S4 as
+// plan_similar_batch decides; S5 queries of a filtered call get their dense mask from the host.  The single-query
+// paths never run for a filtered call.
+//
 // The similar paths are decided in three steps, as the information arrives: plan_similar before any launch (S1, S2, the
 // batch gather, or per query); plan_similar_batch once the gather says which query items own a factor (S3, S4, or S5);
 // plan_similar_query for every S5 query after its own gather.
@@ -54,8 +60,11 @@ struct ScorePlan {
   int passes = 0;           // passes of pass_k results (bounded by the last result of the one before)
   size_t smem = 0;          // dynamic shared memory of the scoring kernel
   int nvp = 0;              // score_one: query vectors per pass (1, 2, 4, 8)
+  bool filtered = false;    // the scan kernel runs in its filtered instantiation (per-query test at the pool insertion)
+  // the bits a launch of the scoring kernel records
+  unsigned launch_bits() const { return kernel | (filtered ? (unsigned)PIO_ALS_FPATH_FILTERED : 0u); }
   // every bit the call leaves in pio_als_stats.last_score_path
-  unsigned path() const { return kernel | (passes > 1 ? (unsigned)PIO_ALS_PATH_MULTI_PASS : 0u); }
+  unsigned path() const { return launch_bits() | (passes > 1 ? (unsigned)PIO_ALS_PATH_MULTI_PASS : 0u); }
 };
 
 // persistent CTAs: `want`, but at least eight tiles / steps of `steps` each (the pools must warm up), and at least one
@@ -131,6 +140,51 @@ inline ScorePlan plan_recommend(const ScoreEnv& e, int n, int topk) {
     set_batched(p, e, PIO_ALS_PATH_DOT_BATCHED, n, SB_QB, topk);
     p.route = ROUTE_BATCH;
   }
+  return p;
+}
+
+// the scanned users of a filtered recommend call: never the single-query or arena routes
+inline ScorePlan plan_recommend_filtered(const ScoreEnv& e, int n, int topk) {
+  ScorePlan p;
+  if (n < 1 || topk < 1) return p;
+  if (e.score_blocked && e.kp <= 64 && topk <= DB_MAXK)
+    set_blocked(p, e, PIO_ALS_PATH_DOT_BLOCKED, (n + SB_QB - 1) / SB_QB, SB_QB, topk);
+  else
+    set_batched(p, e, PIO_ALS_PATH_DOT_BATCHED, n, SB_QB, topk);
+  p.route = ROUTE_BATCH;
+  p.filtered = true;
+  return p;
+}
+
+// L: the n white-listed queries of a filtered call, one CTA each, one candidate list per warp
+inline ScorePlan plan_listed(int n, int topk) {
+  ScorePlan p;
+  if (n < 1 || topk < 1) return p;
+  set_passes(p, topk);
+  p.route = ROUTE_BATCH;
+  p.kernel = PIO_ALS_FPATH_LISTED;
+  p.threads = LS_THREADS;
+  p.gx = 1;
+  p.ngroups = n;
+  p.qpg = 1;
+  p.lists = LS_WARPS;
+  p.smem = listed_smem_bytes(p.pass_k);
+  return p;
+}
+
+// Which queries of a filtered call are listed and which are scanned: has_wl[j] != 0 sends query j to the listed route
+// (has_wl == nullptr: none).  Both lists keep the call's order; results go back to row listed[i] / scanned[i].
+inline void split_listed(const unsigned char* has_wl, int n, std::vector<int>* listed, std::vector<int>* scanned) {
+  listed->clear();
+  scanned->clear();
+  for (int j = 0; j < n; ++j) (has_wl && has_wl[j] ? listed : scanned)->push_back(j);
+}
+
+// the scanned queries of a filtered similar call before any launch: the batch gather, or per query (S5)
+inline ScorePlan plan_similar_filtered(int n_queries, long long total, int topk) {
+  ScorePlan p;
+  if (n_queries < 1 || topk < 1) return p;
+  p.route = total > 0 && total < (1ll << 31) ? ROUTE_BATCH : ROUTE_PER_QUERY;
   return p;
 }
 

@@ -19,6 +19,7 @@
 //   score_cos_topk_multi_kernel        2..16 users / long similar queries on the three-launch serving path
 //   score_cos_topk_batched_kernel    one long similar query, its vectors in shared memory
 //   score_cos_topk_kernel            fallback for single queries too large for that
+//   score_listed_kernel              white-listed queries of a filtered batch: scored over their lists, not the matrix
 //   topk_merge_kernel                merges the per-CTA / per-warp candidate lists of a query; multi-pass bounds (topk > 128)
 // Block sizes, pool shapes and every kernel's dynamic shared memory (*_smem_bytes) are in topk_geometry.h.
 // Pools: WarpPool (entries in shared memory, cooperative worst-entry search) and SortedPool (sorted in the registers of a
@@ -49,6 +50,42 @@ constexpr int TK_NO_BOUND = -2;
 constexpr int TK_EXHAUSTED = -3;
 __device__ __forceinline__ bool below_bound(const ScoreIdx& b, double s, int i) {
   return b.i == TK_NO_BOUND || (b.i >= 0 && better(b.s, b.i, s, i));
+}
+
+// Per-query filters of a batch call (pio_als_query_filter on the device).  Exclusion entries are 64-bit keys
+// (query << 32 | item id), sorted over the whole call, so the list of a query is the ascending range
+// ex[ex_ptr[q] .. ex_ptr[q + 1]); ids outside the item range and duplicates stay in the list and match nothing new.  A
+// set row is one bit per item.  The batch kernels test a candidate only when it is about to enter a pool (it has passed
+// the pool's threshold test): an excluded item never enters a pool, so thresholds are formed from allowed items only
+// and the scan itself is the unfiltered one.
+struct QueryFilterDev {
+  const unsigned long long* ex = nullptr;
+  const long long* ex_ptr = nullptr;   // [queries + 1]; nullptr: no exclusion lists
+  const int* set_ix = nullptr;         // [queries] row of set_bits, or -1; nullptr: no sets
+  const unsigned* set_bits = nullptr;  // [n_sets][set_words]
+  int set_words = 0;
+  int qbase = 0;                       // the launch's first query in the numbering of ex / ex_ptr / set_ix
+};
+// is item `ext` (>= 0) no candidate of query q (numbered inside the launch)?
+__device__ __forceinline__ bool qf_drop(const QueryFilterDev& f, int q, int ext) {
+  q += f.qbase;
+  if (f.set_ix) {
+    const int r = __ldg(f.set_ix + q);
+    if (r >= 0 && ((__ldg(f.set_bits + (size_t)r * f.set_words + (ext >> 5)) >> (ext & 31)) & 1u)) return true;
+  }
+  if (f.ex_ptr) {
+    const unsigned long long key = ((unsigned long long)(unsigned)q << 32) | (unsigned)ext;
+    long long lo = __ldg(f.ex_ptr + q);
+    const long long end = __ldg(f.ex_ptr + q + 1);
+    long long hi = end;
+    while (lo < hi) {
+      const long long mid = (lo + hi) >> 1;
+      if (__ldg(f.ex + mid) < key) lo = mid + 1;
+      else hi = mid;
+    }
+    if (lo < end && __ldg(f.ex + lo) == key) return true;
+  }
+  return false;
 }
 
 // Block-wide selection: every thread holds TK_ITEMS candidates (score, index; index -1 = none).
@@ -159,12 +196,13 @@ __device__ __forceinline__ void wpool_offer(WarpPool& wp, bool want, double s, i
   }
 }
 
+template <bool FILT>
 __global__ void __launch_bounds__(SB_THREADS, 2)
 score_dot_topk_batched_kernel(const float* __restrict__ Y, int n_items, int kp,
                               const float* __restrict__ xq, const uint8_t* __restrict__ qvalid, int n_queries,
                               const int* __restrict__ cand_ext, const uint8_t* __restrict__ mask,
                               const double* __restrict__ weight, const ScoreIdx* __restrict__ bound,
-                              int topk, ScoreIdx* __restrict__ cand) {
+                              int topk, ScoreIdx* __restrict__ cand, const QueryFilterDev flt) {
   extern __shared__ __align__(16) unsigned char sb_smem[];
   const int row = kp + 4;                                         // floats per staged row (16-byte skew per row)
   double* xd = reinterpret_cast<double*>(sb_smem);                // [kp][SB_QB]
@@ -251,7 +289,9 @@ score_dot_topk_batched_kernel(const float* __restrict__ Y, int n_items, int kp,
         for (int it = lane; it < SB_THREADS; it += 32) {
           const int e = sext[it];
           const double sv = scs[q * SB_THREADS + it];
-          wpool_offer(wp[j], e >= 0 && below_bound(bnd[j], sv, e), sv, e, topk, hs + (size_t)q * topk, hi + (size_t)q * topk);
+          bool want = e >= 0 && below_bound(bnd[j], sv, e);
+          if (FILT) want = want && (wp[j].cnt < topk || sv >= wp[j].thr) && !qf_drop(flt, q0 + q, e);
+          wpool_offer(wp[j], want, sv, e, topk, hs + (size_t)q * topk, hi + (size_t)q * topk);
         }
       }
     }
@@ -410,12 +450,21 @@ __device__ __noinline__ void db_insert(DbPoolHdr* hd, double* ps, int* pi, unsig
   __syncwarp();
 }
 
-template <int KP>
+// the same with the query's filter: a lane's candidate that its query excludes is withdrawn before the insertion
+__device__ __noinline__ void dbf_insert(DbPoolHdr* hd, double* ps, int* pi, unsigned long long* cthr, bool w0, double s0,
+                                        int e0, bool w1, double s1, int e1, int topk, const QueryFilterDev& flt, int q) {
+  if (w0 && qf_drop(flt, q, e0)) w0 = false;
+  if (w1 && qf_drop(flt, q, e1)) w1 = false;
+  if (!__any_sync(0xffffffffu, w0 || w1)) return;
+  db_insert(hd, ps, pi, cthr, w0, s0, e0, w1, s1, e1, topk);
+}
+
+template <int KP, bool FILT>
 __global__ void __launch_bounds__(32 * DB_WARPS, 1)
 score_dot_blocked_kernel(const float* __restrict__ Y, int n_items, const float* __restrict__ xq,
                          const uint8_t* __restrict__ qvalid, int n_queries, const int* __restrict__ cand_ext,
                          const uint8_t* __restrict__ mask, const double* __restrict__ weight, int topk,
-                         ScoreIdx* __restrict__ cand) {
+                         ScoreIdx* __restrict__ cand, const QueryFilterDev flt) {
   constexpr int ROW = KP + 4, F4 = KP / 4;
   constexpr int RPI = 32 / F4;                 // rows per warp-wide copy instruction (512 contiguous bytes)
   constexpr int CPW = DB_ROWS / RPI / DB_WPR;  // copy instructions per warp and step
@@ -540,8 +589,12 @@ score_dot_blocked_kernel(const float* __restrict__ Y, int n_items, const float* 
       const bool w0 = ext[0] >= 0 && (cnt < topk || acc[0][q] >= thr) && s1_key(acc[0][q]) >= ck;
       const bool w1 = ext[1] >= 0 && (cnt < topk || acc[1][q] >= thr) && s1_key(acc[1][q]) >= ck;
       if (!__any_sync(0xffffffffu, w0 || w1)) continue;
-      db_insert(&hdr[q], ps + (size_t)q * topk, pi + (size_t)q * topk, &cthr[sub * DB_QW + q], w0, acc[0][q], ext[0], w1,
-                acc[1][q], ext[1], topk);
+      if (FILT)
+        dbf_insert(&hdr[q], ps + (size_t)q * topk, pi + (size_t)q * topk, &cthr[sub * DB_QW + q], w0, acc[0][q], ext[0], w1,
+                   acc[1][q], ext[1], topk, flt, q0 + sub * DB_QW + q);
+      else
+        db_insert(&hdr[q], ps + (size_t)q * topk, pi + (size_t)q * topk, &cthr[sub * DB_QW + q], w0, acc[0][q], ext[0], w1,
+                  acc[1][q], ext[1], topk);
     }
   }
   asm volatile("cp.async.wait_group 0;\n" ::);
@@ -582,13 +635,23 @@ __device__ __noinline__ void cb_insert(DbPoolHdr* hd, double* ps, int* pi, unsig
   db_insert(hd, ps, pi, cthr, w0, s0, e0, w1, s1, e1, topk);
 }
 
-template <int KP>
+__device__ __noinline__ void cbf_insert(DbPoolHdr* hd, double* ps, int* pi, unsigned long long* cthr, bool w0, double s0,
+                                        int e0, bool w1, double s1, int e1, int topk, const int* __restrict__ qid, int nid,
+                                        const QueryFilterDev& flt, int q) {
+  if (w0 && qf_drop(flt, q, e0)) w0 = false;
+  if (w1 && qf_drop(flt, q, e1)) w1 = false;
+  if (!__any_sync(0xffffffffu, w0 || w1)) return;
+  cb_insert(hd, ps, pi, cthr, w0, s0, e0, w1, s1, e1, topk, qid, nid);
+}
+
+template <int KP, bool FILT>
 __global__ void __launch_bounds__(32 * DB_WARPS, 1)
 score_cos_blocked_kernel(const float* __restrict__ Y, int n_items, int k, const float* __restrict__ qf,
                          const int* __restrict__ bin_q0, const int* __restrict__ bin_v0, int n_bins,
                          const int* __restrict__ vq, const long long* __restrict__ qid_ptr, const int* __restrict__ qid,
                          const int* __restrict__ cand_ext, const uint8_t* __restrict__ mask,
-                         const double* __restrict__ weight, int keep_query, int topk, ScoreIdx* __restrict__ cand) {
+                         const double* __restrict__ weight, int keep_query, int topk, ScoreIdx* __restrict__ cand,
+                         const QueryFilterDev flt) {
   constexpr int ROW = KP + 4, F4 = KP / 4;
   constexpr int RPI = 32 / F4;
   constexpr int CPW = DB_ROWS / RPI / DB_WPR;
@@ -769,8 +832,12 @@ score_cos_blocked_kernel(const float* __restrict__ Y, int n_items, int k, const 
       const bool w0 = ext[0] >= 0 && sc[0][q] > 0.0 && (cnt < topk || sc[0][q] >= thr) && s1_key(sc[0][q]) >= ck;
       const bool w1 = ext[1] >= 0 && sc[1][q] > 0.0 && (cnt < topk || sc[1][q] >= thr) && s1_key(sc[1][q]) >= ck;
       if (!__any_sync(0xffffffffu, w0 || w1)) continue;
-      cb_insert(&hdr[q], ps + (size_t)q * topk, pi + (size_t)q * topk, &cthr[sub * CB_QPW + q], w0, sc[0][q], ext[0], w1,
-                sc[1][q], ext[1], topk, qid_of[q], nid_of[q]);
+      if (FILT)
+        cbf_insert(&hdr[q], ps + (size_t)q * topk, pi + (size_t)q * topk, &cthr[sub * CB_QPW + q], w0, sc[0][q], ext[0], w1,
+                   sc[1][q], ext[1], topk, qid_of[q], nid_of[q], flt, bq0 + q);
+      else
+        cb_insert(&hdr[q], ps + (size_t)q * topk, pi + (size_t)q * topk, &cthr[sub * CB_QPW + q], w0, sc[0][q], ext[0], w1,
+                  sc[1][q], ext[1], topk, qid_of[q], nid_of[q]);
     }
   }
   asm volatile("cp.async.wait_group 0;\n" ::);
@@ -914,12 +981,14 @@ score_cos_topk_batched_kernel(const float* __restrict__ Y, int n_items, int kp, 
 //   vq[v]                  : query (0..SM_QG-1 inside the group) of vector v
 //   qid_ptr / qid          : all query item ids (external) of every query, for the exclusion rule
 
+template <bool FILT>
 __global__ void __launch_bounds__(SB_THREADS, 2)
 score_cos_topk_multi_kernel(const float* __restrict__ Y, int n_items, int kp, int k, const float* __restrict__ qf,
                             const int* __restrict__ gvec0, const int* __restrict__ vq, const long long* __restrict__ qid_ptr,
                             const int* __restrict__ qid, int n_queries, const int* __restrict__ cand_ext,
                             const uint8_t* __restrict__ mask, const double* __restrict__ weight,
-                            const ScoreIdx* __restrict__ bound, int keep_query, int topk, ScoreIdx* __restrict__ cand) {
+                            const ScoreIdx* __restrict__ bound, int keep_query, int topk, ScoreIdx* __restrict__ cand,
+                            const QueryFilterDev flt) {
   extern __shared__ __align__(16) unsigned char sb_smem[];
   const int row = kp + 4;
   double* xd = reinterpret_cast<double*>(sb_smem);                          // [kp][SM_NV]
@@ -1043,6 +1112,7 @@ score_cos_topk_multi_kernel(const float* __restrict__ Y, int n_items, int kp, in
         const int e = sext[it];
         const double sv = scs[warp * SB_THREADS + it];
         bool want = e >= 0 && sv > 0.0 && below_bound(bnd, sv, e);
+        if (FILT) want = want && (wp.cnt < topk || sv >= wp.thr) && !qf_drop(flt, myq, e);
         if (want && !keep_query) {
           if (ids_in_smem) {
             for (int t = 0; t < (int)(ie - ib); ++t)
@@ -1113,6 +1183,112 @@ score_cos_topk_kernel(const float* __restrict__ Y, int n_items, int kp, int k,
     }
   }
   block_select_topk(sc, ix, topk, cand + (size_t)blockIdx.x * topk);
+}
+
+// ---- white-listed queries: scored over their lists ------------------------------------------------------------------
+// A query with a white list has few candidates: scanning the item matrix for it would leave its pool unfilled for the
+// whole scan (every item takes the insertion path).  Here one CTA takes one query and walks its sorted white list
+// (wl: keys query << 32 | item id, like the exclusion lists; duplicates are adjacent and taken once, ids outside the
+// item range skipped), one entry per lane: the item's row is read from the factor matrix and scored with the
+// arithmetic of the scan kernels (fp64, index order; cosine terms in query order) -> the same bits.  Every rule of the
+// scan applies: owns a factor, item_mask, set row, exclusion list, the query's own items (COS, unless keep_query),
+// score > 0 (COS), weights, pass bound.  Each warp pools what it scored; the merge orders the LS_WARPS lists.
+//   DOT: xq [queries][kp] user vectors, qvalid[q] == 0 -> no candidates
+//   COS: xq [all query ids][kp] the gathered vector of every query id (zeros for an id without a factor: its cosine
+//        terms are exactly 0), qid_ptr / qid the id list of every query
+// grid: (1, queries of the launch); cand: [queries][LS_WARPS][topk]; bound: per query of the launch, or nullptr.
+template <bool COS>
+__global__ void __launch_bounds__(LS_THREADS)
+score_listed_kernel(const float* __restrict__ Y, int kp, const int* __restrict__ perm, const unsigned* __restrict__ deg,
+                    int n_ext, const float* __restrict__ xq, const uint8_t* __restrict__ qvalid,
+                    const long long* __restrict__ qid_ptr, const int* __restrict__ qid,
+                    const unsigned long long* __restrict__ wl, const long long* __restrict__ wl_ptr,
+                    const uint8_t* __restrict__ mask, const double* __restrict__ weight,
+                    const ScoreIdx* __restrict__ bound, int keep_query, int topk, ScoreIdx* __restrict__ cand,
+                    const QueryFilterDev flt) {
+  extern __shared__ __align__(16) unsigned char ls_smem[];
+  double* hs = reinterpret_cast<double*>(ls_smem);            // [LS_WARPS][topk]
+  int* hi = reinterpret_cast<int*>(hs + (size_t)LS_WARPS * topk);
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const int q = flt.qbase + blockIdx.y;
+  double* ps = hs + (size_t)warp * topk;
+  int* pi = hi + (size_t)warp * topk;
+  WarpPool wp;
+  wp.thr = 0.0; wp.wid = -1; wp.worst = 0; wp.cnt = 0;
+  ScoreIdx bnd;
+  bnd.s = 0.0;
+  bnd.i = TK_NO_BOUND;
+  if (bound) bnd = bound[blockIdx.y];
+  const long long wb = wl_ptr[q], we = wl_ptr[q + 1];
+  long long ib = 0, ie = 0;
+  if (COS) { ib = qid_ptr[q]; ie = qid_ptr[q + 1]; }
+  const bool live = COS ? ie > ib : qvalid[q] != 0;
+  const int f4row = kp / 4;
+  for (long long base = wb + warp * 32; live && base < we; base += LS_THREADS) {
+    const long long t = base + lane;
+    int ext = -1;
+    if (t < we) {
+      const unsigned long long key = wl[t];
+      const unsigned id = (unsigned)key;
+      if (id < (unsigned)n_ext && !(t > wb && wl[t - 1] == key)) ext = (int)id;
+    }
+    if (ext >= 0 && deg[ext] == 0) ext = -1;
+    if (ext >= 0 && mask && mask[ext]) ext = -1;
+    if (ext >= 0 && qf_drop(flt, blockIdx.y, ext)) ext = -1;
+    if (COS && ext >= 0 && !keep_query)
+      for (long long v = ib; v < ie; ++v)
+        if (qid[v] == ext) { ext = -1; break; }
+    double score = 0.0;
+    if (ext >= 0) {
+      const float4* yrow = reinterpret_cast<const float4*>(Y + (size_t)perm[ext] * kp);
+      if (COS) {
+        double n2 = 0.0;
+        for (int c4 = 0; c4 < f4row; ++c4) {
+          const float4 y4 = __ldg(yrow + c4);
+          const double b0 = (double)y4.x, b1 = (double)y4.y, b2 = (double)y4.z, b3 = (double)y4.w;
+          n2 = fma(b0, b0, n2);
+          n2 = fma(b1, b1, n2);
+          n2 = fma(b2, b2, n2);
+          n2 = fma(b3, b3, n2);
+        }
+        const double s2 = sqrt(n2);
+        for (long long v = ib; v < ie; ++v) {
+          const float4* xrow = reinterpret_cast<const float4*>(xq + (size_t)v * kp);
+          double n1 = 0.0, d = 0.0;
+          for (int c4 = 0; c4 < f4row; ++c4) {
+            const float4 y4 = __ldg(yrow + c4), x4 = __ldg(xrow + c4);
+            const double ye[4] = {(double)y4.x, (double)y4.y, (double)y4.z, (double)y4.w};
+            const double xe[4] = {(double)x4.x, (double)x4.y, (double)x4.z, (double)x4.w};
+#pragma unroll
+            for (int e = 0; e < 4; ++e) {
+              n1 = fma(xe[e], xe[e], n1);     // squares of fp32 values are exact in fp64: fma == n1 += a * a
+              d = fma(xe[e], ye[e], d);
+            }
+          }
+          const double n1n2 = sqrt(n1) * s2;
+          score += (n1n2 == 0.0) ? 0.0 : d / n1n2;
+        }
+      } else {
+        const float4* xrow = reinterpret_cast<const float4*>(xq + (size_t)q * kp);
+        for (int c4 = 0; c4 < f4row; ++c4) {
+          const float4 y4 = __ldg(yrow + c4), x4 = __ldg(xrow + c4);
+          score = fma((double)x4.x, (double)y4.x, score);   // index order t = 0..k-1, like blas.ddot over Array[Double]
+          score = fma((double)x4.y, (double)y4.y, score);
+          score = fma((double)x4.z, (double)y4.z, score);
+          score = fma((double)x4.w, (double)y4.w, score);
+        }
+      }
+      if (weight) score = score * weight[ext];
+    }
+    wpool_offer(wp, ext >= 0 && (!COS || score > 0.0) && below_bound(bnd, score, ext), score, ext, topk, ps, pi);
+  }
+  __syncwarp();
+  for (int t = lane; t < topk; t += 32) {
+    ScoreIdx e;
+    e.s = t < wp.cnt ? ps[t] : 0.0;
+    e.i = t < wp.cnt ? pi[t] : -1;
+    cand[((size_t)blockIdx.y * LS_WARPS + warp) * topk + t] = e;
+  }
 }
 
 // grid: n_queries. Merges n_cand unsorted candidates per query (i = -1: empty) -> final topk, best first.

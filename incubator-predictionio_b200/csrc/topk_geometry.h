@@ -74,6 +74,11 @@ PIO_HD inline size_t cos_multi_smem_bytes(int kp, int topk) {
          sizeof(int) * (SM_NV + SM_QG * SM_QIDS) + 16;
 }
 
+// ---- score_listed_kernel: one white-listed query per CTA, scored over its list ----
+constexpr int LS_THREADS = 256;
+constexpr int LS_WARPS = LS_THREADS / 32;   // one pool, and one candidate list, per warp
+PIO_HD inline size_t listed_smem_bytes(int topk) { return (sizeof(double) + sizeof(int)) * (size_t)LS_WARPS * topk; }
+
 // ---- score_one_kernel: one query, one launch ----
 constexpr int S1_THREADS = 256;
 constexpr int S1_STAGES = 3;

@@ -83,9 +83,16 @@ class MatrixFactorizationModel:
         return [Rating(user, int(items[0, t]), float(scores[0, t])) for t in range(int(cnt[0]))]
 
     def recommendProductsForUsers(self, users: np.ndarray, num: int, item_mask: Optional[np.ndarray] = None,
-                                  item_weight: Optional[np.ndarray] = None):
+                                  item_weight: Optional[np.ndarray] = None, query_filter=None):
         """Batched top-N (what batchPredict's cartesian + groupBy computes, ALSAlgorithm.scala:117-158)."""
-        return self._handle().recommend(np.ascontiguousarray(users, np.int32), num, item_mask, item_weight)
+        return self._handle().recommend(np.ascontiguousarray(users, np.int32), num, item_mask, item_weight, query_filter)
+
+    def similarProductsBatch(self, queries: Sequence[Sequence[int]], num: int, item_mask: Optional[np.ndarray] = None,
+                             item_weight: Optional[np.ndarray] = None, exclude_query: bool = True, query_filter=None):
+        """similarProducts for many queries in one call; query_filter (native.QueryFilter) carries what differs per
+        query: exclusion lists, white lists, category set rows."""
+        return self._handle().similar_batch(queries, num, item_mask, item_weight, keep_query_items=not exclude_query,
+                                            query_filter=query_filter)
 
     def similarProducts(self, query_items: Sequence[int], num: int, item_mask: Optional[np.ndarray] = None,
                         item_weight: Optional[np.ndarray] = None, exclude_query: bool = True):

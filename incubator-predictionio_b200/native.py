@@ -30,7 +30,8 @@ EXPORTED_SYMBOLS = [
     "pio_als_destroy", "pio_als_last_error", "pio_als_set_ratings_coo", "pio_als_set_ratings_coo_device", "pio_als_set_ratings_coo_sharded",
     "pio_als_set_ratings_coo_sharded_device",
     "pio_als_set_init", "pio_als_run", "pio_als_get_factors", "pio_als_train", "pio_als_recommend",
-    "pio_als_similar", "pio_als_similar_batch", "pio_als_model_import", "pio_als_save", "pio_als_load", "pio_als_get_stats", "pio_als_get_phase_ms",
+    "pio_als_similar", "pio_als_similar_batch", "pio_als_recommend_filtered", "pio_als_similar_batch_filtered",
+    "pio_als_model_import", "pio_als_save", "pio_als_load", "pio_als_get_stats", "pio_als_get_phase_ms",
     "pio_als_synth_ratings_device", "pio_nb_train", "pio_nb_predict", "pio_ids_encode", "pio_cooc_train",
     "pio_events_scan", "pio_events_scan_keys", "pio_events_fold", "pio_events_scan_props", "pio_events_fold_props",
     "pio_events_index_create",
@@ -71,7 +72,66 @@ class Stats(C.Structure):
 
 # pio_als_stats.last_score_path bits (PIO_ALS_PATH_* in pio_als.h)
 SCORE_PATH_BITS = {"score_one": 0x01, "dot_blocked": 0x02, "cos_blocked": 0x04, "dot_batched": 0x08, "cos_multi": 0x10,
-                   "cos_batched": 0x20, "cos_fallback": 0x40, "multi_pass": 0x80}
+                   "cos_batched": 0x20, "cos_fallback": 0x40, "multi_pass": 0x80, "filtered": 0x100, "listed": 0x200}
+
+
+class _QueryFilterStruct(C.Structure):
+    """pio_als_query_filter"""
+    _fields_ = [
+        ("ex_ptr", C.c_void_p), ("ex_items", C.c_void_p), ("has_wl", C.c_void_p), ("wl_ptr", C.c_void_p),
+        ("wl_items", C.c_void_p), ("set_ix", C.c_void_p), ("item_sets", C.c_void_p), ("n_sets", C.c_int32),
+    ]
+
+
+def _csr(lists, n):
+    """(ptr int64 [n + 1], flat int32) of n id lists; None entries are empty lists."""
+    ptr = np.zeros(n + 1, np.int64)
+    arrs = [np.zeros(0, np.int32) if l is None else np.asarray(l, np.int32).reshape(-1) for l in lists]
+    if len(arrs) != n:
+        raise ValueError(f"expected {n} lists, got {len(arrs)}")
+    if n:
+        ptr[1:] = np.cumsum([a.shape[0] for a in arrs])
+    flat = np.ascontiguousarray(np.concatenate(arrs) if n and ptr[-1] else np.zeros(0, np.int32), np.int32)
+    return ptr, flat
+
+
+class QueryFilter:
+    """The per-query filters of a batch scoring call (pio_als_query_filter), built from per-query Python lists or arrays.
+
+    exclude    : n id lists (None = empty), the items query j may not return (black lists, seen items)
+    white      : n entries, None = no white list, else the only items query j may return (an empty list: none)
+    set_ix     : n rows of item_sets, -1 = none; item_sets: [n_sets, n_items] uint8, 1 = not a candidate
+    Ids outside the item range and duplicates are ignored by the library."""
+
+    def __init__(self, n_queries: int, exclude=None, white=None, set_ix=None, item_sets=None):
+        self.n = int(n_queries)
+        self.ex_ptr = self.ex_items = self.has_wl = self.wl_ptr = self.wl_items = self.set_ix = self.item_sets = None
+        self.n_sets = 0
+        if exclude is not None:
+            self.ex_ptr, self.ex_items = _csr(exclude, self.n)
+        if white is not None:
+            if len(white) != self.n:
+                raise ValueError(f"expected {self.n} white lists, got {len(white)}")
+            self.has_wl = np.array([w is not None for w in white], np.uint8)
+            self.wl_ptr, self.wl_items = _csr(white, self.n)
+        if set_ix is not None:
+            self.set_ix = np.ascontiguousarray(set_ix, np.int32)
+            if self.set_ix.shape != (self.n,):
+                raise ValueError("set_ix must have one entry per query")
+            if item_sets is not None:
+                self.item_sets = np.ascontiguousarray(item_sets, np.uint8)
+                if self.item_sets.ndim != 2:
+                    raise ValueError("item_sets must be [n_sets, n_items]")
+                self.n_sets = int(self.item_sets.shape[0])
+
+    def struct(self, n_queries: int, n_items: int) -> _QueryFilterStruct:
+        """The C struct over this object's arrays (which must outlive the call)."""
+        if n_queries != self.n:
+            raise ValueError(f"query filter built for {self.n} queries, call has {n_queries}")
+        if self.item_sets is not None and self.item_sets.shape[1] != n_items:
+            raise ValueError("item_sets rows must have n_items entries")
+        return _QueryFilterStruct(_addr(self.ex_ptr), _addr(self.ex_items), _addr(self.has_wl), _addr(self.wl_ptr),
+                                  _addr(self.wl_items), _addr(self.set_ix), _addr(self.item_sets), self.n_sets)
 
 
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
@@ -115,6 +175,10 @@ def lib():
         L.pio_als_similar.argtypes = [vp, vp, ci, ci, vp, vp, ci, vp, vp, vp]
         L.pio_als_similar_batch.restype = ci
         L.pio_als_similar_batch.argtypes = [vp, vp, vp, ci, ci, vp, vp, ci, vp, vp, vp]
+        L.pio_als_recommend_filtered.restype = ci
+        L.pio_als_recommend_filtered.argtypes = [vp, vp, ci, ci, vp, vp, vp, vp, vp, vp]
+        L.pio_als_similar_batch_filtered.restype = ci
+        L.pio_als_similar_batch_filtered.argtypes = [vp, vp, vp, ci, ci, vp, vp, ci, vp, vp, vp, vp]
         i64 = C.c_int64
         L.pio_events_index_lookup.restype = ci
         L.pio_events_index_lookup.argtypes = [vp, vp, vp, C.c_int32, i64, i64, vp, vp, vp, vp]
@@ -276,13 +340,19 @@ class NativeALS:
             raise ValueError("item_weight must have n_items entries")
         return mk, wt
 
-    def recommend(self, users, topk, item_mask=None, item_weight=None):
+    def recommend(self, users, topk, item_mask=None, item_weight=None, query_filter=None):
+        """query_filter (QueryFilter, one entry per user): pio_als_recommend_filtered."""
         users = np.ascontiguousarray(users, np.int32)
         n = users.shape[0]
         oi = np.full((n, topk), -1, np.int32)
         os_ = np.zeros((n, topk), np.float32)
         oc = np.zeros(n, np.int32)
         mk, wt = self._mask_weight(item_mask, item_weight)
+        if query_filter is not None:
+            qf = query_filter.struct(n, self.n_items)
+            self._check(lib().pio_als_recommend_filtered(self._h, users.ctypes.data, n, topk, _addr(mk), _addr(wt),
+                                                         C.addressof(qf), oi.ctypes.data, os_.ctypes.data, oc.ctypes.data))
+            return oi, os_, oc
         self._check(lib().pio_als_recommend(self._h, users.ctypes.data, n, topk, _addr(mk), _addr(wt), oi.ctypes.data,
                                             os_.ctypes.data, oc.ctypes.data))
         return oi, os_, oc
@@ -298,8 +368,9 @@ class NativeALS:
                                           os_.ctypes.data, oc.ctypes.data))
         return oi, os_, int(oc[0])
 
-    def similar_batch(self, queries, topk, item_mask=None, item_weight=None, keep_query_items=False):
-        """queries: sequence of item-index sequences; returns (items [n, topk], scores [n, topk], count [n])."""
+    def similar_batch(self, queries, topk, item_mask=None, item_weight=None, keep_query_items=False, query_filter=None):
+        """queries: sequence of item-index sequences; returns (items [n, topk], scores [n, topk], count [n]).
+        query_filter (QueryFilter, one entry per query): pio_als_similar_batch_filtered."""
         n = len(queries)
         ptr = np.zeros(n + 1, np.int64)
         ptr[1:] = np.cumsum([len(q) for q in queries])
@@ -309,6 +380,13 @@ class NativeALS:
         os_ = np.zeros((n, topk), np.float32)
         oc = np.zeros(n, np.int32)
         mk, wt = self._mask_weight(item_mask, item_weight)
+        if query_filter is not None:
+            qf = query_filter.struct(n, self.n_items)
+            self._check(lib().pio_als_similar_batch_filtered(
+                self._h, ptr.ctypes.data, flat.ctypes.data, n, topk, _addr(mk), _addr(wt),
+                SIM_KEEP_QUERY_ITEMS if keep_query_items else 0, C.addressof(qf), oi.ctypes.data, os_.ctypes.data,
+                oc.ctypes.data))
+            return oi, os_, oc
         self._check(lib().pio_als_similar_batch(self._h, ptr.ctypes.data, flat.ctypes.data, n, topk, _addr(mk), _addr(wt),
                                                 SIM_KEEP_QUERY_ITEMS if keep_query_items else 0, oi.ctypes.data,
                                                 os_.ctypes.data, oc.ctypes.data))

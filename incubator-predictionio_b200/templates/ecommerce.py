@@ -15,9 +15,11 @@ from typing import Dict, List, Optional, Set
 
 import numpy as np
 
+from .. import native
 from ..controller import (Engine, EngineFactory, LFirstServing, P2LAlgorithm, Params, PDataSource, PersistentModel,
                           IdentityPreparator)
 from ..mllib import ALS, MatrixFactorizationModel
+from .category_index import category_index
 from ..storage import (BiMap, EntityEventColumns, EntityEventIndex, LEventStore, PEventStore, require_values,
                        string_list)
 
@@ -325,6 +327,100 @@ class ECommAlgorithm(P2LAlgorithm):
                 cand.sort(key=lambda kv: (-kv[1], kv[0]))
                 top = cand[:query.num]
         return PredictedResult([ItemScore(model.itemIntStringMap(i), s) for i, s in top])
+
+    def predictMany(self, model: ECommModel, queries) -> list:
+        """predict for many queries: one lookup per event index for the whole batch (seen items, recent items),
+        `unavailableItems` and `weightedItems` read once, then one filtered batch call per branch.  Known users are
+        scored by dot products with their black list (query blackList, seen items, unavailable items) as exclusion
+        list; unknown users with recent items by cosine sums that keep the recent items as candidates; the rest get
+        the popularity rule of predict on the host."""
+        qs = list(queries)
+        out: List[Optional[PredictedResult]] = [None] * len(qs)
+        for j, q in enumerate(qs):
+            if q.num < 1:
+                out[j] = self.predict(model, q)
+        rows = [j for j in range(len(qs)) if out[j] is None]
+        if not rows:
+            return out
+        imap, n_items = model.itemStringIntMap, len(model.mf.productHas)
+        seen = [set() for _ in rows]
+        if self.ap.unseenOnly:
+            seen = [{e.targetEntityId for e in evs} for evs in self._index("seen").find_many([qs[j].user for j in rows])]
+        unavailable: Set[str] = set()
+        try:
+            cons = self._index("constraint").find("unavailableItems", limit=1)
+            if cons:
+                unavailable = set(cons[0].properties.get("items"))
+        except FileNotFoundError:
+            pass
+        weights = self._weights(model)
+        black = [sorted({b for b in (imap.get(x) for x in set(qs[j].blackList or ()) | seen[r] | unavailable)
+                         if b is not None}) for r, j in enumerate(rows)]
+        white = [None if qs[j].whiteList is None else [w for w in (imap.get(x) for x in qs[j].whiteList) if w is not None]
+                 for j in rows]
+        set_of: Dict[frozenset, int] = {}
+        set_rows: List[np.ndarray] = []
+        set_ix = np.full(len(rows), -1, np.int32)
+        for r, j in enumerate(rows):
+            if qs[j].categories is not None:
+                key = frozenset(qs[j].categories)
+                if key not in set_of:
+                    set_of[key] = len(set_rows)
+                    set_rows.append(category_index(model).excluded(qs[j].categories))
+                set_ix[r] = set_of[key]
+        # the branch of every query: known user, unknown user with recent items, or the default
+        similar, recent_of = [], {}
+        unknown = [r for r, j in enumerate(rows)
+                   if not ((u := model.userStringIntMap.get(qs[j].user)) is not None and model.mf.userHas[u])]
+        unknown_set = set(unknown)
+        known = [r for r in range(len(rows)) if r not in unknown_set]
+        if unknown:
+            found = self._index("similar").find_many([qs[rows[r]].user for r in unknown], limit=10)
+            for r, evs in zip(unknown, found):
+                rec = {imap.get(e.targetEntityId) for e in evs}
+                rec.discard(None)
+                rec = sorted(i for i in rec if model.mf.productHas[i])
+                if rec:
+                    similar.append(r)
+                    recent_of[r] = rec
+
+        def part(rs):
+            return native.QueryFilter(len(rs), [black[r] for r in rs], [white[r] for r in rs],
+                                      set_ix[rs] if set_rows else None, np.stack(set_rows) if set_rows else None)
+
+        def result(pairs):
+            return PredictedResult([ItemScore(model.itemIntStringMap(i), s) for i, s in pairs])
+
+        if known:
+            users = np.array([model.userStringIntMap.get(qs[rows[r]].user) for r in known], np.int32)
+            num = max(qs[rows[r]].num for r in known)
+            items, scores, cnt = model.mf.recommendProductsForUsers(users, num, None, weights, query_filter=part(known))
+            for k, r in enumerate(known):
+                n = min(int(cnt[k]), qs[rows[r]].num)
+                out[rows[r]] = result([(int(items[k, t]), float(scores[k, t])) for t in range(n) if scores[k, t] > 0])
+        if similar:
+            num = max(qs[rows[r]].num for r in similar)
+            items, scores, cnt = model.mf.similarProductsBatch([recent_of[r] for r in similar], num, None, weights,
+                                                               exclude_query=False, query_filter=part(similar))
+            for k, r in enumerate(similar):
+                n = min(int(cnt[k]), qs[rows[r]].num)
+                out[rows[r]] = result([(int(items[k, t]), float(scores[k, t])) for t in range(n)])
+        for r in unknown:
+            if r in recent_of:
+                continue
+            # predictDefault: popularity count x weight over the query's candidates (no > 0 filter in the reference)
+            mask = np.zeros(n_items, bool)
+            if white[r] is not None:
+                mask[:] = True
+                mask[white[r]] = False
+            mask[black[r]] = True
+            if set_ix[r] >= 0:
+                mask |= set_rows[set_ix[r]].astype(bool)
+            cand = [(int(i), float(model.popularCount.get(int(i), 0)) * (float(weights[i]) if weights is not None else 1.0))
+                    for i in np.flatnonzero(~mask)]
+            cand.sort(key=lambda kv: (-kv[1], kv[0]))
+            out[rows[r]] = result(cand[:qs[rows[r]].num])
+        return out
 
 
 class ECommerceRecommendationEngine(EngineFactory):

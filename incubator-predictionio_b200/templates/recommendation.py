@@ -242,6 +242,28 @@ class ALSAlgorithm(PAlgorithm):
         rs = model.recommendProductsWithFilter(userInt, query.num, [b for b in blackList if b is not None])
         return PredictedResult([ItemScore(inv(r.product), r.rating) for r in rs])
 
+    def predictMany(self, model: ALSModel, queries) -> list:
+        """predict for many queries in one filtered batch call: each known user is scored with its own black list
+        (native.QueryFilter exclusion lists) for the largest `num` of the batch; a query keeps its first `num`."""
+        qs = list(queries)
+        out = [PredictedResult([]) for _ in qs]
+        rows = [j for j, q in enumerate(qs) if q.num >= 1 and model.userStringIntMap.get(q.user) is not None]
+        for j, q in enumerate(qs):
+            if q.num < 1 and model.userStringIntMap.get(q.user) is not None:
+                out[j] = self.predict(model, q)
+        if not rows:
+            return out
+        inv = model.itemStringIntMap.inverse
+        users = np.array([model.userStringIntMap.get(qs[j].user) for j in rows], np.int32)
+        black = [[b for b in (model.itemStringIntMap.get(x) for x in (qs[j].blackList or ())) if b is not None]
+                 for j in rows]
+        num = max(qs[j].num for j in rows)
+        items, scores, cnt = model.recommendProductsForUsers(users, num, query_filter=native.QueryFilter(len(rows), black))
+        for r, j in enumerate(rows):
+            n = min(int(cnt[r]), qs[j].num)
+            out[j] = PredictedResult([ItemScore(inv(int(items[r, t])), float(scores[r, t])) for t in range(n)])
+        return out
+
     def batchPredict(self, model: ALSModel, queries):
         """One batched GPU top-N instead of cartesian + groupBy (ALSAlgorithm.scala:117-158)."""
         qs = list(queries)

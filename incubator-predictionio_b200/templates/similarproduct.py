@@ -15,6 +15,8 @@ from typing import Dict, List, Optional, Set
 
 import numpy as np
 
+from .. import native
+from .category_index import CategoryIndex, category_index  # noqa: F401
 from ..controller import (Engine, EngineFactory, LServing, P2LAlgorithm, Params, PDataSource, PersistentModel,
                           PPreparator)
 from ..mllib import ALS, MatrixFactorizationModel
@@ -278,6 +280,50 @@ class ALSAlgorithm(P2LAlgorithm):
         items, scores, cnt = model.mf.similarProducts(sorted(queryList), query.num, mask)
         return PredictedResult([ItemScore(model.itemIntStringMap(int(items[t])), float(scores[t])) for t in range(cnt)])
 
+    def predictMany(self, model: ALSModel, queries) -> list:
+        """predict for many queries in one filtered batch call.  A query's blackList is its exclusion list, its
+        whiteList its white list, and its category rules one shared item_sets row per distinct (categories,
+        categoryBlackList) pair of the batch, built from the model's CategoryIndex."""
+        qs = list(queries)
+        out = [PredictedResult([]) for _ in qs]
+        sim = model.itemStringIntMap
+        rows, qlists = [], []
+        for j, q in enumerate(qs):
+            ql = {sim.get(x) for x in q.items}
+            ql.discard(None)
+            if not ql:
+                continue
+            if q.num < 1:
+                out[j] = self.predict(model, q)
+                continue
+            rows.append(j)
+            qlists.append(sorted(ql))
+        if not rows:
+            return out
+        ids = lambda xs: [i for i in (sim.get(x) for x in xs) if i is not None]   # noqa: E731
+        black = [None if qs[j].blackList is None else ids(qs[j].blackList) for j in rows]
+        white = [None if qs[j].whiteList is None else ids(qs[j].whiteList) for j in rows]
+        set_of, set_rows, set_ix = {}, [], np.full(len(rows), -1, np.int32)
+        for r, j in enumerate(rows):
+            q = qs[j]
+            if q.categories is None and q.categoryBlackList is None:
+                continue
+            key = (None if q.categories is None else frozenset(q.categories),
+                   None if q.categoryBlackList is None else frozenset(q.categoryBlackList))
+            if key not in set_of:
+                set_of[key] = len(set_rows)
+                set_rows.append(category_index(model).excluded(q.categories, q.categoryBlackList))
+            set_ix[r] = set_of[key]
+        qf = native.QueryFilter(len(rows), black, white, set_ix if set_rows else None,
+                                np.stack(set_rows) if set_rows else None)
+        num = max(qs[j].num for j in rows)
+        items, scores, cnt = model.mf.similarProductsBatch(qlists, num, query_filter=qf)
+        for r, j in enumerate(rows):
+            n = min(int(cnt[r]), qs[j].num)
+            out[j] = PredictedResult([ItemScore(model.itemIntStringMap(int(items[r, t])), float(scores[r, t]))
+                                      for t in range(n)])
+        return out
+
 
 class LikeAlgorithm(ALSAlgorithm):
     """like -> +1, dislike -> -1, the latest event of a (user,item) pair wins (LikeAlgorithm.scala:59-108);
@@ -347,7 +393,6 @@ class CooccurrenceAlgorithm(P2LAlgorithm):
         self.ap = ap
 
     def train(self, sc, data) -> CooccurrenceModel:
-        from .. import native
         c = _columns(data)
         if c is None:
             itemMap = BiMap.stringInt(data.items.keys())

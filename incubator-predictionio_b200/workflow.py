@@ -27,7 +27,7 @@ import sys
 import uuid
 from dataclasses import dataclass, field
 from pathlib import Path
-from typing import Any, Dict, List, Optional, Sequence
+from typing import Any, Dict, Iterator, List, Optional, Sequence, Tuple
 
 from .controller import (Engine, EngineFactory, EngineParams, PersistentModelManifest, StopAfterPrepareInterruption,
                          StopAfterReadInterruption, Unit, extract_params)
@@ -339,6 +339,78 @@ def deploy(engineInstanceId: Optional[str] = None, engineId: str = "", engineVer
     sc = WorkflowContext(inst.batch, inst.env, mode="Serving", sparkConf=inst.sparkConf)
     models = engine.prepareDeploy(sc, engineParams, inst.id, Models.get(inst.id))
     return QueryServer(engine, engineParams, models, inst)
+
+
+# ---- batchpredict: a file of queries in, a file of predictions out ------------------------------------
+class BatchPredict:
+    """`pio batchpredict` (core/src/main/scala/org/apache/predictionio/workflow/BatchPredict.scala): every non-blank line
+    of the input is one JSON query; the output holds one compact JSON line {"query": ..., "prediction": ...} per query,
+    in input order.  Where the reference maps `predict` over the queries one by one, the queries here go through
+    every algorithm's predictMany in chunks, a few device calls each."""
+    QUERY_CHUNK = 16384   # queries per predictMany call: enough users / queries for the blocked batch kernels
+
+    @staticmethod
+    def parser() -> argparse.ArgumentParser:
+        ap = argparse.ArgumentParser("BatchPredict")
+        ap.add_argument("--input", default="batchpredict-input.json")
+        ap.add_argument("--output", default="batchpredict-output.json")
+        ap.add_argument("--engine-instance-id")
+        ap.add_argument("--engine-id", default="")
+        ap.add_argument("--engine-version", default="")
+        ap.add_argument("--engine-variant", default="default")
+        ap.add_argument("--query-partitions", type=int)   # partitions of the query RDD: no meaning on one GPU
+        ap.add_argument("--query-chunk", type=int, default=BatchPredict.QUERY_CHUNK)
+        ap.add_argument("--env")
+        ap.add_argument("--verbose", action="store_true")
+        ap.add_argument("--debug", action="store_true")
+        ap.add_argument("--json-extractor", default="Both")
+        return ap
+
+    @staticmethod
+    def read_queries(path: Path, qcls) -> List[Tuple[Any, Any]]:
+        """(query JSON, extracted Query) of every line that is not blank after strip; a line that does not parse raises
+        ValueError naming its line number."""
+        out = []
+        with open(path, encoding="utf-8") as fh:
+            for no, line in enumerate(fh, 1):
+                text = line.strip()
+                if not text:
+                    continue
+                try:
+                    qj = json.loads(text)
+                    out.append((qj, extract_params(qcls, qj) if dataclasses.is_dataclass(qcls) else qj))
+                except Exception as e:   # noqa: BLE001 -- whatever the decoder or the Query class objects to
+                    raise ValueError(f"{path}: line {no} is not a valid query: {e}") from e
+        return out
+
+    @staticmethod
+    def run(server: "QueryServer", queries: Sequence[Tuple[Any, Any]], chunk: int) -> Iterator[Dict[str, Any]]:
+        """The output records of `queries` (pairs of read_queries), in order."""
+        chunk = max(1, int(chunk))
+        for c0 in range(0, len(queries), chunk):
+            part = queries[c0:c0 + chunk]
+            supplemented = [server.serving.supplementBase(q) for _, q in part]
+            per_algo = [a.predictMany(m, supplemented) for a, m in zip(server.algorithms, server.models)]
+            for j, (qj, q) in enumerate(part):
+                r = server.serving.serveBase(q, [p[j] for p in per_algo])
+                yield {"query": to_json(q), "prediction": to_json(r)}   # the extracted Query, as the reference writes it
+
+    @staticmethod
+    def main(argv: Optional[Sequence[str]] = None) -> int:
+        """Returns the number of predictions written."""
+        a, _unknown = BatchPredict.parser().parse_known_args(argv)
+        logging.basicConfig(level=logging.DEBUG if a.debug else logging.INFO if a.verbose else logging.WARNING)
+        if not a.engine_instance_id and not (a.engine_id and a.engine_version):
+            raise SystemExit("BatchPredict: give --engine-instance-id, or --engine-id and --engine-version")
+        server = deploy(a.engine_instance_id, a.engine_id, a.engine_version, a.engine_variant)
+        queries = BatchPredict.read_queries(Path(a.input), server.algorithms[0].queryClass())   # before anything is written
+        n = 0
+        with open(a.output, "w", encoding="utf-8") as out:
+            for rec in BatchPredict.run(server, queries, a.query_chunk):
+                out.write(json.dumps(rec, separators=(",", ":")) + "\n")
+                n += 1
+        logger.info("BatchPredict: %d predictions written to %s", n, a.output)
+        return n
 
 
 if __name__ == "__main__":

@@ -228,6 +228,105 @@ JNIEXPORT void JNICALL JNAME(similarBatch)(JNIEnv* env, jobject self, jlong h, j
   check(env, H(h), rc);
 }
 
+/* the filter arrays of the two filtered calls, pinned for one call (any of them may be null) */
+typedef struct filter_pins {
+  jlong *ex_ptr, *wl_ptr;
+  jint *ex_items, *wl_items, *set_ix;
+  jbyte *has_wl, *item_sets;
+} filter_pins;
+static pio_als_query_filter pin_filter(JNIEnv* env, filter_pins* p, jlongArray exPtr, jintArray exItems, jbyteArray hasWl,
+                                       jlongArray wlPtr, jintArray wlItems, jintArray setIx, jbyteArray itemSets, jint nSets) {
+  pio_als_query_filter f;
+  p->ex_ptr = pin(env, exPtr);
+  p->ex_items = pin(env, exItems);
+  p->has_wl = pin(env, hasWl);
+  p->wl_ptr = pin(env, wlPtr);
+  p->wl_items = pin(env, wlItems);
+  p->set_ix = pin(env, setIx);
+  p->item_sets = pin(env, itemSets);
+  f.ex_ptr = (const int64_t*)p->ex_ptr;
+  f.ex_items = (const int32_t*)p->ex_items;
+  f.has_wl = (const uint8_t*)p->has_wl;
+  f.wl_ptr = (const int64_t*)p->wl_ptr;
+  f.wl_items = (const int32_t*)p->wl_items;
+  f.set_ix = (const int32_t*)p->set_ix;
+  f.item_sets = (const uint8_t*)p->item_sets;
+  f.n_sets = nSets;
+  return f;
+}
+static void unpin_filter(JNIEnv* env, filter_pins* p, jlongArray exPtr, jintArray exItems, jbyteArray hasWl, jlongArray wlPtr,
+                         jintArray wlItems, jintArray setIx, jbyteArray itemSets) {
+  unpin(env, itemSets, p->item_sets, JNI_ABORT);
+  unpin(env, setIx, p->set_ix, JNI_ABORT);
+  unpin(env, wlItems, p->wl_items, JNI_ABORT);
+  unpin(env, wlPtr, p->wl_ptr, JNI_ABORT);
+  unpin(env, hasWl, p->has_wl, JNI_ABORT);
+  unpin(env, exItems, p->ex_items, JNI_ABORT);
+  unpin(env, exPtr, p->ex_ptr, JNI_ABORT);
+}
+
+/* void recommendFiltered(long h, int[] users, int topk, byte[] itemMask, double[] itemWeight, long[] exPtr, int[] exItems,
+ *                        byte[] hasWl, long[] wlPtr, int[] wlItems, int[] setIx, byte[] itemSets, int nSets,
+ *                        int[] outItems, float[] outScores, int[] outCount)       pio_als_query_filter as arrays */
+JNIEXPORT void JNICALL JNAME(recommendFiltered)(JNIEnv* env, jobject self, jlong h, jintArray users, jint topk,
+                                                jbyteArray itemMask, jdoubleArray itemWeight, jlongArray exPtr,
+                                                jintArray exItems, jbyteArray hasWl, jlongArray wlPtr, jintArray wlItems,
+                                                jintArray setIx, jbyteArray itemSets, jint nSets, jintArray outItems,
+                                                jfloatArray outScores, jintArray outCount) {
+  jsize n = (*env)->GetArrayLength(env, users);
+  jint* us = pin(env, users);
+  jbyte* mk = pin(env, itemMask);
+  jdouble* wt = pin(env, itemWeight);
+  jint* oi = pin(env, outItems);
+  jfloat* os = pin(env, outScores);
+  jint* oc = pin(env, outCount);
+  filter_pins fp;
+  pio_als_query_filter f = pin_filter(env, &fp, exPtr, exItems, hasWl, wlPtr, wlItems, setIx, itemSets, nSets);
+  int rc = pio_als_recommend_filtered(H(h), (const int32_t*)us, (int)n, topk, (const uint8_t*)mk, wt, &f, (int32_t*)oi, os,
+                                      (int32_t*)oc);
+  (void)self;
+  unpin_filter(env, &fp, exPtr, exItems, hasWl, wlPtr, wlItems, setIx, itemSets);
+  unpin(env, outCount, oc, 0);
+  unpin(env, outScores, os, 0);
+  unpin(env, outItems, oi, 0);
+  unpin(env, itemWeight, wt, JNI_ABORT);
+  unpin(env, itemMask, mk, JNI_ABORT);
+  unpin(env, users, us, JNI_ABORT);
+  check(env, H(h), rc);
+}
+
+/* void similarBatchFiltered(long h, long[] queryPtr, int[] queryItems, int topk, byte[] itemMask, double[] itemWeight,
+ *                           int flags, <the filter arrays as above>, int[] outItems, float[] outScores, int[] outCount) */
+JNIEXPORT void JNICALL JNAME(similarBatchFiltered)(JNIEnv* env, jobject self, jlong h, jlongArray queryPtr,
+                                                   jintArray queryItems, jint topk, jbyteArray itemMask,
+                                                   jdoubleArray itemWeight, jint flags, jlongArray exPtr, jintArray exItems,
+                                                   jbyteArray hasWl, jlongArray wlPtr, jintArray wlItems, jintArray setIx,
+                                                   jbyteArray itemSets, jint nSets, jintArray outItems,
+                                                   jfloatArray outScores, jintArray outCount) {
+  jsize nqr = (*env)->GetArrayLength(env, queryPtr) - 1;
+  jlong* qp = pin(env, queryPtr);
+  jint* q = pin(env, queryItems);
+  jbyte* mk = pin(env, itemMask);
+  jdouble* wt = pin(env, itemWeight);
+  jint* oi = pin(env, outItems);
+  jfloat* os = pin(env, outScores);
+  jint* oc = pin(env, outCount);
+  filter_pins fp;
+  pio_als_query_filter f = pin_filter(env, &fp, exPtr, exItems, hasWl, wlPtr, wlItems, setIx, itemSets, nSets);
+  int rc = pio_als_similar_batch_filtered(H(h), (const int64_t*)qp, (const int32_t*)q, (int)nqr, topk, (const uint8_t*)mk, wt,
+                                          flags, &f, (int32_t*)oi, os, (int32_t*)oc);
+  (void)self;
+  unpin_filter(env, &fp, exPtr, exItems, hasWl, wlPtr, wlItems, setIx, itemSets);
+  unpin(env, outCount, oc, 0);
+  unpin(env, outScores, os, 0);
+  unpin(env, outItems, oi, 0);
+  unpin(env, itemWeight, wt, JNI_ABORT);
+  unpin(env, itemMask, mk, JNI_ABORT);
+  unpin(env, queryItems, q, JNI_ABORT);
+  unpin(env, queryPtr, qp, JNI_ABORT);
+  check(env, H(h), rc);
+}
+
 /* void save(long h, String path) */
 JNIEXPORT void JNICALL JNAME(save)(JNIEnv* env, jobject self, jlong h, jstring path) {
   const char* p = (*env)->GetStringUTFChars(env, path, NULL);

@@ -39,6 +39,16 @@ object NativeALS {
     flags: Int, outItems: Array[Int], outScores: Array[Float]): Int
   @native def similarBatch(h: Long, queryPtr: Array[Long], queryItems: Array[Int], topk: Int, itemMask: Array[Byte],
     itemWeight: Array[Double], flags: Int, outItems: Array[Int], outScores: Array[Float], outCount: Array[Int]): Unit
+  /** recommend / similarBatch with a filter per query (pio_als_query_filter as arrays, any of them null): exclusion
+    * lists (exPtr / exItems), white lists (hasWl / wlPtr / wlItems) and shared set rows (setIx into itemSets). */
+  @native def recommendFiltered(h: Long, users: Array[Int], topk: Int, itemMask: Array[Byte], itemWeight: Array[Double],
+    exPtr: Array[Long], exItems: Array[Int], hasWl: Array[Byte], wlPtr: Array[Long], wlItems: Array[Int],
+    setIx: Array[Int], itemSets: Array[Byte], nSets: Int, outItems: Array[Int], outScores: Array[Float],
+    outCount: Array[Int]): Unit
+  @native def similarBatchFiltered(h: Long, queryPtr: Array[Long], queryItems: Array[Int], topk: Int,
+    itemMask: Array[Byte], itemWeight: Array[Double], flags: Int, exPtr: Array[Long], exItems: Array[Int],
+    hasWl: Array[Byte], wlPtr: Array[Long], wlItems: Array[Int], setIx: Array[Int], itemSets: Array[Byte], nSets: Int,
+    outItems: Array[Int], outScores: Array[Float], outCount: Array[Int]): Unit
   @native def save(h: Long, path: String): Unit
   @native def load(path: String, device: Int): Long
   @native def importModel(rank: Int, nUsers: Int, nItems: Int, device: Int, userFactors: Array[Float],
