@@ -272,6 +272,46 @@ PIO_API int pio_als_synth_ratings_device(int device, int32_t n_users, int32_t n_
 PIO_API int pio_ids_encode(int device, const uint8_t* bytes, const int64_t* offsets, int64_t n, int32_t* out_index,
                            int64_t* out_first, int32_t* out_n_unique);
 
+/* k-fold evaluation on the device: the recommendation template's `pio eval` (examples/scala-parallel-recommendation/
+ * blacklist-items/src/main/scala/{DataSource.scala readEval, Evaluation.scala}) without per-rating host objects
+ * (DESIGN.md 4.11).  An opaque object owns device copies of n ratings given by GLOBAL user / item indices (pio_ids_encode
+ * of the whole columns) and their fp64 values; rating e is in the test set of fold e % k_fold and in the training set of
+ * every other fold.  Per fold f, as the template computes them from that fold's strings:
+ *   users / items  BiMap.stringInt of the training ratings: fold-local indices in order of first training occurrence
+ *   training COO   the training ratings in rating order (fold-local indices, float32 ratings)
+ *   queries        the distinct users of the test ratings in order of first occurrence among them (the template's
+ *                  by_user order); each with its fold-local training index, or -1 when it has no training rating
+ * Errors: status codes as above, text via pio_als_last_error(NULL); arguments are checked before any device work. */
+typedef struct pio_eval_folds pio_eval_folds;
+
+/* user, item: n global indices >= 0 each (HOST); rating: n fp64 (HOST); 1 <= n < 2^31, k_fold >= 1. */
+PIO_API int pio_eval_folds_create(int device, const int32_t* user, const int32_t* item, const double* rating, int64_t n,
+                                  int32_t k_fold, pio_eval_folds** out);
+/* out[0] users, out[1] items, out[2] training ratings, out[3] queries of fold `fold`. */
+PIO_API int pio_eval_folds_sizes(const pio_eval_folds* ef, int32_t fold, int64_t out[4]);
+/* HOST, each nullable: user (out[0] entries) / item (out[1]) = global index of each fold-local index; query_user
+ * (out[3]) = global user of each query; query_train_user (out[3]) = its fold-local training index or -1. */
+PIO_API int pio_eval_folds_maps(const pio_eval_folds* ef, int32_t fold, int32_t* user, int32_t* item,
+                                int32_t* query_user, int32_t* query_train_user);
+/* pio_als_set_ratings_coo_device(h, fold's training COO, PIO_ALS_DEDUP_NONE) on a handle created with the fold's
+ * user and item counts on the same device (world_size 1). */
+PIO_API int pio_eval_folds_set_ratings(pio_eval_folds* ef, int32_t fold, pio_als_handle* h);
+/* Keeps a top-N result of fold `fold` on the object: items (n_queries x num, fold-local item indices, as
+ * pio_als_recommend returns them for the fold's query_train_user) and count (valid entries per query, 0..num);
+ * n_queries must be the fold's.  *out_result names it until pio_eval_folds_result_free; results of any folds may be
+ * kept at once. */
+PIO_API int pio_eval_folds_result_add(pio_eval_folds* ef, int32_t fold, const int32_t* items, const int32_t* count,
+                                      int32_t n_queries, int32_t num, int32_t* out_result);
+PIO_API int pio_eval_folds_result_free(pio_eval_folds* ef, int32_t result);
+/* Per query q of the result's fold (HOST, n_queries each), ratings compared in fp64 with rating >= threshold:
+ *   hits[q]  of the first min(k, count[q]) predicted items, those whose largest test rating of q passes
+ *   npos[q]  distinct test items of q whose largest rating passes (items unknown to the fold's training count too)
+ *   nraw[q]  test ratings of q that pass
+ * PrecisionAtK = hits / min(k, npos) where npos > 0; PositiveCount = nraw (Evaluation.scala:32-62).  k >= 1. */
+PIO_API int pio_eval_folds_rank_counts(pio_eval_folds* ef, int32_t result, int32_t k, double threshold, int32_t* hits,
+                                       int32_t* npos, int32_t* nraw);
+PIO_API int pio_eval_folds_destroy(pio_eval_folds* ef);
+
 /* Event file scan: PEventStore.find (data/src/main/scala/org/apache/predictionio/data/store/PEventStore.scala:59-119)
  * over text in the `pio import` / `pio export` JSON-lines format (tools/src/main/scala/org/apache/predictionio/tools/
  * imprt/FileToEvents.scala:93-103), producing event columns instead of Event objects (DESIGN.md 3.1).

@@ -391,6 +391,29 @@ class Engine:
             results.append((ei, qpa))
         return results
 
+    def evalColumns(self, sc, engineParams: EngineParams, readCache: Optional[list] = None):
+        """eval for components that keep a fold's data as columns: DataSource.readEvalColumns gives per fold
+        (trainingData, evalInfo, queries), every algorithm's batchPredictColumns(sc, model, queries) scores the queries in
+        one call and Serving.serveColumns(queries, predictions) combines them.  Returns [(evalInfo, queries, served), ...],
+        or None when the datasource declines (readEvalColumns returned None: its data needs eval).  readCache: a list
+        shared by the calls of one evaluation, holding readEvalColumns' result per datasource (class, params), so that
+        parameter sets with equal datasource params read and split the data once."""
+        dataSource, preparator, algorithms, serving = self._components(engineParams)
+        key = (type(dataSource), engineParams.dataSourceParams[1])
+        cached = [v for k, v in (readCache or ()) if k == key]
+        folds = cached[0] if cached else dataSource.readEvalColumns(sc)
+        if readCache is not None and not cached:
+            readCache.append((key, folds))
+        if folds is None:
+            return None
+        results = []
+        for td, ei, queries in folds:
+            pd = preparator.prepareBase(sc, td)
+            models = [a.trainBase(sc, pd) for a in algorithms]
+            predictions = [a.batchPredictColumns(sc, m, queries) for a, m in zip(algorithms, models)]
+            results.append((ei, queries, serving.serveColumns(queries, predictions)))
+        return results
+
 
 class EngineFactory:
     def apply(self) -> Engine:

@@ -54,6 +54,7 @@
 #include "events_index.cuh"
 #include "cooc.cuh"
 #include "forest.cuh"
+#include "eval_folds.cuh"
 
 namespace pio {
 
@@ -4904,6 +4905,335 @@ __attribute__((visibility("default"))) int pio_rf_debug_timing(double out[70]) {
   out[0] = t.h2d, out[1] = t.split, out[2] = t.bin, out[3] = t.hist, out[4] = t.sel, out[5] = t.upd;
   out[6] = t.levels, out[7] = t.groups;
   for (int l = 0; l <= RF_MAX_DEPTH; ++l) out[8 + l] = t.hist_l[l], out[39 + l] = t.sel_l[l];
+  return PIO_ALS_OK;
+}
+
+}  // extern "C"
+
+// ---- k-fold evaluation (eval_folds.cuh; DESIGN.md 4.11) ----------------------------------------------------------------
+struct pio_eval_folds {
+  struct Fold {
+    int n_users = 0, n_items = 0, nq = 0;
+    long long n_train = 0, n_test = 0;
+    int *uloc = nullptr, *iloc = nullptr;   // global -> fold-local (-1: not in the training set)
+    int *ul2g = nullptr, *il2g = nullptr;   // fold-local -> global
+    int *q2g = nullptr, *qtrain = nullptr;  // per query: global user, fold-local training user or -1
+    int *qptr = nullptr;                    // [nq + 1] test ratings of query q, sorted by global item: raw[qptr[q] ..)
+    double* raw = nullptr;
+    int *dptr = nullptr, *ditem = nullptr;  // [nq + 1] distinct test items of query q: ditem / dmax[dptr[q] ..)
+    double* dmax = nullptr;
+  };
+  struct Result {
+    int fold = 0, nq = 0, num = 0;
+    int *items = nullptr, *count = nullptr;
+  };
+  int device = 0, k_fold = 1, n_users = 0, n_items = 0;   // n_users / n_items: global index ranges
+  long long n = 0;
+  cudaStream_t st = nullptr;
+  int *gu = nullptr, *gi = nullptr;
+  double* r = nullptr;
+  std::vector<Fold> folds;
+  std::map<int32_t, Result> results;
+  int32_t next_result = 0;
+  std::vector<void*> mem;   // the object's device memory, results excepted
+};
+
+namespace pio {
+
+__global__ void evf_fill_kernel(int* __restrict__ p, long long n, int v) {
+  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < n) p[i] = v;
+}
+
+template <class T>
+static int evf_alloc(pio_eval_folds* ef, T** p, size_t n) {
+  CK0(cudaMalloc((void**)p, (n ? n : 1) * sizeof(T)));
+  ef->mem.push_back((void*)*p);
+  return PIO_ALS_OK;
+}
+
+static int evf_read(const uint32_t* d, cudaStream_t st, uint32_t* out) {
+  CK0(cudaMemcpyAsync(out, d, sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
+  CK0(cudaStreamSynchronize(st));
+  return PIO_ALS_OK;
+}
+
+#define EVF(call)                          \
+  do {                                     \
+    const int rc_ = (call);                \
+    if (rc_ != PIO_ALS_OK) return rc_;     \
+  } while (0)
+
+// Fold f's maps of one side (global ids 0 .. n_ids): loc (global -> local), l2g and their count.  flag: n + 1 entries.
+static int evf_side(pio_eval_folds* ef, int f, const int* e1, const int* e2, int n_ids, uint32_t* flag, int** loc,
+                    int** l2g, int* count) {
+  const cudaStream_t st = ef->st;
+  const long long n = ef->n;
+  CK0(cudaMemsetAsync(flag, 0, sizeof(uint32_t) * (size_t)(n + 1), st));
+  evf::train_flag_kernel<<<nblk(n_ids, 256), 256, 0, st>>>(e1, e2, n_ids, ef->k_fold, f, flag);
+  CK0(scan_exclusive_u32(flag, flag, (size_t)n + 1, st, nullptr));
+  uint32_t total = 0;
+  EVF(evf_read(flag + n, st, &total));
+  *count = (int)total;
+  EVF(evf_alloc(ef, loc, (size_t)n_ids));
+  EVF(evf_alloc(ef, l2g, (size_t)total));
+  evf::train_index_kernel<<<nblk(n_ids, 256), 256, 0, st>>>(e1, e2, n_ids, ef->k_fold, f, flag, *loc, *l2g);
+  CK0(cudaGetLastError());
+  return PIO_ALS_OK;
+}
+
+// Uploads the ratings and builds every fold: maps, queries and sorted test lists.
+static int evf_build(pio_eval_folds* ef, const int32_t* user, const int32_t* item, const double* rating) {
+  const cudaStream_t st = ef->st;
+  const long long n = ef->n;
+  const int K = ef->k_fold;
+  EVF(evf_alloc(ef, &ef->gu, (size_t)n));
+  EVF(evf_alloc(ef, &ef->gi, (size_t)n));
+  EVF(evf_alloc(ef, &ef->r, (size_t)n));
+  CK0(cudaMemcpyAsync(ef->gu, user, sizeof(int) * (size_t)n, cudaMemcpyHostToDevice, st));
+  CK0(cudaMemcpyAsync(ef->gi, item, sizeof(int) * (size_t)n, cudaMemcpyHostToDevice, st));
+  CK0(cudaMemcpyAsync(ef->r, rating, sizeof(double) * (size_t)n, cudaMemcpyHostToDevice, st));
+  CallMem tmp(st);
+  int *ue1, *ue2, *ie1, *ie2, *qfirst;
+  uint32_t *uflag, *iflag, *qflag, *dflag;
+  const long long m_max = (n + K - 1) / K;   // fold 0 has the most test ratings
+  for (int** p : {&ue1, &ue2, &qfirst}) CK0(tmp.device(p, (size_t)ef->n_users));
+  for (int** p : {&ie1, &ie2}) CK0(tmp.device(p, (size_t)ef->n_items));
+  for (uint32_t** p : {&uflag, &iflag}) CK0(tmp.device(p, (size_t)n + 1));
+  for (uint32_t** p : {&qflag, &dflag}) CK0(tmp.device(p, (size_t)m_max + 1));
+  SortBufs sb;
+  for (int i : {0, 1}) {
+    CK0(tmp.device(&sb.k[i], (size_t)m_max));
+    CK0(tmp.device(&sb.v[i], (size_t)m_max));
+  }
+  struct { const int* g; int* e1; int* e2; int n_ids; } sides[2] = {{ef->gu, ue1, ue2, ef->n_users},
+                                                                    {ef->gi, ie1, ie2, ef->n_items}};
+  for (auto& s : sides) {
+    for (int* p : {s.e1, s.e2}) evf_fill_kernel<<<nblk(s.n_ids, 256), 256, 0, st>>>(p, s.n_ids, evf::NONE);
+    evf::first_pos_kernel<<<nblk(n, 256), 256, 0, st>>>(s.g, n, s.e1);
+    evf::second_pos_kernel<<<nblk(n, 256), 256, 0, st>>>(s.g, n, K, s.e1, s.e2);
+  }
+  CK0(cudaGetLastError());
+  const int ibits = ceil_log2((uint64_t)ef->n_items);
+  ef->folds.resize(K);
+  for (int f = 0; f < K; ++f) {
+    pio_eval_folds::Fold& F = ef->folds[f];
+    const long long m = (n + K - 1 - f) / K;
+    F.n_test = m;
+    F.n_train = n - m;
+    EVF(evf_side(ef, f, ue1, ue2, ef->n_users, uflag, &F.uloc, &F.ul2g, &F.n_users));
+    EVF(evf_side(ef, f, ie1, ie2, ef->n_items, iflag, &F.iloc, &F.il2g, &F.n_items));
+    if (m == 0) continue;
+    evf_fill_kernel<<<nblk(ef->n_users, 256), 256, 0, st>>>(qfirst, ef->n_users, evf::NONE);
+    evf::query_first_kernel<<<nblk(m, 256), 256, 0, st>>>(ef->gu, K, f, m, qfirst);
+    evf::query_flag_kernel<<<nblk(m + 1, 256), 256, 0, st>>>(ef->gu, K, f, m, qfirst, qflag);
+    CK0(scan_exclusive_u32(qflag, qflag, (size_t)m + 1, st, nullptr));
+    uint32_t nq = 0;
+    EVF(evf_read(qflag + m, st, &nq));
+    F.nq = (int)nq;
+    EVF(evf_alloc(ef, &F.q2g, nq));
+    EVF(evf_alloc(ef, &F.qtrain, nq));
+    EVF(evf_alloc(ef, &F.qptr, (size_t)nq + 1));
+    EVF(evf_alloc(ef, &F.dptr, (size_t)nq + 1));
+    EVF(evf_alloc(ef, &F.raw, (size_t)m));
+    sb.live = 0;
+    evf::query_index_kernel<<<nblk(m, 256), 256, 0, st>>>(ef->gu, ef->gi, K, f, m, qfirst, qflag, F.uloc, ibits, F.q2g,
+                                                         F.qtrain, sb.keys(), sb.vals());
+    CK0(radix_sort_pairs(sb, (size_t)m, ceil_log2(nq) + ibits, st, nullptr));
+    evf::test_slots_kernel<<<nblk(m + 1, 256), 256, 0, st>>>(sb.keys(), sb.vals(), m, K, f, ef->r, ibits, (int)nq, F.raw,
+                                                            F.qptr, dflag);
+    CK0(scan_exclusive_u32(dflag, dflag, (size_t)m + 1, st, nullptr));
+    uint32_t nd = 0;
+    EVF(evf_read(dflag + m, st, &nd));
+    EVF(evf_alloc(ef, &F.ditem, nd));
+    EVF(evf_alloc(ef, &F.dmax, nd));
+    evf::test_distinct_kernel<<<nblk(m, 256), 256, 0, st>>>(sb.keys(), m, F.raw, dflag, (1ull << ibits) - 1ull, F.ditem,
+                                                           F.dmax);
+    evf::test_dptr_kernel<<<nblk((long long)nq + 1, 256), 256, 0, st>>>(F.qptr, dflag, (int)nq, F.dptr);
+    CK0(cudaGetLastError());
+  }
+  CK0(cudaStreamSynchronize(st));
+  return PIO_ALS_OK;
+}
+
+static int evf_fold(const pio_eval_folds* ef, int32_t fold, const char* what) {
+  if (!ef) return fail(nullptr, PIO_ALS_ERR_ARG, "%s: null object", what);
+  if (fold < 0 || fold >= ef->k_fold)
+    return fail(nullptr, PIO_ALS_ERR_ARG, "%s: fold %d outside 0..%d", what, fold, ef->k_fold - 1);
+  return PIO_ALS_OK;
+}
+
+}  // namespace pio
+
+extern "C" {
+
+int pio_eval_folds_create(int device, const int32_t* user, const int32_t* item, const double* rating, int64_t n,
+                          int32_t k_fold, pio_eval_folds** out) {
+  if (!out) return fail(nullptr, PIO_ALS_ERR_ARG, "bad pio_eval_folds_create arguments");
+  *out = nullptr;
+  if (!user || !item || !rating || n < 1 || k_fold < 1)
+    return fail(nullptr, PIO_ALS_ERR_ARG, "bad pio_eval_folds_create arguments (n >= 1 and k_fold >= 1)");
+  if (n >= (1ll << 31)) return fail(nullptr, PIO_ALS_ERR_ARG, "n must be < 2^31");
+  int32_t mu = -1, mi = -1;
+  for (int64_t e = 0; e < n; ++e) {
+    if (user[e] < 0 || item[e] < 0)
+      return fail(nullptr, PIO_ALS_ERR_ARG, "rating %lld: negative user or item index", (long long)e);
+    mu = std::max(mu, user[e]);
+    mi = std::max(mi, item[e]);
+  }
+  CK0(cudaSetDevice(device));
+  auto* ef = new pio_eval_folds;
+  ef->device = device;
+  ef->k_fold = k_fold;
+  ef->n = n;
+  ef->n_users = mu + 1;
+  ef->n_items = mi + 1;
+  const cudaError_t e = cudaStreamCreateWithFlags(&ef->st, cudaStreamNonBlocking);
+  if (e != cudaSuccess) {
+    delete ef;
+    return fail(nullptr, PIO_ALS_ERR_CUDA, "cudaStreamCreate: %s", cudaGetErrorString(e));
+  }
+  const int rc = evf_build(ef, user, item, rating);
+  if (rc != PIO_ALS_OK) {
+    pio_eval_folds_destroy(ef);
+    return rc;
+  }
+  *out = ef;
+  return PIO_ALS_OK;
+}
+
+int pio_eval_folds_sizes(const pio_eval_folds* ef, int32_t fold, int64_t out[4]) {
+  EVF(evf_fold(ef, fold, "pio_eval_folds_sizes"));
+  if (!out) return fail(nullptr, PIO_ALS_ERR_ARG, "pio_eval_folds_sizes: null out");
+  const pio_eval_folds::Fold& F = ef->folds[fold];
+  out[0] = F.n_users, out[1] = F.n_items, out[2] = F.n_train, out[3] = F.nq;
+  return PIO_ALS_OK;
+}
+
+int pio_eval_folds_maps(const pio_eval_folds* ef, int32_t fold, int32_t* user, int32_t* item, int32_t* query_user,
+                        int32_t* query_train_user) {
+  EVF(evf_fold(ef, fold, "pio_eval_folds_maps"));
+  CK0(cudaSetDevice(ef->device));
+  const pio_eval_folds::Fold& F = ef->folds[fold];
+  const struct { int32_t* to; const int* from; int count; } jobs[4] = {
+      {user, F.ul2g, F.n_users}, {item, F.il2g, F.n_items}, {query_user, F.q2g, F.nq}, {query_train_user, F.qtrain, F.nq}};
+  for (const auto& j : jobs)
+    if (j.to && j.count) CK0(cudaMemcpyAsync(j.to, j.from, sizeof(int32_t) * (size_t)j.count, cudaMemcpyDeviceToHost, ef->st));
+  CK0(cudaStreamSynchronize(ef->st));
+  return PIO_ALS_OK;
+}
+
+int pio_eval_folds_set_ratings(pio_eval_folds* ef, int32_t fold, pio_als_handle* h) {
+  EVF(evf_fold(ef, fold, "pio_eval_folds_set_ratings"));
+  const pio_eval_folds::Fold& F = ef->folds[fold];
+  if (!h) return fail(nullptr, PIO_ALS_ERR_ARG, "pio_eval_folds_set_ratings: null handle");
+  if (h->cfg.device != ef->device || h->cfg.world_size != 1 || h->cfg.n_users != F.n_users || h->cfg.n_items != F.n_items)
+    return fail(nullptr, PIO_ALS_ERR_ARG, "pio_eval_folds_set_ratings: the handle (device %d, world_size %d, %d users, "
+                "%d items) does not match fold %d (device %d, %d users, %d items)", h->cfg.device, h->cfg.world_size,
+                h->cfg.n_users, h->cfg.n_items, fold, ef->device, F.n_users, F.n_items);
+  if (F.n_train == 0) return fail(nullptr, PIO_ALS_ERR_ARG, "fold %d has no training ratings", fold);
+  CK0(cudaSetDevice(ef->device));
+  int rc;
+  {
+    CallMem tmp(ef->st);
+    int *du = nullptr, *di = nullptr;
+    float* dv = nullptr;
+    CK0(tmp.device(&du, (size_t)F.n_train));
+    CK0(tmp.device(&di, (size_t)F.n_train));
+    CK0(tmp.device(&dv, (size_t)F.n_train));
+    evf::train_coo_kernel<<<nblk(ef->n, 256), 256, 0, ef->st>>>(ef->gu, ef->gi, ef->r, ef->n, ef->k_fold, fold, F.uloc,
+                                                               F.iloc, du, di, dv);
+    CK0(cudaGetLastError());
+    CK0(cudaStreamSynchronize(ef->st));
+    rc = pio_als_set_ratings_coo_device(h, du, di, dv, F.n_train, PIO_ALS_DEDUP_NONE, nullptr);
+  }
+  if (rc != PIO_ALS_OK) return fail(nullptr, rc, "%s", h->err.c_str());
+  return PIO_ALS_OK;
+}
+
+int pio_eval_folds_result_add(pio_eval_folds* ef, int32_t fold, const int32_t* items, const int32_t* count,
+                              int32_t n_queries, int32_t num, int32_t* out_result) {
+  EVF(evf_fold(ef, fold, "pio_eval_folds_result_add"));
+  const pio_eval_folds::Fold& F = ef->folds[fold];
+  if (!out_result || num < 1 || n_queries != F.nq || (n_queries > 0 && (!items || !count)))
+    return fail(nullptr, PIO_ALS_ERR_ARG, "bad pio_eval_folds_result_add arguments (fold %d has %d queries)", fold, F.nq);
+  for (int32_t q = 0; q < n_queries; ++q) {
+    if (count[q] < 0 || count[q] > num)
+      return fail(nullptr, PIO_ALS_ERR_ARG, "query %d: count %d outside 0..%d", q, count[q], num);
+    for (int32_t j = 0; j < count[q]; ++j) {
+      const int32_t it = items[(int64_t)q * num + j];
+      if (it < 0 || it >= F.n_items)
+        return fail(nullptr, PIO_ALS_ERR_ARG, "query %d: item %d outside the fold's %d items", q, it, F.n_items);
+    }
+  }
+  CK0(cudaSetDevice(ef->device));
+  pio_eval_folds::Result R;
+  R.fold = fold, R.nq = n_queries, R.num = num;
+  cudaError_t e = cudaMalloc((void**)&R.items, sizeof(int32_t) * ((size_t)n_queries * num + 1));
+  if (e == cudaSuccess) e = cudaMalloc((void**)&R.count, sizeof(int32_t) * ((size_t)n_queries + 1));
+  if (e == cudaSuccess && n_queries > 0)
+    e = cudaMemcpyAsync(R.items, items, sizeof(int32_t) * (size_t)n_queries * num, cudaMemcpyHostToDevice, ef->st);
+  if (e == cudaSuccess && n_queries > 0)
+    e = cudaMemcpyAsync(R.count, count, sizeof(int32_t) * (size_t)n_queries, cudaMemcpyHostToDevice, ef->st);
+  if (e == cudaSuccess) e = cudaStreamSynchronize(ef->st);
+  if (e != cudaSuccess) {
+    cudaFree(R.items);
+    cudaFree(R.count);
+    return fail(nullptr, PIO_ALS_ERR_CUDA, "pio_eval_folds_result_add: %s", cudaGetErrorString(e));
+  }
+  *out_result = ef->next_result++;
+  ef->results[*out_result] = R;
+  return PIO_ALS_OK;
+}
+
+int pio_eval_folds_result_free(pio_eval_folds* ef, int32_t result) {
+  if (!ef) return fail(nullptr, PIO_ALS_ERR_ARG, "pio_eval_folds_result_free: null object");
+  auto it = ef->results.find(result);
+  if (it == ef->results.end()) return fail(nullptr, PIO_ALS_ERR_ARG, "no result %d", result);
+  cudaSetDevice(ef->device);
+  cudaFree(it->second.items);
+  cudaFree(it->second.count);
+  ef->results.erase(it);
+  return PIO_ALS_OK;
+}
+
+int pio_eval_folds_rank_counts(pio_eval_folds* ef, int32_t result, int32_t k, double threshold, int32_t* hits,
+                               int32_t* npos, int32_t* nraw) {
+  if (!ef) return fail(nullptr, PIO_ALS_ERR_ARG, "pio_eval_folds_rank_counts: null object");
+  auto it = ef->results.find(result);
+  if (it == ef->results.end()) return fail(nullptr, PIO_ALS_ERR_ARG, "no result %d", result);
+  const pio_eval_folds::Result& R = it->second;
+  if (k < 1 || (R.nq > 0 && (!hits || !npos || !nraw)))
+    return fail(nullptr, PIO_ALS_ERR_ARG, "bad pio_eval_folds_rank_counts arguments (k >= 1)");
+  if (R.nq == 0) return PIO_ALS_OK;
+  CK0(cudaSetDevice(ef->device));
+  const pio_eval_folds::Fold& F = ef->folds[R.fold];
+  const cudaStream_t st = ef->st;
+  CallMem tmp(st);
+  int* d = nullptr;
+  CK0(tmp.device(&d, 3 * (size_t)R.nq));
+  evf::rank_counts_kernel<<<nblk(R.nq, evf::RC_WARPS), 32 * evf::RC_WARPS, 0, st>>>(
+      R.items, R.count, R.num, R.nq, k, threshold, F.il2g, F.qptr, F.raw, F.dptr, F.ditem, F.dmax, d, d + R.nq,
+      d + 2 * (size_t)R.nq);
+  CK0(cudaGetLastError());
+  int32_t* outs[3] = {hits, npos, nraw};
+  for (int j = 0; j < 3; ++j)
+    CK0(cudaMemcpyAsync(outs[j], d + (size_t)j * R.nq, sizeof(int32_t) * (size_t)R.nq, cudaMemcpyDeviceToHost, st));
+  CK0(cudaStreamSynchronize(st));
+  return PIO_ALS_OK;
+}
+
+int pio_eval_folds_destroy(pio_eval_folds* ef) {
+  if (!ef) return PIO_ALS_OK;
+  cudaSetDevice(ef->device);
+  if (ef->st) cudaStreamSynchronize(ef->st);
+  for (auto& kv : ef->results) {
+    cudaFree(kv.second.items);
+    cudaFree(kv.second.count);
+  }
+  for (void* p : ef->mem) cudaFree(p);
+  if (ef->st) cudaStreamDestroy(ef->st);
+  delete ef;
   return PIO_ALS_OK;
 }
 

@@ -104,12 +104,21 @@ class MetricEvaluatorResult:
     engineParamsScores: List[Tuple[Any, MetricScores]]
 
 
+class EvalColumns(list):
+    """One parameter set's folds from Engine.evalColumns, [(evalInfo, queries, served), ...]: metrics take it through
+    calculate_columns."""
+
+
+def _calculate(metric, sc, ds):
+    return metric.calculate_columns(sc, ds) if isinstance(ds, EvalColumns) else metric.calculate(sc, ds)
+
+
 class MetricEvaluator:
     def __init__(self, metric: Metric, otherMetrics: Sequence[Metric] = ()):
         self.metric, self.otherMetrics = metric, list(otherMetrics)
 
     def evaluateBase(self, sc, engineEvalDataSet) -> MetricEvaluatorResult:
-        results = [(ep, MetricScores(self.metric.calculate(sc, ds), [m.calculate(sc, ds) for m in self.otherMetrics]))
+        results = [(ep, MetricScores(_calculate(self.metric, sc, ds), [_calculate(m, sc, ds) for m in self.otherMetrics]))
                    for ep, ds in engineEvalDataSet]
         best = 0
         for i in range(1, len(results)):   # reduce { (x, y) => if (compare(x, y) >= 0) x else y }: first maximum wins
@@ -131,12 +140,35 @@ class EngineParamsGenerator:
 
 def run_evaluation(evaluation: Evaluation, generator: EngineParamsGenerator, sc=None) -> MetricEvaluatorResult:
     """CoreWorkflow.runEvaluation / EvaluationWorkflow.runEvaluation: Engine.batchEval over the parameter sets, then the
-    evaluator.  One WorkflowContext (= one GPU) serves all trainings."""
+    evaluator.  One WorkflowContext (= one GPU) serves all trainings.
+
+    A parameter set whose components all keep folds as columns (_columnar) runs through Engine.evalColumns: the split,
+    the trainings' input, top-N and the metrics' counts stay on the device, and the datasource is read once per
+    (class, params) for all parameter sets.  Any other runs through Engine.eval."""
     from .workflow import WorkflowContext
     sc = sc or WorkflowContext(mode="Evaluation")
     engine = evaluation.engine
     data = []
+    read_cache = []
     for ep in generator.engineParamsList:
-        folds = engine.eval(sc, ep)                      # [(evalInfo, [(q, p, a), ...]), ...] -- one training per fold
+        folds = None
+        if _columnar(engine, ep, evaluation.evaluator, sc):
+            cols = engine.evalColumns(sc, ep, read_cache)
+            folds = None if cols is None else EvalColumns(cols)
+        if folds is None:
+            folds = engine.eval(sc, ep)                  # [(evalInfo, [(q, p, a), ...]), ...] -- one training per fold
         data.append((ep, folds))
     return evaluation.evaluator.evaluateBase(sc, data)
+
+
+def _columnar(engine, ep, evaluator, sc) -> bool:
+    """Every piece opts in to columns: the datasource (readEvalColumns), every algorithm (batchPredictColumns), the
+    serving (serveColumns, with the default supplement: a supplemented query would not be the datasource's) and every
+    metric of the evaluator (calculate_columns); and one process (world_size 1) runs the evaluation."""
+    from .controller import LServing
+    if getattr(sc, "world_size", 1) != 1:
+        return False
+    dataSource, _, algorithms, serving = engine._components(ep)
+    return (hasattr(dataSource, "readEvalColumns") and all(hasattr(a, "batchPredictColumns") for a in algorithms)
+            and hasattr(serving, "serveColumns") and type(serving).supplement is LServing.supplement
+            and all(hasattr(m, "calculate_columns") for m in (evaluator.metric, *evaluator.otherMetrics)))

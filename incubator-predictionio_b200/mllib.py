@@ -140,6 +140,22 @@ class ALS:
             raise ValueError("requirement failed: ratings cannot be empty")
         nu = int(n_users) if n_users is not None else int(u.max()) + 1
         npr = int(n_products) if n_products is not None else int(p.max()) + 1
+        h = self._native(nu, npr, sc, init is not None)
+        uf, pf, uh, ph = h.train(u, p, r, self.iterations, dedup=DEDUP[self.dedup], ts=ts,
+                                 user_init=None if init is None else init[0],
+                                 item_init=None if init is None else init[1])
+        return MatrixFactorizationModel(self.rank, uf, pf, uh, ph, h)
+
+    def runFilled(self, set_ratings, n_users: int, n_products: int, sc=None) -> MatrixFactorizationModel:
+        """run() on ratings that are already on the device: set_ratings(handle) loads them into the new handle (e.g.
+        EvalFolds.set_ratings of one fold); hash-initialised factors."""
+        h = self._native(int(n_users), int(n_products), sc, False)
+        set_ratings(h)
+        h.run(self.iterations)
+        uf, pf, uh, ph = h.get_factors()
+        return MatrixFactorizationModel(self.rank, uf, pf, uh, ph, h)
+
+    def _native(self, nu: int, npr: int, sc, caller_init: bool) -> native.NativeALS:
         world, wrank, nccl_id = 1, 0, None
         device = self.device
         if sc is not None:
@@ -147,13 +163,9 @@ class ALS:
             world, wrank, nccl_id = getattr(sc, "world_size", 1), getattr(sc, "world_rank", 0), None
             if world > 1:
                 nccl_id = sc.new_nccl_id()
-        h = native.NativeALS(self.rank, nu, npr, lam=self.lambda_, implicit=self.implicitPrefs, alpha=self.alpha,
-                             seed=self.seed, device=device, world_size=world, world_rank=wrank, nccl_id=nccl_id,
-                             init_mode=native.INIT_CALLER if init is not None else native.INIT_HASH)
-        uf, pf, uh, ph = h.train(u, p, r, self.iterations, dedup=DEDUP[self.dedup], ts=ts,
-                                 user_init=None if init is None else init[0],
-                                 item_init=None if init is None else init[1])
-        return MatrixFactorizationModel(self.rank, uf, pf, uh, ph, h)
+        return native.NativeALS(self.rank, nu, npr, lam=self.lambda_, implicit=self.implicitPrefs, alpha=self.alpha,
+                                seed=self.seed, device=device, world_size=world, world_rank=wrank, nccl_id=nccl_id,
+                                init_mode=native.INIT_CALLER if caller_init else native.INIT_HASH)
 
     @staticmethod
     def train(ratings, rank, iterations, lambda_=0.01, blocks=-1, seed=0, **kw) -> MatrixFactorizationModel:

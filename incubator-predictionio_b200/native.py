@@ -37,7 +37,9 @@ EXPORTED_SYMBOLS = [
     "pio_events_index_create",
     "pio_events_index_append", "pio_events_index_add_host", "pio_events_index_lookup", "pio_events_index_get_stats",
     "pio_events_index_destroy", "pio_rf_train", "pio_rf_forest_size", "pio_rf_forest_get", "pio_rf_forest_destroy",
-    "pio_rf_predict",
+    "pio_rf_predict", "pio_eval_folds_create", "pio_eval_folds_sizes", "pio_eval_folds_maps",
+    "pio_eval_folds_set_ratings", "pio_eval_folds_result_add", "pio_eval_folds_result_free",
+    "pio_eval_folds_rank_counts", "pio_eval_folds_destroy",
 ]
 
 
@@ -462,6 +464,95 @@ def ids_encode(strings, device=0):
     _check(lib().pio_ids_encode(C.c_int(device), _ptr(buf, C.c_uint8) if buf.size else None, _ptr(off, C.c_int64),
                                 C.c_int64(n), _ptr(idx, C.c_int32), _ptr(first, C.c_int64), C.byref(nu)))
     return idx, first[:nu.value]
+
+
+class EvalFolds:
+    """pio_eval_folds: the k-fold split of n ratings on the device (rating e tests in fold e % k_fold and trains in every
+    other fold), from global user / item indices (ids_encode of the whole columns) and fp64 ratings.  Per fold: the
+    fold-local BiMap.stringInt indices of its training ratings, its training COO, and its queries (distinct test users in
+    order of first occurrence).  The device memory goes with this object; EvalResult objects keep it alive."""
+
+    def __init__(self, user, item, rating, k_fold: int, device: int = 0):
+        self._h = C.c_void_p()
+        user = np.ascontiguousarray(user, np.int32)
+        item = np.ascontiguousarray(item, np.int32)
+        rating = np.ascontiguousarray(rating, np.float64)
+        if not (user.shape == item.shape == rating.shape) or user.ndim != 1:
+            raise ValueError("user/item/rating must be 1-D arrays of equal length")
+        self.k_fold, self.device = int(k_fold), int(device)
+        _check(lib().pio_eval_folds_create(C.c_int(device), _ptr(user, C.c_int32), _ptr(item, C.c_int32),
+                                           _ptr(rating, C.c_double), C.c_int64(user.shape[0]), C.c_int32(k_fold),
+                                           C.byref(self._h)))
+
+    def close(self):
+        if self._h:
+            lib().pio_eval_folds_destroy(self._h)
+            self._h = C.c_void_p()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    def sizes(self, fold: int) -> tuple:
+        """(users, items, training ratings, queries) of fold `fold`."""
+        out = np.zeros(4, np.int64)
+        _check(lib().pio_eval_folds_sizes(self._h, C.c_int32(fold), _ptr(out, C.c_int64)))
+        return tuple(int(x) for x in out)
+
+    def maps(self, fold: int) -> dict:
+        """Global index of each fold-local user / item, and per query its global user and fold-local training user
+        (-1: none)."""
+        nu, ni, _, nq = self.sizes(fold)
+        out = {"user": np.empty(nu, np.int32), "item": np.empty(ni, np.int32), "query_user": np.empty(nq, np.int32),
+               "query_train_user": np.empty(nq, np.int32)}
+        _check(lib().pio_eval_folds_maps(self._h, C.c_int32(fold), *_addrs(out, "user", "item", "query_user",
+                                                                           "query_train_user")))
+        return out
+
+    def set_ratings(self, fold: int, als: "NativeALS"):
+        """The fold's training COO into `als` (created with the fold's user and item counts)."""
+        _check(lib().pio_eval_folds_set_ratings(self._h, C.c_int32(fold), als._h))
+
+    def add_result(self, fold: int, items, count) -> "EvalResult":
+        """Keeps a top-N result of the fold (items [n_queries, num] of fold-local indices, count [n_queries])."""
+        items = np.ascontiguousarray(items, np.int32)
+        count = np.ascontiguousarray(count, np.int32)
+        if items.ndim != 2 or count.shape != (items.shape[0],):
+            raise ValueError("items must be [n_queries, num] and count [n_queries]")
+        rid = C.c_int32(-1)
+        _check(lib().pio_eval_folds_result_add(self._h, C.c_int32(fold), _ptr(items, C.c_int32), _ptr(count, C.c_int32),
+                                               C.c_int32(items.shape[0]), C.c_int32(items.shape[1]), C.byref(rid)))
+        return EvalResult(self, fold, rid.value, items, count)
+
+
+class EvalResult:
+    """A fold's top-N result kept on the device by its EvalFolds (which it keeps alive); `items` / `count` are the host
+    arrays it was made from."""
+
+    def __init__(self, folds: EvalFolds, fold: int, rid: int, items: np.ndarray, count: np.ndarray):
+        self.folds, self.fold, self._rid, self.items, self.count = folds, fold, rid, items, count
+        self.n_queries = int(count.shape[0])
+
+    def rank_counts(self, k: int, threshold: float):
+        """Per query (int32 each): hits among the first min(k, count) items, distinct test items with a largest rating
+        >= threshold, and test ratings >= threshold."""
+        out = {name: np.zeros(self.n_queries, np.int32) for name in ("hits", "npos", "nraw")}
+        _check(lib().pio_eval_folds_rank_counts(self.folds._h, C.c_int32(self._rid), C.c_int32(k), C.c_double(threshold),
+                                                *_addrs(out, "hits", "npos", "nraw")))
+        return out["hits"], out["npos"], out["nraw"]
+
+    def close(self):
+        if self._rid is not None and self.folds._h:
+            lib().pio_eval_folds_result_free(self.folds._h, C.c_int32(self._rid))
+        self._rid = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
 
 
 EVENTS_TARGET_ANY, EVENTS_TARGET_ABSENT, EVENTS_TARGET_EQUALS = 0, 1, 2

@@ -86,11 +86,20 @@ class RatingColumns:
 
 
 class TrainingData(SanityCheck):
-    """Ratings as a list of Rating, or as RatingColumns (the list is then built on first use of `.ratings`)."""
+    """Ratings as a list of Rating, as RatingColumns (the list is then built on first use of `.ratings`), or as one fold
+    of DataSource.readEvalColumns on the device (the columns are then cut on first use of `.columns`)."""
 
-    def __init__(self, ratings: Optional[List[Rating]] = None, columns: Optional[RatingColumns] = None):
+    def __init__(self, ratings: Optional[List[Rating]] = None, columns: Optional[RatingColumns] = None,
+                 fold: Optional["EvalFold"] = None):
         self._ratings = ratings
-        self.columns = columns
+        self._columns = columns
+        self.fold = fold
+
+    @property
+    def columns(self) -> Optional[RatingColumns]:
+        if self._columns is None and self.fold is not None:
+            self._columns = self.fold.training_columns()
+        return self._columns
 
     @property
     def ratings(self) -> List[Rating]:
@@ -99,7 +108,9 @@ class TrainingData(SanityCheck):
         return self._ratings
 
     def __len__(self) -> int:
-        return len(self.columns) if self._ratings is None else len(self._ratings)
+        if self._ratings is not None:
+            return len(self._ratings)
+        return self.fold.n_train if self._columns is None and self.fold is not None else len(self.columns)
 
     def sanityCheck(self):
         pass
@@ -107,6 +118,34 @@ class TrainingData(SanityCheck):
     def __repr__(self):
         head = self.columns.take(np.arange(min(2, len(self)))).to_ratings() if self._ratings is None else self._ratings[:2]
         return f"ratings: [{len(self)}] ({head}...)"
+
+
+class EvalFold:
+    """One fold of DataSource.readEvalColumns, on the device (native.EvalFolds): its training ratings, which
+    ALSAlgorithm.train loads into the ALS handle without leaving the device, and its queries -- the distinct users of its
+    test ratings in order of first occurrence, each asking for `num` items, as readEval's by_user dict holds them."""
+
+    def __init__(self, folds: native.EvalFolds, fold: int, cols: RatingColumns, ufirst: np.ndarray, ifirst: np.ndarray,
+                 num: int):
+        self.folds, self.fold, self.cols, self.ufirst, self.ifirst, self.num = folds, fold, cols, ufirst, ifirst, num
+        self.n_users, self.n_items, self.n_train, self.n_queries = folds.sizes(fold)
+        self._maps = None
+
+    @property
+    def maps(self) -> dict:
+        """native.EvalFolds.maps of this fold."""
+        if self._maps is None:
+            self._maps = self.folds.maps(self.fold)
+        return self._maps
+
+    def bimaps(self) -> Tuple[BiMap, BiMap]:
+        """userStringIntMap, itemStringIntMap: BiMap.stringInt of the fold's training users and items."""
+        m = self.maps
+        return tuple(BiMap({s: k for k, s in enumerate(string_list(take_strings(*col, first[m[side]])))})
+                     for col, first, side in ((self.cols.user, self.ufirst, "user"), (self.cols.item, self.ifirst, "item")))
+
+    def training_columns(self) -> RatingColumns:
+        return self.cols.take(np.flatnonzero(np.arange(len(self.cols)) % self.folds.k_fold != self.fold))
 
 
 PreparedData = TrainingData
@@ -147,10 +186,28 @@ class DataSource(PDataSource):
                           [(Query(u, ep.queryNum, set()), ActualResult(rs)) for u, rs in by_user.items()]))
         return folds
 
+    def readEvalColumns(self, sc) -> Optional[list]:
+        """readEval's folds, split on the device: per fold (TrainingData of its EvalFold, None, the EvalFold as its
+        queries).  None when some rating has no targetEntityId: those folds take readEval's object path."""
+        assert self.dsp.evalParams is not None, "Must specify evalParams"
+        ep = self.dsp.evalParams
+        cols = self.getRatingColumns(sc)
+        if ep.kFold < 1 or not len(cols) or not cols.has_item.all():
+            return None
+        dev = getattr(sc, "device", 0) or 0
+        u, ufirst = native.ids_encode(cols.user, dev)
+        i, ifirst = native.ids_encode(cols.item, dev)
+        folds = native.EvalFolds(u, i, cols.rating, ep.kFold, dev)
+        out = []
+        for f in range(ep.kFold):
+            fold = EvalFold(folds, f, cols, ufirst, ifirst, ep.queryNum)
+            out.append((TrainingData(fold=fold), None, fold))
+        return out
+
 
 class Preparator(PPreparator):
     def prepare(self, sc, trainingData: TrainingData) -> PreparedData:
-        return PreparedData(trainingData._ratings, trainingData.columns)
+        return PreparedData(trainingData._ratings, trainingData._columns, trainingData.fold)
 
 
 @dataclass
@@ -170,10 +227,27 @@ def _model_path(id: str) -> Path:
 
 
 class ALSModel(MatrixFactorizationModel, PersistentModel):
-    def __init__(self, m: MatrixFactorizationModel, userStringIntMap: BiMap, itemStringIntMap: BiMap):
+    """make_maps (instead of the two maps): a function returning (userStringIntMap, itemStringIntMap), called on first
+    use of either."""
+
+    def __init__(self, m: MatrixFactorizationModel, userStringIntMap: Optional[BiMap], itemStringIntMap: Optional[BiMap],
+                 make_maps=None):
         super().__init__(m.rank, m.userFeatures, m.productFeatures, m.userHas, m.productHas, m._h)
-        self.userStringIntMap = userStringIntMap
-        self.itemStringIntMap = itemStringIntMap
+        self._bimaps = (userStringIntMap, itemStringIntMap) if make_maps is None else None
+        self._make_maps = make_maps
+
+    def _maps(self) -> Tuple[BiMap, BiMap]:
+        if self._bimaps is None:
+            self._bimaps = self._make_maps()
+        return self._bimaps
+
+    @property
+    def userStringIntMap(self) -> BiMap:
+        return self._maps()[0]
+
+    @property
+    def itemStringIntMap(self) -> BiMap:
+        return self._maps()[1]
 
     def save(self, id: str, params, sc) -> bool:  # ALSModel.scala:63-74
         d = _model_path(id)
@@ -208,6 +282,17 @@ class ALSAlgorithm(PAlgorithm):
         if not len(data):
             raise ValueError("requirement failed: RDD[Rating] in PreparedData cannot be empty. Please check if "
                              "DataSource generates TrainingData and Preparator generates PreparedData correctly.")
+        seed = sc.agree_seed(self.ap.seed) if hasattr(sc, "agree_seed") else (self.ap.seed or 0)
+        als = ALS()
+        als.setUserBlocks(-1).setProductBlocks(-1).setRank(self.ap.rank).setIterations(self.ap.numIterations)
+        als.setLambda(self.ap.lambda_).setImplicitPrefs(self.ap.implicitPrefs).setAlpha(1.0).setSeed(seed)
+        als.setCheckpointInterval(10)
+        fold = data.fold
+        if fold is not None and data._ratings is None and data._columns is None:
+            # an evaluation fold (DataSource.readEvalColumns): its COO is on the device already, indexed as BiMap.stringInt
+            # of its training strings would index it; the string maps are built only if someone asks for them
+            m = als.runFilled(lambda h: fold.folds.set_ratings(fold.fold, h), fold.n_users, fold.n_items, sc=sc)
+            return ALSModel(m, None, None, make_maps=fold.bimaps)
         cols = data.columns
         if cols is not None and data._ratings is None and cols.has_item.all():
             # BiMap.stringInt on the GPU: indices in first-occurrence order, the maps built from the distinct ids only
@@ -225,11 +310,6 @@ class ALSAlgorithm(PAlgorithm):
             u = np.fromiter((userStringIntMap(r.user) for r in data.ratings), np.int32, n)
             i = np.fromiter((itemStringIntMap(r.item) for r in data.ratings), np.int32, n)
             v = np.fromiter((r.rating for r in data.ratings), np.float32, n)
-        seed = sc.agree_seed(self.ap.seed) if hasattr(sc, "agree_seed") else (self.ap.seed or 0)
-        als = ALS()
-        als.setUserBlocks(-1).setProductBlocks(-1).setRank(self.ap.rank).setIterations(self.ap.numIterations)
-        als.setLambda(self.ap.lambda_).setImplicitPrefs(self.ap.implicitPrefs).setAlpha(1.0).setSeed(seed)
-        als.setCheckpointInterval(10)
         m = als.run((u, i, v), n_users=userStringIntMap.size, n_products=itemStringIntMap.size, sc=sc)
         return ALSModel(m, userStringIntMap, itemStringIntMap)
 
@@ -281,9 +361,23 @@ class ALSAlgorithm(PAlgorithm):
             out = [(ix, PredictedResult([])) for ix, _ in qs]
         return out
 
+    def batchPredictColumns(self, sc, model: ALSModel, queries: EvalFold) -> native.EvalResult:
+        """batchPredict over an EvalFold's queries, kept on the device for the metrics' rank counts: the same users array
+        (-1 for a user without training ratings) and the same num in one pio_als_recommend call."""
+        users = queries.maps["query_train_user"]
+        num = queries.num
+        if num > 0 and queries.n_queries:
+            items, _, cnt = model.recommendProductsForUsers(users, num)
+            return queries.folds.add_result(queries.fold, items, np.minimum(cnt, num))
+        n = queries.n_queries
+        return queries.folds.add_result(queries.fold, np.full((n, 1), -1, np.int32), np.zeros(n, np.int32))
+
 
 class Serving(LServing):
     def serve(self, query: Query, predictedResults) -> PredictedResult:
+        return predictedResults[0]
+
+    def serveColumns(self, queries, predictedResults):
         return predictedResults[0]
 
 
@@ -296,6 +390,14 @@ class RecommendationEngine(EngineFactory):
 from ..controller import EngineParams  # noqa: E402
 from ..evaluation import (AverageMetric, EngineParamsGenerator, Evaluation, MetricEvaluator,  # noqa: E402
                           OptionAverageMetric)
+
+
+def _mean_in_order(values) -> float:
+    """sum(v) / len(v) over the per-query values of every fold in order, exactly as AverageMetric.calculate computes it:
+    the quotients are the correctly rounded fp64 divisions Python's int / int makes, and the sum is Python's own (its
+    float summation is compensated, which no numpy reduction reproduces)."""
+    v = np.concatenate(values).tolist() if values else []
+    return sum(v) / len(v) if v else float("nan")
 
 
 class PrecisionAtK(OptionAverageMetric):
@@ -317,6 +419,16 @@ class PrecisionAtK(OptionAverageMetric):
         tp = sum(1 for s in p.itemScores[:self.k] if s.item in positives)
         return tp / min(self.k, len(positives))
 
+    def calculate_columns(self, sc, evalColumns) -> float:
+        """calculate over Engine.evalColumns' folds: the same per-query values, in the same order, from the device's
+        rank counts."""
+        v = []
+        for _, _, result in evalColumns:
+            hits, npos, _ = result.rank_counts(self.k, self.ratingThreshold)
+            ok = npos > 0
+            v.append(hits[ok] / np.minimum(self.k, npos[ok]).astype(np.float64))
+        return _mean_in_order(v)
+
 
 class PositiveCount(AverageMetric):
     """Evaluation.scala:53-62."""
@@ -330,6 +442,9 @@ class PositiveCount(AverageMetric):
 
     def calculate_one(self, q, p, a: ActualResult) -> float:
         return float(sum(1 for r in a.ratings if r.rating >= self.ratingThreshold))
+
+    def calculate_columns(self, sc, evalColumns) -> float:
+        return _mean_in_order([r.rank_counts(1, self.ratingThreshold)[2].astype(np.float64) for _, _, r in evalColumns])
 
 
 class RecommendationEvaluation(Evaluation):
