@@ -37,14 +37,23 @@ __global__ void cooc_user_head_kernel(const uint64_t* __restrict__ dk, long long
   const long long e = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (e < m) uflag[e] = (e == 0 || (dk[e] >> bits_i) != (dk[e - 1] >> bits_i)) ? 1u : 0u;
 }
-// element e (rank r inside its user's sorted item list) pairs with the r earlier items of the user: npairs[e] = r
-__global__ void cooc_rank_kernel(const uint64_t* __restrict__ dk, long long m, int bits_i, uint32_t* __restrict__ rank) {
+// element e (rank r inside its user's sorted item list) pairs with the r earlier items of the user: npairs[e] = r.
+// *total (zeroed by the caller) receives the sum of the ranks in 64 bits: the uint32 scan of the ranks wraps once a
+// user has more than ~92 700 distinct items, so the pair count must not be read back from it.
+__global__ void cooc_rank_kernel(const uint64_t* __restrict__ dk, long long m, int bits_i, uint32_t* __restrict__ rank,
+                                 unsigned long long* __restrict__ total) {
   const long long e = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-  if (e >= m) return;
-  const uint64_t usr = dk[e] >> bits_i;
-  long long s = e;
-  while (s > 0 && (dk[s - 1] >> bits_i) == usr) --s;   // users' lists are short next to m; templates view <= 1e3 items
-  rank[e] = (uint32_t)(e - s);
+  unsigned long long r = 0;
+  if (e < m) {
+    const uint64_t usr = dk[e] >> bits_i;
+    long long s = e;
+    while (s > 0 && (dk[s - 1] >> bits_i) == usr) --s;   // users' lists are short next to m; templates view <= 1e3 items
+    r = (unsigned long long)(e - s);
+    rank[e] = (uint32_t)r;
+  }
+#pragma unroll
+  for (int d = 16; d > 0; d >>= 1) r += __shfl_down_sync(0xffffffffu, r, d);
+  if ((threadIdx.x & 31) == 0 && r) atomicAdd(total, r);
 }
 __global__ void cooc_pairs_kernel(const uint64_t* __restrict__ dk, const uint32_t* __restrict__ rank,
                                   const uint32_t* __restrict__ off, long long m, int bits_i, uint64_t* __restrict__ pk,

@@ -2985,6 +2985,46 @@ __attribute__((visibility("default"))) int pio_als_debug_lockstep(int device, in
   return PIO_ALS_OK;
 }
 
+/* debug only (not in pio_als.h): the stable radix sort of sort_scan.cuh on n (key, payload) pairs (HOST buffers, sorted
+ * in place) by key bits [0, nbits), read back from whichever half of the ping-pong holds the result.  Used by
+ * tests/test_gpu_sort_scan.py. */
+__attribute__((visibility("default"))) int pio_debug_radix_sort(int device, uint64_t* keys, uint32_t* vals, int64_t n,
+                                                                int nbits) {
+  if (!keys || !vals || n < 1 || n >= (1ll << 32) || nbits < 1 || nbits > 64) return PIO_ALS_ERR_ARG;
+  CK0(cudaSetDevice(device));
+  CallMem tmp(0);
+  SortBufs sb;
+  for (int i : {0, 1}) {
+    CK0(tmp.device(&sb.k[i], (size_t)n));
+    CK0(tmp.device(&sb.v[i], (size_t)n));
+  }
+  CK0(cudaMemcpy(sb.keys(), keys, sizeof(uint64_t) * (size_t)n, cudaMemcpyHostToDevice));
+  CK0(cudaMemcpy(sb.vals(), vals, sizeof(uint32_t) * (size_t)n, cudaMemcpyHostToDevice));
+  CK0(radix_sort_pairs(sb, (size_t)n, nbits, 0, nullptr));
+  CK0(cudaDeviceSynchronize());
+  CK0(cudaMemcpy(keys, sb.keys(), sizeof(uint64_t) * (size_t)n, cudaMemcpyDeviceToHost));
+  CK0(cudaMemcpy(vals, sb.vals(), sizeof(uint32_t) * (size_t)n, cudaMemcpyDeviceToHost));
+  return PIO_ALS_OK;
+}
+
+/* debug only (not in pio_als.h): the exclusive uint32 scan of sort_scan.cuh (sums mod 2^32) on n values (HOST buffers),
+ * out of place, or in place on one device buffer when in_place != 0.  Used by tests/test_gpu_sort_scan.py. */
+__attribute__((visibility("default"))) int pio_debug_scan_u32(int device, const uint32_t* in, uint32_t* out, int64_t n,
+                                                              int in_place) {
+  if (!in || !out || n < 1) return PIO_ALS_ERR_ARG;
+  CK0(cudaSetDevice(device));
+  CallMem tmp(0);
+  uint32_t *din = nullptr, *dout = nullptr;
+  CK0(tmp.device(&din, (size_t)n));
+  if (in_place) dout = din;
+  else CK0(tmp.device(&dout, (size_t)n));
+  CK0(cudaMemcpy(din, in, sizeof(uint32_t) * (size_t)n, cudaMemcpyHostToDevice));
+  CK0(scan_exclusive_u32(din, dout, (size_t)n, 0, nullptr));
+  CK0(cudaDeviceSynchronize());
+  CK0(cudaMemcpy(out, dout, sizeof(uint32_t) * (size_t)n, cudaMemcpyDeviceToHost));
+  return PIO_ALS_OK;
+}
+
 int pio_als_get_stats(const pio_als_handle* h, pio_als_stats* out) {
   if (!h || !out) return PIO_ALS_ERR_ARG;
   *out = h->st;
@@ -4255,16 +4295,19 @@ int pio_cooc_train(int device, const int32_t* user, const int32_t* item, int64_t
   CK0(cudaStreamSynchronize(st));
   const long long m = (long long)lp + lf;
   cooc_compact_kernel<<<nblk(n, 256), 256, 0, st>>>(ks, flag, pos, n, dk);
-  // 2. pairs (item1 < item2) per user
-  cooc_rank_kernel<<<nblk(m, 256), 256, 0, st>>>(dk, m, bits_i, rank);
+  // 2. pairs (item1 < item2) per user; their total is counted in 64 bits and checked before the uint32 scan of the
+  // ranks is used as an index
+  unsigned long long* dtot = nullptr;
+  CK0(tmp.device(&dtot, 1));
+  CK0(cudaMemsetAsync(dtot, 0, sizeof(unsigned long long), st));
+  cooc_rank_kernel<<<nblk(m, 256), 256, 0, st>>>(dk, m, bits_i, rank, dtot);
+  unsigned long long tot = 0;
+  CK0(cudaMemcpyAsync(&tot, dtot, sizeof(tot), cudaMemcpyDeviceToHost, st));
+  CK0(cudaStreamSynchronize(st));
+  if (tot >= (1ull << 31)) return fail(nullptr, PIO_ALS_ERR_ARG, "more than 2^31-1 co-occurrence pairs (%llu)", tot);
+  const long long np = (long long)tot;
   uint32_t* off = flag;
   CK0(scan_exclusive_u32(rank, off, (size_t)m, st, nullptr));
-  uint32_t lr = 0, lo = 0;
-  CK0(cudaMemcpyAsync(&lr, rank + m - 1, 4, cudaMemcpyDeviceToHost, st));
-  CK0(cudaMemcpyAsync(&lo, off + m - 1, 4, cudaMemcpyDeviceToHost, st));
-  CK0(cudaStreamSynchronize(st));
-  const long long np = (long long)lo + lr;
-  if (np >= (1ll << 31)) return fail(nullptr, PIO_ALS_ERR_ARG, "more than 2^31-1 co-occurrence pairs (%lld)", np);
   std::vector<int> h_item((size_t)n_items * topn, -1), h_cnt((size_t)n_items * topn, 0), h_n((size_t)n_items, 0);
   if (np > 0) {
     SortBufs ps, rs;

@@ -100,7 +100,7 @@ constexpr int RS_WARP_ITEMS = 32 * RS_ROUNDS;        // 512
 constexpr int RS_TILE = RS_THREADS * RS_ROUNDS;      // 4096
 
 __global__ void __launch_bounds__(RS_THREADS)
-rs_hist_kernel(const uint64_t* __restrict__ keys, size_t n, int shift, uint32_t* __restrict__ hist,
+rs_hist_kernel(const uint64_t* __restrict__ keys, size_t n, int shift, unsigned dmask, uint32_t* __restrict__ hist,
                unsigned nblocks) {
   __shared__ uint32_t sh[256];
   sh[threadIdx.x] = 0;
@@ -109,7 +109,7 @@ rs_hist_kernel(const uint64_t* __restrict__ keys, size_t n, int shift, uint32_t*
 #pragma unroll 4
   for (int i = 0; i < RS_ROUNDS; ++i) {
     const size_t idx = base + (size_t)i * RS_THREADS + threadIdx.x;
-    if (idx < n) atomicAdd(&sh[(unsigned)(keys[idx] >> shift) & 255u], 1u);
+    if (idx < n) atomicAdd(&sh[(unsigned)(keys[idx] >> shift) & dmask], 1u);
   }
   __syncthreads();
   hist[(size_t)threadIdx.x * nblocks + blockIdx.x] = sh[threadIdx.x];
@@ -117,7 +117,7 @@ rs_hist_kernel(const uint64_t* __restrict__ keys, size_t n, int shift, uint32_t*
 
 __global__ void __launch_bounds__(RS_THREADS)
 rs_scatter_kernel(const uint64_t* __restrict__ kin, const uint32_t* __restrict__ vin,
-                  uint64_t* __restrict__ kout, uint32_t* __restrict__ vout, size_t n, int shift,
+                  uint64_t* __restrict__ kout, uint32_t* __restrict__ vout, size_t n, int shift, unsigned dmask,
                   const uint32_t* __restrict__ offs, unsigned nblocks) {
   __shared__ uint32_t wcnt[RS_WARPS][256];
   const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
@@ -134,7 +134,7 @@ rs_scatter_kernel(const uint64_t* __restrict__ kin, const uint32_t* __restrict__
     const bool valid = idx < n;
     key[r] = valid ? kin[idx] : 0ull;
     val[r] = valid ? vin[idx] : 0u;
-    const unsigned d = valid ? ((unsigned)(key[r] >> shift) & 255u) : 256u;
+    const unsigned d = valid ? ((unsigned)(key[r] >> shift) & dmask) : 256u;
     const uint32_t peers = __match_any_sync(0xffffffffu, d);
     uint32_t prev = 0;
     if (valid) prev = wcnt[w][d];
@@ -177,7 +177,7 @@ rs_scatter_kernel(const uint64_t* __restrict__ kin, const uint32_t* __restrict__
   for (int r = 0; r < RS_ROUNDS; ++r) {
     const size_t idx = wbase + (size_t)r * 32 + lane;
     if (idx < n) {
-      const unsigned d = (unsigned)(key[r] >> shift) & 255u;
+      const unsigned d = (unsigned)(key[r] >> shift) & dmask;
       const uint32_t lp = lstart[d] + wcnt[w][d] + rnk[r];
       skey[lp] = key[r];
       sval[lp] = val[r];
@@ -193,7 +193,7 @@ rs_scatter_kernel(const uint64_t* __restrict__ kin, const uint32_t* __restrict__
     const uint32_t pidx = (uint32_t)r * RS_THREADS + threadIdx.x;
     if (pidx < cnt) {
       const uint64_t kk = skey[pidx];
-      const unsigned d = (unsigned)(kk >> shift) & 255u;
+      const unsigned d = (unsigned)(kk >> shift) & dmask;
       const size_t pos = (size_t)goff[d] + (pidx - lstart[d]);
       kout[pos] = kk;
       vout[pos] = sval[pidx];
@@ -217,7 +217,8 @@ struct SortBufs {
   void flip() { live ^= 1; }   // the spare half becomes live: for data the caller writes there
 };
 
-// Stable sort of the live half by key bits [0, nbits); the spare half is clobbered.
+// Stable sort of the live half by key bits [0, nbits); the spare half is clobbered.  Bits at and above nbits do not
+// order the keys: the last pass masks its digit to the bits below nbits.
 inline cudaError_t radix_sort_pairs(SortBufs& b, size_t n, int nbits, cudaStream_t st, int64_t* launches) {
   if (n == 0) return cudaSuccess;
   const unsigned nblocks = (unsigned)((n + RS_TILE - 1) / RS_TILE);
@@ -226,12 +227,13 @@ inline cudaError_t radix_sort_pairs(SortBufs& b, size_t n, int nbits, cudaStream
   if (e != cudaSuccess) return e;
   e = cudaFuncSetAttribute(rs_scatter_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)RS_SCATTER_SMEM);
   for (int shift = 0; e == cudaSuccess && shift < nbits; shift += 8) {
-    rs_hist_kernel<<<nblocks, RS_THREADS, 0, st>>>(b.keys(), n, shift, hist, nblocks);
+    const unsigned dmask = nbits - shift >= 8 ? 255u : (1u << (nbits - shift)) - 1u;
+    rs_hist_kernel<<<nblocks, RS_THREADS, 0, st>>>(b.keys(), n, shift, dmask, hist, nblocks);
     if (launches) ++*launches;
     e = scan_exclusive_u32(hist, hist, (size_t)256 * nblocks, st, launches);
     if (e != cudaSuccess) break;
     rs_scatter_kernel<<<nblocks, RS_THREADS, RS_SCATTER_SMEM, st>>>(b.keys(), b.vals(), b.spare_keys(), b.spare_vals(),
-                                                                    n, shift, hist, nblocks);
+                                                                    n, shift, dmask, hist, nblocks);
     if (launches) ++*launches;
     b.flip();
   }

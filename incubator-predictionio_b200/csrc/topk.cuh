@@ -1750,7 +1750,8 @@ nb_partial_kernel(const int* __restrict__ label, const float* __restrict__ x, lo
   const long long r0 = (long long)blockIdx.x * per;
   const long long r1 = r0 + per < n ? r0 + per : n;
   // each warp walks its strided rows; lanes serialise their updates in lane order so the
-  // summation order is fixed (values are typically small integers, sums exact in fp64)
+  // summation order is fixed (values are typically small integers, sums exact in fp64).
+  // Slot f (the count at f == n_feat) belongs to lane f % 32 at every width.
   for (long long base = r0 + (long long)w * 32; base < r1; base += 8 * 32) {
     const long long r = base + lane;
     int c = -1;
@@ -1759,11 +1760,8 @@ nb_partial_kernel(const int* __restrict__ label, const float* __restrict__ x, lo
       const int cc = __shfl_sync(0xffffffffu, c, src);
       if (cc < 0) continue;
       const long long rr = base + src;
-      if (lane <= n_feat) {
-        const double v = lane < n_feat ? (double)x[rr * n_feat + lane] : 1.0;
-        my[cc * (n_feat + 1) + lane] += v;
-      }
-      for (int f = lane + 32; f < n_feat; f += 32) my[cc * (n_feat + 1) + f] += (double)x[rr * n_feat + f];
+      for (int f = lane; f <= n_feat; f += 32)
+        my[cc * (n_feat + 1) + f] += f < n_feat ? (double)x[rr * n_feat + f] : 1.0;
     }
   }
   __syncthreads();
