@@ -4429,11 +4429,15 @@ constexpr int64_t RF_NODE_BUDGET = 1ll << 30;   // node ids of one tree group (i
 constexpr int64_t RF_HIST_BUDGET = 1ll << 29;   // the global histogram of one chunk of a level's node slots
 constexpr int RF_SMEM = 96 * 1024;              // shared-memory histogram of one pass (two blocks per SM)
 
-// where the last pio_rf_train on this thread spent its time (wall ms; every phase ends in a stream synchronise)
+// where the last pio_rf_train on this thread spent its time (wall ms; every phase ends in a stream synchronise), and
+// which paths it took
 struct RfTiming {
   double h2d = 0, split = 0, bin = 0, hist = 0, sel = 0, upd = 0;
   int levels = 0, groups = 0;
   double hist_l[RF_MAX_DEPTH + 1] = {}, sel_l[RF_MAX_DEPTH + 1] = {};
+  int bin_bytes = 0, staged = 0;                 // bin code width; thresholds staged in shared memory
+  int64_t smem_launches = 0, global_launches = 0;  // hist_kernel<BinT, true> / <BinT, false> launches
+  int64_t max_chunks = 0, max_passes = 0;        // most chunks in one level, most shared-memory passes in one chunk
 };
 static thread_local RfTiming g_rf_timing;
 
@@ -4583,8 +4587,13 @@ static int rf_bin_and_grow(const RfCtx& c) {
   CK0(cudaGetLastError());
   CK0(cudaStreamSynchronize(st));
   tm.bin = rf_ms(t0);
+  tm.bin_bytes = (int)sizeof(BinT), tm.staged = staged;
 
+  // PIO_RF_TREES_PER_PASS / PIO_RF_HIST_BUDGET (bytes): tree grouping and histogram chunking for tests; neither changes
+  // the forest
   const char* env = getenv("PIO_RF_TREES_PER_PASS");
+  const char* env_hb = getenv("PIO_RF_HIST_BUDGET");
+  const int64_t hist_budget = env_hb && atoll(env_hb) > 0 ? atoll(env_hb) : RF_HIST_BUDGET;
   const auto groups = rf_plan_groups(T, n, RF_NODE_BUDGET, env ? atoi(env) : 0);
   int gmax = 0;
   for (const auto& g : groups) gmax = std::max(gmax, g.second - g.first);
@@ -4595,7 +4604,7 @@ static int rf_bin_and_grow(const RfCtx& c) {
   rf::Cdf cdf;
   rf_poisson_table(cdf.v);
   const int64_t slot_bytes = (int64_t)K * NB * C * 8, smem_slot = (int64_t)K * NB * C * 4;
-  const int64_t chunk_max = std::max<int64_t>(1, RF_HIST_BUDGET / slot_bytes);
+  const int64_t chunk_max = std::max<int64_t>(1, hist_budget / slot_bytes);
   const int64_t pass_slots = RF_SMEM / smem_slot;
   if (pass_slots >= 1) {
     CK0(cudaFuncSetAttribute(rf::hist_kernel<BinT, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, RF_SMEM));
@@ -4633,6 +4642,7 @@ static int rf_bin_and_grow(const RfCtx& c) {
       CK0(cudaMemcpyAsync(dsub, hsub.data(), 4 * hsub.size(), cudaMemcpyHostToDevice, st));
       CK0(cudaStreamSynchronize(st));
       rf_ms(t0);
+      tm.max_chunks = std::max(tm.max_chunks, (S + cap - 1) / cap);
       for (int64_t c0 = 0; c0 < S; c0 += cap) {
         const int64_t c1 = std::min(S, c0 + cap);
         CK0(cudaMemsetAsync(dhist, 0, (size_t)(c1 - c0) * slot_bytes, st));
@@ -4647,9 +4657,12 @@ static int rf_bin_and_grow(const RfCtx& c) {
             a.g1 = active[a.s1 - 1].first;
             rf::hist_kernel<BinT, true><<<grid, rf::THREADS, (size_t)(a.s1 - a.s0) * smem_slot, st>>>(a);
           }
+          const int64_t passes = (c1 - c0 + pass_slots - 1) / pass_slots;
+          tm.smem_launches += passes, tm.max_passes = std::max(tm.max_passes, passes);
         } else {
           const unsigned grid = (unsigned)std::min<int64_t>(nblk(n, rf::THREADS), (int64_t)c.sm * 8);
           rf::hist_kernel<BinT, false><<<grid, rf::THREADS, 0, st>>>(a);
+          ++tm.global_launches;
         }
         CK0(cudaGetLastError());
         CK0(cudaStreamSynchronize(st));
@@ -4948,6 +4961,18 @@ __attribute__((visibility("default"))) int pio_rf_debug_timing(double out[70]) {
   out[0] = t.h2d, out[1] = t.split, out[2] = t.bin, out[3] = t.hist, out[4] = t.sel, out[5] = t.upd;
   out[6] = t.levels, out[7] = t.groups;
   for (int l = 0; l <= RF_MAX_DEPTH; ++l) out[8 + l] = t.hist_l[l], out[39 + l] = t.sel_l[l];
+  return PIO_ALS_OK;
+}
+
+/* debug only (not in pio_als.h): which paths the last pio_rf_train on this thread took: out[0] bin code bytes (1 or 2),
+ * [1] thresholds staged in shared memory (0 / 1), [2] shared-memory hist_kernel launches, [3] global hist_kernel
+ * launches, [4] most histogram chunks in one level, [5] most shared-memory passes in one chunk, [6] levels, [7] tree
+ * groups.  Used by tests/test_gpu_forest_bounds.py. */
+__attribute__((visibility("default"))) int pio_rf_debug_paths(int64_t out[8]) {
+  if (!out) return PIO_ALS_ERR_ARG;
+  const RfTiming& t = g_rf_timing;
+  out[0] = t.bin_bytes, out[1] = t.staged, out[2] = t.smem_launches, out[3] = t.global_launches;
+  out[4] = t.max_chunks, out[5] = t.max_passes, out[6] = t.levels, out[7] = t.groups;
   return PIO_ALS_OK;
 }
 

@@ -940,6 +940,16 @@ def rf_train_timing() -> dict:
             "hist_level_ms": list(out[8:8 + levels]), "select_level_ms": list(out[39:39 + levels])}
 
 
+def rf_train_paths() -> dict:
+    """Which paths the last rf_train on this thread took: bin code width in bytes, thresholds staged in shared memory,
+    shared-memory and global histogram launches, the most histogram chunks in one level, the most shared-memory passes
+    in one chunk, levels and tree groups."""
+    out = (C.c_int64 * 8)()
+    _check(lib().pio_rf_debug_paths(out))
+    keys = ("bin_bytes", "staged", "smem_launches", "global_launches", "max_chunks", "max_passes", "levels", "groups")
+    return {k: int(v) for k, v in zip(keys, out)}
+
+
 def nb_predict(x, pi, theta, device=0):
     x = np.ascontiguousarray(x, np.float32)
     pi = np.ascontiguousarray(pi, np.float64)

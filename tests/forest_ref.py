@@ -191,7 +191,8 @@ def thresholds(v, cnt, num_bins):
         return np.zeros(0)
     num_splits = num_bins - 1
     if m - 1 <= num_splits:
-        return np.array([(v[i - 1] + v[i]) / 2.0 for i in range(1, m)])
+        with np.errstate(over="ignore"):                        # the midpoint of two values near +-1.8e308 is +-inf
+            return np.array([(v[i - 1] + v[i]) / 2.0 for i in range(1, m)])
     stride = float(int(np.sum(cnt))) / float(num_splits + 1)
     out, cur, target = [], int(cnt[0]), stride
     for i in range(1, m):
@@ -270,63 +271,82 @@ def train(labels, x, num_classes, num_trees, strategy, impurity, max_depth, max_
     n_thr = np.array([len(t) for t in thr])
     nb = int(n_thr.max()) + 1
     bins = np.stack([np.searchsorted(thr[f], x[:, f], side="left") for f in range(n_feat)], axis=1)
-    trees, runner_up = [], []
+    trees, runner_up, level_slots = [], [], []
     for t in range(num_trees):
         w = np.ones(n, np.int64) if num_trees == 1 else bag_weights(seed, t, n)
         nodes = {}
         at = np.ones(n, np.int64)                               # heap index of each row's node; 0 = at a leaf
         active, level = [1], 0
+        level_slots.append([])
         while active:
+            level_slots[-1].append(len(active))
             act = np.array(active)
             sub = np.stack([node_subset(seed, t, i, n_feat, k) for i in active])           # [S, K]
-            live = at > 0
-            slot = np.searchsorted(act, at[live])
-            hist = np.zeros((len(act), k, nb, num_classes), np.int64)
-            for kk in range(k):
-                b = bins[live][np.arange(live.sum()), sub[slot, kk]]
-                idx = (slot * nb + b) * num_classes + cls[live]
-                hist[:, kk] = np.bincount(idx, weights=w[live], minlength=len(act) * nb * num_classes).astype(
-                    np.int64).reshape(len(act), nb, num_classes)
-            gain, left, total = _gains(hist, n_thr[sub], kind)
-            flat = gain.reshape(len(act), -1)
-            best = flat.argmax(axis=1) if flat.shape[1] else np.zeros(len(act), np.int64)
+            live = np.flatnonzero(at > 0)
+            slot = np.searchsorted(act, at[live])              # each live row's slot, before this level moves any row
             nxt = []
-            for s, i in enumerate(active):
-                g = flat[s, best[s]] if flat.shape[1] else -np.inf
-                if np.isfinite(g):
-                    # the best gain among candidates whose left counts differ from the best's (equal counts give equal
-                    # gains on any device)
-                    lc = left[s].reshape(-1, num_classes)
-                    other = (lc != lc[best[s]]).any(axis=1)
-                    runner_up.append((g, flat[s][other].max() if other.any() else -np.inf))
-                tot = total[s]
-                rec = dict(counts=tot, impurity=float(impurity_of(tot, kind)), prediction=int(np.argmax(tot)),
-                           gain=0.0, leaf=True, feature=-1, threshold=0.0)
-                nodes[i] = rec
-                rows = at == i
-                if not np.isfinite(g) or g <= 0 or level == max_depth:
-                    at[rows] = 0
-                    continue
-                kk, j = divmod(int(best[s]), nb - 1)
-                f = int(sub[s, kk])
-                rec.update(leaf=False, feature=f, threshold=float(thr[f][j]), gain=float(g))
-                lc = left[s, kk, j]
-                for child, cc in ((2 * i, lc), (2 * i + 1, tot - lc)):
-                    ci = float(impurity_of(cc, kind))
-                    if level + 1 == max_depth or ci == 0.0:
-                        nodes[child] = dict(counts=cc, impurity=ci, prediction=int(np.argmax(cc)), gain=0.0,
-                                            leaf=True, feature=-1, threshold=0.0)
-                    else:
-                        nxt.append(child)
-                go_left = bins[:, f] <= j
-                at[rows & go_left] = 2 * i if (2 * i) in nxt else 0
-                at[rows & ~go_left] = 2 * i + 1 if (2 * i + 1) in nxt else 0
+            # the level's histograms and gains in batches of slots, so that a level of many large slots fits in memory
+            step = max(1, BATCH_ENTRIES // (k * nb * num_classes))
+            for b0 in range(0, len(act), step):
+                b1 = min(len(act), b0 + step)
+                sel = (slot >= b0) & (slot < b1)
+                lr, ls = live[sel], slot[sel] - b0
+                hist = np.zeros((b1 - b0, k, nb, num_classes), np.int64)
+                for kk in range(k):
+                    b = bins[lr, sub[b0 + ls, kk]]
+                    idx = (ls * nb + b) * num_classes + cls[lr]
+                    hist[:, kk] = np.bincount(idx, weights=w[lr], minlength=(b1 - b0) * nb * num_classes).astype(
+                        np.int64).reshape(b1 - b0, nb, num_classes)
+                gain, left, total = _gains(hist, n_thr[sub[b0:b1]], kind)
+                flat = gain.reshape(b1 - b0, -1)
+                best = flat.argmax(axis=1) if flat.shape[1] else np.zeros(b1 - b0, np.int64)
+                for s in range(b1 - b0):
+                    _decide(nodes, nxt, at, bins, thr, sub[b0 + s], active[b0 + s], flat[s], best[s], left[s],
+                            total[s], nb, num_classes, kind, level, max_depth, runner_up)
             active, level = sorted(nxt), level + 1
         trees.append(nodes)
     forest = flatten(trees, num_classes)
     if return_nodes:
-        return forest, dict(thresholds=thr, runner_up=runner_up, subset_size=k, trees=trees)
+        return forest, dict(thresholds=thr, runner_up=runner_up, subset_size=k, trees=trees, level_slots=level_slots)
     return forest
+
+
+# entries of one batch of slot histograms in train (int64; cumulative counts and impurities are as large again)
+BATCH_ENTRIES = 1 << 22
+
+
+def _decide(nodes, nxt, at, bins, thr, sub, i, flat, best, left, tot, nb, num_classes, kind, level, max_depth,
+            runner_up):
+    """Node i's record from its candidates' gains `flat` [K (NB - 1)], the first maximum `best`, left counts `left`
+    [K, NB - 1, C] and class totals `tot`; its children go to `nxt` (or are leaves) and its rows move to them in `at`."""
+    g = flat[best] if flat.shape[0] else -np.inf
+    if np.isfinite(g):
+        # the best gain among candidates whose left counts differ from the best's (equal counts give equal gains on
+        # any device)
+        lc = left.reshape(-1, num_classes)
+        other = (lc != lc[best]).any(axis=1)
+        runner_up.append((g, flat[other].max() if other.any() else -np.inf))
+    rec = dict(counts=tot, impurity=float(impurity_of(tot, kind)), prediction=int(np.argmax(tot)), gain=0.0, leaf=True,
+               feature=-1, threshold=0.0)
+    nodes[i] = rec
+    rows = at == i
+    if not np.isfinite(g) or g <= 0 or level == max_depth:
+        at[rows] = 0
+        return
+    kk, j = divmod(int(best), nb - 1)
+    f = int(sub[kk])
+    rec.update(leaf=False, feature=f, threshold=float(thr[f][j]), gain=float(g))
+    lc = left[kk, j]
+    for child, cc in ((2 * i, lc), (2 * i + 1, tot - lc)):
+        ci = float(impurity_of(cc, kind))
+        if level + 1 == max_depth or ci == 0.0:
+            nodes[child] = dict(counts=cc, impurity=ci, prediction=int(np.argmax(cc)), gain=0.0, leaf=True, feature=-1,
+                                threshold=0.0)
+        else:
+            nxt.append(child)
+    go_left = bins[:, f] <= j
+    at[rows & go_left] = 2 * i if (2 * i) in nxt else 0
+    at[rows & ~go_left] = 2 * i + 1 if (2 * i + 1) in nxt else 0
 
 
 def _prune(nodes, i):
