@@ -129,7 +129,8 @@ __global__ void head_flags_kernel(const uint64_t* keys, long long n, uint32_t* f
   const long long e = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (e < n) flag[e] = (e == 0 || keys[e] != keys[e - 1]) ? 1u : 0u;
 }
-// one thread per run head: fold the run in event order (sum) or pick the latest event (keep-last)
+// one thread per run head: fold the run in event order (sum: reduceByKey(_ + _), so a run of one keeps its rating's
+// bits, -0.0 included) or pick the latest event (keep-last)
 __global__ void dedup_compact_kernel(const uint64_t* keys, const uint32_t* pay, const uint32_t* pos,
                                      long long n, int bits_i, const float* rating, const long long* ts,
                                      int mode, int* ou, int* oi, float* orr) {
@@ -139,8 +140,8 @@ __global__ void dedup_compact_kernel(const uint64_t* keys, const uint32_t* pay, 
   if (e > 0 && keys[e - 1] == key) return;
   float acc;
   if (mode == PIO_ALS_DEDUP_SUM) {
-    acc = 0.f;
-    for (long long t = e; t < n && keys[t] == key; ++t) acc += rating[pay[t]];
+    acc = rating[pay[e]];
+    for (long long t = e + 1; t < n && keys[t] == key; ++t) acc += rating[pay[t]];
   } else {
     long long best_t = ts ? ts[pay[e]] : 0;
     uint32_t best_p = pay[e];
@@ -1560,6 +1561,9 @@ static int set_ratings_impl(pio_als_handle* h, const int32_t* user, const int32_
   if (nnz < 0 || (nnz == 0 && !may_be_empty))
     return fail(h, PIO_ALS_ERR_ARG, "ratings cannot be empty (the templates require(!ratings.take(1).isEmpty))");
   if (nnz > 0 && (!user || !item || !rating)) return fail(h, PIO_ALS_ERR_ARG, "null rating arrays");
+  // before anything is staged: a host copy of nnz events would read past arrays the call is about to refuse
+  if (nnz >= (1ll << 32)) return fail(h, PIO_ALS_ERR_ARG, "nnz must be < 2^32 per call");
+  if (dedup_mode < 0 || dedup_mode > 2) return fail(h, PIO_ALS_ERR_ARG, "bad dedup_mode %d", dedup_mode);
   std::lock_guard<std::mutex> lk(h->mu);
   CK(h, cudaSetDevice(h->cfg.device));
   cudaStream_t st = h->stream;
@@ -1622,6 +1626,39 @@ int pio_als_set_ratings_coo_sharded(pio_als_handle* h, const int32_t* user, cons
 int pio_als_set_ratings_coo_sharded_device(pio_als_handle* h, const int32_t* d_user, const int32_t* d_item,
                                            const float* d_rating, int64_t nnz_local, int dedup_mode, const int64_t* d_ts) {
   return set_ratings_impl(h, d_user, d_item, d_rating, nnz_local, dedup_mode, d_ts, true, true);
+}
+
+/* debug only (not in pio_als.h): what the last set_ratings built on one side (0 = users, 1 = items) of this rank.
+ * scalars[11]: n, R, n_internal, bits, nnz_local, n_active, n_heavy, n_parts, nnz after dedup over all ranks, heavy_t,
+ * part_len.  Arrays (HOST; each may be null, sizes from scalars): deg / npos / perm / rpos [n], inv [n_internal], the
+ * local ptr [R + 1], idx / val [nnz_local], nreg [R], part_beg / part_end [n_parts], row_part_ptr [n_heavy + 1].  Only
+ * copies out; changes nothing.  Used by tests/test_gpu_ingest.py. */
+__attribute__((visibility("default"))) int pio_als_debug_side(pio_als_handle* h, int side, int64_t scalars[11],
+                                                              uint32_t* deg, uint32_t* npos, int32_t* perm, int32_t* inv,
+                                                              int32_t* rpos, int64_t* ptr, int32_t* idx, float* val,
+                                                              float* nreg, int64_t* part_beg, int64_t* part_end,
+                                                              int32_t* row_part_ptr) {
+  if (!h || !scalars || (side != 0 && side != 1)) return PIO_ALS_ERR_ARG;
+  std::lock_guard<std::mutex> lk(h->mu);
+  if (!h->have_ratings) return fail(h, PIO_ALS_ERR_STATE, "pio_als_debug_side before set_ratings");
+  CK(h, cudaSetDevice(h->cfg.device));
+  const Side& s = side == 0 ? h->U : h->I;
+  const int64_t v[11] = {s.n, s.R, s.n_internal, s.bits, s.nnz_local, s.n_active, s.n_heavy, s.n_parts, h->st.nnz,
+                         s.plan.heavy_t, s.plan.part_len};
+  std::copy(v, v + 11, scalars);
+  const cudaStream_t st = h->stream;
+  const struct { void* to; const void* from; size_t bytes; } jobs[] = {
+      {deg, s.deg, sizeof(uint32_t) * (size_t)s.n},          {npos, s.npos, sizeof(uint32_t) * (size_t)s.n},
+      {perm, s.perm, sizeof(int32_t) * (size_t)s.n},         {inv, s.inv, sizeof(int32_t) * (size_t)s.n_internal},
+      {rpos, s.rpos, sizeof(int32_t) * (size_t)s.n},         {ptr, s.ptr, sizeof(int64_t) * ((size_t)s.R + 1)},
+      {idx, s.idx, sizeof(int32_t) * (size_t)s.nnz_local},   {val, s.val, sizeof(float) * (size_t)s.nnz_local},
+      {nreg, s.nreg, sizeof(float) * (size_t)s.R},           {part_beg, s.part_beg, sizeof(int64_t) * (size_t)s.n_parts},
+      {part_end, s.part_end, sizeof(int64_t) * (size_t)s.n_parts}};
+  for (const auto& j : jobs)
+    if (j.to && j.bytes) CK(h, cudaMemcpyAsync(j.to, j.from, j.bytes, cudaMemcpyDeviceToHost, st));
+  if (row_part_ptr && s.n_heavy > 0) std::copy(s.h_row_part_ptr.begin(), s.h_row_part_ptr.end(), row_part_ptr);
+  CK(h, cudaStreamSynchronize(st));
+  return PIO_ALS_OK;
 }
 
 int pio_als_set_init(pio_als_handle* h, const float* user_factors, const float* item_factors) {

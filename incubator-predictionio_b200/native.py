@@ -433,6 +433,30 @@ class NativeALS:
         out["last_score_path"] = {name for name, bit in SCORE_PATH_BITS.items() if st.last_score_path & bit}
         return out
 
+    _SIDE_SCALARS = ("n", "R", "n_internal", "bits", "nnz_local", "n_active", "n_heavy", "n_parts", "nnz", "heavy_t",
+                     "part_len")
+
+    def debug_side(self, side: str) -> dict:
+        """What the last set_ratings built on one side ("user" or "item") of this rank (pio_als_debug_side, debug only):
+        the scalars of _SIDE_SCALARS, then deg / npos / perm / rpos per external row, inv per internal row (-1: padding),
+        the local CSR ptr / idx / val, nreg per local row, and the heavy rows' part bounds part_beg / part_end and
+        row_part_ptr."""
+        f = lib().pio_als_debug_side
+        sc = np.zeros(len(self._SIDE_SCALARS), np.int64)
+        which = {"user": 0, "item": 1}[side]
+        nul = [None] * 12
+        self._check(f(self._h, C.c_int(which), _ptr(sc, C.c_int64), *nul))
+        out = dict(zip(self._SIDE_SCALARS, (int(x) for x in sc)))
+        n, R, nl = out["n"], out["R"], out["nnz_local"]
+        arrs = dict(deg=np.empty(n, np.uint32), npos=np.empty(n, np.uint32), perm=np.empty(n, np.int32),
+                    inv=np.empty(out["n_internal"], np.int32), rpos=np.empty(n, np.int32), ptr=np.empty(R + 1, np.int64),
+                    idx=np.empty(nl, np.int32), val=np.empty(nl, np.float32), nreg=np.empty(R, np.float32),
+                    part_beg=np.empty(out["n_parts"], np.int64), part_end=np.empty(out["n_parts"], np.int64),
+                    row_part_ptr=np.zeros(out["n_heavy"] + 1, np.int32))
+        self._check(f(self._h, C.c_int(which), _ptr(sc, C.c_int64), *(C.c_void_p(a.ctypes.data) for a in arrs.values())))
+        out.update(arrs)
+        return out
+
     def phase_ms(self) -> dict:
         """Device-time breakdown of the last run (pio_als_get_phase_ms)."""
         out = (C.c_double * 8)()

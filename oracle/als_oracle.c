@@ -275,8 +275,8 @@ ORACLE_API int64_t oracle_csr_dedup_sum(int32_t n_rows, int64_t *ptr, int32_t *c
       qsort(buf, (size_t)n, sizeof(dd_ent), dd_cmp);
       int64_t o = 0;
       for (int64_t t = 0; t < n;) {
-        float acc = 0.f;
-        int64_t u = t;
+        float acc = buf[t].v;   /* reduceByKey(_ + _): a run of one keeps its value, -0.0 included */
+        int64_t u = t + 1;
         while (u < n && buf[u].c == buf[t].c) { acc = acc + buf[u].v; ++u; }
         col[b + o] = buf[t].c;
         val[b + o] = acc;

@@ -237,14 +237,14 @@ def dedup_coo(user, item, rating, mode="none", ts=None):
     head[1:] = ks[1:] != ks[:-1]
     starts = np.flatnonzero(head)
     if mode == "sum":
-        # sequential fp32 sums in input order (matches a left fold)
+        # sequential fp32 sums in input order (reduceByKey(_ + _): a run of one keeps its rating, -0.0 included)
         seg = np.cumsum(head) - 1
         out = np.zeros(starts.shape[0], np.float32)
         rs = rating[order]
         for s in range(starts.shape[0]):
             e = starts[s + 1] if s + 1 < starts.shape[0] else ks.shape[0]
-            acc = np.float32(0)
-            for v in rs[starts[s]:e]:
+            acc = rs[starts[s]]
+            for v in rs[starts[s] + 1:e]:
                 acc = np.float32(acc + v)
             out[s] = acc
         del seg

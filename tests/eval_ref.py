@@ -56,18 +56,21 @@ def split(user, item, rating, k_fold: int):
 def rank_counts(fold: dict, items: np.ndarray, count: np.ndarray, k: int, threshold: float):
     """hits, npos, nraw per query of `fold` for a top-N result (items [n_queries, num] of fold-local indices, count valid
     entries per query): hits among the first min(k, count) items of a test item with a rating >= threshold, the number of
-    distinct such test items, and the number of test ratings >= threshold."""
+    distinct such test items, and the number of test ratings >= threshold.  Vectorised over sorted (query, item) keys."""
     nq = fold["query_user"].shape[0]
     num = items.shape[1]
-    hits, npos, nraw = (np.zeros(nq, np.int64) for _ in range(3))
-    for q in range(nq):
-        mine = fold["test_q"] == q
-        ok = fold["test_rating"][mine] >= threshold
-        positives = set(fold["test_item"][mine][ok].tolist())
-        nraw[q] = int(ok.sum())
-        npos[q] = len(positives)
-        kk = min(k, int(count[q]), num)
-        hits[q] = sum(int(fold["item"][items[q, j]]) in positives for j in range(kk))
+    ok = fold["test_rating"] >= threshold
+    q = fold["test_q"].astype(np.int64)
+    width = int(max(int(fold["test_item"].max(initial=0)), int(fold["item"].max(initial=0)))) + 1
+    positives = np.unique(q[ok] * width + fold["test_item"][ok].astype(np.int64))   # sorted (query, item) keys
+    nraw = np.bincount(q[ok], minlength=nq).astype(np.int64)
+    npos = np.bincount(positives // width, minlength=nq).astype(np.int64)
+    kk = np.minimum(np.minimum(int(k), np.asarray(count, np.int64)), num)
+    qq, jj = np.nonzero(np.arange(num)[None, :] < kk[:, None])
+    want = qq * width + fold["item"][items[qq, jj]].astype(np.int64)
+    at = np.minimum(np.searchsorted(positives, want), max(positives.shape[0] - 1, 0))
+    hit = positives[at] == want if positives.shape[0] else np.zeros(want.shape[0], bool)
+    hits = np.bincount(qq[hit], minlength=nq).astype(np.int64)
     return hits, npos, nraw
 
 

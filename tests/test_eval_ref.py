@@ -102,6 +102,43 @@ def _predictions(rng, fold, num):
     return items, count
 
 
+def _rank_counts_loop(fold, items, count, k, threshold):
+    """eval_ref.rank_counts written one query at a time, straight from its definition."""
+    nq = fold["query_user"].shape[0]
+    num = items.shape[1]
+    hits, npos, nraw = (np.zeros(nq, np.int64) for _ in range(3))
+    for q in range(nq):
+        mine = fold["test_q"] == q
+        ok = fold["test_rating"][mine] >= threshold
+        positives = set(fold["test_item"][mine][ok].tolist())
+        nraw[q] = int(ok.sum())
+        npos[q] = len(positives)
+        kk = min(k, int(count[q]), num)
+        hits[q] = sum(int(fold["item"][items[q, j]]) in positives for j in range(kk))
+    return hits, npos, nraw
+
+
+@pytest.mark.parametrize("seed,n,n_users,n_items,k_fold", CASES)
+@pytest.mark.parametrize("num", [1, 4, 10])
+def test_vectorised_rank_counts_equal_the_loop(seed, n, n_users, n_items, k_fold, num):
+    users, items, ratings = _case(seed, n, n_users, n_items)
+    gu, _ = _global(users)
+    gi, _ = _global(items)
+    ratings = ratings.copy()
+    ratings[::11] = np.nan
+    ratings[::13] = -np.inf
+    ratings[::17] = np.inf
+    rng = np.random.default_rng(seed + 7)
+    for f, fold in enumerate(eval_ref.split(gu, gi, ratings, k_fold)):
+        it, cnt = _predictions(rng, fold, num)
+        for k in (1, num, num + 5, 1000):
+            for thr in (-np.inf, 0.0, *THRESHOLDS, np.inf):
+                got = eval_ref.rank_counts(fold, it, cnt, k, thr)
+                want = _rank_counts_loop(fold, it, cnt, k, thr)
+                for g, x in zip(got, want):
+                    assert np.array_equal(g, x), (f, k, thr)
+
+
 class _RefResult:
     """A fold result whose rank counts come from eval_ref (what native.EvalResult returns from the device)."""
 
