@@ -35,6 +35,10 @@
  *       examples/scala-parallel-classification/add-algorithm/src/main/scala/NaiveBayesAlgorithm.scala:41-57
  *   pio_rf_train / pio_rf_predict replace RandomForest.trainClassifier / model.predict
  *       examples/scala-parallel-classification/add-algorithm/src/main/scala/RandomForestAlgorithm.scala:46-70
+ *   pio_eval_folds_* run the recommendation template's k-fold evaluation
+ *       examples/scala-parallel-recommendation/blacklist-items/src/main/scala/{DataSource.scala readEval, Evaluation.scala}
+ *   pio_cls_folds_* run the classification template's k-fold evaluation
+ *       examples/scala-parallel-classification/add-algorithm/src/main/scala/{DataSource.scala readEval, Evaluation.scala}
  */
 #ifndef PIO_ALS_H_
 #define PIO_ALS_H_
@@ -551,6 +555,48 @@ PIO_API int pio_rf_forest_destroy(pio_rf_forest* f);
 PIO_API int pio_rf_predict(int device, int32_t n_trees, const int32_t* tree_off, int64_t n_nodes, const int32_t* feature,
                            const double* threshold, const int32_t* left, const int32_t* right, const int32_t* prediction,
                            int32_t num_classes, const double* x, int64_t n, int32_t n_feat, int32_t* out);
+
+/* k-fold evaluation of the classification template on the device: its `pio eval` (examples/scala-parallel-classification/
+ * add-algorithm/src/main/scala/{DataSource.scala readEval, Evaluation.scala, PrecisionEvaluation.scala}) without a host
+ * copy of a fold's rows per training (DESIGN.md 4.12).  An opaque object owns device copies of n labeled points (fp64
+ * labels, n x n_feat fp64 features, row-major) and each row's index among the distinct labels; row i is in the test set
+ * of fold i % k_fold and in the training set of every other fold, in row order.  Labels must be finite; -0.0 and 0.0 are
+ * one label.  Errors: status codes as above, text via pio_als_last_error(NULL); arguments are checked before any device
+ * work. */
+typedef struct pio_cls_folds pio_cls_folds;
+
+/* label: n (HOST), x: n x n_feat (HOST); 1 <= n < 2^31, n_feat >= 1, k_fold >= 1. */
+PIO_API int pio_cls_folds_create(int device, const double* label, const double* x, int64_t n, int32_t n_feat,
+                                 int32_t k_fold, pio_cls_folds** out);
+/* out[0] training rows, out[1] test rows of fold `fold`. */
+PIO_API int pio_cls_folds_sizes(const pio_cls_folds* f, int32_t fold, int64_t out[2]);
+/* The distinct labels of the fold's training rows, ascending (np.unique of them): *n_class their number, labels
+ * (nullable) receives them. */
+PIO_API int pio_cls_folds_classes(const pio_cls_folds* f, int32_t fold, int32_t* n_class, double* labels);
+/* pio_nb_train on the fold's training rows: features rounded to float32, class = index among the fold's training
+ * labels.  n_class must be the fold's (pio_cls_folds_classes); pi: n_class, theta: n_class x n_feat (HOST).  A negative
+ * float32 feature in a training row fails with PIO_ALS_ERR_NUMERIC and MLlib's message. */
+PIO_API int pio_cls_folds_nb_train(pio_cls_folds* f, int32_t fold, double lambda, int32_t n_class, double* pi,
+                                   double* theta);
+/* pio_rf_train on the fold's training rows, with its checks and messages (a row number is the row's position in the
+ * fold's training set); the forest is identical to pio_rf_train's on those rows copied to the host. */
+PIO_API int pio_cls_folds_rf_train(pio_cls_folds* f, int32_t fold, const pio_rf_params* params, pio_rf_forest** out);
+/* Predicts every test row of the fold and keeps the predicted labels on the object (8 bytes per row) until
+ * pio_cls_folds_result_free: nb_predict with a NaiveBayes model (pio_nb_predict's class index -> class_label[index],
+ * class_label: n_class entries), rf_predict with a forest given as pio_rf_predict takes it (label = class index). */
+PIO_API int pio_cls_folds_nb_predict(pio_cls_folds* f, int32_t fold, int32_t n_class, const double* pi,
+                                     const double* theta, const double* class_label, int32_t* out_result);
+PIO_API int pio_cls_folds_rf_predict(pio_cls_folds* f, int32_t fold, int32_t n_trees, const int32_t* tree_off,
+                                     int64_t n_nodes, const int32_t* feature, const double* threshold,
+                                     const int32_t* left, const int32_t* right, const int32_t* prediction,
+                                     int32_t num_classes, int32_t* out_result);
+/* The predicted label of every test row of the result's fold, in row order (HOST, out[1] of pio_cls_folds_sizes). */
+PIO_API int pio_cls_folds_result_labels(const pio_cls_folds* f, int32_t result, double* out);
+/* out[0] test rows, out[1] rows with predicted == actual label, out[2] rows with predicted == label, out[3] those of
+ * out[2] that are correct (fp64 ==).  Accuracy = out[1] / out[0], Precision(label) = out[3] / out[2]. */
+PIO_API int pio_cls_folds_result_counts(const pio_cls_folds* f, int32_t result, double label, int64_t out[4]);
+PIO_API int pio_cls_folds_result_free(pio_cls_folds* f, int32_t result);
+PIO_API int pio_cls_folds_destroy(pio_cls_folds* f);
 
 #ifdef __cplusplus
 }

@@ -245,6 +245,9 @@ class LFirstServing(LServing):
     def serve(self, query, predictions):
         return predictions[0]
 
+    def serveColumns(self, queries, predictions):
+        return predictions[0]
+
 
 # ---- EngineParams / Engine ----------------------------------------------------------------------
 @dataclass

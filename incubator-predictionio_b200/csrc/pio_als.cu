@@ -55,6 +55,7 @@
 #include "cooc.cuh"
 #include "forest.cuh"
 #include "eval_folds.cuh"
+#include "cls_folds.cuh"
 
 namespace pio {
 
@@ -2941,6 +2942,13 @@ __attribute__((visibility("default"))) int pio_als_debug_timing(pio_als_handle* 
     if (e_ != cudaSuccess) return fail(nullptr, PIO_ALS_ERR_CUDA, "%s failed: %s", #call, cudaGetErrorString(e_)); \
   } while (0)
 
+// a status-returning call: return its status unless it is PIO_ALS_OK
+#define EVF(call)                          \
+  do {                                     \
+    const int rc_ = (call);                \
+    if (rc_ != PIO_ALS_OK) return rc_;     \
+  } while (0)
+
 /* debug only (not in pio_als.h): the lockstep Cholesky of als_lockstep.cuh on n dense SPD systems (A: n x N x N
  * row-major, b: n x N; HOST buffers), N = 64 or 128; x = (A + ridge I)^-1 b.  reps > 1 repeats fill + solve for timing
  * (ms_out = device time of the launch).  Used by tests/test_gpu_lockstep.py and tools/bench_solver.py. */
@@ -4390,33 +4398,33 @@ int pio_cooc_train(int device, const int32_t* user, const int32_t* item, int64_t
 }
 
 // ---- NaiveBayes ---------------------------------------------------------------------------------
-int pio_nb_train(int device, const int32_t* label, const float* x, int64_t n, int n_feat, int n_class, double lambda,
-                 double* pi, double* theta) {
-  if (!label || !x || !pi || !theta || n <= 0 || n_feat < 1 || n_class < 1)
-    return fail(nullptr, PIO_ALS_ERR_ARG, "bad NaiveBayes arguments");
+}  // extern "C"
+
+namespace pio {
+
+static int nb_check_width(int n_feat, int n_class) {
+  if ((size_t)n_class * (n_feat + 1) * 8 * sizeof(double) > 200 * 1024)
+    return fail(nullptr, PIO_ALS_ERR_ARG, "n_class*(n_feat+1) too large");
+  return PIO_ALS_OK;
+}
+
+// pi / theta of n device rows (class index dl, float32 features dx) on stream st: the per-class sums on the device, the
+// log-probabilities on the host.  pio_nb_train and pio_cls_folds_nb_train both end here.
+static int nb_fit(CallMem& tmp, cudaStream_t st, const int* dl, const float* dx, int64_t n, int n_feat, int n_class,
+                  double lambda, double* pi, double* theta) {
   const int width = n_class * (n_feat + 1);
-  if ((size_t)width * 8 * sizeof(double) > 200 * 1024) return fail(nullptr, PIO_ALS_ERR_ARG, "n_class*(n_feat+1) too large");
-  CK0(cudaSetDevice(device));
-  for (int64_t r = 0; r < n; ++r)
-    if (label[r] < 0 || label[r] >= n_class) return fail(nullptr, PIO_ALS_ERR_ARG, "label out of range at row %lld", (long long)r);
-  CallMem tmp(0);
-  int* dl = nullptr;
-  float* dx = nullptr;
   double *dp = nullptr, *dout = nullptr;
   const int nb = 296;
-  CK0(tmp.device(&dl, (size_t)n));
-  CK0(tmp.device(&dx, (size_t)n * n_feat));
   CK0(tmp.device(&dp, (size_t)nb * width));
   CK0(tmp.device(&dout, (size_t)width));
-  CK0(cudaMemcpy(dl, label, sizeof(int) * n, cudaMemcpyHostToDevice));
-  CK0(cudaMemcpy(dx, x, sizeof(float) * n * n_feat, cudaMemcpyHostToDevice));
   const size_t smem = sizeof(double) * 8 * width;
   CK0(cudaFuncSetAttribute(nb_partial_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  nb_partial_kernel<<<nb, 256, smem>>>(dl, dx, n, n_feat, n_class, dp);
-  nb_reduce_kernel<<<nblk(width, 128), 128>>>(dp, nb, width, dout);
+  nb_partial_kernel<<<nb, 256, smem, st>>>(dl, dx, n, n_feat, n_class, dp);
+  nb_reduce_kernel<<<nblk(width, 128), 128, 0, st>>>(dp, nb, width, dout);
   CK0(cudaGetLastError());
   std::vector<double> acc(width);
-  CK0(cudaMemcpy(acc.data(), dout, sizeof(double) * width, cudaMemcpyDeviceToHost));
+  CK0(cudaMemcpyAsync(acc.data(), dout, sizeof(double) * width, cudaMemcpyDeviceToHost, st));
+  CK0(cudaStreamSynchronize(st));
   // MLlib multinomial: pi_c = log(n_c + l) - log(N + C l); theta_cj = log(s_cj + l) - log(sum_j s_cj + F l)
   const double logden = log((double)n + n_class * lambda);
   for (int c = 0; c < n_class; ++c) {
@@ -4427,6 +4435,28 @@ int pio_nb_train(int device, const int32_t* label, const float* x, int64_t n, in
     for (int j = 0; j < n_feat; ++j) theta[c * n_feat + j] = log(acc[c * (n_feat + 1) + j] + lambda) - lt;
   }
   return PIO_ALS_OK;
+}
+
+}  // namespace pio
+
+extern "C" {
+
+int pio_nb_train(int device, const int32_t* label, const float* x, int64_t n, int n_feat, int n_class, double lambda,
+                 double* pi, double* theta) {
+  if (!label || !x || !pi || !theta || n <= 0 || n_feat < 1 || n_class < 1)
+    return fail(nullptr, PIO_ALS_ERR_ARG, "bad NaiveBayes arguments");
+  EVF(nb_check_width(n_feat, n_class));
+  CK0(cudaSetDevice(device));
+  for (int64_t r = 0; r < n; ++r)
+    if (label[r] < 0 || label[r] >= n_class) return fail(nullptr, PIO_ALS_ERR_ARG, "label out of range at row %lld", (long long)r);
+  CallMem tmp(0);
+  int* dl = nullptr;
+  float* dx = nullptr;
+  CK0(tmp.device(&dl, (size_t)n));
+  CK0(tmp.device(&dx, (size_t)n * n_feat));
+  CK0(cudaMemcpy(dl, label, sizeof(int) * n, cudaMemcpyHostToDevice));
+  CK0(cudaMemcpy(dx, x, sizeof(float) * n * n_feat, cudaMemcpyHostToDevice));
+  return nb_fit(tmp, 0, dl, dx, n, n_feat, n_class, lambda, pi, theta);
 }
 
 int pio_nb_predict(int device, const float* x, int64_t n, int n_feat, int n_class, const double* pi, const double* theta,
@@ -4499,7 +4529,30 @@ static std::string rf_fmt(double v) {
   return s;
 }
 
-static int rf_check(const pio_rf_params* p, const double* label, const double* x, int64_t n, int F) {
+// the row checks' messages, row r being the r-th row of the training set: a non-finite label, else the first non-finite
+// feature of the row
+static int rf_fail_finite(int64_t r, double label, const double* xr, int F) {
+  if (!isfinite(label))
+    return fail(nullptr, PIO_ALS_ERR_ARG, "label of row %lld is not finite (%s).", (long long)r, rf_fmt(label).c_str());
+  for (int f = 0; f < F; ++f)
+    if (!isfinite(xr[f]))
+      return fail(nullptr, PIO_ALS_ERR_ARG, "feature %d of row %lld is not finite (%s).", f, (long long)r,
+                  rf_fmt(xr[f]).c_str());
+  return PIO_ALS_OK;
+}
+static int rf_fail_label(const pio_rf_params* p, double label) {
+  const char* agg = p->impurity == RF_GINI ? "GiniAggregator" : "EntropyAggregator";
+  if (label >= p->num_classes)
+    return fail(nullptr, PIO_ALS_ERR_ARG, "%s given label %s but requires label < numClasses (= %d).", agg,
+                rf_fmt(label).c_str(), p->num_classes);
+  if (label < 0)
+    return fail(nullptr, PIO_ALS_ERR_ARG, "%s given label %sbut requires label is non-negative.", agg,
+                rf_fmt(label).c_str());
+  return PIO_ALS_OK;
+}
+
+// the parameters and the shape (n rows, F features), before any row is read
+static int rf_check_params(const pio_rf_params* p, int64_t n, int F) {
   const int C = p->num_classes;
   if (C < 2)
     return fail(nullptr, PIO_ALS_ERR_ARG, "DecisionTree Strategy for Classification must have numClasses >= 2, but "
@@ -4528,25 +4581,14 @@ static int rf_check(const pio_rf_params* p, const double* label, const double* x
     return fail(nullptr, PIO_ALS_ERR_ARG, "unknown impurity code %d", p->impurity);
   if (n < 1 || F < 1) return fail(nullptr, PIO_ALS_ERR_ARG, "RandomForest requires at least one row and one feature.");
   if (n >= (1ll << 31)) return fail(nullptr, PIO_ALS_ERR_ARG, "at most 2^31 - 1 rows are supported.");
+  return PIO_ALS_OK;
+}
+
+static int rf_check(const pio_rf_params* p, const double* label, const double* x, int64_t n, int F) {
+  EVF(rf_check_params(p, n, F));
   if (!label || !x) return fail(nullptr, PIO_ALS_ERR_ARG, "bad pio_rf_train arguments");
-  for (int64_t r = 0; r < n; ++r) {
-    if (!isfinite(label[r]))
-      return fail(nullptr, PIO_ALS_ERR_ARG, "label of row %lld is not finite (%s).", (long long)r,
-                  rf_fmt(label[r]).c_str());
-    for (int f = 0; f < F; ++f)
-      if (!isfinite(x[r * F + f]))
-        return fail(nullptr, PIO_ALS_ERR_ARG, "feature %d of row %lld is not finite (%s).", f, (long long)r,
-                    rf_fmt(x[r * F + f]).c_str());
-  }
-  const char* agg = p->impurity == RF_GINI ? "GiniAggregator" : "EntropyAggregator";
-  for (int64_t r = 0; r < n; ++r) {
-    if (label[r] >= C)
-      return fail(nullptr, PIO_ALS_ERR_ARG, "%s given label %s but requires label < numClasses (= %d).", agg,
-                  rf_fmt(label[r]).c_str(), C);
-    if (label[r] < 0)
-      return fail(nullptr, PIO_ALS_ERR_ARG, "%s given label %sbut requires label is non-negative.", agg,
-                  rf_fmt(label[r]).c_str());
-  }
+  for (int64_t r = 0; r < n; ++r) EVF(rf_fail_finite(r, label[r], x + r * F, F));
+  for (int64_t r = 0; r < n; ++r) EVF(rf_fail_label(p, label[r]));
   return PIO_ALS_OK;
 }
 
@@ -4780,38 +4822,13 @@ static int rf_bin_and_grow(const RfCtx& c) {
   return PIO_ALS_OK;
 }
 
-}  // namespace pio
-
-extern "C" {
-
-int pio_rf_train(int device, const pio_rf_params* p, const double* label, const double* x, int64_t n, int32_t n_feat,
-                 pio_rf_forest** out) {
-  if (!p || !out) return fail(nullptr, PIO_ALS_ERR_ARG, "bad pio_rf_train arguments");
-  *out = nullptr;
-  const int rc = rf_check(p, label, x, n, n_feat);
-  if (rc != PIO_ALS_OK) return rc;
-  const int F = n_feat, C = p->num_classes, K = rf_subset_size(p->feature_subset_strategy, F, p->num_trees);
-  g_rf_timing = RfTiming();
+// The forest from n rows already on the device (dx: n x F fp64, dcls: class bytes) on stream st: split search, bin
+// codes, then every tree group level by level.  pio_rf_train and pio_cls_folds_rf_train both end here; g_rf_timing's
+// later phases are timed from t0.
+static int rf_fit(const pio_rf_params* p, const double* dx, const uint8_t* dcls, int64_t n, int F, int sm, CallMem& tmp,
+                  cudaStream_t st, std::chrono::steady_clock::time_point t0, pio_rf_forest** out) {
+  const int C = p->num_classes, K = rf_subset_size(p->feature_subset_strategy, F, p->num_trees);
   RfTiming& tm = g_rf_timing;
-  auto t0 = std::chrono::steady_clock::now();
-  CK0(cudaSetDevice(device));
-  int sm = 0;
-  CK0(cudaDeviceGetAttribute(&sm, cudaDevAttrMultiProcessorCount, device));
-  std::vector<uint8_t> hcls((size_t)n);
-  for (int64_t r = 0; r < n; ++r) hcls[r] = (uint8_t)(int)trunc(label[r]);
-  CallMem tmp;
-  cudaStream_t st;
-  CK0(tmp.stream(&st));
-  double* dx = nullptr;
-  uint8_t* dcls = nullptr;
-  CK0(tmp.device(&dx, (size_t)n * F));
-  CK0(tmp.device(&dcls, (size_t)n));
-  rf_ms(t0);
-  CK0(cudaMemcpyAsync(dx, x, sizeof(double) * (size_t)n * F, cudaMemcpyHostToDevice, st));
-  CK0(cudaMemcpyAsync(dcls, hcls.data(), (size_t)n, cudaMemcpyHostToDevice, st));
-  CK0(cudaStreamSynchronize(st));
-  tm.h2d = rf_ms(t0);
-
   // split sample, then per feature its sorted distinct values: thresholds on the host (findSplitsForContinuousFeature)
   const double frac = rf_sample_fraction(n, p->max_bins);
   uint32_t* rows = nullptr;
@@ -4910,6 +4927,93 @@ int pio_rf_train(int device, const pio_rf_params* p, const double* label, const 
   return PIO_ALS_OK;
 }
 
+// a forest as the flat arrays of pio_rf_forest_get (HOST)
+struct RfFlat {
+  int32_t n_trees;
+  const int32_t* tree_off;
+  int64_t n_nodes;
+  const int32_t *feature;
+  const double* threshold;
+  const int32_t *left, *right, *prediction;
+  int32_t num_classes;
+};
+
+// a walk must end: children come after their parent (preorder) and stay in their tree
+static int rf_check_flat(const RfFlat& a, int32_t n_feat) {
+  if (!a.tree_off || !a.feature || !a.threshold || !a.left || !a.right || !a.prediction || a.n_trees < 1 ||
+      a.n_nodes < 1 || a.n_nodes >= (1ll << 31) || a.num_classes < 1 || a.num_classes > RF_MAX_CLASSES || n_feat < 1)
+    return fail(nullptr, PIO_ALS_ERR_ARG, "bad pio_rf_predict arguments");
+  for (int32_t t = 0; t < a.n_trees; ++t) {
+    const int64_t lo = a.tree_off[t], hi = t + 1 < a.n_trees ? a.tree_off[t + 1] : a.n_nodes;
+    if (lo < 0 || lo >= hi || hi > a.n_nodes) return fail(nullptr, PIO_ALS_ERR_ARG, "bad tree offsets");
+    for (int64_t i = lo; i < hi; ++i) {
+      if (a.prediction[i] < 0 || a.prediction[i] >= a.num_classes) return fail(nullptr, PIO_ALS_ERR_ARG, "bad prediction");
+      if (a.feature[i] >= n_feat) return fail(nullptr, PIO_ALS_ERR_ARG, "node %lld uses feature %d of %d", (long long)i,
+                                              a.feature[i], n_feat);
+      if (a.feature[i] >= 0 && (a.left[i] <= i || a.left[i] >= hi || a.right[i] <= i || a.right[i] >= hi))
+        return fail(nullptr, PIO_ALS_ERR_ARG, "bad children at node %lld", (long long)i);
+    }
+  }
+  return PIO_ALS_OK;
+}
+
+// the vote (class index) of n >= 1 device rows dx (n x F) into dout, on stream st
+static int rf_predict_device(CallMem& tmp, cudaStream_t st, const RfFlat& a, const double* dx, int64_t n, int F,
+                             int* dout) {
+  const int64_t nn = a.n_nodes;
+  int *dto = nullptr, *df = nullptr, *dl = nullptr, *dr = nullptr, *dp = nullptr;
+  double* dt = nullptr;
+  CK0(tmp.device(&dto, (size_t)a.n_trees));
+  CK0(tmp.device(&df, (size_t)nn));
+  CK0(tmp.device(&dl, (size_t)nn));
+  CK0(tmp.device(&dr, (size_t)nn));
+  CK0(tmp.device(&dp, (size_t)nn));
+  CK0(tmp.device(&dt, (size_t)nn));
+  CK0(cudaMemcpyAsync(dto, a.tree_off, 4 * (size_t)a.n_trees, cudaMemcpyHostToDevice, st));
+  CK0(cudaMemcpyAsync(df, a.feature, 4 * (size_t)nn, cudaMemcpyHostToDevice, st));
+  CK0(cudaMemcpyAsync(dl, a.left, 4 * (size_t)nn, cudaMemcpyHostToDevice, st));
+  CK0(cudaMemcpyAsync(dr, a.right, 4 * (size_t)nn, cudaMemcpyHostToDevice, st));
+  CK0(cudaMemcpyAsync(dp, a.prediction, 4 * (size_t)nn, cudaMemcpyHostToDevice, st));
+  CK0(cudaMemcpyAsync(dt, a.threshold, 8 * (size_t)nn, cudaMemcpyHostToDevice, st));
+  rf::predict_kernel<<<nblk(n, 128), 128, sizeof(int) * 128 * (size_t)a.num_classes, st>>>(
+      dto, a.n_trees, df, dt, dl, dr, dp, a.num_classes, dx, n, F, dout);
+  CK0(cudaGetLastError());
+  return PIO_ALS_OK;
+}
+
+}  // namespace pio
+
+extern "C" {
+
+int pio_rf_train(int device, const pio_rf_params* p, const double* label, const double* x, int64_t n, int32_t n_feat,
+                 pio_rf_forest** out) {
+  if (!p || !out) return fail(nullptr, PIO_ALS_ERR_ARG, "bad pio_rf_train arguments");
+  *out = nullptr;
+  const int rc = rf_check(p, label, x, n, n_feat);
+  if (rc != PIO_ALS_OK) return rc;
+  g_rf_timing = RfTiming();
+  RfTiming& tm = g_rf_timing;
+  auto t0 = std::chrono::steady_clock::now();
+  CK0(cudaSetDevice(device));
+  int sm = 0;
+  CK0(cudaDeviceGetAttribute(&sm, cudaDevAttrMultiProcessorCount, device));
+  std::vector<uint8_t> hcls((size_t)n);
+  for (int64_t r = 0; r < n; ++r) hcls[r] = (uint8_t)(int)trunc(label[r]);
+  CallMem tmp;
+  cudaStream_t st;
+  CK0(tmp.stream(&st));
+  double* dx = nullptr;
+  uint8_t* dcls = nullptr;
+  CK0(tmp.device(&dx, (size_t)n * n_feat));
+  CK0(tmp.device(&dcls, (size_t)n));
+  rf_ms(t0);
+  CK0(cudaMemcpyAsync(dx, x, sizeof(double) * (size_t)n * n_feat, cudaMemcpyHostToDevice, st));
+  CK0(cudaMemcpyAsync(dcls, hcls.data(), (size_t)n, cudaMemcpyHostToDevice, st));
+  CK0(cudaStreamSynchronize(st));
+  tm.h2d = rf_ms(t0);
+  return rf_fit(p, dx, dcls, n, n_feat, sm, tmp, st, t0, out);
+}
+
 int pio_rf_forest_size(const pio_rf_forest* f, int32_t* n_trees, int64_t* n_nodes) {
   if (!f) return fail(nullptr, PIO_ALS_ERR_ARG, "null forest");
   if (n_trees) *n_trees = f->n_trees;
@@ -4943,46 +5047,20 @@ int pio_rf_forest_destroy(pio_rf_forest* f) {
 int pio_rf_predict(int device, int32_t n_trees, const int32_t* tree_off, int64_t n_nodes, const int32_t* feature,
                    const double* threshold, const int32_t* left, const int32_t* right, const int32_t* prediction,
                    int32_t num_classes, const double* x, int64_t n, int32_t n_feat, int32_t* out) {
-  if (!tree_off || !feature || !threshold || !left || !right || !prediction || !out || n_trees < 1 || n_nodes < 1 ||
-      n_nodes >= (1ll << 31) || num_classes < 1 || num_classes > RF_MAX_CLASSES || n_feat < 1 || n < 0 || (n > 0 && !x))
-    return fail(nullptr, PIO_ALS_ERR_ARG, "bad pio_rf_predict arguments");
-  // a walk must end: children come after their parent (preorder) and stay in their tree
-  for (int32_t t = 0; t < n_trees; ++t) {
-    const int64_t a = tree_off[t], b = t + 1 < n_trees ? tree_off[t + 1] : n_nodes;
-    if (a < 0 || a >= b || b > n_nodes) return fail(nullptr, PIO_ALS_ERR_ARG, "bad tree offsets");
-    for (int64_t i = a; i < b; ++i) {
-      if (prediction[i] < 0 || prediction[i] >= num_classes) return fail(nullptr, PIO_ALS_ERR_ARG, "bad prediction");
-      if (feature[i] >= n_feat) return fail(nullptr, PIO_ALS_ERR_ARG, "node %lld uses feature %d of %d", (long long)i,
-                                            feature[i], n_feat);
-      if (feature[i] >= 0 && (left[i] <= i || left[i] >= b || right[i] <= i || right[i] >= b))
-        return fail(nullptr, PIO_ALS_ERR_ARG, "bad children at node %lld", (long long)i);
-    }
-  }
+  if (!out || n < 0 || (n > 0 && !x)) return fail(nullptr, PIO_ALS_ERR_ARG, "bad pio_rf_predict arguments");
+  const RfFlat fl{n_trees, tree_off, n_nodes, feature, threshold, left, right, prediction, num_classes};
+  EVF(rf_check_flat(fl, n_feat));
   if (n == 0) return PIO_ALS_OK;
   CK0(cudaSetDevice(device));
   CallMem tmp;
   cudaStream_t st;
   CK0(tmp.stream(&st));
-  int *dto = nullptr, *df = nullptr, *dl = nullptr, *dr = nullptr, *dp = nullptr, *dout = nullptr;
-  double *dt = nullptr, *dx = nullptr;
-  CK0(tmp.device(&dto, (size_t)n_trees));
-  CK0(tmp.device(&df, (size_t)n_nodes));
-  CK0(tmp.device(&dl, (size_t)n_nodes));
-  CK0(tmp.device(&dr, (size_t)n_nodes));
-  CK0(tmp.device(&dp, (size_t)n_nodes));
-  CK0(tmp.device(&dt, (size_t)n_nodes));
+  int* dout = nullptr;
+  double* dx = nullptr;
   CK0(tmp.device(&dx, (size_t)n * n_feat));
   CK0(tmp.device(&dout, (size_t)n));
-  CK0(cudaMemcpyAsync(dto, tree_off, 4 * (size_t)n_trees, cudaMemcpyHostToDevice, st));
-  CK0(cudaMemcpyAsync(df, feature, 4 * (size_t)n_nodes, cudaMemcpyHostToDevice, st));
-  CK0(cudaMemcpyAsync(dl, left, 4 * (size_t)n_nodes, cudaMemcpyHostToDevice, st));
-  CK0(cudaMemcpyAsync(dr, right, 4 * (size_t)n_nodes, cudaMemcpyHostToDevice, st));
-  CK0(cudaMemcpyAsync(dp, prediction, 4 * (size_t)n_nodes, cudaMemcpyHostToDevice, st));
-  CK0(cudaMemcpyAsync(dt, threshold, 8 * (size_t)n_nodes, cudaMemcpyHostToDevice, st));
   CK0(cudaMemcpyAsync(dx, x, 8 * (size_t)n * n_feat, cudaMemcpyHostToDevice, st));
-  rf::predict_kernel<<<nblk(n, 128), 128, sizeof(int) * 128 * (size_t)num_classes, st>>>(
-      dto, n_trees, df, dt, dl, dr, dp, num_classes, dx, n, n_feat, dout);
-  CK0(cudaGetLastError());
+  EVF(rf_predict_device(tmp, st, fl, dx, n, n_feat, dout));
   CK0(cudaMemcpyAsync(out, dout, 4 * (size_t)n, cudaMemcpyDeviceToHost, st));
   CK0(cudaStreamSynchronize(st));
   return PIO_ALS_OK;
@@ -5062,12 +5140,6 @@ static int evf_read(const uint32_t* d, cudaStream_t st, uint32_t* out) {
   CK0(cudaStreamSynchronize(st));
   return PIO_ALS_OK;
 }
-
-#define EVF(call)                          \
-  do {                                     \
-    const int rc_ = (call);                \
-    if (rc_ != PIO_ALS_OK) return rc_;     \
-  } while (0)
 
 // Fold f's maps of one side (global ids 0 .. n_ids): loc (global -> local), l2g and their count.  flag: n + 1 entries.
 static int evf_side(pio_eval_folds* ef, int f, const int* e1, const int* e2, int n_ids, uint32_t* flag, int** loc,
@@ -5339,6 +5411,377 @@ int pio_eval_folds_destroy(pio_eval_folds* ef) {
   for (void* p : ef->mem) cudaFree(p);
   if (ef->st) cudaStreamDestroy(ef->st);
   delete ef;
+  return PIO_ALS_OK;
+}
+
+}  // extern "C"
+
+// ---- k-fold evaluation of the classification template (cls_folds.cuh; DESIGN.md 4.12) -----------------------------------
+struct pio_cls_folds {
+  struct Result {
+    int fold = 0;
+    long long m = 0;
+    double* pred = nullptr;   // [m] predicted label of every test row of the fold
+  };
+  int device = 0, k = 1, F = 1, C = 0;   // C: distinct labels of all rows
+  long long n = 0;
+  cudaStream_t st = nullptr;
+  double *label = nullptr, *x = nullptr;
+  int* cls = nullptr;                    // [n] index of the row's label among the distinct labels
+  std::vector<double> classes;           // the distinct labels, ascending
+  std::vector<int> fmin, fmax;           // per class: smallest / largest fold holding one of its rows
+  std::map<int32_t, Result> results;
+  int32_t next_result = 0;
+  std::vector<void*> mem;                // the object's device memory, results excepted
+};
+
+namespace pio {
+
+static long long clf_n_test(const pio_cls_folds* cf, int f) { return (cf->n + cf->k - 1 - f) / cf->k; }
+
+static int clf_fold(const pio_cls_folds* cf, int32_t fold, const char* what) {
+  if (!cf) return fail(nullptr, PIO_ALS_ERR_ARG, "%s: null object", what);
+  if (fold < 0 || fold >= cf->k)
+    return fail(nullptr, PIO_ALS_ERR_ARG, "%s: fold %d outside 0..%d", what, fold, cf->k - 1);
+  return PIO_ALS_OK;
+}
+
+// fold f's training classes: lmap[c] = index of class c among them (-1: every row of c tests in fold f); returns their
+// number
+static int clf_train_classes(const pio_cls_folds* cf, int f, std::vector<int>* lmap, std::vector<double>* labels) {
+  int nc = 0;
+  if (lmap) lmap->assign(cf->C, -1);
+  for (int c = 0; c < cf->C; ++c) {
+    if (cf->fmin[c] == f && cf->fmax[c] == f) continue;
+    if (lmap) (*lmap)[c] = nc;
+    if (labels) labels->push_back(cf->classes[c]);
+    ++nc;
+  }
+  return nc;
+}
+
+// grid of the grid-stride kernels: one thread per row up to 16 blocks per SM of an H100
+static unsigned clf_grid(long long n) { return (unsigned)std::max<long long>(1, std::min<long long>(nblk(n, clf::THREADS), 132 * 16)); }
+
+// the first training row of fold f failing check `mode` (cls_folds.cuh): its row, or -1 (none)
+static int clf_first_bad(pio_cls_folds* cf, int f, int mode, int num_classes, CallMem& tmp, long long* row) {
+  unsigned long long* d = nullptr;
+  CK0(tmp.device(&d, 1));
+  const unsigned long long none = (unsigned long long)cf->n;
+  CK0(cudaMemcpyAsync(d, &none, 8, cudaMemcpyHostToDevice, cf->st));
+  clf::first_bad_kernel<<<clf_grid(cf->n), clf::THREADS, 0, cf->st>>>(cf->label, cf->x, cf->n, cf->F, cf->k, f, mode,
+                                                                      num_classes, d);
+  CK0(cudaGetLastError());
+  unsigned long long e = 0;
+  CK0(cudaMemcpyAsync(&e, d, 8, cudaMemcpyDeviceToHost, cf->st));
+  CK0(cudaStreamSynchronize(cf->st));
+  *row = e == none ? -1 : (long long)e;
+  return PIO_ALS_OK;
+}
+
+// label and features of row e, to the host
+static int clf_row(const pio_cls_folds* cf, long long e, double* label, std::vector<double>* xr) {
+  xr->resize(cf->F);
+  CK0(cudaMemcpyAsync(label, cf->label + e, 8, cudaMemcpyDeviceToHost, cf->st));
+  CK0(cudaMemcpyAsync(xr->data(), cf->x + e * cf->F, 8 * (size_t)cf->F, cudaMemcpyDeviceToHost, cf->st));
+  CK0(cudaStreamSynchronize(cf->st));
+  return PIO_ALS_OK;
+}
+
+static long long clf_train_pos(const pio_cls_folds* cf, long long e, int f) { return e - (e + cf->k - 1 - f) / cf->k; }
+
+// Uploads the rows and encodes the labels: distinct labels, each row's class, each class's fold range.
+static int clf_build(pio_cls_folds* cf, const double* label, const double* x) {
+  const cudaStream_t st = cf->st;
+  const long long n = cf->n;
+  for (double** p : {&cf->label, &cf->x}) {
+    const size_t cnt = p == &cf->label ? (size_t)n : (size_t)n * cf->F;
+    CK0(cudaMalloc((void**)p, 8 * cnt));
+    cf->mem.push_back(*p);
+  }
+  CK0(cudaMalloc((void**)&cf->cls, 4 * (size_t)n));
+  cf->mem.push_back(cf->cls);
+  CK0(cudaMemcpyAsync(cf->label, label, 8 * (size_t)n, cudaMemcpyHostToDevice, st));
+  CK0(cudaMemcpyAsync(cf->x, x, 8 * (size_t)n * cf->F, cudaMemcpyHostToDevice, st));
+  CallMem tmp(st);
+  SortBufs sb;
+  uint32_t *head = nullptr, *pos = nullptr;
+  uint64_t* ukey = nullptr;
+  for (int i : {0, 1}) {
+    CK0(tmp.device(&sb.k[i], (size_t)n));
+    CK0(tmp.device(&sb.v[i], (size_t)n));
+  }
+  CK0(tmp.device(&head, (size_t)n));
+  CK0(tmp.device(&pos, (size_t)n));
+  CK0(tmp.device(&ukey, (size_t)n));
+  clf::label_keys_kernel<<<nblk(n, 256), 256, 0, st>>>(cf->label, n, sb.keys(), sb.vals());
+  CK0(radix_sort_pairs(sb, (size_t)n, 64, st, nullptr));
+  rf::run_head_kernel<<<nblk(n, 256), 256, 0, st>>>(sb.keys(), n, head);
+  CK0(scan_exclusive_u32(head, pos, (size_t)n, st, nullptr));
+  clf::class_index_kernel<<<nblk(n, 256), 256, 0, st>>>(sb.keys(), sb.vals(), head, pos, n, cf->cls, ukey);
+  CK0(cudaGetLastError());
+  uint32_t lh = 0, lp = 0;
+  CK0(cudaMemcpyAsync(&lh, head + n - 1, 4, cudaMemcpyDeviceToHost, st));
+  CK0(cudaMemcpyAsync(&lp, pos + n - 1, 4, cudaMemcpyDeviceToHost, st));
+  CK0(cudaStreamSynchronize(st));
+  cf->C = (int)(lp + lh);
+  std::vector<uint64_t> hk(cf->C);
+  CK0(cudaMemcpyAsync(hk.data(), ukey, 8 * (size_t)cf->C, cudaMemcpyDeviceToHost, st));
+  int *dmin = nullptr, *dmax = nullptr;
+  CK0(tmp.device(&dmin, (size_t)cf->C));
+  CK0(tmp.device(&dmax, (size_t)cf->C));
+  cf->fmin.assign(cf->C, cf->k);
+  cf->fmax.assign(cf->C, -1);
+  CK0(cudaMemcpyAsync(dmin, cf->fmin.data(), 4 * (size_t)cf->C, cudaMemcpyHostToDevice, st));
+  CK0(cudaMemcpyAsync(dmax, cf->fmax.data(), 4 * (size_t)cf->C, cudaMemcpyHostToDevice, st));
+  clf::class_folds_kernel<<<clf_grid(n), clf::THREADS, 0, st>>>(cf->cls, n, cf->k, dmin, dmax);
+  CK0(cudaGetLastError());
+  CK0(cudaMemcpyAsync(cf->fmin.data(), dmin, 4 * (size_t)cf->C, cudaMemcpyDeviceToHost, st));
+  CK0(cudaMemcpyAsync(cf->fmax.data(), dmax, 4 * (size_t)cf->C, cudaMemcpyDeviceToHost, st));
+  CK0(cudaStreamSynchronize(st));
+  cf->classes.resize(cf->C);
+  for (int c = 0; c < cf->C; ++c) {
+    const uint64_t b = (hk[c] >> 63) ? (hk[c] & ~(1ull << 63)) : ~hk[c];
+    memcpy(&cf->classes[c], &b, 8);
+    if (!isfinite(cf->classes[c]))
+      return fail(nullptr, PIO_ALS_ERR_ARG, "pio_cls_folds_create: labels must be finite (%s)", rf_fmt(cf->classes[c]).c_str());
+  }
+  return PIO_ALS_OK;
+}
+
+// keeps the predicted labels of fold f's m test rows, class_label[idx] with idx on the device; *out_result names them
+static int clf_keep_result(pio_cls_folds* cf, int f, long long m, CallMem& tmp, const int* didx, const double* class_label,
+                           int n_labels, int32_t* out_result) {
+  double* dlab = nullptr;
+  CK0(tmp.device(&dlab, (size_t)n_labels));
+  CK0(cudaMemcpyAsync(dlab, class_label, 8 * (size_t)n_labels, cudaMemcpyHostToDevice, cf->st));
+  pio_cls_folds::Result R;
+  R.fold = f, R.m = m;
+  CK0(cudaMalloc((void**)&R.pred, 8 * (size_t)(m ? m : 1)));
+  if (m > 0) clf::pred_label_kernel<<<nblk(m, 256), 256, 0, cf->st>>>(didx, m, dlab, R.pred);
+  const cudaError_t e0 = cudaGetLastError(), e1 = cudaStreamSynchronize(cf->st);
+  if (e0 != cudaSuccess || e1 != cudaSuccess) {
+    cudaFree(R.pred);
+    return fail(nullptr, PIO_ALS_ERR_CUDA, "predicted labels: %s", cudaGetErrorString(e0 != cudaSuccess ? e0 : e1));
+  }
+  *out_result = cf->next_result++;
+  cf->results[*out_result] = R;
+  return PIO_ALS_OK;
+}
+
+}  // namespace pio
+
+extern "C" {
+
+int pio_cls_folds_create(int device, const double* label, const double* x, int64_t n, int32_t n_feat, int32_t k_fold,
+                         pio_cls_folds** out) {
+  if (!out) return fail(nullptr, PIO_ALS_ERR_ARG, "bad pio_cls_folds_create arguments");
+  *out = nullptr;
+  if (!label || !x || n < 1 || n_feat < 1 || k_fold < 1)
+    return fail(nullptr, PIO_ALS_ERR_ARG, "bad pio_cls_folds_create arguments (n >= 1, n_feat >= 1 and k_fold >= 1)");
+  if (n >= (1ll << 31)) return fail(nullptr, PIO_ALS_ERR_ARG, "n must be < 2^31");
+  CK0(cudaSetDevice(device));
+  auto* cf = new pio_cls_folds;
+  cf->device = device, cf->k = k_fold, cf->F = n_feat, cf->n = n;
+  const cudaError_t e = cudaStreamCreateWithFlags(&cf->st, cudaStreamNonBlocking);
+  if (e != cudaSuccess) {
+    delete cf;
+    return fail(nullptr, PIO_ALS_ERR_CUDA, "cudaStreamCreate: %s", cudaGetErrorString(e));
+  }
+  const int rc = clf_build(cf, label, x);
+  if (rc != PIO_ALS_OK) {
+    pio_cls_folds_destroy(cf);
+    return rc;
+  }
+  *out = cf;
+  return PIO_ALS_OK;
+}
+
+int pio_cls_folds_sizes(const pio_cls_folds* cf, int32_t fold, int64_t out[2]) {
+  EVF(clf_fold(cf, fold, "pio_cls_folds_sizes"));
+  if (!out) return fail(nullptr, PIO_ALS_ERR_ARG, "pio_cls_folds_sizes: null out");
+  const long long m = clf_n_test(cf, fold);
+  out[0] = cf->n - m, out[1] = m;
+  return PIO_ALS_OK;
+}
+
+int pio_cls_folds_classes(const pio_cls_folds* cf, int32_t fold, int32_t* n_class, double* labels) {
+  EVF(clf_fold(cf, fold, "pio_cls_folds_classes"));
+  if (!n_class) return fail(nullptr, PIO_ALS_ERR_ARG, "pio_cls_folds_classes: null n_class");
+  std::vector<double> v;
+  *n_class = clf_train_classes(cf, fold, nullptr, &v);
+  if (labels && !v.empty()) memcpy(labels, v.data(), 8 * v.size());
+  return PIO_ALS_OK;
+}
+
+int pio_cls_folds_nb_train(pio_cls_folds* cf, int32_t fold, double lambda, int32_t n_class, double* pi, double* theta) {
+  EVF(clf_fold(cf, fold, "pio_cls_folds_nb_train"));
+  std::vector<int> lmap;
+  const int nc = clf_train_classes(cf, fold, &lmap, nullptr);
+  if (!pi || !theta || n_class != nc)
+    return fail(nullptr, PIO_ALS_ERR_ARG, "bad pio_cls_folds_nb_train arguments (fold %d has %d training classes)", fold,
+                nc);
+  const long long nt = cf->n - clf_n_test(cf, fold);
+  if (nt == 0) return fail(nullptr, PIO_ALS_ERR_ARG, "fold %d has no training rows", fold);
+  EVF(nb_check_width(cf->F, nc));
+  CK0(cudaSetDevice(cf->device));
+  CallMem tmp(cf->st);
+  long long bad = -1;
+  EVF(clf_first_bad(cf, fold, clf::CHECK_NEG_F32, 0, tmp, &bad));
+  if (bad >= 0) return fail(nullptr, PIO_ALS_ERR_NUMERIC, "Naive Bayes requires nonnegative feature values");
+  int *dmap = nullptr, *dl = nullptr;
+  float* dx = nullptr;
+  CK0(tmp.device(&dmap, (size_t)cf->C));
+  CK0(tmp.device(&dl, (size_t)nt));
+  CK0(tmp.device(&dx, (size_t)nt * cf->F));
+  CK0(cudaMemcpyAsync(dmap, lmap.data(), 4 * (size_t)cf->C, cudaMemcpyHostToDevice, cf->st));
+  clf::nb_gather_kernel<<<clf_grid(cf->n), clf::THREADS, 0, cf->st>>>(cf->cls, cf->x, cf->n, cf->F, cf->k, fold, dmap,
+                                                                     dl, dx);
+  CK0(cudaGetLastError());
+  return nb_fit(tmp, cf->st, dl, dx, nt, cf->F, nc, lambda, pi, theta);
+}
+
+int pio_cls_folds_rf_train(pio_cls_folds* cf, int32_t fold, const pio_rf_params* p, pio_rf_forest** out) {
+  EVF(clf_fold(cf, fold, "pio_cls_folds_rf_train"));
+  if (!p || !out) return fail(nullptr, PIO_ALS_ERR_ARG, "bad pio_cls_folds_rf_train arguments");
+  *out = nullptr;
+  const long long nt = cf->n - clf_n_test(cf, fold);
+  EVF(rf_check_params(p, nt, cf->F));
+  CK0(cudaSetDevice(cf->device));
+  {
+    CallMem chk(cf->st);
+    for (int mode : {clf::CHECK_FINITE, clf::CHECK_LABEL}) {
+      long long e = -1;
+      EVF(clf_first_bad(cf, fold, mode, p->num_classes, chk, &e));
+      if (e < 0) continue;
+      double lab = 0;
+      std::vector<double> xr;
+      EVF(clf_row(cf, e, &lab, &xr));
+      EVF(mode == clf::CHECK_FINITE ? rf_fail_finite(clf_train_pos(cf, e, fold), lab, xr.data(), cf->F)
+                                    : rf_fail_label(p, lab));
+    }
+  }
+  g_rf_timing = RfTiming();
+  RfTiming& tm = g_rf_timing;
+  auto t0 = std::chrono::steady_clock::now();
+  int sm = 0;
+  CK0(cudaDeviceGetAttribute(&sm, cudaDevAttrMultiProcessorCount, cf->device));
+  CallMem tmp;
+  cudaStream_t st;
+  CK0(tmp.stream(&st));
+  double* dx = nullptr;
+  uint8_t* dcls = nullptr;
+  CK0(tmp.device(&dx, (size_t)nt * cf->F));
+  CK0(tmp.device(&dcls, (size_t)nt));
+  rf_ms(t0);
+  clf::rf_gather_kernel<<<clf_grid(cf->n), clf::THREADS, 0, st>>>(cf->label, cf->x, cf->n, cf->F, cf->k, fold, dcls, dx);
+  CK0(cudaGetLastError());
+  CK0(cudaStreamSynchronize(st));
+  tm.h2d = rf_ms(t0);   // the gather stands where pio_rf_train copies the rows in
+  return rf_fit(p, dx, dcls, nt, cf->F, sm, tmp, st, t0, out);
+}
+
+int pio_cls_folds_nb_predict(pio_cls_folds* cf, int32_t fold, int32_t n_class, const double* pi, const double* theta,
+                             const double* class_label, int32_t* out_result) {
+  EVF(clf_fold(cf, fold, "pio_cls_folds_nb_predict"));
+  if (!pi || !theta || !class_label || !out_result || n_class < 1)
+    return fail(nullptr, PIO_ALS_ERR_ARG, "bad pio_cls_folds_nb_predict arguments");
+  CK0(cudaSetDevice(cf->device));
+  const long long m = clf_n_test(cf, fold);
+  CallMem tmp(cf->st);
+  int* didx = nullptr;
+  CK0(tmp.device(&didx, (size_t)m));
+  if (m > 0) {
+    float* dx = nullptr;
+    double *dpi = nullptr, *dth = nullptr;
+    CK0(tmp.device(&dx, (size_t)m * cf->F));
+    CK0(tmp.device(&dpi, (size_t)n_class));
+    CK0(tmp.device(&dth, (size_t)n_class * cf->F));
+    CK0(cudaMemcpyAsync(dpi, pi, 8 * (size_t)n_class, cudaMemcpyHostToDevice, cf->st));
+    CK0(cudaMemcpyAsync(dth, theta, 8 * (size_t)n_class * cf->F, cudaMemcpyHostToDevice, cf->st));
+    clf::test_gather_kernel<float><<<nblk(m, 256), 256, 0, cf->st>>>(cf->x, cf->F, cf->k, fold, m, dx);
+    nb_predict_kernel<<<nblk(m, 256), 256, 0, cf->st>>>(dx, m, cf->F, n_class, dpi, dth, didx);
+    CK0(cudaGetLastError());
+  }
+  return clf_keep_result(cf, fold, m, tmp, didx, class_label, n_class, out_result);
+}
+
+int pio_cls_folds_rf_predict(pio_cls_folds* cf, int32_t fold, int32_t n_trees, const int32_t* tree_off, int64_t n_nodes,
+                             const int32_t* feature, const double* threshold, const int32_t* left, const int32_t* right,
+                             const int32_t* prediction, int32_t num_classes, int32_t* out_result) {
+  EVF(clf_fold(cf, fold, "pio_cls_folds_rf_predict"));
+  if (!out_result) return fail(nullptr, PIO_ALS_ERR_ARG, "bad pio_cls_folds_rf_predict arguments");
+  const RfFlat fl{n_trees, tree_off, n_nodes, feature, threshold, left, right, prediction, num_classes};
+  EVF(rf_check_flat(fl, cf->F));
+  CK0(cudaSetDevice(cf->device));
+  const long long m = clf_n_test(cf, fold);
+  CallMem tmp(cf->st);
+  int* didx = nullptr;
+  CK0(tmp.device(&didx, (size_t)m));
+  if (m > 0) {
+    double* dx = nullptr;
+    CK0(tmp.device(&dx, (size_t)m * cf->F));
+    clf::test_gather_kernel<double><<<nblk(m, 256), 256, 0, cf->st>>>(cf->x, cf->F, cf->k, fold, m, dx);
+    CK0(cudaGetLastError());
+    EVF(rf_predict_device(tmp, cf->st, fl, dx, m, cf->F, didx));
+  }
+  std::vector<double> cl(num_classes);   // the forest predicts the class index as its label
+  for (int c = 0; c < num_classes; ++c) cl[c] = c;
+  return clf_keep_result(cf, fold, m, tmp, didx, cl.data(), num_classes, out_result);
+}
+
+int pio_cls_folds_result_labels(const pio_cls_folds* cf, int32_t result, double* out) {
+  if (!cf) return fail(nullptr, PIO_ALS_ERR_ARG, "pio_cls_folds_result_labels: null object");
+  auto it = cf->results.find(result);
+  if (it == cf->results.end()) return fail(nullptr, PIO_ALS_ERR_ARG, "no result %d", result);
+  const pio_cls_folds::Result& R = it->second;
+  if (R.m == 0) return PIO_ALS_OK;
+  if (!out) return fail(nullptr, PIO_ALS_ERR_ARG, "pio_cls_folds_result_labels: null out");
+  CK0(cudaSetDevice(cf->device));
+  CK0(cudaMemcpyAsync(out, R.pred, 8 * (size_t)R.m, cudaMemcpyDeviceToHost, cf->st));
+  CK0(cudaStreamSynchronize(cf->st));
+  return PIO_ALS_OK;
+}
+
+int pio_cls_folds_result_counts(const pio_cls_folds* cf, int32_t result, double label, int64_t out[4]) {
+  if (!cf || !out) return fail(nullptr, PIO_ALS_ERR_ARG, "bad pio_cls_folds_result_counts arguments");
+  auto it = cf->results.find(result);
+  if (it == cf->results.end()) return fail(nullptr, PIO_ALS_ERR_ARG, "no result %d", result);
+  const pio_cls_folds::Result& R = it->second;
+  unsigned long long h[3] = {0, 0, 0};
+  if (R.m > 0) {
+    CK0(cudaSetDevice(cf->device));
+    CallMem tmp(cf->st);
+    unsigned long long* d = nullptr;
+    CK0(tmp.device(&d, 3));
+    CK0(cudaMemsetAsync(d, 0, 3 * 8, cf->st));
+    clf::counts_kernel<<<clf_grid(R.m), clf::THREADS, 0, cf->st>>>(R.pred, cf->label, R.m, cf->k, R.fold, label, d);
+    CK0(cudaGetLastError());
+    CK0(cudaMemcpyAsync(h, d, 3 * 8, cudaMemcpyDeviceToHost, cf->st));
+    CK0(cudaStreamSynchronize(cf->st));
+  }
+  out[0] = R.m, out[1] = (int64_t)h[0], out[2] = (int64_t)h[1], out[3] = (int64_t)h[2];
+  return PIO_ALS_OK;
+}
+
+int pio_cls_folds_result_free(pio_cls_folds* cf, int32_t result) {
+  if (!cf) return fail(nullptr, PIO_ALS_ERR_ARG, "pio_cls_folds_result_free: null object");
+  auto it = cf->results.find(result);
+  if (it == cf->results.end()) return fail(nullptr, PIO_ALS_ERR_ARG, "no result %d", result);
+  cudaSetDevice(cf->device);
+  cudaFree(it->second.pred);
+  cf->results.erase(it);
+  return PIO_ALS_OK;
+}
+
+int pio_cls_folds_destroy(pio_cls_folds* cf) {
+  if (!cf) return PIO_ALS_OK;
+  cudaSetDevice(cf->device);
+  if (cf->st) cudaStreamSynchronize(cf->st);
+  for (auto& kv : cf->results) cudaFree(kv.second.pred);
+  for (void* p : cf->mem) cudaFree(p);
+  if (cf->st) cudaStreamDestroy(cf->st);
+  delete cf;
   return PIO_ALS_OK;
 }
 

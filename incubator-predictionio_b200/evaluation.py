@@ -9,8 +9,12 @@ trainings); the metric arithmetic itself is host-side bookkeeping.
 """
 from __future__ import annotations
 
+import dataclasses
+import datetime as _dt
+import json
 import math
 from dataclasses import dataclass
+from pathlib import Path
 from typing import Any, List, Optional, Sequence, Tuple
 
 
@@ -113,17 +117,53 @@ def _calculate(metric, sc, ds):
     return metric.calculate_columns(sc, ds) if isinstance(ds, EvalColumns) else metric.calculate(sc, ds)
 
 
-class MetricEvaluator:
-    def __init__(self, metric: Metric, otherMetrics: Sequence[Metric] = ()):
-        self.metric, self.otherMetrics = metric, list(otherMetrics)
+def _params_json(p) -> Any:
+    """A Params value as engine.json holds it: dataclass fields under their JSON names (`lambda_` -> `lambda`)."""
+    if dataclasses.is_dataclass(p) and not isinstance(p, type):
+        return {f.metadata.get("json", f.name): _params_json(getattr(p, f.name)) for f in dataclasses.fields(p)}
+    if isinstance(p, (set, frozenset)):
+        return sorted(_params_json(v) for v in p)
+    if isinstance(p, (list, tuple)):
+        return [_params_json(v) for v in p]
+    return p
 
-    def evaluateBase(self, sc, engineEvalDataSet) -> MetricEvaluatorResult:
+
+def _qualified_name(obj) -> str:
+    cls = obj if isinstance(obj, type) else type(obj)
+    return f"{cls.__module__}.{cls.__qualname__}"
+
+
+class MetricEvaluator:
+    """outputPath: where evaluateBase writes the best engine params as an engine variant (saveEngineJson), which
+    `CreateWorkflow.main --engine-variant` then trains."""
+
+    def __init__(self, metric: Metric, otherMetrics: Sequence[Metric] = (), outputPath: Optional[str] = None):
+        self.metric, self.otherMetrics, self.outputPath = metric, list(otherMetrics), outputPath
+
+    def saveEngineJson(self, evaluation, engineParams, outputPath: str) -> None:
+        """MetricEvaluator.scala saveEngineJson: the engine params as an engine variant whose engineFactory is the
+        evaluation's qualified class name (workflow.get_engine resolves it to the evaluation's engine)."""
+        name = _qualified_name(evaluation)
+
+        def named(np_):
+            return {"name": np_[0], "params": _params_json(np_[1])}
+
+        variant = {"id": f"{name} {_dt.datetime.now(_dt.timezone.utc).isoformat()}", "description": "",
+                   "engineFactory": name, "datasource": named(engineParams.dataSourceParams),
+                   "preparator": named(engineParams.preparatorParams),
+                   "algorithms": [named(a) for a in engineParams.algorithmParamsList],
+                   "serving": named(engineParams.servingParams)}
+        Path(outputPath).write_text(json.dumps(variant, indent=2))
+
+    def evaluateBase(self, sc, engineEvalDataSet, evaluation=None) -> MetricEvaluatorResult:
         results = [(ep, MetricScores(_calculate(self.metric, sc, ds), [_calculate(m, sc, ds) for m in self.otherMetrics]))
                    for ep, ds in engineEvalDataSet]
         best = 0
         for i in range(1, len(results)):   # reduce { (x, y) => if (compare(x, y) >= 0) x else y }: first maximum wins
             if self.metric.compare(results[best][1].score, results[i][1].score) < 0:
                 best = i
+        if self.outputPath is not None and evaluation is not None:
+            self.saveEngineJson(evaluation, results[best][0], self.outputPath)
         return MetricEvaluatorResult(results[best][1], results[best][0], best, self.metric.header,
                                      [m.header for m in self.otherMetrics], results)
 
@@ -158,7 +198,7 @@ def run_evaluation(evaluation: Evaluation, generator: EngineParamsGenerator, sc=
         if folds is None:
             folds = engine.eval(sc, ep)                  # [(evalInfo, [(q, p, a), ...]), ...] -- one training per fold
         data.append((ep, folds))
-    return evaluation.evaluator.evaluateBase(sc, data)
+    return evaluation.evaluator.evaluateBase(sc, data, evaluation)
 
 
 def _columnar(engine, ep, evaluator, sc) -> bool:

@@ -202,6 +202,20 @@ class NaiveBayes:
         pi, theta = native.nb_train(idx.astype(np.int32), x, classes.shape[0], lambda_, device)
         return NaiveBayesModel(classes, pi, theta, device)
 
+    @staticmethod
+    def trainFold(folds: native.ClsFolds, fold: int, lambda_: float = 1.0) -> NaiveBayesModel:
+        """train on the training rows of one fold of a native.ClsFolds, without them leaving the device: the same model
+        as train(labels[rows], features[rows].astype(float32), lambda_), and the same ValueError for a negative
+        feature."""
+        classes = folds.classes(fold)
+        try:
+            pi, theta = folds.nb_train(fold, lambda_, classes.shape[0])
+        except native.NativeError as e:
+            if e.code != native.ERR_NUMERIC:
+                raise
+            raise ValueError(native.lib().pio_als_last_error(None).decode()) from None
+        return NaiveBayesModel(classes, pi, theta, folds.device)
+
 
 class RandomForestModel:
     """A trained classification forest as flat per-node numpy arrays (native.rf_train's dict), so that a pickle of the
@@ -254,13 +268,29 @@ class RandomForest:
         """MLlib's 8-argument RandomForest.trainClassifier (continuous features only) plus an explicit seed; the rules are
         those of tests/forest_ref.py.  labels: n float labels (class = trunc(label)); features: n x F, trained in fp64.
         Bad arguments and labels raise ValueError with MLlib's messages before any device work."""
+        return RandomForest._train(lambda imp: native.rf_train(labels, features, numClasses, numTrees,
+                                                               featureSubsetStrategy, imp, maxDepth, maxBins, seed,
+                                                               device),
+                                   numClasses, categoricalFeaturesInfo, impurity, device)
+
+    @staticmethod
+    def trainClassifierFold(folds: native.ClsFolds, fold: int, numClasses: int, categoricalFeaturesInfo, numTrees: int,
+                            featureSubsetStrategy: str, impurity: str, maxDepth: int, maxBins: int,
+                            seed: int = 0) -> RandomForestModel:
+        """trainClassifier on the training rows of one fold of a native.ClsFolds, without them leaving the device: the
+        same forest, node for node, and the same ValueErrors (a row number counts the fold's training rows)."""
+        return RandomForest._train(lambda imp: folds.rf_train(fold, numClasses, numTrees, featureSubsetStrategy, imp,
+                                                              maxDepth, maxBins, seed),
+                                   numClasses, categoricalFeaturesInfo, impurity, folds.device)
+
+    @staticmethod
+    def _train(fit, numClasses, categoricalFeaturesInfo, impurity, device) -> RandomForestModel:
         if impurity not in RandomForest.IMPURITIES:
             raise ValueError(f"Did not recognize Impurity name: {impurity}")
         if categoricalFeaturesInfo:
             raise ValueError("categoricalFeaturesInfo must be empty: categorical features are not supported")
         try:
-            nodes = native.rf_train(labels, features, numClasses, numTrees, featureSubsetStrategy,
-                                    RandomForest.IMPURITIES[impurity], maxDepth, maxBins, seed, device)
+            nodes = fit(RandomForest.IMPURITIES[impurity])
         except native.NativeError as e:
             if e.code != native.ERR_ARG:
                 raise

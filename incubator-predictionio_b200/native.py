@@ -39,7 +39,10 @@ EXPORTED_SYMBOLS = [
     "pio_events_index_destroy", "pio_rf_train", "pio_rf_forest_size", "pio_rf_forest_get", "pio_rf_forest_destroy",
     "pio_rf_predict", "pio_eval_folds_create", "pio_eval_folds_sizes", "pio_eval_folds_maps",
     "pio_eval_folds_set_ratings", "pio_eval_folds_result_add", "pio_eval_folds_result_free",
-    "pio_eval_folds_rank_counts", "pio_eval_folds_destroy",
+    "pio_eval_folds_rank_counts", "pio_eval_folds_destroy", "pio_cls_folds_create", "pio_cls_folds_sizes",
+    "pio_cls_folds_classes", "pio_cls_folds_nb_train", "pio_cls_folds_rf_train", "pio_cls_folds_nb_predict",
+    "pio_cls_folds_rf_predict", "pio_cls_folds_result_labels", "pio_cls_folds_result_counts",
+    "pio_cls_folds_result_free", "pio_cls_folds_destroy",
 ]
 
 
@@ -579,6 +582,114 @@ class EvalResult:
             pass
 
 
+class ClsFolds:
+    """pio_cls_folds: the k-fold split of n labeled points on the device (row i tests in fold i % k_fold and trains in
+    every other fold, in row order), from fp64 labels and n x n_feat fp64 features.  Folds train NaiveBayes / RandomForest
+    and predict their test rows without their rows leaving the device.  The device memory goes with this object;
+    ClsResult objects keep it alive."""
+
+    def __init__(self, label, x, k_fold: int, device: int = 0):
+        self._h = C.c_void_p()
+        label = np.ascontiguousarray(label, np.float64)
+        x = np.ascontiguousarray(x, np.float64)
+        if x.ndim != 2 or label.shape != (x.shape[0],):
+            raise ValueError("x must be n x n_feat and label must have n entries")
+        self.k_fold, self.device, self.n_feat = int(k_fold), int(device), int(x.shape[1])
+        _check(lib().pio_cls_folds_create(C.c_int(device), _ptr(label, C.c_double), _ptr(x, C.c_double),
+                                          C.c_int64(x.shape[0]), C.c_int32(x.shape[1]), C.c_int32(k_fold),
+                                          C.byref(self._h)))
+
+    def close(self):
+        if self._h:
+            lib().pio_cls_folds_destroy(self._h)
+            self._h = C.c_void_p()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    def sizes(self, fold: int) -> tuple:
+        """(training rows, test rows) of fold `fold`."""
+        out = np.zeros(2, np.int64)
+        _check(lib().pio_cls_folds_sizes(self._h, C.c_int32(fold), _ptr(out, C.c_int64)))
+        return int(out[0]), int(out[1])
+
+    def classes(self, fold: int) -> np.ndarray:
+        """The distinct labels of the fold's training rows, ascending."""
+        nc = C.c_int32(0)
+        _check(lib().pio_cls_folds_classes(self._h, C.c_int32(fold), C.byref(nc), None))
+        out = np.empty(nc.value, np.float64)
+        _check(lib().pio_cls_folds_classes(self._h, C.c_int32(fold), C.byref(nc), _ptr(out, C.c_double)))
+        return out
+
+    def nb_train(self, fold: int, lam: float, n_class: int):
+        """(pi, theta) of NaiveBayes on the fold's training rows; n_class = len(classes(fold))."""
+        pi = np.zeros(n_class, np.float64)
+        theta = np.zeros((n_class, self.n_feat), np.float64)
+        _check(lib().pio_cls_folds_nb_train(self._h, C.c_int32(fold), C.c_double(lam), C.c_int32(n_class),
+                                            _ptr(pi, C.c_double), _ptr(theta, C.c_double)))
+        return pi, theta
+
+    def rf_train(self, fold: int, num_classes, num_trees, strategy, impurity, max_depth, max_bins, seed=0) -> dict:
+        """rf_train on the fold's training rows: the forest as rf_train's dict of flat per-node arrays."""
+        p = _rf_params(num_classes, num_trees, strategy, impurity, max_depth, max_bins, seed)
+        h = C.c_void_p()
+        _check(lib().pio_cls_folds_rf_train(self._h, C.c_int32(fold), C.byref(p), C.byref(h)))
+        return _rf_forest_take(h)
+
+    def nb_predict(self, fold: int, pi, theta, class_label) -> "ClsResult":
+        """The NaiveBayes model's predicted labels (class_label[class]) of the fold's test rows, kept on the device."""
+        pi = np.ascontiguousarray(pi, np.float64)
+        theta = np.ascontiguousarray(theta, np.float64)
+        class_label = np.ascontiguousarray(class_label, np.float64)
+        if theta.shape != (pi.shape[0], self.n_feat) or class_label.shape != pi.shape:
+            raise ValueError("theta must be n_class x n_feat and class_label must have n_class entries")
+        rid = C.c_int32(-1)
+        _check(lib().pio_cls_folds_nb_predict(self._h, C.c_int32(fold), C.c_int32(pi.shape[0]), _ptr(pi, C.c_double),
+                                              _ptr(theta, C.c_double), _ptr(class_label, C.c_double), C.byref(rid)))
+        return ClsResult(self, fold, rid.value)
+
+    def rf_predict(self, fold: int, forest: dict, num_classes: int) -> "ClsResult":
+        """The forest's predicted labels (class index) of the fold's test rows, kept on the device."""
+        args, _arrays = _rf_flat(forest, num_classes)
+        rid = C.c_int32(-1)
+        _check(lib().pio_cls_folds_rf_predict(self._h, C.c_int32(fold), *args, C.byref(rid)))
+        return ClsResult(self, fold, rid.value)
+
+
+class ClsResult:
+    """The predicted labels of one fold's test rows, kept on the device by its ClsFolds (which it keeps alive)."""
+
+    def __init__(self, folds: ClsFolds, fold: int, rid: int):
+        self.folds, self.fold, self._rid = folds, fold, rid
+        self.n_rows = folds.sizes(fold)[1]
+
+    def labels(self) -> np.ndarray:
+        out = np.empty(self.n_rows, np.float64)
+        _check(lib().pio_cls_folds_result_labels(self.folds._h, C.c_int32(self._rid), _ptr(out, C.c_double)))
+        return out
+
+    def counts(self, label: float = 0.0) -> tuple:
+        """(test rows, rows predicted correctly, rows predicted as `label`, those of them that are correct)."""
+        out = np.zeros(4, np.int64)
+        _check(lib().pio_cls_folds_result_counts(self.folds._h, C.c_int32(self._rid), C.c_double(label),
+                                                 _ptr(out, C.c_int64)))
+        return tuple(int(v) for v in out)
+
+    def close(self):
+        if self._rid is not None and self.folds._h:
+            lib().pio_cls_folds_result_free(self.folds._h, C.c_int32(self._rid))
+        self._rid = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+
 EVENTS_TARGET_ANY, EVENTS_TARGET_ABSENT, EVENTS_TARGET_EQUALS = 0, 1, 2
 EVENTS_MIN_EVENT_BYTES = 64
 EVENTS_HAS_VALUE, EVENTS_HAS_TARGET = 1, 2
@@ -920,12 +1031,21 @@ def rf_train(label, x, num_classes, num_trees, strategy, impurity, max_depth, ma
     x = np.ascontiguousarray(x, np.float64)
     if x.ndim != 2 or label.shape != (x.shape[0],):
         raise ValueError("x must be n x n_feat and label must have n entries")
-    p = RfParams(num_classes=int(num_classes), num_trees=int(num_trees), max_depth=int(max_depth),
-                 max_bins=int(max_bins), impurity=int(impurity), feature_subset_strategy=str(strategy).encode("utf-8"),
-                 seed=int(seed))
+    p = _rf_params(num_classes, num_trees, strategy, impurity, max_depth, max_bins, seed)
     h = C.c_void_p()
     _check(lib().pio_rf_train(C.c_int(device), C.byref(p), _ptr(label, C.c_double), _ptr(x, C.c_double),
                               C.c_int64(x.shape[0]), C.c_int32(x.shape[1]), C.byref(h)))
+    return _rf_forest_take(h)
+
+
+def _rf_params(num_classes, num_trees, strategy, impurity, max_depth, max_bins, seed) -> RfParams:
+    return RfParams(num_classes=int(num_classes), num_trees=int(num_trees), max_depth=int(max_depth),
+                    max_bins=int(max_bins), impurity=int(impurity), feature_subset_strategy=str(strategy).encode("utf-8"),
+                    seed=int(seed))
+
+
+def _rf_forest_take(h) -> dict:
+    """The flat arrays of the pio_rf_forest h, which is destroyed."""
     try:
         nt, nn = C.c_int32(0), C.c_int64(0)
         _check(lib().pio_rf_forest_size(h, C.byref(nt), C.byref(nn)))
@@ -942,16 +1062,25 @@ def rf_train(label, x, num_classes, num_trees, strategy, impurity, max_depth, ma
 def rf_predict(forest, num_classes, x, device=0):
     """pio_rf_predict: the forest's vote (class index, int32 [n]) for the rows of x (n x n_feat)."""
     x = np.ascontiguousarray(x, np.float64)
-    a = {k: np.ascontiguousarray(forest[k], np.int32) for k in ("tree_off", *RF_FOREST_INT)}
-    thr = np.ascontiguousarray(forest["threshold"], np.float64)
     n = x.shape[0]
     out = np.empty(n, np.int32)
     vp = C.c_void_p
-    _check(lib().pio_rf_predict(C.c_int(device), C.c_int32(a["tree_off"].shape[0] - 1), vp(_addr(a["tree_off"])),
-                                C.c_int64(thr.shape[0]), vp(_addr(a["feature"])), vp(_addr(thr)), vp(_addr(a["left"])),
-                                vp(_addr(a["right"])), vp(_addr(a["prediction"])), C.c_int32(num_classes), vp(_addr(x)),
-                                C.c_int64(n), C.c_int32(x.shape[1]), vp(_addr(out))))
+    args, _arrays = _rf_flat(forest, num_classes)
+    _check(lib().pio_rf_predict(C.c_int(device), *args, vp(_addr(x)), C.c_int64(n), C.c_int32(x.shape[1]),
+                                vp(_addr(out))))
     return out
+
+
+def _rf_flat(forest, num_classes):
+    """(pio_rf_predict's forest arguments n_trees .. num_classes, the contiguous arrays they point into): the arrays
+    must outlive the call."""
+    a = {k: np.ascontiguousarray(forest[k], np.int32) for k in ("tree_off", *RF_FOREST_INT)}
+    a["threshold"] = np.ascontiguousarray(forest["threshold"], np.float64)
+    vp = C.c_void_p
+    args = [C.c_int32(a["tree_off"].shape[0] - 1), vp(_addr(a["tree_off"])), C.c_int64(a["threshold"].shape[0]),
+            vp(_addr(a["feature"])), vp(_addr(a["threshold"])), vp(_addr(a["left"])), vp(_addr(a["right"])),
+            vp(_addr(a["prediction"])), C.c_int32(num_classes)]
+    return args, a
 
 
 def rf_train_timing() -> dict:

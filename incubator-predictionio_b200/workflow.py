@@ -115,9 +115,16 @@ def load_class(path: str):
 
 
 def get_engine(engineFactory: str) -> Engine:
+    """The engine of an engine factory, an engine, or an evaluation (the engineFactory of a variant that
+    MetricEvaluator.saveEngineJson wrote)."""
+    from .evaluation import Evaluation
     obj = load_class(engineFactory)
+    if isinstance(obj, type) and issubclass(obj, Evaluation):
+        return obj.engine
     if isinstance(obj, type):
         obj = obj()
+    if isinstance(obj, Evaluation):
+        return obj.engine
     if isinstance(obj, Engine):
         return obj
     if isinstance(obj, EngineFactory) or hasattr(obj, "apply"):
@@ -255,9 +262,22 @@ class CreateWorkflow:
         return ap
 
     @staticmethod
-    def main(argv: Optional[Sequence[str]] = None) -> Optional[EngineInstance]:
+    def runEvaluation(evaluationClass: str, generatorClass: Optional[str], batch: str = ""):
+        """CoreWorkflow.runEvaluation: the evaluation over the generator's engine params, on one WorkflowContext."""
+        from .evaluation import run_evaluation
+        if not generatorClass:
+            raise SystemExit("--evaluation-class needs --engine-params-generator-class")
+        sc = WorkflowContext(batch, mode="Evaluation")
+        return run_evaluation(_instance(evaluationClass), _instance(generatorClass), sc)
+
+    @staticmethod
+    def main(argv: Optional[Sequence[str]] = None):
+        """Trains the engine variant and returns its EngineInstance; with --evaluation-class and
+        --engine-params-generator-class, runs that evaluation (`pio eval`) instead and returns its MetricEvaluatorResult."""
         wfc, _unknown = CreateWorkflow.parser().parse_known_args(argv)  # errorOnUnknownArgument = false
         logging.basicConfig(level=logging.DEBUG if wfc.debug else logging.INFO if wfc.verbose else logging.WARNING)
+        if wfc.evaluation_class:
+            return CreateWorkflow.runEvaluation(wfc.evaluation_class, wfc.engine_params_generator_class, wfc.batch)
         variant_path = wfc.engine_variant[5:] if wfc.engine_variant.startswith("file:") else wfc.engine_variant
         variantJson = json.loads(Path(variant_path).read_text())
         engineFactory = wfc.engine_factory or variantJson.get("engineFactory", "")
@@ -267,8 +287,6 @@ class CreateWorkflow:
         engine = get_engine(engineFactory)
         sparkConf = {str(k): str(v) for k, v in _flatten(variantJson.get("sparkConf", {}))}
         pioEnv = dict(kv.split("=", 1) for kv in wfc.env.split(",")) if wfc.env else {}
-        if wfc.evaluation_class:
-            raise SystemExit("evaluation workflow: use Engine.eval from Python (out of scope of this runner)")
         engineParams = engine.jValueToEngineParams(variantJson)
         now = _dt.datetime.now(_dt.timezone.utc).isoformat()
         boot = WorkflowContext(wfc.batch, pioEnv, mode="Training", sparkConf=sparkConf)
@@ -285,6 +303,11 @@ class CreateWorkflow:
                                                     stopAfterRead=wfc.stop_after_read,
                                                     stopAfterPrepare=wfc.stop_after_prepare))
         return EngineInstances.get(inst.id)
+
+
+def _instance(path: str):
+    obj = load_class(path)
+    return obj() if isinstance(obj, type) else obj
 
 
 def _flatten(d, prefix=""):
