@@ -66,6 +66,7 @@ extern "C" {
 #define PIO_ALS_ERR_NUMERIC (-4)  /* a normal equation was not positive definite (MLlib: dppsv info != 0) */
 #define PIO_ALS_ERR_IO (-5)
 #define PIO_ALS_ERR_COMM (-6)     /* NCCL */
+#define PIO_ALS_ERR_NOMEM (-7)    /* host memory exhausted (pio_cooc_model_create, pio_cooc_predict_filtered) */
 
 /* how repeated (user,item) pairs are treated by pio_als_set_ratings_coo */
 #define PIO_ALS_DEDUP_NONE 0      /* recommendation template: every event is its own rating (ALSAlgorithm.scala:62-65) */
@@ -504,6 +505,48 @@ PIO_API int pio_events_index_destroy(pio_events_index* ix);
  * item index.  Limits: n_items <= 2^20, fewer than 2^31 (user, item1, item2) triples. */
 PIO_API int pio_cooc_train(int device, const int32_t* user, const int32_t* item, int64_t n, int32_t n_users,
                            int32_t n_items, int topn, int32_t* out_item, int32_t* out_count, int32_t* out_n);
+
+/* Batch scoring of CooccurrenceAlgorithm.predict (CooccurrenceAlgorithm.scala:107-175) over a trained co-occurrence model
+ * (DESIGN.md 4.9).  An opaque object holds the model: top_items / top_counts n_items x topn and top_n n_items, HOST
+ * arrays in the layout pio_cooc_train returns.  Errors: status codes as above, text via pio_als_last_error(NULL). */
+typedef struct pio_cooc_model pio_cooc_model;
+
+typedef struct pio_cooc_stats {
+  int64_t kernel_launches;        /* kernels launched on behalf of this model, over all calls */
+  int64_t last_expanded;          /* (query, candidate) entries the last pio_cooc_predict_filtered expanded, all parts */
+  int64_t last_rows;              /* distinct (query, item) rows of the last call that passed the filters */
+  int64_t last_budget;            /* expanded entries per part the last call was split by */
+  int32_t last_parts;             /* parts of the last call (0: no query, or rejected) */
+  int32_t last_max_part_queries;  /* most queries in one part of the last call */
+} pio_cooc_stats;
+
+/* Default number of expanded entries per part of a pio_cooc_predict_filtered call (about 48 bytes of device memory
+ * each); the environment variable PIO_COOC_PREDICT_BUDGET (a positive integer) overrides it.  Results do not depend
+ * on it. */
+#define PIO_COOC_PREDICT_BUDGET (1ll << 24)
+
+/* Checks the arrays on the host -- 0 <= top_n[i] <= topn, top_items[i][t] in [0, n_items) and top_counts[i][t] >= 0 for
+ * t < top_n[i] -- and copies them: PIO_ALS_ERR_ARG naming the item and slot of the first violation.  n_items >= 1, topn
+ * >= 1.  The device copy is made on `device` by the first pio_cooc_predict_filtered, so that a model
+ * holds no device memory until it scores. */
+PIO_API int pio_cooc_model_create(int device, int32_t n_items, int32_t topn, const int32_t* top_items,
+                                  const int32_t* top_counts, const int32_t* top_n, pio_cooc_model** out);
+PIO_API int pio_cooc_model_destroy(pio_cooc_model* m);
+/* n_queries queries: query j = q_items[q_ptr[j] .. q_ptr[j+1]) (HOST); ids outside [0, n_items) and repeats are ignored.
+ * Row j of out_items (int32) / out_scores (int64), n_queries x topk, best first, padded with -1 / 0, and out_count[j]
+ * (nullable): for the set Q of query j's known items, the candidates are the items of the first top_n[q] entries of each
+ * q in Q, scored by the sum of their counts over Q (exact, int64); a candidate is dropped when query j has a white list
+ * (f->has_wl[j]) that does not hold it, when its exclusion list or set row (f: pio_als_query_filter, nullable, with the
+ * argument rules of pio_als_similar_batch_filtered) holds it, or when it is in Q; the rest are ordered by score
+ * descending, then item index ascending, and cut at topk >= 1.
+ * The batch runs in parts of consecutive queries whose expansions -- the sum of top_n over each query's listed known
+ * ids, a repeated id counted each time -- stay within PIO_COOC_PREDICT_BUDGET entries, at least one query per part.
+ * Rejected with PIO_ALS_ERR_ARG before any device work: bad arguments, q_ptr not non-decreasing from 0 or naming
+ * entries of a NULL q_items, a bad filter, and a query whose expansion is 2^32 entries or more. */
+PIO_API int pio_cooc_predict_filtered(pio_cooc_model* m, const int64_t* q_ptr, const int32_t* q_items,
+                                      int32_t n_queries, int32_t topk, const pio_als_query_filter* f,
+                                      int32_t* out_items, int64_t* out_scores, int32_t* out_count);
+PIO_API int pio_cooc_model_get_stats(const pio_cooc_model* m, pio_cooc_stats* out);
 
 /* MLlib multinomial NaiveBayes (classification template). HOST buffers.
  * label: class index 0..n_class-1; x: n x n_feat, non-negative. pi: n_class, theta: n_class x n_feat

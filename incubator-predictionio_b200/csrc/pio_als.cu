@@ -20,6 +20,7 @@
 #include <deque>
 #include <exception>
 #include <map>
+#include <memory>
 #include <mutex>
 #include <string>
 #include <type_traits>
@@ -53,6 +54,7 @@
 #include "events_fold.cuh"
 #include "events_index.cuh"
 #include "cooc.cuh"
+#include "cooc_predict.cuh"
 #include "forest.cuh"
 #include "eval_folds.cuh"
 #include "cls_folds.cuh"
@@ -462,15 +464,26 @@ struct pio_als_handle {
 
 namespace pio {
 
-static int fail(pio_als_handle* h, int code, const char* fmt, ...) {
+static int vfail(std::string& sink, int code, const char* fmt, va_list ap) {
   char buf[512];
+  vsnprintf(buf, sizeof buf, fmt, ap);
+  sink = buf;
+  return code;
+}
+// the message goes to the handle, or (h == nullptr) to the thread's last error
+static int fail(pio_als_handle* h, int code, const char* fmt, ...) {
   va_list ap;
   va_start(ap, fmt);
-  vsnprintf(buf, sizeof buf, fmt, ap);
+  const int rc = vfail(h ? h->err : g_create_error, code, fmt, ap);
   va_end(ap);
-  if (h) h->err = buf;
-  else g_create_error = buf;
-  return code;
+  return rc;
+}
+static int fail_to(std::string* sink, int code, const char* fmt, ...) {
+  va_list ap;
+  va_start(ap, fmt);
+  const int rc = vfail(*sink, code, fmt, ap);
+  va_end(ap);
+  return rc;
 }
 // PIO_ALS_INGEST_TRACE=1: wall-clock milliseconds per ingest phase (stream drained at every mark) on stderr
 static void tmark(pio_als_handle* h, const char* what) {
@@ -2329,37 +2342,63 @@ static const char* query_filter_error(const pio_als_query_filter* f, int n) {
   return nullptr;
 }
 
+// What the per-query filter uploads need from their caller: the stream they run on, the item count of the set rows, the
+// launch counter they add to and where a failure's message goes.  The ALS scoring calls pass their handle's
+// (filter_env); the co-occurrence model passes its own.
+struct FilterEnv {
+  cudaStream_t st;
+  int n_items;
+  int64_t* launches;
+  std::string* err;
+};
+static FilterEnv filter_env(pio_als_handle* h) { return FilterEnv{h->stream, h->I.n, &h->st.kernel_launches, &h->err}; }
+#define CKF(env, call)                                                                                        \
+  do {                                                                                                        \
+    cudaError_t e_ = (call);                                                                                  \
+    if (e_ != cudaSuccess)                                                                                    \
+      return fail_to((env).err, PIO_ALS_ERR_CUDA, "%s failed: %s (%s:%d)", #call, cudaGetErrorString(e_), \
+                     __FILE__, __LINE__);                                                                     \
+  } while (0)
+// one launch of n_threads threads in blocks of 256 on env's stream, counted, failing on a launch error
+template <typename... KArgs, typename... Args>
+static int env_launch(const FilterEnv& env, void (*kernel)(KArgs...), long long n_threads, Args... args) {
+  kernel<<<nblk(n_threads, 256), 256, 0, env.st>>>(args...);
+  ++*env.launches;
+  CKF(env, cudaGetLastError());
+  return PIO_ALS_OK;
+}
+
 // the lists ptr / items of the queries idx on the device, as sorted keys; the queries are renumbered 0 .. idx.size() - 1
 struct DevLists {
   const unsigned long long* keys = nullptr;
   long long* ptr = nullptr;
 };
-static int upload_lists(pio_als_handle* h, const int64_t* ptr, const int32_t* items, const std::vector<int>& idx, Scratch& tmp,
-                        DevLists* out) {
-  cudaStream_t st = h->stream;
+static int upload_lists(const FilterEnv& env, const int64_t* ptr, const int32_t* items, const std::vector<int>& idx,
+                        Scratch& tmp, DevLists* out) {
+  cudaStream_t st = env.st;
   const int n = (int)idx.size();
   std::vector<long long> rel((size_t)n + 1, 0);
   for (int i = 0; i < n; ++i) rel[i + 1] = rel[i] + (ptr ? ptr[idx[i] + 1] - ptr[idx[i]] : 0);
   const long long total = rel[n];
-  CK(h, tmp.alloc(&out->ptr, rel.size()));
-  CK(h, cudaMemcpyAsync(out->ptr, rel.data(), sizeof(long long) * rel.size(), cudaMemcpyHostToDevice, st));
+  CKF(env, tmp.alloc(&out->ptr, rel.size()));
+  CKF(env, cudaMemcpyAsync(out->ptr, rel.data(), sizeof(long long) * rel.size(), cudaMemcpyHostToDevice, st));
   if (total == 0) return PIO_ALS_OK;
   std::vector<int> flat((size_t)total);
   for (int i = 0; i < n; ++i)
     if (rel[i + 1] > rel[i]) memcpy(flat.data() + rel[i], items + ptr[idx[i]], sizeof(int) * (size_t)(rel[i + 1] - rel[i]));
   int* d_items = nullptr;
   SortBufs sb;
-  CK(h, tmp.alloc(&d_items, (size_t)total));
+  CKF(env, tmp.alloc(&d_items, (size_t)total));
   for (int b = 0; b < 2; ++b) {
-    CK(h, tmp.alloc(&sb.k[b], (size_t)total));
-    CK(h, tmp.alloc(&sb.v[b], (size_t)total));
+    CKF(env, tmp.alloc(&sb.k[b], (size_t)total));
+    CKF(env, tmp.alloc(&sb.v[b], (size_t)total));
   }
-  CK(h, cudaMemcpyAsync(d_items, flat.data(), sizeof(int) * (size_t)total, cudaMemcpyHostToDevice, st));
-  const int rc = score_launch(h, qf_keys_kernel, dim3(nblk(total, 256)), dim3(256), 0, 0, (const int*)d_items,
-                              (const long long*)out->ptr, n, total, (unsigned long long*)sb.k[0]);
+  CKF(env, cudaMemcpyAsync(d_items, flat.data(), sizeof(int) * (size_t)total, cudaMemcpyHostToDevice, st));
+  const int rc = env_launch(env, qf_keys_kernel, total, (const int*)d_items, (const long long*)out->ptr, n, total,
+                               (unsigned long long*)sb.k[0]);
   if (rc) return rc;
-  CK(h, cudaMemsetAsync(sb.v[0], 0, sizeof(uint32_t) * (size_t)total, st));   // the sort carries a payload; none is needed
-  CK(h, radix_sort_pairs(sb, (size_t)total, 32 + ceil_log2((uint64_t)n), st, &h->st.kernel_launches));
+  CKF(env, cudaMemsetAsync(sb.v[0], 0, sizeof(uint32_t) * (size_t)total, st));   // the sort carries a payload; none is needed
+  CKF(env, radix_sort_pairs(sb, (size_t)total, 32 + ceil_log2((uint64_t)n), st, env.launches));
   out->keys = (const unsigned long long*)sb.keys();
   return PIO_ALS_OK;
 }
@@ -2370,27 +2409,31 @@ struct CallFilter {
   unsigned* set_bits = nullptr;
   int set_words = 0;
 };
-static int upload_call_filter(pio_als_handle* h, const uint8_t* item_mask, const double* item_weight,
-                              const pio_als_query_filter* f, Scratch& tmp, CallFilter* out) {
-  int rc = upload_filter(h, item_mask, item_weight, &tmp, 0, &out->dense);
-  if (rc) return rc;
+// the set rows of f (n_items bytes each) as bits, into out->set_bits / set_words
+static int upload_set_rows(const FilterEnv& env, const pio_als_query_filter* f, Scratch& tmp, CallFilter* out) {
   if (!f->set_ix || f->n_sets == 0 || !f->item_sets) return PIO_ALS_OK;
-  const int n_items = h->I.n;
+  const int n_items = env.n_items;
   out->set_words = (n_items + 31) / 32;
   const long long n_words = (long long)f->n_sets * out->set_words;
   uint8_t* d_sets = nullptr;
-  CK(h, tmp.alloc(&d_sets, (size_t)f->n_sets * n_items));
-  CK(h, tmp.alloc(&out->set_bits, (size_t)n_words));
-  CK(h, cudaMemcpyAsync(d_sets, f->item_sets, (size_t)f->n_sets * n_items, cudaMemcpyHostToDevice, h->stream));
-  return score_launch(h, qf_pack_sets_kernel, dim3(nblk(n_words, 256)), dim3(256), 0, 0, (const uint8_t*)d_sets, n_items,
-                      out->set_words, n_words, out->set_bits);
+  CKF(env, tmp.alloc(&d_sets, (size_t)f->n_sets * n_items));
+  CKF(env, tmp.alloc(&out->set_bits, (size_t)n_words));
+  CKF(env, cudaMemcpyAsync(d_sets, f->item_sets, (size_t)f->n_sets * n_items, cudaMemcpyHostToDevice, env.st));
+  return env_launch(env, qf_pack_sets_kernel, n_words, (const uint8_t*)d_sets, n_items, out->set_words, n_words,
+                       out->set_bits);
+}
+static int upload_call_filter(pio_als_handle* h, const uint8_t* item_mask, const double* item_weight,
+                              const pio_als_query_filter* f, Scratch& tmp, CallFilter* out) {
+  const int rc = upload_filter(h, item_mask, item_weight, &tmp, 0, &out->dense);
+  if (rc) return rc;
+  return upload_set_rows(filter_env(h), f, tmp, out);
 }
 // the exclusion lists and set rows of the queries idx (renumbered 0 .. idx.size() - 1)
-static int upload_part_filter(pio_als_handle* h, const pio_als_query_filter* f, const CallFilter& cf,
+static int upload_part_filter(const FilterEnv& env, const pio_als_query_filter* f, const CallFilter& cf,
                               const std::vector<int>& idx, Scratch& tmp, QueryFilterDev* out) {
   if (f->ex_ptr) {
     DevLists ex;
-    const int rc = upload_lists(h, f->ex_ptr, f->ex_items, idx, tmp, &ex);
+    const int rc = upload_lists(env, f->ex_ptr, f->ex_items, idx, tmp, &ex);
     if (rc) return rc;
     out->ex = ex.keys;
     out->ex_ptr = ex.ptr;
@@ -2399,8 +2442,8 @@ static int upload_part_filter(pio_als_handle* h, const pio_als_query_filter* f, 
     std::vector<int> six(idx.size());
     for (size_t i = 0; i < idx.size(); ++i) six[i] = f->set_ix[idx[i]];
     int* d_six = nullptr;
-    CK(h, tmp.alloc(&d_six, six.size()));
-    CK(h, cudaMemcpyAsync(d_six, six.data(), sizeof(int) * six.size(), cudaMemcpyHostToDevice, h->stream));
+    CKF(env, tmp.alloc(&d_six, six.size()));
+    CKF(env, cudaMemcpyAsync(d_six, six.data(), sizeof(int) * six.size(), cudaMemcpyHostToDevice, env.st));
     out->set_ix = d_six;
     out->set_bits = cf.set_bits;
     out->set_words = cf.set_words;
@@ -2451,11 +2494,11 @@ static int recommend_part(pio_als_handle* h, const int32_t* users, const std::ve
                     h->U.n, d_xq, d_valid);
   if (rc) return rc;
   QueryFilterDev qf;
-  rc = upload_part_filter(h, f, cf, idx, tmp, &qf);
+  rc = upload_part_filter(filter_env(h), f, cf, idx, tmp, &qf);
   if (rc) return rc;
   if (listed) {
     DevLists wl;
-    rc = upload_lists(h, f->wl_ptr, f->wl_items, idx, tmp, &wl);
+    rc = upload_lists(filter_env(h), f->wl_ptr, f->wl_items, idx, tmp, &wl);
     if (rc) return rc;
     rc = run_passes(h, p, n, topk, d_cand, o, [&](const Chunk& c) {
       return score_launch(h, score_listed_kernel<false>, c.grid, dim3(p.threads), p.smem, p.launch_bits(), h->I.F, KP, h->I.perm,
@@ -2493,7 +2536,7 @@ static int similar_part(pio_als_handle* h, const std::vector<int64_t>& sp, const
   bool done = false;
   if (listed || first.route == ROUTE_BATCH) {
     if (total >= (1ll << 31)) return fail(h, PIO_ALS_ERR_ARG, "white-listed queries with 2^31 or more query items in all");
-    rc = upload_part_filter(h, f, cf, idx, tmp, &qf);
+    rc = upload_part_filter(filter_env(h), f, cf, idx, tmp, &qf);
     if (rc) return rc;
     // all query item vectors in one gather (zeros for an id without a factor)
     int* d_qid = nullptr;
@@ -2510,7 +2553,7 @@ static int similar_part(pio_als_handle* h, const std::vector<int64_t>& sp, const
     }
     if (listed) {
       DevLists wl;
-      rc = upload_lists(h, f->wl_ptr, f->wl_items, idx, tmp, &wl);
+      rc = upload_lists(filter_env(h), f->wl_ptr, f->wl_items, idx, tmp, &wl);
       if (rc) return rc;
       std::vector<long long> rel(sp.begin(), sp.end());
       long long* d_qptr = nullptr;
@@ -4394,6 +4437,318 @@ int pio_cooc_train(int device, const int32_t* user, const int32_t* item, int64_t
   memcpy(out_item, h_item.data(), 4 * h_item.size());
   memcpy(out_count, h_cnt.data(), 4 * h_cnt.size());
   memcpy(out_n, h_n.data(), 4 * h_n.size());
+  return PIO_ALS_OK;
+}
+
+}  // extern "C"
+
+// ---- co-occurrence batch scoring (similarproduct CooccurrenceAlgorithm.predict) --------------------------------------------
+struct pio_cooc_model {
+  int device = 0, n_items = 0, topn = 0;
+  std::vector<int32_t> top_n;           // sizes a call's parts before any device work
+  std::vector<int64_t> row_sum;         // per item, the sum of its counts: a query's scores are at most the sum over its ids
+  std::vector<int32_t> items, counts;   // host copies until the first call uploads them
+  cudaStream_t st = nullptr;
+  int *d_items = nullptr, *d_counts = nullptr, *d_n = nullptr;   // set together, once every copy has landed
+  mutable std::mutex mu;                // serialises the calls, and guards stats
+  pio_cooc_stats stats{};
+};
+
+namespace pio {
+
+// A call's parts: consecutive queries [first[p], first[p + 1]).  A part closes before the query that would take its
+// listed expansion over the budget or its listed ids past 2^31 - 1; each part holds at least one query.
+struct CoocPlan {
+  std::vector<int> first;
+  std::vector<uint64_t> bound;   // per part, the largest score bound of its queries
+};
+static int cooc_plan(const pio_cooc_model* m, const int64_t* q_ptr, const int32_t* q_items, int n, long long budget,
+                     CoocPlan* p) {
+  long long acc = 0, acc_ids = 0;
+  for (int j = 0; j < n; ++j) {
+    unsigned long long ex = 0, bound = 0;
+    for (int64_t t = q_ptr[j]; t < q_ptr[j + 1]; ++t) {
+      const int32_t it = q_items[t];
+      if (it < 0 || it >= m->n_items) continue;
+      ex += (unsigned)m->top_n[it];
+      bound += (unsigned long long)m->row_sum[it];
+    }
+    const long long ids = q_ptr[j + 1] - q_ptr[j];
+    if (ex >= (1ull << 32))
+      return fail(nullptr, PIO_ALS_ERR_ARG, "query %d expands to %llu entries: at most 2^32 - 1 fit one part", j, ex);
+    if (ids >= (1ll << 31)) return fail(nullptr, PIO_ALS_ERR_ARG, "query %d lists 2^31 or more ids", j);
+    if (j == 0 || acc + (long long)ex > budget || acc_ids + ids >= (1ll << 31)) {
+      p->first.push_back(j);
+      p->bound.push_back(0);
+      acc = acc_ids = 0;
+    }
+    acc += (long long)ex;
+    acc_ids += ids;
+    p->bound.back() = std::max<uint64_t>(p->bound.back(), bound);
+  }
+  p->first.push_back(n);
+  return PIO_ALS_OK;
+}
+
+// The model's device copy, made on its own stream by the first call.  The device pointers are published only after the
+// copies have completed, so a failed upload leaves nothing half made: its allocations are freed and the next call
+// starts over.
+static int cooc_upload(pio_cooc_model* m, const FilterEnv& env) {
+  if (m->d_items) return PIO_ALS_OK;
+  if (!m->st) CKF(env, cudaStreamCreateWithFlags(&m->st, cudaStreamNonBlocking));
+  const size_t cells = (size_t)m->n_items * m->topn;
+  const size_t len[3] = {cells, cells, (size_t)m->n_items};
+  const int32_t* src[3] = {m->items.data(), m->counts.data(), m->top_n.data()};
+  int* d[3] = {nullptr, nullptr, nullptr};
+  cudaError_t e = cudaSuccess;
+  for (int k = 0; k < 3 && e == cudaSuccess; ++k) e = cudaMalloc((void**)&d[k], sizeof(int) * len[k]);
+  for (int k = 0; k < 3 && e == cudaSuccess; ++k)
+    e = cudaMemcpyAsync(d[k], src[k], sizeof(int) * len[k], cudaMemcpyHostToDevice, m->st);
+  if (e == cudaSuccess) e = cudaStreamSynchronize(m->st);   // the host copies are read until here
+  if (e != cudaSuccess) {
+    cudaStreamSynchronize(m->st);
+    for (int* p : d)
+      if (p) cudaFree(p);
+    return fail_to(env.err, PIO_ALS_ERR_CUDA, "uploading the co-occurrence model: %s", cudaGetErrorString(e));
+  }
+  m->d_items = d[0], m->d_counts = d[1], m->d_n = d[2];
+  std::vector<int32_t>().swap(m->items);
+  std::vector<int32_t>().swap(m->counts);
+  return PIO_ALS_OK;
+}
+
+// the queries [j0, j1) of a call: rows j0 .. j1 - 1 of the caller's outputs
+static int cooc_part(pio_cooc_model* m, const FilterEnv& env, const int64_t* q_ptr, const int32_t* q_items, int j0, int j1,
+                     int topk, uint64_t bound, const pio_als_query_filter* f, const CallFilter& cf, int32_t* out_items,
+                     int64_t* out_scores, int32_t* out_count) {
+  const int n = j1 - j0;
+  cudaStream_t st = m->st;
+  Scratch tmp(st);
+  std::vector<int> idx((size_t)n);
+  for (int i = 0; i < n; ++i) idx[i] = j0 + i;
+  DevLists ql;
+  int rc = upload_lists(env, q_ptr, q_items, idx, tmp, &ql);
+  if (rc) return rc;
+  CoocLists L;
+  L.q = ql.keys;
+  L.q_ptr = ql.ptr;
+  QueryFilterDev qf;
+  if (f) {
+    rc = upload_part_filter(env, f, cf, idx, tmp, &qf);
+    if (rc) return rc;
+    if (f->has_wl && std::any_of(f->has_wl + j0, f->has_wl + j1, [](uint8_t x) { return x != 0; })) {
+      DevLists wl;
+      rc = upload_lists(env, f->wl_ptr, f->wl_items, idx, tmp, &wl);
+      if (rc) return rc;
+      uint8_t* d_has = nullptr;
+      CKF(env, tmp.alloc(&d_has, (size_t)n));
+      CKF(env, cudaMemcpyAsync(d_has, f->has_wl + j0, (size_t)n, cudaMemcpyHostToDevice, st));
+      L.has_wl = d_has;
+      L.wl = wl.keys;
+      L.wl_ptr = wl.ptr;
+    }
+  }
+  // sizes and offsets of the expansion
+  const long long T = q_ptr[j1] - q_ptr[j0];
+  uint32_t *size = nullptr, *off = nullptr;
+  long long E = 0;
+  if (T > 0) {
+    CKF(env, tmp.alloc(&size, (size_t)T));
+    CKF(env, tmp.alloc(&off, (size_t)T));
+    rc = env_launch(env, cp_size_kernel, T, ql.keys, T, m->n_items, (const int*)m->d_n, size);
+    if (rc) return rc;
+    CKF(env, scan_exclusive_u32(size, off, (size_t)T, st, env.launches));
+    uint32_t last[2] = {0, 0};
+    CKF(env, cudaMemcpyAsync(&last[0], off + T - 1, 4, cudaMemcpyDeviceToHost, st));
+    CKF(env, cudaMemcpyAsync(&last[1], size + T - 1, 4, cudaMemcpyDeviceToHost, st));
+    CKF(env, cudaStreamSynchronize(st));
+    E = (long long)last[0] + last[1];
+  }
+  m->stats.last_expanded += E;
+  // expand, sort by (query, candidate), sum each run that passes the filters, order each query's rows
+  const int bits_q = ceil_log2((uint64_t)n), bits_i = ceil_log2((uint64_t)m->n_items);
+  SortBufs sb;
+  int* row_q = nullptr;
+  int* row_item = nullptr;
+  long long* row_score = nullptr;
+  long long R = 0;
+  if (E > 0) {
+    for (int b = 0; b < 2; ++b) {
+      CKF(env, tmp.alloc(&sb.k[b], (size_t)E));
+      CKF(env, tmp.alloc(&sb.v[b], (size_t)E));
+    }
+    rc = env_launch(env, cp_expand_kernel, T * 32, ql.keys, (const uint32_t*)size, (const uint32_t*)off, T,
+                    (const int*)m->d_items, (const int*)m->d_counts, m->topn, bits_i, sb.keys(), sb.vals());
+    if (rc) return rc;
+    CKF(env, radix_sort_pairs(sb, (size_t)E, bits_q + bits_i, st, env.launches));
+    uint32_t *pass = nullptr, *pos = nullptr;
+    CKF(env, tmp.alloc(&pass, (size_t)E));
+    CKF(env, tmp.alloc(&pos, (size_t)E));
+    rc = env_launch(env, cp_pass_kernel, E, (const uint64_t*)sb.keys(), E, bits_i, L, qf, pass);
+    if (rc) return rc;
+    CKF(env, scan_exclusive_u32(pass, pos, (size_t)E, st, env.launches));
+    uint32_t last[2] = {0, 0};
+    CKF(env, cudaMemcpyAsync(&last[0], pos + E - 1, 4, cudaMemcpyDeviceToHost, st));
+    CKF(env, cudaMemcpyAsync(&last[1], pass + E - 1, 4, cudaMemcpyDeviceToHost, st));
+    CKF(env, cudaStreamSynchronize(st));
+    R = (long long)last[0] + last[1];
+    if (R > 0) {
+      CKF(env, tmp.alloc(&row_q, (size_t)R));
+      CKF(env, tmp.alloc(&row_item, (size_t)R));
+      CKF(env, tmp.alloc(&row_score, (size_t)R));
+      rc = env_launch(env, cp_rows_kernel, E, (const uint64_t*)sb.keys(), (const uint32_t*)sb.vals(), E, bits_i,
+                      (const uint32_t*)pass, (const uint32_t*)pos, (uint64_t)bound, row_q, row_item, row_score,
+                      sb.spare_keys(), sb.spare_vals());
+      if (rc) return rc;
+      sb.flip();
+      // stable LSD: by score descending, then by query; rows enter in (query, item) order, so equal scores stay
+      // item-ascending
+      const int sbits = bound ? 64 - __builtin_clzll(bound) : 0;
+      CKF(env, radix_sort_pairs(sb, (size_t)R, sbits, st, env.launches));
+      rc = env_launch(env, cp_query_keys_kernel, R, (const uint32_t*)sb.vals(), R, (const int*)row_q, sb.spare_keys(),
+                      sb.spare_vals());
+      if (rc) return rc;
+      sb.flip();
+      CKF(env, radix_sort_pairs(sb, (size_t)R, bits_q, st, env.launches));
+    }
+  }
+  m->stats.last_rows += R;
+  int* d_oi = nullptr;
+  long long* d_os = nullptr;
+  int* d_oc = nullptr;
+  CKF(env, tmp.alloc(&d_oi, (size_t)n * topk));
+  CKF(env, tmp.alloc(&d_os, (size_t)n * topk));
+  CKF(env, tmp.alloc(&d_oc, (size_t)n));
+  cp_take_kernel<<<n, 128, 0, st>>>((const uint64_t*)sb.keys(), (const uint32_t*)sb.vals(), R, topk, row_item, row_score,
+                                    d_oi, d_os, d_oc);
+  ++*env.launches;
+  CKF(env, cudaGetLastError());
+  CKF(env, cudaMemcpyAsync(out_items + (size_t)j0 * topk, d_oi, sizeof(int) * (size_t)n * topk, cudaMemcpyDeviceToHost, st));
+  CKF(env, cudaMemcpyAsync(out_scores + (size_t)j0 * topk, d_os, sizeof(long long) * (size_t)n * topk,
+                           cudaMemcpyDeviceToHost, st));
+  if (out_count) CKF(env, cudaMemcpyAsync(out_count + j0, d_oc, sizeof(int) * (size_t)n, cudaMemcpyDeviceToHost, st));
+  CKF(env, cudaStreamSynchronize(st));
+  return PIO_ALS_OK;
+}
+
+}  // namespace pio
+
+extern "C" {
+
+int pio_cooc_model_create(int device, int32_t n_items, int32_t topn, const int32_t* top_items, const int32_t* top_counts,
+                          const int32_t* top_n, pio_cooc_model** out) {
+  if (!out || !top_items || !top_counts || !top_n || n_items < 1 || topn < 1)
+    return fail(nullptr, PIO_ALS_ERR_ARG, "bad pio_cooc_model_create arguments");
+  *out = nullptr;
+  for (int32_t i = 0; i < n_items; ++i) {
+    if (top_n[i] < 0 || top_n[i] > topn)
+      return fail(nullptr, PIO_ALS_ERR_ARG, "item %d: top_n %d is outside [0, %d]", i, top_n[i], topn);
+    for (int32_t t = 0; t < top_n[i]; ++t) {
+      const size_t c = (size_t)i * topn + t;
+      if (top_items[c] < 0 || top_items[c] >= n_items)
+        return fail(nullptr, PIO_ALS_ERR_ARG, "item %d, slot %d: item %d is outside [0, %d)", i, t, top_items[c], n_items);
+      if (top_counts[c] < 0)
+        return fail(nullptr, PIO_ALS_ERR_ARG, "item %d, slot %d: count %d is negative", i, t, top_counts[c]);
+    }
+  }
+  std::unique_ptr<pio_cooc_model> m;
+  try {   // bad_alloc must not cross the C boundary
+    m.reset(new pio_cooc_model);
+    const size_t cells = (size_t)n_items * topn;
+    m->device = device, m->n_items = n_items, m->topn = topn;
+    m->items.assign(top_items, top_items + cells);
+    m->counts.assign(top_counts, top_counts + cells);
+    m->top_n.assign(top_n, top_n + n_items);
+    m->row_sum.assign((size_t)n_items, 0);
+  } catch (const std::bad_alloc&) {
+    return fail(nullptr, PIO_ALS_ERR_NOMEM, "pio_cooc_model_create: out of host memory");
+  }
+  for (int32_t i = 0; i < n_items; ++i)
+    for (int32_t t = 0; t < top_n[i]; ++t) m->row_sum[i] += top_counts[(size_t)i * topn + t];
+  *out = m.release();
+  return PIO_ALS_OK;
+}
+
+int pio_cooc_model_destroy(pio_cooc_model* m) {
+  if (!m) return PIO_ALS_OK;
+  if (m->st) {
+    cudaSetDevice(m->device);
+    cudaStreamSynchronize(m->st);
+    cudaStreamDestroy(m->st);
+  }
+  for (int* p : {m->d_items, m->d_counts, m->d_n})
+    if (p) cudaFree(p);
+  delete m;
+  return PIO_ALS_OK;
+}
+
+}  // extern "C"
+
+namespace pio {
+static int cooc_predict(pio_cooc_model* m, const int64_t* q_ptr, const int32_t* q_items, int32_t n_queries, int32_t topk,
+                        const pio_als_query_filter* f, int32_t* out_items, int64_t* out_scores, int32_t* out_count) {
+  pio_cooc_stats& s = m->stats;
+  s.last_expanded = s.last_rows = s.last_budget = 0;
+  s.last_parts = s.last_max_part_queries = 0;
+  if (n_queries < 0 || topk < 1) return fail(nullptr, PIO_ALS_ERR_ARG, "topk must be >= 1 and n_queries >= 0");
+  if (n_queries == 0) return PIO_ALS_OK;
+  if (!q_ptr || !out_items || !out_scores) return fail(nullptr, PIO_ALS_ERR_ARG, "null argument");
+  if (q_ptr[0] < 0) return fail(nullptr, PIO_ALS_ERR_ARG, "q_ptr must be non-decreasing offsets into q_items");
+  for (int j = 0; j < n_queries; ++j)
+    if (q_ptr[j + 1] < q_ptr[j] || (q_ptr[j + 1] > q_ptr[j] && !q_items))
+      return fail(nullptr, PIO_ALS_ERR_ARG, "q_ptr must be non-decreasing offsets into q_items");
+  if (f)
+    if (const char* what = query_filter_error(f, n_queries)) return fail(nullptr, PIO_ALS_ERR_ARG, "%s", what);
+  // PIO_COOC_PREDICT_BUDGET: expanded entries per part; capped so that a part's offsets fit the 32-bit scan
+  const char* env_b = getenv("PIO_COOC_PREDICT_BUDGET");
+  const long long budget = std::min<long long>(env_b && atoll(env_b) > 0 ? atoll(env_b) : PIO_COOC_PREDICT_BUDGET,
+                                               (1ll << 32) - 1);
+  CoocPlan plan;
+  int rc = cooc_plan(m, q_ptr, q_items, n_queries, budget, &plan);
+  if (rc) return rc;
+  CK0(cudaSetDevice(m->device));
+  const FilterEnv env{nullptr, m->n_items, &s.kernel_launches, &g_create_error};
+  rc = cooc_upload(m, env);
+  if (rc) return rc;
+  FilterEnv penv = env;
+  penv.st = m->st;
+  s.last_budget = budget;
+  Scratch tmp(m->st);
+  CallFilter cf;
+  if (f) {
+    rc = upload_set_rows(penv, f, tmp, &cf);
+    if (rc) return rc;
+  }
+  const int parts = (int)plan.first.size() - 1;
+  for (int p = 0; p < parts; ++p) {
+    const int j0 = plan.first[p], j1 = plan.first[p + 1];
+    s.last_parts = p + 1;
+    s.last_max_part_queries = std::max(s.last_max_part_queries, j1 - j0);
+    rc = cooc_part(m, penv, q_ptr, q_items, j0, j1, topk, plan.bound[p], f, cf, out_items, out_scores, out_count);
+    if (rc) return rc;
+  }
+  return PIO_ALS_OK;
+}
+}  // namespace pio
+
+extern "C" {
+
+int pio_cooc_predict_filtered(pio_cooc_model* m, const int64_t* q_ptr, const int32_t* q_items, int32_t n_queries,
+                              int32_t topk, const pio_als_query_filter* f, int32_t* out_items, int64_t* out_scores,
+                              int32_t* out_count) {
+  if (!m) return fail(nullptr, PIO_ALS_ERR_ARG, "null model");
+  std::lock_guard<std::mutex> lk(m->mu);
+  try {   // bad_alloc must not cross the C boundary; Scratch releases a part's device memory on the way out
+    return cooc_predict(m, q_ptr, q_items, n_queries, topk, f, out_items, out_scores, out_count);
+  } catch (const std::bad_alloc&) {
+    return fail(nullptr, PIO_ALS_ERR_NOMEM, "pio_cooc_predict_filtered: out of host memory");
+  }
+}
+
+int pio_cooc_model_get_stats(const pio_cooc_model* m, pio_cooc_stats* out) {
+  if (!m || !out) return fail(nullptr, PIO_ALS_ERR_ARG, "null argument");
+  std::lock_guard<std::mutex> lk(m->mu);
+  *out = m->stats;
   return PIO_ALS_OK;
 }
 

@@ -23,7 +23,7 @@ ABI_VERSION = 2
 DEDUP_NONE, DEDUP_SUM, DEDUP_KEEP_LAST = 0, 1, 2
 INIT_CALLER, INIT_HASH = 0, 1
 SIM_KEEP_QUERY_ITEMS = 1
-ERR_ARG, ERR_CUDA, ERR_STATE, ERR_NUMERIC, ERR_IO, ERR_COMM = -1, -2, -3, -4, -5, -6
+ERR_ARG, ERR_CUDA, ERR_STATE, ERR_NUMERIC, ERR_IO, ERR_COMM, ERR_NOMEM = -1, -2, -3, -4, -5, -6, -7
 
 EXPORTED_SYMBOLS = [
     "pio_als_abi_version", "pio_als_device_count", "pio_als_nccl_unique_id", "pio_als_create",
@@ -42,7 +42,8 @@ EXPORTED_SYMBOLS = [
     "pio_eval_folds_rank_counts", "pio_eval_folds_destroy", "pio_cls_folds_create", "pio_cls_folds_sizes",
     "pio_cls_folds_classes", "pio_cls_folds_nb_train", "pio_cls_folds_rf_train", "pio_cls_folds_nb_predict",
     "pio_cls_folds_rf_predict", "pio_cls_folds_result_labels", "pio_cls_folds_result_counts",
-    "pio_cls_folds_result_free", "pio_cls_folds_destroy",
+    "pio_cls_folds_result_free", "pio_cls_folds_destroy", "pio_cooc_model_create", "pio_cooc_model_destroy",
+    "pio_cooc_predict_filtered", "pio_cooc_model_get_stats",
 ]
 
 
@@ -188,6 +189,12 @@ def lib():
         L.pio_events_index_lookup.restype = ci
         L.pio_events_index_lookup.argtypes = [vp, vp, vp, C.c_int32, i64, i64, vp, vp, vp, vp]
         L.pio_events_index_destroy.argtypes = [vp]
+        L.pio_cooc_model_create.restype = ci
+        L.pio_cooc_model_create.argtypes = [ci, C.c_int32, C.c_int32, vp, vp, vp, vp]
+        L.pio_cooc_model_destroy.argtypes = [vp]
+        L.pio_cooc_predict_filtered.restype = ci
+        L.pio_cooc_predict_filtered.argtypes = [vp, vp, vp, C.c_int32, C.c_int32, vp, vp, vp, vp]
+        L.pio_cooc_model_get_stats.argtypes = [vp, vp]
         for name in EXPORTED_SYMBOLS:
             getattr(L, name)  # AttributeError if the ABI is incomplete
         _lib = L
@@ -999,6 +1006,58 @@ def cooc_train(user, item, n_users, n_items, topn, device=0):
                                 C.c_int32(n_users), C.c_int32(n_items), C.c_int(topn), _ptr(oi, C.c_int32),
                                 _ptr(oc, C.c_int32), _ptr(on, C.c_int32)))
     return oi, oc, on
+
+
+class CoocStats(C.Structure):
+    _fields_ = [("kernel_launches", C.c_int64), ("last_expanded", C.c_int64), ("last_rows", C.c_int64),
+                ("last_budget", C.c_int64), ("last_parts", C.c_int32), ("last_max_part_queries", C.c_int32)]
+
+
+class CoocModel:
+    """pio_cooc_model: a trained co-occurrence model (cooc_train's three arrays) that scores batches of
+    CooccurrenceAlgorithm queries on `device`.  The arrays are checked and copied when it is created; the device copy is
+    made by the first predict_filtered."""
+
+    def __init__(self, top_items, top_counts, top_n, device: int = 0):
+        ti = np.ascontiguousarray(top_items, np.int32)
+        tc = np.ascontiguousarray(top_counts, np.int32)
+        tn = np.ascontiguousarray(top_n, np.int32)
+        if ti.ndim != 2 or tc.shape != ti.shape or tn.shape != (ti.shape[0],):
+            raise ValueError("top_items / top_counts must be [n_items, n] and top_n [n_items]")
+        self.n_items, self.topn = int(ti.shape[0]), int(ti.shape[1])
+        self._h = C.c_void_p()
+        _check(lib().pio_cooc_model_create(int(device), self.n_items, self.topn, ti.ctypes.data, tc.ctypes.data,
+                                           tn.ctypes.data, C.addressof(self._h)))
+
+    def close(self):
+        if self._h:
+            lib().pio_cooc_model_destroy(self._h)
+            self._h = C.c_void_p()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    def predict_filtered(self, q_lists, num: int, query_filter=None):
+        """q_lists: n item-index sequences; query_filter: QueryFilter with one entry per query, or None.  Returns
+        (items int32 [n, num], scores int64 [n, num], count int32 [n])."""
+        ptr, flat = _csr(q_lists, len(q_lists))
+        n = ptr.shape[0] - 1
+        oi = np.full((n, num), -1, np.int32)
+        os_ = np.zeros((n, num), np.int64)
+        oc = np.zeros(n, np.int32)
+        qf = None if query_filter is None else query_filter.struct(n, self.n_items)
+        _check(lib().pio_cooc_predict_filtered(self._h, ptr.ctypes.data, flat.ctypes.data, n, int(num),
+                                               None if qf is None else C.addressof(qf), oi.ctypes.data,
+                                               os_.ctypes.data, oc.ctypes.data))
+        return oi, os_, oc
+
+    def stats(self) -> dict:
+        st = CoocStats()
+        _check(lib().pio_cooc_model_get_stats(self._h, C.addressof(st)))
+        return {name: getattr(st, name) for name, _ in CoocStats._fields_}
 
 
 def nb_train(label, x, n_class, lam, device=0):

@@ -44,10 +44,11 @@ class CategoryIndex:
         return out.astype(np.uint8)
 
 
-def category_index(model) -> CategoryIndex:
-    """The CategoryIndex of a model (its `items` and `mf`), built on first use and kept on the model: a model's items do
-    not change after training, so nothing ever invalidates it."""
+def category_index(model, n_items: Optional[int] = None) -> CategoryIndex:
+    """The CategoryIndex of a model (its `items`, over n_items items; None: those of its `mf`), built on first use and
+    kept on the model: a model's items do not change after training, so nothing ever invalidates it."""
     ix: Optional[CategoryIndex] = getattr(model, "_category_index", None)
     if ix is None:
-        ix = model._category_index = CategoryIndex(len(model.mf.productHas), model.items)
+        n = len(model.mf.productHas) if n_items is None else n_items
+        ix = model._category_index = CategoryIndex(n, model.items)
     return ix

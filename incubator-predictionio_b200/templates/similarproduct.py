@@ -3,7 +3,7 @@ like/dislike events; Serving merges by standardised score).
 
 Mirrors examples/scala-parallel-similarproduct/multi-events-multi-algos/src/main/scala/:
   Engine.scala, DataSource.scala, Preparator.scala, ALSAlgorithm.scala:33-263, LikeAlgorithm.scala:37-115,
-  Serving.scala:29-69.  CooccurrenceAlgorithm is not ALS and is out of scope (SURVEY section 2 row 2).
+  Serving.scala:29-69, and CooccurrenceAlgorithm.scala:44-175.
 """
 from __future__ import annotations
 
@@ -373,16 +373,35 @@ class CooccurrenceAlgorithmParams(Params):
 
 class CooccurrenceModel:
     """topCooccurrences: item index -> [(other item index, count), ...] (CooccurrenceAlgorithm.scala:31-42); a plain local
-    model (P2LAlgorithm keeps it as is)."""
+    model (P2LAlgorithm keeps it as is).  predictMany scores on a device copy (native.CoocModel on the training device),
+    made on first use and kept out of the pickle, which holds the numpy arrays only."""
+
+    _CACHES = ("_device_model", "_category_index")
 
     def __init__(self, top_items: np.ndarray, top_counts: np.ndarray, top_n: np.ndarray, itemStringIntMap: BiMap,
-                 items: Dict[int, Item]):
+                 items: Dict[int, Item], device: int = 0):
         self.top_items, self.top_counts, self.top_n = top_items, top_counts, top_n
         self.itemStringIntMap, self.items = itemStringIntMap, items
         self.itemIntStringMap = itemStringIntMap.inverse
+        self.device = device
 
     def topCooccurrences(self, i: int):
         return [(int(self.top_items[i, t]), int(self.top_counts[i, t])) for t in range(int(self.top_n[i]))]
+
+    def device_model(self) -> "native.CoocModel":
+        d = self.__dict__.get("_device_model")
+        if d is None:
+            d = self._device_model = native.CoocModel(self.top_items, self.top_counts, self.top_n,
+                                                      getattr(self, "device", 0))
+        return d
+
+    def __getstate__(self):
+        return {k: v for k, v in self.__dict__.items() if k not in self._CACHES}
+
+    def __del__(self):
+        d = self.__dict__.get("_device_model")
+        if d is not None:
+            d.close()
 
 
 class CooccurrenceAlgorithm(P2LAlgorithm):
@@ -419,7 +438,7 @@ class CooccurrenceAlgorithm(P2LAlgorithm):
             ti = np.full((n_items, self.ap.n), -1, np.int32)
             tc = np.zeros((n_items, self.ap.n), np.int32)
             tn = np.zeros(n_items, np.int32)
-        return CooccurrenceModel(ti, tc, tn, itemMap, items)
+        return CooccurrenceModel(ti, tc, tn, itemMap, items, getattr(sc, "device", 0) or 0)
 
     def predict(self, model: CooccurrenceModel, query: Query) -> PredictedResult:
         queryList = {i for i in (model.itemStringIntMap.get(x) for x in query.items) if i is not None}
@@ -446,6 +465,50 @@ class CooccurrenceAlgorithm(P2LAlgorithm):
 
         top = sorted(((i, v) for i, v in counts.items() if candidate(i)), key=lambda kv: (-kv[1], kv[0]))[:query.num]
         return PredictedResult([ItemScore(model.itemIntStringMap(i), float(v)) for i, v in top])
+
+    def predictMany(self, model: CooccurrenceModel, queries) -> list:
+        """predict for many queries in one device call per batch (pio_cooc_predict_filtered).  A query's blackList is its
+        exclusion list, its whiteList its white list, and its categories one shared item_sets row per distinct value of
+        the batch, built from the model's CategoryIndex; categoryBlackList is not a rule of this algorithm."""
+        qs = list(queries)
+        out = [PredictedResult([]) for _ in qs]
+        sim = model.itemStringIntMap
+        rows, qlists = [], []
+        for j, q in enumerate(qs):
+            ql = {sim.get(x) for x in q.items}
+            ql.discard(None)
+            if not ql:
+                continue
+            if q.num < 1:
+                out[j] = self.predict(model, q)
+                continue
+            rows.append(j)
+            qlists.append(sorted(ql))
+        if not rows:
+            return out
+        ids = lambda xs: [i for i in (sim.get(x) for x in xs) if i is not None]   # noqa: E731
+        black = [None if qs[j].blackList is None else ids(qs[j].blackList) for j in rows]
+        white = [None if qs[j].whiteList is None else ids(qs[j].whiteList) for j in rows]
+        set_of, set_rows, set_ix = {}, [], np.full(len(rows), -1, np.int32)
+        for r, j in enumerate(rows):
+            cats = qs[j].categories
+            if cats is None:
+                continue
+            key = frozenset(cats)
+            if key not in set_of:
+                set_of[key] = len(set_rows)
+                set_rows.append(category_index(model, len(model.top_n)).excluded(cats, None))
+            set_ix[r] = set_of[key]
+        qf = native.QueryFilter(len(rows), black, white, set_ix if set_rows else None,
+                                np.stack(set_rows) if set_rows else None)
+        num = min(max(qs[j].num for j in rows), len(model.top_n))   # no query has more candidates than items
+        items, scores, cnt = model.device_model().predict_filtered(qlists, num, qf)
+        name = model.itemIntStringMap
+        for r, j in enumerate(rows):
+            n = min(int(cnt[r]), qs[j].num)
+            out[j] = PredictedResult([ItemScore(name(i), float(v))
+                                      for i, v in zip(items[r, :n].tolist(), scores[r, :n].tolist())])
+        return out
 
 
 class Serving(LServing):
