@@ -548,6 +548,31 @@ PIO_API int pio_cooc_predict_filtered(pio_cooc_model* m, const int64_t* q_ptr, c
                                       int32_t* out_items, int64_t* out_scores, int32_t* out_count);
 PIO_API int pio_cooc_model_get_stats(const pio_cooc_model* m, pio_cooc_stats* out);
 
+/* Default number of entries per part of a pio_serve_zscore_merge call (about 90 bytes of device memory each); the
+ * environment variable PIO_SERVE_MERGE_BUDGET (a positive integer) overrides it.  Results do not depend on it. */
+#define PIO_SERVE_MERGE_BUDGET (1ll << 24)
+
+/* The similarproduct template's Serving.serve (Serving.scala:29-69) over a batch of n_queries queries, on `device`
+ * (DESIGN.md 4.13).  For each of n_algos algorithms a, HOST arrays: items[a] (int32) and scores[a] (fp64), both
+ * n_queries x widths[a], and counts[a] (int32, n_queries): the first counts[a][j] entries of row j are query j's list,
+ * with item ids in one numbering [0, n_items).  num[j] is query j's num.  Per query j:
+ *   - unless num[j] == 1, each list of n entries is standardised: mean = sum / n (0 for n = 0), sd = sqrt(sum((s -
+ *     mean)^2) / (n - 1)) for n > 1 else 0, z = 0 where sd == 0 else (s - mean) / sd, with numpy's pairwise summation
+ *     started from 0.0 (np.add.reduce); with num[j] == 1 the scores are used as they are;
+ *   - the values are summed per item as 0.0 + z0 + z1 + ..., in algorithm order, then list order;
+ *   - the items are ordered by sum descending, equal sums in order of the item's first (algorithm, position), and cut
+ *     at min(num[j], topk).
+ * Row j of out_items (int32) / out_scores (fp64), n_queries x topk, best first, padded with -1 / 0; out_count[j] is the
+ * number of results.  Every operation is rounded as numpy and Python round it, so the results equal Serving.serve's bit
+ * for bit.  The batch runs in parts of consecutive queries whose entries (sums of counts) stay within
+ * PIO_SERVE_MERGE_BUDGET, at least one query per part.  Rejected with PIO_ALS_ERR_ARG before any device work: n_algos,
+ * n_items or topk below 1, a NULL array, a negative width, a count outside [0, widths[a]], an id outside [0, n_items), a
+ * score that is not finite, num[j] < 1, and a query with 2^32 entries or more.  Errors: pio_als_last_error(NULL). */
+PIO_API int pio_serve_zscore_merge(int device, int32_t n_queries, int32_t n_algos, int32_t n_items,
+                                   const int32_t* const* items, const double* const* scores,
+                                   const int32_t* const* counts, const int32_t* widths, const int32_t* num,
+                                   int32_t topk, int32_t* out_items, double* out_scores, int32_t* out_count);
+
 /* MLlib multinomial NaiveBayes (classification template). HOST buffers.
  * label: class index 0..n_class-1; x: n x n_feat, non-negative. pi: n_class, theta: n_class x n_feat
  * (fp64 log-probabilities, as MLlib's NaiveBayesModel.pi/theta). */

@@ -248,6 +248,9 @@ class LFirstServing(LServing):
     def serveColumns(self, queries, predictions):
         return predictions[0]
 
+    def serveManyColumns(self, queries, predictions):
+        return predictions[0]
+
 
 # ---- EngineParams / Engine ----------------------------------------------------------------------
 @dataclass

@@ -55,6 +55,7 @@
 #include "events_index.cuh"
 #include "cooc.cuh"
 #include "cooc_predict.cuh"
+#include "serve_merge.cuh"
 #include "forest.cuh"
 #include "eval_folds.cuh"
 #include "cls_folds.cuh"
@@ -4749,6 +4750,231 @@ int pio_cooc_model_get_stats(const pio_cooc_model* m, pio_cooc_stats* out) {
   if (!m || !out) return fail(nullptr, PIO_ALS_ERR_ARG, "null argument");
   std::lock_guard<std::mutex> lk(m->mu);
   *out = m->stats;
+  return PIO_ALS_OK;
+}
+
+}  // extern "C"
+
+// ---- z-score serving merge (similarproduct Serving.serve) ------------------------------------------------------------------
+namespace pio {
+
+// what the last pio_serve_zscore_merge on this thread did (pio_serve_merge_debug_stats)
+struct ServeMergeStats {
+  long long parts = 0, max_part_queries = 0, entries = 0, rows = 0, budget = 0;
+  double device_ms = 0.0;
+};
+static thread_local ServeMergeStats g_sm_stats;
+
+// The queries [j0, j1) of a call on stream st: rows j0 .. j1 - 1 of the caller's outputs.
+static int sm_part(cudaStream_t st, int n_algos, int n_items, const int32_t* const* items, const double* const* scores,
+                   const int32_t* const* counts, const int32_t* widths, const int32_t* num, int j0, int j1, int topk,
+                   int32_t* out_items, double* out_scores, int32_t* out_count) {
+  const int n = j1 - j0;
+  const long long NL = (long long)n * n_algos;
+  std::vector<uint32_t> h_cnt((size_t)NL), h_off((size_t)NL);
+  long long E = 0;
+  for (int q = 0; q < n; ++q)
+    for (int a = 0; a < n_algos; ++a) {
+      const size_t l = (size_t)q * n_algos + a;
+      h_cnt[l] = (uint32_t)counts[a][j0 + q];
+      h_off[l] = (uint32_t)E;
+      E += h_cnt[l];
+    }
+  Scratch tmp(st);
+  std::vector<const int*> h_items((size_t)n_algos, nullptr);
+  std::vector<const double*> h_scores((size_t)n_algos, nullptr);
+  for (int a = 0; a < n_algos; ++a) {
+    const size_t cells = (size_t)n * widths[a];
+    if (cells == 0) continue;
+    int* di = nullptr;
+    double* ds = nullptr;
+    CK0(tmp.alloc(&di, cells));
+    CK0(tmp.alloc(&ds, cells));
+    CK0(cudaMemcpyAsync(di, items[a] + (size_t)j0 * widths[a], sizeof(int) * cells, cudaMemcpyHostToDevice, st));
+    CK0(cudaMemcpyAsync(ds, scores[a] + (size_t)j0 * widths[a], sizeof(double) * cells, cudaMemcpyHostToDevice, st));
+    h_items[a] = di, h_scores[a] = ds;
+  }
+  const int** d_items = nullptr;
+  const double** d_scores = nullptr;
+  int *d_w = nullptr, *d_num = nullptr;
+  uint32_t *d_cnt = nullptr, *d_off = nullptr;
+  double *d_mean = nullptr, *d_sd = nullptr;
+  CK0(tmp.alloc(&d_items, (size_t)n_algos));
+  CK0(tmp.alloc(&d_scores, (size_t)n_algos));
+  CK0(tmp.alloc(&d_w, (size_t)n_algos));
+  CK0(tmp.alloc(&d_num, (size_t)n));
+  CK0(tmp.alloc(&d_cnt, (size_t)NL));
+  CK0(tmp.alloc(&d_off, (size_t)NL));
+  CK0(tmp.alloc(&d_mean, (size_t)NL));
+  CK0(tmp.alloc(&d_sd, (size_t)NL));
+  CK0(cudaMemcpyAsync(d_items, h_items.data(), sizeof(int*) * n_algos, cudaMemcpyHostToDevice, st));
+  CK0(cudaMemcpyAsync(d_scores, h_scores.data(), sizeof(double*) * n_algos, cudaMemcpyHostToDevice, st));
+  CK0(cudaMemcpyAsync(d_w, widths, sizeof(int) * n_algos, cudaMemcpyHostToDevice, st));
+  CK0(cudaMemcpyAsync(d_num, num + j0, sizeof(int) * n, cudaMemcpyHostToDevice, st));
+  CK0(cudaMemcpyAsync(d_cnt, h_cnt.data(), sizeof(uint32_t) * NL, cudaMemcpyHostToDevice, st));
+  CK0(cudaMemcpyAsync(d_off, h_off.data(), sizeof(uint32_t) * NL, cudaMemcpyHostToDevice, st));
+  const MergeLists L{d_items, d_scores, d_w, n_algos};
+  sm_stats_kernel<<<nblk(NL, 128), 128, 0, st>>>(L, d_cnt, NL, d_num, d_mean, d_sd);
+  CK0(cudaGetLastError());
+  const int bits_q = ceil_log2((uint64_t)n), bits_i = ceil_log2((uint64_t)n_items);
+  SortBufs sb;
+  uint64_t* row_key = nullptr;
+  double* row_sum = nullptr;
+  long long R = 0;
+  if (E > 0) {
+    for (int b = 0; b < 2; ++b) {
+      CK0(tmp.alloc(&sb.k[b], (size_t)E));
+      CK0(tmp.alloc(&sb.v[b], (size_t)E));
+    }
+    double *z = nullptr, *head_sum = nullptr;
+    uint64_t* head_key = nullptr;
+    uint32_t *head = nullptr, *pos = nullptr;
+    CK0(tmp.alloc(&z, (size_t)E));
+    CK0(tmp.alloc(&head_sum, (size_t)E));
+    CK0(tmp.alloc(&head_key, (size_t)E));
+    CK0(tmp.alloc(&head, (size_t)E));
+    CK0(tmp.alloc(&pos, (size_t)E));
+    CK0(cudaMemsetAsync(head, 0, sizeof(uint32_t) * E, st));
+    sm_entries_kernel<<<(unsigned)std::min<long long>(nblk(NL * 32, 256), 132 * 64), 256, 0, st>>>(
+        L, d_cnt, d_off, NL, d_mean, d_sd, bits_i, sb.keys(), sb.vals(), z);
+    CK0(cudaGetLastError());
+    CK0(radix_sort_pairs(sb, (size_t)E, bits_q + bits_i, st, nullptr));
+    sm_sum_kernel<<<nblk(E, 256), 256, 0, st>>>(sb.keys(), sb.vals(), E, z, head, head_key, head_sum);
+    CK0(cudaGetLastError());
+    CK0(scan_exclusive_u32(head, pos, (size_t)E, st, nullptr));
+    uint32_t last[2] = {0, 0};
+    CK0(cudaMemcpyAsync(&last[0], pos + E - 1, 4, cudaMemcpyDeviceToHost, st));
+    CK0(cudaMemcpyAsync(&last[1], head + E - 1, 4, cudaMemcpyDeviceToHost, st));
+    CK0(cudaStreamSynchronize(st));
+    R = (long long)last[0] + last[1];
+    CK0(tmp.alloc(&row_key, (size_t)R));
+    CK0(tmp.alloc(&row_sum, (size_t)R));
+    sm_rows_kernel<<<nblk(E, 256), 256, 0, st>>>(head, pos, E, head_key, head_sum, row_key, row_sum, sb.spare_keys(),
+                                                 sb.spare_vals());
+    CK0(cudaGetLastError());
+    sb.flip();
+    // stable LSD: by sum descending, then by query; rows enter in (query, first appearance) order, so equal sums keep it
+    CK0(radix_sort_pairs(sb, (size_t)R, 64, st, nullptr));
+    sm_query_keys_kernel<<<nblk(R, 256), 256, 0, st>>>(sb.vals(), R, row_key, bits_i, sb.spare_keys(), sb.spare_vals());
+    CK0(cudaGetLastError());
+    sb.flip();
+    CK0(radix_sort_pairs(sb, (size_t)R, bits_q, st, nullptr));
+  }
+  int* d_oi = nullptr;
+  double* d_os = nullptr;
+  int* d_oc = nullptr;
+  CK0(tmp.alloc(&d_oi, (size_t)n * topk));
+  CK0(tmp.alloc(&d_os, (size_t)n * topk));
+  CK0(tmp.alloc(&d_oc, (size_t)n));
+  sm_take_kernel<<<n, 128, 0, st>>>(sb.keys(), sb.vals(), R, topk, d_num, row_key, bits_i, row_sum, d_oi, d_os, d_oc);
+  CK0(cudaGetLastError());
+  CK0(cudaMemcpyAsync(out_items + (size_t)j0 * topk, d_oi, sizeof(int) * (size_t)n * topk, cudaMemcpyDeviceToHost, st));
+  CK0(cudaMemcpyAsync(out_scores + (size_t)j0 * topk, d_os, sizeof(double) * (size_t)n * topk, cudaMemcpyDeviceToHost,
+                      st));
+  CK0(cudaMemcpyAsync(out_count + j0, d_oc, sizeof(int) * (size_t)n, cudaMemcpyDeviceToHost, st));
+  CK0(cudaStreamSynchronize(st));
+  g_sm_stats.entries += E;
+  g_sm_stats.rows += R;
+  return PIO_ALS_OK;
+}
+
+static int serve_zscore_merge(int device, int32_t n_queries, int32_t n_algos, int32_t n_items,
+                              const int32_t* const* items, const double* const* scores, const int32_t* const* counts,
+                              const int32_t* widths, const int32_t* num, int32_t topk, int32_t* out_items,
+                              double* out_scores, int32_t* out_count) {
+  g_sm_stats = ServeMergeStats{};
+  if (n_queries < 0 || n_algos < 1 || n_items < 1 || topk < 1)
+    return fail(nullptr, PIO_ALS_ERR_ARG, "n_queries must be >= 0, n_algos, n_items and topk >= 1");
+  if (n_queries == 0) return PIO_ALS_OK;
+  if (!items || !scores || !counts || !widths || !num || !out_items || !out_scores || !out_count)
+    return fail(nullptr, PIO_ALS_ERR_ARG, "null argument");
+  for (int a = 0; a < n_algos; ++a) {
+    if (widths[a] < 0) return fail(nullptr, PIO_ALS_ERR_ARG, "algorithm %d: width %d is negative", a, widths[a]);
+    if (!counts[a] || (widths[a] > 0 && (!items[a] || !scores[a])))
+      return fail(nullptr, PIO_ALS_ERR_ARG, "algorithm %d: null items, scores or counts", a);
+  }
+  // every query's lists: counts within the widths, ids in the numbering, finite scores; entries per query under 2^32
+  std::vector<unsigned long long> ent((size_t)n_queries, 0);
+  for (int j = 0; j < n_queries; ++j) {
+    if (num[j] < 1) return fail(nullptr, PIO_ALS_ERR_ARG, "query %d: num %d is below 1", j, num[j]);
+    for (int a = 0; a < n_algos; ++a) {
+      const int32_t c = counts[a][j];
+      if (c < 0 || c > widths[a])
+        return fail(nullptr, PIO_ALS_ERR_ARG, "query %d, algorithm %d: count %d is outside [0, %d]", j, a, c, widths[a]);
+      const size_t row = (size_t)j * widths[a];
+      for (int32_t t = 0; t < c; ++t) {
+        if (items[a][row + t] < 0 || items[a][row + t] >= n_items)
+          return fail(nullptr, PIO_ALS_ERR_ARG, "query %d, algorithm %d, entry %d: item %d is outside [0, %d)", j, a, t,
+                      items[a][row + t], n_items);
+        if (!isfinite(scores[a][row + t]))
+          return fail(nullptr, PIO_ALS_ERR_ARG, "query %d, algorithm %d, entry %d: the score is not finite", j, a, t);
+      }
+      ent[j] += (unsigned)c;
+    }
+    if (ent[j] >= (1ull << 32))
+      return fail(nullptr, PIO_ALS_ERR_ARG, "query %d has %llu entries: at most 2^32 - 1 fit one part", j, ent[j]);
+  }
+  // PIO_SERVE_MERGE_BUDGET: entries per part; capped so that a part's offsets fit the 32-bit scan
+  const char* env_b = getenv("PIO_SERVE_MERGE_BUDGET");
+  const long long budget = std::min<long long>(env_b && atoll(env_b) > 0 ? atoll(env_b) : PIO_SERVE_MERGE_BUDGET,
+                                               (1ll << 32) - 1);
+  std::vector<int> first;
+  long long acc = 0;
+  for (int j = 0; j < n_queries; ++j) {
+    if (j == 0 || acc + (long long)ent[j] > budget) {
+      first.push_back(j);
+      acc = 0;
+    }
+    acc += (long long)ent[j];
+  }
+  first.push_back(n_queries);
+  g_sm_stats.budget = budget;
+  CK0(cudaSetDevice(device));
+  CallMem mem;
+  cudaStream_t st = nullptr;
+  cudaEvent_t t0 = nullptr, t1 = nullptr;
+  CK0(mem.stream(&st));
+  CK0(mem.event(&t0));
+  CK0(mem.event(&t1));
+  CK0(cudaEventRecord(t0, st));
+  for (size_t p = 0; p + 1 < first.size(); ++p) {
+    g_sm_stats.parts = (long long)p + 1;
+    g_sm_stats.max_part_queries = std::max<long long>(g_sm_stats.max_part_queries, first[p + 1] - first[p]);
+    const int rc = sm_part(st, n_algos, n_items, items, scores, counts, widths, num, first[p], first[p + 1], topk,
+                           out_items, out_scores, out_count);
+    if (rc) return rc;
+  }
+  CK0(cudaEventRecord(t1, st));
+  CK0(cudaEventSynchronize(t1));
+  float ms = 0.f;
+  CK0(cudaEventElapsedTime(&ms, t0, t1));
+  g_sm_stats.device_ms = ms;
+  return PIO_ALS_OK;
+}
+
+}  // namespace pio
+
+extern "C" {
+
+int pio_serve_zscore_merge(int device, int32_t n_queries, int32_t n_algos, int32_t n_items, const int32_t* const* items,
+                           const double* const* scores, const int32_t* const* counts, const int32_t* widths,
+                           const int32_t* num, int32_t topk, int32_t* out_items, double* out_scores, int32_t* out_count) {
+  try {   // bad_alloc must not cross the C boundary; Scratch and CallMem release device memory on the way out
+    return serve_zscore_merge(device, n_queries, n_algos, n_items, items, scores, counts, widths, num, topk, out_items,
+                              out_scores, out_count);
+  } catch (const std::bad_alloc&) {
+    return fail(nullptr, PIO_ALS_ERR_NOMEM, "pio_serve_zscore_merge: out of host memory");
+  }
+}
+
+/* debug only (not in pio_als.h): out[0] parts, out[1] most queries in one part, out[2] entries, out[3] distinct (query,
+ * item) rows, out[4] the entries budget, out[5] device milliseconds from the first upload to the last copy back -- of the
+ * last pio_serve_zscore_merge on this thread.  Used by the tests and tools/serve_merge_bench.py. */
+__attribute__((visibility("default"))) int pio_serve_merge_debug_stats(double out[6]) {
+  if (!out) return PIO_ALS_ERR_ARG;
+  const ServeMergeStats& s = g_sm_stats;
+  out[0] = (double)s.parts, out[1] = (double)s.max_part_queries, out[2] = (double)s.entries, out[3] = (double)s.rows;
+  out[4] = (double)s.budget, out[5] = s.device_ms;
   return PIO_ALS_OK;
 }
 

@@ -10,7 +10,9 @@ from __future__ import annotations
 import ctypes as C
 import os
 import subprocess
+from dataclasses import dataclass, field
 from pathlib import Path
+from typing import Any, Dict, List, Optional, Sequence
 
 import numpy as np
 
@@ -43,7 +45,7 @@ EXPORTED_SYMBOLS = [
     "pio_cls_folds_classes", "pio_cls_folds_nb_train", "pio_cls_folds_rf_train", "pio_cls_folds_nb_predict",
     "pio_cls_folds_rf_predict", "pio_cls_folds_result_labels", "pio_cls_folds_result_counts",
     "pio_cls_folds_result_free", "pio_cls_folds_destroy", "pio_cooc_model_create", "pio_cooc_model_destroy",
-    "pio_cooc_predict_filtered", "pio_cooc_model_get_stats",
+    "pio_cooc_predict_filtered", "pio_cooc_model_get_stats", "pio_serve_zscore_merge",
 ]
 
 
@@ -195,6 +197,9 @@ def lib():
         L.pio_cooc_predict_filtered.restype = ci
         L.pio_cooc_predict_filtered.argtypes = [vp, vp, vp, C.c_int32, C.c_int32, vp, vp, vp, vp]
         L.pio_cooc_model_get_stats.argtypes = [vp, vp]
+        L.pio_serve_zscore_merge.restype = ci
+        L.pio_serve_zscore_merge.argtypes = [ci, C.c_int32, C.c_int32, C.c_int32, vp, vp, vp, vp, vp, C.c_int32, vp, vp,
+                                             vp]
         for name in EXPORTED_SYMBOLS:
             getattr(L, name)  # AttributeError if the ABI is incomplete
         _lib = L
@@ -1058,6 +1063,61 @@ class CoocModel:
         st = CoocStats()
         _check(lib().pio_cooc_model_get_stats(self._h, C.addressof(st)))
         return {name: getattr(st, name) for name, _ in CoocStats._fields_}
+
+
+@dataclass
+class ScoredColumns:
+    """A batch of ranked results as arrays: row j holds query j's first count[j] (item id, score) pairs, best first,
+    padded with -1 / 0, and names[id] is the item string of an id.  The rows of the queries in `objects` are not used:
+    those queries' results are given there as the result objects of predict (or, once served, of serve).  device: the
+    GPU whose model computed them, or None."""
+    items: np.ndarray                 # int32 [Q, w]
+    scores: np.ndarray                # float64 [Q, w]
+    count: np.ndarray                 # int32 [Q]
+    names: Sequence[str]
+    objects: Dict[int, Any] = field(default_factory=dict)
+    device: Optional[int] = None
+
+
+def item_names(string_int) -> List[str]:
+    """The item strings of a string -> index map whose indices are 0 .. size - 1, in index order."""
+    names = [None] * len(string_int)
+    for s, i in string_int.toSeq():
+        names[i] = s
+    return names
+
+
+def serve_zscore_merge(items, scores, counts, num, topk: int, n_items: int, device: int = 0):
+    """pio_serve_zscore_merge: per algorithm a, items[a] int32 [Q, w_a], scores[a] float64 [Q, w_a] and counts[a] [Q],
+    ids in [0, n_items); num [Q] >= 1.  Returns (items int32 [Q, topk], scores float64 [Q, topk], count int32 [Q])."""
+    its = [np.ascontiguousarray(x, np.int32) for x in items]
+    scs = [np.ascontiguousarray(x, np.float64) for x in scores]
+    cns = [np.ascontiguousarray(c, np.int32) for c in counts]
+    num = np.ascontiguousarray(num, np.int32)
+    n, k = num.shape[0], len(its)
+    if not (len(scs) == len(cns) == k) or any(x.ndim != 2 or x.shape[0] != n or s.shape != x.shape or c.shape != (n,)
+                                              for x, s, c in zip(its, scs, cns)):
+        raise ValueError("items / scores must be [n_queries, w] and counts [n_queries] for every algorithm")
+    widths = np.array([x.shape[1] for x in its], np.int32)
+    arr = lambda xs: (C.c_void_p * max(k, 1))(*[x.ctypes.data for x in xs])   # noqa: E731
+    pi, ps, pc = arr(its), arr(scs), arr(cns)
+    oi = np.full((n, topk), -1, np.int32)
+    os_ = np.zeros((n, topk), np.float64)
+    oc = np.zeros(n, np.int32)
+    _check(lib().pio_serve_zscore_merge(int(device), n, k, int(n_items), C.addressof(pi), C.addressof(ps),
+                                        C.addressof(pc), widths.ctypes.data, num.ctypes.data, int(topk), oi.ctypes.data,
+                                        os_.ctypes.data, oc.ctypes.data))
+    return oi, os_, oc
+
+
+def serve_merge_stats() -> dict:
+    """What the last serve_zscore_merge on this thread did: its parts, the most queries in one part, its entries and
+    distinct (query, item) rows, the entries budget, and the device milliseconds from the first upload to the last copy
+    back."""
+    out = (C.c_double * 6)()
+    _check(lib().pio_serve_merge_debug_stats(out))
+    return {"parts": int(out[0]), "max_part_queries": int(out[1]), "entries": int(out[2]), "rows": int(out[3]),
+            "budget": int(out[4]), "device_ms": out[5]}
 
 
 def nb_train(label, x, n_class, lam, device=0):

@@ -322,27 +322,56 @@ class ALSAlgorithm(PAlgorithm):
         rs = model.recommendProductsWithFilter(userInt, query.num, [b for b in blackList if b is not None])
         return PredictedResult([ItemScore(inv(r.product), r.rating) for r in rs])
 
+    def _many(self, model: ALSModel, qs):
+        """predictMany up to its device call: (rows, (items, scores, cnt) or None, objects).  Row r of the arrays is query
+        qs[rows[r]]; objects maps each query of a known user with num < 1 to predict's result."""
+        rows = [j for j, q in enumerate(qs) if q.num >= 1 and model.userStringIntMap.get(q.user) is not None]
+        objects = {j: self.predict(model, q) for j, q in enumerate(qs)
+                   if q.num < 1 and model.userStringIntMap.get(q.user) is not None}
+        if not rows:
+            return rows, None, objects
+        users = np.array([model.userStringIntMap.get(qs[j].user) for j in rows], np.int32)
+        black = [[b for b in (model.itemStringIntMap.get(x) for x in (qs[j].blackList or ())) if b is not None]
+                 for j in rows]
+        num = max(qs[j].num for j in rows)
+        return rows, model.recommendProductsForUsers(users, num, query_filter=native.QueryFilter(len(rows), black)), objects
+
     def predictMany(self, model: ALSModel, queries) -> list:
         """predict for many queries in one filtered batch call: each known user is scored with its own black list
         (native.QueryFilter exclusion lists) for the largest `num` of the batch; a query keeps its first `num`."""
         qs = list(queries)
         out = [PredictedResult([]) for _ in qs]
-        rows = [j for j, q in enumerate(qs) if q.num >= 1 and model.userStringIntMap.get(q.user) is not None]
-        for j, q in enumerate(qs):
-            if q.num < 1 and model.userStringIntMap.get(q.user) is not None:
-                out[j] = self.predict(model, q)
+        rows, res, objects = self._many(model, qs)
+        for j, p in objects.items():
+            out[j] = p
         if not rows:
             return out
         inv = model.itemStringIntMap.inverse
-        users = np.array([model.userStringIntMap.get(qs[j].user) for j in rows], np.int32)
-        black = [[b for b in (model.itemStringIntMap.get(x) for x in (qs[j].blackList or ())) if b is not None]
-                 for j in rows]
-        num = max(qs[j].num for j in rows)
-        items, scores, cnt = model.recommendProductsForUsers(users, num, query_filter=native.QueryFilter(len(rows), black))
+        items, scores, cnt = res
         for r, j in enumerate(rows):
             n = min(int(cnt[r]), qs[j].num)
             out[j] = PredictedResult([ItemScore(inv(int(items[r, t])), float(scores[r, t])) for t in range(n)])
         return out
+
+    def predictManyColumns(self, model: ALSModel, queries) -> native.ScoredColumns:
+        """predictMany as columns, before any result object is built: the same device call, each row cut at its
+        query's num, the float32 scores widened to float64 (as float() does)."""
+        qs = list(queries)
+        rows, res, objects = self._many(model, qs)
+        n, w = len(qs), (res[0].shape[1] if rows else 0)
+        items = np.full((n, w), -1, np.int32)
+        scores = np.zeros((n, w), np.float64)
+        count = np.zeros(n, np.int32)
+        if rows:
+            r = np.asarray(rows, np.int64)
+            count[r] = np.minimum(res[2], np.array([qs[j].num for j in rows], np.int64))
+            keep = np.arange(w) < count[r][:, None]
+            items[r] = np.where(keep, res[0], -1)
+            scores[r] = np.where(keep, res[1].astype(np.float64), 0.0)
+        names = model.__dict__.get("_item_names")
+        if names is None:
+            names = model._item_names = native.item_names(model.itemStringIntMap)
+        return native.ScoredColumns(items, scores, count, names, objects)
 
     def batchPredict(self, model: ALSModel, queries):
         """One batched GPU top-N instead of cartesian + groupBy (ALSAlgorithm.scala:117-158)."""
@@ -379,6 +408,9 @@ class Serving(LServing):
 
     def serveColumns(self, queries, predictedResults):
         return predictedResults[0]
+
+    def serveManyColumns(self, queries, predictions):
+        return predictions[0]
 
 
 class RecommendationEngine(EngineFactory):

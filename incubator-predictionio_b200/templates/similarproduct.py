@@ -280,26 +280,23 @@ class ALSAlgorithm(P2LAlgorithm):
         items, scores, cnt = model.mf.similarProducts(sorted(queryList), query.num, mask)
         return PredictedResult([ItemScore(model.itemIntStringMap(int(items[t])), float(scores[t])) for t in range(cnt)])
 
-    def predictMany(self, model: ALSModel, queries) -> list:
-        """predict for many queries in one filtered batch call.  A query's blackList is its exclusion list, its
-        whiteList its white list, and its category rules one shared item_sets row per distinct (categories,
-        categoryBlackList) pair of the batch, built from the model's CategoryIndex."""
-        qs = list(queries)
-        out = [PredictedResult([]) for _ in qs]
+    def _many(self, model: ALSModel, qs):
+        """predictMany up to its device call: (rows, (items, scores, cnt) or None, objects).  Row r of the arrays is query
+        qs[rows[r]]; objects maps each query with known items and num < 1 to predict's result."""
         sim = model.itemStringIntMap
-        rows, qlists = [], []
+        rows, qlists, objects = [], [], {}
         for j, q in enumerate(qs):
             ql = {sim.get(x) for x in q.items}
             ql.discard(None)
             if not ql:
                 continue
             if q.num < 1:
-                out[j] = self.predict(model, q)
+                objects[j] = self.predict(model, q)
                 continue
             rows.append(j)
             qlists.append(sorted(ql))
         if not rows:
-            return out
+            return rows, None, objects
         ids = lambda xs: [i for i in (sim.get(x) for x in xs) if i is not None]   # noqa: E731
         black = [None if qs[j].blackList is None else ids(qs[j].blackList) for j in rows]
         white = [None if qs[j].whiteList is None else ids(qs[j].whiteList) for j in rows]
@@ -317,12 +314,22 @@ class ALSAlgorithm(P2LAlgorithm):
         qf = native.QueryFilter(len(rows), black, white, set_ix if set_rows else None,
                                 np.stack(set_rows) if set_rows else None)
         num = max(qs[j].num for j in rows)
-        items, scores, cnt = model.mf.similarProductsBatch(qlists, num, query_filter=qf)
-        for r, j in enumerate(rows):
-            n = min(int(cnt[r]), qs[j].num)
-            out[j] = PredictedResult([ItemScore(model.itemIntStringMap(int(items[r, t])), float(scores[r, t]))
-                                      for t in range(n)])
-        return out
+        return rows, model.mf.similarProductsBatch(qlists, num, query_filter=qf), objects
+
+    def predictMany(self, model: ALSModel, queries) -> list:
+        """predict for many queries in one filtered batch call.  A query's blackList is its exclusion list, its
+        whiteList its white list, and its category rules one shared item_sets row per distinct (categories,
+        categoryBlackList) pair of the batch, built from the model's CategoryIndex."""
+        qs = list(queries)
+        rows, res, objects = self._many(model, qs)
+        return _results(qs, rows, res, objects, model.itemIntStringMap)
+
+    def predictManyColumns(self, model: ALSModel, queries) -> native.ScoredColumns:
+        """predictMany as columns, before any result object is built: the same device call, each row cut at its
+        query's num, the float32 scores widened to float64 (as float() does)."""
+        qs = list(queries)
+        rows, res, objects = self._many(model, qs)
+        return _scored_columns(qs, rows, res, objects, model, None)
 
 
 class LikeAlgorithm(ALSAlgorithm):
@@ -376,7 +383,7 @@ class CooccurrenceModel:
     model (P2LAlgorithm keeps it as is).  predictMany scores on a device copy (native.CoocModel on the training device),
     made on first use and kept out of the pickle, which holds the numpy arrays only."""
 
-    _CACHES = ("_device_model", "_category_index")
+    _CACHES = ("_device_model", "_category_index", "_item_names")
 
     def __init__(self, top_items: np.ndarray, top_counts: np.ndarray, top_n: np.ndarray, itemStringIntMap: BiMap,
                  items: Dict[int, Item], device: int = 0):
@@ -466,26 +473,22 @@ class CooccurrenceAlgorithm(P2LAlgorithm):
         top = sorted(((i, v) for i, v in counts.items() if candidate(i)), key=lambda kv: (-kv[1], kv[0]))[:query.num]
         return PredictedResult([ItemScore(model.itemIntStringMap(i), float(v)) for i, v in top])
 
-    def predictMany(self, model: CooccurrenceModel, queries) -> list:
-        """predict for many queries in one device call per batch (pio_cooc_predict_filtered).  A query's blackList is its
-        exclusion list, its whiteList its white list, and its categories one shared item_sets row per distinct value of
-        the batch, built from the model's CategoryIndex; categoryBlackList is not a rule of this algorithm."""
-        qs = list(queries)
-        out = [PredictedResult([]) for _ in qs]
+    def _many(self, model: CooccurrenceModel, qs):
+        """predictMany up to its device call: (rows, (items, scores, cnt) or None, objects), as ALSAlgorithm._many."""
         sim = model.itemStringIntMap
-        rows, qlists = [], []
+        rows, qlists, objects = [], [], {}
         for j, q in enumerate(qs):
             ql = {sim.get(x) for x in q.items}
             ql.discard(None)
             if not ql:
                 continue
             if q.num < 1:
-                out[j] = self.predict(model, q)
+                objects[j] = self.predict(model, q)
                 continue
             rows.append(j)
             qlists.append(sorted(ql))
         if not rows:
-            return out
+            return rows, None, objects
         ids = lambda xs: [i for i in (sim.get(x) for x in xs) if i is not None]   # noqa: E731
         black = [None if qs[j].blackList is None else ids(qs[j].blackList) for j in rows]
         white = [None if qs[j].whiteList is None else ids(qs[j].whiteList) for j in rows]
@@ -502,13 +505,61 @@ class CooccurrenceAlgorithm(P2LAlgorithm):
         qf = native.QueryFilter(len(rows), black, white, set_ix if set_rows else None,
                                 np.stack(set_rows) if set_rows else None)
         num = min(max(qs[j].num for j in rows), len(model.top_n))   # no query has more candidates than items
-        items, scores, cnt = model.device_model().predict_filtered(qlists, num, qf)
-        name = model.itemIntStringMap
+        return rows, model.device_model().predict_filtered(qlists, num, qf), objects
+
+    def predictMany(self, model: CooccurrenceModel, queries) -> list:
+        """predict for many queries in one device call per batch (pio_cooc_predict_filtered).  A query's blackList is its
+        exclusion list, its whiteList its white list, and its categories one shared item_sets row per distinct value of
+        the batch, built from the model's CategoryIndex; categoryBlackList is not a rule of this algorithm."""
+        qs = list(queries)
+        rows, res, objects = self._many(model, qs)
+        return _results(qs, rows, res, objects, model.itemIntStringMap)
+
+    def predictManyColumns(self, model: CooccurrenceModel, queries) -> native.ScoredColumns:
+        """predictMany as columns, before any result object is built: the same device call, each row cut at its
+        query's num, the int64 sums rounded to float64 as float() rounds them."""
+        qs = list(queries)
+        rows, res, objects = self._many(model, qs)
+        return _scored_columns(qs, rows, res, objects, model, getattr(model, "device", 0))
+
+
+def _results(qs, rows, res, objects, name) -> List[PredictedResult]:
+    """The PredictedResult of every query: objects[j], or row r of the arrays res cut at its num, or empty."""
+    out = [PredictedResult([]) for _ in qs]
+    for j, p in objects.items():
+        out[j] = p
+    if rows:
+        items, scores, cnt = res
         for r, j in enumerate(rows):
             n = min(int(cnt[r]), qs[j].num)
             out[j] = PredictedResult([ItemScore(name(i), float(v))
                                       for i, v in zip(items[r, :n].tolist(), scores[r, :n].tolist())])
-        return out
+    return out
+
+
+def _item_names(model) -> List[str]:
+    """The model's item strings by index, built once per model."""
+    names = model.__dict__.get("_item_names")
+    if names is None:
+        names = model._item_names = native.item_names(model.itemStringIntMap)
+    return names
+
+
+def _scored_columns(qs, rows, res, objects, model, device) -> native.ScoredColumns:
+    """ScoredColumns of a batch: row rows[r] holds row r of res, cut at its query's num and padded with -1 / 0, its
+    scores as float64; every other row is empty."""
+    n = len(qs)
+    w = res[0].shape[1] if rows else 0
+    items = np.full((n, w), -1, np.int32)
+    scores = np.zeros((n, w), np.float64)
+    count = np.zeros(n, np.int32)
+    if rows:
+        r = np.asarray(rows, np.int64)
+        count[r] = np.minimum(res[2], np.array([qs[j].num for j in rows], np.int64))
+        keep = np.arange(w) < count[r][:, None]
+        items[r] = np.where(keep, res[0], -1)
+        scores[r] = np.where(keep, res[1].astype(np.float64), 0.0)
+    return native.ScoredColumns(items, scores, count, _item_names(model), dict(objects), device)
 
 
 class Serving(LServing):
@@ -531,6 +582,64 @@ class Serving(LServing):
                 comb[x.item] = comb.get(x.item, 0.0) + x.score
         top = sorted(comb.items(), key=lambda kv: -kv[1])[:query.num]
         return PredictedResult([ItemScore(k, v) for k, v in top])
+
+    def serveManyColumns(self, queries, predictions) -> native.ScoredColumns:
+        """serve for a batch, from the algorithms' ScoredColumns (predictManyColumns): every algorithm's ids mapped into
+        one item numbering, then the z-score merge on the GPU (pio_serve_zscore_merge), which equals serve bit for bit.
+        Queries with num < 1, queries an algorithm answered with objects, and queries with a score that is not finite
+        go through serve and are returned in `objects`."""
+        qs = list(queries)
+        n = len(qs)
+        names, remaps = self._numbering([p.names for p in predictions])
+        num = np.array([q.num for q in qs], np.int64)
+        host = num < 1
+        for p in predictions:
+            host |= ~np.isfinite(p.scores).all(axis=1)
+            host[list(p.objects)] = True
+        sel = np.flatnonzero(~host)
+        width = sum(p.items.shape[1] for p in predictions)
+        topk = int(min(num[sel].max(), width)) if sel.size else 0
+        items = np.full((n, topk), -1, np.int32)
+        scores = np.zeros((n, topk), np.float64)
+        count = np.zeros(n, np.int32)
+        if sel.size and topk:
+            its = [p.items[sel] if r is None else np.where(p.items[sel] >= 0, r[np.maximum(p.items[sel], 0)], -1)
+                   for p, r in zip(predictions, remaps)]
+            device = next((p.device for p in predictions if p.device is not None), 0)
+            items[sel], scores[sel], count[sel] = native.serve_zscore_merge(
+                its, [p.scores[sel] for p in predictions], [p.count[sel] for p in predictions], num[sel], topk,
+                max(len(names), 1), device)
+        objects = {}
+        for j in np.flatnonzero(host).tolist():
+            objects[j] = self.serve(qs[j], [p.objects[j] if j in p.objects else PredictedResult(
+                [ItemScore(p.names[i], v) for i, v in zip(p.items[j, :p.count[j]].tolist(),
+                                                           p.scores[j, :p.count[j]].tolist())])
+                for p in predictions])
+        return native.ScoredColumns(items, scores, count, names, objects)
+
+    def _numbering(self, name_lists):
+        """(names, remaps): one item numbering over the algorithms' models -- the union of their item maps, the first
+        model's ids first -- and per model the array taking its ids there, or None where they are the same ids (always
+        so when the maps are equal, as when the models train from the same columns).  Kept for the models of the last
+        call."""
+        cached = self.__dict__.get("_item_numbering")
+        if cached is not None and len(cached[0]) == len(name_lists) and all(a is b for a, b in zip(cached[0], name_lists)):
+            return cached[1], cached[2]
+        names = name_lists[0]
+        remaps = [None] * len(name_lists)
+        if not all(nl is names or nl == names for nl in name_lists):
+            names = list(names)
+            index = {s: i for i, s in enumerate(names)}
+            for k, nl in enumerate(name_lists):
+                r = np.empty(len(nl), np.int32)
+                for i, s in enumerate(nl):
+                    if s not in index:
+                        index[s] = len(names)
+                        names.append(s)
+                    r[i] = index[s]
+                remaps[k] = None if np.array_equal(r, np.arange(len(nl))) else r
+        self._item_numbering = (list(name_lists), names, remaps)
+        return names, remaps
 
 
 class SimilarProductEngine(EngineFactory):

@@ -21,6 +21,7 @@ import datetime as _dt
 import importlib
 import json
 import logging
+import math
 import os
 import pickle
 import sys
@@ -351,6 +352,11 @@ def to_json(x):
     return x
 
 
+def _float_json(v: float) -> str:
+    """A float as json.dumps writes it."""
+    return repr(v) if math.isfinite(v) else json.dumps(v)
+
+
 def deploy(engineInstanceId: Optional[str] = None, engineId: str = "", engineVersion: str = "",
            engineVariant: str = "default") -> QueryServer:
     inst = EngineInstances.get(engineInstanceId) if engineInstanceId else \
@@ -419,6 +425,46 @@ class BatchPredict:
                 yield {"query": to_json(q), "prediction": to_json(r)}   # the extracted Query, as the reference writes it
 
     @staticmethod
+    def columnar(server: "QueryServer") -> bool:
+        """Every algorithm scores batches as columns (predictManyColumns) and the serving serves them
+        (serveManyColumns) with the default supplement, so that the queries it is handed are the ones read."""
+        from .controller import LServing
+        s = server.serving
+        return (all(hasattr(a, "predictManyColumns") for a in server.algorithms) and hasattr(s, "serveManyColumns")
+                and type(s).supplement is LServing.supplement)
+
+    @staticmethod
+    def lines(server: "QueryServer", queries: Sequence[Tuple[Any, Any]], chunk: int) -> Iterator[str]:
+        """The output lines of `queries`, in order: json.dumps of run's records.  On the column path (columnar) each
+        chunk is scored and served as columns, and a line is written from its row -- the same bytes, since a result
+        {"itemScores": [{"item": ..., "score": ...}, ...]} is written with json's own string and float forms -- or
+        from the served object of a query answered by serve."""
+        sep = (",", ":")
+        if not BatchPredict.columnar(server):
+            for rec in BatchPredict.run(server, queries, chunk):
+                yield json.dumps(rec, separators=sep)
+            return
+        chunk = max(1, int(chunk))
+        quoted = {}   # id(names) -> (names, their JSON strings)
+        for c0 in range(0, len(queries), chunk):
+            qs = [q for _, q in queries[c0:c0 + chunk]]
+            cols = server.serving.serveManyColumns(qs, [a.predictManyColumns(m, qs)
+                                                        for a, m in zip(server.algorithms, server.models)])
+            if quoted.get(id(cols.names), (None,))[0] is not cols.names:
+                quoted[id(cols.names)] = (cols.names, [json.dumps(s) for s in cols.names])
+            names = quoted[id(cols.names)][1]
+            items, scores, count = cols.items.tolist(), cols.scores.tolist(), cols.count.tolist()
+            for j, q in enumerate(qs):
+                head = '{"query":' + json.dumps(to_json(q), separators=sep) + ',"prediction":'
+                if j in cols.objects:
+                    yield head + json.dumps(to_json(cols.objects[j]), separators=sep) + "}"
+                    continue
+                n = count[j]
+                yield head + '{"itemScores":[' + ",".join(
+                    '{"item":' + names[i] + ',"score":' + _float_json(v) + "}"
+                    for i, v in zip(items[j][:n], scores[j][:n])) + "]}}"
+
+    @staticmethod
     def main(argv: Optional[Sequence[str]] = None) -> int:
         """Returns the number of predictions written."""
         a, _unknown = BatchPredict.parser().parse_known_args(argv)
@@ -429,8 +475,8 @@ class BatchPredict:
         queries = BatchPredict.read_queries(Path(a.input), server.algorithms[0].queryClass())   # before anything is written
         n = 0
         with open(a.output, "w", encoding="utf-8") as out:
-            for rec in BatchPredict.run(server, queries, a.query_chunk):
-                out.write(json.dumps(rec, separators=(",", ":")) + "\n")
+            for line in BatchPredict.lines(server, queries, a.query_chunk):
+                out.write(line + "\n")
                 n += 1
         logger.info("BatchPredict: %d predictions written to %s", n, a.output)
         return n
