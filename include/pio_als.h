@@ -66,7 +66,7 @@ extern "C" {
 #define PIO_ALS_ERR_NUMERIC (-4)  /* a normal equation was not positive definite (MLlib: dppsv info != 0) */
 #define PIO_ALS_ERR_IO (-5)
 #define PIO_ALS_ERR_COMM (-6)     /* NCCL */
-#define PIO_ALS_ERR_NOMEM (-7)    /* host memory exhausted (pio_cooc_model_create, pio_cooc_predict_filtered) */
+#define PIO_ALS_ERR_NOMEM (-7)    /* host memory exhausted (pio_cooc_model_*, pio_popular_model_*) */
 
 /* how repeated (user,item) pairs are treated by pio_als_set_ratings_coo */
 #define PIO_ALS_DEDUP_NONE 0      /* recommendation template: every event is its own rating (ALSAlgorithm.scala:62-65) */
@@ -547,6 +547,43 @@ PIO_API int pio_cooc_predict_filtered(pio_cooc_model* m, const int64_t* q_ptr, c
                                       int32_t n_queries, int32_t topk, const pio_als_query_filter* f,
                                       int32_t* out_items, int64_t* out_scores, int32_t* out_count);
 PIO_API int pio_cooc_model_get_stats(const pio_cooc_model* m, pio_cooc_stats* out);
+
+/* Batch top-N of one fixed per-item score under per-query filters: the ecommerce template's predictDefault
+ * (adjust-score ECommAlgorithm.scala:508-538), the popularity rule of users with no factor and no recent items
+ * (DESIGN.md 4.14).  An opaque object holds the scores; the caller folds any weights into them.  Errors: status codes as
+ * above, text via pio_als_last_error(NULL). */
+typedef struct pio_popular_model pio_popular_model;
+
+typedef struct pio_popular_stats {
+  int64_t kernel_launches;        /* over all calls on this model */
+  int64_t last_walked;            /* ranked entries the last call's walk examined, all queries */
+  int64_t last_listed;            /* white-list entries the last call sorted */
+  int32_t last_parts, last_max_part_queries;
+} pio_popular_stats;
+
+/* Default number of entries per part of a pio_popular_predict_filtered call (about 28 bytes of device memory each); the
+ * environment variable PIO_POPULAR_PREDICT_BUDGET (a positive integer) overrides it.  Results do not depend on it. */
+#define PIO_POPULAR_PREDICT_BUDGET (1ll << 24)   /* env PIO_POPULAR_PREDICT_BUDGET overrides */
+
+/* Checks scores[0 .. n_items) on the host -- PIO_ALS_ERR_ARG naming the first NaN; infinities are allowed -- and
+ * copies them.  n_items >= 1.  The device copy and the ranked order are made on `device` by the first
+ * pio_popular_predict_filtered, so that a model holds no device memory until it scores. */
+PIO_API int pio_popular_model_create(int device, int32_t n_items, const double* scores, pio_popular_model** out);
+/* n_queries queries, each with the filter of f (pio_als_query_filter, nullable, with the argument rules of
+ * pio_als_similar_batch_filtered; ids out of range and duplicates are ignored).  The candidates of query j are the
+ * items i in [0, n_items) that are not in j's exclusion list, not set in j's item_sets row, and in j's white list if
+ * has_wl[j].  They are ordered by scores[i] descending, with -0.0 == +0.0; equal scores go by item index ascending; the
+ * list is cut at topk >= 1.  Row j of out_items (int32) / out_scores (fp64), n_queries x topk, padded with -1 / 0;
+ * out_scores holds scores[i] exactly (a -0.0 stays -0.0), and out_count[j] is the number of results.
+ * The batch runs in parts of consecutive queries whose entries -- the entries ex_ptr and wl_ptr name for each query plus
+ * its topk output slots -- stay within PIO_POPULAR_PREDICT_BUDGET, at least one query per part.  Rejected with
+ * PIO_ALS_ERR_ARG before any device work: topk < 1, n_queries < 0, a NULL output, a bad filter, and a query whose
+ * entries are 2^32 or more (a part's entries are numbered in 32 bits). */
+PIO_API int pio_popular_predict_filtered(pio_popular_model* m, int32_t n_queries, int32_t topk,
+                                         const pio_als_query_filter* f, int32_t* out_items, double* out_scores,
+                                         int32_t* out_count);
+PIO_API int pio_popular_model_get_stats(const pio_popular_model* m, pio_popular_stats* out);
+PIO_API int pio_popular_model_destroy(pio_popular_model* m);
 
 /* Default number of entries per part of a pio_serve_zscore_merge call (about 90 bytes of device memory each); the
  * environment variable PIO_SERVE_MERGE_BUDGET (a positive integer) overrides it.  Results do not depend on it. */

@@ -55,6 +55,7 @@
 #include "events_index.cuh"
 #include "cooc.cuh"
 #include "cooc_predict.cuh"
+#include "popular.cuh"
 #include "serve_merge.cuh"
 #include "forest.cuh"
 #include "eval_folds.cuh"
@@ -4747,6 +4748,246 @@ int pio_cooc_predict_filtered(pio_cooc_model* m, const int64_t* q_ptr, const int
 }
 
 int pio_cooc_model_get_stats(const pio_cooc_model* m, pio_cooc_stats* out) {
+  if (!m || !out) return fail(nullptr, PIO_ALS_ERR_ARG, "null argument");
+  std::lock_guard<std::mutex> lk(m->mu);
+  *out = m->stats;
+  return PIO_ALS_OK;
+}
+
+}  // extern "C"
+
+// ---- popularity top-N (ecommerce ECommAlgorithm.predictDefault) ------------------------------------------------------------
+struct pio_popular_model {
+  int device = 0, n_items = 0;
+  std::vector<double> scores;           // host copy until the first call ranks it on the device
+  cudaStream_t st = nullptr;
+  int *d_order = nullptr, *d_rank = nullptr;   // set together with d_sorted, once the ranked order has landed
+  double* d_sorted = nullptr;
+  mutable std::mutex mu;                // serialises the calls, and guards stats
+  pio_popular_stats stats{};
+};
+
+namespace pio {
+
+// A call's parts: consecutive queries [first[p], first[p + 1]).  A part closes before the query that would take its
+// entries (exclusion and white-list entries, plus topk output slots per query) over the budget; each part holds at
+// least one query.
+static int popular_plan(const pio_als_query_filter* f, int n, int topk, long long budget, std::vector<int>* first) {
+  long long acc = 0;
+  for (int j = 0; j < n; ++j) {
+    long long ent = topk;
+    if (f && f->ex_ptr) ent += f->ex_ptr[j + 1] - f->ex_ptr[j];
+    if (f && f->wl_ptr) ent += f->wl_ptr[j + 1] - f->wl_ptr[j];
+    if (ent >= (1ll << 32))
+      return fail(nullptr, PIO_ALS_ERR_ARG, "query %d has %lld list entries and output slots: at most 2^32 - 1 fit one part",
+                  j, ent);
+    if (j == 0 || acc + ent > budget) {
+      first->push_back(j);
+      acc = 0;
+    }
+    acc += ent;
+  }
+  first->push_back(n);
+  return PIO_ALS_OK;
+}
+
+// the ranked order of m's scores into order / sorted / rank, on env's stream, complete when it returns OK
+static int popular_rank(pio_popular_model* m, const FilterEnv& env, int* order, double* sorted, int* rank) {
+  const int n = m->n_items;
+  Scratch tmp(env.st);
+  double* d_scores = nullptr;
+  SortBufs sb;
+  CKF(env, tmp.alloc(&d_scores, (size_t)n));
+  for (int b = 0; b < 2; ++b) {
+    CKF(env, tmp.alloc(&sb.k[b], (size_t)n));
+    CKF(env, tmp.alloc(&sb.v[b], (size_t)n));
+  }
+  CKF(env, cudaMemcpyAsync(d_scores, m->scores.data(), sizeof(double) * (size_t)n, cudaMemcpyHostToDevice, env.st));
+  int rc = env_launch(env, pp_rank_keys_kernel, n, (const double*)d_scores, n, sb.keys(), sb.vals());
+  if (rc) return rc;
+  CKF(env, radix_sort_pairs(sb, (size_t)n, 64, env.st, env.launches));
+  rc = env_launch(env, pp_ranked_kernel, n, (const uint32_t*)sb.vals(), (const double*)d_scores, n, order, sorted, rank);
+  if (rc) return rc;
+  CKF(env, cudaStreamSynchronize(env.st));   // the host scores are read until here
+  return PIO_ALS_OK;
+}
+
+// The model's ranked order, made on its own stream by the first call.  The device pointers are published only after it
+// has completed, so a failed upload leaves nothing half made: its allocations are freed and the next call starts over.
+static int popular_upload(pio_popular_model* m, FilterEnv env) {
+  if (m->d_order) return PIO_ALS_OK;
+  if (!m->st) CKF(env, cudaStreamCreateWithFlags(&m->st, cudaStreamNonBlocking));
+  env.st = m->st;
+  const size_t n = (size_t)m->n_items;
+  int *order = nullptr, *rank = nullptr;
+  double* sorted = nullptr;
+  cudaError_t e = cudaMalloc((void**)&order, sizeof(int) * n);
+  if (e == cudaSuccess) e = cudaMalloc((void**)&rank, sizeof(int) * n);
+  if (e == cudaSuccess) e = cudaMalloc((void**)&sorted, sizeof(double) * n);
+  const int rc = e == cudaSuccess ? popular_rank(m, env, order, sorted, rank) : PIO_ALS_OK;
+  if (e != cudaSuccess || rc) {
+    cudaStreamSynchronize(m->st);
+    for (void* p : {(void*)order, (void*)rank, (void*)sorted})
+      if (p) cudaFree(p);
+    return rc ? rc : fail_to(env.err, PIO_ALS_ERR_CUDA, "uploading the popularity model: %s", cudaGetErrorString(e));
+  }
+  m->d_order = order, m->d_rank = rank, m->d_sorted = sorted;
+  std::vector<double>().swap(m->scores);
+  return PIO_ALS_OK;
+}
+
+// the queries [j0, j1) of a call: rows j0 .. j1 - 1 of the caller's outputs
+static int popular_part(pio_popular_model* m, const FilterEnv& env, int j0, int j1, int topk,
+                        const pio_als_query_filter* f, const CallFilter& cf, int32_t* out_items, double* out_scores,
+                        int32_t* out_count) {
+  const int n = j1 - j0;
+  cudaStream_t st = env.st;
+  Scratch tmp(st);
+  std::vector<int> idx((size_t)n);
+  for (int i = 0; i < n; ++i) idx[i] = j0 + i;
+  QueryFilterDev qf;
+  PopularLists L;
+  long long listed = 0;
+  if (f) {
+    int rc = upload_part_filter(env, f, cf, idx, tmp, &qf);
+    if (rc) return rc;
+    if (f->has_wl && std::any_of(f->has_wl + j0, f->has_wl + j1, [](uint8_t x) { return x != 0; })) {
+      // the white lists as (query << 32 | rank position) keys, sorted: each query's list in rank order
+      DevLists wl;
+      rc = upload_lists(env, f->wl_ptr, f->wl_items, idx, tmp, &wl);
+      if (rc) return rc;
+      listed = f->wl_ptr ? f->wl_ptr[j1] - f->wl_ptr[j0] : 0;
+      SortBufs sb;
+      if (listed > 0) {
+        for (int b = 0; b < 2; ++b) {
+          CKF(env, tmp.alloc(&sb.k[b], (size_t)listed));
+          CKF(env, tmp.alloc(&sb.v[b], (size_t)listed));
+        }
+        rc = env_launch(env, pp_list_keys_kernel, listed, wl.keys, listed, (const int*)m->d_rank, m->n_items, sb.keys(),
+                        sb.vals());
+        if (rc) return rc;
+        CKF(env, radix_sort_pairs(sb, (size_t)listed, 32 + ceil_log2((uint64_t)n), st, env.launches));
+      }
+      uint8_t* d_has = nullptr;
+      CKF(env, tmp.alloc(&d_has, (size_t)n));
+      CKF(env, cudaMemcpyAsync(d_has, f->has_wl + j0, (size_t)n, cudaMemcpyHostToDevice, st));
+      L.has_wl = d_has;
+      L.keys = sb.keys();
+      L.ptr = wl.ptr;
+    }
+  }
+  m->stats.last_listed += listed;
+  int* d_oi = nullptr;
+  double* d_os = nullptr;
+  int* d_oc = nullptr;
+  unsigned long long* d_walked = nullptr;
+  CKF(env, tmp.alloc(&d_oi, (size_t)n * topk));
+  CKF(env, tmp.alloc(&d_os, (size_t)n * topk));
+  CKF(env, tmp.alloc(&d_oc, (size_t)n));
+  CKF(env, tmp.alloc(&d_walked, 1));
+  CKF(env, cudaMemsetAsync(d_walked, 0, sizeof(unsigned long long), st));
+  PopularRanked R;
+  R.order = m->d_order;
+  R.sorted = m->d_sorted;
+  R.n_items = m->n_items;
+  const int rc = env_launch(env, pp_take_kernel, (long long)n * 32, R, n, topk, qf, L, d_oi, d_os, d_oc, d_walked);
+  if (rc) return rc;
+  unsigned long long walked = 0;
+  CKF(env, cudaMemcpyAsync(out_items + (size_t)j0 * topk, d_oi, sizeof(int) * (size_t)n * topk, cudaMemcpyDeviceToHost, st));
+  CKF(env, cudaMemcpyAsync(out_scores + (size_t)j0 * topk, d_os, sizeof(double) * (size_t)n * topk, cudaMemcpyDeviceToHost,
+                           st));
+  CKF(env, cudaMemcpyAsync(out_count + j0, d_oc, sizeof(int) * (size_t)n, cudaMemcpyDeviceToHost, st));
+  CKF(env, cudaMemcpyAsync(&walked, d_walked, sizeof walked, cudaMemcpyDeviceToHost, st));
+  CKF(env, cudaStreamSynchronize(st));
+  m->stats.last_walked += (int64_t)walked;
+  return PIO_ALS_OK;
+}
+
+static int popular_predict(pio_popular_model* m, int32_t n_queries, int32_t topk, const pio_als_query_filter* f,
+                           int32_t* out_items, double* out_scores, int32_t* out_count) {
+  pio_popular_stats& s = m->stats;
+  s.last_walked = s.last_listed = 0;
+  s.last_parts = s.last_max_part_queries = 0;
+  if (n_queries < 0 || topk < 1) return fail(nullptr, PIO_ALS_ERR_ARG, "topk must be >= 1 and n_queries >= 0");
+  if (n_queries == 0) return PIO_ALS_OK;
+  if (!out_items || !out_scores || !out_count) return fail(nullptr, PIO_ALS_ERR_ARG, "null argument");
+  if (f)
+    if (const char* what = query_filter_error(f, n_queries)) return fail(nullptr, PIO_ALS_ERR_ARG, "%s", what);
+  // PIO_POPULAR_PREDICT_BUDGET: entries per part; capped so that a part's entries are numbered in 32 bits
+  const char* env_b = getenv("PIO_POPULAR_PREDICT_BUDGET");
+  const long long budget = std::min<long long>(env_b && atoll(env_b) > 0 ? atoll(env_b) : PIO_POPULAR_PREDICT_BUDGET,
+                                               (1ll << 32) - 1);
+  std::vector<int> first;
+  int rc = popular_plan(f, n_queries, topk, budget, &first);
+  if (rc) return rc;
+  CK0(cudaSetDevice(m->device));
+  FilterEnv env{nullptr, m->n_items, &s.kernel_launches, &g_create_error};
+  rc = popular_upload(m, env);
+  if (rc) return rc;
+  env.st = m->st;
+  Scratch tmp(m->st);
+  CallFilter cf;
+  if (f) {
+    rc = upload_set_rows(env, f, tmp, &cf);
+    if (rc) return rc;
+  }
+  const int parts = (int)first.size() - 1;
+  for (int p = 0; p < parts; ++p) {
+    const int j0 = first[p], j1 = first[p + 1];
+    s.last_parts = p + 1;
+    s.last_max_part_queries = std::max(s.last_max_part_queries, j1 - j0);
+    rc = popular_part(m, env, j0, j1, topk, f, cf, out_items, out_scores, out_count);
+    if (rc) return rc;
+  }
+  return PIO_ALS_OK;
+}
+
+}  // namespace pio
+
+extern "C" {
+
+int pio_popular_model_create(int device, int32_t n_items, const double* scores, pio_popular_model** out) {
+  if (!out || !scores || n_items < 1) return fail(nullptr, PIO_ALS_ERR_ARG, "bad pio_popular_model_create arguments");
+  *out = nullptr;
+  for (int32_t i = 0; i < n_items; ++i)
+    if (std::isnan(scores[i])) return fail(nullptr, PIO_ALS_ERR_ARG, "item %d: score is NaN", i);
+  std::unique_ptr<pio_popular_model> m;
+  try {   // bad_alloc must not cross the C boundary
+    m.reset(new pio_popular_model);
+    m->device = device, m->n_items = n_items;
+    m->scores.assign(scores, scores + n_items);
+  } catch (const std::bad_alloc&) {
+    return fail(nullptr, PIO_ALS_ERR_NOMEM, "pio_popular_model_create: out of host memory");
+  }
+  *out = m.release();
+  return PIO_ALS_OK;
+}
+
+int pio_popular_model_destroy(pio_popular_model* m) {
+  if (!m) return PIO_ALS_OK;
+  if (m->st) {
+    cudaSetDevice(m->device);
+    cudaStreamSynchronize(m->st);
+    cudaStreamDestroy(m->st);
+  }
+  for (void* p : {(void*)m->d_order, (void*)m->d_rank, (void*)m->d_sorted})
+    if (p) cudaFree(p);
+  delete m;
+  return PIO_ALS_OK;
+}
+
+int pio_popular_predict_filtered(pio_popular_model* m, int32_t n_queries, int32_t topk, const pio_als_query_filter* f,
+                                 int32_t* out_items, double* out_scores, int32_t* out_count) {
+  if (!m) return fail(nullptr, PIO_ALS_ERR_ARG, "null model");
+  std::lock_guard<std::mutex> lk(m->mu);
+  try {   // bad_alloc must not cross the C boundary; Scratch releases a part's device memory on the way out
+    return popular_predict(m, n_queries, topk, f, out_items, out_scores, out_count);
+  } catch (const std::bad_alloc&) {
+    return fail(nullptr, PIO_ALS_ERR_NOMEM, "pio_popular_predict_filtered: out of host memory");
+  }
+}
+
+int pio_popular_model_get_stats(const pio_popular_model* m, pio_popular_stats* out) {
   if (!m || !out) return fail(nullptr, PIO_ALS_ERR_ARG, "null argument");
   std::lock_guard<std::mutex> lk(m->mu);
   *out = m->stats;

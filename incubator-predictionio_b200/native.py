@@ -45,7 +45,8 @@ EXPORTED_SYMBOLS = [
     "pio_cls_folds_classes", "pio_cls_folds_nb_train", "pio_cls_folds_rf_train", "pio_cls_folds_nb_predict",
     "pio_cls_folds_rf_predict", "pio_cls_folds_result_labels", "pio_cls_folds_result_counts",
     "pio_cls_folds_result_free", "pio_cls_folds_destroy", "pio_cooc_model_create", "pio_cooc_model_destroy",
-    "pio_cooc_predict_filtered", "pio_cooc_model_get_stats", "pio_serve_zscore_merge",
+    "pio_cooc_predict_filtered", "pio_cooc_model_get_stats", "pio_serve_zscore_merge", "pio_popular_model_create",
+    "pio_popular_predict_filtered", "pio_popular_model_get_stats", "pio_popular_model_destroy",
 ]
 
 
@@ -200,6 +201,12 @@ def lib():
         L.pio_serve_zscore_merge.restype = ci
         L.pio_serve_zscore_merge.argtypes = [ci, C.c_int32, C.c_int32, C.c_int32, vp, vp, vp, vp, vp, C.c_int32, vp, vp,
                                              vp]
+        L.pio_popular_model_create.restype = ci
+        L.pio_popular_model_create.argtypes = [ci, C.c_int32, vp, vp]
+        L.pio_popular_model_destroy.argtypes = [vp]
+        L.pio_popular_predict_filtered.restype = ci
+        L.pio_popular_predict_filtered.argtypes = [vp, C.c_int32, C.c_int32, vp, vp, vp, vp]
+        L.pio_popular_model_get_stats.argtypes = [vp, vp]
         for name in EXPORTED_SYMBOLS:
             getattr(L, name)  # AttributeError if the ABI is incomplete
         _lib = L
@@ -1063,6 +1070,53 @@ class CoocModel:
         st = CoocStats()
         _check(lib().pio_cooc_model_get_stats(self._h, C.addressof(st)))
         return {name: getattr(st, name) for name, _ in CoocStats._fields_}
+
+
+class PopularStats(C.Structure):
+    _fields_ = [("kernel_launches", C.c_int64), ("last_walked", C.c_int64), ("last_listed", C.c_int64),
+                ("last_parts", C.c_int32), ("last_max_part_queries", C.c_int32)]
+
+
+class PopularModel:
+    """pio_popular_model: one fixed fp64 score per item (no NaN) that ranks batches of filtered queries on `device`, best
+    score first, equal scores by item index.  The scores are checked and copied when it is created; the device copy and
+    its ranked order are made by the first predict_filtered."""
+
+    def __init__(self, scores, device: int = 0):
+        sc = np.ascontiguousarray(scores, np.float64)
+        if sc.ndim != 1:
+            raise ValueError("scores must be [n_items]")
+        self.n_items = int(sc.shape[0])
+        self._h = C.c_void_p()
+        _check(lib().pio_popular_model_create(int(device), self.n_items, sc.ctypes.data, C.addressof(self._h)))
+
+    def close(self):
+        if self._h:
+            lib().pio_popular_model_destroy(self._h)
+            self._h = C.c_void_p()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    def predict_filtered(self, n_queries: int, topk: int, query_filter=None):
+        """n_queries queries, each with its entry of query_filter (QueryFilter, or None: no filter).  Returns
+        (items int32 [n, topk], scores float64 [n, topk], count int32 [n])."""
+        n = int(n_queries)
+        oi = np.full((max(n, 0), topk), -1, np.int32)
+        os_ = np.zeros((max(n, 0), topk), np.float64)
+        oc = np.zeros(max(n, 0), np.int32)
+        qf = None if query_filter is None else query_filter.struct(n, self.n_items)
+        _check(lib().pio_popular_predict_filtered(self._h, n, int(topk), None if qf is None else C.addressof(qf),
+                                                  oi.ctypes.data, os_.ctypes.data, oc.ctypes.data))
+        return oi, os_, oc
+
+    def stats(self) -> dict:
+        st = PopularStats()
+        _check(lib().pio_popular_model_get_stats(self._h, C.addressof(st)))
+        return {name: getattr(st, name) for name, _ in PopularStats._fields_}
 
 
 @dataclass

@@ -157,12 +157,42 @@ def _model_path(id: str) -> Path:
 
 
 class ECommModel(PersistentModel):
+    """The factors, the id maps, the item properties and the buy counts.  predictMany scores the popularity rule on a
+    device copy of counts x weights (native.PopularModel on the factors' device), made on first use, rebuilt when the
+    weights change and kept out of the pickle; save writes the counts as a map, as before."""
+
+    _CACHES = ("_popularity", "_popular_model", "_item_names")
+
     def __init__(self, mf: MatrixFactorizationModel, userStringIntMap: BiMap, itemStringIntMap: BiMap,
-                 items: Dict[int, Item], popularCount: Dict[int, int]):
+                 items: Dict[int, Item], popularCount: Dict[int, int], device: int = 0):
         self.mf, self.rank = mf, mf.rank
         self.userStringIntMap, self.itemStringIntMap = userStringIntMap, itemStringIntMap
         self.itemIntStringMap = itemStringIntMap.inverse
         self.items, self.popularCount = items, popularCount
+        self.device = device
+
+    def popularity(self) -> np.ndarray:
+        """popularCount as a dense float64 vector over the item indices (0 for an item nobody bought), built once."""
+        p = self.__dict__.get("_popularity")
+        if p is None:
+            p = np.zeros(len(self.mf.productHas), np.float64)
+            if self.popularCount:
+                p[np.fromiter(self.popularCount.keys(), np.int64)] = np.fromiter(self.popularCount.values(), np.float64)
+            self._popularity = p
+        return p
+
+    def popular_model(self, scores: np.ndarray) -> "native.PopularModel":
+        """The device model of these per-item scores (no NaN), kept while the next call's scores have the same bytes."""
+        key = scores.tobytes()
+        cached = self.__dict__.get("_popular_model")
+        if cached is None or cached[0] != key:
+            if cached is not None:
+                cached[1].close()
+            cached = self._popular_model = (key, native.PopularModel(scores, getattr(self, "device", 0)))
+        return cached[1]
+
+    def __getstate__(self):
+        return {k: v for k, v in self.__dict__.items() if k not in self._CACHES}
 
     def save(self, id, params, sc) -> bool:
         d = _model_path(id)
@@ -177,10 +207,11 @@ class ECommModel(PersistentModel):
     @classmethod
     def apply(cls, id, params, sc) -> "ECommModel":
         d = _model_path(id)
-        mf = MatrixFactorizationModel.load(str(d / "factors.pioals"), getattr(sc, "device", 0))
+        device = getattr(sc, "device", 0) or 0
+        mf = MatrixFactorizationModel.load(str(d / "factors.pioals"), device)
         j = json.loads((d / "maps.json").read_text())
         return cls(mf, BiMap(j["user"]), BiMap(j["item"]), {int(k): Item(v) for k, v in j["items"].items()},
-                   {int(k): int(v) for k, v in j["popular"].items()})
+                   {int(k): int(v) for k, v in j["popular"].items()}, device)
 
 
 class ECommAlgorithm(P2LAlgorithm):
@@ -240,7 +271,7 @@ class ECommAlgorithm(P2LAlgorithm):
             counts = np.bincount(bought, minlength=itemMap.size)
             _, first = np.unique(bought, return_index=True)   # in order of the first buy, as the loop above fills it
             popular = {int(i): int(counts[i]) for i in bought[np.sort(first)]}
-        return ECommModel(m, userMap, itemMap, items, popular)
+        return ECommModel(m, userMap, itemMap, items, popular, getattr(sc, "device", 0) or 0)
 
     # -- serving -------------------------------------------------------------------------------
     def genBlackList(self, query: Query) -> Set[str]:
@@ -328,20 +359,27 @@ class ECommAlgorithm(P2LAlgorithm):
                 top = cand[:query.num]
         return PredictedResult([ItemScore(model.itemIntStringMap(i), s) for i, s in top])
 
-    def predictMany(self, model: ECommModel, queries) -> list:
-        """predict for many queries: one lookup per event index for the whole batch (seen items, recent items),
-        `unavailableItems` and `weightedItems` read once, then one filtered batch call per branch.  Known users are
-        scored by dot products with their black list (query blackList, seen items, unavailable items) as exclusion
-        list; unknown users with recent items by cosine sums that keep the recent items as candidates; the rest get
-        the popularity rule of predict on the host."""
-        qs = list(queries)
-        out: List[Optional[PredictedResult]] = [None] * len(qs)
+    def _many(self, model: ECommModel, qs):
+        """predictMany up to its result objects: (items int32 [Q, w], scores float64 [Q, w], count int32 [Q], objects).
+        Row j holds query j's result, best first, padded with -1 / 0; objects maps each query with num < 1 to predict's
+        result, and each default-branch query of a batch whose popularity scores hold a NaN to the host rule's.
+
+        One lookup per event index for the whole batch (seen items, recent items), `unavailableItems` and
+        `weightedItems` read once, then one filtered device call per branch, each query with its black list (query
+        blackList, seen items, unavailable items) as exclusion list: known users by dot products, unknown users with
+        recent items by cosine sums that keep the recent items as candidates, and the rest by the popularity rule
+        (pio_popular_predict_filtered over counts x weights)."""
+        objects: Dict[int, PredictedResult] = {}
         for j, q in enumerate(qs):
             if q.num < 1:
-                out[j] = self.predict(model, q)
-        rows = [j for j in range(len(qs)) if out[j] is None]
+                objects[j] = self.predict(model, q)
+        rows = [j for j in range(len(qs)) if j not in objects]
+        width = max([qs[j].num for j in rows], default=0)
+        items = np.full((len(qs), width), -1, np.int32)
+        scores = np.zeros((len(qs), width), np.float64)
+        count = np.zeros(len(qs), np.int32)
         if not rows:
-            return out
+            return items, scores, count, objects
         imap, n_items = model.itemStringIntMap, len(model.mf.productHas)
         seen = [set() for _ in rows]
         if self.ap.unseenOnly:
@@ -383,44 +421,79 @@ class ECommAlgorithm(P2LAlgorithm):
                 if rec:
                     similar.append(r)
                     recent_of[r] = rec
+        default = [r for r in unknown if r not in recent_of]
 
         def part(rs):
             return native.QueryFilter(len(rs), [black[r] for r in rs], [white[r] for r in rs],
                                       set_ix[rs] if set_rows else None, np.stack(set_rows) if set_rows else None)
 
-        def result(pairs):
-            return PredictedResult([ItemScore(model.itemIntStringMap(i), s) for i, s in pairs])
+        def put(rs, its, scs, keep):
+            """Rows rows[rs] of the output: the entries of its / scs where keep holds, in order."""
+            js = np.array([rows[r] for r in rs], np.int64)
+            keep = keep[:, :width]
+            first = np.argsort(~keep, axis=1, kind="stable")          # the kept entries first, in their order
+            cnt = keep.sum(axis=1)
+            live = np.arange(keep.shape[1]) < cnt[:, None]
+            w = keep.shape[1]
+            items[js, :w] = np.where(live, np.take_along_axis(its[:, :w], first, axis=1), -1)
+            scores[js, :w] = np.where(live, np.take_along_axis(scs[:, :w].astype(np.float64), first, axis=1), 0.0)
+            count[js] = cnt
+
+        def nums(rs):
+            return np.array([qs[rows[r]].num for r in rs], np.int64)
 
         if known:
             users = np.array([model.userStringIntMap.get(qs[rows[r]].user) for r in known], np.int32)
-            num = max(qs[rows[r]].num for r in known)
-            items, scores, cnt = model.mf.recommendProductsForUsers(users, num, None, weights, query_filter=part(known))
-            for k, r in enumerate(known):
-                n = min(int(cnt[k]), qs[rows[r]].num)
-                out[rows[r]] = result([(int(items[k, t]), float(scores[k, t])) for t in range(n) if scores[k, t] > 0])
+            its, scs, cnt = model.mf.recommendProductsForUsers(users, int(nums(known).max()), None, weights,
+                                                               query_filter=part(known))
+            # predictKnownUser keeps the scores > 0 of the first min(cnt, num)
+            put(known, its, scs, (np.arange(its.shape[1]) < np.minimum(cnt, nums(known))[:, None]) & (scs > 0))
         if similar:
-            num = max(qs[rows[r]].num for r in similar)
-            items, scores, cnt = model.mf.similarProductsBatch([recent_of[r] for r in similar], num, None, weights,
-                                                               exclude_query=False, query_filter=part(similar))
-            for k, r in enumerate(similar):
-                n = min(int(cnt[k]), qs[rows[r]].num)
-                out[rows[r]] = result([(int(items[k, t]), float(scores[k, t])) for t in range(n)])
-        for r in unknown:
-            if r in recent_of:
-                continue
-            # predictDefault: popularity count x weight over the query's candidates (no > 0 filter in the reference)
-            mask = np.zeros(n_items, bool)
-            if white[r] is not None:
-                mask[:] = True
-                mask[white[r]] = False
-            mask[black[r]] = True
-            if set_ix[r] >= 0:
-                mask |= set_rows[set_ix[r]].astype(bool)
-            cand = [(int(i), float(model.popularCount.get(int(i), 0)) * (float(weights[i]) if weights is not None else 1.0))
-                    for i in np.flatnonzero(~mask)]
-            cand.sort(key=lambda kv: (-kv[1], kv[0]))
-            out[rows[r]] = result(cand[:qs[rows[r]].num])
-        return out
+            its, scs, cnt = model.mf.similarProductsBatch([recent_of[r] for r in similar], int(nums(similar).max()), None,
+                                                          weights, exclude_query=False, query_filter=part(similar))
+            put(similar, its, scs, np.arange(its.shape[1]) < np.minimum(cnt, nums(similar))[:, None])
+        if default:
+            # predictDefault: popularity count x weight over the query's candidates (no > 0 filter in the reference);
+            # counts * weights is float(count) * float(w) of predict, and x * 1.0 == x without weights
+            pop = model.popularity() if weights is None else model.popularity() * weights
+            if not np.isnan(pop).any():
+                topk = int(min(nums(default).max(), n_items))
+                its, scs, cnt = model.popular_model(pop).predict_filtered(len(default), topk, part(default))
+                put(default, its, scs, np.arange(topk) < np.minimum(cnt, nums(default))[:, None])
+            else:   # a NaN score: the host rule, which defines what Python's sort makes of it
+                for r in default:
+                    mask = np.zeros(n_items, bool)
+                    if white[r] is not None:
+                        mask[:] = True
+                        mask[white[r]] = False
+                    mask[black[r]] = True
+                    if set_ix[r] >= 0:
+                        mask |= set_rows[set_ix[r]].astype(bool)
+                    cand = [(int(i), float(pop[i])) for i in np.flatnonzero(~mask)]
+                    cand.sort(key=lambda kv: (-kv[1], kv[0]))
+                    objects[rows[r]] = PredictedResult([ItemScore(model.itemIntStringMap(i), s)
+                                                        for i, s in cand[:qs[rows[r]].num]])
+        return items, scores, count, objects
+
+    def predictMany(self, model: ECommModel, queries) -> list:
+        """predict for many queries: the result of every query from _many's device calls (see there)."""
+        qs = list(queries)
+        items, scores, count, objects = self._many(model, qs)
+        name = model.itemIntStringMap
+        return [objects[j] if j in objects else
+                PredictedResult([ItemScore(name(i), s) for i, s in zip(items[j, :n].tolist(), scores[j, :n].tolist())])
+                for j, n in enumerate(count.tolist())]
+
+    def predictManyColumns(self, model: ECommModel, queries) -> native.ScoredColumns:
+        """predictMany as columns, before any result object is built: the same device calls; known-user rows keep the
+        entries predictMany keeps, float32 scores are widened to float64 (as float() does), default rows carry the
+        fp64 popularity scores as returned."""
+        qs = list(queries)
+        items, scores, count, objects = self._many(model, qs)
+        names = model.__dict__.get("_item_names")
+        if names is None:
+            names = model._item_names = native.item_names(model.itemStringIntMap)
+        return native.ScoredColumns(items, scores, count, names, objects, getattr(model, "device", 0))
 
 
 class ECommerceRecommendationEngine(EngineFactory):
