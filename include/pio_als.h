@@ -39,6 +39,8 @@
  *       examples/scala-parallel-recommendation/blacklist-items/src/main/scala/{DataSource.scala readEval, Evaluation.scala}
  *   pio_cls_folds_* run the classification template's k-fold evaluation
  *       examples/scala-parallel-classification/add-algorithm/src/main/scala/{DataSource.scala readEval, Evaluation.scala}
+ *   pio_assoc_train / pio_assoc_model_* replace the complementary purchase template's Algorithm.train
+ *       docs/manual/source/templates/complementarypurchase/dase.html.md.erb:293-314
  */
 #ifndef PIO_ALS_H_
 #define PIO_ALS_H_
@@ -702,6 +704,52 @@ PIO_API int pio_cls_folds_result_labels(const pio_cls_folds* f, int32_t result, 
 PIO_API int pio_cls_folds_result_counts(const pio_cls_folds* f, int32_t result, double label, int64_t out[4]);
 PIO_API int pio_cls_folds_result_free(pio_cls_folds* f, int32_t result);
 PIO_API int pio_cls_folds_destroy(pio_cls_folds* f);
+
+/* Association rules of the complementary purchase template: its Algorithm.train, which the reference elides
+ *   (docs/manual/source/templates/complementarypurchase/dase.html.md.erb:293-314; parameters :241-262).
+ * The rules are stated in tests/assoc_ref.py and DESIGN.md 4.15: the buys of each user, in time order, are cut into
+ * baskets wherever a gap exceeds basket_window * 1000 ms; a basket is the set of its items; baskets of fewer than
+ * min_basket_size items are dropped, T baskets are kept.  Every item set of size 1 .. max_rule_length of a kept basket
+ * is counted and is frequent when count >= min_support * T (fp64).  Every frequent S with |S| >= 2 and c in S gives
+ * the rule cond = S \ {c} -> c with support = count(S) / T, confidence = count(S) / count(cond), lift = confidence /
+ * (count({c}) / T) in fp64, kept when confidence >= min_confidence and lift >= min_lift; per cond the rules are ranked
+ * by lift descending, then by c ascending (this project's tie rule), and cut at max_num_rules_per_cond.
+ * Errors: status codes as above, text via pio_als_last_error(NULL).  Parameters and indices are checked on the host
+ * before any device work. */
+typedef struct pio_assoc_params {
+  int32_t basket_window;            /* seconds */
+  int32_t max_rule_length;          /* >= 2 */
+  double min_support;               /* [0, 1] */
+  double min_confidence;            /* [0, 1] */
+  double min_lift;
+  int32_t min_basket_size;          /* >= 2 */
+  int32_t max_num_rules_per_cond;   /* >= 1 */
+} pio_assoc_params;
+
+typedef struct pio_assoc_model pio_assoc_model;   /* a trained model, host memory only */
+
+/* Most candidate item sets one level may count (about 40 bytes of device memory each).  Before a level is enumerated
+ * its candidates -- the extensions of every occurrence of a frequent set one item shorter by the later frequent items
+ * of its basket -- are counted exactly; above this limit pio_assoc_train fails with PIO_ALS_ERR_ARG naming minSupport,
+ * maxRuleLength and basketWindow, and nothing is allocated or launched for that level. */
+#define PIO_ASSOC_MAX_CANDIDATES (1ll << 29)
+
+/* n buy events (HOST): user in [0, n_users), item in [0, n_items) (the item index orders ties), t_ms milliseconds
+ * since the epoch; 0 <= n < 2^32.  No basket surviving min_basket_size gives an empty model, not an error. */
+PIO_API int pio_assoc_train(int device, const int32_t* user, const int32_t* item, const int64_t* t_ms, int64_t n,
+                            int32_t n_users, int32_t n_items, const pio_assoc_params* params, pio_assoc_model** out);
+/* The model's size: levels (the longest frequent set), frequent sets over all levels, rules, and T. */
+PIO_API int pio_assoc_model_size(const pio_assoc_model* m, int32_t* n_levels, int64_t* n_sets, int64_t* n_rules,
+                                 int64_t* n_transactions);
+/* Flat arrays.  Sets, by length, then in lexicographic order of their items (ascending in each set): level_off
+ * [n_levels + 1] (the sets of length l are [level_off[l - 1], level_off[l])), and per set: set_prefix (the set without
+ * its largest item, as an index into these arrays; -1 for a single item), set_item (its largest item) and set_count.
+ * Rules, grouped by cond in set order and ranked within each cond: rule_cond (set index), rule_conseq (item), support,
+ * confidence, lift.  Any output pointer may be null. */
+PIO_API int pio_assoc_model_get(const pio_assoc_model* m, int64_t* level_off, int64_t* set_prefix, int32_t* set_item,
+                                int64_t* set_count, int64_t* rule_cond, int32_t* rule_conseq, double* support,
+                                double* confidence, double* lift);
+PIO_API int pio_assoc_model_destroy(pio_assoc_model* m);
 
 #ifdef __cplusplus
 }

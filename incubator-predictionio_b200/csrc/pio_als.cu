@@ -60,6 +60,7 @@
 #include "forest.cuh"
 #include "eval_folds.cuh"
 #include "cls_folds.cuh"
+#include "assoc.cuh"
 
 namespace pio {
 
@@ -6604,6 +6605,462 @@ int pio_cls_folds_destroy(pio_cls_folds* cf) {
   for (void* p : cf->mem) cudaFree(p);
   if (cf->st) cudaStreamDestroy(cf->st);
   delete cf;
+  return PIO_ALS_OK;
+}
+
+}  // extern "C"
+
+// ---- association rules (complementary purchase template, DESIGN.md 4.15) ---------------------------------------------
+struct pio_assoc_model {
+  int64_t n_transactions = 0;
+  std::vector<int64_t> level_off{0};   // the sets of level l + 1 are [level_off[l], level_off[l + 1])
+  std::vector<int64_t> set_prefix, set_count;
+  std::vector<int32_t> set_item;
+  std::vector<int64_t> rule_cond;
+  std::vector<int32_t> rule_conseq;
+  std::vector<double> support, confidence, lift;
+};
+
+namespace pio {
+
+// where the last pio_assoc_train on this thread spent its time (wall ms; every phase ends in a stream synchronise)
+struct AssocTiming {
+  double h2d = 0, baskets = 0, level1 = 0, levels = 0, rules = 0, rank = 0, d2h = 0, total = 0;
+  int64_t n_baskets = 0, n_transactions = 0, levels_run = 0, rejected_level = 0;
+  int64_t cand[ASSOC_MAX_LEN + 1] = {};   // candidates counted for level k >= 2, a rejected level's included
+};
+static thread_local AssocTiming g_assoc_timing;
+
+static int assoc_check(const pio_assoc_params* p) {
+  if (p->max_rule_length < 2)
+    return fail(nullptr, PIO_ALS_ERR_ARG, "maxRuleLength must be at least 2 (got %d)", p->max_rule_length);
+  if (p->min_basket_size < 2)
+    return fail(nullptr, PIO_ALS_ERR_ARG, "minBasketSize must be at least 2 (got %d)", p->min_basket_size);
+  if (!(p->min_support >= 0.0 && p->min_support <= 1.0))
+    return fail(nullptr, PIO_ALS_ERR_ARG, "minSupport must be in [0, 1] (got %g)", p->min_support);
+  if (!(p->min_confidence >= 0.0 && p->min_confidence <= 1.0))
+    return fail(nullptr, PIO_ALS_ERR_ARG, "minConfidence must be in [0, 1] (got %g)", p->min_confidence);
+  if (p->max_num_rules_per_cond < 1)
+    return fail(nullptr, PIO_ALS_ERR_ARG, "maxNumRulesPerCond must be at least 1 (got %d)", p->max_num_rules_per_cond);
+  return PIO_ALS_OK;
+}
+
+// exclusive scan of v[0, n) into pos, and *total = the sum (synchronises st)
+static cudaError_t assoc_total(const uint32_t* v, uint32_t* pos, long long n, cudaStream_t st, long long* total) {
+  *total = 0;
+  if (n == 0) return cudaSuccess;
+  cudaError_t e = scan_exclusive_u32(v, pos, (size_t)n, st, nullptr);
+  uint32_t last[2] = {0, 0};
+  if (e == cudaSuccess) e = cudaMemcpyAsync(&last[0], pos + n - 1, 4, cudaMemcpyDeviceToHost, st);
+  if (e == cudaSuccess) e = cudaMemcpyAsync(&last[1], v + n - 1, 4, cudaMemcpyDeviceToHost, st);
+  if (e == cudaSuccess) e = cudaStreamSynchronize(st);
+  *total = (long long)last[0] + last[1];
+  return e;
+}
+
+// a 64-bit device counter, read back (synchronises st)
+static cudaError_t assoc_read(const unsigned long long* d, cudaStream_t st, unsigned long long* out) {
+  cudaError_t e = cudaMemcpyAsync(out, d, sizeof(*out), cudaMemcpyDeviceToHost, st);
+  return e == cudaSuccess ? cudaStreamSynchronize(st) : e;
+}
+
+static int assoc_fit(int device, const int32_t* user, const int32_t* item, const int64_t* t_ms, long long n,
+                     int32_t n_users, int32_t n_items, const pio_assoc_params* p, pio_assoc_model* m) {
+  AssocTiming& tm = g_assoc_timing;
+  const auto t0 = Clock::now();
+  auto tp = t0;
+  auto lap = [&tp]() {
+    const auto now = Clock::now();
+    const double r = std::chrono::duration<double, std::milli>(now - tp).count();
+    tp = now;
+    return r;
+  };
+  CK0(cudaSetDevice(device));
+  CallMem call;
+  cudaStream_t st;
+  CK0(call.stream(&st));
+  const int bits_u = ceil_log2((uint64_t)n_users), bits_i = ceil_log2((uint64_t)n_items);
+  Scratch base(st);   // the kept baskets and the level-1 arrays, until the levels are built
+  int* k_item = nullptr;
+  uint32_t *k_basket = nullptr, *cnt1 = nullptr;
+  long long NB = 0, T = 0, M = 0;
+  lap();
+  {
+    // 1. baskets: (user, t, event) order, heads at a user change or a gap over the window, distinct (basket, item)
+    Scratch tmp(st);
+    int *du = nullptr, *di = nullptr;
+    long long* dt = nullptr;
+    uint32_t *head = nullptr, *bscan = nullptr;
+    SortBufs sb;
+    CK0(tmp.alloc(&du, (size_t)n)); CK0(tmp.alloc(&di, (size_t)n)); CK0(tmp.alloc(&dt, (size_t)n));
+    CK0(tmp.alloc(&head, (size_t)n)); CK0(tmp.alloc(&bscan, (size_t)n));
+    for (int b : {0, 1}) {
+      CK0(tmp.alloc(&sb.k[b], (size_t)n));
+      CK0(tmp.alloc(&sb.v[b], (size_t)n));
+    }
+    CK0(cudaMemcpyAsync(du, user, 4 * (size_t)n, cudaMemcpyHostToDevice, st));
+    CK0(cudaMemcpyAsync(di, item, 4 * (size_t)n, cudaMemcpyHostToDevice, st));
+    CK0(cudaMemcpyAsync(dt, t_ms, 8 * (size_t)n, cudaMemcpyHostToDevice, st));
+    CK0(cudaStreamSynchronize(st));
+    tm.h2d = lap();
+    fold_time_key_kernel<<<nblk(n, 256), 256, 0, st>>>(dt, n, sb.keys(), sb.vals());
+    CK0(radix_sort_pairs(sb, (size_t)n, 64, st, nullptr));
+    fold_entity_key_kernel<<<nblk(n, 256), 256, 0, st>>>(sb.vals(), du, n, sb.keys());
+    CK0(radix_sort_pairs(sb, (size_t)n, bits_u, st, nullptr));
+    assoc_basket_head_kernel<<<nblk(n, 256), 256, 0, st>>>(sb.keys(), sb.vals(), dt, n,
+                                                          (long long)p->basket_window * 1000ll, head);
+    CK0(cudaGetLastError());
+    long long n_raw = 0;
+    CK0(assoc_total(head, bscan, n, st, &n_raw));
+    assoc_bi_key_kernel<<<nblk(n, 256), 256, 0, st>>>(head, bscan, sb.vals(), di, n, bits_i, sb.spare_keys(),
+                                                     sb.spare_vals());
+    sb.flip();
+    CK0(radix_sort_pairs(sb, (size_t)n, ceil_log2((uint64_t)n_raw) + bits_i, st, nullptr));
+    uint32_t *flag = head, *pos = bscan;
+    cooc_head_kernel<<<nblk(n, 256), 256, 0, st>>>(sb.keys(), n, flag);
+    long long D = 0;
+    CK0(assoc_total(flag, pos, n, st, &D));
+    uint64_t* dk = sb.spare_keys();
+    cooc_compact_kernel<<<nblk(n, 256), 256, 0, st>>>(sb.keys(), flag, pos, n, dk);
+    // 2. basket sizes, minBasketSize, T
+    uint32_t *bh = nullptr, *bord = nullptr, *keep = nullptr, *kord = nullptr, *eflag = nullptr, *epos = nullptr;
+    CK0(tmp.alloc(&bh, (size_t)D)); CK0(tmp.alloc(&bord, (size_t)D));
+    cooc_user_head_kernel<<<nblk(D, 256), 256, 0, st>>>(dk, D, bits_i, bh);
+    CK0(assoc_total(bh, bord, D, st, &NB));
+    CK0(tmp.alloc(&keep, (size_t)NB)); CK0(tmp.alloc(&kord, (size_t)NB));
+    assoc_basket_size_kernel<<<nblk(D, 256), 256, 0, st>>>(dk, bh, bord, D, bits_i, p->min_basket_size, keep);
+    CK0(assoc_total(keep, kord, NB, st, &T));
+    CK0(tmp.alloc(&eflag, (size_t)D)); CK0(tmp.alloc(&epos, (size_t)D));
+    assoc_kept_flag_kernel<<<nblk(D, 256), 256, 0, st>>>(bh, bord, keep, D, eflag);
+    CK0(assoc_total(eflag, epos, D, st, &M));
+    CK0(base.alloc(&k_item, (size_t)M)); CK0(base.alloc(&k_basket, (size_t)M));
+    CK0(base.alloc(&cnt1, (size_t)n_items));
+    CK0(cudaMemsetAsync(cnt1, 0, 4 * (size_t)n_items, st));
+    assoc_kept_kernel<<<nblk(D, 256), 256, 0, st>>>(dk, bh, bord, kord, eflag, epos, D, bits_i, k_item, k_basket, cnt1);
+    CK0(cudaGetLastError());
+    CK0(cudaStreamSynchronize(st));
+  }
+  tm.baskets = lap();
+  tm.n_baskets = NB;
+  tm.n_transactions = m->n_transactions = T;
+  if (T == 0) {
+    tm.total = std::chrono::duration<double, std::milli>(Clock::now() - t0).count();
+    return PIO_ALS_OK;
+  }
+  const double thr = p->min_support * (double)T;   // count >= minSupport * T, compared in fp64
+  // 3. level 1, and the baskets pruned to their frequent items: the occurrences of the level-1 sets
+  Scratch sets(st);                                 // keys and counts of every level, until the rules are made
+  std::vector<uint64_t*> lkeys{nullptr};
+  std::vector<uint32_t*> lcount{nullptr};
+  std::vector<long long> ln{0};
+  auto occ_mem = std::make_unique<Scratch>(st);
+  uint32_t *occ_pos = nullptr, *occ_id = nullptr, *end = nullptr;
+  int* p_item = nullptr;
+  long long NO = 0;
+  {
+    uint32_t *f1 = nullptr, *id1 = nullptr;
+    CK0(base.alloc(&f1, (size_t)n_items)); CK0(base.alloc(&id1, (size_t)n_items));
+    assoc_l1_flag_kernel<<<nblk(n_items, 256), 256, 0, st>>>(cnt1, n_items, thr, f1);
+    long long L1 = 0;
+    CK0(assoc_total(f1, id1, n_items, st, &L1));
+    if (L1 > 0) {
+      uint64_t* k1 = nullptr;
+      uint32_t* c1 = nullptr;
+      CK0(sets.alloc(&k1, (size_t)L1)); CK0(sets.alloc(&c1, (size_t)L1));
+      assoc_l1_emit_kernel<<<nblk(n_items, 256), 256, 0, st>>>(cnt1, f1, id1, n_items, k1, c1);
+      lkeys.push_back(k1), lcount.push_back(c1), ln.push_back(L1);
+      Scratch tmp(st);
+      uint32_t *pflag = nullptr, *ppos = nullptr, *p_basket = nullptr, *hd = nullptr, *sidx = nullptr, *seg = nullptr;
+      CK0(tmp.alloc(&pflag, (size_t)M)); CK0(tmp.alloc(&ppos, (size_t)M));
+      assoc_prune_flag_kernel<<<nblk(M, 256), 256, 0, st>>>(k_item, f1, M, pflag);
+      CK0(assoc_total(pflag, ppos, M, st, &NO));
+      CK0(base.alloc(&p_item, (size_t)NO)); CK0(base.alloc(&end, (size_t)NO));
+      CK0(tmp.alloc(&p_basket, (size_t)NO)); CK0(tmp.alloc(&hd, (size_t)NO)); CK0(tmp.alloc(&sidx, (size_t)NO));
+      CK0(occ_mem->alloc(&occ_pos, (size_t)NO)); CK0(occ_mem->alloc(&occ_id, (size_t)NO));
+      assoc_prune_kernel<<<nblk(M, 256), 256, 0, st>>>(k_item, k_basket, pflag, ppos, id1, M, p_item, p_basket, occ_pos,
+                                                       occ_id);
+      assoc_seg_start_kernel<<<nblk(NO, 256), 256, 0, st>>>(p_basket, NO, hd);
+      long long n_seg = 0;
+      CK0(assoc_total(hd, sidx, NO, st, &n_seg));
+      CK0(tmp.alloc(&seg, (size_t)n_seg + 1));
+      const uint32_t np32 = (uint32_t)NO;
+      CK0(cudaMemcpyAsync(seg + n_seg, &np32, 4, cudaMemcpyHostToDevice, st));
+      assoc_seg_pos_kernel<<<nblk(NO, 256), 256, 0, st>>>(hd, sidx, NO, seg);
+      assoc_seg_end_kernel<<<nblk(NO, 256), 256, 0, st>>>(hd, sidx, seg, NO, end);
+      CK0(cudaGetLastError());
+      CK0(cudaStreamSynchronize(st));
+    }
+  }
+  tm.level1 = lap();
+  // 4. levels 2 .. maxRuleLength: extend the occurrences of the frequent (k-1)-sets, count, keep the frequent sets
+  long long n_sets = ln.back();
+  for (int k = 2; k <= p->max_rule_length && (int)ln.size() == k && NO > 0; ++k) {
+    Scratch tmp(st);
+    uint32_t *ext = nullptr, *off = nullptr;
+    unsigned long long* dtot = nullptr;
+    CK0(tmp.alloc(&ext, (size_t)NO)); CK0(tmp.alloc(&off, (size_t)NO)); CK0(tmp.alloc(&dtot, 1));
+    CK0(cudaMemsetAsync(dtot, 0, sizeof(unsigned long long), st));
+    assoc_ext_kernel<<<nblk(NO, 256), 256, 0, st>>>(occ_pos, end, NO, ext, dtot);
+    unsigned long long tot = 0;
+    CK0(assoc_read(dtot, st, &tot));
+    if (k <= ASSOC_MAX_LEN) tm.cand[k] = (int64_t)tot;
+    if (tot > (unsigned long long)PIO_ASSOC_MAX_CANDIDATES) {
+      tm.rejected_level = k;
+      return fail(nullptr, PIO_ALS_ERR_ARG,
+                  "the item sets of length %d have %llu candidates, more than the limit of %lld: raise minSupport, "
+                  "lower maxRuleLength or shorten basketWindow", k, tot, (long long)PIO_ASSOC_MAX_CANDIDATES);
+    }
+    if (tot == 0) break;
+    if (k > ASSOC_MAX_LEN)
+      return fail(nullptr, PIO_ALS_ERR_ARG, "item sets longer than %d items are not supported", ASSOC_MAX_LEN);
+    ++tm.levels_run;
+    const long long C = (long long)tot;
+    CK0(scan_exclusive_u32(ext, off, (size_t)NO, st, nullptr));
+    SortBufs cs;
+    uint32_t *cand_pos = nullptr, *hf = nullptr, *rix = nullptr;
+    for (int b : {0, 1}) {
+      CK0(tmp.alloc(&cs.k[b], (size_t)C));
+      CK0(tmp.alloc(&cs.v[b], (size_t)C));
+    }
+    CK0(tmp.alloc(&cand_pos, (size_t)C)); CK0(tmp.alloc(&hf, (size_t)C)); CK0(tmp.alloc(&rix, (size_t)C));
+    assoc_expand_kernel<<<nblk(NO, 256), 256, 0, st>>>(occ_pos, occ_id, ext, off, NO, p_item, bits_i, cs.keys(),
+                                                       cs.vals(), cand_pos);
+    CK0(radix_sort_pairs(cs, (size_t)C, ceil_log2((uint64_t)ln[k - 1]) + bits_i, st, nullptr));
+    cooc_head_kernel<<<nblk(C, 256), 256, 0, st>>>(cs.keys(), C, hf);
+    long long R = 0, Lk = 0;
+    CK0(assoc_total(hf, rix, C, st, &R));
+    uint64_t* rkey = nullptr;
+    uint32_t *rcnt = nullptr, *rf = nullptr, *rid = nullptr;
+    CK0(tmp.alloc(&rkey, (size_t)R)); CK0(tmp.alloc(&rcnt, (size_t)R)); CK0(tmp.alloc(&rf, (size_t)R));
+    CK0(tmp.alloc(&rid, (size_t)R));
+    assoc_runs_kernel<<<nblk(C, 256), 256, 0, st>>>(cs.keys(), hf, rix, C, thr, rkey, rcnt, rf);
+    CK0(assoc_total(rf, rid, R, st, &Lk));
+    if (Lk == 0) break;
+    if (n_sets + Lk >= (1ll << 31)) return fail(nullptr, PIO_ALS_ERR_ARG, "2^31 or more frequent item sets");
+    n_sets += Lk;
+    uint64_t* kk = nullptr;
+    uint32_t* ck = nullptr;
+    CK0(sets.alloc(&kk, (size_t)Lk)); CK0(sets.alloc(&ck, (size_t)Lk));
+    assoc_level_emit_kernel<<<nblk(R, 256), 256, 0, st>>>(rkey, rcnt, rf, rid, R, kk, ck);
+    lkeys.push_back(kk), lcount.push_back(ck), ln.push_back(Lk);
+    if (k < p->max_rule_length) {
+      uint32_t *oflag = nullptr, *opos = nullptr;
+      CK0(tmp.alloc(&oflag, (size_t)C)); CK0(tmp.alloc(&opos, (size_t)C));
+      assoc_occ_flag_kernel<<<nblk(C, 256), 256, 0, st>>>(hf, rix, rf, C, oflag);
+      long long NO2 = 0;
+      CK0(assoc_total(oflag, opos, C, st, &NO2));
+      auto next = std::make_unique<Scratch>(st);
+      uint32_t *op2 = nullptr, *oi2 = nullptr;
+      CK0(next->alloc(&op2, (size_t)NO2)); CK0(next->alloc(&oi2, (size_t)NO2));
+      assoc_occ_kernel<<<nblk(C, 256), 256, 0, st>>>(cs.vals(), cand_pos, hf, rix, rid, oflag, opos, C, op2, oi2);
+      occ_mem = std::move(next);
+      occ_pos = op2, occ_id = oi2, NO = NO2;
+    }
+    CK0(cudaGetLastError());
+    CK0(cudaStreamSynchronize(st));
+  }
+  tm.levels = lap();
+  const int K = (int)ln.size() - 1;
+  // 5. rules of every set of level k >= 2, counted per set, then written at their scanned offsets
+  AssocLevels L{};
+  for (int l = 1; l <= K; ++l) {
+    L.keys[l] = lkeys[l], L.count[l] = lcount[l], L.n[l] = (uint32_t)ln[l];
+    L.base[l] = l == 1 ? 0u : L.base[l - 1] + L.n[l - 1];
+  }
+  Scratch rules(st);
+  std::vector<uint32_t*> roff((size_t)K + 1, nullptr);
+  std::vector<long long> rbase((size_t)K + 2, 0);
+  {
+    unsigned long long* dtot = nullptr;
+    CK0(rules.alloc(&dtot, 1));
+    for (int k = 2; k <= K; ++k) {
+      uint32_t* npass = nullptr;
+      CK0(rules.alloc(&npass, (size_t)ln[k])); CK0(rules.alloc(&roff[k], (size_t)ln[k]));
+      CK0(cudaMemsetAsync(dtot, 0, sizeof(unsigned long long), st));
+      const AssocRuleArgs a{k, bits_i, (double)T, p->min_confidence, p->min_lift};
+      assoc_rule_kernel<0><<<nblk(ln[k], ASSOC_RULE_THREADS), ASSOC_RULE_THREADS, 0, st>>>(
+          L, a, npass, dtot, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr);
+      CK0(cudaGetLastError());
+      unsigned long long tot = 0;
+      CK0(assoc_read(dtot, st, &tot));
+      if ((unsigned long long)rbase[k] + tot >= (1ull << 31))
+        return fail(nullptr, PIO_ALS_ERR_ARG, "2^31 or more rules pass minConfidence and minLift");
+      CK0(scan_exclusive_u32(npass, roff[k], (size_t)ln[k], st, nullptr));
+      rbase[k + 1] = rbase[k] + (long long)tot;
+    }
+  }
+  const long long RT = K >= 2 ? rbase[K + 1] : 0;
+  uint32_t* r_cond = nullptr;
+  int* r_conseq = nullptr;
+  double *r_sup = nullptr, *r_conf = nullptr, *r_lift = nullptr;
+  CK0(rules.alloc(&r_cond, (size_t)RT)); CK0(rules.alloc(&r_conseq, (size_t)RT));
+  CK0(rules.alloc(&r_sup, (size_t)RT)); CK0(rules.alloc(&r_conf, (size_t)RT)); CK0(rules.alloc(&r_lift, (size_t)RT));
+  for (int k = 2; k <= K; ++k) {
+    if (rbase[k + 1] == rbase[k]) continue;
+    const AssocRuleArgs a{k, bits_i, (double)T, p->min_confidence, p->min_lift};
+    const long long b = rbase[k];
+    assoc_rule_kernel<1><<<nblk(ln[k], ASSOC_RULE_THREADS), ASSOC_RULE_THREADS, 0, st>>>(
+        L, a, nullptr, nullptr, roff[k], r_cond + b, r_conseq + b, r_sup + b, r_conf + b, r_lift + b);
+    CK0(cudaGetLastError());
+  }
+  CK0(cudaStreamSynchronize(st));
+  tm.rules = lap();
+  // 6. ranking per condition: lift descending, then the conseq's item index; the first maxNumRulesPerCond
+  long long RK = 0;
+  uint32_t* o_cond = nullptr;
+  int* o_conseq = nullptr;
+  double *o_sup = nullptr, *o_conf = nullptr, *o_lift = nullptr;
+  if (RT > 0) {
+    SortBufs rs;
+    for (int b : {0, 1}) {
+      CK0(rules.alloc(&rs.k[b], (size_t)RT));
+      CK0(rules.alloc(&rs.v[b], (size_t)RT));
+    }
+    assoc_rank_key_kernel<<<nblk(RT, 256), 256, 0, st>>>(nullptr, RT, 0, r_cond, r_conseq, r_lift, rs.keys(), rs.vals());
+    CK0(radix_sort_pairs(rs, (size_t)RT, bits_i, st, nullptr));
+    assoc_rank_key_kernel<<<nblk(RT, 256), 256, 0, st>>>(rs.vals(), RT, 1, r_cond, r_conseq, r_lift, rs.spare_keys(),
+                                                         rs.spare_vals());
+    rs.flip();
+    CK0(radix_sort_pairs(rs, (size_t)RT, 64, st, nullptr));
+    assoc_rank_key_kernel<<<nblk(RT, 256), 256, 0, st>>>(rs.vals(), RT, 2, r_cond, r_conseq, r_lift, rs.spare_keys(),
+                                                         rs.spare_vals());
+    rs.flip();
+    CK0(radix_sort_pairs(rs, (size_t)RT, ceil_log2((uint64_t)n_sets), st, nullptr));
+    uint32_t *ccount = nullptr, *cstart = nullptr, *kcount = nullptr, *kstart = nullptr;
+    CK0(rules.alloc(&ccount, (size_t)n_sets)); CK0(rules.alloc(&cstart, (size_t)n_sets));
+    CK0(rules.alloc(&kcount, (size_t)n_sets)); CK0(rules.alloc(&kstart, (size_t)n_sets));
+    CK0(cudaMemsetAsync(ccount, 0, 4 * (size_t)n_sets, st));
+    assoc_cond_count_kernel<<<nblk(RT, 256), 256, 0, st>>>(rs.keys(), RT, ccount);
+    CK0(scan_exclusive_u32(ccount, cstart, (size_t)n_sets, st, nullptr));
+    const uint32_t per = (uint32_t)p->max_num_rules_per_cond;
+    assoc_cond_keep_kernel<<<nblk(n_sets, 256), 256, 0, st>>>(ccount, n_sets, per, kcount);
+    CK0(assoc_total(kcount, kstart, n_sets, st, &RK));
+    CK0(rules.alloc(&o_cond, (size_t)RK)); CK0(rules.alloc(&o_conseq, (size_t)RK));
+    CK0(rules.alloc(&o_sup, (size_t)RK)); CK0(rules.alloc(&o_conf, (size_t)RK)); CK0(rules.alloc(&o_lift, (size_t)RK));
+    assoc_take_kernel<<<nblk(RT, 256), 256, 0, st>>>(rs.keys(), rs.vals(), RT, cstart, kstart, per, r_cond, r_conseq,
+                                                     r_sup, r_conf, r_lift, o_cond, o_conseq, o_sup, o_conf, o_lift);
+    CK0(cudaGetLastError());
+    CK0(cudaStreamSynchronize(st));
+  }
+  tm.rank = lap();
+  // 7. the model on the host: sets as (global id of the prefix, last item, count), rules in ranked order
+  m->level_off.assign((size_t)K + 1, 0);
+  for (int l = 1; l <= K; ++l) m->level_off[l] = m->level_off[l - 1] + ln[l];
+  m->set_prefix.resize((size_t)n_sets);
+  m->set_item.resize((size_t)n_sets);
+  m->set_count.resize((size_t)n_sets);
+  {
+    std::vector<uint64_t> hk;
+    std::vector<uint32_t> hc;
+    const uint64_t imask = (1ull << bits_i) - 1ull;
+    for (int l = 1; l <= K; ++l) {
+      hk.resize((size_t)ln[l]);
+      hc.resize((size_t)ln[l]);
+      CK0(cudaMemcpyAsync(hk.data(), lkeys[l], 8 * (size_t)ln[l], cudaMemcpyDeviceToHost, st));
+      CK0(cudaMemcpyAsync(hc.data(), lcount[l], 4 * (size_t)ln[l], cudaMemcpyDeviceToHost, st));
+      CK0(cudaStreamSynchronize(st));
+      const int64_t o = m->level_off[l - 1];
+      for (long long j = 0; j < ln[l]; ++j) {
+        m->set_prefix[o + j] = l == 1 ? -1 : m->level_off[l - 2] + (int64_t)(hk[j] >> bits_i);
+        m->set_item[o + j] = (int32_t)(l == 1 ? hk[j] : (hk[j] & imask));
+        m->set_count[o + j] = hc[j];
+      }
+    }
+  }
+  std::vector<uint32_t> hcond((size_t)RK);
+  m->rule_cond.resize((size_t)RK);
+  m->rule_conseq.resize((size_t)RK);
+  m->support.resize((size_t)RK);
+  m->confidence.resize((size_t)RK);
+  m->lift.resize((size_t)RK);
+  if (RK > 0) {
+    CK0(cudaMemcpyAsync(hcond.data(), o_cond, 4 * (size_t)RK, cudaMemcpyDeviceToHost, st));
+    CK0(cudaMemcpyAsync(m->rule_conseq.data(), o_conseq, 4 * (size_t)RK, cudaMemcpyDeviceToHost, st));
+    CK0(cudaMemcpyAsync(m->support.data(), o_sup, 8 * (size_t)RK, cudaMemcpyDeviceToHost, st));
+    CK0(cudaMemcpyAsync(m->confidence.data(), o_conf, 8 * (size_t)RK, cudaMemcpyDeviceToHost, st));
+    CK0(cudaMemcpyAsync(m->lift.data(), o_lift, 8 * (size_t)RK, cudaMemcpyDeviceToHost, st));
+    CK0(cudaStreamSynchronize(st));
+  }
+  for (long long r = 0; r < RK; ++r) m->rule_cond[r] = hcond[r];
+  tm.d2h = lap();
+  tm.total = std::chrono::duration<double, std::milli>(Clock::now() - t0).count();
+  return PIO_ALS_OK;
+}
+
+}  // namespace pio
+
+extern "C" {
+
+int pio_assoc_train(int device, const int32_t* user, const int32_t* item, const int64_t* t_ms, int64_t n,
+                    int32_t n_users, int32_t n_items, const pio_assoc_params* p, pio_assoc_model** out) {
+  if (!p || !out || n < 0 || (n > 0 && (!user || !item || !t_ms)) || n_users < 1 || n_items < 1)
+    return fail(nullptr, PIO_ALS_ERR_ARG, "bad pio_assoc_train arguments");
+  *out = nullptr;
+  EVF(assoc_check(p));
+  if (n >= (1ll << 32)) return fail(nullptr, PIO_ALS_ERR_ARG, "n must be < 2^32");
+  for (int64_t e = 0; e < n; ++e)
+    if (user[e] < 0 || user[e] >= n_users || item[e] < 0 || item[e] >= n_items)
+      return fail(nullptr, PIO_ALS_ERR_ARG, "event %lld has a user/item index out of range", (long long)e);
+  g_assoc_timing = AssocTiming();
+  try {
+    std::unique_ptr<pio_assoc_model> m(new pio_assoc_model());
+    if (n > 0) EVF(assoc_fit(device, user, item, t_ms, (long long)n, n_users, n_items, p, m.get()));
+    *out = m.release();
+  } catch (const std::bad_alloc&) {
+    return fail(nullptr, PIO_ALS_ERR_NOMEM, "pio_assoc_train: out of host memory");
+  }
+  return PIO_ALS_OK;
+}
+
+int pio_assoc_model_size(const pio_assoc_model* m, int32_t* n_levels, int64_t* n_sets, int64_t* n_rules,
+                         int64_t* n_transactions) {
+  if (!m) return fail(nullptr, PIO_ALS_ERR_ARG, "null association model");
+  if (n_levels) *n_levels = (int32_t)m->level_off.size() - 1;
+  if (n_sets) *n_sets = (int64_t)m->set_item.size();
+  if (n_rules) *n_rules = (int64_t)m->rule_conseq.size();
+  if (n_transactions) *n_transactions = m->n_transactions;
+  return PIO_ALS_OK;
+}
+
+int pio_assoc_model_get(const pio_assoc_model* m, int64_t* level_off, int64_t* set_prefix, int32_t* set_item,
+                        int64_t* set_count, int64_t* rule_cond, int32_t* rule_conseq, double* support,
+                        double* confidence, double* lift) {
+  if (!m) return fail(nullptr, PIO_ALS_ERR_ARG, "null association model");
+  auto put = [](auto* dst, const auto& v) {
+    if (dst && !v.empty()) memcpy(dst, v.data(), v.size() * sizeof(v[0]));
+  };
+  put(level_off, m->level_off);
+  put(set_prefix, m->set_prefix);
+  put(set_item, m->set_item);
+  put(set_count, m->set_count);
+  put(rule_cond, m->rule_cond);
+  put(rule_conseq, m->rule_conseq);
+  put(support, m->support);
+  put(confidence, m->confidence);
+  put(lift, m->lift);
+  return PIO_ALS_OK;
+}
+
+int pio_assoc_model_destroy(pio_assoc_model* m) {
+  delete m;
+  return PIO_ALS_OK;
+}
+
+/* debug only (not in pio_als.h): the last pio_assoc_train on this thread, wall ms of phases that each end in a stream
+ * synchronise: out[0] host-to-device copy, [1] baskets, [2] level 1 and the pruned baskets, [3] levels >= 2, [4] rules,
+ * [5] ranking, [6] device-to-host copy and the host model, [7] total; [8] baskets before minBasketSize, [9]
+ * transactions T, [10] levels >= 2 enumerated, [11] the level rejected by the candidate limit (0: none); [16 + k]
+ * candidates counted for level k (2 <= k <= 32).  Used by tools/assoc_bench.py and tests/test_gpu_assoc.py. */
+__attribute__((visibility("default"))) int pio_assoc_debug_timing(double out[64]) {
+  if (!out) return PIO_ALS_ERR_ARG;
+  const AssocTiming& t = g_assoc_timing;
+  out[0] = t.h2d, out[1] = t.baskets, out[2] = t.level1, out[3] = t.levels, out[4] = t.rules, out[5] = t.rank;
+  out[6] = t.d2h, out[7] = t.total;
+  out[8] = (double)t.n_baskets, out[9] = (double)t.n_transactions, out[10] = (double)t.levels_run;
+  out[11] = (double)t.rejected_level;
+  for (int k = 12; k < 16; ++k) out[k] = 0;
+  for (int k = 0; k <= ASSOC_MAX_LEN; ++k) out[16 + k] = (double)t.cand[k];
+  for (int k = 16 + ASSOC_MAX_LEN + 1; k < 64; ++k) out[k] = 0;
   return PIO_ALS_OK;
 }
 

@@ -46,7 +46,8 @@ EXPORTED_SYMBOLS = [
     "pio_cls_folds_rf_predict", "pio_cls_folds_result_labels", "pio_cls_folds_result_counts",
     "pio_cls_folds_result_free", "pio_cls_folds_destroy", "pio_cooc_model_create", "pio_cooc_model_destroy",
     "pio_cooc_predict_filtered", "pio_cooc_model_get_stats", "pio_serve_zscore_merge", "pio_popular_model_create",
-    "pio_popular_predict_filtered", "pio_popular_model_get_stats", "pio_popular_model_destroy",
+    "pio_popular_predict_filtered", "pio_popular_model_get_stats", "pio_popular_model_destroy", "pio_assoc_train",
+    "pio_assoc_model_size", "pio_assoc_model_get", "pio_assoc_model_destroy",
 ]
 
 
@@ -1274,6 +1275,67 @@ def rf_train_paths() -> dict:
     _check(lib().pio_rf_debug_paths(out))
     keys = ("bin_bytes", "staged", "smem_launches", "global_launches", "max_chunks", "max_passes", "levels", "groups")
     return {k: int(v) for k, v in zip(keys, out)}
+
+
+class AssocParams(C.Structure):
+    """pio_assoc_params"""
+    _fields_ = [("basket_window", C.c_int32), ("max_rule_length", C.c_int32), ("min_support", C.c_double),
+                ("min_confidence", C.c_double), ("min_lift", C.c_double), ("min_basket_size", C.c_int32),
+                ("max_num_rules_per_cond", C.c_int32)]
+
+
+ASSOC_MAX_CANDIDATES = 1 << 29   # PIO_ASSOC_MAX_CANDIDATES
+
+
+def assoc_train(user, item, t_ms, n_users, n_items, basket_window, max_rule_length, min_support, min_confidence,
+                min_lift, min_basket_size, max_num_rules_per_cond, device=0) -> dict:
+    """pio_assoc_train: the complementary purchase template's association rules from buy events (user / item indices,
+    t_ms milliseconds).  Returns flat arrays: level_off (int64 [n_levels + 1]); per frequent set set_prefix (int64, -1
+    for one item), set_item (int32, the set's largest item) and set_count (int64); per rule, grouped by cond and
+    ranked, rule_cond (int64 set index), rule_conseq (int32), support, confidence and lift (float64); and
+    n_transactions."""
+    user = np.ascontiguousarray(user, np.int32)
+    item = np.ascontiguousarray(item, np.int32)
+    t_ms = np.ascontiguousarray(t_ms, np.int64)
+    n = user.shape[0]
+    if item.shape != (n,) or t_ms.shape != (n,):
+        raise ValueError("user, item and t_ms must have one entry per event")
+    p = AssocParams(int(basket_window), int(max_rule_length), float(min_support), float(min_confidence),
+                    float(min_lift), int(min_basket_size), int(max_num_rules_per_cond))
+    h = C.c_void_p()
+    vp = C.c_void_p
+    _check(lib().pio_assoc_train(C.c_int(device), vp(_addr(user)), vp(_addr(item)), vp(_addr(t_ms)), C.c_int64(n),
+                                 C.c_int32(n_users), C.c_int32(n_items), C.byref(p), C.byref(h)))
+    try:
+        nl, ns, nr, nt = C.c_int32(0), C.c_int64(0), C.c_int64(0), C.c_int64(0)
+        _check(lib().pio_assoc_model_size(h, C.byref(nl), C.byref(ns), C.byref(nr), C.byref(nt)))
+        out = {"level_off": np.zeros(nl.value + 1, np.int64), "set_prefix": np.empty(ns.value, np.int64),
+               "set_item": np.empty(ns.value, np.int32), "set_count": np.empty(ns.value, np.int64),
+               "rule_cond": np.empty(nr.value, np.int64), "rule_conseq": np.empty(nr.value, np.int32),
+               "support": np.empty(nr.value, np.float64), "confidence": np.empty(nr.value, np.float64),
+               "lift": np.empty(nr.value, np.float64)}
+        _check(lib().pio_assoc_model_get(h, *[vp(_addr(out[k])) for k in ASSOC_ARRAYS]))
+    finally:
+        lib().pio_assoc_model_destroy(h)
+    out["n_transactions"] = int(nt.value)
+    return out
+
+
+ASSOC_ARRAYS = ("level_off", "set_prefix", "set_item", "set_count", "rule_cond", "rule_conseq", "support", "confidence",
+                "lift")
+
+
+def assoc_train_timing() -> dict:
+    """Where the last assoc_train on this thread spent its time (wall ms of phases that each end in a device
+    synchronise), the baskets before minBasketSize, the transactions, the levels >= 2 enumerated, the level the
+    candidate limit rejected (0: none) and the candidates counted for each level k >= 2."""
+    out = (C.c_double * 64)()
+    _check(lib().pio_assoc_debug_timing(out))
+    keys = ("h2d_ms", "baskets_ms", "level1_ms", "levels_ms", "rules_ms", "rank_ms", "d2h_ms", "total_ms")
+    res = {k: out[j] for j, k in enumerate(keys)}
+    res.update(baskets=int(out[8]), transactions=int(out[9]), levels_run=int(out[10]), rejected_level=int(out[11]),
+               candidates={k: int(out[16 + k]) for k in range(2, 33) if out[16 + k]})
+    return res
 
 
 def nb_predict(x, pi, theta, device=0):
