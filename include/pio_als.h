@@ -630,6 +630,7 @@ PIO_API int pio_nb_predict(int device, const float* x, int64_t n, int n_feat, in
  * of MLlib's GiniAggregator / EntropyAggregator, a non-finite label or feature is rejected. */
 #define PIO_RF_GINI 0
 #define PIO_RF_ENTROPY 1
+#define PIO_RF_VARIANCE 2               /* pio_rf_train_regressor only */
 
 typedef struct pio_rf_params {
   int32_t num_classes;                  /* >= 2 */
@@ -657,6 +658,37 @@ PIO_API int pio_rf_forest_get(const pio_rf_forest* f, int32_t* tree_off, int32_t
                               int32_t* left, int32_t* right, int32_t* prediction, double* impurity, double* gain,
                               int64_t* count);
 PIO_API int pio_rf_forest_destroy(pio_rf_forest* f);
+
+/* RandomForest.trainRegressor (rules: tests/forest_reg_ref.py): params->impurity must be PIO_RF_VARIANCE (gini and
+ * entropy are refused with MLlib's message), num_classes is ignored, and featureSubsetStrategy "auto" means all features
+ * for one tree and onethird for more.  arity: n_feat entries, 0 for a continuous feature, else its number of categories
+ * (>= 2, at most min(max_bins, n)); a categorical feature's values must lie in [0, arity) and its bin is trunc(value);
+ * arity == NULL: every feature is continuous.  label: n finite values, the largest |label| 0 or in [2^-256, 2^256).
+ * Labels are quantised to integers (|yq| <= 2^44) so that every sum is exact and the forest does not depend on the order
+ * of device atomics.  Every check runs before any device work.  The forest is read with pio_rf_forest_size /
+ * pio_rf_forest_get (prediction: all 0) and pio_rf_forest_reg_get. */
+PIO_API int pio_rf_train_regressor(int device, const pio_rf_params* params, const int32_t* arity, const double* label,
+                                   const double* x, int64_t n, int32_t n_feat, pio_rf_forest** out);
+/* What a regression forest adds: the number of left-category ids over all nodes (PIO_ALS_ERR_ARG for a classifier). */
+PIO_API int pio_rf_forest_reg_size(const pio_rf_forest* f, int64_t* n_cat_ids);
+/* Per node: value (its mean label, the prediction of a leaf); cat_off [n_nodes + 1] and cat_ids: the left categories of
+ * a categorical node (x goes left iff x equals one of them), ascending, none for a leaf or a continuous node (which
+ * sends x <= threshold left).  Any output pointer may be null. */
+PIO_API int pio_rf_forest_reg_get(const pio_rf_forest* f, double* value, int64_t* cat_off, int32_t* cat_ids);
+/* The forest's mean prediction for n rows x (n x n_feat fp64, HOST) into out: the trees' predictions summed in tree
+ * order from 0.0, divided by n_trees.  The forest is given as pio_rf_forest_get / pio_rf_forest_reg_get return it. */
+PIO_API int pio_rf_predict_regression(int device, int32_t n_trees, const int32_t* tree_off, int64_t n_nodes,
+                                      const int32_t* feature, const double* threshold, const int32_t* left,
+                                      const int32_t* right, const double* value, const int64_t* cat_off,
+                                      const int32_t* cat_ids, const double* x, int64_t n, int32_t n_feat, double* out);
+
+/* The lead scoring template's sessions from its view and buy events (rules: tests/leadscoring_ref.py): session[r] in
+ * [0, n_sessions) is event r's session, is_buy[r] 0 for a view and 1 for a buy, t_ms[r] its time in milliseconds.  Per
+ * session: landing[s] the event index of its landing view, the earliest view, and among equally early views the last in
+ * event order (-1: the session has no view); buy[s] 1 iff some buy of the session is strictly after the landing view.
+ * HOST buffers; the arguments are checked before any device work. */
+PIO_API int pio_lead_sessions(int device, const int32_t* session, const uint8_t* is_buy, const int64_t* t_ms, int64_t n,
+                              int32_t n_sessions, int64_t* landing, uint8_t* buy);
 /* The forest's majority vote (ties to the smaller class) for n rows x (n x n_feat fp64, HOST) into out (class index),
  * from the flat arrays of pio_rf_forest_get. */
 PIO_API int pio_rf_predict(int device, int32_t n_trees, const int32_t* tree_off, int64_t n_nodes, const int32_t* feature,

@@ -28,7 +28,9 @@ constexpr int RF_MAX_CLASSES = 64;
 constexpr int RF_MAX_BINS = 65536;
 constexpr int RF_MAX_DEPTH = 30;
 constexpr int RF_POISSON_N = 16;        // weights are capped at 16: the table holds P(X <= k) for k = 0 .. 15
-constexpr int RF_GINI = 0, RF_ENTROPY = 1;
+constexpr int RF_GINI = 0, RF_ENTROPY = 1, RF_VARIANCE = 2;
+constexpr int RF_LABEL_BITS = 44;       // the regressor's quantised labels: |yq| <= 2^44 (tests/forest_reg_ref.py)
+constexpr int RF_LABEL_EXP_MAX = 256;   // its labels: |y| < 2^256, and max |y| >= 2^-256 unless every label is 0
 
 // stream tags of the counter hash
 constexpr uint64_t RF_TAG_SAMPLE = 1, RF_TAG_BAG = 2, RF_TAG_SUBSET = 3;
@@ -187,6 +189,27 @@ inline double rf_impurity(const int64_t* c, int n_class, int kind) {
   }
   return imp;
 }
+// Variance.calculate on fp64 statistics: (Q - S * S / W) / W, 0 for an empty node
+inline double rf_variance(double W, double S, double Q) {
+  if (W == 0.0) return 0.0;
+  const double ss = S * S;
+  const double m = ss / W;
+  const double d = Q - m;
+  return d / W;
+}
+// the regressor's featureSubsetStrategy: "auto" is all features for one tree and onethird for more
+inline int rf_subset_size_reg(const char* s, int n_feat, int num_trees) {
+  if (s && !strcmp(s, "auto")) s = num_trees == 1 ? "all" : "onethird";
+  return rf_subset_size(s, n_feat, num_trees);
+}
+// the regressor's label shift: s puts max |y| in [2^43, 2^44); 0 when every label is 0
+inline int rf_label_shift(double max_abs) {
+  if (max_abs == 0.0) return 0;
+  int e = 0;
+  frexp(max_abs, &e);
+  return RF_LABEL_BITS - e;
+}
+
 // the class with the largest count, ties to the smaller class
 inline int rf_argmax(const int64_t* c, int n_class) {
   int b = 0;

@@ -58,6 +58,7 @@
 #include "popular.cuh"
 #include "serve_merge.cuh"
 #include "forest.cuh"
+#include "sessions.cuh"
 #include "eval_folds.cuh"
 #include "cls_folds.cuh"
 #include "assoc.cuh"
@@ -5309,6 +5310,10 @@ struct pio_rf_forest {
   std::vector<int32_t> tree_off, feature, left, right, prediction;
   std::vector<double> threshold, impurity, gain;
   std::vector<int64_t> count;
+  bool regression = false;              // pio_rf_train_regressor: the fields below, prediction all 0
+  std::vector<double> value;            // per node: its mean label
+  std::vector<int64_t> cat_off;         // [n_nodes + 1] left categories of each categorical node ...
+  std::vector<int32_t> cat_ids;         // ... ascending
 };
 
 }  // extern "C"
@@ -5337,6 +5342,8 @@ struct RfRec {
   double thr, imp, gain;
   int pred;
   int64_t count;
+  double value;                         // regressor: the node's mean label
+  std::vector<int32_t> cats;            // regressor: left categories of a categorical split, ascending
 };
 using RfTree = std::map<int64_t, RfRec>;
 
@@ -5407,6 +5414,59 @@ static int rf_check_params(const pio_rf_params* p, int64_t n, int F) {
   return PIO_ALS_OK;
 }
 
+// the regressor's checks (tests/forest_reg_ref.py check_args / check_data), all before any device work; *shift: s
+static int rf_check_reg(const pio_rf_params* p, const int32_t* arity, const double* label, const double* x, int64_t n,
+                        int F, int* shift) {
+  if (p->impurity != RF_VARIANCE) {
+    if (p->impurity == RF_GINI || p->impurity == RF_ENTROPY)
+      return fail(nullptr, PIO_ALS_ERR_ARG, "DecisionTree Strategy given invalid impurity for Regression: %s.  Valid "
+                  "settings: Variance", p->impurity == RF_GINI ? "gini" : "entropy");
+    return fail(nullptr, PIO_ALS_ERR_ARG, "unknown impurity code %d", p->impurity);
+  }
+  for (int f = 0; arity && f < F; ++f)
+    if (arity[f] != 0 && arity[f] < 2)
+      return fail(nullptr, PIO_ALS_ERR_ARG, "DecisionTree Strategy given invalid categoricalFeaturesInfo setting: "
+                  "feature %d has %d categories.  The number of categories should be >= 2.", f, arity[f]);
+  if (p->num_trees < 1)
+    return fail(nullptr, PIO_ALS_ERR_ARG, "RandomForest requires numTrees > 0, but was given numTrees = %d.",
+                p->num_trees);
+  if (rf_subset_size_reg(p->feature_subset_strategy, F > 1 ? F : 1, p->num_trees) == 0)
+    return fail(nullptr, PIO_ALS_ERR_ARG, "RandomForest given invalid featureSubsetStrategy: %s. Supported values: "
+                "auto, all, onethird, sqrt, log2, (0.0-1.0], [1-n].",
+                p->feature_subset_strategy ? p->feature_subset_strategy : "null");
+  pio_rf_params q = *p;                                   // the classifier's remaining numeric and shape checks
+  q.num_classes = 2, q.impurity = RF_GINI, q.feature_subset_strategy = "all";
+  EVF(rf_check_params(&q, n, F));
+  if (!label || !x) return fail(nullptr, PIO_ALS_ERR_ARG, "bad pio_rf_train_regressor arguments");
+  for (int64_t r = 0; r < n; ++r) EVF(rf_fail_finite(r, label[r], x + r * F, F));
+  double m = 0.0;
+  int64_t rm = 0;
+  for (int64_t r = 0; r < n; ++r)
+    if (fabs(label[r]) > m) m = fabs(label[r]), rm = r;
+  if (m >= ldexp(1.0, RF_LABEL_EXP_MAX) || (m > 0.0 && m < ldexp(1.0, -RF_LABEL_EXP_MAX)))
+    return fail(nullptr, PIO_ALS_ERR_ARG, "label of row %lld is out of range (%s): the largest |label| must be 0 or in "
+                "[2^-%d, 2^%d).", (long long)rm, rf_fmt(label[rm]).c_str(), RF_LABEL_EXP_MAX, RF_LABEL_EXP_MAX);
+  *shift = rf_label_shift(m);
+  if (!arity) return PIO_ALS_OK;
+  int amax = 0, fmax = -1;
+  for (int f = 0; f < F; ++f)
+    if (arity[f] > amax) amax = arity[f], fmax = f;
+  const int64_t nb = std::min<int64_t>(p->max_bins, n);
+  if (amax > nb)
+    return fail(nullptr, PIO_ALS_ERR_ARG, "DecisionTree requires maxBins (= %lld) to be at least as large as the number "
+                "of values in each categorical feature, but categorical feature %d has %d values. Consider removing "
+                "this and other categorical features with a large number of values, or add more training examples.",
+                (long long)nb, fmax, amax);
+  for (int64_t r = 0; r < n; ++r)
+    for (int f = 0; f < F; ++f) {
+      const double v = x[r * F + f];
+      if (arity[f] > 0 && !(v >= 0.0 && v < (double)arity[f]))
+        return fail(nullptr, PIO_ALS_ERR_ARG, "DecisionTree given invalid data: Feature %d is categorical with values "
+                    "in {0,...,%d}, but a data point gives it value %s.", f, arity[f] - 1, rf_fmt(v).c_str());
+    }
+  return PIO_ALS_OK;
+}
+
 static int rf_check(const pio_rf_params* p, const double* label, const double* x, int64_t n, int F) {
   EVF(rf_check_params(p, n, F));
   if (!label || !x) return fail(nullptr, PIO_ALS_ERR_ARG, "bad pio_rf_train arguments");
@@ -5424,11 +5484,16 @@ static double rf_ms(std::chrono::steady_clock::time_point& t0) {
 
 // LearningNode.toNode(prune = true): an internal node whose two children end as leaves with the same prediction becomes
 // a leaf; returns the node's prediction
+// (the regressor compares its fp64 predictions with ==; the collapsed leaf keeps the left child's)
 static int rf_prune(RfTree& t, int64_t i) {
   RfRec& r = t[i];
   if (r.leaf) return r.pred;
   const int a = rf_prune(t, 2 * i), b = rf_prune(t, 2 * i + 1);
-  if (t[2 * i].leaf && t[2 * i + 1].leaf && a == b) r.leaf = true, r.pred = a, r.feature = -1, r.thr = 0.0, r.gain = 0.0;
+  const RfRec &L = t[2 * i], &R = t[2 * i + 1];
+  if (L.leaf && R.leaf && a == b && L.value == R.value) {
+    r.leaf = true, r.pred = a, r.value = L.value, r.feature = -1, r.thr = 0.0, r.gain = 0.0;
+    r.cats.clear();
+  }
   return r.pred;
 }
 // preorder: the node, its left subtree, its right subtree; returns the node's index in the flat arrays
@@ -5443,6 +5508,11 @@ static int32_t rf_emit(const RfTree& t, int64_t i, pio_rf_forest* o) {
   o->impurity.push_back(r.imp);
   o->gain.push_back(r.leaf ? 0.0 : r.gain);
   o->count.push_back(r.count);
+  if (o->regression) {
+    o->value.push_back(r.value);
+    if (!r.leaf) o->cat_ids.insert(o->cat_ids.end(), r.cats.begin(), r.cats.end());
+    o->cat_off.push_back((int64_t)o->cat_ids.size());
+  }
   if (!r.leaf) {
     const int32_t l = rf_emit(t, 2 * i, o);
     o->left[me] = l;
@@ -5466,10 +5536,158 @@ struct RfCtx {
   const int* dnthr;
   const std::vector<std::vector<double>>* thr;
   pio_rf_forest* out;
+  // the regressor (else nullptr / empty): quantised labels, categories per feature (0: continuous), 2^-s and 2^-2s
+  const long long* dyq;
+  const int* darity;
+  const std::vector<int>* arity;
+  double scale1, scale2;
 };
 
-// bin codes, then every tree group level by level
+// the fp64 statistics of integer sums (tests/forest_reg_ref.py to_f64), and the node record they give
+static RfRec rf_var_rec(const unsigned long long* e, double scale1, double scale2) {
+  const unsigned __int128 sq = ((unsigned __int128)e[2] << 64) | e[1], qq = ((unsigned __int128)e[4] << 64) | e[3];
+  const double W = (double)e[0], S = (double)(__int128)sq * scale1, Q = (double)qq * scale2;
+  RfRec r{true, -1, 0.0, rf_variance(W, S, Q), 0.0, 0, (int64_t)e[0]};
+  r.value = W == 0.0 ? 0.0 : S / W;
+  return r;
+}
+
+using RfActive = std::vector<std::pair<int, int64_t>>;   // (tree of the group, heap index) of each slot of a level
+
+// The regressor's split selection for the slots [c0, c1) of a level whose histogram chunk is in dhist: the centroid
+// order of wide categorical features, select_var_kernel, then on the host each slot's first maximum over its subset
+// features (hbest[S * K + s]: its subset position, -1 for none) and, for a categorical split, its left categories
+// (hcats[s], ascending), read before the next chunk overwrites the split order.
+static int rf_select_var(const RfCtx& c, int level, const RfActive& active, const std::vector<int>& hsub, int64_t c0,
+                         int64_t c1, const unsigned long long* dhist, const int* dsub, uint32_t* dorder, double* dcen,
+                         int2* dseg, double* dgain, int* dbest, unsigned long long* dleft, unsigned long long* dtot,
+                         std::vector<double>& hgain, std::vector<int>& hbest,
+                         std::vector<std::vector<int32_t>>& hcats) {
+  const int K = c.K, NB = c.NB;
+  const int64_t S = (int64_t)active.size();
+  const cudaStream_t st = c.st;
+  const std::vector<int>& ar = *c.arity;
+  std::vector<int2> seg;
+  int amax = 0;
+  for (int64_t s = c0; s < c1; ++s)
+    for (int kk = 0; kk < K; ++kk) {
+      const int f = hsub[(size_t)s * K + kk];
+      if (ar[f] > rf::CAT_SMEM_ARITY) seg.push_back(make_int2((int)(s - c0), kk)), amax = std::max(amax, ar[f]);
+    }
+  if (!seg.empty()) {
+    CK0(cudaMemcpyAsync(dseg, seg.data(), sizeof(int2) * seg.size(), cudaMemcpyHostToDevice, st));
+    const dim3 g((unsigned)((amax + 255) / 256), (unsigned)seg.size());
+    rf::cat_centroid_kernel<<<g, 256, 0, st>>>(dhist, dseg, dsub, c.darity, K, NB, (int)c0, c.scale1, dcen);
+    rf::cat_rank_kernel<<<g, 256, 0, st>>>(dcen, dseg, dsub, c.darity, K, NB, (int)c0, dorder);
+  }
+  rf::VarSelArgs sa{dhist, dsub, c.dnthr, c.darity, dorder, dgain, dbest, dleft, dtot, c.scale1, c.scale2, K, NB,
+                    (int)c0, (int)c0};
+  rf::select_var_kernel<<<(unsigned)((c1 - c0) * K), rf::SEL_WARPS * 32, 0, st>>>(sa);
+  CK0(cudaGetLastError());
+  const size_t m = (size_t)(c1 - c0) * K;
+  CK0(cudaMemcpyAsync(&hgain[c0 * K], dgain + c0 * K, 8 * m, cudaMemcpyDeviceToHost, st));
+  CK0(cudaMemcpyAsync(&hbest[c0 * K], dbest + c0 * K, 4 * m, cudaMemcpyDeviceToHost, st));
+  CK0(cudaStreamSynchronize(st));
+  for (int64_t s = c0; s < c1; ++s) {
+    int pick = -1;
+    for (int kk = 0; kk < K; ++kk)                       // the first maximum: earlier subset features win ties
+      if (hbest[s * K + kk] >= 0 && (pick < 0 || hgain[s * K + kk] > hgain[s * K + pick])) pick = kk;
+    hbest[S * K + s] = pick;
+    if (pick < 0 || !(hgain[s * K + pick] > 0.0) || level == c.p->max_depth) continue;
+    const int f = hsub[(size_t)s * K + pick], j = hbest[s * K + pick];
+    if (ar[f] == 0) continue;
+    hcats[s].resize((size_t)j + 1);
+    CK0(cudaMemcpyAsync(hcats[s].data(), dorder + ((s - c0) * K + pick) * (int64_t)NB, 4 * ((size_t)j + 1),
+                        cudaMemcpyDeviceToHost, st));
+  }
+  CK0(cudaStreamSynchronize(st));
+  for (int64_t s = c0; s < c1; ++s) std::sort(hcats[s].begin(), hcats[s].end());
+  return PIO_ALS_OK;
+}
+
+// The regressor's decisions for a level (tests/forest_reg_ref.py _decide): node records, leaves, children, the next
+// level's slots (`next`) and the rows' moves (update_kernel<BinT, true>, with a bit mask per categorical split).
 template <typename BinT>
+static int rf_decide_var(const RfCtx& c, int level, const RfActive& active, const std::vector<int>& hsub,
+                         const std::vector<double>& hgain, const std::vector<int>& hbest,
+                         const std::vector<std::vector<int32_t>>& hcats, const unsigned long long* dleft,
+                         const unsigned long long* dtot, int* dnode, const BinT* dbins, int G, unsigned ugrid, Scratch& lv,
+                         std::vector<RfTree>& trees, std::chrono::steady_clock::time_point& t0, RfActive& next) {
+  const int K = c.K, W = rf::VAR_WORDS, max_depth = c.p->max_depth;
+  const int64_t S = (int64_t)active.size();
+  const cudaStream_t st = c.st;
+  std::vector<unsigned long long> hleft((size_t)S * K * W), htot((size_t)S * W);
+  CK0(cudaMemcpyAsync(hleft.data(), dleft, 8 * hleft.size(), cudaMemcpyDeviceToHost, st));
+  CK0(cudaMemcpyAsync(htot.data(), dtot, 8 * htot.size(), cudaMemcpyDeviceToHost, st));
+  CK0(cudaStreamSynchronize(st));
+  std::vector<int4> upd(S);
+  std::vector<long long> moff(S, -1);
+  std::vector<uint32_t> mask;
+  for (int64_t s = 0; s < S; ++s) {
+    const int g = active[s].first;
+    const int64_t i = active[s].second;
+    const unsigned long long* tot = &htot[(size_t)s * W];
+    RfRec rec = rf_var_rec(tot, c.scale1, c.scale2);
+    const int kk = hbest[S * K + s];
+    if (kk < 0 || !(hgain[s * K + kk] > 0.0) || level == max_depth) {
+      trees[g][i] = rec;
+      upd[s] = make_int4(-1, 0, -1, -1);
+      continue;
+    }
+    const int f = hsub[(size_t)s * K + kk], j = hbest[s * K + kk], ar = (*c.arity)[f];
+    rec.leaf = false, rec.feature = f, rec.gain = hgain[s * K + kk];
+    if (ar > 0) {
+      rec.cats = hcats[s];
+      moff[s] = (long long)mask.size();
+      mask.resize(mask.size() + (size_t)(ar + 31) / 32, 0u);
+      for (int32_t cat : rec.cats) mask[moff[s] + (cat >> 5)] |= 1u << (cat & 31);
+    } else {
+      rec.thr = (*c.thr)[f][j];
+    }
+    trees[g][i] = rec;
+    unsigned long long side_st[2][rf::VAR_WORDS];
+    const unsigned long long* L = &hleft[((size_t)s * K + kk) * W];
+    memcpy(side_st[0], L, sizeof side_st[0]);
+    const unsigned __int128 ts = ((unsigned __int128)tot[2] << 64) | tot[1], tq = ((unsigned __int128)tot[4] << 64) | tot[3];
+    const unsigned __int128 ls = ((unsigned __int128)L[2] << 64) | L[1], lq = ((unsigned __int128)L[4] << 64) | L[3];
+    const unsigned __int128 rs = ts - ls, rq = tq - lq;
+    side_st[1][0] = tot[0] - L[0];
+    side_st[1][1] = (unsigned long long)rs, side_st[1][2] = (unsigned long long)(rs >> 64);
+    side_st[1][3] = (unsigned long long)rq, side_st[1][4] = (unsigned long long)(rq >> 64);
+    int child_slot[2];
+    for (int side = 0; side < 2; ++side) {
+      const RfRec cr = rf_var_rec(side_st[side], c.scale1, c.scale2);
+      const int64_t child = 2 * i + side;
+      if (level + 1 == max_depth || cr.imp == 0.0) {
+        trees[g][child] = cr;
+        child_slot[side] = -1;
+      } else {
+        child_slot[side] = (int)next.size();
+        next.push_back({g, child});
+      }
+    }
+    upd[s] = make_int4(f, j, child_slot[0], child_slot[1]);
+  }
+  if (!next.empty()) {
+    int4* dupd = nullptr;
+    long long* dmoff = nullptr;
+    uint32_t* dmask = nullptr;
+    CK0(lv.alloc(&dupd, (size_t)S));
+    CK0(lv.alloc(&dmoff, (size_t)S));
+    CK0(lv.alloc(&dmask, std::max<size_t>(1, mask.size())));
+    CK0(cudaMemcpyAsync(dupd, upd.data(), sizeof(int4) * (size_t)S, cudaMemcpyHostToDevice, st));
+    CK0(cudaMemcpyAsync(dmoff, moff.data(), 8 * (size_t)S, cudaMemcpyHostToDevice, st));
+    if (!mask.empty()) CK0(cudaMemcpyAsync(dmask, mask.data(), 4 * mask.size(), cudaMemcpyHostToDevice, st));
+    rf::update_kernel<BinT, true><<<ugrid, rf::THREADS, 0, st>>>(dnode, c.n, G, dbins, c.F, dupd, dmoff, dmask);
+    CK0(cudaGetLastError());
+    CK0(cudaStreamSynchronize(st));
+    g_rf_timing.upd += rf_ms(t0);
+  }
+  return PIO_ALS_OK;
+}
+
+// bin codes, then every tree group level by level; REG: the regressor's statistics and splits (forest.cuh)
+template <typename BinT, bool REG = false>
 static int rf_bin_and_grow(const RfCtx& c) {
   CallMem& tmp = *c.tmp;
   const cudaStream_t st = c.st;
@@ -5485,7 +5703,8 @@ static int rf_bin_and_grow(const RfCtx& c) {
   const size_t thr_bytes = sizeof(double) * (size_t)hoff[F];
   const int staged = thr_bytes <= 48 * 1024 ? 1 : 0;
   const unsigned bgrid = (unsigned)std::min<int64_t>(nblk(n * F, rf::THREADS), (int64_t)c.sm * 16);
-  rf::bin_kernel<BinT><<<bgrid, rf::THREADS, staged ? thr_bytes : 0, st>>>(c.dx, n, F, c.dthr, c.doff, staged, dbins);
+  rf::bin_kernel<BinT><<<bgrid, rf::THREADS, staged ? thr_bytes : 0, st>>>(c.dx, n, F, c.dthr, c.doff, staged, dbins,
+                                                                           c.darity);
   CK0(cudaGetLastError());
   CK0(cudaStreamSynchronize(st));
   tm.bin = rf_ms(t0);
@@ -5505,11 +5724,19 @@ static int rf_bin_and_grow(const RfCtx& c) {
   CK0(tmp.device(&dbag, (size_t)gmax));
   rf::Cdf cdf;
   rf_poisson_table(cdf.v);
-  const int64_t slot_bytes = (int64_t)K * NB * C * 8, smem_slot = (int64_t)K * NB * C * 4;
-  const int64_t chunk_max = std::max<int64_t>(1, hist_budget / slot_bytes);
+  // a histogram entry: C class counts (8 bytes global, 4 in shared memory), or one variance entry of 5 words in both
+  const int64_t slot_bytes = REG ? (int64_t)K * NB * rf::VAR_WORDS * 8 : (int64_t)K * NB * C * 8;
+  const int64_t smem_slot = REG ? slot_bytes : (int64_t)K * NB * C * 4;
+  bool any_cat = false, wide_cat = false;
+  if (REG)
+    for (int a : *c.arity) any_cat |= a > 0, wide_cat |= a > rf::CAT_SMEM_ARITY;
+  // the regressor's chunk also holds the split order (4 bytes per bin) and, for wide categorical features, the centroids
+  // (8 bytes per bin) of each slot
+  const int64_t chunk_slot_bytes = slot_bytes + (any_cat ? (int64_t)K * NB * 4 : 0) + (wide_cat ? (int64_t)K * NB * 8 : 0);
+  const int64_t chunk_max = std::max<int64_t>(1, hist_budget / chunk_slot_bytes);
   const int64_t pass_slots = RF_SMEM / smem_slot;
   if (pass_slots >= 1) {
-    CK0(cudaFuncSetAttribute(rf::hist_kernel<BinT, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, RF_SMEM));
+    CK0(cudaFuncSetAttribute(rf::hist_kernel<BinT, true, REG>, cudaFuncAttributeMaxDynamicSharedMemorySize, RF_SMEM));
   }
   const unsigned ugrid = (unsigned)std::min<int64_t>(nblk(n * gmax, rf::THREADS), (int64_t)c.sm * 16);
   tm.groups = (int)groups.size();
@@ -5535,12 +5762,26 @@ static int rf_bin_and_grow(const RfCtx& c) {
       long long *dleft = nullptr, *dtot = nullptr;
       unsigned long long* dhist = nullptr;
       const int64_t cap = std::min<int64_t>(S, chunk_max);
+      // the classifier: best split and class counts per slot; the regressor: the best split of every subset feature,
+      // variance entries, and the split order of categorical features
+      const int64_t per_sel = REG ? K : 1, words = REG ? rf::VAR_WORDS : C;
       CK0(lv.alloc(&dsub, (size_t)S * K));
-      CK0(lv.alloc(&dbest, (size_t)S * 2));
-      CK0(lv.alloc(&dgain, (size_t)S));
-      CK0(lv.alloc(&dleft, (size_t)S * C));
-      CK0(lv.alloc(&dtot, (size_t)S * C));
-      CK0(lv.alloc(&dhist, (size_t)cap * K * NB * C));
+      CK0(lv.alloc(&dbest, (size_t)S * per_sel * 2));
+      CK0(lv.alloc(&dgain, (size_t)S * per_sel));
+      CK0(lv.alloc(&dleft, (size_t)S * per_sel * words));
+      CK0(lv.alloc(&dtot, (size_t)S * words));
+      CK0(lv.alloc(&dhist, (size_t)cap * K * NB * words));
+      uint32_t* dorder = nullptr;
+      double* dcen = nullptr;
+      int2* dseg = nullptr;
+      if (REG && any_cat) CK0(lv.alloc(&dorder, (size_t)cap * K * NB));
+      if (REG && wide_cat) {
+        CK0(lv.alloc(&dcen, (size_t)cap * K * NB));
+        CK0(lv.alloc(&dseg, (size_t)cap * K));
+      }
+      std::vector<double> hgain(S * per_sel);
+      std::vector<int> hbest(2 * S * per_sel);
+      std::vector<std::vector<int32_t>> hcats(REG ? S : 0);
       CK0(cudaMemcpyAsync(dsub, hsub.data(), 4 * hsub.size(), cudaMemcpyHostToDevice, st));
       CK0(cudaStreamSynchronize(st));
       rf_ms(t0);
@@ -5549,7 +5790,7 @@ static int rf_bin_and_grow(const RfCtx& c) {
         const int64_t c1 = std::min(S, c0 + cap);
         CK0(cudaMemsetAsync(dhist, 0, (size_t)(c1 - c0) * slot_bytes, st));
         rf::HistArgs a{c.dcls, dbins, dnode, T > 1 ? dbag : nullptr, dsub, dhist, n, F, G, K, NB, C,
-                       (int)c0, (int)c1, (int)c0, active[c0].first, active[c1 - 1].first, cdf};
+                       (int)c0, (int)c1, (int)c0, active[c0].first, active[c1 - 1].first, cdf, c.dyq};
         if (pass_slots >= 1) {
           const unsigned grid = (unsigned)std::min<int64_t>(nblk(n, rf::THREADS), (int64_t)c.sm * 2);
           for (int64_t p0 = c0; p0 < c1; p0 += pass_slots) {
@@ -5557,28 +5798,39 @@ static int rf_bin_and_grow(const RfCtx& c) {
             a.s1 = (int)std::min(c1, p0 + pass_slots);
             a.g0 = active[a.s0].first;
             a.g1 = active[a.s1 - 1].first;
-            rf::hist_kernel<BinT, true><<<grid, rf::THREADS, (size_t)(a.s1 - a.s0) * smem_slot, st>>>(a);
+            rf::hist_kernel<BinT, true, REG><<<grid, rf::THREADS, (size_t)(a.s1 - a.s0) * smem_slot, st>>>(a);
           }
           const int64_t passes = (c1 - c0 + pass_slots - 1) / pass_slots;
           tm.smem_launches += passes, tm.max_passes = std::max(tm.max_passes, passes);
         } else {
           const unsigned grid = (unsigned)std::min<int64_t>(nblk(n, rf::THREADS), (int64_t)c.sm * 8);
-          rf::hist_kernel<BinT, false><<<grid, rf::THREADS, 0, st>>>(a);
+          rf::hist_kernel<BinT, false, REG><<<grid, rf::THREADS, 0, st>>>(a);
           ++tm.global_launches;
         }
         CK0(cudaGetLastError());
         CK0(cudaStreamSynchronize(st));
         const double hm = rf_ms(t0);
         tm.hist += hm, tm.hist_l[level] += hm;
-        rf::SelArgs sa{dhist, dsub, c.dnthr, dgain, dbest, dleft, dtot, K, NB, C, c.p->impurity, (int)c0, (int)c0};
-        rf::select_kernel<<<(unsigned)(c1 - c0), rf::SEL_WARPS * 32, 0, st>>>(sa);
+        if constexpr (REG) {
+          EVF(rf_select_var(c, level, active, hsub, c0, c1, dhist, dsub, dorder, dcen, dseg, dgain, dbest,
+                            (unsigned long long*)dleft, (unsigned long long*)dtot, hgain, hbest, hcats));
+        } else {
+          rf::SelArgs sa{dhist, dsub, c.dnthr, dgain, dbest, dleft, dtot, K, NB, C, c.p->impurity, (int)c0, (int)c0};
+          rf::select_kernel<<<(unsigned)(c1 - c0), rf::SEL_WARPS * 32, 0, st>>>(sa);
+        }
         CK0(cudaGetLastError());
         CK0(cudaStreamSynchronize(st));
         const double sm_ = rf_ms(t0);
         tm.sel += sm_, tm.sel_l[level] += sm_;
       }
-      std::vector<double> hgain(S);
-      std::vector<int> hbest(2 * S);
+      if constexpr (REG) {
+        std::vector<std::pair<int, int64_t>> next;
+        EVF(rf_decide_var<BinT>(c, level, active, hsub, hgain, hbest, hcats, (const unsigned long long*)dleft,
+                                (const unsigned long long*)dtot, dnode, dbins, G, ugrid, lv, trees, t0, next));
+        tm.levels = std::max(tm.levels, level + 1);
+        active.swap(next);
+        continue;
+      }
       std::vector<int64_t> hleft(S * C), htot(S * C);
       CK0(cudaMemcpyAsync(hgain.data(), dgain, 8 * (size_t)S, cudaMemcpyDeviceToHost, st));
       CK0(cudaMemcpyAsync(hbest.data(), dbest, 8 * (size_t)S, cudaMemcpyDeviceToHost, st));
@@ -5645,12 +5897,23 @@ static int rf_bin_and_grow(const RfCtx& c) {
   return PIO_ALS_OK;
 }
 
-// The forest from n rows already on the device (dx: n x F fp64, dcls: class bytes) on stream st: split search, bin
-// codes, then every tree group level by level.  pio_rf_train and pio_cls_folds_rf_train both end here; g_rf_timing's
-// later phases are timed from t0.
+// what the regressor adds to rf_fit: device quantised labels and categories per feature (host and device), 2^-s, 2^-2s
+struct RfReg {
+  const long long* dyq;
+  const int* darity;
+  std::vector<int> arity;
+  double scale1, scale2;
+};
+
+// The forest from n rows already on the device (dx: n x F fp64, dcls: class bytes, or reg for the regressor) on stream
+// st: split search, bin codes, then every tree group level by level.  pio_rf_train, pio_rf_train_regressor and
+// pio_cls_folds_rf_train end here; g_rf_timing's later phases are timed from t0.
 static int rf_fit(const pio_rf_params* p, const double* dx, const uint8_t* dcls, int64_t n, int F, int sm, CallMem& tmp,
-                  cudaStream_t st, std::chrono::steady_clock::time_point t0, pio_rf_forest** out) {
-  const int C = p->num_classes, K = rf_subset_size(p->feature_subset_strategy, F, p->num_trees);
+                  cudaStream_t st, std::chrono::steady_clock::time_point t0, pio_rf_forest** out,
+                  const RfReg* reg = nullptr) {
+  const int C = reg ? 1 : p->num_classes;
+  const int K = reg ? rf_subset_size_reg(p->feature_subset_strategy, F, p->num_trees)
+                    : rf_subset_size(p->feature_subset_strategy, F, p->num_trees);
   RfTiming& tm = g_rf_timing;
   // split sample, then per feature its sorted distinct values: thresholds on the host (findSplitsForContinuousFeature)
   const double frac = rf_sample_fraction(n, p->max_bins);
@@ -5689,6 +5952,7 @@ static int rf_fit(const pio_rf_params* p, const double* dx, const uint8_t* dcls,
     std::vector<double> vals;
     std::vector<int64_t> cnts;
     for (int f = 0; f < F; ++f) {
+      if (reg && reg->arity[f] > 0) continue;             // categorical: no thresholds, its bins are its categories
       sb.live = 0;
       rf::sample_keys_kernel<<<nblk(m, 256), 256, 0, st>>>(dx, F, f, rows, m, sb.keys(), sb.vals());
       CK0(radix_sort_pairs(sb, (size_t)m, 64, st, nullptr));
@@ -5723,7 +5987,9 @@ static int rf_fit(const pio_rf_params* p, const double* dx, const uint8_t* dcls,
     hnthr[f] = (int)thr[f].size();
     hoff[f + 1] = (int)hthr.size();
   }
-  const int NB = *std::max_element(hnthr.begin(), hnthr.end()) + 1;
+  int NB = *std::max_element(hnthr.begin(), hnthr.end()) + 1;
+  if (reg)
+    for (int a : reg->arity) NB = std::max(NB, a);
   double* dthr = nullptr;
   int *doff = nullptr, *dnthr = nullptr;
   CK0(tmp.device(&dthr, hthr.size()));
@@ -5740,8 +6006,13 @@ static int rf_fit(const pio_rf_params* p, const double* dx, const uint8_t* dcls,
   fo->n_trees = p->num_trees;
   fo->n_class = C;
   fo->tree_off.push_back(0);
-  RfCtx ctx{&tmp, st, sm, p, n, F, K, C, NB, dx, dcls, dthr, doff, dnthr, &thr, fo};
-  const int rc2 = NB <= 256 ? rf_bin_and_grow<uint8_t>(ctx) : rf_bin_and_grow<uint16_t>(ctx);
+  fo->regression = reg != nullptr;
+  if (reg) fo->n_class = 0, fo->cat_off.push_back(0);
+  RfCtx ctx{&tmp, st, sm, p, n, F, K, C, NB, dx, dcls, dthr, doff, dnthr, &thr, fo,
+            reg ? reg->dyq : nullptr, reg ? reg->darity : nullptr, reg ? &reg->arity : nullptr,
+            reg ? reg->scale1 : 0.0, reg ? reg->scale2 : 0.0};
+  const int rc2 = reg ? (NB <= 256 ? rf_bin_and_grow<uint8_t, true>(ctx) : rf_bin_and_grow<uint16_t, true>(ctx))
+                      : (NB <= 256 ? rf_bin_and_grow<uint8_t>(ctx) : rf_bin_and_grow<uint16_t>(ctx));
   if (rc2 != PIO_ALS_OK) {
     delete fo;
     return rc2;
@@ -5885,6 +6156,159 @@ int pio_rf_predict(int device, int32_t n_trees, const int32_t* tree_off, int64_t
   CK0(cudaMemcpyAsync(dx, x, 8 * (size_t)n * n_feat, cudaMemcpyHostToDevice, st));
   EVF(rf_predict_device(tmp, st, fl, dx, n, n_feat, dout));
   CK0(cudaMemcpyAsync(out, dout, 4 * (size_t)n, cudaMemcpyDeviceToHost, st));
+  CK0(cudaStreamSynchronize(st));
+  return PIO_ALS_OK;
+}
+
+int pio_rf_train_regressor(int device, const pio_rf_params* p, const int32_t* arity, const double* label,
+                           const double* x, int64_t n, int32_t n_feat, pio_rf_forest** out) {
+  if (!p || !out) return fail(nullptr, PIO_ALS_ERR_ARG, "bad pio_rf_train_regressor arguments");
+  *out = nullptr;
+  int shift = 0;
+  EVF(rf_check_reg(p, arity, label, x, n, n_feat, &shift));
+  g_rf_timing = RfTiming();
+  RfTiming& tm = g_rf_timing;
+  auto t0 = std::chrono::steady_clock::now();
+  CK0(cudaSetDevice(device));
+  int sm = 0;
+  CK0(cudaDeviceGetAttribute(&sm, cudaDevAttrMultiProcessorCount, device));
+  RfReg reg;
+  if (arity) reg.arity.assign(arity, arity + n_feat);
+  else reg.arity.assign((size_t)n_feat, 0);
+  reg.scale1 = ldexp(1.0, -shift), reg.scale2 = ldexp(1.0, -2 * shift);
+  std::vector<long long> hyq((size_t)n);
+  for (int64_t r = 0; r < n; ++r) hyq[r] = (long long)nearbyint(ldexp(label[r], shift));   // ties to even
+  CallMem tmp;
+  cudaStream_t st;
+  CK0(tmp.stream(&st));
+  double* dx = nullptr;
+  long long* dyq = nullptr;
+  int* dar = nullptr;
+  CK0(tmp.device(&dx, (size_t)n * n_feat));
+  CK0(tmp.device(&dyq, (size_t)n));
+  CK0(tmp.device(&dar, (size_t)n_feat));
+  rf_ms(t0);
+  CK0(cudaMemcpyAsync(dx, x, sizeof(double) * (size_t)n * n_feat, cudaMemcpyHostToDevice, st));
+  CK0(cudaMemcpyAsync(dyq, hyq.data(), 8 * (size_t)n, cudaMemcpyHostToDevice, st));
+  CK0(cudaMemcpyAsync(dar, reg.arity.data(), 4 * (size_t)n_feat, cudaMemcpyHostToDevice, st));
+  CK0(cudaStreamSynchronize(st));
+  tm.h2d = rf_ms(t0);
+  reg.dyq = dyq, reg.darity = dar;
+  return rf_fit(p, dx, nullptr, n, n_feat, sm, tmp, st, t0, out, &reg);
+}
+
+int pio_rf_forest_reg_size(const pio_rf_forest* f, int64_t* n_cat_ids) {
+  if (!f) return fail(nullptr, PIO_ALS_ERR_ARG, "null forest");
+  if (!f->regression) return fail(nullptr, PIO_ALS_ERR_ARG, "not a regression forest");
+  if (n_cat_ids) *n_cat_ids = (int64_t)f->cat_ids.size();
+  return PIO_ALS_OK;
+}
+
+int pio_rf_forest_reg_get(const pio_rf_forest* f, double* value, int64_t* cat_off, int32_t* cat_ids) {
+  if (!f) return fail(nullptr, PIO_ALS_ERR_ARG, "null forest");
+  if (!f->regression) return fail(nullptr, PIO_ALS_ERR_ARG, "not a regression forest");
+  auto put = [](auto* dst, const auto& v) {
+    if (dst && !v.empty()) memcpy(dst, v.data(), v.size() * sizeof(v[0]));
+  };
+  put(value, f->value);
+  put(cat_off, f->cat_off);
+  put(cat_ids, f->cat_ids);
+  return PIO_ALS_OK;
+}
+
+int pio_rf_predict_regression(int device, int32_t n_trees, const int32_t* tree_off, int64_t n_nodes,
+                              const int32_t* feature, const double* threshold, const int32_t* left,
+                              const int32_t* right, const double* value, const int64_t* cat_off,
+                              const int32_t* cat_ids, const double* x, int64_t n, int32_t n_feat, double* out) {
+  if (!out || !value || !cat_off || n < 0 || (n > 0 && !x) || n_nodes < 1 || n_nodes >= (1ll << 31))
+    return fail(nullptr, PIO_ALS_ERR_ARG, "bad pio_rf_predict_regression arguments");
+  const std::vector<int32_t> zero((size_t)n_nodes, 0);   // rf_check_flat's class check, with one class
+  const RfFlat fl{n_trees, tree_off, n_nodes, feature, threshold, left, right, zero.data(), 1};
+  EVF(rf_check_flat(fl, n_feat));
+  const int64_t nc = cat_off[n_nodes];
+  if (cat_off[0] != 0 || nc < 0 || (nc > 0 && !cat_ids)) return fail(nullptr, PIO_ALS_ERR_ARG, "bad category offsets");
+  for (int64_t i = 0; i < n_nodes; ++i) {
+    if (cat_off[i + 1] < cat_off[i] || cat_off[i + 1] > nc)
+      return fail(nullptr, PIO_ALS_ERR_ARG, "bad category offsets at node %lld", (long long)i);
+    if (cat_off[i + 1] > cat_off[i] && feature[i] < 0)
+      return fail(nullptr, PIO_ALS_ERR_ARG, "leaf %lld has categories", (long long)i);
+    for (int64_t k = cat_off[i]; k < cat_off[i + 1]; ++k)
+      if (cat_ids[k] < 0 || (k > cat_off[i] && cat_ids[k] <= cat_ids[k - 1]))
+        return fail(nullptr, PIO_ALS_ERR_ARG, "categories of node %lld are not ascending non-negative ids", (long long)i);
+  }
+  if (n == 0) return PIO_ALS_OK;
+  CK0(cudaSetDevice(device));
+  CallMem tmp;
+  cudaStream_t st;
+  CK0(tmp.stream(&st));
+  const int64_t nn = n_nodes;
+  int *dto = nullptr, *df = nullptr, *dl = nullptr, *dr = nullptr, *dci = nullptr;
+  double *dt = nullptr, *dv = nullptr, *dx = nullptr, *dout = nullptr;
+  long long* dco = nullptr;
+  CK0(tmp.device(&dto, (size_t)n_trees));
+  CK0(tmp.device(&df, (size_t)nn));
+  CK0(tmp.device(&dl, (size_t)nn));
+  CK0(tmp.device(&dr, (size_t)nn));
+  CK0(tmp.device(&dt, (size_t)nn));
+  CK0(tmp.device(&dv, (size_t)nn));
+  CK0(tmp.device(&dco, (size_t)nn + 1));
+  CK0(tmp.device(&dci, (size_t)std::max<int64_t>(1, nc)));
+  CK0(tmp.device(&dx, (size_t)n * n_feat));
+  CK0(tmp.device(&dout, (size_t)n));
+  CK0(cudaMemcpyAsync(dto, tree_off, 4 * (size_t)n_trees, cudaMemcpyHostToDevice, st));
+  CK0(cudaMemcpyAsync(df, feature, 4 * (size_t)nn, cudaMemcpyHostToDevice, st));
+  CK0(cudaMemcpyAsync(dl, left, 4 * (size_t)nn, cudaMemcpyHostToDevice, st));
+  CK0(cudaMemcpyAsync(dr, right, 4 * (size_t)nn, cudaMemcpyHostToDevice, st));
+  CK0(cudaMemcpyAsync(dt, threshold, 8 * (size_t)nn, cudaMemcpyHostToDevice, st));
+  CK0(cudaMemcpyAsync(dv, value, 8 * (size_t)nn, cudaMemcpyHostToDevice, st));
+  CK0(cudaMemcpyAsync(dco, cat_off, 8 * ((size_t)nn + 1), cudaMemcpyHostToDevice, st));
+  if (nc > 0) CK0(cudaMemcpyAsync(dci, cat_ids, 4 * (size_t)nc, cudaMemcpyHostToDevice, st));
+  CK0(cudaMemcpyAsync(dx, x, 8 * (size_t)n * n_feat, cudaMemcpyHostToDevice, st));
+  rf::predict_reg_kernel<<<nblk(n, 128), 128, 0, st>>>(dto, n_trees, df, dt, dl, dr, dv, dco, dci, dx, n, n_feat, dout);
+  CK0(cudaGetLastError());
+  CK0(cudaMemcpyAsync(out, dout, 8 * (size_t)n, cudaMemcpyDeviceToHost, st));
+  CK0(cudaStreamSynchronize(st));
+  return PIO_ALS_OK;
+}
+
+int pio_lead_sessions(int device, const int32_t* session, const uint8_t* is_buy, const int64_t* t_ms, int64_t n,
+                      int32_t n_sessions, int64_t* landing, uint8_t* buy) {
+  if (n < 0 || n_sessions < 0 || (n > 0 && (!session || !is_buy || !t_ms)) || (n_sessions > 0 && (!landing || !buy)))
+    return fail(nullptr, PIO_ALS_ERR_ARG, "bad pio_lead_sessions arguments");
+  for (int64_t r = 0; r < n; ++r)
+    if (session[r] < 0 || session[r] >= n_sessions)
+      return fail(nullptr, PIO_ALS_ERR_ARG, "event %lld has session %d of %d", (long long)r, session[r], n_sessions);
+  if (n_sessions == 0) return PIO_ALS_OK;
+  CK0(cudaSetDevice(device));
+  CallMem tmp;
+  cudaStream_t st;
+  CK0(tmp.stream(&st));
+  int* ds = nullptr;
+  uint8_t *db = nullptr, *dbuy = nullptr;
+  long long *dt = nullptr, *dland = nullptr;
+  unsigned long long* dmin = nullptr;
+  CK0(tmp.device(&ds, (size_t)std::max<int64_t>(n, 1)));
+  CK0(tmp.device(&db, (size_t)std::max<int64_t>(n, 1)));
+  CK0(tmp.device(&dt, (size_t)std::max<int64_t>(n, 1)));
+  CK0(tmp.device(&dmin, (size_t)n_sessions));
+  CK0(tmp.device(&dland, (size_t)n_sessions));
+  CK0(tmp.device(&dbuy, (size_t)n_sessions));
+  if (n > 0) {
+    CK0(cudaMemcpyAsync(ds, session, 4 * (size_t)n, cudaMemcpyHostToDevice, st));
+    CK0(cudaMemcpyAsync(db, is_buy, (size_t)n, cudaMemcpyHostToDevice, st));
+    CK0(cudaMemcpyAsync(dt, t_ms, 8 * (size_t)n, cudaMemcpyHostToDevice, st));
+  }
+  CK0(cudaMemsetAsync(dmin, 0xff, 8 * (size_t)n_sessions, st));
+  CK0(cudaMemsetAsync(dland, 0xff, 8 * (size_t)n_sessions, st));          // -1: no view
+  CK0(cudaMemsetAsync(dbuy, 0, (size_t)n_sessions, st));
+  if (n > 0) {
+    lead::landing_time_kernel<<<nblk(n, 256), 256, 0, st>>>(ds, db, dt, n, dmin);
+    lead::landing_pick_kernel<<<nblk(n, 256), 256, 0, st>>>(ds, db, dt, n, dmin, dland);
+    lead::buy_flag_kernel<<<nblk(n, 256), 256, 0, st>>>(ds, db, dt, n, dmin, dland, dbuy);
+    CK0(cudaGetLastError());
+  }
+  CK0(cudaMemcpyAsync(landing, dland, 8 * (size_t)n_sessions, cudaMemcpyDeviceToHost, st));
+  CK0(cudaMemcpyAsync(buy, dbuy, (size_t)n_sessions, cudaMemcpyDeviceToHost, st));
   CK0(cudaStreamSynchronize(st));
   return PIO_ALS_OK;
 }

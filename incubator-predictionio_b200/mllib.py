@@ -10,6 +10,8 @@ Same names and argument meaning as the MLlib API the templates call (SURVEY 8(b)
         (examples/scala-parallel-classification/add-algorithm/src/main/scala/NaiveBayesAlgorithm.scala:41-57)
     RandomForest.trainClassifier(...) / RandomForestModel.predict
         (examples/scala-parallel-classification/add-algorithm/src/main/scala/RandomForestAlgorithm.scala:46-70)
+    RandomForest.trainRegressor(...) / RandomForestModel.predict, with ordered categorical features
+        (the lead scoring template, docs/manual/source/templates/leadscoring/dase.html.md.erb)
 
 Ratings are COO arrays (user:int32, product:int32, rating:float32) -- the RDD[Rating(Int,Int,Double)]
 the templates build at ALSAlgorithm.scala:62-65 -- and everything below is one call through the C ABI
@@ -218,13 +220,19 @@ class NaiveBayes:
 
 
 class RandomForestModel:
-    """A trained classification forest as flat per-node numpy arrays (native.rf_train's dict), so that a pickle of the
-    model is the model.  Trees are stored one after the other, each in preorder; `tree_off[t]` is tree t's root."""
+    """A trained forest as flat per-node numpy arrays (native.rf_train's or native.rf_train_regressor's dict), so that a
+    pickle of the model is the model.  Trees are stored one after the other, each in preorder; `tree_off[t]` is tree
+    t's root.  `algo` is "Classification" (the majority vote; the default, which models pickled before regression
+    existed keep) or "Regression" (the mean of the trees' predictions)."""
 
-    def __init__(self, numClasses: int, nodes: dict, device: int = 0):
+    algo = "Classification"
+
+    def __init__(self, numClasses: int, nodes: dict, device: int = 0, algo: str = "Classification"):
         self.numClasses = int(numClasses)
         self.nodes = {k: np.asarray(v) for k, v in nodes.items()}
         self.device = device
+        if algo != "Classification":
+            self.algo = algo
 
     @property
     def numTrees(self) -> int:
@@ -254,7 +262,10 @@ class RandomForestModel:
         return float(self.predictBatch(np.asarray(features, np.float64).reshape(1, -1))[0])
 
     def predictBatch(self, x: np.ndarray) -> np.ndarray:
-        """The forest's majority vote per row, as float labels; on the device."""
+        """The forest's majority vote (classification) or mean prediction (regression) per row, as floats; on the
+        device."""
+        if self.algo == "Regression":
+            return native.rf_predict_regression(self.nodes, np.asarray(x, np.float64), self.device)
         return native.rf_predict(self.nodes, self.numClasses, np.asarray(x, np.float64), self.device).astype(np.float64)
 
 
@@ -272,6 +283,37 @@ class RandomForest:
                                                                featureSubsetStrategy, imp, maxDepth, maxBins, seed,
                                                                device),
                                    numClasses, categoricalFeaturesInfo, impurity, device)
+
+    @staticmethod
+    def trainRegressor(labels, features, categoricalFeaturesInfo, numTrees: int, featureSubsetStrategy: str,
+                       impurity: str, maxDepth: int, maxBins: int, seed: int = 0, device: int = 0) -> RandomForestModel:
+        """MLlib's RandomForest.trainRegressor with ordered categorical features ({feature: arity}); the rules are those
+        of tests/forest_reg_ref.py.  labels: n floats; features: n x F, trained in fp64, a categorical feature's values
+        in [0, arity).  Bad arguments and data raise ValueError with MLlib's messages before any device work."""
+        x = np.asarray(features, np.float64)
+        n_feat = x.shape[1] if x.ndim == 2 else 0
+        if impurity in RandomForest.IMPURITIES:
+            raise ValueError(f"DecisionTree Strategy given invalid impurity for Regression: {impurity}.  Valid "
+                             f"settings: Variance")
+        if impurity != "variance":
+            raise ValueError(f"Did not recognize Impurity name: {impurity}")
+        arity = np.zeros(n_feat, np.int32)
+        for f, a in sorted((categoricalFeaturesInfo or {}).items()):
+            f, a = int(f), int(a)
+            if not 0 <= f < n_feat:
+                raise ValueError(f"categoricalFeaturesInfo names feature {f}, but the data have {n_feat} features.")
+            if a < 2:
+                raise ValueError(f"DecisionTree Strategy given invalid categoricalFeaturesInfo setting: feature {f} has "
+                                 f"{a} categories.  The number of categories should be >= 2.")
+            arity[f] = a
+        try:
+            nodes = native.rf_train_regressor(labels, x, arity, numTrees, featureSubsetStrategy, native.RF_VARIANCE,
+                                              maxDepth, maxBins, seed, device)
+        except native.NativeError as e:
+            if e.code != native.ERR_ARG:
+                raise
+            raise ValueError(native.lib().pio_als_last_error(None).decode()) from None
+        return RandomForestModel(0, nodes, device, algo="Regression")
 
     @staticmethod
     def trainClassifierFold(folds: native.ClsFolds, fold: int, numClasses: int, categoricalFeaturesInfo, numTrees: int,

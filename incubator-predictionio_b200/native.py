@@ -47,7 +47,8 @@ EXPORTED_SYMBOLS = [
     "pio_cls_folds_result_free", "pio_cls_folds_destroy", "pio_cooc_model_create", "pio_cooc_model_destroy",
     "pio_cooc_predict_filtered", "pio_cooc_model_get_stats", "pio_serve_zscore_merge", "pio_popular_model_create",
     "pio_popular_predict_filtered", "pio_popular_model_get_stats", "pio_popular_model_destroy", "pio_assoc_train",
-    "pio_assoc_model_size", "pio_assoc_model_get", "pio_assoc_model_destroy",
+    "pio_assoc_model_size", "pio_assoc_model_get", "pio_assoc_model_destroy", "pio_rf_train_regressor",
+    "pio_rf_forest_reg_size", "pio_rf_forest_reg_get", "pio_rf_predict_regression", "pio_lead_sessions",
 ]
 
 
@@ -1186,7 +1187,7 @@ def nb_train(label, x, n_class, lam, device=0):
     return pi, theta
 
 
-RF_GINI, RF_ENTROPY = 0, 1
+RF_GINI, RF_ENTROPY, RF_VARIANCE = 0, 1, 2
 RF_FOREST_INT = ("feature", "left", "right", "prediction")
 RF_FOREST_F64 = ("threshold", "impurity", "gain")
 
@@ -1218,8 +1219,9 @@ def _rf_params(num_classes, num_trees, strategy, impurity, max_depth, max_bins, 
                     seed=int(seed))
 
 
-def _rf_forest_take(h) -> dict:
-    """The flat arrays of the pio_rf_forest h, which is destroyed."""
+def _rf_forest_take(h, regression=False) -> dict:
+    """The flat arrays of the pio_rf_forest h, which is destroyed (a regressor's: its prediction in float64 and its
+    categories)."""
     try:
         nt, nn = C.c_int32(0), C.c_int64(0)
         _check(lib().pio_rf_forest_size(h, C.byref(nt), C.byref(nn)))
@@ -1228,9 +1230,67 @@ def _rf_forest_take(h) -> dict:
         out.update({k: np.empty(nn.value, np.float64) for k in RF_FOREST_F64})
         _check(lib().pio_rf_forest_get(h, *_addrs(out, "tree_off", "feature", "threshold", "left", "right", "prediction",
                                                   "impurity", "gain", "count")))
+        if regression:
+            nc = C.c_int64(0)
+            _check(lib().pio_rf_forest_reg_size(h, C.byref(nc)))
+            out.update(prediction=np.empty(nn.value, np.float64), cat_off=np.empty(nn.value + 1, np.int64),
+                       cat_ids=np.empty(nc.value, np.int32))
+            _check(lib().pio_rf_forest_reg_get(h, *_addrs(out, "prediction", "cat_off", "cat_ids")))
     finally:
         lib().pio_rf_forest_destroy(h)
     return out
+
+
+def rf_train_regressor(label, x, arity, num_trees, strategy, impurity, max_depth, max_bins, seed=0, device=0):
+    """pio_rf_train_regressor: a RandomForest regressor (impurity RF_VARIANCE) as rf_train's dict of flat per-node
+    arrays, with `prediction` the node's mean label (float64) and, per node, its left categories: cat_off (int64
+    [n_nodes + 1]) and cat_ids (int32, ascending per node).  arity: n_feat categories per feature, 0 = continuous."""
+    label = np.ascontiguousarray(label, np.float64)
+    x = np.ascontiguousarray(x, np.float64)
+    if x.ndim != 2 or label.shape != (x.shape[0],):
+        raise ValueError("x must be n x n_feat and label must have n entries")
+    arity = np.ascontiguousarray(arity, np.int32)
+    if arity.shape != (x.shape[1],):
+        raise ValueError("arity must have one entry per feature")
+    p = _rf_params(0, num_trees, strategy, impurity, max_depth, max_bins, seed)
+    h = C.c_void_p()
+    _check(lib().pio_rf_train_regressor(C.c_int(device), C.byref(p), _ptr(arity, C.c_int32), _ptr(label, C.c_double),
+                                        _ptr(x, C.c_double), C.c_int64(x.shape[0]), C.c_int32(x.shape[1]),
+                                        C.byref(h)))
+    return _rf_forest_take(h, regression=True)
+
+
+def rf_predict_regression(forest, x, device=0):
+    """pio_rf_predict_regression: the forest's mean prediction (float64 [n]) for the rows of x (n x n_feat)."""
+    x = np.ascontiguousarray(x, np.float64)
+    n = x.shape[0]
+    out = np.empty(n, np.float64)
+    a = {k: np.ascontiguousarray(forest[k], np.int32) for k in ("tree_off", "feature", "left", "right", "cat_ids")}
+    a.update({k: np.ascontiguousarray(forest[k], np.float64) for k in ("threshold", "prediction")})
+    a["cat_off"] = np.ascontiguousarray(forest["cat_off"], np.int64)
+    vp = C.c_void_p
+    _check(lib().pio_rf_predict_regression(
+        C.c_int(device), C.c_int32(a["tree_off"].shape[0] - 1), vp(_addr(a["tree_off"])),
+        C.c_int64(a["threshold"].shape[0]), *[vp(_addr(a[k])) for k in ("feature", "threshold", "left", "right",
+                                                                          "prediction", "cat_off", "cat_ids")],
+        vp(_addr(x)), C.c_int64(n), C.c_int32(x.shape[1] if x.ndim == 2 else 0), vp(_addr(out))))
+    return out
+
+
+def lead_sessions(session, is_buy, t_ms, n_sessions, device=0):
+    """pio_lead_sessions: per session, the event index of its landing view (-1: no view) and whether a buy follows it."""
+    session = np.ascontiguousarray(session, np.int32)
+    is_buy = np.ascontiguousarray(is_buy, np.uint8)
+    t_ms = np.ascontiguousarray(t_ms, np.int64)
+    n = session.shape[0]
+    if is_buy.shape != (n,) or t_ms.shape != (n,):
+        raise ValueError("session, is_buy and t_ms must have one entry per event")
+    landing = np.empty(max(n_sessions, 1), np.int64)
+    buy = np.empty(max(n_sessions, 1), np.uint8)
+    vp = C.c_void_p
+    _check(lib().pio_lead_sessions(C.c_int(device), vp(_addr(session)), vp(_addr(is_buy)), vp(_addr(t_ms)),
+                                   C.c_int64(n), C.c_int32(n_sessions), vp(_addr(landing)), vp(_addr(buy))))
+    return landing[:n_sessions], buy[:n_sessions].astype(bool)
 
 
 def rf_predict(forest, num_classes, x, device=0):
