@@ -612,6 +612,32 @@ PIO_API int pio_serve_zscore_merge(int device, int32_t n_queries, int32_t n_algo
                                    const int32_t* const* counts, const int32_t* widths, const int32_t* num,
                                    int32_t topk, int32_t* out_items, double* out_scores, int32_t* out_count);
 
+/* Default number of entries per part of a pio_als_rank_lists call (about 20 bytes of device memory each, 60 on the
+ * radix path); the environment variable PIO_RANK_LISTS_BUDGET (a positive integer) overrides it.  Results do not depend
+ * on it. */
+#define PIO_RANK_LISTS_BUDGET (1ll << 24)
+
+/* The product ranking template's predict (docs/manual/source/templates/productranking/dase.html.md.erb:471-530) for a
+ * batch, on a trained, loaded or imported handle (DESIGN.md 4.17).  HOST buffers.  For each query q, users[q] (an index;
+ * any id outside [0, n_users) is an unknown user) and its list items[list_ptr[q] .. list_ptr[q + 1]) (ids outside
+ * [0, n_items) are unknown items and stay in the list; repeats keep their own slots).  An entry's score is the fp64
+ * index-order dot product of the item's and the user's factors, or 0.0 when either has no factor; a NaN score is
+ * returned as the canonical NaN 0x7ff8000000000000.  The entries are stably ordered by java.lang.Double.compare
+ * descending: NaN first, then +inf ... +0.0, then -0.0, then the negatives; equal scores keep the list's order.
+ *   out_pos[list_ptr[q] + r]     = position in q's list of its r-th ranked entry
+ *   out_scores[list_ptr[q] + r]  = that entry's score
+ *   out_ranked[q]                = 1 when q's user has a factor and at least one entry has a score; 0 (isOriginal)
+ *                                  gives the identity positions and zero scores.
+ * The batch runs in parts of consecutive queries whose entries stay within PIO_RANK_LISTS_BUDGET, at least one query per
+ * part.  Rejected with PIO_ALS_ERR_ARG before any device work: n_queries < 0, a NULL handle or output (users, and items
+ * when there are entries, too), list_ptr[0] != 0, list_ptr decreasing, and a list of 2^31 entries or more.
+ * n_queries == 0 and empty lists are valid. */
+PIO_API int pio_als_rank_lists(pio_als_handle* h, const int32_t* users, int32_t n_queries, const int64_t* list_ptr,
+                               const int32_t* items, int32_t* out_pos, double* out_scores, uint8_t* out_ranked);
+/* What the last pio_als_rank_lists on this thread did: out[0] parts, [1] tile-path queries, [2] radix-path queries,
+ * [3] entries, [4] most entries in one part, [5] device milliseconds from the first upload to the last copy back. */
+PIO_API int pio_rank_lists_debug_stats(double out[6]);
+
 /* MLlib multinomial NaiveBayes (classification template). HOST buffers.
  * label: class index 0..n_class-1; x: n x n_feat, non-negative. pi: n_class, theta: n_class x n_feat
  * (fp64 log-probabilities, as MLlib's NaiveBayesModel.pi/theta). */

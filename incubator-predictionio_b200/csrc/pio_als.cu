@@ -62,6 +62,7 @@
 #include "eval_folds.cuh"
 #include "cls_folds.cuh"
 #include "assoc.cuh"
+#include "rank_lists.cuh"
 
 namespace pio {
 
@@ -7485,6 +7486,188 @@ __attribute__((visibility("default"))) int pio_assoc_debug_timing(double out[64]
   for (int k = 12; k < 16; ++k) out[k] = 0;
   for (int k = 0; k <= ASSOC_MAX_LEN; ++k) out[16 + k] = (double)t.cand[k];
   for (int k = 16 + ASSOC_MAX_LEN + 1; k < 64; ++k) out[k] = 0;
+  return PIO_ALS_OK;
+}
+
+}  // extern "C"
+
+// ---- product ranking (pio_als_rank_lists) -------------------------------------------------------------------------------
+namespace pio {
+
+// what the last pio_als_rank_lists on this thread did (pio_rank_lists_debug_stats)
+struct RankListsStats {
+  long long parts = 0, tile_queries = 0, radix_queries = 0, entries = 0, max_part_entries = 0;
+  double device_ms = 0.0;
+};
+static thread_local RankListsStats g_rl_stats;
+
+// host arrays packed into one upload, each block on a 256-byte boundary
+struct HostPack {
+  std::vector<unsigned char> buf;
+  template <class T>
+  size_t put(const T* src, size_t n) {
+    const size_t at = al256(buf.size());
+    buf.resize(at + n * sizeof(T));
+    if (n) memcpy(buf.data() + at, src, n * sizeof(T));
+    return at;
+  }
+};
+
+// One part of a call (rank_plan.h): its inputs up, the tile CTAs and the radix sorts on the handle's stream, its outputs
+// down into the caller's arrays at the part's offsets.
+static int rank_part(pio_als_handle* h, const RankPart& p, const int32_t* users, const int64_t* list_ptr,
+                     const int32_t* items, int32_t* out_pos, double* out_scores, uint8_t* out_ranked) {
+  cudaStream_t st = h->stream;
+  const int nq = p.q1 - p.q0, nt = p.n_tiles(), nr = (int)p.radix.size();
+  const long long ne = p.e1 - p.e0;
+  std::vector<long long> lp((size_t)nq + 1), c((size_t)nr + 1, 0);
+  for (int j = 0; j <= nq; ++j) lp[j] = list_ptr[p.q0 + j] - p.e0;
+  std::vector<int> tq(p.tile_q), rq(p.radix);
+  for (int& q : tq) q -= p.q0;
+  for (int k = 0; k < nr; ++k) {
+    rq[k] -= p.q0;
+    c[k + 1] = c[k] + (lp[rq[k] + 1] - lp[rq[k]]);
+  }
+  HostPack pk;
+  const size_t at_lp = pk.put(lp.data(), lp.size()), at_tq = pk.put(tq.data(), tq.size()),
+               at_tp = pk.put(p.tile_ptr.data(), p.tile_ptr.size()), at_to = pk.put(p.tile_off.data(), p.tile_off.size()),
+               at_tn = pk.put(p.tile_n.data(), p.tile_n.size()), at_rq = pk.put(rq.data(), rq.size()),
+               at_c = pk.put(c.data(), c.size());
+  Scratch tmp(st);
+  unsigned char* d_pack = nullptr;
+  int *d_users = nullptr, *d_items = nullptr, *d_pos = nullptr;
+  double* d_score = nullptr;
+  uint8_t* d_ranked = nullptr;
+  CK(h, tmp.alloc(&d_pack, pk.buf.size()));
+  CK(h, tmp.alloc(&d_users, (size_t)nq));
+  CK(h, tmp.alloc(&d_items, (size_t)ne));
+  CK(h, tmp.alloc(&d_pos, (size_t)ne));
+  CK(h, tmp.alloc(&d_score, (size_t)ne));
+  CK(h, tmp.alloc(&d_ranked, (size_t)nq));
+  CK(h, cudaMemcpyAsync(d_pack, pk.buf.data(), pk.buf.size(), cudaMemcpyHostToDevice, st));
+  CK(h, cudaMemcpyAsync(d_users, users + p.q0, sizeof(int) * (size_t)nq, cudaMemcpyHostToDevice, st));
+  if (ne) CK(h, cudaMemcpyAsync(d_items, items + p.e0, sizeof(int) * (size_t)ne, cudaMemcpyHostToDevice, st));
+  CK(h, cudaMemsetAsync(d_ranked, 0, (size_t)nq, st));   // an empty list is not ranked
+  const RlSide U{h->U.F, h->U.perm, h->U.deg, h->U.n}, I{h->I.F, h->I.perm, h->I.deg, h->I.n};
+  const RlPart dp{d_users, (const long long*)(d_pack + at_lp), d_items, d_pos, d_score, d_ranked};
+  if (nt) {
+    rl_tile_kernel<<<nt, RL_THREADS, 0, st>>>(U, I, h->KP, dp, (const int*)(d_pack + at_tq), (const int*)(d_pack + at_tp),
+                                              (const int*)(d_pack + at_to), (const int*)(d_pack + at_tn));
+    LAUNCHED(h);
+    CK(h, cudaGetLastError());
+  }
+  if (nr) {
+    const long long n = c[nr];
+    const int* d_rq = (const int*)(d_pack + at_rq);
+    const long long* d_c = (const long long*)(d_pack + at_c);
+    SortBufs sb;
+    double* d_rscore = nullptr;
+    uint8_t* d_has = nullptr;
+    for (int b = 0; b < 2; ++b) {
+      CK(h, tmp.alloc(&sb.k[b], (size_t)n));
+      CK(h, tmp.alloc(&sb.v[b], (size_t)n));
+    }
+    CK(h, tmp.alloc(&d_rscore, (size_t)n));
+    CK(h, tmp.alloc(&d_has, (size_t)nr));
+    CK(h, cudaMemsetAsync(d_has, 0, (size_t)nr, st));
+    const unsigned grid = (unsigned)std::min<long long>(nblk(n, 256), (long long)std::max(h->sm_count, 1) * 16);
+    rl_radix_score_kernel<<<grid, 256, 0, st>>>(U, I, h->KP, dp, d_rq, d_c, nr, n, sb.keys(), sb.vals(), d_rscore, d_has);
+    LAUNCHED(h);
+    CK(h, cudaGetLastError());
+    CK(h, radix_sort_pairs(sb, (size_t)n, 64, st, &h->st.kernel_launches));
+    if (nr > 1) {   // equal keys of a query stay in entry order: a stable sort by the query alone groups them
+      rl_radix_query_keys_kernel<<<grid, 256, 0, st>>>(sb.vals(), d_c, nr, n, sb.spare_keys(), sb.spare_vals());
+      LAUNCHED(h);
+      CK(h, cudaGetLastError());
+      sb.flip();
+      CK(h, radix_sort_pairs(sb, (size_t)n, ceil_log2((uint64_t)nr), st, &h->st.kernel_launches));
+    } else {
+      CK(h, cudaMemsetAsync(sb.keys(), 0, sizeof(uint64_t) * (size_t)n, st));
+    }
+    rl_radix_out_kernel<<<grid, 256, 0, st>>>(dp, d_rq, d_c, sb.keys(), sb.vals(), d_rscore, d_has, n);
+    LAUNCHED(h);
+    CK(h, cudaGetLastError());
+  }
+  if (ne) {
+    CK(h, cudaMemcpyAsync(out_pos + p.e0, d_pos, sizeof(int) * (size_t)ne, cudaMemcpyDeviceToHost, st));
+    CK(h, cudaMemcpyAsync(out_scores + p.e0, d_score, sizeof(double) * (size_t)ne, cudaMemcpyDeviceToHost, st));
+  }
+  CK(h, cudaMemcpyAsync(out_ranked + p.q0, d_ranked, (size_t)nq, cudaMemcpyDeviceToHost, st));
+  CK(h, cudaStreamSynchronize(st));
+  return PIO_ALS_OK;
+}
+
+static int rank_lists(pio_als_handle* h, const int32_t* users, int32_t n_queries, const int64_t* list_ptr,
+                      const int32_t* items, int32_t* out_pos, double* out_scores, uint8_t* out_ranked) {
+  if (n_queries < 0) return fail(h, PIO_ALS_ERR_ARG, "n_queries must be >= 0");
+  if (!list_ptr || !out_pos || !out_scores || !out_ranked || (n_queries > 0 && !users))
+    return fail(h, PIO_ALS_ERR_ARG, "null argument");
+  if (list_ptr[0] != 0) return fail(h, PIO_ALS_ERR_ARG, "list_ptr[0] must be 0, not %lld", (long long)list_ptr[0]);
+  for (int q = 0; q < n_queries; ++q) {
+    const long long len = list_ptr[q + 1] - list_ptr[q];
+    if (len < 0) return fail(h, PIO_ALS_ERR_ARG, "list_ptr decreases at query %d", q);
+    if (len >= (1ll << 31)) return fail(h, PIO_ALS_ERR_ARG, "query %d has %lld entries: a list holds fewer than 2^31", q, len);
+  }
+  if (list_ptr[n_queries] > 0 && !items) return fail(h, PIO_ALS_ERR_ARG, "null argument");
+  if (n_queries == 0) return PIO_ALS_OK;
+  if (!h->U.F || !h->I.F) return fail(h, PIO_ALS_ERR_STATE, "no model");
+  // PIO_RANK_LISTS_BUDGET: entries per part; capped so that a part's entries are numbered in 32 bits
+  const char* env_b = getenv("PIO_RANK_LISTS_BUDGET");
+  const long long budget = std::min<long long>(env_b && atoll(env_b) > 0 ? atoll(env_b) : PIO_RANK_LISTS_BUDGET,
+                                               (1ll << 31) - 1);
+  const std::vector<RankPart> parts = plan_rank_lists(list_ptr, n_queries, budget);
+  CK(h, cudaSetDevice(h->cfg.device));
+  cudaEvent_t ev[2] = {nullptr, nullptr};
+  CK(h, cudaEventCreate(&ev[0]));
+  const cudaError_t e1 = cudaEventCreate(&ev[1]);
+  if (e1 != cudaSuccess) {
+    cudaEventDestroy(ev[0]);
+    CK(h, e1);
+  }
+  struct Events {
+    cudaEvent_t* e;
+    ~Events() { cudaEventDestroy(e[0]), cudaEventDestroy(e[1]); }
+  } own{ev};
+  CK(h, cudaEventRecord(ev[0], h->stream));
+  RankListsStats& s = g_rl_stats;
+  for (const RankPart& p : parts) {
+    s.parts += 1;
+    s.tile_queries += (long long)p.tile_q.size();
+    s.radix_queries += (long long)p.radix.size();
+    s.entries += p.e1 - p.e0;
+    s.max_part_entries = std::max(s.max_part_entries, p.e1 - p.e0);
+    const int rc = rank_part(h, p, users, list_ptr, items, out_pos, out_scores, out_ranked);
+    if (rc) return rc;
+  }
+  CK(h, cudaEventRecord(ev[1], h->stream));
+  CK(h, cudaEventSynchronize(ev[1]));
+  float ms = 0.f;
+  CK(h, cudaEventElapsedTime(&ms, ev[0], ev[1]));
+  s.device_ms = ms;
+  return PIO_ALS_OK;
+}
+
+}  // namespace pio
+
+extern "C" {
+
+int pio_als_rank_lists(pio_als_handle* h, const int32_t* users, int32_t n_queries, const int64_t* list_ptr,
+                       const int32_t* items, int32_t* out_pos, double* out_scores, uint8_t* out_ranked) {
+  g_rl_stats = RankListsStats{};
+  if (!h) return fail(nullptr, PIO_ALS_ERR_ARG, "null handle");
+  std::lock_guard<std::mutex> lk(h->mu);
+  try {   // bad_alloc must not cross the C boundary; Scratch releases device memory on the way out
+    return rank_lists(h, users, n_queries, list_ptr, items, out_pos, out_scores, out_ranked);
+  } catch (const std::bad_alloc&) {
+    return fail(h, PIO_ALS_ERR_NOMEM, "pio_als_rank_lists: out of host memory");
+  }
+}
+
+int pio_rank_lists_debug_stats(double out[6]) {
+  if (!out) return PIO_ALS_ERR_ARG;
+  const RankListsStats& s = g_rl_stats;
+  out[0] = (double)s.parts, out[1] = (double)s.tile_queries, out[2] = (double)s.radix_queries;
+  out[3] = (double)s.entries, out[4] = (double)s.max_part_entries, out[5] = s.device_ms;
   return PIO_ALS_OK;
 }
 

@@ -103,6 +103,13 @@ class MatrixFactorizationModel:
         return self._handle().similar(np.asarray(list(query_items), np.int32), num, item_mask, item_weight,
                                       keep_query_items=not exclude_query)
 
+    def rankLists(self, users, list_ptr, items):
+        """The product ranking template's predict for a batch (pio_als_rank_lists): query q is user users[q] with the
+        list items[list_ptr[q] .. list_ptr[q + 1]); ids out of range are unknown.  Returns (pos int32 [total], scores
+        float64 [total], ranked bool [n]), each query's entries ordered by score descending as Double.compare orders
+        them, equal scores in list order."""
+        return self._handle().rank_lists(users, list_ptr, items)
+
     def predict(self, user: int, product: int) -> float:
         return float(np.dot(self.userFeatures[user].astype(np.float64), self.productFeatures[product].astype(np.float64)))
 

@@ -49,6 +49,7 @@ EXPORTED_SYMBOLS = [
     "pio_popular_predict_filtered", "pio_popular_model_get_stats", "pio_popular_model_destroy", "pio_assoc_train",
     "pio_assoc_model_size", "pio_assoc_model_get", "pio_assoc_model_destroy", "pio_rf_train_regressor",
     "pio_rf_forest_reg_size", "pio_rf_forest_reg_get", "pio_rf_predict_regression", "pio_lead_sessions",
+    "pio_als_rank_lists", "pio_rank_lists_debug_stats",
 ]
 
 
@@ -209,6 +210,8 @@ def lib():
         L.pio_popular_predict_filtered.restype = ci
         L.pio_popular_predict_filtered.argtypes = [vp, C.c_int32, C.c_int32, vp, vp, vp, vp]
         L.pio_popular_model_get_stats.argtypes = [vp, vp]
+        L.pio_als_rank_lists.restype = ci
+        L.pio_als_rank_lists.argtypes = [vp, vp, C.c_int32, vp, vp, vp, vp, vp]
         for name in EXPORTED_SYMBOLS:
             getattr(L, name)  # AttributeError if the ABI is incomplete
         _lib = L
@@ -417,6 +420,25 @@ class NativeALS:
                                                 SIM_KEEP_QUERY_ITEMS if keep_query_items else 0, oi.ctypes.data,
                                                 os_.ctypes.data, oc.ctypes.data))
         return oi, os_, oc
+
+    def rank_lists(self, users, list_ptr, items):
+        """pio_als_rank_lists: query q is user users[q] with the list items[list_ptr[q] .. list_ptr[q + 1]).  Returns
+        (pos int32 [total], scores float64 [total], ranked bool [n]): pos[list_ptr[q] + r] is the position in q's list
+        of its r-th ranked entry, scores[...] that entry's score; ranked[q] False means isOriginal (identity order,
+        zero scores)."""
+        users = np.ascontiguousarray(users, np.int32)
+        ptr = np.ascontiguousarray(list_ptr, np.int64)
+        items = np.ascontiguousarray(items, np.int32)
+        n = users.shape[0]
+        if users.ndim != 1 or ptr.shape != (n + 1,) or items.ndim != 1 or (n and items.shape[0] < ptr[-1]):
+            raise ValueError("users must be [n], list_ptr [n + 1] and items at least list_ptr[n] long")
+        total = int(ptr[-1])
+        pos = np.empty(total, np.int32)
+        scores = np.empty(total, np.float64)
+        ranked = np.empty(n, np.uint8)
+        self._check(lib().pio_als_rank_lists(self._h, users.ctypes.data, n, ptr.ctypes.data, items.ctypes.data,
+                                             pos.ctypes.data, scores.ctypes.data, ranked.ctypes.data))
+        return pos, scores, ranked.astype(bool)
 
     # -- persistence / introspection -----------------------------------------------------------
     def save(self, path: str):
@@ -1174,6 +1196,15 @@ def serve_merge_stats() -> dict:
     _check(lib().pio_serve_merge_debug_stats(out))
     return {"parts": int(out[0]), "max_part_queries": int(out[1]), "entries": int(out[2]), "rows": int(out[3]),
             "budget": int(out[4]), "device_ms": out[5]}
+
+
+def rank_lists_stats() -> dict:
+    """What the last NativeALS.rank_lists on this thread did: its parts, the queries on the tile and the radix path, its
+    entries, the most entries in one part, and the device milliseconds from the first upload to the last copy back."""
+    out = (C.c_double * 6)()
+    _check(lib().pio_rank_lists_debug_stats(out))
+    return {"parts": int(out[0]), "tile_queries": int(out[1]), "radix_queries": int(out[2]), "entries": int(out[3]),
+            "max_part_entries": int(out[4]), "device_ms": out[5]}
 
 
 def nb_train(label, x, n_class, lam, device=0):
