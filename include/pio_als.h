@@ -809,6 +809,55 @@ PIO_API int pio_assoc_model_get(const pio_assoc_model* m, int64_t* level_off, in
                                 double* confidence, double* lift);
 PIO_API int pio_assoc_model_destroy(pio_assoc_model* m);
 
+/* The complementary purchase template's predict (Algorithm.predict; rules: tests/assoc_predict_ref.py, DESIGN.md 4.15.1)
+ * for a batch, on `device`.  An opaque object holds a model's frequent-set trie and the cond of each rule, in the layout
+ * of pio_assoc_model_get; the rules' conseq and scores stay with the caller.  Errors: status codes as above, text via
+ * pio_als_last_error(NULL). */
+typedef struct pio_assoc_index pio_assoc_index;
+
+/* Default number of entries per part of a pio_assoc_predict call (listed ids plus the bound on the frequent sets found
+ * inside the queries; about 60 bytes of device memory each); the environment variable PIO_ASSOC_PREDICT_BUDGET (a
+ * positive integer) overrides it.  Results do not depend on it. */
+#define PIO_ASSOC_PREDICT_BUDGET (1ll << 24)
+
+/* level_off [n_levels + 1], set_prefix / set_item [level_off[n_levels]] and rule_cond [n_rules] (HOST), as
+ * pio_assoc_model_get returns them, are checked and copied: PIO_ALS_ERR_ARG names the first set or rule that breaks the
+ * trie -- level_off starting at 0 and non-decreasing, fewer than 2^31 sets; level 1 distinct items ascending with prefix
+ * -1; a set of level l >= 2 with a prefix of level l - 1 and an item that has a level-1 set and is larger than its
+ * prefix's, prefixes non-decreasing within a level and items ascending under one prefix; every set item in [0,
+ * n_items) -- or a rule_cond outside [0, n_sets) or decreasing.  n_items >= 1; n_levels == 0 is an empty model.  The
+ * device copy, each set's child range, each set's rule range and each item's level-1 set are made on `device` by the
+ * first pio_assoc_predict, so that an index holds no device memory until it predicts. */
+PIO_API int pio_assoc_index_create(int device, int32_t n_items, int32_t n_levels, const int64_t* level_off,
+                                   const int64_t* set_prefix, const int32_t* set_item, int64_t n_rules,
+                                   const int64_t* rule_cond, pio_assoc_index** out);
+PIO_API int pio_assoc_index_destroy(pio_assoc_index* ix);
+/* n_queries queries: query j lists the item ids q_items[q_ptr[j] .. q_ptr[j+1]) (HOST); ids outside [0, n_items) are
+ * unknown and skipped, and a repeated id keeps its first position.  The conds of query j are the frequent sets of 1 ..
+ * max_cond_len items (at most the model's levels) whose items are all listed; each one with rules is returned, ordered
+ * by size, then in lexicographic order of its items' first positions in the query -- the order of Scala's subsets(n)
+ * over the de-duplicated query.  Per cond: its items in query order, its first rule (the index of the first rule of
+ * its range in rule_cond) and min(rules of the cond, max(num[j], 0)) rules: a cond with num[j] <= 0 is still
+ * returned, with no rules.  *n_conds and *n_cond_items give the result's size; the result stays on the index until
+ * pio_assoc_predict_get takes it or the next call replaces it.  The batch runs in parts of consecutive queries within
+ * PIO_ASSOC_PREDICT_BUDGET entries, at least one query per part; a query's entries are its listed ids plus the sum over
+ * k of min(C(f, k), sets of level k), f = its listed ids that have a level-1 set.  Rejected with PIO_ALS_ERR_ARG before
+ * any device work: n_queries or max_cond_len below 0, a NULL argument (q_ptr and num when n_queries > 0, q_items when
+ * ids are listed), q_ptr not non-decreasing from q_ptr[0] >= 0, a query listing 2^31 ids or more, and a query whose
+ * entries are 2^32 or more.  A rejected call leaves no result and the index usable. */
+PIO_API int pio_assoc_predict(pio_assoc_index* ix, int32_t max_cond_len, const int64_t* q_ptr, const int32_t* q_items,
+                              int32_t n_queries, const int32_t* num, int64_t* n_conds, int64_t* n_cond_items);
+/* Copies the last pio_assoc_predict result out and releases it (PIO_ALS_ERR_STATE when there is none): q_cond_ptr
+ * [n_queries + 1] (query j's conds are [q_cond_ptr[j], q_cond_ptr[j + 1])), cond_ptr [n_conds + 1] (cond c's items are
+ * cond_items[cond_ptr[c] .. cond_ptr[c + 1])), cond_items [n_cond_items], rule_first [n_conds] (int64) and rule_n
+ * [n_conds].  Any output pointer may be null. */
+PIO_API int pio_assoc_predict_get(pio_assoc_index* ix, int64_t* q_cond_ptr, int64_t* cond_ptr, int32_t* cond_items,
+                                  int64_t* rule_first, int32_t* rule_n);
+/* What the last pio_assoc_predict on this thread did: out[0] parts, [1] most queries in one part, [2] the entries
+ * budget, [3] conds returned, [4] device milliseconds from the first upload to the last copy back, [7 + k] frequent
+ * sets found inside the queries at level k (1 <= k <= 32). */
+PIO_API int pio_assoc_predict_debug_stats(double out[40]);
+
 #ifdef __cplusplus
 }
 #endif

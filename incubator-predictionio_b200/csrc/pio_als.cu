@@ -63,6 +63,7 @@
 #include "cls_folds.cuh"
 #include "assoc.cuh"
 #include "rank_lists.cuh"
+#include "assoc_predict.cuh"
 
 namespace pio {
 
@@ -7668,6 +7669,528 @@ int pio_rank_lists_debug_stats(double out[6]) {
   const RankListsStats& s = g_rl_stats;
   out[0] = (double)s.parts, out[1] = (double)s.tile_queries, out[2] = (double)s.radix_queries;
   out[3] = (double)s.entries, out[4] = (double)s.max_part_entries, out[5] = s.device_ms;
+  return PIO_ALS_OK;
+}
+
+}  // extern "C"
+
+// ---- association rule predict (complementary purchase Algorithm.predict on batches, DESIGN.md 4.15.1) --------------------
+namespace pio {
+// the conds of a pio_assoc_predict call, in the contract's order (pio_als.h)
+struct ApResult {
+  std::vector<int64_t> q_cond_ptr, cond_ptr, rule_first;
+  std::vector<int32_t> cond_items, rule_n;
+};
+}  // namespace pio
+
+struct pio_assoc_index {
+  int device = 0, n_items = 0, n_levels = 0;
+  std::vector<int64_t> level_off;                  // [n_levels + 1]
+  std::vector<uint8_t> frequent;                   // per item: it has a level-1 set (sizes a call's parts on the host)
+  std::vector<int64_t> set_prefix, rule_cond;      // host copies until the first call uploads them
+  std::vector<int32_t> set_item;
+  int64_t n_sets = 0, n_rules = 0;
+  cudaStream_t st = nullptr;
+  bool uploaded = false;
+  long long *d_prefix = nullptr, *d_rule_lo = nullptr, *d_rule_hi = nullptr;
+  int *d_item = nullptr, *d_child_lo = nullptr, *d_child_hi = nullptr, *d_item_set = nullptr;
+  std::mutex mu;                                   // serialises the calls
+  bool has_result = false;                         // the last call's result, until pio_assoc_predict_get takes it
+  pio::ApResult res;
+};
+
+namespace pio {
+
+// what the last pio_assoc_predict on this thread did (pio_assoc_predict_debug_stats)
+struct AssocPredictStats {
+  long long parts = 0, max_part_queries = 0, budget = 0, conds = 0;
+  double device_ms = 0.0;
+  long long entries[33] = {};   // frontier entries (frequent sets found inside the queries) per level 1 .. 32
+};
+static thread_local AssocPredictStats g_ap_stats;
+
+static void ap_free_device(pio_assoc_index* ix) {
+  for (void* p : {(void*)ix->d_prefix, (void*)ix->d_rule_lo, (void*)ix->d_rule_hi, (void*)ix->d_item,
+                  (void*)ix->d_child_lo, (void*)ix->d_child_hi, (void*)ix->d_item_set})
+    if (p) cudaFree(p);
+  ix->d_prefix = ix->d_rule_lo = ix->d_rule_hi = nullptr;
+  ix->d_item = ix->d_child_lo = ix->d_child_hi = ix->d_item_set = nullptr;
+}
+
+// The device copy and the derived ranges, made on the index's stream by the first call; published only once they have
+// all landed, so a failed upload leaves nothing half made and the next call starts over.
+static int ap_upload(pio_assoc_index* ix, const FilterEnv& env) {
+  if (ix->uploaded) return PIO_ALS_OK;
+  if (!ix->st) CKF(env, cudaStreamCreateWithFlags(&ix->st, cudaStreamNonBlocking));
+  const size_t ns = (size_t)std::max<int64_t>(ix->n_sets, 1), nr = (size_t)std::max<int64_t>(ix->n_rules, 1);
+  cudaStream_t st = ix->st;
+  cudaError_t e = cudaSuccess;
+  auto step = [&e](cudaError_t r) {
+    if (e == cudaSuccess) e = r;
+  };
+  long long* d_cond = nullptr;
+  step(cudaMalloc((void**)&ix->d_prefix, 8 * ns));
+  step(cudaMalloc((void**)&ix->d_item, 4 * ns));
+  step(cudaMalloc((void**)&ix->d_child_lo, 4 * ns));
+  step(cudaMalloc((void**)&ix->d_child_hi, 4 * ns));
+  step(cudaMalloc((void**)&ix->d_rule_lo, 8 * ns));
+  step(cudaMalloc((void**)&ix->d_rule_hi, 8 * ns));
+  step(cudaMalloc((void**)&ix->d_item_set, 4 * (size_t)ix->n_items));
+  step(cudaMalloc((void**)&d_cond, 8 * nr));
+  if (e == cudaSuccess) {
+    step(cudaMemsetAsync(ix->d_child_lo, 0, 4 * ns, st));
+    step(cudaMemsetAsync(ix->d_child_hi, 0, 4 * ns, st));
+    step(cudaMemsetAsync(ix->d_rule_lo, 0, 8 * ns, st));
+    step(cudaMemsetAsync(ix->d_rule_hi, 0, 8 * ns, st));
+    step(cudaMemsetAsync(ix->d_item_set, 0xff, 4 * (size_t)ix->n_items, st));   // -1: not frequent
+  }
+  if (e == cudaSuccess && ix->n_sets > 0) {
+    step(cudaMemcpyAsync(ix->d_prefix, ix->set_prefix.data(), 8 * (size_t)ix->n_sets, cudaMemcpyHostToDevice, st));
+    step(cudaMemcpyAsync(ix->d_item, ix->set_item.data(), 4 * (size_t)ix->n_sets, cudaMemcpyHostToDevice, st));
+    const long long n1 = ix->level_off[1], s0 = n1;
+    if (e == cudaSuccess) {
+      ap_item_set_kernel<<<nblk(n1, 256), 256, 0, st>>>(ix->d_item, n1, ix->d_item_set);
+      ++*env.launches;
+      if (ix->n_sets > s0) {
+        ap_children_kernel<<<nblk(ix->n_sets - s0, 256), 256, 0, st>>>(ix->d_prefix, s0, ix->n_sets, ix->d_child_lo,
+                                                                        ix->d_child_hi);
+        ++*env.launches;
+      }
+      step(cudaGetLastError());
+    }
+  }
+  if (e == cudaSuccess && ix->n_rules > 0) {
+    step(cudaMemcpyAsync(d_cond, ix->rule_cond.data(), 8 * (size_t)ix->n_rules, cudaMemcpyHostToDevice, st));
+    if (e == cudaSuccess) {
+      ap_rules_kernel<<<nblk(ix->n_rules, 256), 256, 0, st>>>(d_cond, ix->n_rules, ix->d_rule_lo, ix->d_rule_hi);
+      ++*env.launches;
+      step(cudaGetLastError());
+    }
+  }
+  step(cudaStreamSynchronize(st));   // the host copies are read until here
+  if (d_cond) cudaFree(d_cond);
+  if (e != cudaSuccess) {
+    cudaStreamSynchronize(st);
+    ap_free_device(ix);
+    return fail_to(env.err, PIO_ALS_ERR_CUDA, "uploading the association index: %s", cudaGetErrorString(e));
+  }
+  ix->uploaded = true;
+  std::vector<int64_t>().swap(ix->set_prefix);
+  std::vector<int64_t>().swap(ix->rule_cond);
+  std::vector<int32_t>().swap(ix->set_item);
+  return PIO_ALS_OK;
+}
+
+// exclusive scan of v[0, n) into pos and the total, read back (synchronises the stream)
+static int ap_total(const FilterEnv& env, const uint32_t* v, uint32_t* pos, long long n, long long* total) {
+  *total = 0;
+  if (n == 0) return PIO_ALS_OK;
+  CKF(env, scan_exclusive_u32(v, pos, (size_t)n, env.st, env.launches));
+  uint32_t last[2] = {0, 0};
+  CKF(env, cudaMemcpyAsync(&last[0], pos + n - 1, 4, cudaMemcpyDeviceToHost, env.st));
+  CKF(env, cudaMemcpyAsync(&last[1], v + n - 1, 4, cudaMemcpyDeviceToHost, env.st));
+  CKF(env, cudaStreamSynchronize(env.st));
+  *total = (long long)last[0] + last[1];
+  return PIO_ALS_OK;
+}
+
+// the conds of one level of one part, sorted by (query, positions), on the host
+struct ApLevel {
+  int k = 0;
+  std::vector<int32_t> q, items, n;
+  std::vector<int64_t> rule;
+};
+
+// the frontier of one level: (set, index into L) per entry, in its own device memory
+struct ApFrontier {
+  std::unique_ptr<Scratch> mem;
+  int* set = nullptr;
+  uint32_t* t = nullptr;
+  long long n = 0;
+};
+
+// The queries [j0, j1) of a call: the walk over levels 1 .. K on the device, then each query's conds appended to res
+// level by level.
+static int ap_part(pio_assoc_index* ix, const FilterEnv& env, const int64_t* q_ptr, const int32_t* q_items,
+                   const int32_t* num, int j0, int j1, int K, ApResult* res) {
+  cudaStream_t st = env.st;
+  const int nq = j1 - j0;
+  const long long E = q_ptr[j1] - q_ptr[j0];
+  std::vector<long long> rel((size_t)nq + 1);
+  long long longest = 1;
+  for (int j = 0; j <= nq; ++j) rel[j] = q_ptr[j0 + j] - q_ptr[j0];
+  for (int j = 0; j < nq; ++j) longest = std::max(longest, rel[j + 1] - rel[j]);
+  const int bits_q = ceil_log2((uint64_t)nq), bits_i = ceil_log2((uint64_t)ix->n_items),
+            bits_p = ceil_log2((uint64_t)longest);
+  Scratch tmp(st);
+  long long* d_ptr = nullptr;
+  int *d_items = nullptr, *d_num = nullptr;
+  CKF(env, tmp.alloc(&d_ptr, (size_t)nq + 1));
+  CKF(env, tmp.alloc(&d_items, (size_t)E));
+  CKF(env, tmp.alloc(&d_num, (size_t)nq));
+  CKF(env, cudaMemcpyAsync(d_ptr, rel.data(), 8 * rel.size(), cudaMemcpyHostToDevice, st));
+  if (E) CKF(env, cudaMemcpyAsync(d_items, q_items + q_ptr[j0], 4 * (size_t)E, cudaMemcpyHostToDevice, st));
+  CKF(env, cudaMemcpyAsync(d_num, num + j0, 4 * (size_t)nq, cudaMemcpyHostToDevice, st));
+  // L: every query's distinct frequent items sorted by item, with the first position of each; the level-1 frontier
+  int *L_q = nullptr, *L_item = nullptr;
+  uint32_t *L_pos = nullptr, *L_start = nullptr, *L_end = nullptr;
+  ApFrontier f;
+  f.mem.reset(new Scratch(st));
+  if (E > 0) {
+    Scratch lv(st);
+    uint32_t *flag = nullptr, *at = nullptr;
+    long long U0 = 0;
+    CKF(env, lv.alloc(&flag, (size_t)E));
+    CKF(env, lv.alloc(&at, (size_t)E));
+    int rc = env_launch(env, ap_known_kernel, E, (const int*)d_items, E, ix->n_items, (const int*)ix->d_item_set, flag);
+    if (rc) return rc;
+    EVF(ap_total(env, flag, at, E, &U0));
+    if (U0 > 0) {
+      SortBufs sb;
+      for (int b = 0; b < 2; ++b) {
+        CKF(env, lv.alloc(&sb.k[b], (size_t)U0));
+        CKF(env, lv.alloc(&sb.v[b], (size_t)U0));
+      }
+      rc = env_launch(env, ap_entry_keys_kernel, E, (const int*)d_items, (const long long*)d_ptr, nq, E,
+                      (const uint32_t*)flag, (const uint32_t*)at, bits_i, sb.keys(), sb.vals());
+      if (rc) return rc;
+      CKF(env, radix_sort_pairs(sb, (size_t)U0, bits_q + bits_i, st, env.launches));   // stable: first positions lead
+      rc = env_launch(env, ap_first_kernel, U0, (const uint64_t*)sb.keys(), U0, flag);
+      if (rc) return rc;
+      EVF(ap_total(env, flag, at, U0, &f.n));
+      CKF(env, tmp.alloc(&L_q, (size_t)f.n));
+      CKF(env, tmp.alloc(&L_item, (size_t)f.n));
+      CKF(env, tmp.alloc(&L_pos, (size_t)f.n));
+      CKF(env, f.mem->alloc(&f.set, (size_t)f.n));
+      CKF(env, f.mem->alloc(&f.t, (size_t)f.n));
+      rc = env_launch(env, ap_list_kernel, U0, (const uint64_t*)sb.keys(), (const uint32_t*)sb.vals(), U0,
+                      (const uint32_t*)flag, (const uint32_t*)at, bits_i, (const int*)ix->d_item_set, L_q, L_item, L_pos,
+                      f.set, f.t);
+      if (rc) return rc;
+    }
+  }
+  CKF(env, tmp.alloc(&L_start, (size_t)nq));
+  CKF(env, tmp.alloc(&L_end, (size_t)nq));
+  CKF(env, cudaMemsetAsync(L_start, 0, 4 * (size_t)nq, st));
+  CKF(env, cudaMemsetAsync(L_end, 0, 4 * (size_t)nq, st));
+  if (f.n > 0) {
+    const int rc = env_launch(env, ap_list_ranges_kernel, f.n, (const int*)L_q, f.n, L_start, L_end);
+    if (rc) return rc;
+  }
+  AssocPredictStats& s = g_ap_stats;
+  std::vector<ApLevel> levels;
+  for (int k = 1; k <= K && f.n > 0; ++k) {
+    s.entries[std::min(k, 32)] += f.n;
+    Scratch lv(st);
+    uint32_t *has = nullptr, *at = nullptr;
+    CKF(env, lv.alloc(&has, (size_t)f.n));
+    CKF(env, lv.alloc(&at, (size_t)f.n));
+    int rc = env_launch(env, ap_has_rules_kernel, f.n, (const int*)f.set, f.n, (const long long*)ix->d_rule_lo,
+                        (const long long*)ix->d_rule_hi, has);
+    if (rc) return rc;
+    long long R = 0;
+    EVF(ap_total(env, has, at, f.n, &R));
+    if (R > 0) {
+      int *c_set = nullptr, *c_item = nullptr, *o_q = nullptr, *o_item = nullptr, *o_n = nullptr;
+      uint32_t *c_t = nullptr, *c_pos = nullptr;
+      long long* o_rule = nullptr;
+      const size_t Rk = (size_t)R * k;
+      CKF(env, lv.alloc(&c_set, (size_t)R));
+      CKF(env, lv.alloc(&c_t, (size_t)R));
+      CKF(env, lv.alloc(&c_pos, Rk));
+      CKF(env, lv.alloc(&c_item, Rk));
+      rc = env_launch(env, ap_cond_kernel, f.n, (const int*)f.set, (const uint32_t*)f.t, f.n, k, (const uint32_t*)has,
+                      (const uint32_t*)at, (const long long*)ix->d_prefix, (const int*)ix->d_item, (const int*)L_q,
+                      (const int*)L_item, (const uint32_t*)L_pos, (const uint32_t*)L_start, c_set, c_t, c_pos, c_item);
+      if (rc) return rc;
+      // stable LSD passes over the fields (query, position 1, ..., position k), least significant first, as many
+      // fields per pass as fit 64 bits: exact for any query length and any k
+      SortBufs sb;
+      for (int b = 0; b < 2; ++b) {
+        CKF(env, lv.alloc(&sb.k[b], (size_t)R));
+        CKF(env, lv.alloc(&sb.v[b], (size_t)R));
+      }
+      rc = env_launch(env, ap_iota_kernel, R, sb.vals(), R);
+      if (rc) return rc;
+      for (int f1 = k; f1 >= 0;) {
+        int f0 = f1, bits = f1 == 0 ? bits_q : bits_p;
+        while (f0 > 0 && bits + (f0 - 1 == 0 ? bits_q : bits_p) <= 64) bits += (--f0 == 0 ? bits_q : bits_p);
+        rc = env_launch(env, ap_key_kernel, R, (const uint32_t*)sb.vals(), R, k, f0, f1, bits_q, bits_p,
+                        (const uint32_t*)c_t, (const int*)L_q, (const uint32_t*)c_pos, sb.keys());
+        if (rc) return rc;
+        CKF(env, radix_sort_pairs(sb, (size_t)R, bits, st, env.launches));
+        f1 = f0 - 1;
+      }
+      CKF(env, lv.alloc(&o_q, (size_t)R));
+      CKF(env, lv.alloc(&o_item, Rk));
+      CKF(env, lv.alloc(&o_rule, (size_t)R));
+      CKF(env, lv.alloc(&o_n, (size_t)R));
+      rc = env_launch(env, ap_emit_kernel, R, (const uint32_t*)sb.vals(), R, k, (const int*)c_set, (const uint32_t*)c_t,
+                      (const int*)c_item, (const int*)L_q, (const long long*)ix->d_rule_lo,
+                      (const long long*)ix->d_rule_hi, (const int*)d_num, o_q, o_item, o_rule, o_n);
+      if (rc) return rc;
+      levels.emplace_back();
+      ApLevel& l = levels.back();
+      l.k = k;
+      l.q.resize((size_t)R), l.items.resize(Rk), l.rule.resize((size_t)R), l.n.resize((size_t)R);
+      CKF(env, cudaMemcpyAsync(l.q.data(), o_q, 4 * (size_t)R, cudaMemcpyDeviceToHost, st));
+      CKF(env, cudaMemcpyAsync(l.items.data(), o_item, 4 * Rk, cudaMemcpyDeviceToHost, st));
+      CKF(env, cudaMemcpyAsync(l.rule.data(), o_rule, 8 * (size_t)R, cudaMemcpyDeviceToHost, st));
+      CKF(env, cudaMemcpyAsync(l.n.data(), o_n, 4 * (size_t)R, cudaMemcpyDeviceToHost, st));
+      CKF(env, cudaStreamSynchronize(st));
+    }
+    if (k == K) break;
+    // the next level: count each entry's extensions, scan, fill
+    uint32_t* cnt = has;   // reused: the level's conds are built
+    long long G = 0;
+    rc = env_launch(env, ap_count_kernel, f.n, (const int*)f.set, (const uint32_t*)f.t, f.n, (const int*)L_q,
+                    (const int*)L_item, (const uint32_t*)L_end, (const int*)ix->d_child_lo, (const int*)ix->d_child_hi,
+                    (const int*)ix->d_item, cnt);
+    if (rc) return rc;
+    EVF(ap_total(env, cnt, at, f.n, &G));
+    ApFrontier g;
+    g.mem.reset(new Scratch(st));
+    g.n = G;
+    if (G > 0) {
+      CKF(env, g.mem->alloc(&g.set, (size_t)G));
+      CKF(env, g.mem->alloc(&g.t, (size_t)G));
+      rc = env_launch(env, ap_fill_kernel, f.n, (const int*)f.set, (const uint32_t*)f.t, f.n, (const int*)L_q,
+                      (const int*)L_item, (const uint32_t*)L_end, (const int*)ix->d_child_lo,
+                      (const int*)ix->d_child_hi, (const int*)ix->d_item, (const uint32_t*)at, g.set, g.t);
+      if (rc) return rc;
+    }
+    f = std::move(g);
+  }
+  // each query's conds: level by level, each level already in (query, positions) order
+  std::vector<size_t> cur(levels.size(), 0);
+  for (int q = 0; q < nq; ++q) {
+    for (size_t li = 0; li < levels.size(); ++li) {
+      const ApLevel& l = levels[li];
+      for (size_t& c = cur[li]; c < l.q.size() && l.q[c] == q; ++c) {
+        res->cond_items.insert(res->cond_items.end(), l.items.begin() + c * l.k, l.items.begin() + (c + 1) * l.k);
+        res->cond_ptr.push_back((int64_t)res->cond_items.size());
+        res->rule_first.push_back(l.rule[c]);
+        res->rule_n.push_back(l.n[c]);
+      }
+    }
+    res->q_cond_ptr[j0 + q + 1] = (int64_t)res->rule_first.size();
+  }
+  return PIO_ALS_OK;
+}
+
+// An upper bound of the frontier entries of a query with f listed frequent ids: sum over k <= K of min(C(f, k), the
+// sets of level k).  C(f, k) is exact while it fits 64 bits; beyond that the level's size bounds it.
+static unsigned long long ap_bound(const pio_assoc_index* ix, long long f, int K) {
+  unsigned long long b = 0;
+  unsigned __int128 c = 1;
+  bool big = false;
+  for (int k = 1; k <= K; ++k) {
+    const unsigned long long lk = (unsigned long long)(ix->level_off[k] - ix->level_off[k - 1]);
+    if (!big) {
+      c = c * (unsigned __int128)(f - k + 1 > 0 ? f - k + 1 : 0) / (unsigned __int128)k;
+      big = c > (unsigned __int128)~0ull;
+    }
+    b += big ? lk : std::min<unsigned long long>((unsigned long long)c, lk);
+  }
+  return b;
+}
+
+static int assoc_predict(pio_assoc_index* ix, int32_t max_cond_len, const int64_t* q_ptr, const int32_t* q_items,
+                         int32_t n_queries, const int32_t* num, int64_t* n_conds, int64_t* n_cond_items) {
+  ix->has_result = false;
+  ix->res = ApResult();
+  if (n_queries < 0 || max_cond_len < 0)
+    return fail(nullptr, PIO_ALS_ERR_ARG, "n_queries and max_cond_len must be >= 0");
+  if (!n_conds || !n_cond_items || (n_queries > 0 && (!q_ptr || !num)))
+    return fail(nullptr, PIO_ALS_ERR_ARG, "null argument");
+  if (n_queries > 0 && q_ptr[0] < 0) return fail(nullptr, PIO_ALS_ERR_ARG, "q_ptr must be non-decreasing offsets from 0");
+  for (int j = 0; j < n_queries; ++j) {
+    const long long len = q_ptr[j + 1] - q_ptr[j];
+    if (len < 0) return fail(nullptr, PIO_ALS_ERR_ARG, "q_ptr decreases at query %d", j);
+    if (len > 0 && !q_items) return fail(nullptr, PIO_ALS_ERR_ARG, "null q_items");
+    if (len >= (1ll << 31)) return fail(nullptr, PIO_ALS_ERR_ARG, "query %d lists 2^31 or more ids", j);
+  }
+  const int K = std::min(max_cond_len, ix->n_levels);
+  // PIO_ASSOC_PREDICT_BUDGET: entries per part (listed ids plus the bound of frontier entries); capped so that a part's
+  // entries are numbered in 32 bits
+  const char* env_b = getenv("PIO_ASSOC_PREDICT_BUDGET");
+  const long long budget = std::min<long long>(env_b && atoll(env_b) > 0 ? atoll(env_b) : PIO_ASSOC_PREDICT_BUDGET,
+                                               (1ll << 32) - 1);
+  std::vector<int> first;
+  long long acc = 0;
+  for (int j = 0; j < n_queries; ++j) {
+    long long freq = 0;
+    for (int64_t e = q_ptr[j]; e < q_ptr[j + 1]; ++e) {
+      const int32_t it = q_items[e];
+      freq += it >= 0 && it < ix->n_items && ix->frequent[it];
+    }
+    const unsigned long long w = (unsigned long long)(q_ptr[j + 1] - q_ptr[j]) + ap_bound(ix, freq, K);
+    if (w >= (1ull << 32))
+      return fail(nullptr, PIO_ALS_ERR_ARG,
+                  "query %d may find %llu frequent sets inside its %lld ids: at most 2^32 - 1 fit one part", j, w,
+                  (long long)(q_ptr[j + 1] - q_ptr[j]));
+    if (j == 0 || acc + (long long)w > budget) {
+      first.push_back(j);
+      acc = 0;
+    }
+    acc += (long long)w;
+  }
+  first.push_back(n_queries);
+  AssocPredictStats& s = g_ap_stats;
+  s.budget = budget;
+  ApResult res;   // moved onto ix on success
+  res.q_cond_ptr.assign((size_t)n_queries + 1, 0);
+  if (n_queries > 0 && K > 0) {
+    CK0(cudaSetDevice(ix->device));
+    int64_t launches = 0;
+    const FilterEnv env0{nullptr, ix->n_items, &launches, &g_create_error};
+    EVF(ap_upload(ix, env0));
+    FilterEnv env = env0;
+    env.st = ix->st;
+    cudaEvent_t ev[2] = {nullptr, nullptr};
+    CK0(cudaEventCreate(&ev[0]));
+    const cudaError_t e1 = cudaEventCreate(&ev[1]);
+    if (e1 != cudaSuccess) {
+      cudaEventDestroy(ev[0]);
+      CK0(e1);
+    }
+    struct Events {
+      cudaEvent_t* e;
+      ~Events() { cudaEventDestroy(e[0]), cudaEventDestroy(e[1]); }
+    } own{ev};
+    CK0(cudaEventRecord(ev[0], ix->st));
+    for (size_t p = 0; p + 1 < first.size(); ++p) {
+      const int j0 = first[p], j1 = first[p + 1];
+      s.parts += 1;
+      s.max_part_queries = std::max<long long>(s.max_part_queries, j1 - j0);
+      EVF(ap_part(ix, env, q_ptr, q_items, num, j0, j1, K, &res));
+    }
+    CK0(cudaEventRecord(ev[1], ix->st));
+    CK0(cudaEventSynchronize(ev[1]));
+    float ms = 0.f;
+    CK0(cudaEventElapsedTime(&ms, ev[0], ev[1]));
+    s.device_ms = ms;
+  }
+  res.cond_ptr.insert(res.cond_ptr.begin(), 0);
+  s.conds = (long long)res.rule_first.size();
+  *n_conds = (int64_t)res.rule_first.size();
+  *n_cond_items = (int64_t)res.cond_items.size();
+  ix->res = std::move(res);
+  ix->has_result = true;
+  return PIO_ALS_OK;
+}
+
+}  // namespace pio
+
+extern "C" {
+
+int pio_assoc_index_create(int device, int32_t n_items, int32_t n_levels, const int64_t* level_off,
+                           const int64_t* set_prefix, const int32_t* set_item, int64_t n_rules,
+                           const int64_t* rule_cond, pio_assoc_index** out) {
+  if (!out || n_items < 1 || n_levels < 0 || !level_off || n_rules < 0 || (n_rules > 0 && !rule_cond))
+    return fail(nullptr, PIO_ALS_ERR_ARG, "bad pio_assoc_index_create arguments");
+  *out = nullptr;
+  if (level_off[0] != 0) return fail(nullptr, PIO_ALS_ERR_ARG, "level_off[0] must be 0");
+  for (int l = 0; l < n_levels; ++l)
+    if (level_off[l + 1] < level_off[l]) return fail(nullptr, PIO_ALS_ERR_ARG, "level_off decreases at level %d", l + 1);
+  const int64_t n_sets = level_off[n_levels];
+  if (n_sets >= (1ll << 31)) return fail(nullptr, PIO_ALS_ERR_ARG, "%lld sets: at most 2^31 - 1", (long long)n_sets);
+  if (n_sets > 0 && (!set_prefix || !set_item)) return fail(nullptr, PIO_ALS_ERR_ARG, "null set arrays");
+  std::vector<uint8_t> frequent;
+  try {
+    frequent.assign((size_t)n_items, 0);
+  } catch (const std::bad_alloc&) {
+    return fail(nullptr, PIO_ALS_ERR_NOMEM, "pio_assoc_index_create: out of host memory");
+  }
+  for (int64_t s = 0; n_levels > 0 && s < level_off[1]; ++s)
+    if (set_item[s] >= 0 && set_item[s] < n_items) frequent[set_item[s]] = 1;
+  // the trie: level 1 holds distinct items ascending; a set of level l >= 2 extends a set of level l - 1 by a larger
+  // frequent item, with prefixes non-decreasing and, under one prefix, items ascending
+  for (int l = 1; l <= n_levels; ++l)
+    for (int64_t s = level_off[l - 1]; s < level_off[l]; ++s) {
+      const int64_t p = set_prefix[s];
+      const int32_t it = set_item[s];
+      if (it < 0 || it >= n_items || !frequent[it])
+        return fail(nullptr, PIO_ALS_ERR_ARG, "set %lld: item %d is not a level-1 item in [0, %d)", (long long)s, it,
+                    n_items);
+      if (l == 1 ? p != -1 : (p < level_off[l - 2] || p >= level_off[l - 1]))
+        return fail(nullptr, PIO_ALS_ERR_ARG, "set %lld: prefix %lld is not a set of level %d", (long long)s,
+                    (long long)p, l - 1);
+      const bool same = s > level_off[l - 1] && set_prefix[s - 1] == p;
+      if ((s > level_off[l - 1] && set_prefix[s - 1] > p) || (same && set_item[s - 1] >= it))
+        return fail(nullptr, PIO_ALS_ERR_ARG, "set %lld is out of lexicographic order", (long long)s);
+      if (l > 1 && set_item[p] >= it)
+        return fail(nullptr, PIO_ALS_ERR_ARG, "set %lld: item %d is not larger than its prefix's", (long long)s, it);
+    }
+  for (int64_t r = 0; r < n_rules; ++r)
+    if (rule_cond[r] < 0 || rule_cond[r] >= n_sets || (r > 0 && rule_cond[r] < rule_cond[r - 1]))
+      return fail(nullptr, PIO_ALS_ERR_ARG, "rule %lld: cond %lld is not a set index grouped in set order",
+                  (long long)r, (long long)rule_cond[r]);
+  std::unique_ptr<pio_assoc_index> ix;
+  try {   // bad_alloc must not cross the C boundary
+    ix.reset(new pio_assoc_index);
+    ix->device = device, ix->n_items = n_items, ix->n_levels = n_levels, ix->n_sets = n_sets, ix->n_rules = n_rules;
+    ix->level_off.assign(level_off, level_off + n_levels + 1);
+    ix->set_prefix.assign(set_prefix, set_prefix + n_sets);
+    ix->set_item.assign(set_item, set_item + n_sets);
+    ix->rule_cond.assign(rule_cond, rule_cond + n_rules);
+    ix->frequent.swap(frequent);
+  } catch (const std::bad_alloc&) {
+    return fail(nullptr, PIO_ALS_ERR_NOMEM, "pio_assoc_index_create: out of host memory");
+  }
+  *out = ix.release();
+  return PIO_ALS_OK;
+}
+
+int pio_assoc_index_destroy(pio_assoc_index* ix) {
+  if (!ix) return PIO_ALS_OK;
+  if (ix->st) {
+    cudaSetDevice(ix->device);
+    cudaStreamSynchronize(ix->st);
+    cudaStreamDestroy(ix->st);
+  }
+  ap_free_device(ix);
+  delete ix;
+  return PIO_ALS_OK;
+}
+
+int pio_assoc_predict(pio_assoc_index* ix, int32_t max_cond_len, const int64_t* q_ptr, const int32_t* q_items,
+                      int32_t n_queries, const int32_t* num, int64_t* n_conds, int64_t* n_cond_items) {
+  g_ap_stats = AssocPredictStats{};
+  if (!ix) return fail(nullptr, PIO_ALS_ERR_ARG, "null association index");
+  std::lock_guard<std::mutex> lk(ix->mu);
+  try {   // bad_alloc must not cross the C boundary; Scratch releases a part's device memory on the way out
+    return assoc_predict(ix, max_cond_len, q_ptr, q_items, n_queries, num, n_conds, n_cond_items);
+  } catch (const std::bad_alloc&) {
+    return fail(nullptr, PIO_ALS_ERR_NOMEM, "pio_assoc_predict: out of host memory");
+  }
+}
+
+int pio_assoc_predict_get(pio_assoc_index* ix, int64_t* q_cond_ptr, int64_t* cond_ptr, int32_t* cond_items,
+                          int64_t* rule_first, int32_t* rule_n) {
+  if (!ix) return fail(nullptr, PIO_ALS_ERR_ARG, "null association index");
+  std::lock_guard<std::mutex> lk(ix->mu);
+  if (!ix->has_result) return fail(nullptr, PIO_ALS_ERR_STATE, "no pio_assoc_predict result to get");
+  auto put = [](auto* dst, auto& v) {
+    if (dst && !v.empty()) memcpy(dst, v.data(), v.size() * sizeof(v[0]));
+    std::remove_reference_t<decltype(v)>().swap(v);
+  };
+  put(q_cond_ptr, ix->res.q_cond_ptr);
+  put(cond_ptr, ix->res.cond_ptr);
+  put(cond_items, ix->res.cond_items);
+  put(rule_first, ix->res.rule_first);
+  put(rule_n, ix->res.rule_n);
+  ix->has_result = false;
+  return PIO_ALS_OK;
+}
+
+int pio_assoc_predict_debug_stats(double out[40]) {
+  if (!out) return PIO_ALS_ERR_ARG;
+  const AssocPredictStats& s = g_ap_stats;
+  out[0] = (double)s.parts, out[1] = (double)s.max_part_queries, out[2] = (double)s.budget, out[3] = (double)s.conds;
+  out[4] = s.device_ms;
+  for (int j = 5; j < 8; ++j) out[j] = 0;
+  for (int k = 1; k <= 32; ++k) out[7 + k] = (double)s.entries[k];   // out[8 .. 39]
   return PIO_ALS_OK;
 }
 

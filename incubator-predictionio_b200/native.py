@@ -49,7 +49,8 @@ EXPORTED_SYMBOLS = [
     "pio_popular_predict_filtered", "pio_popular_model_get_stats", "pio_popular_model_destroy", "pio_assoc_train",
     "pio_assoc_model_size", "pio_assoc_model_get", "pio_assoc_model_destroy", "pio_rf_train_regressor",
     "pio_rf_forest_reg_size", "pio_rf_forest_reg_get", "pio_rf_predict_regression", "pio_lead_sessions",
-    "pio_als_rank_lists", "pio_rank_lists_debug_stats",
+    "pio_als_rank_lists", "pio_rank_lists_debug_stats", "pio_assoc_index_create", "pio_assoc_index_destroy",
+    "pio_assoc_predict", "pio_assoc_predict_get", "pio_assoc_predict_debug_stats",
 ]
 
 
@@ -212,6 +213,13 @@ def lib():
         L.pio_popular_model_get_stats.argtypes = [vp, vp]
         L.pio_als_rank_lists.restype = ci
         L.pio_als_rank_lists.argtypes = [vp, vp, C.c_int32, vp, vp, vp, vp, vp]
+        L.pio_assoc_index_create.restype = ci
+        L.pio_assoc_index_create.argtypes = [ci, C.c_int32, C.c_int32, vp, vp, vp, i64, vp, vp]
+        L.pio_assoc_index_destroy.argtypes = [vp]
+        L.pio_assoc_predict.restype = ci
+        L.pio_assoc_predict.argtypes = [vp, C.c_int32, vp, vp, C.c_int32, vp, vp, vp]
+        L.pio_assoc_predict_get.restype = ci
+        L.pio_assoc_predict_get.argtypes = [vp, vp, vp, vp, vp, vp]
         for name in EXPORTED_SYMBOLS:
             getattr(L, name)  # AttributeError if the ABI is incomplete
         _lib = L
@@ -1427,6 +1435,85 @@ def assoc_train_timing() -> dict:
     res.update(baskets=int(out[8]), transactions=int(out[9]), levels_run=int(out[10]), rejected_level=int(out[11]),
                candidates={k: int(out[16 + k]) for k in range(2, 33) if out[16 + k]})
     return res
+
+
+class AssocIndex:
+    """pio_assoc_index: a model's frequent-set trie and the cond of each rule (assoc_train's level_off, set_prefix,
+    set_item and rule_cond) that finds the conds of batches of queries on `device`.  The arrays are checked and copied
+    when it is created; the device copy is made by the first predict."""
+
+    def __init__(self, level_off, set_prefix, set_item, rule_cond, n_items: int, device: int = 0):
+        lo = np.ascontiguousarray(level_off, np.int64)
+        sp = np.ascontiguousarray(set_prefix, np.int64)
+        si = np.ascontiguousarray(set_item, np.int32)
+        rc = np.ascontiguousarray(rule_cond, np.int64)
+        if lo.ndim != 1 or lo.shape[0] < 1 or sp.shape != si.shape or rc.ndim != 1:
+            raise ValueError("level_off must be [n_levels + 1], set_prefix / set_item [n_sets] and rule_cond [n_rules]")
+        if int(lo[-1]) != sp.shape[0]:
+            raise ValueError(f"level_off ends at {int(lo[-1])}, but there are {sp.shape[0]} sets")
+        self.n_items, self.n_levels = int(n_items), int(lo.shape[0] - 1)
+        self._h = C.c_void_p()
+        _check(lib().pio_assoc_index_create(int(device), self.n_items, self.n_levels, lo.ctypes.data, sp.ctypes.data,
+                                            si.ctypes.data, rc.shape[0], rc.ctypes.data, C.addressof(self._h)))
+
+    def close(self):
+        if self._h:
+            lib().pio_assoc_index_destroy(self._h)
+            self._h = C.c_void_p()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    def predict(self, q_ptr, q_items, num, max_cond_len: int):
+        """Query j lists the ids q_items[q_ptr[j]:q_ptr[j + 1]] and wants num[j] rules per cond.  Returns (q_cond_ptr
+        int64 [n + 1], cond_ptr int64 [n_conds + 1], cond_items int32, rule_first int64 [n_conds], rule_n int32
+        [n_conds]): query j's conds are [q_cond_ptr[j], q_cond_ptr[j + 1]), each with its items in query order, its first
+        rule and its number of rules, in the order of Algorithm.predict."""
+        ptr = np.ascontiguousarray(q_ptr, np.int64)
+        flat = np.ascontiguousarray(q_items, np.int32)
+        num = np.ascontiguousarray(num, np.int32)
+        n = ptr.shape[0] - 1
+        if n < 0 or num.shape != (n,):
+            raise ValueError("q_ptr must be [n + 1] and num [n]")
+        nc, ni = C.c_int64(0), C.c_int64(0)
+        _check(lib().pio_assoc_predict(self._h, int(max_cond_len), ptr.ctypes.data, flat.ctypes.data, n,
+                                       num.ctypes.data, C.addressof(nc), C.addressof(ni)))
+        out = (np.zeros(n + 1, np.int64), np.zeros(nc.value + 1, np.int64), np.empty(ni.value, np.int32),
+               np.empty(nc.value, np.int64), np.empty(nc.value, np.int32))
+        _check(lib().pio_assoc_predict_get(self._h, *[a.ctypes.data for a in out]))
+        return out
+
+
+def assoc_predict_stats() -> dict:
+    """What the last AssocIndex.predict on this thread did: its parts, the most queries in one part, the entries
+    budget, the conds returned, the device milliseconds from the first upload to the last copy back, and the frequent
+    sets found inside the queries per level."""
+    out = (C.c_double * 40)()
+    _check(lib().pio_assoc_predict_debug_stats(out))
+    return {"parts": int(out[0]), "max_part_queries": int(out[1]), "budget": int(out[2]), "conds": int(out[3]),
+            "device_ms": out[4], "entries": {k: int(out[7 + k]) for k in range(1, 33) if out[7 + k]}}
+
+
+@dataclass
+class RuleColumns:
+    """A batch of association-rule results as arrays (AssocIndex.predict's five, plus the model's rule arrays): query j's
+    rules are conds [q_cond_ptr[j], q_cond_ptr[j + 1]), cond c lists the item ids cond_items[cond_ptr[c]:cond_ptr[c + 1]]
+    and has the rules rule_first[c] .. rule_first[c] + rule_n[c] - 1, rule r scoring item rule_conseq[r] with
+    support[r], confidence[r] and lift[r]; names[id] is the item string of an id.  device: the GPU that found them."""
+    q_cond_ptr: np.ndarray
+    cond_ptr: np.ndarray
+    cond_items: np.ndarray
+    rule_first: np.ndarray
+    rule_n: np.ndarray
+    rule_conseq: np.ndarray
+    support: np.ndarray
+    confidence: np.ndarray
+    lift: np.ndarray
+    names: Sequence[str]
+    device: Optional[int] = None
 
 
 def nb_predict(x, pi, theta, device=0):

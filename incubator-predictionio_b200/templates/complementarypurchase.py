@@ -4,12 +4,13 @@ Mirrors docs/manual/source/templates/complementarypurchase/dase.html.md.erb (Que
 ItemScore, DataSource, Preparator, AlgorithmParams, Algorithm.train / predict, Serving) and quickstart.html.md.erb.
 The doc elides how transactions, counts and rules are built (lines 293-314); tests/assoc_ref.py states them and
 DESIGN.md 4.15 describes the device pipeline.  Training runs on the GPU (native.assoc_train); predict is a dictionary
-lookup and stays on the host.
+lookup and stays on the host; predictMany and BatchPredict find every query's conds in the frequent-set trie on the GPU
+(native.AssocIndex, DESIGN.md 4.15.1).
 """
 from __future__ import annotations
 
 from dataclasses import dataclass
-from itertools import combinations
+from itertools import combinations, islice
 from typing import Dict, FrozenSet, List, Optional, Tuple
 
 import numpy as np
@@ -134,17 +135,19 @@ class Model:
     the frequent item sets (set_prefix, set_item, set_count; sets by length, then in lexicographic order of their item
     indices) and the rules grouped by condition and ranked (rule_cond, rule_conseq, support, confidence, lift), with
     itemStringIntMap numbering the items.  `rules` (cond as a frozenset of item indices -> (first, end) of its rules)
-    is built on first use and kept out of the pickle."""
+    is built on first use, and so is the device index predictMany uses (native.AssocIndex on `device`, the training
+    GPU); both are kept out of the pickle."""
 
-    _CACHES = ("_rules",)
+    _CACHES = ("_rules", "_index", "_item_names")
 
-    def __init__(self, arrays: dict, itemStringIntMap: BiMap, maxRuleLength: int):
+    def __init__(self, arrays: dict, itemStringIntMap: BiMap, maxRuleLength: int, device: int = 0):
         for k in native.ASSOC_ARRAYS:
             setattr(self, k, np.asarray(arrays[k]))
         self.n_transactions = int(arrays["n_transactions"])
         self.itemStringIntMap = itemStringIntMap
         self.itemIntStringMap = itemStringIntMap.inverse
         self.maxRuleLength = maxRuleLength
+        self.device = device
 
     def set_items(self, s: int) -> Tuple[int, ...]:
         """The item indices of frequent set s, ascending."""
@@ -168,8 +171,26 @@ class Model:
             self._rules = r = {key: tuple(v) for key, v in r.items()}
         return r
 
+    def device_index(self) -> "native.AssocIndex":
+        ix = self.__dict__.get("_index")
+        if ix is None:
+            ix = self._index = native.AssocIndex(self.level_off, self.set_prefix, self.set_item, self.rule_cond,
+                                                 max(self.itemStringIntMap.size, 1), getattr(self, "device", 0))
+        return ix
+
+    def item_names(self) -> List[str]:
+        names = self.__dict__.get("_item_names")
+        if names is None:
+            names = self._item_names = native.item_names(self.itemStringIntMap)
+        return names
+
     def __getstate__(self):
         return {k: v for k, v in self.__dict__.items() if k not in self._CACHES}
+
+    def __del__(self):
+        ix = self.__dict__.get("_index")
+        if ix is not None:
+            ix.close()
 
 
 class Algorithm(P2LAlgorithm):
@@ -211,7 +232,7 @@ class Algorithm(P2LAlgorithm):
             if e.code == native.ERR_ARG:
                 raise ValueError(str(e)) from e
             raise
-        return Model(arrays, itemMap, ap.maxRuleLength)
+        return Model(arrays, itemMap, ap.maxRuleLength, getattr(sc, "device", 0) or 0)
 
     def predict(self, model: Model, query: Query) -> PredictedResult:
         """Every subset of the query's items of size 1 .. maxRuleLength - 1 (by size, then in lexicographic order of
@@ -236,10 +257,64 @@ class Algorithm(P2LAlgorithm):
                               float(model.lift[r])) for r in range(lo, hi)]))
         return PredictedResult(out)
 
+    def predictManyColumns(self, model: Model, queries) -> native.RuleColumns:
+        """predict for many queries as columns, before any result object is built: the query strings mapped to item
+        indices (unknown: -1), then one device call per batch (native.AssocIndex.predict), which finds the conds of
+        every query in the frequent-set trie in predict's order."""
+        res = model.device_index().predict(*query_arrays(model, list(queries)), model.maxRuleLength - 1)
+        return native.RuleColumns(*res, model.rule_conseq, model.support, model.confidence, model.lift,
+                                  model.item_names(), getattr(model, "device", 0))
+
+    def predictMany(self, model: Model, queries) -> List[PredictedResult]:
+        """[predict(model, q) for q in queries], from predictManyColumns' arrays: the same Rules in the same order, with
+        the same cond lists and ItemScore floats."""
+        return rule_results(self.predictManyColumns(model, queries))
+
+
+def query_arrays(model: Model, queries):
+    """(ptr, ids, num) of a batch: query j's items as item indices in ids[ptr[j]:ptr[j + 1]] (-1: unknown to the
+    model) and its num, clipped to int32 (min(rules, max(num, 0)) is unchanged)."""
+    get = model.itemStringIntMap.getOrElse
+    lists = [[get(x, -1) for x in q.items] for q in queries]
+    ptr = np.zeros(len(lists) + 1, np.int64)
+    ptr[1:] = np.cumsum([len(l) for l in lists])
+    ids = np.fromiter((i for l in lists for i in l), np.int32, int(ptr[-1]))
+    num = np.clip(np.array([int(q.num) for q in queries], np.int64), -1, 2 ** 31 - 1)
+    return ptr, ids, num
+
+
+def used_rules(cols: native.RuleColumns) -> np.ndarray:
+    """The rule index of every ItemScore of a batch, in output order (the model's rule arrays are not copied whole)."""
+    n = cols.rule_n.astype(np.int64)
+    start = np.cumsum(n) - n
+    return np.repeat(cols.rule_first - start, n) + np.arange(int(n.sum()), dtype=np.int64)
+
+
+def rule_results(cols: native.RuleColumns) -> List[PredictedResult]:
+    """The PredictedResult of every query of a RuleColumns batch."""
+    names = cols.names
+    r = used_rules(cols)
+    scores = iter(zip(cols.rule_conseq[r].tolist(), cols.support[r].tolist(), cols.confidence[r].tolist(),
+                      cols.lift[r].tolist()))
+    qp, cp, items, count = (cols.q_cond_ptr.tolist(), cols.cond_ptr.tolist(), cols.cond_items.tolist(),
+                            cols.rule_n.tolist())
+    out = []
+    for j in range(len(qp) - 1):
+        rules = []
+        for c in range(qp[j], qp[j + 1]):
+            rules.append(Rule([names[i] for i in items[cp[c]:cp[c + 1]]],
+                              [ItemScore(names[i], a, b, d) for i, a, b, d in islice(scores, count[c])]))
+        out.append(PredictedResult(rules))
+    return out
+
 
 class Serving(LServing):
     def serve(self, query: Query, predictedResults) -> PredictedResult:
         return predictedResults[0]
+
+    def serveManyColumns(self, queries, predictions) -> native.RuleColumns:
+        """serve for a batch of columns: the first algorithm's."""
+        return predictions[0]
 
 
 class ComplementaryPurchaseEngine(EngineFactory):

@@ -32,6 +32,7 @@ from typing import Any, Dict, Iterator, List, Optional, Sequence, Tuple
 
 from .controller import (Engine, EngineFactory, EngineParams, PersistentModelManifest, StopAfterPrepareInterruption,
                          StopAfterReadInterruption, Unit, extract_params)
+from .native import RuleColumns
 
 logger = logging.getLogger("pio.workflow")
 
@@ -453,6 +454,9 @@ class BatchPredict:
             if quoted.get(id(cols.names), (None,))[0] is not cols.names:
                 quoted[id(cols.names)] = (cols.names, [json.dumps(s) for s in cols.names])
             names = quoted[id(cols.names)][1]
+            if isinstance(cols, RuleColumns):
+                yield from BatchPredict._rule_lines(qs, cols, names)
+                continue
             items, scores, count = cols.items.tolist(), cols.scores.tolist(), cols.count.tolist()
             for j, q in enumerate(qs):
                 head = '{"query":' + json.dumps(to_json(q), separators=sep) + ',"prediction":'
@@ -463,6 +467,31 @@ class BatchPredict:
                 yield head + '{"itemScores":[' + ",".join(
                     '{"item":' + names[i] + ',"score":' + _float_json(v) + "}"
                     for i, v in zip(items[j][:n], scores[j][:n])) + "]}}"
+
+    @staticmethod
+    def _rule_lines(qs, cols: "RuleColumns", names: Sequence[str]) -> Iterator[str]:
+        """The lines of a batch of association-rule results, {"rules": [{"cond": [...], "itemScores": [{"item", "support",
+        "confidence", "lift"}, ...]}, ...]} written from the columns with json's own string and float forms: the bytes
+        of json.dumps of the result objects.  A rule's itemScore is written once per batch."""
+        sep = (",", ":")
+        qp, cp, items = cols.q_cond_ptr.tolist(), cols.cond_ptr.tolist(), cols.cond_items.tolist()
+        first, count = cols.rule_first.tolist(), cols.rule_n.tolist()
+        scored = {}   # rule index -> its itemScore JSON
+
+        def score(r: int) -> str:
+            t = scored.get(r)
+            if t is None:
+                t = scored[r] = ('{"item":' + names[int(cols.rule_conseq[r])] + ',"support":' +
+                                 _float_json(float(cols.support[r])) + ',"confidence":' +
+                                 _float_json(float(cols.confidence[r])) + ',"lift":' + _float_json(float(cols.lift[r])) +
+                                 "}")
+            return t
+
+        for j, q in enumerate(qs):
+            rules = ",".join('{"cond":[' + ",".join(names[i] for i in items[cp[c]:cp[c + 1]]) + '],"itemScores":[' +
+                             ",".join(score(r) for r in range(first[c], first[c] + count[c])) + "]}"
+                             for c in range(qp[j], qp[j + 1]))
+            yield '{"query":' + json.dumps(to_json(q), separators=sep) + ',"prediction":{"rules":[' + rules + "]}}"
 
     @staticmethod
     def main(argv: Optional[Sequence[str]] = None) -> int:
