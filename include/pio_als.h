@@ -858,6 +858,53 @@ PIO_API int pio_assoc_predict_get(pio_assoc_index* ix, int64_t* q_cond_ptr, int6
  * sets found inside the queries at level k (1 <= k <= 32). */
 PIO_API int pio_assoc_predict_debug_stats(double out[40]);
 
+/* The text classification template (docs/manual/source/demo/textclassification.html.md.erb; DESIGN.md 4.18): hashed
+ * n-gram term frequencies, IDF and multinomial Naive Bayes on sparse TF-IDF vectors.  HOST buffers.  Documents enter as
+ * raw JSON string tokens (what pio_events_scan_keys returns, or json.dumps of a string): document d is
+ * tok_bytes[tok_off[d] .. tok_off[d + 1]), quotes included.  Each is decoded on the device (an escaped unpaired
+ * surrogate becomes '?'), split on U+0020 as Java's String.split(" ") splits, stripped of the model's stop words (exact
+ * byte equality), cut into n-gram windows (Scala's sliding(nGram), tokens joined with no separator) and hashed with
+ * Spark 2.1's murmur3 (hashUnsafeBytes, seed 42) into nonNegativeMod(h, numFeatures).  Every call runs in parts of
+ * consecutive documents within PIO_TEXT_BUDGET raw token bytes (a document over it forms a part of its own); results
+ * do not depend on the budget.  Rejected with PIO_ALS_ERR_ARG before any device work: nGram < 1, numFeatures < 1,
+ * lambda < 0 or NaN, n_docs < 0, tok_off decreasing, a token of 2^31 bytes or more, and a token that does not start and
+ * end with '"'. */
+#define PIO_TEXT_BUDGET (1ll << 26)
+typedef struct pio_text_model pio_text_model;
+/* The featurizer of PreparatorParams(nGram, numFeatures) with n_stop stop words stop_bytes[stop_off[w] ..
+ * stop_off[w + 1]) (UTF-8; repeats are ignored), on `device`.  It scores once pio_text_model_set has given it a model. */
+PIO_API int pio_text_model_create(int device, const uint8_t* stop_bytes, const int64_t* stop_off, int32_t n_stop,
+                                  int32_t n_gram, int32_t num_features, pio_text_model** out);
+PIO_API int pio_text_model_destroy(pio_text_model* m);
+/* A trained or loaded model: idf [numFeatures], pi [n_class], theta [n_class x numFeatures] row-major, copied to the
+ * device once. */
+PIO_API int pio_text_model_set(pio_text_model* m, int32_t n_class, const double* idf, const double* pi,
+                               const double* theta);
+/* IDF.fit and NaiveBayes.train(lambda) on n_docs >= 1 documents, label[d] in [0, n_class) (the index of the document's
+ * label among the sorted labels).  Out: df [numFeatures] (documents holding the feature), idf_j = log((m + 1.0) /
+ * (df_j + 1.0)), pi_c = log(n_c + l) - log(m + C l), theta_cj = log(s_cj + l) - log(sum_j s_cj + D l) with the sum in j
+ * order; s_cj, the class's sum of tf * idf_j, is exact and rounded once.  PIO_ALS_ERR_NUMERIC when a nonzero tf * idf_j
+ * lies outside [2^-44, 2^63), or the corpus has 2^33 (document, feature) entries or more.  Logarithms are taken on the
+ * host. */
+PIO_API int pio_text_train_nb(pio_text_model* m, const uint8_t* tok_bytes, const int64_t* tok_off, int32_t n_docs,
+                              const int32_t* label, int32_t n_class, double lambda, int64_t* out_df, double* out_idf,
+                              double* out_pi, double* out_theta);
+/* The TF (use_idf 0) or TF-IDF (use_idf 1: tf * idf_j, one fp64 multiply; needs a model) vectors of a batch as COO;
+ * *out_nnz = its entries.  pio_text_features_get copies the result out once: doc_ptr [n_docs + 1], index [nnz]
+ * (ascending within a document) and value [nnz]. */
+PIO_API int pio_text_features(pio_text_model* m, const uint8_t* tok_bytes, const int64_t* tok_off, int32_t n_docs,
+                              int32_t use_idf, int64_t* out_nnz);
+PIO_API int pio_text_features_get(pio_text_model* m, int64_t* doc_ptr, int32_t* index, double* value);
+/* out_scores [n_docs x n_class]: per query q and class c, the left fold from 0.0 of theta_cj * x_j over q's TF-IDF
+ * entries in index order, each product and add rounded on its own, then + pi_c: the reference's dense
+ * innerProduct(theta_c, x.toArray) + pi_c, which is NaN when theta_c has a non-finite entry at an index q lacks. */
+PIO_API int pio_text_scores(pio_text_model* m, const uint8_t* tok_bytes, const int64_t* tok_off, int32_t n_docs,
+                            double* out_scores);
+/* What the last pio_text_train_nb / _features / _scores on this thread did: out[0] parts, [1] documents, [2] n-gram
+ * windows, [3] (document, feature) entries, [4] most token bytes in one part, [5] the budget, [6] device
+ * milliseconds. */
+PIO_API int pio_text_debug_stats(double out[7]);
+
 #ifdef __cplusplus
 }
 #endif

@@ -201,6 +201,61 @@ PIO_EV_HD int decode_string(const uint8_t* s, int b, int e, uint8_t* out) {
   return o;
 }
 
+// decode_string for a string token in which a \u escape may name an unpaired surrogate (json.dumps writes one for a
+// Python string that holds it): such an escape becomes '?', as Java's getBytes(UTF_8) writes an unpaired surrogate, and
+// an escaped pair still becomes one 4-byte character.  A malformed escape also becomes '?'.  Never writes more than
+// e - b - 2 bytes and never reads outside [b, e).
+PIO_EV_HD int decode_string_lenient(const uint8_t* s, int b, int e, uint8_t* out) {
+  int i = b + 1, o = 0;
+  const int end = e - 1;
+  while (i < end) {
+    const uint8_t c = s[i];
+    if (c != '\\') {
+      out[o++] = c;
+      ++i;
+      continue;
+    }
+    const uint8_t d = s[i + 1];
+    if (d != 'u') {
+      out[o++] = d == 'b' ? 8 : d == 'f' ? 12 : d == 'n' ? 10 : d == 'r' ? 13 : d == 't' ? 9 : d;
+      i += 2;
+      continue;
+    }
+    const int h = hex4(s, end, i + 2);
+    i += 6;
+    uint32_t u = (uint32_t)h;
+    if (h < 0 || (h >= 0xDC00 && h <= 0xDFFF)) {
+      out[o++] = '?';
+      continue;
+    }
+    if (h >= 0xD800 && h <= 0xDBFF) {
+      const int l = i + 1 < end && s[i] == '\\' && s[i + 1] == 'u' ? hex4(s, end, i + 2) : -1;
+      if (l < 0xDC00 || l > 0xDFFF) {
+        out[o++] = '?';
+        continue;
+      }
+      u = 0x10000u + ((u - 0xD800u) << 10) + ((uint32_t)l - 0xDC00u);
+      i += 6;
+    }
+    if (u < 0x80) {
+      out[o++] = (uint8_t)u;
+    } else if (u < 0x800) {
+      out[o++] = (uint8_t)(0xC0 | (u >> 6));
+      out[o++] = (uint8_t)(0x80 | (u & 0x3F));
+    } else if (u < 0x10000) {
+      out[o++] = (uint8_t)(0xE0 | (u >> 12));
+      out[o++] = (uint8_t)(0x80 | ((u >> 6) & 0x3F));
+      out[o++] = (uint8_t)(0x80 | (u & 0x3F));
+    } else {
+      out[o++] = (uint8_t)(0xF0 | (u >> 18));
+      out[o++] = (uint8_t)(0x80 | ((u >> 12) & 0x3F));
+      out[o++] = (uint8_t)(0x80 | ((u >> 6) & 0x3F));
+      out[o++] = (uint8_t)(0x80 | (u & 0x3F));
+    }
+  }
+  return o;
+}
+
 PIO_EV_HD bool bytes_eq(const uint8_t* a, const uint8_t* b, int n) {
   for (int k = 0; k < n; ++k)
     if (a[k] != b[k]) return false;

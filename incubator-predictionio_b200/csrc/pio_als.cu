@@ -64,6 +64,8 @@
 #include "assoc.cuh"
 #include "rank_lists.cuh"
 #include "assoc_predict.cuh"
+#include "text_nb.cuh"
+#include "text_plan.h"
 
 namespace pio {
 
@@ -8191,6 +8193,491 @@ int pio_assoc_predict_debug_stats(double out[40]) {
   out[4] = s.device_ms;
   for (int j = 5; j < 8; ++j) out[j] = 0;
   for (int k = 1; k <= 32; ++k) out[7 + k] = (double)s.entries[k];   // out[8 .. 39]
+  return PIO_ALS_OK;
+}
+
+}  // extern "C"
+
+// ---- text classification (pio_text_*) -----------------------------------------------------------------------------------
+struct pio_text_model {
+  int device = 0, n_gram = 1, num_features = 1, n_stop = 0, n_class = 0;
+  unsigned stop_mask = 0;
+  cudaStream_t st = nullptr;
+  int* d_slot = nullptr;
+  uint8_t* d_stop = nullptr;
+  long long* d_stop_off = nullptr;
+  double *d_idf = nullptr, *d_pi = nullptr, *d_theta = nullptr;
+  int* d_nonfinite = nullptr;
+  std::mutex mu;                                   // serialises the calls
+  bool has_features = false;                       // the last pio_text_features result, until _get takes it
+  std::vector<int64_t> f_ptr;
+  std::vector<int32_t> f_idx;
+  std::vector<double> f_val;
+};
+
+namespace pio {
+
+// what the last pio_text_* call on this thread did (pio_text_debug_stats)
+struct TextStats {
+  long long parts = 0, docs = 0, windows = 0, entries = 0, max_part_bytes = 0, budget = 0;
+  double device_ms = 0.0;
+};
+static thread_local TextStats g_tx_stats;
+
+// One part's (document, index, count) entries, in (document, index) order; documents local to the part.
+struct TxEntries {
+  uint32_t *doc = nullptr, *idx = nullptr, *cnt = nullptr;
+  long long n = 0;
+};
+
+static int tx_check_tokens(const uint8_t* tok_bytes, const int64_t* tok_off, int32_t n) {
+  if (n < 0) return fail(nullptr, PIO_ALS_ERR_ARG, "n_docs must be >= 0");
+  if (!tok_off || (n > 0 && !tok_bytes)) return fail(nullptr, PIO_ALS_ERR_ARG, "null token argument");
+  if (tok_off[0] < 0) return fail(nullptr, PIO_ALS_ERR_ARG, "tok_off[0] must be >= 0");
+  for (int d = 0; d < n; ++d) {
+    const long long len = tok_off[d + 1] - tok_off[d];
+    if (len < 0) return fail(nullptr, PIO_ALS_ERR_ARG, "tok_off decreases at document %d", d);
+    if (len >= (1ll << 31)) return fail(nullptr, PIO_ALS_ERR_ARG, "document %d: a token holds fewer than 2^31 bytes", d);
+    if (len < 2 || tok_bytes[tok_off[d]] != '"' || tok_bytes[tok_off[d + 1] - 1] != '"')
+      return fail(nullptr, PIO_ALS_ERR_ARG, "document %d is not a JSON string token", d);
+  }
+  return PIO_ALS_OK;
+}
+
+static std::vector<TextPart> tx_plan(const int64_t* tok_off, int32_t n) {
+  // PIO_TEXT_BUDGET: raw token bytes per part; capped so that a part's bytes are numbered in 31 bits
+  const char* env_b = getenv("PIO_TEXT_BUDGET");
+  const long long budget = std::min<long long>(env_b && atoll(env_b) > 0 ? atoll(env_b) : PIO_TEXT_BUDGET,
+                                               (1ll << 31) - 1);
+  g_tx_stats.budget = budget;
+  return plan_text(tok_off, n, budget);
+}
+
+// The entries of part p: decode, split, stop words, n-gram hashes, the sort and its runs.  The entries go into `keep`
+// (they outlive the part); everything else is released when the part returns.
+static int tx_part(pio_text_model* m, Scratch& keep, const uint8_t* tok_bytes, const int64_t* tok_off,
+                   const TextPart& p, TxEntries* out) {
+  cudaStream_t st = m->st;
+  const int nd = p.d1 - p.d0;
+  const long long nb = p.b1 - p.b0;
+  TextStats& s = g_tx_stats;
+  s.parts += 1, s.docs += nd, s.max_part_bytes = std::max(s.max_part_bytes, nb);
+  std::vector<long long> off((size_t)nd + 1);
+  for (int j = 0; j <= nd; ++j) off[j] = tok_off[p.d0 + j] - p.b0;
+  Scratch tmp(st);
+  uint8_t *d_raw = nullptr, *d_dec = nullptr;
+  long long* d_off = nullptr;
+  uint32_t *d_tb = nullptr, *d_tn = nullptr, *d_ntok = nullptr, *d_nwin = nullptr, *d_woff = nullptr;
+  CK0(tmp.alloc(&d_raw, (size_t)nb));
+  CK0(tmp.alloc(&d_dec, (size_t)nb));
+  CK0(tmp.alloc(&d_off, (size_t)nd + 1));
+  CK0(tmp.alloc(&d_tb, (size_t)nb));
+  CK0(tmp.alloc(&d_tn, (size_t)nb));
+  CK0(tmp.alloc(&d_ntok, (size_t)nd));
+  CK0(tmp.alloc(&d_nwin, (size_t)nd));
+  CK0(tmp.alloc(&d_woff, (size_t)nd));
+  CK0(cudaMemcpyAsync(d_raw, tok_bytes + p.b0, (size_t)nb, cudaMemcpyHostToDevice, st));
+  CK0(cudaMemcpyAsync(d_off, off.data(), sizeof(long long) * off.size(), cudaMemcpyHostToDevice, st));
+  const TxStop stop{m->d_slot, m->d_stop, m->d_stop_off, m->stop_mask, m->n_stop};
+  tx_split_kernel<<<nblk(nd, 256), 256, 0, st>>>(d_raw, d_off, nd, stop, m->n_gram, d_dec, d_tb, d_tn, d_ntok, d_nwin);
+  CK0(cudaGetLastError());
+  CK0(scan_exclusive_u32(d_nwin, d_woff, (size_t)nd, st, nullptr));
+  uint32_t last[2] = {0, 0};
+  CK0(cudaMemcpyAsync(&last[0], d_woff + nd - 1, 4, cudaMemcpyDeviceToHost, st));
+  CK0(cudaMemcpyAsync(&last[1], d_nwin + nd - 1, 4, cudaMemcpyDeviceToHost, st));
+  CK0(cudaStreamSynchronize(st));
+  const long long W = (long long)last[0] + last[1];
+  s.windows += W;
+  out->n = 0;
+  if (W == 0) return PIO_ALS_OK;
+  SortBufs sb;
+  for (int b = 0; b < 2; ++b) {
+    CK0(tmp.alloc(&sb.k[b], (size_t)W));
+    CK0(tmp.alloc(&sb.v[b], (size_t)W));
+  }
+  const int fbits = ceil_log2((uint64_t)m->num_features), dbits = ceil_log2((uint64_t)nd);
+  tx_hash_kernel<<<nblk(W, 256), 256, 0, st>>>(d_dec, d_off, d_tb, d_tn, d_ntok, d_woff, nd, W, m->n_gram,
+                                               m->num_features, fbits, sb.keys(), sb.vals());
+  CK0(cudaGetLastError());
+  CK0(radix_sort_pairs(sb, (size_t)W, fbits + dbits, st, nullptr));
+  uint32_t *d_flag = nullptr, *d_rid = nullptr;
+  CK0(tmp.alloc(&d_flag, (size_t)W));
+  CK0(tmp.alloc(&d_rid, (size_t)W));
+  tx_head_flag_kernel<<<nblk(W, 256), 256, 0, st>>>(sb.keys(), W, d_flag);
+  CK0(cudaGetLastError());
+  CK0(scan_exclusive_u32(d_flag, d_rid, (size_t)W, st, nullptr));
+  CK0(cudaMemcpyAsync(&last[0], d_rid + W - 1, 4, cudaMemcpyDeviceToHost, st));
+  CK0(cudaMemcpyAsync(&last[1], d_flag + W - 1, 4, cudaMemcpyDeviceToHost, st));
+  CK0(cudaStreamSynchronize(st));
+  const long long nu = (long long)last[0] + last[1];
+  uint32_t* d_start = nullptr;
+  CK0(tmp.alloc(&d_start, (size_t)nu));
+  CK0(keep.alloc(&out->doc, (size_t)nu));
+  CK0(keep.alloc(&out->idx, (size_t)nu));
+  CK0(keep.alloc(&out->cnt, (size_t)nu));
+  tx_head_kernel<<<nblk(W, 256), 256, 0, st>>>(sb.keys(), d_flag, d_rid, W, d_start);
+  tx_entry_kernel<<<nblk(nu, 256), 256, 0, st>>>(sb.keys(), d_start, nu, W, fbits, out->doc, out->idx, out->cnt);
+  CK0(cudaGetLastError());
+  out->n = nu;
+  s.entries += nu;
+  return PIO_ALS_OK;
+}
+
+// device time of a call: one event pair on the model's stream
+struct TxTimer {
+  cudaEvent_t ev[2] = {nullptr, nullptr};
+  ~TxTimer() {
+    if (ev[0]) cudaEventDestroy(ev[0]);
+    if (ev[1]) cudaEventDestroy(ev[1]);
+  }
+  int start(cudaStream_t st) {
+    CK0(cudaEventCreate(&ev[0]));
+    CK0(cudaEventCreate(&ev[1]));
+    CK0(cudaEventRecord(ev[0], st));
+    return PIO_ALS_OK;
+  }
+  int stop(cudaStream_t st) {
+    CK0(cudaEventRecord(ev[1], st));
+    CK0(cudaEventSynchronize(ev[1]));
+    float ms = 0.f;
+    CK0(cudaEventElapsedTime(&ms, ev[0], ev[1]));
+    g_tx_stats.device_ms = ms;
+    return PIO_ALS_OK;
+  }
+};
+
+static int text_train(pio_text_model* m, const uint8_t* tok_bytes, const int64_t* tok_off, int32_t n,
+                      const int32_t* label, int32_t n_class, double lambda, int64_t* out_df, double* out_idf,
+                      double* out_pi, double* out_theta) {
+  EVF(tx_check_tokens(tok_bytes, tok_off, n));
+  if (n < 1) return fail(nullptr, PIO_ALS_ERR_ARG, "training needs at least one document");
+  if (n_class < 1) return fail(nullptr, PIO_ALS_ERR_ARG, "n_class must be >= 1");
+  if (!(lambda >= 0.0)) return fail(nullptr, PIO_ALS_ERR_ARG, "lambda must be >= 0 (got %g)", lambda);
+  if (!label || !out_df || !out_idf || !out_pi || !out_theta) return fail(nullptr, PIO_ALS_ERR_ARG, "null argument");
+  std::vector<long long> n_c((size_t)n_class, 0);
+  for (int d = 0; d < n; ++d) {
+    if (label[d] < 0 || label[d] >= n_class)
+      return fail(nullptr, PIO_ALS_ERR_ARG, "label %d of document %d is not in [0, %d)", label[d], d, n_class);
+    ++n_c[label[d]];
+  }
+  const long long D = m->num_features, CD = (long long)n_class * D;
+  const std::vector<TextPart> parts = tx_plan(tok_off, n);
+  CK0(cudaSetDevice(m->device));
+  cudaStream_t st = m->st;
+  TxTimer timer;
+  EVF(timer.start(st));
+  Scratch keep(st);
+  unsigned long long* d_df = nullptr;
+  CK0(keep.alloc(&d_df, (size_t)D));
+  CK0(cudaMemsetAsync(d_df, 0, sizeof(unsigned long long) * (size_t)D, st));
+  std::vector<TxEntries> ents(parts.size());
+  std::vector<int*> labs(parts.size(), nullptr);
+  long long total = 0;
+  for (size_t k = 0; k < parts.size(); ++k) {
+    const TextPart& p = parts[k];
+    EVF(tx_part(m, keep, tok_bytes, tok_off, p, &ents[k]));
+    CK0(keep.alloc(&labs[k], (size_t)(p.d1 - p.d0)));
+    CK0(cudaMemcpyAsync(labs[k], label + p.d0, sizeof(int) * (size_t)(p.d1 - p.d0), cudaMemcpyHostToDevice, st));
+    if (ents[k].n) tx_df_kernel<<<nblk(ents[k].n, 256), 256, 0, st>>>(ents[k].idx, ents[k].n, d_df);
+    CK0(cudaGetLastError());
+    total += ents[k].n;
+  }
+  if (total >= (1ll << 33))
+    return fail(nullptr, PIO_ALS_ERR_NUMERIC, "%lld (document, feature) entries: the exact class sums hold fewer "
+                "than 2^33", total);
+  CK0(cudaMemcpyAsync(out_df, d_df, sizeof(int64_t) * (size_t)D, cudaMemcpyDeviceToHost, st));
+  CK0(cudaStreamSynchronize(st));
+  // IDF.fit with minDocFreq 0: log((m + 1) / (df + 1)), the division first
+  for (long long j = 0; j < D; ++j) out_idf[j] = log(((double)n + 1.0) / ((double)out_df[j] + 1.0));
+  double* d_idf = nullptr;
+  unsigned long long* d_acc = nullptr;
+  double* d_s = nullptr;
+  int* d_bad = nullptr;
+  CK0(keep.alloc(&d_idf, (size_t)D));
+  CK0(keep.alloc(&d_acc, (size_t)CD * 3));
+  CK0(keep.alloc(&d_s, (size_t)CD));
+  CK0(keep.alloc(&d_bad, 1));
+  CK0(cudaMemcpyAsync(d_idf, out_idf, sizeof(double) * (size_t)D, cudaMemcpyHostToDevice, st));
+  CK0(cudaMemsetAsync(d_acc, 0, sizeof(unsigned long long) * 3 * (size_t)CD, st));
+  CK0(cudaMemsetAsync(d_bad, 0, sizeof(int), st));
+  for (size_t k = 0; k < parts.size(); ++k) {
+    if (!ents[k].n) continue;
+    // the class of each entry, from its document's label
+    tx_label_kernel<<<nblk(ents[k].n, 256), 256, 0, st>>>(ents[k].doc, labs[k], ents[k].n, (int*)ents[k].doc);
+    tx_sum_kernel<<<nblk(ents[k].n, 256), 256, 0, st>>>(ents[k].idx, ents[k].cnt, (const int*)ents[k].doc, d_idf,
+                                                        ents[k].n, D, d_acc, d_bad);
+    CK0(cudaGetLastError());
+  }
+  tx_round_kernel<<<nblk(CD, 256), 256, 0, st>>>(d_acc, CD, d_s);
+  CK0(cudaGetLastError());
+  int bad = 0;
+  CK0(cudaMemcpyAsync(&bad, d_bad, sizeof(int), cudaMemcpyDeviceToHost, st));
+  CK0(cudaMemcpyAsync(out_theta, d_s, sizeof(double) * (size_t)CD, cudaMemcpyDeviceToHost, st));
+  EVF(timer.stop(st));
+  if (bad)
+    return fail(nullptr, PIO_ALS_ERR_NUMERIC, "a TF-IDF value is outside [2^-44, 2^63): the exact class sums cannot "
+                "hold it");
+  // multinomial NaiveBayes: pi_c = log(n_c + l) - log(N + C l); theta_cj = log(s_cj + l) - log(sum_j s_cj + D l)
+  const double logden = log((double)n + n_class * lambda);
+  for (int c = 0; c < n_class; ++c) {
+    out_pi[c] = log((double)n_c[c] + lambda) - logden;
+    double* row = out_theta + (long long)c * D;
+    double tot = 0.0;
+    for (long long j = 0; j < D; ++j) tot += row[j];
+    const double lt = log(tot + (double)D * lambda);
+    for (long long j = 0; j < D; ++j) row[j] = log(row[j] + lambda) - lt;
+  }
+  return PIO_ALS_OK;
+}
+
+// the entries of every part of a batch, with their values (tf, or tf * idf), handed to `each` part by part
+template <class Each>
+static int tx_batch(pio_text_model* m, const uint8_t* tok_bytes, const int64_t* tok_off, int32_t n, bool use_idf,
+                    Each each) {
+  const std::vector<TextPart> parts = tx_plan(tok_off, n);
+  cudaStream_t st = m->st;
+  TxTimer timer;
+  EVF(timer.start(st));
+  for (const TextPart& p : parts) {
+    Scratch keep(st);
+    TxEntries e;
+    EVF(tx_part(m, keep, tok_bytes, tok_off, p, &e));
+    double* d_val = nullptr;
+    CK0(keep.alloc(&d_val, (size_t)e.n));
+    if (e.n) tx_value_kernel<<<nblk(e.n, 256), 256, 0, st>>>(e.idx, e.cnt, use_idf ? m->d_idf : nullptr, e.n, d_val);
+    CK0(cudaGetLastError());
+    EVF(each(p, e, d_val, keep));
+  }
+  return timer.stop(st);
+}
+
+static int text_features(pio_text_model* m, const uint8_t* tok_bytes, const int64_t* tok_off, int32_t n,
+                         int32_t use_idf, int64_t* out_nnz) {
+  m->has_features = false;
+  std::vector<int64_t>().swap(m->f_ptr);
+  std::vector<int32_t>().swap(m->f_idx);
+  std::vector<double>().swap(m->f_val);
+  EVF(tx_check_tokens(tok_bytes, tok_off, n));
+  if (!out_nnz) return fail(nullptr, PIO_ALS_ERR_ARG, "null argument");
+  if (use_idf && !m->d_idf) return fail(nullptr, PIO_ALS_ERR_STATE, "no idf: the model has not been set");
+  std::vector<int64_t> ptr((size_t)n + 1, 0);
+  std::vector<int32_t> idx;
+  std::vector<double> val;
+  if (n > 0) {
+    CK0(cudaSetDevice(m->device));
+    std::vector<uint32_t> doc;
+    EVF(tx_batch(m, tok_bytes, tok_off, n, use_idf != 0, [&](const TextPart& p, const TxEntries& e, double* d_val,
+                                                              Scratch&) -> int {
+      const size_t at = idx.size();
+      doc.resize((size_t)e.n);
+      idx.resize(at + (size_t)e.n);
+      val.resize(at + (size_t)e.n);
+      if (e.n) {
+        CK0(cudaMemcpyAsync(doc.data(), e.doc, 4 * (size_t)e.n, cudaMemcpyDeviceToHost, m->st));
+        CK0(cudaMemcpyAsync(idx.data() + at, e.idx, 4 * (size_t)e.n, cudaMemcpyDeviceToHost, m->st));
+        CK0(cudaMemcpyAsync(val.data() + at, d_val, 8 * (size_t)e.n, cudaMemcpyDeviceToHost, m->st));
+      }
+      CK0(cudaStreamSynchronize(m->st));
+      for (long long u = 0; u < e.n; ++u) ++ptr[(size_t)p.d0 + doc[u] + 1];
+      return PIO_ALS_OK;
+    }));
+    for (int d = 0; d < n; ++d) ptr[d + 1] += ptr[d];
+  }
+  *out_nnz = (int64_t)idx.size();
+  m->f_ptr.swap(ptr), m->f_idx.swap(idx), m->f_val.swap(val);
+  m->has_features = true;
+  return PIO_ALS_OK;
+}
+
+static int text_scores(pio_text_model* m, const uint8_t* tok_bytes, const int64_t* tok_off, int32_t n,
+                       double* out_scores) {
+  EVF(tx_check_tokens(tok_bytes, tok_off, n));
+  if (!out_scores && n > 0) return fail(nullptr, PIO_ALS_ERR_ARG, "null argument");
+  if (!m->d_theta) return fail(nullptr, PIO_ALS_ERR_STATE, "no model: pio_text_model_set has not been called");
+  if (n == 0) return PIO_ALS_OK;
+  CK0(cudaSetDevice(m->device));
+  const int C = m->n_class;
+  return tx_batch(m, tok_bytes, tok_off, n, true, [&](const TextPart& p, const TxEntries& e, double* d_val,
+                                                      Scratch& keep) -> int {
+    const int nq = p.d1 - p.d0;
+    double* d_out = nullptr;
+    CK0(keep.alloc(&d_out, (size_t)nq * C));
+    tx_score_kernel<<<nblk((long long)nq * C, 256), 256, 0, m->st>>>(e.doc, e.idx, d_val, e.n, nq, C,
+                                                                     m->num_features, m->d_theta, m->d_pi,
+                                                                     m->d_nonfinite, d_out);
+    CK0(cudaGetLastError());
+    CK0(cudaMemcpyAsync(out_scores + (long long)p.d0 * C, d_out, sizeof(double) * (size_t)nq * C,
+                        cudaMemcpyDeviceToHost, m->st));
+    CK0(cudaStreamSynchronize(m->st));
+    return PIO_ALS_OK;
+  });
+}
+
+static void tx_free_model(pio_text_model* m) {
+  for (void* p : {(void*)m->d_idf, (void*)m->d_pi, (void*)m->d_theta, (void*)m->d_nonfinite})
+    if (p) cudaFree(p);
+  m->d_idf = m->d_pi = m->d_theta = nullptr;
+  m->d_nonfinite = nullptr;
+  m->n_class = 0;
+}
+
+}  // namespace pio
+
+extern "C" {
+
+int pio_text_model_create(int device, const uint8_t* stop_bytes, const int64_t* stop_off, int32_t n_stop,
+                          int32_t n_gram, int32_t num_features, pio_text_model** out) {
+  if (!out) return fail(nullptr, PIO_ALS_ERR_ARG, "null argument");
+  *out = nullptr;
+  if (n_gram < 1) return fail(nullptr, PIO_ALS_ERR_ARG, "nGram must be >= 1 (got %d)", n_gram);
+  if (num_features < 1) return fail(nullptr, PIO_ALS_ERR_ARG, "numFeatures must be >= 1 (got %d)", num_features);
+  if (n_stop < 0 || (n_stop > 0 && (!stop_off || !stop_bytes)))
+    return fail(nullptr, PIO_ALS_ERR_ARG, "bad stop words");
+  for (int w = 0; w < n_stop; ++w)
+    if (stop_off[w + 1] < stop_off[w] || stop_off[w] < 0)
+      return fail(nullptr, PIO_ALS_ERR_ARG, "stop_off decreases at word %d", w);
+  std::unique_ptr<pio_text_model> m;
+  try {   // bad_alloc must not cross the C boundary
+    m.reset(new pio_text_model);
+    m->device = device, m->n_gram = n_gram, m->num_features = num_features;
+    // the stop words, de-duplicated, in an open-addressing set at most half full
+    std::vector<long long> off{0};
+    std::vector<uint8_t> bytes;
+    size_t slots = 2;
+    while (slots < 2 * (size_t)n_stop) slots <<= 1;
+    std::vector<int> slot(slots, -1);
+    const unsigned mask = (unsigned)(slots - 1);
+    for (int w = 0; w < n_stop; ++w) {
+      const uint8_t* p = stop_bytes + stop_off[w];
+      const long long len = stop_off[w + 1] - stop_off[w];
+      unsigned i = (unsigned)tx_hash(p, len) & mask;
+      bool dup = false;
+      for (; slot[i] >= 0; i = (i + 1) & mask) {
+        const int v = slot[i];
+        if (off[v + 1] - off[v] == len && !memcmp(bytes.data() + off[v], p, (size_t)len)) {
+          dup = true;
+          break;
+        }
+      }
+      if (dup) continue;
+      slot[i] = (int)off.size() - 1;
+      bytes.insert(bytes.end(), p, p + len);
+      off.push_back((long long)bytes.size());
+    }
+    m->n_stop = (int)off.size() - 1, m->stop_mask = mask;
+    CK0(cudaSetDevice(device));
+    CK0(cudaStreamCreateWithFlags(&m->st, cudaStreamNonBlocking));
+    std::unique_ptr<pio_text_model, int (*)(pio_text_model*)> guard(m.release(), pio_text_model_destroy);
+    pio_text_model* g = guard.get();
+    CK0(cudaMalloc((void**)&g->d_slot, sizeof(int) * slots));
+    CK0(cudaMalloc((void**)&g->d_stop, std::max<size_t>(bytes.size(), 1)));
+    CK0(cudaMalloc((void**)&g->d_stop_off, sizeof(long long) * off.size()));
+    CK0(cudaMemcpy(g->d_slot, slot.data(), sizeof(int) * slots, cudaMemcpyHostToDevice));
+    if (!bytes.empty()) CK0(cudaMemcpy(g->d_stop, bytes.data(), bytes.size(), cudaMemcpyHostToDevice));
+    CK0(cudaMemcpy(g->d_stop_off, off.data(), sizeof(long long) * off.size(), cudaMemcpyHostToDevice));
+    *out = guard.release();
+  } catch (const std::bad_alloc&) {
+    return fail(nullptr, PIO_ALS_ERR_NOMEM, "pio_text_model_create: out of host memory");
+  }
+  return PIO_ALS_OK;
+}
+
+int pio_text_model_destroy(pio_text_model* m) {
+  if (!m) return PIO_ALS_OK;
+  cudaSetDevice(m->device);
+  if (m->st) {
+    cudaStreamSynchronize(m->st);
+    cudaStreamDestroy(m->st);
+  }
+  for (void* p : {(void*)m->d_slot, (void*)m->d_stop, (void*)m->d_stop_off})
+    if (p) cudaFree(p);
+  tx_free_model(m);
+  delete m;
+  return PIO_ALS_OK;
+}
+
+int pio_text_model_set(pio_text_model* m, int32_t n_class, const double* idf, const double* pi, const double* theta) {
+  if (!m) return fail(nullptr, PIO_ALS_ERR_ARG, "null text model");
+  if (n_class < 1 || !idf || !pi || !theta) return fail(nullptr, PIO_ALS_ERR_ARG, "bad pio_text_model_set arguments");
+  std::lock_guard<std::mutex> lk(m->mu);
+  try {
+    const long long D = m->num_features, CD = (long long)n_class * D;
+    std::vector<int> nonfinite((size_t)n_class, 0);   // per class: the entries of theta that are not finite
+    for (long long t = 0; t < CD; ++t) nonfinite[t / D] += !std::isfinite(theta[t]);
+    CK0(cudaSetDevice(m->device));
+    tx_free_model(m);
+    CK0(cudaMalloc((void**)&m->d_idf, sizeof(double) * (size_t)D));
+    CK0(cudaMalloc((void**)&m->d_pi, sizeof(double) * (size_t)n_class));
+    CK0(cudaMalloc((void**)&m->d_theta, sizeof(double) * (size_t)CD));
+    CK0(cudaMalloc((void**)&m->d_nonfinite, sizeof(int) * (size_t)n_class));
+    CK0(cudaMemcpy(m->d_idf, idf, sizeof(double) * (size_t)D, cudaMemcpyHostToDevice));
+    CK0(cudaMemcpy(m->d_pi, pi, sizeof(double) * (size_t)n_class, cudaMemcpyHostToDevice));
+    CK0(cudaMemcpy(m->d_theta, theta, sizeof(double) * (size_t)CD, cudaMemcpyHostToDevice));
+    CK0(cudaMemcpy(m->d_nonfinite, nonfinite.data(), sizeof(int) * (size_t)n_class, cudaMemcpyHostToDevice));
+    m->n_class = n_class;
+  } catch (const std::bad_alloc&) {
+    return fail(nullptr, PIO_ALS_ERR_NOMEM, "pio_text_model_set: out of host memory");
+  }
+  return PIO_ALS_OK;
+}
+
+int pio_text_train_nb(pio_text_model* m, const uint8_t* tok_bytes, const int64_t* tok_off, int32_t n_docs,
+                      const int32_t* label, int32_t n_class, double lambda, int64_t* out_df, double* out_idf,
+                      double* out_pi, double* out_theta) {
+  g_tx_stats = TextStats{};
+  if (!m) return fail(nullptr, PIO_ALS_ERR_ARG, "null text model");
+  std::lock_guard<std::mutex> lk(m->mu);
+  try {   // Scratch releases device memory on the way out
+    return text_train(m, tok_bytes, tok_off, n_docs, label, n_class, lambda, out_df, out_idf, out_pi, out_theta);
+  } catch (const std::bad_alloc&) {
+    return fail(nullptr, PIO_ALS_ERR_NOMEM, "pio_text_train_nb: out of host memory");
+  }
+}
+
+int pio_text_features(pio_text_model* m, const uint8_t* tok_bytes, const int64_t* tok_off, int32_t n_docs,
+                      int32_t use_idf, int64_t* out_nnz) {
+  g_tx_stats = TextStats{};
+  if (!m) return fail(nullptr, PIO_ALS_ERR_ARG, "null text model");
+  std::lock_guard<std::mutex> lk(m->mu);
+  try {
+    return text_features(m, tok_bytes, tok_off, n_docs, use_idf, out_nnz);
+  } catch (const std::bad_alloc&) {
+    return fail(nullptr, PIO_ALS_ERR_NOMEM, "pio_text_features: out of host memory");
+  }
+}
+
+int pio_text_features_get(pio_text_model* m, int64_t* doc_ptr, int32_t* index, double* value) {
+  if (!m) return fail(nullptr, PIO_ALS_ERR_ARG, "null text model");
+  std::lock_guard<std::mutex> lk(m->mu);
+  if (!m->has_features) return fail(nullptr, PIO_ALS_ERR_STATE, "no pio_text_features result to get");
+  auto put = [](auto* dst, auto& v) {
+    if (dst && !v.empty()) memcpy(dst, v.data(), v.size() * sizeof(v[0]));
+    std::remove_reference_t<decltype(v)>().swap(v);
+  };
+  put(doc_ptr, m->f_ptr);
+  put(index, m->f_idx);
+  put(value, m->f_val);
+  m->has_features = false;
+  return PIO_ALS_OK;
+}
+
+int pio_text_scores(pio_text_model* m, const uint8_t* tok_bytes, const int64_t* tok_off, int32_t n_docs,
+                    double* out_scores) {
+  g_tx_stats = TextStats{};
+  if (!m) return fail(nullptr, PIO_ALS_ERR_ARG, "null text model");
+  std::lock_guard<std::mutex> lk(m->mu);
+  try {
+    return text_scores(m, tok_bytes, tok_off, n_docs, out_scores);
+  } catch (const std::bad_alloc&) {
+    return fail(nullptr, PIO_ALS_ERR_NOMEM, "pio_text_scores: out of host memory");
+  }
+}
+
+int pio_text_debug_stats(double out[7]) {
+  if (!out) return PIO_ALS_ERR_ARG;
+  const TextStats& s = g_tx_stats;
+  out[0] = (double)s.parts, out[1] = (double)s.docs, out[2] = (double)s.windows, out[3] = (double)s.entries;
+  out[4] = (double)s.max_part_bytes, out[5] = (double)s.budget, out[6] = s.device_ms;
   return PIO_ALS_OK;
 }
 

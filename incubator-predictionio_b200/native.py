@@ -8,6 +8,7 @@ call raises ``NativeError``.
 from __future__ import annotations
 
 import ctypes as C
+import json
 import os
 import subprocess
 from dataclasses import dataclass, field
@@ -50,7 +51,9 @@ EXPORTED_SYMBOLS = [
     "pio_assoc_model_size", "pio_assoc_model_get", "pio_assoc_model_destroy", "pio_rf_train_regressor",
     "pio_rf_forest_reg_size", "pio_rf_forest_reg_get", "pio_rf_predict_regression", "pio_lead_sessions",
     "pio_als_rank_lists", "pio_rank_lists_debug_stats", "pio_assoc_index_create", "pio_assoc_index_destroy",
-    "pio_assoc_predict", "pio_assoc_predict_get", "pio_assoc_predict_debug_stats",
+    "pio_assoc_predict", "pio_assoc_predict_get", "pio_assoc_predict_debug_stats", "pio_text_model_create",
+    "pio_text_model_destroy", "pio_text_model_set", "pio_text_train_nb", "pio_text_features", "pio_text_features_get",
+    "pio_text_scores", "pio_text_debug_stats",
 ]
 
 
@@ -220,6 +223,19 @@ def lib():
         L.pio_assoc_predict.argtypes = [vp, C.c_int32, vp, vp, C.c_int32, vp, vp, vp]
         L.pio_assoc_predict_get.restype = ci
         L.pio_assoc_predict_get.argtypes = [vp, vp, vp, vp, vp, vp]
+        L.pio_text_model_create.restype = ci
+        L.pio_text_model_create.argtypes = [ci, vp, vp, C.c_int32, C.c_int32, C.c_int32, vp]
+        L.pio_text_model_destroy.argtypes = [vp]
+        L.pio_text_model_set.restype = ci
+        L.pio_text_model_set.argtypes = [vp, C.c_int32, vp, vp, vp]
+        L.pio_text_train_nb.restype = ci
+        L.pio_text_train_nb.argtypes = [vp, vp, vp, C.c_int32, vp, C.c_int32, C.c_double, vp, vp, vp, vp]
+        L.pio_text_features.restype = ci
+        L.pio_text_features.argtypes = [vp, vp, vp, C.c_int32, C.c_int32, vp]
+        L.pio_text_features_get.restype = ci
+        L.pio_text_features_get.argtypes = [vp, vp, vp, vp]
+        L.pio_text_scores.restype = ci
+        L.pio_text_scores.argtypes = [vp, vp, vp, C.c_int32, vp]
         for name in EXPORTED_SYMBOLS:
             getattr(L, name)  # AttributeError if the ABI is incomplete
         _lib = L
@@ -1525,3 +1541,92 @@ def nb_predict(x, pi, theta, device=0):
     _check(lib().pio_nb_predict(C.c_int(device), _ptr(x, C.c_float), C.c_int64(n), C.c_int(f), C.c_int(pi.shape[0]),
                                 _ptr(pi, C.c_double), _ptr(theta, C.c_double), _ptr(out, C.c_int32)))
     return out
+
+
+def text_tokens(texts):
+    """The raw JSON string tokens of a batch of Python strings, as the text calls take them: (bytes uint8, offsets
+    int64 [n + 1]).  json.dumps writes an unpaired surrogate as a \\u escape, which the device decodes to '?'."""
+    return _str_column([json.dumps(t).encode("ascii") for t in texts])
+
+
+class TextModel:
+    """pio_text_model: the featurizer of PreparatorParams(nGram, numFeatures) with its stop words on `device`, and,
+    once set, a Naive Bayes model (idf, pi, theta) that scores batches.  Documents go in as raw JSON string tokens
+    (tok_bytes, tok_off), as the keyed event scan returns them or text_tokens makes them."""
+
+    def __init__(self, stop_words, n_gram: int, num_features: int, device: int = 0):
+        words = [w.encode("utf-8", "replace") if isinstance(w, str) else bytes(w) for w in stop_words]
+        sb, so = _str_column(words)
+        self.n_gram, self.num_features, self.device = int(n_gram), int(num_features), int(device)
+        self.n_class = 0
+        self._h = C.c_void_p()
+        _check(lib().pio_text_model_create(self.device, sb.ctypes.data if sb.size else None, so.ctypes.data,
+                                           len(words), self.n_gram, self.num_features, C.addressof(self._h)))
+
+    def close(self):
+        if self._h:
+            lib().pio_text_model_destroy(self._h)
+            self._h = C.c_void_p()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    @staticmethod
+    def _tokens(tok_bytes, tok_off):
+        b = np.ascontiguousarray(tok_bytes, np.uint8)
+        o = np.ascontiguousarray(tok_off, np.int64)
+        if o.ndim != 1 or o.shape[0] < 1 or (o.shape[0] > 1 and int(o[-1]) > b.shape[0]):
+            raise ValueError("tok_off must be [n + 1] offsets into tok_bytes")
+        return b, o, int(o.shape[0] - 1)
+
+    def set_model(self, idf, pi, theta):
+        idf = np.ascontiguousarray(idf, np.float64)
+        pi = np.ascontiguousarray(pi, np.float64)
+        theta = np.ascontiguousarray(theta, np.float64)
+        c = pi.shape[0]
+        if idf.shape != (self.num_features,) or theta.shape != (c, self.num_features):
+            raise ValueError("idf must be [numFeatures], pi [C] and theta [C, numFeatures]")
+        _check(lib().pio_text_model_set(self._h, c, idf.ctypes.data, pi.ctypes.data, theta.ctypes.data))
+        self.n_class = c
+
+    def train_nb(self, tok_bytes, tok_off, label, n_class: int, lam: float):
+        """pio_text_train_nb: (df int64 [D], idf [D], pi [C], theta [C, D])."""
+        b, o, n = self._tokens(tok_bytes, tok_off)
+        label = np.ascontiguousarray(label, np.int32)
+        if label.shape != (n,):
+            raise ValueError("one label per document")
+        D = self.num_features
+        df, idf = np.empty(D, np.int64), np.empty(D, np.float64)
+        pi, theta = np.empty(max(int(n_class), 1), np.float64), np.empty((max(int(n_class), 1), D), np.float64)
+        _check(lib().pio_text_train_nb(self._h, b.ctypes.data, o.ctypes.data, n, label.ctypes.data, int(n_class),
+                                       float(lam), df.ctypes.data, idf.ctypes.data, pi.ctypes.data, theta.ctypes.data))
+        return df, idf, pi, theta
+
+    def features(self, tok_bytes, tok_off, use_idf: bool):
+        """pio_text_features: the TF or TF-IDF COO (doc_ptr int64 [n + 1], index int32, value float64)."""
+        b, o, n = self._tokens(tok_bytes, tok_off)
+        nnz = C.c_int64(0)
+        _check(lib().pio_text_features(self._h, b.ctypes.data, o.ctypes.data, n, int(bool(use_idf)),
+                                       C.addressof(nnz)))
+        out = (np.zeros(n + 1, np.int64), np.empty(nnz.value, np.int32), np.empty(nnz.value, np.float64))
+        _check(lib().pio_text_features_get(self._h, *[a.ctypes.data for a in out]))
+        return out
+
+    def scores(self, tok_bytes, tok_off):
+        """pio_text_scores: the raw scores [n, C] (innerProduct(theta_c, x) + pi_c)."""
+        b, o, n = self._tokens(tok_bytes, tok_off)
+        out = np.empty((n, max(self.n_class, 1)), np.float64)
+        _check(lib().pio_text_scores(self._h, b.ctypes.data, o.ctypes.data, n, out.ctypes.data))
+        return out[:, :self.n_class]
+
+
+def text_stats() -> dict:
+    """What the last TextModel call on this thread did: its parts, documents, n-gram windows, (document, feature)
+    entries, the most token bytes in one part, the budget and the device milliseconds."""
+    out = (C.c_double * 7)()
+    _check(lib().pio_text_debug_stats(out))
+    return {"parts": int(out[0]), "docs": int(out[1]), "windows": int(out[2]), "entries": int(out[3]),
+            "max_part_bytes": int(out[4]), "budget": int(out[5]), "device_ms": out[6]}
