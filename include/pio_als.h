@@ -41,6 +41,8 @@
  *       examples/scala-parallel-classification/add-algorithm/src/main/scala/{DataSource.scala readEval, Evaluation.scala}
  *   pio_assoc_train / pio_assoc_model_* replace the complementary purchase template's Algorithm.train
  *       docs/manual/source/templates/complementarypurchase/dase.html.md.erb:293-314
+ *   pio_text_folds_* run the text classification template's k-fold evaluation
+ *       docs/manual/source/demo/textclassification.html.md.erb (readEval, Accuracy, EngineParamsList)
  */
 #ifndef PIO_ALS_H_
 #define PIO_ALS_H_
@@ -904,6 +906,38 @@ PIO_API int pio_text_scores(pio_text_model* m, const uint8_t* tok_bytes, const i
  * windows, [3] (document, feature) entries, [4] most token bytes in one part, [5] the budget, [6] device
  * milliseconds. */
 PIO_API int pio_text_debug_stats(double out[7]);
+
+/* k-fold evaluation of the text classification template on the device (DESIGN.md 4.18.1): its `pio eval` with the
+ * documents featurized once per (nGram, numFeatures) and each fold's model trained and its test documents scored from
+ * the resident (document, feature) entries.  Document d is in the test set of fold d % k_fold and in the training set
+ * of every other fold, in document order.  A fold's model equals pio_text_train_nb's on the fold's training documents
+ * byte for byte, and its scores equal pio_text_scores' of its test documents.  HOST buffers.  Errors: status codes as
+ * above, text via pio_als_last_error(NULL); arguments are checked before any device work. */
+typedef struct pio_text_folds pio_text_folds;
+/* n_docs >= 1 documents as raw JSON string tokens (checked as pio_text_train_nb checks them; copied), the stop words as
+ * pio_text_model_create takes them, k_fold >= 1. */
+PIO_API int pio_text_folds_create(int device, const uint8_t* stop_bytes, const int64_t* stop_off, int32_t n_stop,
+                                  const uint8_t* tok_bytes, const int64_t* tok_off, int32_t n_docs, int32_t k_fold,
+                                  pio_text_folds** out);
+PIO_API int pio_text_folds_destroy(pio_text_folds* f);
+/* Featurizes every document with PreparatorParams(n_gram, num_features) and keeps the entries (12 bytes each) on the
+ * device until the next featurization; a no-op when the pair is the current one.  PIO_ALS_ERR_NUMERIC at 2^32 entries
+ * or more. */
+PIO_API int pio_text_folds_featurize(pio_text_folds* f, int32_t n_gram, int32_t num_features);
+/* out[0] training documents, out[1] test documents of fold `fold`. */
+PIO_API int pio_text_folds_sizes(const pio_text_folds* f, int32_t fold, int64_t out[2]);
+/* pio_text_train_nb on the fold's training documents under the current featurization: cls_doc [n_docs] holds each
+ * document's class in [0, n_class) (the index of its label among the fold's training labels; test documents' entries
+ * are ignored).  Out as pio_text_train_nb's, with its errors. */
+PIO_API int pio_text_folds_train_nb(pio_text_folds* f, int32_t fold, const int32_t* cls_doc, int32_t n_class,
+                                    double lambda, int64_t* out_df, double* out_idf, double* out_pi, double* out_theta);
+/* pio_text_scores of the fold's test documents, in document order, under the model idf [numFeatures], pi [n_class],
+ * theta [n_class x numFeatures]: out_scores [out[1] of pio_text_folds_sizes x n_class]. */
+PIO_API int pio_text_folds_scores(pio_text_folds* f, int32_t fold, int32_t n_class, const double* idf,
+                                  const double* pi, const double* theta, double* out_scores);
+/* out[0] featurizations done, [1] entries of the current one, [2] its parts, device milliseconds of [3] the
+ * featurizations, [4] the trainings and [5] the scorings, over the object's life. */
+PIO_API int pio_text_folds_debug_stats(const pio_text_folds* f, double out[6]);
 
 #ifdef __cplusplus
 }

@@ -8346,49 +8346,62 @@ struct TxTimer {
   }
 };
 
-static int text_train(pio_text_model* m, const uint8_t* tok_bytes, const int64_t* tok_off, int32_t n,
-                      const int32_t* label, int32_t n_class, double lambda, int64_t* out_df, double* out_idf,
-                      double* out_pi, double* out_theta) {
-  EVF(tx_check_tokens(tok_bytes, tok_off, n));
-  if (n < 1) return fail(nullptr, PIO_ALS_ERR_ARG, "training needs at least one document");
-  if (n_class < 1) return fail(nullptr, PIO_ALS_ERR_ARG, "n_class must be >= 1");
-  if (!(lambda >= 0.0)) return fail(nullptr, PIO_ALS_ERR_ARG, "lambda must be >= 0 (got %g)", lambda);
-  if (!label || !out_df || !out_idf || !out_pi || !out_theta) return fail(nullptr, PIO_ALS_ERR_ARG, "null argument");
-  std::vector<long long> n_c((size_t)n_class, 0);
-  for (int d = 0; d < n; ++d) {
-    if (label[d] < 0 || label[d] >= n_class)
-      return fail(nullptr, PIO_ALS_ERR_ARG, "label %d of document %d is not in [0, %d)", label[d], d, n_class);
-    ++n_c[label[d]];
+// One list of training entries: feature index, term count and class per entry (any order).
+struct TxTrainList {
+  const uint32_t *idx = nullptr, *cnt = nullptr;
+  const int* cls = nullptr;
+  long long n = 0;
+};
+
+// IDF.fit with minDocFreq 0 over m documents: log((m + 1) / (df + 1)), the division first
+static void tx_idf(long long m, const int64_t* df, long long D, double* idf) {
+  for (long long j = 0; j < D; ++j) idf[j] = log(((double)m + 1.0) / ((double)df[j] + 1.0));
+}
+
+// multinomial NaiveBayes from the rounded class sums s (in theta, overwritten) of m documents, n_c of class c:
+// pi_c = log(n_c + l) - log(m + C l); theta_cj = log(s_cj + l) - log(sum_j s_cj + D l), the sum in j order
+static void tx_nb_logs(long long m, const std::vector<long long>& n_c, double lambda, long long D, double* pi,
+                       double* theta) {
+  const int n_class = (int)n_c.size();
+  const double logden = log((double)m + n_class * lambda);
+  for (int c = 0; c < n_class; ++c) {
+    pi[c] = log((double)n_c[c] + lambda) - logden;
+    double* row = theta + (long long)c * D;
+    double tot = 0.0;
+    for (long long j = 0; j < D; ++j) tot += row[j];
+    const double lt = log(tot + (double)D * lambda);
+    for (long long j = 0; j < D; ++j) row[j] = log(row[j] + lambda) - lt;
   }
-  const long long D = m->num_features, CD = (long long)n_class * D;
-  const std::vector<TextPart> parts = tx_plan(tok_off, n);
-  CK0(cudaSetDevice(m->device));
-  cudaStream_t st = m->st;
-  TxTimer timer;
-  EVF(timer.start(st));
-  Scratch keep(st);
+}
+
+// per class: the entries of theta [C x D] that are not finite (tx_score_kernel's NaN rule)
+static std::vector<int> tx_nonfinite(const double* theta, int n_class, long long D) {
+  std::vector<int> nonfinite((size_t)n_class, 0);
+  for (long long t = 0; t < (long long)n_class * D; ++t) nonfinite[t / D] += !std::isfinite(theta[t]);
+  return nonfinite;
+}
+
+// IDF.fit and NaiveBayes.train over the entries of m training documents (n_c per class), with the timer started by the
+// caller: df on the device, idf on the host, the exact class sums on the device, the logarithms on the host.
+static int tx_fit(cudaStream_t st, Scratch& keep, TxTimer& timer, const std::vector<TxTrainList>& lists, long long m,
+                  const std::vector<long long>& n_c, double lambda, long long D, int64_t* out_df, double* out_idf,
+                  double* out_pi, double* out_theta) {
+  const long long CD = (long long)n_c.size() * D;
   unsigned long long* d_df = nullptr;
   CK0(keep.alloc(&d_df, (size_t)D));
   CK0(cudaMemsetAsync(d_df, 0, sizeof(unsigned long long) * (size_t)D, st));
-  std::vector<TxEntries> ents(parts.size());
-  std::vector<int*> labs(parts.size(), nullptr);
   long long total = 0;
-  for (size_t k = 0; k < parts.size(); ++k) {
-    const TextPart& p = parts[k];
-    EVF(tx_part(m, keep, tok_bytes, tok_off, p, &ents[k]));
-    CK0(keep.alloc(&labs[k], (size_t)(p.d1 - p.d0)));
-    CK0(cudaMemcpyAsync(labs[k], label + p.d0, sizeof(int) * (size_t)(p.d1 - p.d0), cudaMemcpyHostToDevice, st));
-    if (ents[k].n) tx_df_kernel<<<nblk(ents[k].n, 256), 256, 0, st>>>(ents[k].idx, ents[k].n, d_df);
+  for (const TxTrainList& l : lists) {
+    if (l.n) tx_df_kernel<<<nblk(l.n, 256), 256, 0, st>>>(l.idx, l.n, d_df);
     CK0(cudaGetLastError());
-    total += ents[k].n;
+    total += l.n;
   }
   if (total >= (1ll << 33))
     return fail(nullptr, PIO_ALS_ERR_NUMERIC, "%lld (document, feature) entries: the exact class sums hold fewer "
                 "than 2^33", total);
   CK0(cudaMemcpyAsync(out_df, d_df, sizeof(int64_t) * (size_t)D, cudaMemcpyDeviceToHost, st));
   CK0(cudaStreamSynchronize(st));
-  // IDF.fit with minDocFreq 0: log((m + 1) / (df + 1)), the division first
-  for (long long j = 0; j < D; ++j) out_idf[j] = log(((double)n + 1.0) / ((double)out_df[j] + 1.0));
+  tx_idf(m, out_df, D, out_idf);
   double* d_idf = nullptr;
   unsigned long long* d_acc = nullptr;
   double* d_s = nullptr;
@@ -8400,12 +8413,8 @@ static int text_train(pio_text_model* m, const uint8_t* tok_bytes, const int64_t
   CK0(cudaMemcpyAsync(d_idf, out_idf, sizeof(double) * (size_t)D, cudaMemcpyHostToDevice, st));
   CK0(cudaMemsetAsync(d_acc, 0, sizeof(unsigned long long) * 3 * (size_t)CD, st));
   CK0(cudaMemsetAsync(d_bad, 0, sizeof(int), st));
-  for (size_t k = 0; k < parts.size(); ++k) {
-    if (!ents[k].n) continue;
-    // the class of each entry, from its document's label
-    tx_label_kernel<<<nblk(ents[k].n, 256), 256, 0, st>>>(ents[k].doc, labs[k], ents[k].n, (int*)ents[k].doc);
-    tx_sum_kernel<<<nblk(ents[k].n, 256), 256, 0, st>>>(ents[k].idx, ents[k].cnt, (const int*)ents[k].doc, d_idf,
-                                                        ents[k].n, D, d_acc, d_bad);
+  for (const TxTrainList& l : lists) {
+    if (l.n) tx_sum_kernel<<<nblk(l.n, 256), 256, 0, st>>>(l.idx, l.cnt, l.cls, d_idf, l.n, D, d_acc, d_bad);
     CK0(cudaGetLastError());
   }
   tx_round_kernel<<<nblk(CD, 256), 256, 0, st>>>(d_acc, CD, d_s);
@@ -8417,17 +8426,49 @@ static int text_train(pio_text_model* m, const uint8_t* tok_bytes, const int64_t
   if (bad)
     return fail(nullptr, PIO_ALS_ERR_NUMERIC, "a TF-IDF value is outside [2^-44, 2^63): the exact class sums cannot "
                 "hold it");
-  // multinomial NaiveBayes: pi_c = log(n_c + l) - log(N + C l); theta_cj = log(s_cj + l) - log(sum_j s_cj + D l)
-  const double logden = log((double)n + n_class * lambda);
-  for (int c = 0; c < n_class; ++c) {
-    out_pi[c] = log((double)n_c[c] + lambda) - logden;
-    double* row = out_theta + (long long)c * D;
-    double tot = 0.0;
-    for (long long j = 0; j < D; ++j) tot += row[j];
-    const double lt = log(tot + (double)D * lambda);
-    for (long long j = 0; j < D; ++j) row[j] = log(row[j] + lambda) - lt;
-  }
+  tx_nb_logs(m, n_c, lambda, D, out_pi, out_theta);
   return PIO_ALS_OK;
+}
+
+static int tx_check_fit(int32_t n_class, double lambda) {
+  if (n_class < 1) return fail(nullptr, PIO_ALS_ERR_ARG, "n_class must be >= 1");
+  if (!(lambda >= 0.0)) return fail(nullptr, PIO_ALS_ERR_ARG, "lambda must be >= 0 (got %g)", lambda);
+  return PIO_ALS_OK;
+}
+
+static int text_train(pio_text_model* m, const uint8_t* tok_bytes, const int64_t* tok_off, int32_t n,
+                      const int32_t* label, int32_t n_class, double lambda, int64_t* out_df, double* out_idf,
+                      double* out_pi, double* out_theta) {
+  EVF(tx_check_tokens(tok_bytes, tok_off, n));
+  if (n < 1) return fail(nullptr, PIO_ALS_ERR_ARG, "training needs at least one document");
+  EVF(tx_check_fit(n_class, lambda));
+  if (!label || !out_df || !out_idf || !out_pi || !out_theta) return fail(nullptr, PIO_ALS_ERR_ARG, "null argument");
+  std::vector<long long> n_c((size_t)n_class, 0);
+  for (int d = 0; d < n; ++d) {
+    if (label[d] < 0 || label[d] >= n_class)
+      return fail(nullptr, PIO_ALS_ERR_ARG, "label %d of document %d is not in [0, %d)", label[d], d, n_class);
+    ++n_c[label[d]];
+  }
+  const std::vector<TextPart> parts = tx_plan(tok_off, n);
+  CK0(cudaSetDevice(m->device));
+  cudaStream_t st = m->st;
+  TxTimer timer;
+  EVF(timer.start(st));
+  Scratch keep(st);
+  std::vector<TxTrainList> lists(parts.size());
+  for (size_t k = 0; k < parts.size(); ++k) {
+    const TextPart& p = parts[k];
+    TxEntries e;
+    int* lab = nullptr;
+    EVF(tx_part(m, keep, tok_bytes, tok_off, p, &e));
+    CK0(keep.alloc(&lab, (size_t)(p.d1 - p.d0)));
+    CK0(cudaMemcpyAsync(lab, label + p.d0, sizeof(int) * (size_t)(p.d1 - p.d0), cudaMemcpyHostToDevice, st));
+    // the class of each entry, from its document's label, in place of its document
+    if (e.n) tx_label_kernel<<<nblk(e.n, 256), 256, 0, st>>>(e.doc, lab, e.n, (int*)e.doc);
+    CK0(cudaGetLastError());
+    lists[k] = TxTrainList{e.idx, e.cnt, (const int*)e.doc, e.n};
+  }
+  return tx_fit(st, keep, timer, lists, n, n_c, lambda, m->num_features, out_df, out_idf, out_pi, out_theta);
 }
 
 // the entries of every part of a batch, with their values (tf, or tf * idf), handed to `each` part by part
@@ -8602,8 +8643,7 @@ int pio_text_model_set(pio_text_model* m, int32_t n_class, const double* idf, co
   std::lock_guard<std::mutex> lk(m->mu);
   try {
     const long long D = m->num_features, CD = (long long)n_class * D;
-    std::vector<int> nonfinite((size_t)n_class, 0);   // per class: the entries of theta that are not finite
-    for (long long t = 0; t < CD; ++t) nonfinite[t / D] += !std::isfinite(theta[t]);
+    const std::vector<int> nonfinite = tx_nonfinite(theta, n_class, D);
     CK0(cudaSetDevice(m->device));
     tx_free_model(m);
     CK0(cudaMalloc((void**)&m->d_idf, sizeof(double) * (size_t)D));
@@ -8678,6 +8718,278 @@ int pio_text_debug_stats(double out[7]) {
   const TextStats& s = g_tx_stats;
   out[0] = (double)s.parts, out[1] = (double)s.docs, out[2] = (double)s.windows, out[3] = (double)s.entries;
   out[4] = (double)s.max_part_bytes, out[5] = (double)s.budget, out[6] = s.device_ms;
+  return PIO_ALS_OK;
+}
+
+}  // extern "C"
+
+// ---- k-fold evaluation of the text classification template (pio_text_folds_*; DESIGN.md 4.18.1) ------------------------
+struct pio_text_folds {
+  int k = 1;
+  int32_t n = 0;                                   // documents; document d tests in fold d % k
+  std::vector<uint8_t> tok_bytes;                  // the documents' raw tokens, offsets from 0
+  std::vector<int64_t> tok_off;
+  pio_text_model* fz = nullptr;                    // the stop words, the stream and the featurizer's parameters
+  // the current featurization: every entry (global document, index, count) in (document, index) order
+  std::unique_ptr<pio::Scratch> ents;
+  uint32_t *doc = nullptr, *idx = nullptr, *cnt = nullptr;
+  long long nu = 0;
+  int n_gram = 0, num_features = 0;                // 0: nothing featurized
+  long long featurizations = 0, parts = 0;
+  double featurize_ms = 0.0, train_ms = 0.0, scores_ms = 0.0;
+};
+
+namespace pio {
+
+static long long tf_n_test(const pio_text_folds* t, int f) { return ((long long)t->n + t->k - 1 - f) / t->k; }
+
+static int tf_fold(const pio_text_folds* t, int32_t fold, const char* what) {
+  if (!t) return fail(nullptr, PIO_ALS_ERR_ARG, "%s: null object", what);
+  if (fold < 0 || fold >= t->k)
+    return fail(nullptr, PIO_ALS_ERR_ARG, "%s: fold %d outside 0..%d", what, fold, t->k - 1);
+  if (!t->n_gram) return fail(nullptr, PIO_ALS_ERR_STATE, "%s: pio_text_folds_featurize has not been called", what);
+  return PIO_ALS_OK;
+}
+
+static int tf_featurize(pio_text_folds* t, int32_t n_gram, int32_t num_features) {
+  if (n_gram < 1) return fail(nullptr, PIO_ALS_ERR_ARG, "nGram must be >= 1 (got %d)", n_gram);
+  if (num_features < 1) return fail(nullptr, PIO_ALS_ERR_ARG, "numFeatures must be >= 1 (got %d)", num_features);
+  if (t->n_gram == n_gram && t->num_features == num_features) return PIO_ALS_OK;
+  pio_text_model* m = t->fz;
+  t->ents.reset();
+  t->doc = t->idx = t->cnt = nullptr;
+  t->nu = 0, t->n_gram = 0, t->num_features = 0;
+  m->n_gram = n_gram, m->num_features = num_features;
+  const std::vector<TextPart> parts = tx_plan(t->tok_off.data(), t->n);
+  CK0(cudaSetDevice(m->device));
+  cudaStream_t st = m->st;
+  TxTimer timer;
+  EVF(timer.start(st));
+  std::unique_ptr<Scratch> keep(new Scratch(st));
+  {
+    Scratch part_mem(st);   // the parts' own entries, released once they are copied into one list
+    std::vector<TxEntries> pe(parts.size());
+    long long total = 0;
+    for (size_t q = 0; q < parts.size(); ++q) {
+      EVF(tx_part(m, part_mem, t->tok_bytes.data(), t->tok_off.data(), parts[q], &pe[q]));
+      total += pe[q].n;
+    }
+    if (total >= (1ll << 32))
+      return fail(nullptr, PIO_ALS_ERR_NUMERIC, "%lld (document, feature) entries: the fold lists hold fewer than "
+                  "2^32", total);
+    CK0(keep->alloc(&t->doc, (size_t)total));
+    CK0(keep->alloc(&t->idx, (size_t)total));
+    CK0(keep->alloc(&t->cnt, (size_t)total));
+    long long at = 0;
+    for (size_t q = 0; q < parts.size(); ++q) {
+      const TxEntries& e = pe[q];
+      if (!e.n) continue;
+      tx_doc_base_kernel<<<nblk(e.n, 256), 256, 0, st>>>(e.doc, e.n, (uint32_t)parts[q].d0, t->doc + at);
+      CK0(cudaGetLastError());
+      CK0(cudaMemcpyAsync(t->idx + at, e.idx, 4 * (size_t)e.n, cudaMemcpyDeviceToDevice, st));
+      CK0(cudaMemcpyAsync(t->cnt + at, e.cnt, 4 * (size_t)e.n, cudaMemcpyDeviceToDevice, st));
+      at += e.n;
+    }
+    t->nu = total;
+  }
+  EVF(timer.stop(st));
+  t->ents = std::move(keep);
+  t->n_gram = n_gram, t->num_features = num_features;
+  t->featurizations += 1, t->parts = (long long)parts.size(), t->featurize_ms += g_tx_stats.device_ms;
+  return PIO_ALS_OK;
+}
+
+// fold f's training (test = false) or test list, cut from the resident entries into `tmp`: key (the document's class
+// cls_doc[d], or the test position (d - f) / k), index and count per entry, in (document, index) order
+static int tf_list(pio_text_folds* t, Scratch& tmp, int f, bool test, const int* d_cls_doc, uint32_t** key,
+                   uint32_t** idx, uint32_t** cnt, long long* n_out) {
+  cudaStream_t st = t->fz->st;
+  const long long nu = t->nu;
+  uint32_t *flag = nullptr, *pos = nullptr;
+  long long n = 0;
+  if (nu) {
+    CK0(tmp.alloc(&flag, (size_t)nu));
+    CK0(tmp.alloc(&pos, (size_t)nu));
+    tx_fold_flag_kernel<<<nblk(nu, 256), 256, 0, st>>>(t->doc, nu, t->k, f, test, flag);
+    CK0(cudaGetLastError());
+    CK0(scan_exclusive_u32(flag, pos, (size_t)nu, st, nullptr));
+    uint32_t last[2] = {0, 0};
+    CK0(cudaMemcpyAsync(&last[0], pos + nu - 1, 4, cudaMemcpyDeviceToHost, st));
+    CK0(cudaMemcpyAsync(&last[1], flag + nu - 1, 4, cudaMemcpyDeviceToHost, st));
+    CK0(cudaStreamSynchronize(st));
+    n = (long long)last[0] + last[1];
+  }
+  CK0(tmp.alloc(key, (size_t)n));
+  CK0(tmp.alloc(idx, (size_t)n));
+  CK0(tmp.alloc(cnt, (size_t)n));
+  if (n) {
+    tx_fold_gather_kernel<<<nblk(nu, 256), 256, 0, st>>>(t->doc, t->idx, t->cnt, pos, nu, t->k, f, test, d_cls_doc,
+                                                         *key, *idx, *cnt);
+    CK0(cudaGetLastError());
+  }
+  *n_out = n;
+  return PIO_ALS_OK;
+}
+
+static int tf_train(pio_text_folds* t, int f, const int32_t* cls_doc, int32_t n_class, double lambda, int64_t* out_df,
+                    double* out_idf, double* out_pi, double* out_theta) {
+  EVF(tx_check_fit(n_class, lambda));
+  if (!cls_doc || !out_df || !out_idf || !out_pi || !out_theta) return fail(nullptr, PIO_ALS_ERR_ARG, "null argument");
+  const long long m = t->n - tf_n_test(t, f);
+  if (m < 1) return fail(nullptr, PIO_ALS_ERR_ARG, "training needs at least one document");
+  std::vector<long long> n_c((size_t)n_class, 0);
+  for (int d = 0; d < t->n; ++d) {
+    if (d % t->k == f) continue;
+    if (cls_doc[d] < 0 || cls_doc[d] >= n_class)
+      return fail(nullptr, PIO_ALS_ERR_ARG, "class %d of document %d is not in [0, %d)", cls_doc[d], d, n_class);
+    ++n_c[cls_doc[d]];
+  }
+  CK0(cudaSetDevice(t->fz->device));
+  cudaStream_t st = t->fz->st;
+  TxTimer timer;
+  EVF(timer.start(st));
+  Scratch tmp(st);
+  int* d_cls_doc = nullptr;
+  CK0(tmp.alloc(&d_cls_doc, (size_t)t->n));
+  CK0(cudaMemcpyAsync(d_cls_doc, cls_doc, sizeof(int) * (size_t)t->n, cudaMemcpyHostToDevice, st));
+  TxTrainList l;
+  uint32_t *key = nullptr, *idx = nullptr, *cnt = nullptr;
+  EVF(tf_list(t, tmp, f, false, d_cls_doc, &key, &idx, &cnt, &l.n));
+  l.idx = idx, l.cnt = cnt, l.cls = (const int*)key;
+  g_tx_stats.entries = l.n;
+  const int rc = tx_fit(st, tmp, timer, {l}, m, n_c, lambda, t->num_features, out_df, out_idf, out_pi, out_theta);
+  t->train_ms += g_tx_stats.device_ms;
+  return rc;
+}
+
+static int tf_scores(pio_text_folds* t, int f, int32_t n_class, const double* idf, const double* pi,
+                     const double* theta, double* out) {
+  if (n_class < 1 || !idf || !pi || !theta) return fail(nullptr, PIO_ALS_ERR_ARG, "bad pio_text_folds_scores arguments");
+  const long long nq = tf_n_test(t, f), D = t->num_features, CD = (long long)n_class * D;
+  if (nq == 0) return PIO_ALS_OK;
+  if (!out) return fail(nullptr, PIO_ALS_ERR_ARG, "null argument");
+  const std::vector<int> nonfinite = tx_nonfinite(theta, n_class, D);
+  CK0(cudaSetDevice(t->fz->device));
+  cudaStream_t st = t->fz->st;
+  TxTimer timer;
+  EVF(timer.start(st));
+  Scratch tmp(st);
+  double *d_idf = nullptr, *d_pi = nullptr, *d_theta = nullptr, *d_val = nullptr, *d_out = nullptr;
+  int* d_nonfinite = nullptr;
+  CK0(tmp.alloc(&d_idf, (size_t)D));
+  CK0(tmp.alloc(&d_pi, (size_t)n_class));
+  CK0(tmp.alloc(&d_theta, (size_t)CD));
+  CK0(tmp.alloc(&d_nonfinite, (size_t)n_class));
+  CK0(tmp.alloc(&d_out, (size_t)(nq * n_class)));
+  CK0(cudaMemcpyAsync(d_idf, idf, sizeof(double) * (size_t)D, cudaMemcpyHostToDevice, st));
+  CK0(cudaMemcpyAsync(d_pi, pi, sizeof(double) * (size_t)n_class, cudaMemcpyHostToDevice, st));
+  CK0(cudaMemcpyAsync(d_theta, theta, sizeof(double) * (size_t)CD, cudaMemcpyHostToDevice, st));
+  CK0(cudaMemcpyAsync(d_nonfinite, nonfinite.data(), sizeof(int) * (size_t)n_class, cudaMemcpyHostToDevice, st));
+  uint32_t *q = nullptr, *idx = nullptr, *cnt = nullptr;
+  long long ne = 0;
+  EVF(tf_list(t, tmp, f, true, nullptr, &q, &idx, &cnt, &ne));
+  g_tx_stats.entries = ne;
+  CK0(tmp.alloc(&d_val, (size_t)ne));
+  if (ne) tx_value_kernel<<<nblk(ne, 256), 256, 0, st>>>(idx, cnt, d_idf, ne, d_val);
+  CK0(cudaGetLastError());
+  tx_score_kernel<<<nblk(nq * n_class, 256), 256, 0, st>>>(q, idx, d_val, ne, (int)nq, n_class, D, d_theta, d_pi,
+                                                           d_nonfinite, d_out);
+  CK0(cudaGetLastError());
+  CK0(cudaMemcpyAsync(out, d_out, sizeof(double) * (size_t)(nq * n_class), cudaMemcpyDeviceToHost, st));
+  EVF(timer.stop(st));
+  t->scores_ms += g_tx_stats.device_ms;
+  return PIO_ALS_OK;
+}
+
+}  // namespace pio
+
+extern "C" {
+
+int pio_text_folds_create(int device, const uint8_t* stop_bytes, const int64_t* stop_off, int32_t n_stop,
+                          const uint8_t* tok_bytes, const int64_t* tok_off, int32_t n_docs, int32_t k_fold,
+                          pio_text_folds** out) {
+  g_tx_stats = TextStats{};
+  if (!out) return fail(nullptr, PIO_ALS_ERR_ARG, "null argument");
+  *out = nullptr;
+  EVF(tx_check_tokens(tok_bytes, tok_off, n_docs));
+  if (n_docs < 1 || k_fold < 1)
+    return fail(nullptr, PIO_ALS_ERR_ARG, "bad pio_text_folds_create arguments (n_docs >= 1 and k_fold >= 1)");
+  try {
+    std::unique_ptr<pio_text_folds> t(new pio_text_folds);
+    t->k = k_fold, t->n = n_docs;
+    t->tok_bytes.assign(tok_bytes + tok_off[0], tok_bytes + tok_off[n_docs]);
+    t->tok_off.resize((size_t)n_docs + 1);
+    for (int d = 0; d <= n_docs; ++d) t->tok_off[d] = tok_off[d] - tok_off[0];
+    EVF(pio_text_model_create(device, stop_bytes, stop_off, n_stop, 1, 1, &t->fz));
+    *out = t.release();
+  } catch (const std::bad_alloc&) {
+    return fail(nullptr, PIO_ALS_ERR_NOMEM, "pio_text_folds_create: out of host memory");
+  }
+  return PIO_ALS_OK;
+}
+
+int pio_text_folds_destroy(pio_text_folds* t) {
+  if (!t) return PIO_ALS_OK;
+  if (t->fz) {
+    cudaSetDevice(t->fz->device);
+    t->ents.reset();   // frees on the featurizer's stream, which pio_text_model_destroy drains
+    pio_text_model_destroy(t->fz);
+  }
+  delete t;
+  return PIO_ALS_OK;
+}
+
+int pio_text_folds_featurize(pio_text_folds* t, int32_t n_gram, int32_t num_features) {
+  g_tx_stats = TextStats{};
+  if (!t) return fail(nullptr, PIO_ALS_ERR_ARG, "null text folds");
+  std::lock_guard<std::mutex> lk(t->fz->mu);
+  try {
+    return tf_featurize(t, n_gram, num_features);
+  } catch (const std::bad_alloc&) {
+    return fail(nullptr, PIO_ALS_ERR_NOMEM, "pio_text_folds_featurize: out of host memory");
+  }
+}
+
+int pio_text_folds_sizes(const pio_text_folds* t, int32_t fold, int64_t out[2]) {
+  if (!t) return fail(nullptr, PIO_ALS_ERR_ARG, "pio_text_folds_sizes: null object");
+  if (fold < 0 || fold >= t->k)
+    return fail(nullptr, PIO_ALS_ERR_ARG, "pio_text_folds_sizes: fold %d outside 0..%d", fold, t->k - 1);
+  if (!out) return fail(nullptr, PIO_ALS_ERR_ARG, "pio_text_folds_sizes: null out");
+  const long long m = tf_n_test(t, fold);
+  out[0] = t->n - m, out[1] = m;
+  return PIO_ALS_OK;
+}
+
+int pio_text_folds_train_nb(pio_text_folds* t, int32_t fold, const int32_t* cls_doc, int32_t n_class, double lambda,
+                            int64_t* out_df, double* out_idf, double* out_pi, double* out_theta) {
+  g_tx_stats = TextStats{};
+  if (!t) return fail(nullptr, PIO_ALS_ERR_ARG, "null text folds");
+  std::lock_guard<std::mutex> lk(t->fz->mu);
+  EVF(tf_fold(t, fold, "pio_text_folds_train_nb"));
+  try {
+    return tf_train(t, fold, cls_doc, n_class, lambda, out_df, out_idf, out_pi, out_theta);
+  } catch (const std::bad_alloc&) {
+    return fail(nullptr, PIO_ALS_ERR_NOMEM, "pio_text_folds_train_nb: out of host memory");
+  }
+}
+
+int pio_text_folds_scores(pio_text_folds* t, int32_t fold, int32_t n_class, const double* idf, const double* pi,
+                          const double* theta, double* out_scores) {
+  g_tx_stats = TextStats{};
+  if (!t) return fail(nullptr, PIO_ALS_ERR_ARG, "null text folds");
+  std::lock_guard<std::mutex> lk(t->fz->mu);
+  EVF(tf_fold(t, fold, "pio_text_folds_scores"));
+  try {
+    return tf_scores(t, fold, n_class, idf, pi, theta, out_scores);
+  } catch (const std::bad_alloc&) {
+    return fail(nullptr, PIO_ALS_ERR_NOMEM, "pio_text_folds_scores: out of host memory");
+  }
+}
+
+int pio_text_folds_debug_stats(const pio_text_folds* t, double out[6]) {
+  if (!t || !out) return PIO_ALS_ERR_ARG;
+  out[0] = (double)t->featurizations, out[1] = (double)t->nu, out[2] = (double)t->parts;
+  out[3] = t->featurize_ms, out[4] = t->train_ms, out[5] = t->scores_ms;
   return PIO_ALS_OK;
 }
 

@@ -16,6 +16,11 @@
 //   tx_round_kernel    train: each s_cj rounded once to the nearest double, ties to even
 //   tx_value_kernel    features / scores: x_j = tf, or tf * idf_j (one fp64 multiply)
 //   tx_score_kernel    scores: per (query, class) a left fold over the query's entries, then + pi_c
+// The k-fold evaluation (pio_text_folds_*, DESIGN.md 4.18.1) keeps every part's entries, documents made global
+// (tx_doc_base_kernel), and cuts fold f's lists from them (document d tests in fold d % k):
+//   tx_fold_flag_kernel / scan / tx_fold_gather_kernel   the training entries tagged with their document's class, or the
+//                      test entries renumbered t = (d - f) / k; both keep (document, index) order
+// and runs the kernels above on those lists unchanged.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -314,6 +319,42 @@ tx_score_kernel(const uint32_t* __restrict__ doc, const uint32_t* __restrict__ i
   }
   if (nonfinite[c] > present) acc = __longlong_as_double(0x7FF8000000000000ll);
   out[t] = __dadd_rn(acc, pi[c]);
+}
+
+// a part's entries with their documents made global: out[u] = doc[u] + d0
+__global__ void __launch_bounds__(256)
+tx_doc_base_kernel(const uint32_t* __restrict__ doc, long long nu, uint32_t d0, uint32_t* __restrict__ out) {
+  const long long u = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (u < nu) out[u] = doc[u] + d0;
+}
+
+__device__ __forceinline__ bool tx_in_fold_list(uint32_t d, int k, int f, bool test) {
+  return ((int)(d % (uint32_t)k) == f) == test;
+}
+
+// 1 where entry u belongs to fold f's list: its test list (test) or its training list
+__global__ void __launch_bounds__(256)
+tx_fold_flag_kernel(const uint32_t* __restrict__ doc, long long nu, int k, int f, bool test,
+                    uint32_t* __restrict__ flag) {
+  const long long u = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (u < nu) flag[u] = tx_in_fold_list(doc[u], k, f, test);
+}
+
+// entry u of the list goes to position pos[u] (the exclusive scan of the flags) with its index and count, and as its
+// key either its document's class cls_doc[d] (the training list) or, cls_doc null, its test position (d - f) / k
+__global__ void __launch_bounds__(256)
+tx_fold_gather_kernel(const uint32_t* __restrict__ doc, const uint32_t* __restrict__ idx,
+                      const uint32_t* __restrict__ cnt, const uint32_t* __restrict__ pos, long long nu, int k, int f,
+                      bool test, const int* __restrict__ cls_doc, uint32_t* __restrict__ okey,
+                      uint32_t* __restrict__ oidx, uint32_t* __restrict__ ocnt) {
+  const long long u = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (u >= nu) return;
+  const uint32_t d = doc[u];
+  if (!tx_in_fold_list(d, k, f, test)) return;
+  const uint32_t p = pos[u];
+  okey[p] = cls_doc ? (uint32_t)cls_doc[d] : (d - (uint32_t)f) / (uint32_t)k;
+  oidx[p] = idx[u];
+  ocnt[p] = cnt[u];
 }
 
 }  // namespace pio

@@ -53,7 +53,9 @@ EXPORTED_SYMBOLS = [
     "pio_als_rank_lists", "pio_rank_lists_debug_stats", "pio_assoc_index_create", "pio_assoc_index_destroy",
     "pio_assoc_predict", "pio_assoc_predict_get", "pio_assoc_predict_debug_stats", "pio_text_model_create",
     "pio_text_model_destroy", "pio_text_model_set", "pio_text_train_nb", "pio_text_features", "pio_text_features_get",
-    "pio_text_scores", "pio_text_debug_stats",
+    "pio_text_scores", "pio_text_debug_stats", "pio_text_folds_create", "pio_text_folds_destroy",
+    "pio_text_folds_featurize", "pio_text_folds_sizes", "pio_text_folds_train_nb", "pio_text_folds_scores",
+    "pio_text_folds_debug_stats",
 ]
 
 
@@ -236,6 +238,19 @@ def lib():
         L.pio_text_features_get.argtypes = [vp, vp, vp, vp]
         L.pio_text_scores.restype = ci
         L.pio_text_scores.argtypes = [vp, vp, vp, C.c_int32, vp]
+        L.pio_text_folds_create.restype = ci
+        L.pio_text_folds_create.argtypes = [ci, vp, vp, C.c_int32, vp, vp, C.c_int32, C.c_int32, vp]
+        L.pio_text_folds_destroy.argtypes = [vp]
+        L.pio_text_folds_featurize.restype = ci
+        L.pio_text_folds_featurize.argtypes = [vp, C.c_int32, C.c_int32]
+        L.pio_text_folds_sizes.restype = ci
+        L.pio_text_folds_sizes.argtypes = [vp, C.c_int32, vp]
+        L.pio_text_folds_train_nb.restype = ci
+        L.pio_text_folds_train_nb.argtypes = [vp, C.c_int32, vp, C.c_int32, C.c_double, vp, vp, vp, vp]
+        L.pio_text_folds_scores.restype = ci
+        L.pio_text_folds_scores.argtypes = [vp, C.c_int32, C.c_int32, vp, vp, vp, vp]
+        L.pio_text_folds_debug_stats.restype = ci
+        L.pio_text_folds_debug_stats.argtypes = [vp, vp]
         for name in EXPORTED_SYMBOLS:
             getattr(L, name)  # AttributeError if the ABI is incomplete
         _lib = L
@@ -1549,19 +1564,31 @@ def text_tokens(texts):
     return _str_column([json.dumps(t).encode("ascii") for t in texts])
 
 
+def _stop_column(stop_words):
+    """Stop words (str, as UTF-8 with unpaired surrogates as '?', or bytes) as a string column."""
+    return _str_column([w.encode("utf-8", "replace") if isinstance(w, str) else bytes(w) for w in stop_words])
+
+
+def _text_tokens_arg(tok_bytes, tok_off):
+    b = np.ascontiguousarray(tok_bytes, np.uint8)
+    o = np.ascontiguousarray(tok_off, np.int64)
+    if o.ndim != 1 or o.shape[0] < 1 or (o.shape[0] > 1 and int(o[-1]) > b.shape[0]):
+        raise ValueError("tok_off must be [n + 1] offsets into tok_bytes")
+    return b, o, int(o.shape[0] - 1)
+
+
 class TextModel:
     """pio_text_model: the featurizer of PreparatorParams(nGram, numFeatures) with its stop words on `device`, and,
     once set, a Naive Bayes model (idf, pi, theta) that scores batches.  Documents go in as raw JSON string tokens
     (tok_bytes, tok_off), as the keyed event scan returns them or text_tokens makes them."""
 
     def __init__(self, stop_words, n_gram: int, num_features: int, device: int = 0):
-        words = [w.encode("utf-8", "replace") if isinstance(w, str) else bytes(w) for w in stop_words]
-        sb, so = _str_column(words)
+        sb, so = _stop_column(stop_words)
         self.n_gram, self.num_features, self.device = int(n_gram), int(num_features), int(device)
         self.n_class = 0
         self._h = C.c_void_p()
         _check(lib().pio_text_model_create(self.device, sb.ctypes.data if sb.size else None, so.ctypes.data,
-                                           len(words), self.n_gram, self.num_features, C.addressof(self._h)))
+                                           so.shape[0] - 1, self.n_gram, self.num_features, C.addressof(self._h)))
 
     def close(self):
         if self._h:
@@ -1574,13 +1601,7 @@ class TextModel:
         except Exception:
             pass
 
-    @staticmethod
-    def _tokens(tok_bytes, tok_off):
-        b = np.ascontiguousarray(tok_bytes, np.uint8)
-        o = np.ascontiguousarray(tok_off, np.int64)
-        if o.ndim != 1 or o.shape[0] < 1 or (o.shape[0] > 1 and int(o[-1]) > b.shape[0]):
-            raise ValueError("tok_off must be [n + 1] offsets into tok_bytes")
-        return b, o, int(o.shape[0] - 1)
+    _tokens = staticmethod(_text_tokens_arg)
 
     def set_model(self, idf, pi, theta):
         idf = np.ascontiguousarray(idf, np.float64)
@@ -1630,3 +1651,76 @@ def text_stats() -> dict:
     _check(lib().pio_text_debug_stats(out))
     return {"parts": int(out[0]), "docs": int(out[1]), "windows": int(out[2]), "entries": int(out[3]),
             "max_part_bytes": int(out[4]), "budget": int(out[5]), "device_ms": out[6]}
+
+
+class TextFolds:
+    """pio_text_folds: the k-fold split of a text classification evaluation on the device (document d tests in fold
+    d % k_fold and trains in every other fold, in document order).  The documents -- raw JSON string tokens, as
+    TextModel takes them -- are featurized once per (nGram, numFeatures) and kept on the device as (document, feature)
+    entries; each fold trains Naive Bayes and scores its test documents from them."""
+
+    def __init__(self, tok_bytes, tok_off, stop_words, k_fold: int, device: int = 0):
+        b, o, n = _text_tokens_arg(tok_bytes, tok_off)
+        sb, so = _stop_column(stop_words)
+        self.n_docs, self.k_fold, self.device = n, int(k_fold), int(device)
+        self.n_gram = self.num_features = 0
+        self._h = C.c_void_p()
+        _check(lib().pio_text_folds_create(self.device, sb.ctypes.data if sb.size else None, so.ctypes.data,
+                                           so.shape[0] - 1, b.ctypes.data if b.size else None, o.ctypes.data, n,
+                                           self.k_fold, C.addressof(self._h)))
+
+    def close(self):
+        if self._h:
+            lib().pio_text_folds_destroy(self._h)
+            self._h = C.c_void_p()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    def featurize(self, n_gram: int, num_features: int) -> None:
+        """The entries of PreparatorParams(n_gram, num_features); a no-op when they are the current ones."""
+        _check(lib().pio_text_folds_featurize(self._h, int(n_gram), int(num_features)))
+        self.n_gram, self.num_features = int(n_gram), int(num_features)
+
+    def sizes(self, fold: int) -> tuple:
+        """(training documents, test documents) of fold `fold`."""
+        out = np.zeros(2, np.int64)
+        _check(lib().pio_text_folds_sizes(self._h, int(fold), out.ctypes.data))
+        return int(out[0]), int(out[1])
+
+    def train_nb(self, fold: int, cls_doc, n_class: int, lam: float):
+        """TextModel.train_nb on the fold's training documents under the current featurization: (df, idf, pi, theta).
+        cls_doc: every document's class among the fold's training labels (test documents' are ignored)."""
+        cls_doc = np.ascontiguousarray(cls_doc, np.int32)
+        if cls_doc.shape != (self.n_docs,):
+            raise ValueError("one class per document")
+        D, c = self.num_features, max(int(n_class), 1)
+        df, idf = np.empty(D, np.int64), np.empty(D, np.float64)
+        pi, theta = np.empty(c, np.float64), np.empty((c, D), np.float64)
+        _check(lib().pio_text_folds_train_nb(self._h, int(fold), cls_doc.ctypes.data, int(n_class), float(lam),
+                                             df.ctypes.data, idf.ctypes.data, pi.ctypes.data, theta.ctypes.data))
+        return df, idf, pi, theta
+
+    def scores(self, fold: int, idf, pi, theta) -> np.ndarray:
+        """TextModel.scores of the fold's test documents, in document order: [n_test, C]."""
+        idf = np.ascontiguousarray(idf, np.float64)
+        pi = np.ascontiguousarray(pi, np.float64)
+        theta = np.ascontiguousarray(theta, np.float64)
+        c = pi.shape[0]
+        if idf.shape != (self.num_features,) or theta.shape != (c, self.num_features):
+            raise ValueError("idf must be [numFeatures], pi [C] and theta [C, numFeatures] of the current featurization")
+        out = np.empty((self.sizes(fold)[1], c), np.float64)
+        _check(lib().pio_text_folds_scores(self._h, int(fold), c, idf.ctypes.data, pi.ctypes.data, theta.ctypes.data,
+                                           out.ctypes.data))
+        return out
+
+    def stats(self) -> dict:
+        """Featurizations done, entries and parts of the current one, and device milliseconds of the featurizations,
+        the trainings and the scorings over the object's life."""
+        out = (C.c_double * 6)()
+        _check(lib().pio_text_folds_debug_stats(self._h, out))
+        return {"featurizations": int(out[0]), "entries": int(out[1]), "parts": int(out[2]),
+                "featurize_ms": out[3], "train_ms": out[4], "scores_ms": out[5]}

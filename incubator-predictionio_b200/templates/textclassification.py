@@ -6,6 +6,8 @@ Observation and stop words, PreparatorParams / PreparedData, NBAlgorithmParams /
 Accuracy, EngineParamsList).  tests/textclassification_ref.py restates the rules and marks the project's own readings.
 Texts never pass through Python on the training path: the event scan returns each `text` as its raw JSON token and the
 device decodes, splits, hashes and counts them (native.TextModel, DESIGN.md 4.18); the logarithms are taken on the host.
+readEvalColumns keeps the evaluation's folds on the device (native.TextFolds, DESIGN.md 4.18.1): the documents are
+featurized once, and each fold trains and scores from the resident entries; readEval is the object path it equals.
 The doc's "lr" algorithm (logistic regression) has no code in the doc and is rejected, and so is SPPMI.
 """
 from __future__ import annotations
@@ -21,6 +23,7 @@ from .. import native
 from .. import storage
 from ..controller import Engine, EngineFactory, EngineParams, LServing, P2LAlgorithm, Params, PDataSource, PPreparator
 from ..evaluation import AverageMetric, EngineParamsGenerator, Evaluation, MetricEvaluator
+from .classification import _ratio
 
 
 @dataclass
@@ -54,11 +57,42 @@ class Observation:
 
 class TrainingData:
     """The e-mails as columns -- their `text` as raw JSON string tokens (tok_bytes, tok_off), label (1.0 for "spam",
-    else 0.0) and category -- and the stop words.  `data` (a list of Observation) is built on first use."""
+    else 0.0) and category -- and the stop words.  `data` (a list of Observation) is built on first use.  Or one fold
+    of DataSource.readEvalColumns on the device: NBAlgorithm then trains from the fold, and the columns are cut from the
+    read as readEval cuts them only on first use."""
 
-    def __init__(self, tokens, labels, categories: List[str], stopWords):
-        self.tokens, self.labels, self.categories = tokens, np.asarray(labels, np.float64), list(categories)
+    def __init__(self, tokens=None, labels=None, categories: List[str] = (), stopWords=(),
+                 fold: Optional["TextFold"] = None):
+        self.fold, self._cols = fold, None
+        if fold is None:
+            self._cols = (tokens, np.asarray(labels, np.float64), list(categories))
         self.stopWords = set(stopWords)
+
+    def _cut(self):
+        if self._cols is None:
+            t = self.fold.training_subset()
+            self._cols = (t.tokens, t.labels, t.categories)
+        return self._cols
+
+    @property
+    def tokens(self):
+        return self._cut()[0]
+
+    @property
+    def labels(self) -> np.ndarray:
+        return self._cut()[1]
+
+    @property
+    def categories(self) -> List[str]:
+        return self._cut()[2]
+
+    @property
+    def on_device(self) -> bool:
+        """True while the training documents exist only as the fold on the device."""
+        return self.fold is not None and self._cols is None
+
+    def __len__(self) -> int:
+        return self.fold.n_train if self.on_device else int(self.labels.shape[0])
 
     @property
     def data(self) -> List[Observation]:
@@ -97,6 +131,52 @@ def _scan(appName, entityType, event, keys, sc):
         present = np.concatenate([present, h_present])[order]
         lines = all_lines[order]
     return lines, tok, present
+
+
+class TextFold:
+    """One fold of DataSource.readEvalColumns (native.TextFolds): its training documents, which NBAlgorithm trains from
+    on the device, and its queries -- the test documents, which batchPredictColumns scores there.  `data` is the whole
+    read."""
+
+    def __init__(self, folds: native.TextFolds, fold: int, data: TrainingData):
+        self.folds, self.fold, self.data = folds, fold, data
+        self.n_train, self.n_test = folds.sizes(fold)
+        self._train_classes = None
+
+    def rows(self, test: bool) -> np.ndarray:
+        fold_of = np.arange(len(self.data)) % self.folds.k_fold
+        return np.flatnonzero(fold_of == self.fold if test else fold_of != self.fold)
+
+    def training_subset(self) -> TrainingData:
+        """readEval's TrainingData of the fold."""
+        return self.data.subset(self.rows(False))
+
+    def train_classes(self):
+        """(classes, each document's class index among them, categoryMap) of the fold's training documents: classes
+        as NBAlgorithm.train takes them (np.unique of the labels), and category_map's rule -- the last category of a
+        label in event order, keys in order of first appearance -- without a loop over the documents."""
+        if self._train_classes is None:
+            labels, train = self.data.labels, self.rows(False)
+            classes = np.unique(labels[train])
+            cls_doc = np.searchsorted(classes, labels).astype(np.int32)
+            c_train = cls_doc[train]
+            _, first = np.unique(c_train, return_index=True)
+            _, last_rev = np.unique(c_train[::-1], return_index=True)
+            last = train[c_train.shape[0] - 1 - last_rev]
+            cats = self.data.categories
+            order = np.argsort(first, kind="stable")
+            cm = {float(classes[c]): cats[int(last[c])] for c in order.tolist()}
+            self._train_classes = (classes, cls_doc, cm)
+        return self._train_classes
+
+    def actual(self) -> np.ndarray:
+        """The test documents' categories (ActualResult), in document order."""
+        cats = self.data.categories
+        return np.array([cats[i] for i in self.rows(True).tolist()], dtype=object)
+
+
+def _no_evalK():
+    raise AssertionError("requirement failed: DataSourceParams.evalK must not be None")
 
 
 def _first_bytes(col):
@@ -142,7 +222,7 @@ class DataSource(PDataSource):
         """Document i tests in fold i % evalK: per fold (TrainingData of the other documents, None,
         [(Query(text), ActualResult(category))])."""
         if self.dsp.evalK is None:
-            raise AssertionError("requirement failed: DataSourceParams.evalK must not be None")
+            _no_evalK()
         k = self.dsp.evalK
         td = self._read(sc)
         obs = td.data
@@ -152,6 +232,22 @@ class DataSource(PDataSource):
             train, test = np.flatnonzero(fold_of != f), np.flatnonzero(fold_of == f)
             qas = [(Query(obs[i].text), ActualResult(obs[i].category)) for i in test.tolist()]
             out.append((td.subset(train), None, qas))
+        return out
+
+    def readEvalColumns(self, sc) -> Optional[list]:
+        """readEval's folds, kept on the device: per fold (TrainingData of its TextFold, None, the TextFold as its
+        queries).  None -- readEval's object path -- when evalK < 1 or there are no documents."""
+        if self.dsp.evalK is None:
+            _no_evalK()
+        k = self.dsp.evalK
+        td = self._read(sc)
+        if k < 1 or len(td) == 0:
+            return None
+        folds = native.TextFolds(*td.tokens, sorted(td.stopWords), k, getattr(sc, "device", 0) or 0)
+        out = []
+        for f in range(k):
+            fold = TextFold(folds, f, td)
+            out.append((TrainingData(stopWords=td.stopWords, fold=fold), None, fold))
         return out
 
 
@@ -187,7 +283,9 @@ class PreparedData:
     def __init__(self, td: TrainingData, pp: PreparatorParams, device: int = 0):
         check_preparator(pp)
         self.td, self.nGram, self.numFeatures, self.device = td, pp.nGram, pp.numFeatures, device
-        self.categoryMap = category_map(td.labels, td.categories)
+        self.fold = td.fold if td.on_device else None
+        self.categoryMap = self.fold.train_classes()[2] if self.fold is not None else \
+            category_map(td.labels, td.categories)
 
     def featurizer(self) -> native.TextModel:
         return native.TextModel(sorted(self.td.stopWords), self.nGram, self.numFeatures, self.device)
@@ -281,9 +379,11 @@ class NBAlgorithm(P2LAlgorithm):
 
     def train(self, sc, pd: PreparedData) -> NBModel:
         td = pd.td
-        if td.labels.shape[0] == 0:
+        if len(td) == 0:
             raise ValueError("requirement failed: the training data is empty: make sure event fields match imported "
                              "data")
+        if pd.fold is not None:
+            return self._train_fold(pd)
         classes = np.unique(td.labels)
         label_idx = np.searchsorted(classes, td.labels).astype(np.int32)
         tm = pd.featurizer()
@@ -294,8 +394,24 @@ class NBAlgorithm(P2LAlgorithm):
         return NBModel(classes, pi, theta, idf, df, pd.categoryMap, pd.nGram, pd.numFeatures, td.stopWords,
                        pd.device)
 
+    def _train_fold(self, pd: PreparedData) -> NBModel:
+        """train on the fold's training documents from the entries on the device."""
+        fold = pd.fold
+        classes, cls_doc, cm = fold.train_classes()
+        fold.folds.featurize(pd.nGram, pd.numFeatures)
+        df, idf, pi, theta = fold.folds.train_nb(fold.fold, cls_doc, classes.shape[0], self.ap.lambda_)
+        return NBModel(classes, pi, theta, idf, df, cm, pd.nGram, pd.numFeatures, pd.td.stopWords, pd.device)
+
     def predict(self, model: NBModel, query: Query) -> PredictedResult:
         return self.predictMany(model, [query])[0]
+
+    def batchPredictColumns(self, sc, model: NBModel, queries: TextFold) -> "PredictedColumns":
+        """predict of every test document of the fold: the raw scores on the device, then predictMany's confidences
+        and categories on the host."""
+        queries.folds.featurize(model.nGram, model.numFeatures)
+        best, conf = confidences(queries.folds.scores(queries.fold, model.idf, model.pi, model.theta))
+        cats = np.array([model.categoryMap.get(y, "") for y in model.labels.tolist()], dtype=object)
+        return PredictedColumns(cats[best], conf)
 
     def predictMany(self, model: NBModel, queries) -> List[PredictedResult]:
         """predict of every query, in one device call for the raw scores."""
@@ -315,6 +431,13 @@ class LRAlgorithm(P2LAlgorithm):
                                   'template: use "nb"')
 
 
+@dataclass
+class PredictedColumns:
+    """The PredictedResults of a fold's test documents as columns: category (object array of str) and confidence."""
+    category: np.ndarray
+    confidence: np.ndarray
+
+
 class Serving(LServing):
     def serve(self, query: Query, predictedResults) -> PredictedResult:
         """predictedResults.maxBy(_.confidence): the first, replaced only by a strictly greater confidence."""
@@ -323,6 +446,15 @@ class Serving(LServing):
             if p.confidence > best.confidence:
                 best = p
         return best
+
+    def serveColumns(self, queries, predictions) -> PredictedColumns:
+        """serve of every query over the algorithms' columns: a later algorithm wins only where its confidence is
+        strictly greater, so a NaN never wins."""
+        cat, conf = predictions[0].category, predictions[0].confidence
+        for p in predictions[1:]:
+            better = p.confidence > conf
+            cat, conf = np.where(better, p.category, cat), np.where(better, p.confidence, conf)
+        return PredictedColumns(cat, conf)
 
 
 class TextClassificationEngine(EngineFactory):
@@ -335,6 +467,11 @@ class Accuracy(AverageMetric):
 
     def calculate_one(self, q: Query, p: PredictedResult, a: ActualResult) -> float:
         return 1.0 if p.category == a.category else 0.0
+
+    def calculate_columns(self, sc, evalColumns) -> float:
+        """calculate over Engine.evalColumns' folds: correct predictions over test documents."""
+        correct = sum(int((served.category == fold.actual()).sum()) for _, fold, served in evalColumns)
+        return _ratio(correct, sum(fold.n_test for _, fold, _ in evalColumns))
 
 
 class AccuracyEvaluation(Evaluation):
