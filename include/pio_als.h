@@ -43,6 +43,8 @@
  *       docs/manual/source/templates/complementarypurchase/dase.html.md.erb:293-314
  *   pio_text_folds_* run the text classification template's k-fold evaluation
  *       docs/manual/source/demo/textclassification.html.md.erb (readEval, Accuracy, EngineParamsList)
+ *   pio_fr_* replace the dimensionality-reduction template's string2Vector, PCA, transform and LogisticRegression
+ *       docs/manual/source/machinelearning/dimensionalityreduction.html.md (PreparedData, LRModel)
  */
 #ifndef PIO_ALS_H_
 #define PIO_ALS_H_
@@ -938,6 +940,59 @@ PIO_API int pio_text_folds_scores(pio_text_folds* f, int32_t fold, int32_t n_cla
 /* out[0] featurizations done, [1] entries of the current one, [2] its parts, device milliseconds of [3] the
  * featurizations, [4] the trainings and [5] the scorings, over the object's life. */
 PIO_API int pio_text_folds_debug_stats(const pio_text_folds* f, double out[6]);
+
+/* The dimensionality-reduction classification template (DESIGN.md 4.19): feature strings ("v0, v1, ...", Java's
+ * e.split(", ").map(_.toDouble)) parsed on the device, PCA's column means and Gramian, the projection onto the
+ * principal components, and one-vs-rest logistic regression's loss and gradient over the projected rows.  The
+ * covariance, its SVD and the L-BFGS driver run on the host.  HOST buffers.  Errors: status codes as above, text via
+ * pio_als_last_error(NULL); arguments are checked before any device work.
+ *
+ * Per-row parse status (out_status): PIO_FR_OK parsed on the device, PIO_FR_HOST parsed by the host's restatement of
+ * Double.parseDouble (a piece off the exact fast path), PIO_FR_BAD a piece that is not a Java double, PIO_FR_NONFINITE
+ * a NaN or infinite value, PIO_FR_LEN a row whose length differs from p.  Rows are parsed in parts of consecutive rows
+ * under PIO_FR_BUDGET raw token bytes; nothing depends on the budget. */
+#define PIO_FR_OK 0
+#define PIO_FR_HOST 1
+#define PIO_FR_BAD (-1)
+#define PIO_FR_NONFINITE (-2)
+#define PIO_FR_LEN (-3)
+typedef struct pio_fr_data pio_fr_data;
+PIO_API int pio_fr_data_create(int device, pio_fr_data** out);
+PIO_API int pio_fr_data_destroy(pio_fr_data* d);
+/* Parses n_rows >= 1 rows, each a raw JSON string token (tok_bytes[tok_off[r] .. tok_off[r + 1])), into the resident
+ * n_rows x p matrix; p is the length of row 0 (1 <= p <= 65535, else PIO_ALS_ERR_ARG).  out_status [n_rows]; *out_p.
+ * The rows are usable when every status is PIO_FR_OK or PIO_FR_HOST; if row 0 is bad the other statuses are 0 and the
+ * handle holds no rows. */
+PIO_API int pio_fr_parse(pio_fr_data* d, const uint8_t* tok_bytes, const int64_t* tok_off, int32_t n_rows,
+                         int32_t* out_status, int32_t* out_p);
+/* The column sums in a fixed order divided by n (out_mean [p]) and X^T X (out_gram [p x p], symmetric); n >= 2. */
+PIO_API int pio_fr_gramian(pio_fr_data* d, double* out_mean, double* out_gram);
+/* y_ri = fold_j(pc[j * k + i] * (x_rj - mean_j)) (pc: p x k row-major, the principal components as columns), kept on
+ * the device as the training rows of the logistic regression; out_y [n x k] may be NULL. */
+PIO_API int pio_fr_project(pio_fr_data* d, int32_t k, const double* mean, const double* pc, double* out_y);
+/* Starts the logistic regressions over the projected rows: cls [n] each row's class in [0, n_class); out_sigma [k] the
+ * unbiased standard deviation of each column (two passes, in the fixed block order). */
+PIO_API int pio_fr_lr_prepare(pio_fr_data* d, const int32_t* cls, int32_t n_class, double* out_sigma);
+/* Loss and gradient of n_active binary regressions (class labels[a] against the rest), each at wb[a] = (w [k], b) in
+ * the standardized space, with L2 parameter reg_param: out_f [n_active], out_g [n_active x (k + 1)]. */
+PIO_API int pio_fr_lr_eval(pio_fr_data* d, int32_t n_active, const int32_t* labels, const double* wb, double reg_param,
+                           double* out_f, double* out_g);
+/* out[0] parts, [1] rows, [2] host-parsed rows, device milliseconds of [3] the parse, [4] mean + Gramian, [5] the
+ * projection, [6] sigma and [7] the loss-and-gradient calls, [8] loss-and-gradient calls, [9] the Gramian's slices. */
+PIO_API int pio_fr_data_debug_stats(const pio_fr_data* d, double out[10]);
+
+/* A trained model that serves query batches: mean [p], pc [p x k] as pio_fr_project takes it, coef [n_label x k], b
+ * [n_label]. */
+typedef struct pio_fr_model pio_fr_model;
+PIO_API int pio_fr_model_create(int device, int32_t p, int32_t k, int32_t n_label, const double* mean, const double* pc,
+                                const double* coef, const double* b, pio_fr_model** out);
+PIO_API int pio_fr_model_destroy(pio_fr_model* m);
+/* Parses n >= 0 queries as pio_fr_parse does (out_status [n]; every row must have length p), projects them and scores
+ * every label: out_scores [n x n_label] = fold_j(coef_lj * y_j) + b_l, undefined on rows whose status is bad. */
+PIO_API int pio_fr_model_scores(pio_fr_model* m, const uint8_t* tok_bytes, const int64_t* tok_off, int32_t n,
+                                int32_t* out_status, double* out_scores);
+/* What the last pio_fr_model_scores did: out[0] parts, [1] rows, [2] host-parsed rows, [3] device milliseconds. */
+PIO_API int pio_fr_model_debug_stats(const pio_fr_model* m, double out[4]);
 
 #ifdef __cplusplus
 }

@@ -66,6 +66,8 @@
 #include "assoc_predict.cuh"
 #include "text_nb.cuh"
 #include "text_plan.h"
+#include "dense_pca.cuh"
+#include "logreg.cuh"
 
 namespace pio {
 
@@ -8990,6 +8992,558 @@ int pio_text_folds_debug_stats(const pio_text_folds* t, double out[6]) {
   if (!t || !out) return PIO_ALS_ERR_ARG;
   out[0] = (double)t->featurizations, out[1] = (double)t->nu, out[2] = (double)t->parts;
   out[3] = t->featurize_ms, out[4] = t->train_ms, out[5] = t->scores_ms;
+  return PIO_ALS_OK;
+}
+
+}  // extern "C"
+
+// ---- dimensionality-reduction classification (pio_fr_*; DESIGN.md 4.19) ---------------------------------------------
+struct pio_fr_data {
+  int device = 0;
+  cudaStream_t st = nullptr;
+  std::mutex mu;                                   // serialises the calls
+  long long n = 0;                                 // rows parsed
+  int p = 0, k = 0, n_class = 0;
+  bool rows_ok = false;                            // every row parsed and of length p
+  double *d_x = nullptr;                           // n x p row-major
+  double *d_y = nullptr, *d_yt = nullptr;          // the projected rows: n x k row-major, and k x n
+  double* d_sigma = nullptr;                       // [k], after pio_fr_lr_prepare
+  int* d_cls = nullptr;                            // [n]
+  long long parts = 0, host_rows = 0, lr_evals = 0;
+  int slices = 0;
+  double parse_ms = 0, gram_ms = 0, project_ms = 0, sigma_ms = 0, lr_ms = 0;
+};
+
+struct pio_fr_model {
+  int device = 0, p = 0, k = 0, n_label = 0;
+  cudaStream_t st = nullptr;
+  std::mutex mu;
+  double *d_mean = nullptr, *d_a = nullptr, *d_coef = nullptr, *d_b = nullptr;
+  long long parts = 0, rows = 0, host_rows = 0;
+  double device_ms = 0;
+};
+
+namespace pio {
+
+// Double.parseDouble's grammar on one piece [a, b): after String.trim, an optional sign, then NaN, Infinity, a decimal
+// significand (digits with an optional point, at least one digit) with an optional exponent, or a hex significand
+// (0x / 0X, hex digits with an optional point) with its required binary exponent; then an optional f, F, d or D.  The
+// value is strtod's of the piece without its suffix, which is correctly rounded as Java's is.  False: not a double.
+static bool fr_java_double(const uint8_t* s, int a, int b, double* v) {
+  while (a < b && s[a] <= ' ') ++a;
+  while (b > a && s[b - 1] <= ' ') --b;
+  if (a >= b) return false;
+  const std::string t((const char*)s + a, (size_t)(b - a));
+  size_t i = 0;
+  const bool neg = t[0] == '-';
+  if (t[0] == '+' || t[0] == '-') i = 1;
+  const std::string rest = t.substr(i);
+  if (rest == "NaN") return *v = std::numeric_limits<double>::quiet_NaN(), true;
+  if (rest == "Infinity") return *v = neg ? -HUGE_VAL : HUGE_VAL, true;
+  const bool hex = rest.size() >= 2 && rest[0] == '0' && (rest[1] == 'x' || rest[1] == 'X');
+  auto digit = [hex](char c) { return hex ? isxdigit((unsigned char)c) != 0 : (c >= '0' && c <= '9'); };
+  size_t j = hex ? 2 : 0;
+  int digits = 0;
+  for (; j < rest.size() && digit(rest[j]); ++j) ++digits;
+  if (j < rest.size() && rest[j] == '.')
+    for (++j; j < rest.size() && digit(rest[j]); ++j) ++digits;
+  if (!digits) return false;
+  const bool has_exp = j < rest.size() && (hex ? (rest[j] == 'p' || rest[j] == 'P') : (rest[j] == 'e' || rest[j] == 'E'));
+  if (hex && !has_exp) return false;
+  if (has_exp) {
+    ++j;
+    if (j < rest.size() && (rest[j] == '+' || rest[j] == '-')) ++j;
+    int ed = 0;
+    for (; j < rest.size() && rest[j] >= '0' && rest[j] <= '9'; ++j) ++ed;
+    if (!ed) return false;
+  }
+  const size_t end = j;
+  if (j < rest.size() && strchr("fFdD", rest[j])) ++j;
+  if (j != rest.size()) return false;
+  const std::string num = t.substr(0, i) + rest.substr(0, end);
+  *v = strtod(num.c_str(), nullptr);
+  return true;
+}
+
+// The host's parse of one row (a raw JSON string token of len bytes): its values, and FR_OK, FR_BAD (the first piece
+// that is not a double, as map(_.toDouble) throws there), FR_NONFINITE or, when p >= 0, FR_LEN.
+static int fr_host_row(const uint8_t* tok, long long len, int p, std::vector<uint8_t>& dec, std::vector<double>& vals) {
+  dec.resize((size_t)std::max<long long>(len, 1));
+  const int L = ev::decode_string_lenient(tok, 0, (int)len, dec.data());
+  const uint8_t* s = dec.data();
+  vals.clear();
+  if (L == 0) return FR_BAD;                         // "".split(", ") is [""]
+  std::vector<std::pair<int, int>> pieces;
+  for (int i = 0, start = 0;;) {
+    const bool end = i >= L;
+    if (end || (s[i] == ',' && i + 1 < L && s[i + 1] == ' ')) {
+      pieces.emplace_back(start, i);
+      if (end) break;
+      i += 2;
+      start = i;
+    } else {
+      ++i;
+    }
+  }
+  while (!pieces.empty() && pieces.back().first == pieces.back().second) pieces.pop_back();   // trailing "" dropped
+  bool finite = true;
+  for (const auto& pc : pieces) {
+    double v;
+    if (!fr_java_double(s, pc.first, pc.second, &v)) return FR_BAD;
+    finite &= std::isfinite(v) != 0;
+    vals.push_back(v);
+  }
+  if (!finite) return FR_NONFINITE;
+  if (p >= 0 && (int)vals.size() != p) return FR_LEN;
+  return FR_OK;
+}
+
+static int fr_check_tokens(const uint8_t* tok_bytes, const int64_t* tok_off, int32_t n) {
+  if (n < 0) return fail(nullptr, PIO_ALS_ERR_ARG, "n_rows must be >= 0");
+  if (!tok_off || (n > 0 && !tok_bytes)) return fail(nullptr, PIO_ALS_ERR_ARG, "null token argument");
+  if (tok_off[0] < 0) return fail(nullptr, PIO_ALS_ERR_ARG, "tok_off[0] must be >= 0");
+  for (int r = 0; r < n; ++r) {
+    const long long len = tok_off[r + 1] - tok_off[r];
+    if (len < 0) return fail(nullptr, PIO_ALS_ERR_ARG, "tok_off decreases at row %d", r);
+    if (len >= (1ll << 31)) return fail(nullptr, PIO_ALS_ERR_ARG, "row %d: a token holds fewer than 2^31 bytes", r);
+    if (len < 2 || tok_bytes[tok_off[r]] != '"' || tok_bytes[tok_off[r + 1] - 1] != '"')
+      return fail(nullptr, PIO_ALS_ERR_ARG, "row %d is not a JSON string token", r);
+  }
+  return PIO_ALS_OK;
+}
+
+// device milliseconds between two events on a stream
+struct FrTimer {
+  cudaEvent_t ev[2] = {nullptr, nullptr};
+  ~FrTimer() {
+    if (ev[0]) cudaEventDestroy(ev[0]);
+    if (ev[1]) cudaEventDestroy(ev[1]);
+  }
+  int start(cudaStream_t st) {
+    CK0(cudaEventCreate(&ev[0]));
+    CK0(cudaEventCreate(&ev[1]));
+    CK0(cudaEventRecord(ev[0], st));
+    return PIO_ALS_OK;
+  }
+  int stop(cudaStream_t st, double* ms_out) {
+    CK0(cudaEventRecord(ev[1], st));
+    CK0(cudaEventSynchronize(ev[1]));
+    float ms = 0.f;
+    CK0(cudaEventElapsedTime(&ms, ev[0], ev[1]));
+    *ms_out = ms;
+    return PIO_ALS_OK;
+  }
+};
+
+// Parses rows [0, n) into d_x (n x p) part by part: the device's fast path, then the host's parse of the rows it hands
+// back.  Status per row into status; *parts and *host_rows counted.
+static int fr_parse_rows(cudaStream_t st, const uint8_t* tok_bytes, const int64_t* tok_off, int32_t n, int p,
+                         double* d_x, int32_t* status, long long* parts_out, long long* host_out) {
+  const char* env_b = getenv("PIO_FR_BUDGET");
+  const long long budget = std::min<long long>(env_b && atoll(env_b) > 0 ? atoll(env_b) : (256ll << 20),
+                                               (1ll << 31) - 1);
+  const std::vector<TextPart> parts = plan_text(tok_off, n, budget);
+  std::vector<uint8_t> dec;
+  std::vector<double> vals, host_vals;
+  for (const TextPart& pt : parts) {
+    const int nr = pt.d1 - pt.d0;
+    const long long nb = pt.b1 - pt.b0;
+    std::vector<long long> off((size_t)nr + 1);
+    for (int j = 0; j <= nr; ++j) off[j] = tok_off[pt.d0 + j] - pt.b0;
+    Scratch tmp(st);
+    uint8_t *d_raw = nullptr, *d_dec = nullptr;
+    long long* d_off = nullptr;
+    int* d_status = nullptr;
+    CK0(tmp.alloc(&d_raw, (size_t)nb));
+    CK0(tmp.alloc(&d_dec, (size_t)nb));
+    CK0(tmp.alloc(&d_off, (size_t)nr + 1));
+    CK0(tmp.alloc(&d_status, (size_t)nr));
+    CK0(cudaMemcpyAsync(d_raw, tok_bytes + pt.b0, (size_t)nb, cudaMemcpyHostToDevice, st));
+    CK0(cudaMemcpyAsync(d_off, off.data(), sizeof(long long) * off.size(), cudaMemcpyHostToDevice, st));
+    double* xp = d_x + (long long)pt.d0 * p;
+    fr_parse_kernel<<<nblk(nr, 128), 128, 0, st>>>(d_raw, d_off, nr, p, d_dec, xp, d_status);
+    CK0(cudaGetLastError());
+    CK0(cudaMemcpyAsync(status + pt.d0, d_status, sizeof(int) * (size_t)nr, cudaMemcpyDeviceToHost, st));
+    CK0(cudaStreamSynchronize(st));
+    std::vector<int> rows;
+    host_vals.clear();
+    for (int r = pt.d0; r < pt.d1; ++r) {
+      if (status[r] != FR_HOST) continue;
+      const int rc = fr_host_row(tok_bytes + tok_off[r], tok_off[r + 1] - tok_off[r], p, dec, vals);
+      if (rc != FR_OK) {
+        status[r] = rc;
+        continue;
+      }
+      ++*host_out;
+      rows.push_back(r);
+      host_vals.insert(host_vals.end(), vals.begin(), vals.end());
+    }
+    for (size_t q = 0; q < rows.size(); ++q)
+      CK0(cudaMemcpyAsync(d_x + (long long)rows[q] * p, host_vals.data() + q * p, sizeof(double) * p,
+                          cudaMemcpyHostToDevice, st));
+    CK0(cudaStreamSynchronize(st));
+    ++*parts_out;
+  }
+  return PIO_ALS_OK;
+}
+
+static void fr_free_rows(pio_fr_data* d) {
+  for (void* q : {(void*)d->d_x, (void*)d->d_y, (void*)d->d_yt, (void*)d->d_sigma, (void*)d->d_cls})
+    if (q) cudaFree(q);
+  d->d_x = d->d_y = d->d_yt = d->d_sigma = nullptr;
+  d->d_cls = nullptr;
+  d->n = 0, d->p = 0, d->k = 0, d->n_class = 0, d->rows_ok = false;
+}
+
+static int fr_parse(pio_fr_data* d, const uint8_t* tok_bytes, const int64_t* tok_off, int32_t n, int32_t* status,
+                    int32_t* out_p) {
+  EVF(fr_check_tokens(tok_bytes, tok_off, n));
+  if (n < 1) return fail(nullptr, PIO_ALS_ERR_ARG, "pio_fr_parse needs at least one row");
+  if (!status || !out_p) return fail(nullptr, PIO_ALS_ERR_ARG, "null argument");
+  CK0(cudaSetDevice(d->device));
+  fr_free_rows(d);
+  d->parts = d->host_rows = d->lr_evals = 0;
+  d->parse_ms = d->gram_ms = d->project_ms = d->sigma_ms = d->lr_ms = 0;
+  *out_p = 0;
+  for (int r = 0; r < n; ++r) status[r] = FR_OK;
+  std::vector<uint8_t> dec;
+  std::vector<double> vals;
+  const int rc0 = fr_host_row(tok_bytes + tok_off[0], tok_off[1] - tok_off[0], -1, dec, vals);
+  if (rc0 != FR_OK) {
+    status[0] = rc0;
+    return PIO_ALS_OK;
+  }
+  const long long p = (long long)vals.size();
+  if (p < 1 || p > 65535)
+    return fail(nullptr, PIO_ALS_ERR_ARG, "row 0 holds %lld values: between 1 and 65535 are supported", p);
+  CK0(cudaMalloc((void**)&d->d_x, sizeof(double) * (size_t)n * (size_t)p));
+  FrTimer timer;
+  EVF(timer.start(d->st));
+  EVF(fr_parse_rows(d->st, tok_bytes, tok_off, n, (int)p, d->d_x, status, &d->parts, &d->host_rows));
+  EVF(timer.stop(d->st, &d->parse_ms));
+  d->n = n, d->p = (int)p, *out_p = (int)p;
+  bool ok = true;
+  for (int r = 0; r < n; ++r) ok &= status[r] == FR_OK || status[r] == FR_HOST;
+  d->rows_ok = ok;
+  return PIO_ALS_OK;
+}
+
+static int fr_gramian(pio_fr_data* d, double* out_mean, double* out_gram) {
+  if (!out_mean || !out_gram) return fail(nullptr, PIO_ALS_ERR_ARG, "null argument");
+  if (!d->rows_ok) return fail(nullptr, PIO_ALS_ERR_STATE, "no parsed rows: pio_fr_parse has not succeeded");
+  if (d->n < 2) return fail(nullptr, PIO_ALS_ERR_ARG, "the Gramian's mean and covariance need at least 2 rows");
+  CK0(cudaSetDevice(d->device));
+  cudaStream_t st = d->st;
+  const long long n = d->n, p = d->p;
+  const FrSlices sl = fr_slices(n, p);
+  d->slices = sl.count;
+  Scratch tmp(st);
+  double *d_part = nullptr, *d_cs = nullptr, *d_g = nullptr;
+  CK0(tmp.alloc(&d_part, (size_t)sl.count * p * p));
+  CK0(tmp.alloc(&d_cs, (size_t)sl.count * p));
+  CK0(tmp.alloc(&d_g, (size_t)p * p));
+  FrTimer timer;
+  EVF(timer.start(st));
+  fr_colsum_kernel<<<dim3(nblk(p, 128), sl.count), 128, 0, st>>>(d->d_x, n, (int)p, sl.rows, d_cs);
+  const unsigned T = nblk(p, FR_TILE);
+  fr_gram_kernel<<<dim3(T, T, sl.count), 256, 0, st>>>(d->d_x, n, (int)p, sl.rows, d_part);
+  fr_gram_fold_kernel<<<nblk(p * p, 256), 256, 0, st>>>(d_part, sl.count, (int)p, d_g);
+  CK0(cudaGetLastError());
+  std::vector<double> cs((size_t)sl.count * p);
+  CK0(cudaMemcpyAsync(cs.data(), d_cs, sizeof(double) * cs.size(), cudaMemcpyDeviceToHost, st));
+  CK0(cudaMemcpyAsync(out_gram, d_g, sizeof(double) * (size_t)p * p, cudaMemcpyDeviceToHost, st));
+  EVF(timer.stop(st, &d->gram_ms));
+  for (long long j = 0; j < p; ++j) {
+    double acc = 0.0;
+    for (int s = 0; s < sl.count; ++s) acc += cs[(size_t)s * p + j];
+    out_mean[j] = acc / (double)n;
+  }
+  return PIO_ALS_OK;
+}
+
+// a = pc^T: k x p row-major from pc p x k row-major
+static std::vector<double> fr_components(const double* pc, long long p, long long k) {
+  std::vector<double> a((size_t)(p * k));
+  for (long long j = 0; j < p; ++j)
+    for (long long o = 0; o < k; ++o) a[(size_t)(o * p + j)] = pc[j * k + o];
+  return a;
+}
+
+static int fr_project(pio_fr_data* d, int32_t k, const double* mean, const double* pc, double* out_y) {
+  if (!mean || !pc) return fail(nullptr, PIO_ALS_ERR_ARG, "null argument");
+  if (!d->rows_ok) return fail(nullptr, PIO_ALS_ERR_STATE, "no parsed rows: pio_fr_parse has not succeeded");
+  if (k < 1 || k > d->p) return fail(nullptr, PIO_ALS_ERR_ARG, "k = %d out of range (0, p = %d]", k, d->p);
+  CK0(cudaSetDevice(d->device));
+  cudaStream_t st = d->st;
+  const long long n = d->n, p = d->p;
+  for (double* q : {d->d_y, d->d_yt, d->d_sigma})
+    if (q) cudaFree(q);
+  d->d_y = d->d_yt = d->d_sigma = nullptr;
+  d->k = 0, d->n_class = 0;
+  const std::vector<double> a = fr_components(pc, p, k);
+  Scratch tmp(st);
+  double *d_mean = nullptr, *d_a = nullptr;
+  CK0(tmp.alloc(&d_mean, (size_t)p));
+  CK0(tmp.alloc(&d_a, a.size()));
+  CK0(cudaMalloc((void**)&d->d_y, sizeof(double) * (size_t)(n * k)));
+  CK0(cudaMalloc((void**)&d->d_yt, sizeof(double) * (size_t)(n * k)));
+  FrTimer timer;
+  EVF(timer.start(st));
+  CK0(cudaMemcpyAsync(d_mean, mean, sizeof(double) * (size_t)p, cudaMemcpyHostToDevice, st));
+  CK0(cudaMemcpyAsync(d_a, a.data(), sizeof(double) * a.size(), cudaMemcpyHostToDevice, st));
+  fr_fold_kernel<<<dim3(nblk(n, FR_TILE), nblk(k, FR_TILE)), 256, 0, st>>>(d->d_x, n, (int)p, d_a, k, d_mean, nullptr,
+                                                                           d->d_y, k, 1, d->d_yt, 1, n);
+  CK0(cudaGetLastError());
+  if (out_y) CK0(cudaMemcpyAsync(out_y, d->d_y, sizeof(double) * (size_t)(n * k), cudaMemcpyDeviceToHost, st));
+  EVF(timer.stop(st, &d->project_ms));
+  d->k = k;
+  return PIO_ALS_OK;
+}
+
+static int fr_lr_prepare(pio_fr_data* d, const int32_t* cls, int32_t n_class, double* out_sigma) {
+  if (!cls || !out_sigma) return fail(nullptr, PIO_ALS_ERR_ARG, "null argument");
+  if (!d->k) return fail(nullptr, PIO_ALS_ERR_STATE, "no projected rows: pio_fr_project has not been called");
+  if (n_class < 1) return fail(nullptr, PIO_ALS_ERR_ARG, "n_class must be >= 1");
+  const long long n = d->n, k = d->k;
+  for (long long i = 0; i < n; ++i)
+    if (cls[i] < 0 || cls[i] >= n_class)
+      return fail(nullptr, PIO_ALS_ERR_ARG, "class %d of row %lld is not in [0, %d)", cls[i], i, n_class);
+  CK0(cudaSetDevice(d->device));
+  cudaStream_t st = d->st;
+  if (d->d_cls) cudaFree(d->d_cls);
+  if (d->d_sigma) cudaFree(d->d_sigma);
+  d->d_cls = nullptr, d->d_sigma = nullptr, d->n_class = 0;
+  CK0(cudaMalloc((void**)&d->d_cls, sizeof(int) * (size_t)n));
+  CK0(cudaMalloc((void**)&d->d_sigma, sizeof(double) * (size_t)k));
+  const int nb = (int)nblk(n, FR_LR_BLOCK);
+  Scratch tmp(st);
+  double *d_part = nullptr, *d_sum = nullptr;
+  CK0(tmp.alloc(&d_part, (size_t)nb * k));
+  CK0(tmp.alloc(&d_sum, (size_t)k));
+  FrTimer timer;
+  EVF(timer.start(st));
+  CK0(cudaMemcpyAsync(d->d_cls, cls, sizeof(int) * (size_t)n, cudaMemcpyHostToDevice, st));
+  std::vector<double> s((size_t)k);
+  for (int pass = 0; pass < 2; ++pass) {
+    fr_lr_colsum_kernel<<<dim3(nb, nblk(k, 128)), 128, 0, st>>>(d->d_y, n, (int)k, pass ? d->d_sigma : nullptr,
+                                                                  d_part);
+    fr_lr_fold_kernel<<<dim3(nblk(k, 128), 1), 128, 0, st>>>(d_part, nb, (int)k, d_sum);
+    CK0(cudaGetLastError());
+    CK0(cudaMemcpyAsync(s.data(), d_sum, sizeof(double) * (size_t)k, cudaMemcpyDeviceToHost, st));
+    CK0(cudaStreamSynchronize(st));
+    for (long long j = 0; j < k; ++j) s[j] = pass ? sqrt(s[j] / (double)(n - 1)) : s[j] / (double)n;
+    // the first pass leaves the column means in d_sigma as the centres of the second
+    CK0(cudaMemcpyAsync(d->d_sigma, s.data(), sizeof(double) * (size_t)k, cudaMemcpyHostToDevice, st));
+    CK0(cudaStreamSynchronize(st));
+  }
+  EVF(timer.stop(st, &d->sigma_ms));
+  memcpy(out_sigma, s.data(), sizeof(double) * (size_t)k);
+  d->n_class = n_class;
+  return PIO_ALS_OK;
+}
+
+static int fr_lr_eval(pio_fr_data* d, int32_t na, const int32_t* labels, const double* wb, double reg, double* out_f,
+                      double* out_g) {
+  if (!labels || !wb || !out_f || !out_g) return fail(nullptr, PIO_ALS_ERR_ARG, "null argument");
+  if (!d->n_class) return fail(nullptr, PIO_ALS_ERR_STATE, "pio_fr_lr_prepare has not been called");
+  if (na < 1 || na > 65535) return fail(nullptr, PIO_ALS_ERR_ARG, "n_active must be in [1, 65535] (got %d)", na);
+  if (!(reg >= 0.0)) return fail(nullptr, PIO_ALS_ERR_ARG, "reg_param must be >= 0 (got %g)", reg);
+  for (int a = 0; a < na; ++a)
+    if (labels[a] < 0 || labels[a] >= d->n_class)
+      return fail(nullptr, PIO_ALS_ERR_ARG, "label %d of slot %d is not in [0, %d)", labels[a], a, d->n_class);
+  CK0(cudaSetDevice(d->device));
+  cudaStream_t st = d->st;
+  const long long n = d->n, k = d->k, w = k + 2;
+  const int nb = (int)nblk(n, FR_LR_BLOCK);
+  Scratch tmp(st);
+  double *d_wb = nullptr, *d_mult = nullptr, *d_loss = nullptr, *d_part = nullptr, *d_out = nullptr;
+  int* d_lab = nullptr;
+  CK0(tmp.alloc(&d_wb, (size_t)na * (k + 1)));
+  CK0(tmp.alloc(&d_lab, (size_t)na));
+  CK0(tmp.alloc(&d_mult, (size_t)na * n));
+  CK0(tmp.alloc(&d_loss, (size_t)na * n));
+  CK0(tmp.alloc(&d_part, (size_t)na * nb * w));
+  CK0(tmp.alloc(&d_out, (size_t)na * w));
+  FrTimer timer;
+  EVF(timer.start(st));
+  CK0(cudaMemcpyAsync(d_wb, wb, sizeof(double) * (size_t)na * (k + 1), cudaMemcpyHostToDevice, st));
+  CK0(cudaMemcpyAsync(d_lab, labels, sizeof(int) * (size_t)na, cudaMemcpyHostToDevice, st));
+  fr_lr_margin_kernel<<<dim3(nblk(n, 256), na), 256, 0, st>>>(d->d_yt, n, (int)k, d->d_sigma, d->d_cls, d_wb, d_lab,
+                                                              d_mult, d_loss);
+  fr_lr_grad_kernel<<<dim3(nb, nblk(w, 128), na), 128, 0, st>>>(d->d_y, n, (int)k, d->d_sigma, d_mult, d_loss, nb,
+                                                                d_part);
+  fr_lr_fold_kernel<<<dim3(nblk(w, 128), na), 128, 0, st>>>(d_part, nb, (int)w, d_out);
+  CK0(cudaGetLastError());
+  std::vector<double> sums((size_t)na * w);
+  CK0(cudaMemcpyAsync(sums.data(), d_out, sizeof(double) * sums.size(), cudaMemcpyDeviceToHost, st));
+  double ms = 0;
+  EVF(timer.stop(st, &ms));
+  d->lr_ms += ms;
+  ++d->lr_evals;
+  // loss = lossSum / n + 0.5 reg sum_j w_j^2; gradient = sum / n + reg w_j, the intercept's unregularized
+  for (int a = 0; a < na; ++a) {
+    const double* sa = sums.data() + (size_t)a * w;
+    const double* wa = wb + (size_t)a * (k + 1);
+    double* ga = out_g + (size_t)a * (k + 1);
+    double sq = 0.0;
+    for (long long j = 0; j < k; ++j) {
+      sq += wa[j] * wa[j];
+      ga[j] = sa[j] / (double)n + reg * wa[j];
+    }
+    ga[k] = sa[k] / (double)n;
+    out_f[a] = sa[k + 1] / (double)n + 0.5 * reg * sq;
+  }
+  return PIO_ALS_OK;
+}
+
+static int fr_model_scores(pio_fr_model* m, const uint8_t* tok_bytes, const int64_t* tok_off, int32_t n,
+                           int32_t* status, double* out) {
+  EVF(fr_check_tokens(tok_bytes, tok_off, n));
+  if (n > 0 && (!status || !out)) return fail(nullptr, PIO_ALS_ERR_ARG, "null argument");
+  m->parts = m->rows = m->host_rows = 0;
+  m->device_ms = 0;
+  if (n == 0) return PIO_ALS_OK;
+  CK0(cudaSetDevice(m->device));
+  cudaStream_t st = m->st;
+  const long long p = m->p, k = m->k, L = m->n_label;
+  Scratch tmp(st);
+  double *d_x = nullptr, *d_y = nullptr, *d_s = nullptr;
+  CK0(tmp.alloc(&d_x, (size_t)n * p));
+  CK0(tmp.alloc(&d_y, (size_t)n * k));
+  CK0(tmp.alloc(&d_s, (size_t)n * L));
+  FrTimer timer;
+  EVF(timer.start(st));
+  EVF(fr_parse_rows(st, tok_bytes, tok_off, n, (int)p, d_x, status, &m->parts, &m->host_rows));
+  fr_fold_kernel<<<dim3(nblk(n, FR_TILE), nblk(k, FR_TILE)), 256, 0, st>>>(d_x, n, (int)p, m->d_a, (int)k, m->d_mean,
+                                                                           nullptr, d_y, k, 1, nullptr, 0, 0);
+  fr_fold_kernel<<<dim3(nblk(n, FR_TILE), nblk(L, FR_TILE)), 256, 0, st>>>(d_y, n, (int)k, m->d_coef, (int)L,
+                                                                           nullptr, m->d_b, d_s, L, 1, nullptr, 0, 0);
+  CK0(cudaGetLastError());
+  CK0(cudaMemcpyAsync(out, d_s, sizeof(double) * (size_t)n * L, cudaMemcpyDeviceToHost, st));
+  EVF(timer.stop(st, &m->device_ms));
+  m->rows = n;
+  return PIO_ALS_OK;
+}
+
+}  // namespace pio
+
+extern "C" {
+
+int pio_fr_data_create(int device, pio_fr_data** out) {
+  if (!out) return fail(nullptr, PIO_ALS_ERR_ARG, "null argument");
+  *out = nullptr;
+  try {
+    std::unique_ptr<pio_fr_data> d(new pio_fr_data);
+    d->device = device;
+    CK0(cudaSetDevice(device));
+    CK0(cudaStreamCreateWithFlags(&d->st, cudaStreamNonBlocking));
+    *out = d.release();
+  } catch (const std::bad_alloc&) {
+    return fail(nullptr, PIO_ALS_ERR_NOMEM, "pio_fr_data_create: out of host memory");
+  }
+  return PIO_ALS_OK;
+}
+
+int pio_fr_data_destroy(pio_fr_data* d) {
+  if (!d) return PIO_ALS_OK;
+  cudaSetDevice(d->device);
+  if (d->st) cudaStreamSynchronize(d->st);
+  fr_free_rows(d);
+  if (d->st) cudaStreamDestroy(d->st);
+  delete d;
+  return PIO_ALS_OK;
+}
+
+#define FR_CALL(obj, what, body)                                                      \
+  do {                                                                                \
+    if (!(obj)) return fail(nullptr, PIO_ALS_ERR_ARG, "%s: null object", what);       \
+    std::lock_guard<std::mutex> lk((obj)->mu);                                        \
+    try {                                                                             \
+      return body;                                                                    \
+    } catch (const std::bad_alloc&) {                                                 \
+      return fail(nullptr, PIO_ALS_ERR_NOMEM, "%s: out of host memory", what);        \
+    }                                                                                 \
+  } while (0)
+
+int pio_fr_parse(pio_fr_data* d, const uint8_t* tok_bytes, const int64_t* tok_off, int32_t n_rows,
+                 int32_t* out_status, int32_t* out_p) {
+  FR_CALL(d, "pio_fr_parse", fr_parse(d, tok_bytes, tok_off, n_rows, out_status, out_p));
+}
+
+int pio_fr_gramian(pio_fr_data* d, double* out_mean, double* out_gram) {
+  FR_CALL(d, "pio_fr_gramian", fr_gramian(d, out_mean, out_gram));
+}
+
+int pio_fr_project(pio_fr_data* d, int32_t k, const double* mean, const double* pc, double* out_y) {
+  FR_CALL(d, "pio_fr_project", fr_project(d, k, mean, pc, out_y));
+}
+
+int pio_fr_lr_prepare(pio_fr_data* d, const int32_t* cls, int32_t n_class, double* out_sigma) {
+  FR_CALL(d, "pio_fr_lr_prepare", fr_lr_prepare(d, cls, n_class, out_sigma));
+}
+
+int pio_fr_lr_eval(pio_fr_data* d, int32_t n_active, const int32_t* labels, const double* wb, double reg_param,
+                   double* out_f, double* out_g) {
+  FR_CALL(d, "pio_fr_lr_eval", fr_lr_eval(d, n_active, labels, wb, reg_param, out_f, out_g));
+}
+
+int pio_fr_data_debug_stats(const pio_fr_data* d, double out[10]) {
+  if (!d || !out) return PIO_ALS_ERR_ARG;
+  out[0] = (double)d->parts, out[1] = (double)d->n, out[2] = (double)d->host_rows, out[3] = d->parse_ms;
+  out[4] = d->gram_ms, out[5] = d->project_ms, out[6] = d->sigma_ms, out[7] = d->lr_ms, out[8] = (double)d->lr_evals;
+  out[9] = (double)d->slices;
+  return PIO_ALS_OK;
+}
+
+int pio_fr_model_create(int device, int32_t p, int32_t k, int32_t n_label, const double* mean, const double* pc,
+                        const double* coef, const double* b, pio_fr_model** out) {
+  if (!out) return fail(nullptr, PIO_ALS_ERR_ARG, "null argument");
+  *out = nullptr;
+  if (p < 1 || p > 65535 || k < 1 || k > p || n_label < 1 || n_label > 65535)
+    return fail(nullptr, PIO_ALS_ERR_ARG, "bad model shape: p = %d, k = %d, n_label = %d (1 <= k <= p <= 65535, "
+                "n_label >= 1)", p, k, n_label);
+  if (!mean || !pc || !coef || !b) return fail(nullptr, PIO_ALS_ERR_ARG, "null argument");
+  try {
+    const std::vector<double> a = fr_components(pc, p, k);
+    std::unique_ptr<pio_fr_model> m(new pio_fr_model);
+    m->device = device, m->p = p, m->k = k, m->n_label = n_label;
+    CK0(cudaSetDevice(device));
+    CK0(cudaStreamCreateWithFlags(&m->st, cudaStreamNonBlocking));
+    std::unique_ptr<pio_fr_model, int (*)(pio_fr_model*)> g(m.release(), pio_fr_model_destroy);
+    CK0(cudaMalloc((void**)&g->d_mean, sizeof(double) * (size_t)p));
+    CK0(cudaMalloc((void**)&g->d_a, sizeof(double) * a.size()));
+    CK0(cudaMalloc((void**)&g->d_coef, sizeof(double) * (size_t)n_label * k));
+    CK0(cudaMalloc((void**)&g->d_b, sizeof(double) * (size_t)n_label));
+    CK0(cudaMemcpy(g->d_mean, mean, sizeof(double) * (size_t)p, cudaMemcpyHostToDevice));
+    CK0(cudaMemcpy(g->d_a, a.data(), sizeof(double) * a.size(), cudaMemcpyHostToDevice));
+    CK0(cudaMemcpy(g->d_coef, coef, sizeof(double) * (size_t)n_label * k, cudaMemcpyHostToDevice));
+    CK0(cudaMemcpy(g->d_b, b, sizeof(double) * (size_t)n_label, cudaMemcpyHostToDevice));
+    *out = g.release();
+  } catch (const std::bad_alloc&) {
+    return fail(nullptr, PIO_ALS_ERR_NOMEM, "pio_fr_model_create: out of host memory");
+  }
+  return PIO_ALS_OK;
+}
+
+int pio_fr_model_destroy(pio_fr_model* m) {
+  if (!m) return PIO_ALS_OK;
+  cudaSetDevice(m->device);
+  if (m->st) cudaStreamSynchronize(m->st);
+  for (void* q : {(void*)m->d_mean, (void*)m->d_a, (void*)m->d_coef, (void*)m->d_b})
+    if (q) cudaFree(q);
+  if (m->st) cudaStreamDestroy(m->st);
+  delete m;
+  return PIO_ALS_OK;
+}
+
+int pio_fr_model_scores(pio_fr_model* m, const uint8_t* tok_bytes, const int64_t* tok_off, int32_t n,
+                        int32_t* out_status, double* out_scores) {
+  FR_CALL(m, "pio_fr_model_scores", fr_model_scores(m, tok_bytes, tok_off, n, out_status, out_scores));
+}
+
+int pio_fr_model_debug_stats(const pio_fr_model* m, double out[4]) {
+  if (!m || !out) return PIO_ALS_ERR_ARG;
+  out[0] = (double)m->parts, out[1] = (double)m->rows, out[2] = (double)m->host_rows, out[3] = m->device_ms;
   return PIO_ALS_OK;
 }
 

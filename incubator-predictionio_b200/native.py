@@ -55,7 +55,9 @@ EXPORTED_SYMBOLS = [
     "pio_text_model_destroy", "pio_text_model_set", "pio_text_train_nb", "pio_text_features", "pio_text_features_get",
     "pio_text_scores", "pio_text_debug_stats", "pio_text_folds_create", "pio_text_folds_destroy",
     "pio_text_folds_featurize", "pio_text_folds_sizes", "pio_text_folds_train_nb", "pio_text_folds_scores",
-    "pio_text_folds_debug_stats",
+    "pio_text_folds_debug_stats", "pio_fr_data_create", "pio_fr_data_destroy", "pio_fr_parse", "pio_fr_gramian",
+    "pio_fr_project", "pio_fr_lr_prepare", "pio_fr_lr_eval", "pio_fr_data_debug_stats", "pio_fr_model_create",
+    "pio_fr_model_destroy", "pio_fr_model_scores", "pio_fr_model_debug_stats",
 ]
 
 
@@ -251,6 +253,17 @@ def lib():
         L.pio_text_folds_scores.argtypes = [vp, C.c_int32, C.c_int32, vp, vp, vp, vp]
         L.pio_text_folds_debug_stats.restype = ci
         L.pio_text_folds_debug_stats.argtypes = [vp, vp]
+        i32 = C.c_int32
+        for name, args in (("pio_fr_data_create", [ci, vp]), ("pio_fr_data_destroy", [vp]),
+                           ("pio_fr_parse", [vp, vp, vp, i32, vp, vp]), ("pio_fr_gramian", [vp, vp, vp]),
+                           ("pio_fr_project", [vp, i32, vp, vp, vp]), ("pio_fr_lr_prepare", [vp, vp, i32, vp]),
+                           ("pio_fr_lr_eval", [vp, i32, vp, vp, C.c_double, vp, vp]),
+                           ("pio_fr_data_debug_stats", [vp, vp]),
+                           ("pio_fr_model_create", [ci, i32, i32, i32, vp, vp, vp, vp, vp]),
+                           ("pio_fr_model_destroy", [vp]), ("pio_fr_model_scores", [vp, vp, vp, i32, vp, vp]),
+                           ("pio_fr_model_debug_stats", [vp, vp])):
+            getattr(L, name).restype = ci
+            getattr(L, name).argtypes = args
         for name in EXPORTED_SYMBOLS:
             getattr(L, name)  # AttributeError if the ABI is incomplete
         _lib = L
@@ -1724,3 +1737,130 @@ class TextFolds:
         _check(lib().pio_text_folds_debug_stats(self._h, out))
         return {"featurizations": int(out[0]), "entries": int(out[1]), "parts": int(out[2]),
                 "featurize_ms": out[3], "train_ms": out[4], "scores_ms": out[5]}
+
+
+# pio_fr_parse's per-row status (PIO_FR_* in pio_als.h)
+FR_OK, FR_HOST, FR_BAD, FR_NONFINITE, FR_LEN = 0, 1, -1, -2, -3
+
+
+class FeatureData:
+    """pio_fr_data: the dimensionality-reduction template's training rows on `device`.  parse() reads feature strings
+    -- raw JSON string tokens, as the keyed event scan returns them or text_tokens makes them -- into a resident n x p
+    fp64 matrix; gramian() gives its column means and X^T X; project() keeps the rows' projections onto the principal
+    components; lr_prepare() and lr_eval() give the one-vs-rest logistic regressions' sigma, loss and gradient."""
+
+    def __init__(self, device: int = 0):
+        self.device = int(device)
+        self.n = self.p = self.k = 0
+        self._h = C.c_void_p()
+        _check(lib().pio_fr_data_create(self.device, C.addressof(self._h)))
+
+    def close(self):
+        if self._h:
+            lib().pio_fr_data_destroy(self._h)
+            self._h = C.c_void_p()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    def parse(self, tok_bytes, tok_off):
+        """(per-row status int32 [n], p): p is row 0's length (0 when row 0 is bad)."""
+        b, o, n = _text_tokens_arg(tok_bytes, tok_off)
+        status = np.zeros(max(n, 1), np.int32)
+        p = C.c_int32(0)
+        _check(lib().pio_fr_parse(self._h, b.ctypes.data if b.size else None, o.ctypes.data, n, status.ctypes.data,
+                                  C.addressof(p)))
+        self.n, self.p, self.k = n, int(p.value), 0
+        return status[:n], self.p
+
+    def gramian(self):
+        """(mean [p], X^T X [p, p])."""
+        mean, g = np.empty(self.p, np.float64), np.empty((self.p, self.p), np.float64)
+        _check(lib().pio_fr_gramian(self._h, mean.ctypes.data, g.ctypes.data))
+        return mean, g
+
+    def project(self, mean, pc, copy_out: bool = False):
+        """Keeps y = (x - mean) . pc of every row on the device (pc: [p, k]); the rows [n, k] when copy_out."""
+        mean = np.ascontiguousarray(mean, np.float64)
+        pc = np.ascontiguousarray(pc, np.float64)
+        if mean.shape != (self.p,) or pc.ndim != 2 or pc.shape[0] != self.p:
+            raise ValueError("mean must be [p] and pc [p, k]")
+        k = int(pc.shape[1])
+        y = np.empty((self.n, k), np.float64) if copy_out else None
+        _check(lib().pio_fr_project(self._h, k, mean.ctypes.data, pc.ctypes.data, _addr(y)))
+        self.k = k
+        return y
+
+    def lr_prepare(self, cls, n_class: int) -> np.ndarray:
+        """Each row's class in [0, n_class): the columns' unbiased standard deviations sigma [k]."""
+        cls = np.ascontiguousarray(cls, np.int32)
+        if cls.shape != (self.n,):
+            raise ValueError("one class per row")
+        sigma = np.empty(self.k, np.float64)
+        _check(lib().pio_fr_lr_prepare(self._h, cls.ctypes.data, int(n_class), sigma.ctypes.data))
+        return sigma
+
+    def lr_eval(self, labels, wb, reg_param: float):
+        """Loss [a] and gradient [a, k + 1] of the binary regressions of labels[a] against the rest at wb[a]."""
+        labels = np.ascontiguousarray(labels, np.int32)
+        wb = np.ascontiguousarray(wb, np.float64)
+        na = labels.shape[0]
+        if wb.shape != (na, self.k + 1):
+            raise ValueError("wb must be [n_active, k + 1]")
+        f, g = np.empty(max(na, 1), np.float64), np.empty((max(na, 1), self.k + 1), np.float64)
+        _check(lib().pio_fr_lr_eval(self._h, na, labels.ctypes.data, wb.ctypes.data, float(reg_param), f.ctypes.data,
+                                    g.ctypes.data))
+        return f[:na], g[:na]
+
+    def stats(self) -> dict:
+        out = (C.c_double * 10)()
+        _check(lib().pio_fr_data_debug_stats(self._h, out))
+        return {"parts": int(out[0]), "rows": int(out[1]), "host_rows": int(out[2]), "parse_ms": out[3],
+                "gram_ms": out[4], "project_ms": out[5], "sigma_ms": out[6], "lr_ms": out[7], "lr_evals": int(out[8]),
+                "slices": int(out[9])}
+
+
+class FeatureModel:
+    """pio_fr_model: a trained dimensionality-reduction model on `device` -- mean [p], the principal components pc
+    [p, k], coef [L, k] and intercepts b [L] -- that scores batches of feature strings."""
+
+    def __init__(self, mean, pc, coef, b, device: int = 0):
+        mean = np.ascontiguousarray(mean, np.float64)
+        pc = np.ascontiguousarray(pc, np.float64)
+        coef = np.ascontiguousarray(coef, np.float64)
+        b = np.ascontiguousarray(b, np.float64)
+        if pc.ndim != 2 or mean.shape != (pc.shape[0],) or coef.ndim != 2 or coef.shape[1] != pc.shape[1] or \
+                b.shape != (coef.shape[0],):
+            raise ValueError("mean must be [p], pc [p, k], coef [L, k] and b [L]")
+        self.p, self.k, self.n_label, self.device = int(pc.shape[0]), int(pc.shape[1]), int(coef.shape[0]), int(device)
+        self._h = C.c_void_p()
+        _check(lib().pio_fr_model_create(self.device, self.p, self.k, self.n_label, mean.ctypes.data, pc.ctypes.data,
+                                         coef.ctypes.data, b.ctypes.data, C.addressof(self._h)))
+
+    def close(self):
+        if self._h:
+            lib().pio_fr_model_destroy(self._h)
+            self._h = C.c_void_p()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    def scores(self, tok_bytes, tok_off):
+        """(per-row status [n], fold(coef . y) + b [n, L]) of the feature strings' projections y."""
+        b, o, n = _text_tokens_arg(tok_bytes, tok_off)
+        status = np.zeros(max(n, 1), np.int32)
+        out = np.empty((max(n, 1), self.n_label), np.float64)
+        _check(lib().pio_fr_model_scores(self._h, b.ctypes.data if b.size else None, o.ctypes.data, n,
+                                         status.ctypes.data, out.ctypes.data))
+        return status[:n], out[:n]
+
+    def stats(self) -> dict:
+        out = (C.c_double * 4)()
+        _check(lib().pio_fr_model_debug_stats(self._h, out))
+        return {"parts": int(out[0]), "rows": int(out[1]), "host_rows": int(out[2]), "device_ms": out[3]}
